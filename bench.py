@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — env-steps/sec (collect + update) of the CartPole-v1 PPO hot path on B200.
+"""bench.py — env-steps/sec (collect + update) of the CartPole-v1 PPO hot path on H100.
 
 Workload (BASELINE.json configs[1]): CartPole-v1 PPO, 4096 parallel envs PER GPU (weak scaling),
 MLP policy/critic, 128-step rollout, 4 PPO epochs, 1 minibatch, device-resident env.step + GAE +
@@ -9,10 +9,11 @@ ppo_update kernels.  A "step" is one iteration = 128 vec-env steps + critic pass
     python bench.py --gpus 1 --steps 10 --warmup 3
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference          # CPU restatement of the reference path (oracle port)
+    python bench.py --gpus 1 --steps 10 --dump-outputs DIR   # also save the last timed step's outputs
 
-One JSON line on rank 0 (see the contract in the task statement).  Timing: CUDA events per
-iteration on the launching stream, L2 flushed (256 MB write) between timed iterations, max over
-ranks; clocks sampled with nvidia-smi during the timed region.
+One JSON line on rank 0.  Timing: CUDA events per iteration on the launching stream, L2 flushed
+(256 MB write) between timed iterations, max over ranks; clocks sampled with nvidia-smi during the
+timed region.
 """
 import argparse
 import json
@@ -38,7 +39,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d["hbm_gbs"], "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 class ClockSampler:
@@ -195,11 +196,30 @@ def gae_roofline(flush, steps=10):
     return out
 
 
-def time_iterations(drv, steps, warmup, flush, world):
+def dump_outputs(drv, out_dir):
+    """What the timed iteration hands its caller, as float32 / float64 .npy files in `out_dir`: the updated policy and
+    critic parameters, the summed update losses, and the rollout buffer as the iteration leaves it (~25 MB at the C2
+    shape).  The iteration ends with the slot shift (after_update), so slot 0 of policy_obs and masks already holds the
+    next rollout's start (= slot T); every other slot, and all of actions, rewards, log-probs, values, returns and
+    advantages, is what the update trained on."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    d, tr = drv.buffer.data, drv.trainer
+    arrays = {"policy_params": tr.algo_module.models["policy"].flat_params, "critic_params": tr.algo_module.models["critic"].flat_params,
+              "train_info": tr.train_info, "policy_obs": d.policy_obs, "actions": d.actions, "action_log_probs": d.action_log_probs,
+              "rewards": d.rewards, "masks": d.masks, "value_preds": d.value_preds, "returns": d.returns, "advantages": d.advantages}
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        np.save(os.path.join(out_dir, name + ".npy"), a if a.dtype == np.float64 else a.astype(np.float32))
+
+
+def time_iterations(drv, steps, warmup, flush, world, dump_dir=None):
     """W untimed + K timed device iterations (collect + update) through `OnPolicyDriver.device_iteration` — one captured
     CUDA graph replay per iteration when eligible (the product's default), else ~25 launches — CUDA events per iteration
     on the launching stream, 256 MB L2 flush between timed iterations, max over ranks.  The per-phase times come from a
     separate short eager pass (events cannot be read inside a graph).
+    With `dump_dir`, the outputs of the last timed iteration are written there (dump_outputs) before the phase pass.
     Returns (seconds, phases_ms, launches, wall window)."""
     import torch
     import torch.distributed as dist
@@ -226,6 +246,8 @@ def time_iterations(drv, steps, warmup, flush, world):
     barrier()
     window = (t0, time.time())
     launches = drv.gpu_launches + drv.trainer.gpu_launches - l0
+    if dump_dir is not None and dist_rank() == 0:
+        dump_outputs(drv, dump_dir)
     total_s = sum(a.elapsed_time(b) for a, b in events) * 1e-3
     # phases: eager pass
     drv.phase_events = []
@@ -241,6 +263,10 @@ def time_iterations(drv, steps, warmup, flush, world):
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     return float(t.item()), {k: statistics.mean(v) for k, v in phases.items()}, launches, window
+
+
+def dist_rank():
+    return int(os.environ.get("RANK", 0))
 
 
 def time_e2e(rank, world, steps, workload="c2", envs=None, extra_flags=()):
@@ -285,7 +311,7 @@ def side_result(rank, world, flush, workload, steps, envs=None, extra_flags=(), 
            "value": n * Tn * steps * world / sec, "unit": "env-steps/s", "ms_per_step": sec / steps * 1e3,
            "phases_ms": {k: round(v, 4) for k, v in phases.items()}, "gpu_launches": launches, "steps": steps,
            "cuda_graph": getattr(drv, "_graph", None) is not None,
-           "update_kernel": "tcgen05 split-fp16" if drv.trainer.use_tensor_cores else ("GRU warp kernels (fp32)" if drv.trainer.recurrent else "fp32 FFMA")}
+           "update_kernel": "wgmma split-fp16" if drv.trainer.use_tensor_cores else ("GRU warp kernels (fp32)" if drv.trainer.recurrent else "fp32 FFMA")}
     del drv
     if e2e:
         es, h2d, d2h = time_e2e(rank, world, steps, workload, envs, extra_flags)
@@ -331,16 +357,6 @@ def c5_result(steps=3, grouped=True):
                       else "one group, synchronous (act -> D2H -> env.step -> H2D per step)"}
 
 
-def ncu_traffic():
-    """dram bytes per launch of the GAE kernel from the committed ncu capture summary (profiles/), or None."""
-    for name in ("r2_ncu_gae.json", "r1_ncu_gae.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(p):
-            d = json.load(open(p))
-            return d.get("dram_bytes_per_launch"), f"ncu --set full, profiles/{name} (dram__bytes_read.sum + dram__bytes_write.sum)"
-    return None, "no ncu capture summary under profiles/"
-
-
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -351,13 +367,13 @@ def run_ours(args):
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device(f"cuda:{local}"))
 
-    flush = torch.empty(256 * 1024 * 1024 // 4, device="cuda")  # 256 MB > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device="cuda")  # 256 MB > 50 MB L2
     cfg, env, net, agent = build_agent(rank, world, "c2")
     drv = make_driver(cfg, env, net, agent, rank, world)
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
-    total_s, phases, launches, window = time_iterations(drv, args.steps, args.warmup, flush, world)
+    total_s, phases, launches, window = time_iterations(drv, args.steps, args.warmup, flush, world, dump_dir=args.dump_outputs)
     sampler.window = window
     clocks = sampler.stop() if rank == 0 else None
     env_steps = N_ENVS * T * args.steps * world
@@ -391,11 +407,10 @@ def run_ours(args):
     gae_in_step = phases.get("gae", 0.0) * 1e-3
     upd_s = phases.get("update", 0.0) * 1e-3
     flops_update = 53e3 * N_ENVS * T * EPOCHS  # fwd+bwd of both nets, SURVEY.md §8d
-    sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
-    fp32_peak = 148 * 128 * 2 * sm_mhz * 1e6 / 1e12
+    sm_mhz = (clocks or {}).get("sm_mhz") or 1980.0
+    fp32_peak = torch.cuda.get_device_properties(0).multi_processor_count * 128 * 2 * sm_mhz * 1e6 / 1e12
     pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-    tensor_peak = pk.get("bf16_tflops", 1668.8)   # fp16 and bf16 dense MMAs run at the same rate
-    traffic, traffic_src = ncu_traffic()
+    tensor_peak = pk.get("bf16_tflops", 989.4)   # H100 SXM data sheet, dense; fp16 and bf16 MMAs run at the same rate
 
     extras = {}
     if world == 1 and not args.no_extras:
@@ -424,7 +439,7 @@ def run_ours(args):
         "metric": METRIC, "value": value, "unit": "env-steps/s",
         "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": total_s / args.steps * 1e3,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": "f32 (nets, losses, Adam; the three 64x64 GEMM groups of the update run as split-fp16 tcgen05 MMAs with fp32 "
+        "dtype": "f32 (nets, losses, Adam; the three 64x64 GEMM groups of the update run as split-fp16 wgmma MMAs with fp32 "
                  "accumulation = fp32-class accuracy, the mode the 1e-4 parity tests run in), f64 (CartPole state)",
         "data": "synthetic: device-resident CartPole-v1, random-init nets, seed 0",
         "config": {"workload": WORKLOAD, "global_envs": N_ENVS * world, "rollout_T": T, "parallelism": f"env-shard dp{world}",
@@ -444,11 +459,10 @@ def run_ours(args):
         "roofline": {"bound": "hbm", "kernel": "gae_scan_kernel (orl_gae), >=1 GB shape, L2 flushed", "achieved": gae["1GB"]["GBps"],
                      "peak": hbm_peak, "peak_source": how, "unit": "GB/s", "frac": gae["1GB"]["GBps"] / hbm_peak,
                      "algorithmic_bytes_per_launch": 128 * (1 << 21) * 24,
-                     "traffic": traffic, "traffic_source": traffic_src,
                      "config_shape": {**gae["config"], "frac": gae["config"]["GBps"] / hbm_peak,
                                       "in_step_avg_s": gae_in_step,
                                       "in_step_GBps": N_ENVS * T * 24 / max(gae_in_step, 1e-12) / 1e9}},
-        "roofline_dominant": {"kernel": "ppo_fwdbwd_tc_kernel (tcgen05 kind::f16, split-fp16 operands, 2 CTAs/SM)" if tc_update else "ppo_fwdbwd_kernel (fp32 FFMA)",
+        "roofline_dominant": {"kernel": "ppo_fwdbwd_tc_kernel (wgmma f16, split-fp16 operands, 1 CTA/SM)" if tc_update else "ppo_fwdbwd_kernel (fp32 FFMA)",
                               "share_of_step": upd_s / max(total_s / args.steps, 1e-12),
                               "bound": "tensor" if tc_update else "fp32 pipe",
                               "avg_s_per_iteration": upd_s, "launches_per_iteration": EPOCHS * MINIBATCH,
@@ -457,7 +471,7 @@ def run_ours(args):
                               "frac": flops_update / max(upd_s, 1e-12) / 1e12 / (tensor_peak if tc_update else fp32_peak),
                               "frac_of_fp32_pipe_peak": flops_update / max(upd_s, 1e-12) / 1e12 / fp32_peak,
                               "note": "algorithmic FLOPs (53 kFLOP/row, SURVEY.md 8d); the split issues 3 MMAs per product and M=128 "
-                                      "tiles with unused lanes, so tensor-pipe activity is higher than this fraction (ncu, profiles/)"},
+                                      "tiles with unused rows, so tensor-pipe activity is higher than this fraction"},
         "cpu_baseline": cpu,
         "clocks": clocks,
     }
@@ -494,7 +508,7 @@ def _best_cpu_threads(n_envs):
 
 
 def cpu_baseline_sample(n_envs=256, iters=1):
-    """cpu_baseline leg: the unmodified reference (`kind: reference`, baseline/_ref through
+    """cpu_baseline leg: the unmodified reference (`kind: reference`, oracle/_ref through
     oracle/run_reference.py, SyncVectorEnv, 128 of the 4096 envs, all host cores) with the oracle port
     (oracle/loop.py) timed beside it as a second, labelled number."""
     from oracle import loop as oloop
@@ -510,18 +524,18 @@ def cpu_baseline_sample(n_envs=256, iters=1):
     port = {"value": n_envs * T * iters / dt, "unit": "env-steps/s", "cores": threads, "kind": "port",
             "sample": f"{iters} iteration(s) of {n_envs} envs x T={T}, {EPOCHS} epochs (oracle/loop.py, torch-CPU + numpy)"}
     if not reference_available():
-        return {**port, "note": "baseline/_ref missing: port only"}
+        return {**port, "note": "oracle/_ref missing: port only"}
     try:
         ref = reference_run(REF_ENVS, 5, 3)
     except Exception as e:  # noqa: BLE001
         return {**port, "note": f"reference run failed ({str(e)[-200:]}): port only"}
     return {"value": ref["env_steps_per_s"], "unit": "env-steps/s", "cores": ref["torch_threads"], "kind": "reference",
             "sample": f"5 PPOAgent.train iterations (after 3 warm-up) of {REF_ENVS} of the {N_ENVS} envs x T={T}, {EPOCHS} epochs; unmodified "
-                      f"reference from baseline/_ref, SyncVectorEnv, {ref['host_cores']} host cores", "port": port}
+                      f"reference from oracle/_ref, SyncVectorEnv, {ref['host_cores']} host cores", "port": port}
 
 
 def reference_run(envs, iters, warmup, asynchronous=False, timeout=300):
-    """One timed run of the UNMODIFIED reference (baseline/_ref, oracle/run_reference.py) in a fresh
+    """One timed run of the UNMODIFIED reference (oracle/_ref, oracle/run_reference.py) in a fresh
     process: `PPOAgent.train` on the host cores, all of them (the child resets torchrun's OMP_NUM_THREADS=1)."""
     cmd = [sys.executable, os.path.join(ROOT, "oracle", "run_reference.py"), "--env", "CartPole-v1", "--envs", str(envs),
            "--T", str(T), "--epochs", str(EPOCHS), "--minibatch", str(MINIBATCH), "--iters", str(iters), "--warmup", str(warmup)]
@@ -536,7 +550,7 @@ def reference_run(envs, iters, warmup, asynchronous=False, timeout=300):
 
 
 def reference_available():
-    return os.path.isfile(os.path.join(ROOT, "baseline", "_ref", "openrl", "__init__.py"))
+    return os.path.isfile(os.path.join(ROOT, "oracle", "_ref", "openrl", "__init__.py"))
 
 
 REF_ENVS = 128   # north_star's target point; the reference's per-env Python loop makes cost linear in envs
@@ -569,7 +583,7 @@ def run_reference(args):
             extra["c1"] = {"error": str(e)[-300:]}
         extra["not_run"] = "AsyncVectorEnv at 4096 envs = 4097 processes: infeasible on this host; Sync at 4096 envs is ~30 s/iteration"
         cores, sample = sync["torch_threads"], (f"each step = one PPOAgent.train iteration of {REF_ENVS} of the {N_ENVS} envs x T={T}, {EPOCHS} epochs, "
-                                                 f"unmodified reference (baseline/_ref) + SyncVectorEnv, {sync['host_cores']} host cores")
+                                                 f"unmodified reference (oracle/_ref) + SyncVectorEnv, {sync['host_cores']} host cores")
         dt = sync["seconds"]
     else:
         from oracle import loop as oloop
@@ -584,7 +598,7 @@ def run_reference(args):
         for _ in range(steps):
             tr.iteration()
         dt = time.perf_counter() - t0
-        value, kind, cores, extra = n_envs * T * steps / dt, "port", threads, {"note": "baseline/_ref missing: oracle port timed instead"}
+        value, kind, cores, extra = n_envs * T * steps / dt, "port", threads, {"note": "oracle/_ref missing: oracle port timed instead"}
         sample = f"each step = one iteration of {n_envs} of the {N_ENVS} envs x T={T}, {EPOCHS} epochs (oracle/loop.py)"
     cb = {"value": value, "unit": "env-steps/s", "cores": cores, "kind": kind, "sample": sample}
     print(json.dumps({**base, "value": value, "ms_per_step": dt / steps * 1e3, "cpu_baseline": cb, "reference_runs": extra,
@@ -600,6 +614,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true", help="development: skip the cpu_baseline leg")
     ap.add_argument("--no-extras", action="store_true", help="skip the extras block (other configs / modes)")
     ap.add_argument("--only-extra", default="", help="development: comma-separated names of the extras to run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step (parameters, losses, rollout buffer) to DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * openrl_b200.h — C-ABI of libopenrl_b200.so (hand-written sm_100a CUDA).
+ * openrl_b200.h — C-ABI of libopenrl_b200.so (hand-written sm_90a CUDA).
  *
  * Drop-in boundary for OpenRL's rollout-collection + PPO/MAPPO-update hot path.
  * The reference has no FFI: its seams are Python constructor-injection points
@@ -230,9 +230,9 @@ int orl_policy_eval(const float* policy_params, int obs_dim, int n_actions, int 
 #define ORL_PPO_A2C 256               /* A2CAlgorithm.prepare_loss (openrl/algorithms/a2c.py:39-140): policy loss
                                          -adv * log-prob instead of the clipped surrogate; ratio reported as 0 */
 #define ORL_PPO_DUAL_CLIP 512         /* cfg.dual_clip_ppo: ratio = min(ratio, dual_clip_coeff) (ppo.py:304-305) */
-#define ORL_PPO_TENSORCORE 128        /* the 64x64 GEMMs of the trunk (forward, backward-data, weight gradients) on tcgen05
+#define ORL_PPO_TENSORCORE 128        /* the 64x64 GEMMs of the trunk (forward, backward-data, weight gradients) on wgmma
                                          tensor cores with split-fp16 operands (x = hi + lo, three MMA passes, FP32
-                                         accumulate in TMEM): fp32-class accuracy, same 1e-4 loss-parity bar as the FFMA
+                                         accumulate in registers): fp32-class accuracy, same 1e-4 loss-parity bar as the FFMA
                                          kernel.  Categorical heads, obs widths <= 8, |obs| < 65504.  Minibatch tiles are
                                          staged by TMA when `indices` is NULL, by cp.async gathers otherwise.
                                          Without the flag everything is fp32 FFMA. */

@@ -1,4 +1,4 @@
-"""openrl_b200 — B200-native (sm_100a) implementation of OpenRL's rollout-collection +
+"""openrl_b200 — H100-native (sm_90a) implementation of OpenRL's rollout-collection +
 PPO/MAPPO-update hot path behind OpenRL's own Python surface (`make`, `PPONet`, `PPOAgent`).
 
 Host code is Python (as the reference's is); all numeric inner loops are hand-written CUDA in

@@ -1,4 +1,4 @@
-"""In-tree nvcc build of libopenrl_b200.so for sm_100a (B200).
+"""In-tree nvcc build of libopenrl_b200.so for sm_90a (H100).
 
 `python -m openrl_b200.build` (or __graft_entry__.build()).  nvcc cross-compiles without a
 GPU; the .so is git-ignored but travels to the GPU box with the repo snapshot.
@@ -16,7 +16,7 @@ BUILD = os.path.join(CSRC, "build")
 LIB = os.path.join(CSRC, "libopenrl_b200.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-I", INCLUDE, "-I", CSRC]
 # per-file extra flags: the GAE scan must reproduce numpy's unfused float32 arithmetic
 EXTRA = {"orl_gae.cu": ["--fmad=false"]}

@@ -53,7 +53,7 @@ FLAGS = [
     ("use_attn", _bool, False), ("use_conv1d", _bool, False), ("use_influence_policy", _bool, False),
     # openrl_b200 additions (not in the reference): how sampling noise / minibatch order are drawn
     ("parity_mode", _bool, False),
-    # 64x64 trunk GEMMs of the update on tcgen05 tensor cores (split-fp16 operands, FP32 accumulate:
+    # 64x64 trunk GEMMs of the update on wgmma tensor cores (split-fp16 operands, FP32 accumulate:
     # fp32-class accuracy, so it is also the parity-mode update); Categorical heads, obs widths <= 8,
     # fp32 FFMA kernel otherwise.  `use_tf32` is the round-1 name of the same switch.
     ("use_tensor_cores", _bool, True),

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libopenrl_b200 (sm_100a only).
+// Shared device/host helpers for libopenrl_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,4 +1,4 @@
-// Forward-only passes of the 64-wide MLPs on the tensor cores (tcgen05, split-fp16 operands, fp32 accumulate —
+// Forward-only passes of the 64-wide MLPs on the tensor cores (wgmma, split-fp16 operands, fp32 accumulate —
 // the same building blocks and accuracy class as the update kernel, orl_ppo_tc.cu / orl_tc16.cuh):
 //
 //   critic_values_tc_kernel : ValueNetwork.forward over a flat batch of rows (value_network.py:113-136), the
@@ -7,9 +7,10 @@
 //                             buffer insert, onpolicy_driver.py:154-203,236-279) for single-agent device envs
 //                             (CartPole-v1, GridWorldEnv): a CTA owns 128 envs for all T steps, ONE launch.
 //
-// CTA = 256 threads = 128 rows x 2 column halves (warps w, w+4 share rows [32(w%4), +32) = their TMEM lane quadrant).
+// CTA = 256 threads = 128 rows x 2 column halves (warps w, w+4 share rows [32(w%4), +32)).
 // Per 128-row tile: fc1 (K = d <= 8, FFMA) + activation + LayerNorm-1 in registers -> n1 as fp16 hi/lo panels ->
-// Z3 = n1 . W3f^T as 12 MMAs (3 split passes x K/16) into TMEM -> LayerNorm-3 + head in registers.  The rollout's
+// Z3 = n1 . W3f^T as 12 wgmma (3 split passes x K/16; warpgroup g computes rows [64g, +64)) -> fp32 staging tile in
+// shared memory -> every thread reads its row's columns -> LayerNorm-3 + head in registers.  The rollout's
 // per-step critical path is one row's work (no shared-memory GEMM, no cross-row shuffles): ~1/3 of the FFMA kernel's.
 #include <algorithm>
 #include <cstdlib>
@@ -25,11 +26,14 @@ using namespace orl::tc;
 
 constexpr int F_M = 128, F_NT = 256, FCW = 32;
 constexpr uint32_t FPANEL = F_M * 16, FPANEL_W = H * 16;
-constexpr uint32_t FOFF_R1H = 0, FOFF_R1L = 8 * FPANEL, FOFF_WH = 16 * FPANEL, FOFF_WL = FOFF_WH + 8 * FPANEL_W, FOFF_SMALL = FOFF_WL + 8 * FPANEL_W;
-// fp32: w1t[8][64] b1[64] b3f[64] whf[8][64] bhf[8] | xs[2][128][2] xh[8][2][128] xst[128][8] | mbarrier, tmem holder
+// Z3 staging tile: 128 rows x 64 fp32, row pitch 68 floats (row-per-thread float4 reads are conflict-free)
+constexpr int S_LD = 68;
+constexpr uint32_t FOFF_R1H = 0, FOFF_R1L = 8 * FPANEL, FOFF_WH = 16 * FPANEL, FOFF_WL = FOFF_WH + 8 * FPANEL_W, FOFF_S = FOFF_WL + 8 * FPANEL_W,
+                   FOFF_SMALL = FOFF_S + F_M * S_LD * 4;
+// fp32: w1t[8][64] b1[64] b3f[64] whf[8][64] bhf[8] | xs[2][128][2] xh[8][2][128] xst[128][8]
 constexpr uint32_t F_SMALL_FLOATS = 8 * H + H + H + MAX_OUT * H + MAX_OUT;
 constexpr uint32_t F_XCH_FLOATS = 2 * F_M * 2 + 2 * F_M * 8 + F_M * 8;
-constexpr uint32_t F_SMEM = FOFF_SMALL + 4 * (F_SMALL_FLOATS + F_XCH_FLOATS) + 16 + 16;
+constexpr uint32_t F_SMEM = FOFF_SMALL + 4 * (F_SMALL_FLOATS + F_XCH_FLOATS);
 
 #define F_FOR_OUT(j) _Pragma("unroll") for (int j = 0; j < NOUT; ++j) if (NOUT != 8 || j < n)
 #define F_ROWGROUP_SYNC()                                                      \
@@ -47,24 +51,20 @@ __device__ __forceinline__ float f_act(float z, int activation_id) { return ACT 
 
 struct FwdCtx {
     uint8_t *R1h, *R1l;
-    float *w1t, *b1s, *b3f, *whf, *bhf, *xs, *xh, *xst;
-    uint64_t* bar;
-    uint32_t tmem, aR1h, aR1l, aWh, aWl;
+    float *S, *w1t, *b1s, *b3f, *whf, *bhf, *xs, *xh, *xst;
+    uint32_t aR1h, aR1l, aWh, aWl;
 };
 
-// carve shared memory, stage + fold the weights (fc3 matrix as split fp16), allocate 64 TMEM columns; ends with a CTA barrier.
-// XCH_BYTES = size of the exchange area that follows the small fp32 weights (the mbarrier and the TMEM holder come after it)
-template <uint32_t XCH_BYTES = 4 * F_XCH_FLOATS>
+// carve shared memory, stage + fold the weights (fc3 matrix as split fp16); ends with a CTA barrier.
 __device__ __forceinline__ FwdCtx fwd_setup(uint8_t* smem, const float* __restrict__ params, int d, int n) {
-    const int tid = threadIdx.x, warp = tid >> 5, nt = blockDim.x;
+    const int tid = threadIdx.x, nt = blockDim.x;
     FwdCtx c;
     c.R1h = smem + FOFF_R1H; c.R1l = smem + FOFF_R1L;
     uint8_t* Wh = smem + FOFF_WH; uint8_t* Wl = smem + FOFF_WL;
+    c.S = reinterpret_cast<float*>(smem + FOFF_S);
     c.w1t = reinterpret_cast<float*>(smem + FOFF_SMALL);
     c.b1s = c.w1t + 8 * H; c.b3f = c.b1s + H; c.whf = c.b3f + H; c.bhf = c.whf + MAX_OUT * H;
     c.xs = c.bhf + MAX_OUT; c.xh = c.xs + 2 * F_M * 2; c.xst = c.xh + 2 * F_M * 8;   // the 2-half layout of the exchange area
-    c.bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(c.xs) + XCH_BYTES);
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(c.bar + 2);
     const NetOffsets po = net_offsets(d, n);
     for (int i = tid; i < 8 * H; i += nt) { const int k = i / H, j = i % H; c.w1t[i] = (k < d) ? params[po.w1 + j * d + k] : 0.f; }
     for (int i = tid; i < H; i += nt) c.b1s[i] = params[po.b1 + i];
@@ -87,23 +87,18 @@ __device__ __forceinline__ FwdCtx fwd_setup(uint8_t* smem, const float* __restri
         if (j < n) { s = params[po.bh + j]; for (int k = 0; k < H; ++k) s = fmaf(params[po.wh + j * H + k], params[po.be3 + k], s); }
         c.bhf[j] = s;
     }
-    if (tid == 0) mbar_init(c.bar, 1);
-    if (warp == 0) tmem_alloc(tmem_holder, 64);
     fence_proxy_async();
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    c.tmem = *tmem_holder;
     c.aR1h = smem_u32(c.R1h); c.aR1l = smem_u32(c.R1l); c.aWh = smem_u32(Wh); c.aWl = smem_u32(Wl);
     return c;
 }
 
 // One 128-row tile forward: x (this thread's row, zero padded) -> out[j] = head(j) incl. the folded bias, valid in
-// BOTH column halves of the row.  `par` = parity of the tile counter (the MMA mbarrier completes once per tile).
+// BOTH column halves of the row.
 // `overlap()` runs between the MMA issue and the wait for its completion: work that does not depend on this tile's
-// result (the rollout's speculative env step and sampling noise) hides in the tensor-core latency.
+// result (the rollout's sampling noise) hides in the tensor-core latency.
 template <int NOUT, int ACT, typename Overlap>
-__device__ __forceinline__ void fwd_tile(const FwdCtx& c, const float (&x)[8], int d, int n, int activation_id, uint32_t par,
+__device__ __forceinline__ void fwd_tile(const FwdCtx& c, const float (&x)[8], int d, int n, int activation_id,
                                          float (&out)[MAX_OUT], Overlap&& overlap) {
     const int tid = threadIdx.x, warp = tid >> 5, row = tid & 127, half = tid >> 7, cb = FCW * half;
     float n1[FCW];
@@ -142,27 +137,32 @@ __device__ __forceinline__ void fwd_tile(const FwdCtx& c, const float (&x)[8], i
         split_store8(c.R1h + off, c.R1l + off, n1 + q8, 1.0f);
     }
     fence_proxy_async();
-    tcgen05_fence_before();
     __syncthreads();
-    if (warp == 0 && elect_one()) {   // Z3 = n1 . W3f^T
-        tcgen05_fence_after();
+    {   // Z3 = n1 . W3f^T: warpgroup `half` computes rows [64 half, +64)
         const uint64_t dK_A = desc_const(FPANEL, 128), dK_W = desc_const(FPANEL_W, 128);
-        const uint32_t idesc = make_idesc_f16(128, 64, false, false);
-#pragma unroll 1
+        float z[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) z[i] = 0.f;
+        wgmma_fence();
+#pragma unroll
         for (int pass = 0; pass < 3; ++pass) {
-            const uint32_t aa = pass == 0 ? c.aR1l : c.aR1h, bb = pass == 1 ? c.aWl : c.aWh;
-#pragma unroll 1
+            const uint32_t aa = (pass == 0 ? c.aR1l : c.aR1h) + half * 64 * 16, bb = pass == 1 ? c.aWl : c.aWh;
+#pragma unroll
             for (int kk = 0; kk < 4; ++kk)
-                mma_f16(c.tmem, desc_at(dK_A, aa + 2 * kk * FPANEL), desc_at(dK_W, bb + 2 * kk * FPANEL_W), idesc, (pass | kk) > 0);
+                wgmma_f16_n64<0, 0>(z, desc_at(dK_A, aa + 2 * kk * FPANEL), desc_at(dK_W, bb + 2 * kk * FPANEL_W), (pass | kk) > 0);
         }
-        mma_commit(c.bar);
+        wgmma_commit();
+        overlap();
+        wgmma_wait0();
+        frag_store<64>(z, c.S + half * 64 * S_LD, S_LD);
     }
-    overlap();
-    mbar_wait(c.bar, par);
-    tcgen05_fence_after();
+    __syncthreads();   // the staging tile is complete; the next tile's stores follow its CTA barrier in front of the MMAs
     float n3[FCW];
-    tmem_ld_row32(c.tmem + ((uint32_t)((warp & 3) * 32) << 16) + cb, n3);
-    tcgen05_fence_before();   // the next tile's MMA (after the next CTA barrier) overwrites these columns
+#pragma unroll
+    for (int q4 = 0; q4 < FCW; q4 += 4) {
+        const float4 v = *reinterpret_cast<const float4*>(c.S + row * S_LD + cb + q4);
+        n3[q4] = v.x; n3[q4 + 1] = v.y; n3[q4 + 2] = v.z; n3[q4 + 3] = v.w;
+    }
     float s3 = 0.f, q3 = 0.f;
 #pragma unroll
     for (int i = 0; i < FCW; ++i) { n3[i] += c.b3f[cb + i]; s3 += n3[i]; q3 = fmaf(n3[i], n3[i], q3); }
@@ -206,22 +206,18 @@ __global__ void __launch_bounds__(F_NT, 2) critic_values_tc_kernel(const float* 
     const FwdCtx c = fwd_setup(smem_f, params, d, 1);
     const int tid = threadIdx.x, warp = tid >> 5, row = tid & 127, half = tid >> 7;
     const long long n_tiles = (rows + F_M - 1) / F_M;
-    uint32_t it = 0;
-    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const long long r = tile * F_M + row;
         float x[8];
 #pragma unroll
         for (int k = 0; k < 8; ++k) x[k] = (r < rows && k < d) ? obs[r * d + k] : 0.f;
         float out[MAX_OUT];
-        fwd_tile<1, ACT>(c, x, d, 1, activation_id, it & 1u, out, [] {});
+        fwd_tile<1, ACT>(c, x, d, 1, activation_id, out, [] {});
         if (half == 0 && r < rows) values[r] = out[0];
         // the exchange slots are reused by the next tile: its first write follows this row group's last read only
         // through the barriers inside fwd_tile of the NEXT tile -> order them here
         F_ROWGROUP_SYNC();
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(c.tmem, 64);
 }
 
 // Categorical sampling of one row from its logits (rollout tail, half 0): masks, log-softmax, argmax / multinomial rule
@@ -280,13 +276,12 @@ __global__ void __launch_bounds__(F_NT, 1) rollout_tc_kernel(const OrlRolloutArg
     float x[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) x[k] = (valid && k < d) ? a.policy_obs[((size_t)a.t_begin * B + e) * d + k] : 0.f;
-    uint32_t it = 0;
     {
-        for (int t = a.t_begin; t < a.t_end; ++t, ++it) {
+        for (int t = a.t_begin; t < a.t_end; ++t) {
             float logit[MAX_OUT];
             float q[MAX_OUT];
             const size_t grow = (size_t)t * B + (valid ? e : 0);
-            fwd_tile<NOUT, ACT>(c, x, d, n, a.activation_id, it & 1u, logit, [&] {
+            fwd_tile<NOUT, ACT>(c, x, d, n, a.activation_id, logit, [&] {
                 if (half == 0 && valid && !a.deterministic) row_noise<NOUT>(a, n, grow, rng_base + (uint64_t)t, e, q);
             });
             if (half == 0 && valid) {
@@ -313,18 +308,16 @@ __global__ void __launch_bounds__(F_NT, 1) rollout_tc_kernel(const OrlRolloutArg
             }
         }
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(c.tmem, 64);
 }
 
 
 // ---- CartPole rollout: 4 forward threads + 2 env threads per row -----------------------------------------------------
-// The rollout is a chain of T dependent steps whose length is one row's work.  Measured (ncu, profiles/r2_ncu_summary.md):
-// the f64 CartPole physics (sin / cos and three dependent divides: ~250 dependent instructions at ~12 cycles each) is
-// ~3000 of the ~7000 cycles of a step when it runs after sampling, the policy forward ~4000.  So:
-//   * CTA = 768 threads = 128 rows x 6 groups.  Groups 0-3 (warps w, w+4, w+8, w+12 share rows [32(w%4), +32) = their TMEM
-//     lane quadrant) are the column quarters of the policy forward: quarter qd owns hidden columns [16 qd, +16).
+// The rollout is a chain of T dependent steps whose length is one row's work.  The f64 CartPole physics (sin / cos and
+// three dependent divides: ~250 dependent instructions) is a large share of a step when it runs after sampling, the
+// policy forward most of the rest.  So:
+//   * CTA = 768 threads = 128 rows x 6 groups.  Groups 0-3 (warps w, w+4, w+8, w+12 share rows [32(w%4), +32)) are the
+//     column quarters of the policy forward: quarter qd owns hidden columns [16 qd, +16).  They are also the four
+//     warpgroups of the fc3 GEMM: warpgroup g computes rows [64 (g % 2), +64) x columns [32 (g / 2), +32) of Z3.
 //   * Groups 4 and 5 are the env.  As soon as the state of step t is known, group 4 advances the physics for action 0 and
 //     draws the reset state (PCG64), group 5 advances the physics for action 1 and draws the sampling noise of step t+1 -
 //     concurrently with the whole forward pass of step t - and publish the candidates through (parity double-buffered)
@@ -337,7 +330,7 @@ constexpr int Q_NT = 768, Q_FWD = 512, QCW = 16;
 constexpr uint32_t Q_XCH_FLOATS = 4 * F_M * 2 + MAX_OUT * 4 * F_M + 2 * MAX_OUT * F_M + 2 * F_M + 4 * F_M;
 constexpr uint32_t Q_F64 = 2 * (2 * 4 + 4) * F_M;
 constexpr uint32_t Q_XCH_BYTES = 4 * Q_XCH_FLOATS + 8 * Q_F64;
-constexpr uint32_t Q_SMEM = FOFF_SMALL + 4 * F_SMALL_FLOATS + Q_XCH_BYTES + 16 + 16;
+constexpr uint32_t Q_SMEM = FOFF_SMALL + 4 * F_SMALL_FLOATS + Q_XCH_BYTES;
 static_assert((FOFF_SMALL + 4 * F_SMALL_FLOATS + 4 * Q_XCH_FLOATS) % 8 == 0, "f64 exchange area must be 8-byte aligned");
 
 // named barriers: 1-4 = the 4 forward warps of a row group (128 threads), 5-8 = those + the row group's two env warps
@@ -352,7 +345,7 @@ __global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlR
     extern __shared__ __align__(1024) uint8_t smem_f[];
     const int N = a.n_envs, B = N, d = 4;
     const int n = NOUT == 8 ? a.n_actions : NOUT;
-    const FwdCtx c = fwd_setup<Q_XCH_BYTES>(smem_f, a.policy_params, d, n);
+    const FwdCtx c = fwd_setup(smem_f, a.policy_params, d, n);
     const int tid = threadIdx.x, warp = tid >> 5, row = tid & 127, qd = tid >> 7, cb = QCW * (qd & 3);
     float* xs = c.xs;                                   // [4][128][2]
     float* xh = xs + 4 * F_M * 2;                       // [8][4][128]
@@ -427,7 +420,6 @@ __global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlR
         float x[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) x[k] = valid ? a.policy_obs[((size_t)a.t_begin * B + e) * 4 + k] : 0.f;
-        const uint32_t tmem_row = c.tmem + ((uint32_t)((warp & 3) * 32) << 16);
         Q_PUBLISH_SYNC();   // the first step's noise is in place
         for (int t = a.t_begin; t < a.t_end; ++t, ++it) {
             const uint32_t pb = it & 1u;
@@ -468,26 +460,32 @@ __global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlR
                 split_store8(c.R1h + off, c.R1l + off, n1 + q8, 1.0f);
             }
             fence_proxy_async();
-            tcgen05_fence_before();
             Q_FWD_SYNC();
-            if (warp == 0 && elect_one()) {   // Z3 = n1 . W3f^T
-                tcgen05_fence_after();
+            {   // Z3 = n1 . W3f^T: warpgroup qd computes rows [64 (qd & 1), +64) x columns [32 (qd >> 1), +32)
                 const uint64_t dK_A = desc_const(FPANEL, 128), dK_W = desc_const(FPANEL_W, 128);
-                const uint32_t idesc = make_idesc_f16(128, 64, false, false);
-#pragma unroll 1
+                const int mb = qd & 1, nb = qd >> 1;
+                float z[16];
+#pragma unroll
+                for (int i = 0; i < 16; ++i) z[i] = 0.f;
+                wgmma_fence();
+#pragma unroll
                 for (int pass = 0; pass < 3; ++pass) {
-                    const uint32_t aa = pass == 0 ? c.aR1l : c.aR1h, bb = pass == 1 ? c.aWl : c.aWh;
-#pragma unroll 1
+                    const uint32_t aa = (pass == 0 ? c.aR1l : c.aR1h) + mb * 64 * 16, bb = (pass == 1 ? c.aWl : c.aWh) + nb * 32 * 16;
+#pragma unroll
                     for (int kk = 0; kk < 4; ++kk)
-                        mma_f16(c.tmem, desc_at(dK_A, aa + 2 * kk * FPANEL), desc_at(dK_W, bb + 2 * kk * FPANEL_W), idesc, (pass | kk) > 0);
+                        wgmma_f16_n32<0, 0>(z, desc_at(dK_A, aa + 2 * kk * FPANEL), desc_at(dK_W, bb + 2 * kk * FPANEL_W), (pass | kk) > 0);
                 }
-                mma_commit(c.bar);
+                wgmma_commit();
+                wgmma_wait0();
+                frag_store<32>(z, c.S + mb * 64 * S_LD + 32 * nb, S_LD);
             }
-            mbar_wait(c.bar, pb);
-            tcgen05_fence_after();
+            Q_FWD_SYNC();   // the staging tile is complete; the next step's stores follow its forward barrier in front of the MMAs
             float n3[QCW];
-            tmem_ld_row16(tmem_row + cb, n3);
-            tcgen05_fence_before();   // the next step's MMA (after the next forward barrier) overwrites these columns
+#pragma unroll
+            for (int q4 = 0; q4 < QCW; q4 += 4) {
+                const float4 v = *reinterpret_cast<const float4*>(c.S + row * S_LD + cb + q4);
+                n3[q4] = v.x; n3[q4 + 1] = v.y; n3[q4 + 2] = v.z; n3[q4 + 3] = v.w;
+            }
             float s3 = 0.f, q3 = 0.f;
 #pragma unroll
             for (int i = 0; i < QCW; ++i) { n3[i] += c.b3f[cb + i]; s3 += n3[i]; q3 = fmaf(n3[i], n3[i], q3); }
@@ -561,9 +559,6 @@ __global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlR
         }
         if (valid && qd == 0) { a.ep_return[e] = ret; a.ep_length[e] = len; }
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(c.tmem, 64);
 }
 
 template <typename K>

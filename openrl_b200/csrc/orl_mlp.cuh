@@ -1,4 +1,4 @@
-// Tile primitives for the 64-wide policy / value MLPs of the PPO hot path (sm_100a, fp32 FFMA).
+// Tile primitives for the 64-wide policy / value MLPs of the PPO hot path (sm_90a, fp32 FFMA).
 //
 // Network (reference: MLPBase/MLPLayer openrl/modules/networks/utils/mlp.py:8-46,100-176 with
 // layer_N == 1, hidden 64; heads openrl/modules/networks/utils/act.py, value_network.py:106-109):

@@ -372,7 +372,7 @@ __global__ void __launch_bounds__(P_NT, 1) ppo_fwdbwd_kernel(const OrlPpoArgs a)
 
 // Sum over the G partial rows of one net for 32 consecutive bucket elements per CTA (8 warps): warp w adds rows
 // w, w+8, ... (coalesced 128-byte loads, 8 independent loads in flight per thread), the 8 partial sums are combined in
-// warp order -> a fixed summation order (deterministic), ~2 us instead of ~12 us for the G = 148 sequential loads per thread.
+// warp order -> a fixed summation order (deterministic), ~2 us instead of ~12 us for the G = 132 sequential loads per thread.
 constexpr int RED_W = 8, RED_NT = 32 * RED_W;
 __device__ __forceinline__ float reduce_partials(const float* __restrict__ partials, int net, int G, int stride, int el,
                                                  float (*part)[32]) {

@@ -1,14 +1,14 @@
-// PPO minibatch forward+backward on the 5th-gen tensor cores (tcgen05, split-fp16 operands, FP32
-// accumulate in TMEM) — produces the same folded partial gradients and loss sums as ppo_fwdbwd_kernel
+// PPO minibatch forward+backward on the Hopper tensor cores (wgmma, split-fp16 operands, FP32
+// accumulate) — produces the same folded partial gradients and loss sums as ppo_fwdbwd_kernel
 // (orl_ppo.cu) at fp32-class accuracy (orl_tc16.cuh).  Selected with ORL_PPO_TENSORCORE; categorical
 // heads, obs widths <= 8 (CartPole, GridWorld).  Reference: openrl/algorithms/ppo.py:46-361.
 //
-// CTA = 256 threads = 128 tile rows x 2 column halves, TWO CTAs per SM (<= 113 KB shared memory, 256
-// TMEM columns each): warps w and w+4 own the same 32 rows (TMEM lane quadrant w%4) and 32 columns
-// each, so every row-wise operation (fc1 with K = d <= 8, LayerNorm forward/backward, head, loss) is
-// thread-local apart from three two-float exchanges and one head exchange through shared memory
-// (named barriers per row group).  While one CTA waits on its MMAs or barriers the other CTA of the
-// SM issues — the inter-tile overlap is done by the hardware CTA scheduler.
+// CTA = 256 threads = 128 tile rows x 2 column halves = 2 warpgroups, one CTA per SM (~147 KB shared
+// memory): warps w and w+4 own the same 32 rows and 32 columns each, so every row-wise operation (fc1
+// with K = d <= 8, LayerNorm forward/backward, head, loss) is thread-local apart from three two-float
+// exchanges and one head exchange through shared memory (named barriers per row group).  The per-tile
+// GEMM results (Z3, dN1) arrive in the warpgroups' accumulator registers in the wgmma fragment layout
+// and reach the row-owning threads through an fp32 staging tile in shared memory.
 //
 // All matrix operands live in row-major panel buffers (orl_tc16.cuh) as fp16 hi/lo pairs, written by
 // the row-owning threads with 16-byte stores and read K-major or MN-major by descriptor only:
@@ -18,11 +18,11 @@
 // Four GEMMs per 128-row tile, each as three MMA passes (Al.Bh, Ah.Bl, Ah.Bh), issued by one thread:
 //   GEMM1  Z3 [128x64]  = n1 . W3f^T                 A = R1 K-major,  B = W K-major     (fwd fc3)
 //   GEMM2  dN1[128x64]  = dZ3 . W3f                  A = R2 K-major,  B = W MN-major    (bwd-data fc3)
-//   GEMM3a Ga [128x80] += R2^T . R1                  both MN-major, K = 128 tile rows:
+//   GEMM3a Ga [128x80] += R2^T . R1                  both MN-major, K = 128 tile rows (warpgroup g: rows [64g, +64)):
 //            lanes 0..63  : G3 = dZ3^T n1 (cols 0..63), db3 (col 64 = the ones column)
 //            lanes 64..71 : Q = U^T n1, su = U^T 1, smu = U^T mu3, sdl = U^T std3  (-> GH, dbh, below)
-//   GEMM3b Gb [128x16] += dZ1^T . [CST | X]          both MN-major: db1 (col 0), G1 = dZ1^T X (cols 8..15)
-// Ga / Gb stay in TMEM for the whole kernel.  GH = dL^T n3 needs no n3 tile: with n3 = (Z3 + b3f - mu3) rstd3
+//   GEMM3b Gb [64x16]  += dZ1^T . [CST | X]          both MN-major: db1 (col 0), G1 = dZ1^T X (cols 8..15); warpgroup 1
+// Ga / Gb stay in accumulator registers for the whole kernel.  GH = dL^T n3 needs no n3 tile: with n3 = (Z3 + b3f - mu3) rstd3
 // and Z3 = n1 W3f^T,   GH[j][k] = sum_i Q[j][i] W3f[k][i] + b3f[k] su[j] - smu[j]   (evaluated once at the end).
 // fp16 carries 22 significand bits as hi + lo only while hi >= 2^-3 (below, lo is subnormal), so every backward
 // operand is scaled by a power of two chosen per minibatch to put its TYPICAL magnitude near 2^4: dZ3 / dZ1 by
@@ -58,10 +58,14 @@ constexpr uint32_t PANEL_W = H * 16;
 constexpr int R1_PANELS = 10, R2_PANELS = 9;
 constexpr int P_CST = 8, P_X = 9, P_U = 8;
 constexpr int N_LOSS_TC = 8;
+// staging tile of the per-tile GEMM results: 128 rows x 64 fp32, row pitch 68 floats (conflict-free row reads);
+// the final Ga [128][GA_LD] / Gb [64][GB_LD] staging reuses R1 / R2
+constexpr int S_LD = 68, GA_LD = 84, GB_LD = 20;
 // shared-memory carve-up (bytes)
 constexpr uint32_t OFF_R1H = 0, OFF_R1L = OFF_R1H + R1_PANELS * PANEL, OFF_R2H = OFF_R1L + R1_PANELS * PANEL,
                    OFF_R2L = OFF_R2H + R2_PANELS * PANEL, OFF_WH = OFF_R2L + R2_PANELS * PANEL, OFF_WL = OFF_WH + 8 * PANEL_W,
-                   OFF_STAGE = OFF_WL + 8 * PANEL_W;
+                   OFF_S = OFF_WL + 8 * PANEL_W, OFF_STAGE = OFF_S + T_M * S_LD * 4;
+static_assert((T_M * GA_LD + 64 * GB_LD) * 4 <= OFF_WH, "the Ga / Gb staging fits in R1 + R2");
 static_assert(OFF_STAGE % 128 == 0, "TMA destination alignment");
 static_assert(OFF_R2L + 16 * PANEL <= OFF_STAGE + 4096, "the 16-panel A descriptors stay inside the allocation");
 constexpr int N_SCAL = 4;                      // scalar columns staged per row
@@ -86,10 +90,10 @@ struct AdvNormTc { float m0, s0, m1, s1; bool two; };
 
 __host__ __device__ inline uint32_t tc_stage_bytes(int d) { return (uint32_t)((T_M * d * 4 + 127) & ~127) + N_SCAL * T_M * 4; }
 __host__ __device__ inline uint32_t tc_small_off(int d) { return OFF_STAGE + tc_stage_bytes(d); }
-// fp32 weights: w1t[8][64] b1[64] b3f[64] whf[8][64] bhf[8] swh[8]; exchange: xs[2][128][2] xh[8][2][128]; 5 mbarriers + tmem holder
+// fp32 weights: w1t[8][64] b1[64] b3f[64] whf[8][64] bhf[8] swh[8]; exchange: xs[2][128][2] xh[8][2][128]; staging mbarrier
 constexpr uint32_t SMALL_FLOATS = 8 * H + H + H + MAX_OUT * H + 2 * MAX_OUT;
 constexpr uint32_t XCH_FLOATS = 2 * T_M * 2 + 2 * T_M * 8;
-__host__ __device__ inline uint32_t tc_smem_bytes(int d) { return tc_small_off(d) + 4 * (SMALL_FLOATS + XCH_FLOATS) + 5 * 8 + 16; }
+__host__ __device__ inline uint32_t tc_smem_bytes(int d) { return tc_small_off(d) + 4 * (SMALL_FLOATS + XCH_FLOATS) + 8; }
 
 // ACT == 1: ReLU (the reference's default activation_id) compiled in; ACT == -1: runtime activation_id (tanh / leaky / elu
 // expand to ~60 instructions per element, which the fully unrolled row code cannot afford in the instruction cache)
@@ -105,13 +109,14 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     const float* params = POLICY ? a.policy_params : a.critic_params;
     const float* obs = POLICY ? a.policy_obs : a.critic_obs;
     const int tid = threadIdx.x, warp = tid >> 5;
-    const int row = tid & 127, half = tid >> 7;   // this thread: tile row, column half
+    const int row = tid & 127, half = tid >> 7;   // this thread: tile row, column half (= its warpgroup)
     const int cb = CW * half;                     // first column of the half
     const NetOffsets po = net_offsets(d, n);
 
     uint8_t* R1h = smem + OFF_R1H; uint8_t* R1l = smem + OFF_R1L;
     uint8_t* R2h = smem + OFF_R2H; uint8_t* R2l = smem + OFF_R2L;
     uint8_t* Wh = smem + OFF_WH;   uint8_t* Wl = smem + OFF_WL;
+    float* S = reinterpret_cast<float*>(smem + OFF_S);                                  // [128][S_LD]
     float* st_obs = reinterpret_cast<float*>(smem + OFF_STAGE);                        // [128][d]
     float* st_sc = reinterpret_cast<float*>(smem + OFF_STAGE + ((T_M * d * 4 + 127) & ~127));   // [4][128]
     float* w1t = reinterpret_cast<float*>(smem + tc_small_off(d));   // [8][64] k-major, zero padded
@@ -122,8 +127,7 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     float* swh = bhf + MAX_OUT;                  // [8] row sums of whf
     float* xs = swh + MAX_OUT;                   // [2][128][2] statistics exchange
     float* xh = xs + 2 * T_M * 2;                // [2][128][8] head exchange (flush scratch afterwards)
-    uint64_t* bars = reinterpret_cast<uint64_t*>(xh + 2 * T_M * 8);  // 0..3 MMA groups, 4 staging
-    uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 5);
+    uint64_t* bar_st = reinterpret_cast<uint64_t*>(xh + 2 * T_M * 8);  // TMA staging
 
     // ---- stage weights (folded); the fc3 matrix as split fp16 ----
     for (int i = tid; i < 8 * H; i += T_NT) { const int k = i / H, j = i % H; w1t[i] = (k < d) ? params[po.w1 + j * d + k] : 0.f; }
@@ -157,18 +161,15 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         *reinterpret_cast<uint4*>(R1h + P_X * PANEL + row * 16) = z;   *reinterpret_cast<uint4*>(R1l + P_X * PANEL + row * 16) = z;
         *reinterpret_cast<uint4*>(R2h + P_U * PANEL + row * 16) = z;   *reinterpret_cast<uint4*>(R2l + P_U * PANEL + row * 16) = z;
     }
-    if (tid == 0) {
-#pragma unroll
-        for (int i = 0; i < 5; ++i) mbar_init(&bars[i], 1);
-    }
-    if (warp == 0) tmem_alloc(tmem_holder, 256);
+    if (tid == 0) mbar_init(bar_st, 1);
     fence_proxy_async();
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem = *tmem_holder;
-    const uint32_t tmem_row = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-    constexpr uint32_t TM_Z = 0, TM_GA = 64, TM_GB = 144;
+    // weight-gradient accumulators for the whole kernel: Ga rows [64 half, +64), Gb (warpgroup 1)
+    float ga[40], gb[8];
+#pragma unroll
+    for (int i = 0; i < 40; ++i) ga[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) gb[i] = 0.f;
 
     // ---- minibatch constants ----
     const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS, val_masks = a.flags & ORL_PPO_VALUE_ACTIVE_MASKS;
@@ -213,8 +214,6 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     // ---- MMA descriptors (constant parts) ----
     const uint64_t dK_A = desc_const(PANEL, 128), dK_W = desc_const(PANEL_W, 128);      // K-major
     const uint64_t dMN_A = desc_const(128, PANEL), dMN_W = desc_const(128, PANEL_W);    // MN-major
-    const uint32_t id_g1 = make_idesc_f16(128, 64, false, false), id_g2 = make_idesc_f16(128, 64, false, true);
-    const uint32_t id_3a = make_idesc_f16(128, 80, true, true), id_3b = make_idesc_f16(128, 16, true, true);
     const uint32_t aR1h = smem_u32(R1h), aR1l = smem_u32(R1l), aR2h = smem_u32(R2h), aR2l = smem_u32(R2l), aWh = smem_u32(Wh), aWl = smem_u32(Wl);
 
     // ---- staging of the minibatch rows, one tile ahead ----
@@ -225,12 +224,12 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     const uint32_t stage_tx = (uint32_t)(T_M * d * 4) + (POLICY ? 4u : 3u) * T_M * 4;
     auto issue_tma = [&](long long tile) {   // one thread
         const int r0 = (int)(a.row_begin + tile * T_M);
-        mbar_expect_tx(&bars[4], stage_tx);
-        tma_load_2d(st_obs, POLICY ? &maps.obs_p : &maps.obs_c, 0, r0, &bars[4]);
-        tma_load_1d(st_sc + 0 * T_M, POLICY ? &maps.actions : &maps.value_preds, r0, &bars[4]);
-        tma_load_1d(st_sc + 1 * T_M, POLICY ? &maps.old_logp : &maps.returns, r0, &bars[4]);
-        if (POLICY) tma_load_1d(st_sc + 2 * T_M, &maps.adv, r0, &bars[4]);
-        tma_load_1d(st_sc + 3 * T_M, &maps.active, r0, &bars[4]);
+        mbar_expect_tx(bar_st, stage_tx);
+        tma_load_2d(st_obs, POLICY ? &maps.obs_p : &maps.obs_c, 0, r0, bar_st);
+        tma_load_1d(st_sc + 0 * T_M, POLICY ? &maps.actions : &maps.value_preds, r0, bar_st);
+        tma_load_1d(st_sc + 1 * T_M, POLICY ? &maps.old_logp : &maps.returns, r0, bar_st);
+        if (POLICY) tma_load_1d(st_sc + 2 * T_M, &maps.adv, r0, bar_st);
+        tma_load_1d(st_sc + 3 * T_M, &maps.active, r0, bar_st);
     };
     auto issue_gather = [&](long long gi) {   // every thread: half 0 the observation row, half 1 the scalars
         const bool v = gi >= 0;
@@ -269,7 +268,7 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     for (long long tile = cta; tile < n_tiles; tile += G, ++it) {
         const uint32_t par = it & 1u;
         // ---- this tile's rows from the staging buffer ----
-        if (TMA) mbar_wait(&bars[4], par);
+        if (TMA) mbar_wait(bar_st, par);
         else { cp_async_wait_all(); __syncthreads(); }
         const bool valid = gi >= 0;
         float x[8];
@@ -322,8 +321,8 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
 #pragma unroll
         for (int i = 0; i < CW; ++i) n1[i] = (n1[i] - mu1) * rstd1;
 
-        // previous tile's GEMM3b must have finished reading R1
-        if (it > 0) mbar_wait(&bars[3], (it - 1) & 1u);
+        // previous tile's GEMM3b (warpgroup 1) must have finished reading R1
+        if (it > 0) __syncthreads();
 #pragma unroll
         for (int q8 = 0; q8 < CW; q8 += 8) {
             const uint32_t off = (uint32_t)((cb + q8) >> 3) * PANEL + row * 16;
@@ -331,20 +330,20 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         }
         if (half == 0) split_store8(R1h + P_X * PANEL + row * 16, R1l + P_X * PANEL + row * 16, x, SX);
         fence_proxy_async();
-        tcgen05_fence_before();
         __syncthreads();
-        if (warp == 0 && elect_one()) {   // GEMM1: Z3 = n1 . W3f^T
-            tcgen05_fence_after();
-#pragma unroll 1
-            for (int pass = 0; pass < 3; ++pass) {
-                const uint32_t aa = pass == 0 ? aR1l : aR1h, bb = pass == 1 ? aWl : aWh;
-#pragma unroll 1
-                for (int kk = 0; kk < 4; ++kk)
-                    mma_f16(tmem + TM_Z, desc_at(dK_A, aa + 2 * kk * PANEL), desc_at(dK_W, bb + 2 * kk * PANEL_W), id_g1, (pass | kk) > 0);
-            }
-            mma_commit(&bars[0]);
-            if (TMA && tile + G < n_tiles) issue_tma(tile + G);   // the staging buffer was consumed before the barrier above
+        float z[32];   // GEMM1: Z3 = n1 . W3f^T, rows [64 half, +64)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) z[i] = 0.f;
+        wgmma_fence();
+#pragma unroll
+        for (int pass = 0; pass < 3; ++pass) {
+            const uint32_t aa = (pass == 0 ? aR1l : aR1h) + half * 64 * 16, bb = pass == 1 ? aWl : aWh;
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk)
+                wgmma_f16_n64<0, 0>(z, desc_at(dK_A, aa + 2 * kk * PANEL), desc_at(dK_W, bb + 2 * kk * PANEL_W), (pass | kk) > 0);
         }
+        wgmma_commit();
+        if (TMA && tid == 0 && tile + G < n_tiles) issue_tma(tile + G);   // the staging buffer was consumed before the barrier above
         long long gi_cur = gi;
         if (!TMA) {
             issue_gather(gi_next);
@@ -354,12 +353,17 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
             gi = row_index(tile + G);
         }
 
-        mbar_wait(&bars[0], par);
-        tcgen05_fence_after();
+        wgmma_wait0();
+        frag_store<64>(z, S + half * 64 * S_LD, S_LD);
+        __syncthreads();
 
-        // ---- Z3 (TMEM) + b3f -> LayerNorm-3 -> n3 (registers only) ----
+        // ---- Z3 (staging tile) + b3f -> LayerNorm-3 -> n3 (registers only) ----
         float n3[CW];
-        tmem_ld_row32(tmem_row + TM_Z + cb, n3);
+#pragma unroll
+        for (int q4 = 0; q4 < CW; q4 += 4) {
+            const float4 v = *reinterpret_cast<const float4*>(S + row * S_LD + cb + q4);
+            n3[q4] = v.x; n3[q4 + 1] = v.y; n3[q4 + 2] = v.z; n3[q4 + 3] = v.w;
+        }
         float s3 = 0.f, q3 = 0.f;
 #pragma unroll
         for (int i = 0; i < CW; ++i) { n3[i] += b3f[cb + i]; s3 += n3[i]; q3 = fmaf(n3[i], n3[i], q3); }
@@ -481,33 +485,37 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
             split_store8(R1h + P_CST * PANEL + row * 16, R1l + P_CST * PANEL + row * 16, c8, 1.0f);
         }
         fence_proxy_async();
-        tcgen05_fence_before();
         __syncthreads();
-        if (warp == 0 && elect_one()) {   // GEMM2: dN1 = dZ3 . W3f ; GEMM3a: Ga += R2^T . R1
-            tcgen05_fence_after();
-#pragma unroll 1
-            for (int pass = 0; pass < 3; ++pass) {
-                const uint32_t aa = pass == 0 ? aR2l : aR2h, bb = pass == 1 ? aWl : aWh;
-#pragma unroll 1
-                for (int kk = 0; kk < 4; ++kk)
-                    mma_f16(tmem + TM_Z, desc_at(dK_A, aa + 2 * kk * PANEL), desc_at(dMN_W, bb + kk * 256), id_g2, (pass | kk) > 0);
-            }
-            mma_commit(&bars[1]);
-#pragma unroll 1
-            for (int pass = 0; pass < 3; ++pass) {
-                const uint32_t aa = pass == 0 ? aR2l : aR2h, bb = pass == 1 ? aR1l : aR1h;
-#pragma unroll 1
-                for (int kk = 0; kk < 8; ++kk)
-                    mma_f16(tmem + TM_GA, desc_at(dMN_A, aa + kk * 256), desc_at(dMN_A, bb + kk * 256), id_3a, (it | pass | kk) > 0);
-            }
-            mma_commit(&bars[2]);
+        // GEMM2: dN1 = dZ3 . W3f (rows [64 half, +64)) ; GEMM3a: Ga += R2^T . R1 (rows [64 half, +64))
+#pragma unroll
+        for (int i = 0; i < 32; ++i) z[i] = 0.f;
+        wgmma_fence();
+#pragma unroll
+        for (int pass = 0; pass < 3; ++pass) {
+            const uint32_t aa = (pass == 0 ? aR2l : aR2h) + half * 64 * 16, bb = pass == 1 ? aWl : aWh;
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk)
+                wgmma_f16_n64<0, 1>(z, desc_at(dK_A, aa + 2 * kk * PANEL), desc_at(dMN_W, bb + kk * 256), (pass | kk) > 0);
         }
-        mbar_wait(&bars[1], par);
-        tcgen05_fence_after();
-        // ---- dN1 (TMEM) -> LayerNorm-1 backward -> activation backward -> dZ1 (into the n1 panels of R1) ----
+#pragma unroll
+        for (int pass = 0; pass < 3; ++pass) {
+            const uint32_t aa = (pass == 0 ? aR2l : aR2h) + half * 8 * PANEL, bb = pass == 1 ? aR1l : aR1h;
+#pragma unroll
+            for (int kk = 0; kk < 8; ++kk)
+                wgmma_f16_n80<1, 1>(ga, desc_at(dMN_A, aa + kk * 256), desc_at(dMN_A, bb + kk * 256), 1u);
+        }
+        wgmma_commit();
+        wgmma_wait0();
+        frag_store<64>(z, S + half * 64 * S_LD, S_LD);
+        __syncthreads();   // dN1 is staged, and both warpgroups' GEMM3a have finished reading n1 from R1
+        // ---- dN1 (staging tile) -> LayerNorm-1 backward -> activation backward -> dZ1 (into the n1 panels of R1) ----
         {
             float g[CW];
-            tmem_ld_row32(tmem_row + TM_Z + cb, g);
+#pragma unroll
+            for (int q4 = 0; q4 < CW; q4 += 4) {
+                const float4 v = *reinterpret_cast<const float4*>(S + row * S_LD + cb + q4);
+                g[q4] = v.x; g[q4 + 1] = v.y; g[q4 + 2] = v.z; g[q4 + 3] = v.w;
+            }
             float t1 = 0.f, t2 = 0.f;
 #pragma unroll
             for (int i = 0; i < CW; ++i) { t1 += g[i]; t2 = fmaf(g[i], n1[i], t2); }
@@ -525,7 +533,6 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
                 const float aval = fmaf(n1[i], std1, mu1);                          // activation output
                 g[i] = da * (K1 * act_bwd_t<ACT>(aval, (posmask >> i) & 1u, a.activation_id));
             }
-            mbar_wait(&bars[2], par);   // GEMM3a has finished reading n1 from R1
 #pragma unroll
             for (int q8 = 0; q8 < CW; q8 += 8) {
                 const uint32_t off = (uint32_t)((cb + q8) >> 3) * PANEL + row * 16;
@@ -533,32 +540,37 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
             }
         }
         fence_proxy_async();
-        tcgen05_fence_before();
         __syncthreads();
-        if (warp == 0 && elect_one()) {   // GEMM3b: Gb += dZ1^T . [CST | X]
-            tcgen05_fence_after();
-#pragma unroll 1
+        if (half == 1) {   // GEMM3b: Gb += dZ1^T . [CST | X]
+            wgmma_fence();
+#pragma unroll
             for (int pass = 0; pass < 3; ++pass) {
                 const uint32_t aa = pass == 0 ? aR1l : aR1h, bb = (pass == 1 ? aR1l : aR1h) + P_CST * PANEL;
-#pragma unroll 1
+#pragma unroll
                 for (int kk = 0; kk < 8; ++kk)
-                    mma_f16(tmem + TM_GB, desc_at(dMN_A, aa + kk * 256), desc_at(dMN_A, bb + kk * 256), id_3b, (it | pass | kk) > 0);
+                    wgmma_f16_n16<1, 1>(gb, desc_at(dMN_A, aa + kk * 256), desc_at(dMN_A, bb + kk * 256), 1u);
             }
-            mma_commit(&bars[3]);
+            wgmma_commit();
+            wgmma_wait0();
         }
     }
 
-    // ---- flush: Ga / Gb (TMEM) -> partial folded gradients ----
+    // ---- flush: Ga / Gb (accumulator registers -> staging in R1 / R2) -> partial folded gradients ----
     float* part = a.partials + (size_t)((POLICY ? 0 : G) + cta) * stride;
     const FoldOffsets fo = fold_offsets(d, n);
     float* qs = xh;              // [8][64] Q rows, then su[8], smu[8], sdl[8]
     float* qsu = qs + MAX_OUT * H;
     if (it > 0) {
-        mbar_wait(&bars[3], (it - 1) & 1u);
-        tcgen05_fence_after();
-        {   // Ga columns [32*half, 32*half+32) of this lane
+        float* gas = reinterpret_cast<float*>(smem);   // [128][GA_LD]
+        float* gbs = gas + T_M * GA_LD;                // [64][GB_LD]
+        __syncthreads();   // every MMA has completed: R1 / R2 are free
+        frag_store<80>(ga, gas + half * 64 * GA_LD, GA_LD);
+        if (half == 1) frag_store<16>(gb, gbs, GB_LD);
+        __syncthreads();
+        {   // Ga columns [32*half, 32*half+32) of this row
             float v[32];
-            tmem_ld_row32(tmem_row + TM_GA + 32 * half, v);
+#pragma unroll
+            for (int c = 0; c < 32; ++c) v[c] = gas[row * GA_LD + 32 * half + c];
             if (row < H) {
 #pragma unroll
                 for (int c = 0; c < 32; ++c) part[fo.g3 + row * H + 32 * half + c] = v[c] * invSz;
@@ -568,13 +580,11 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
             }
         }
         if (half == 0) {
-            float c8[8];
-            tmem_ld_row8(tmem_row + TM_GA + 64, c8);
+            const float* c8 = gas + row * GA_LD + 64;
             if (row < H) part[fo.db3 + row] = c8[0] * invSz;
             else if (row < H + n) { qsu[row - H] = c8[0]; qsu[8 + row - H] = c8[1]; qsu[16 + row - H] = c8[2]; }
-            float g16[16];
-            tmem_ld_row16(tmem_row + TM_GB, g16);
             if (row < H) {
+                const float* g16 = gbs + row * GB_LD;
                 part[fo.db1 + row] = g16[0] * invS1;
 #pragma unroll
                 for (int c = 0; c < 8; ++c) if (c < d) part[fo.g1 + row * d + c] = g16[8 + c] * (invS1 * (1.f / SX));
@@ -607,25 +617,21 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
             part[stride - N_LOSS_TC + tid] = sv;
         }
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 256);
 }
 
-// blockIdx -> (net, cta): with `pair_nets` the two CTAs that share an SM (blocks b and b + #SMs under round-robin
-// placement, #SMs even) run the SAME net, i.e. the same instruction stream (instruction-cache footprint halves);
-// otherwise CTAs [0, G) are the policy net and [G, 2G) the critic net.
+// blockIdx -> (net, cta): CTAs [0, G) are the policy net and [G, 2G) the critic net.  With one CTA per SM and
+// G = #SMs they run as two waves, the policy CTAs first.
 template <int NOUT, int ACT, bool TMA>
-__global__ void __launch_bounds__(T_NT, 2) ppo_fwdbwd_tc_kernel(const OrlPpoArgs a, const __grid_constant__ TcMaps maps, int stride, int pair_nets) {
+__global__ void __launch_bounds__(T_NT, 1) ppo_fwdbwd_tc_kernel(const OrlPpoArgs a, const __grid_constant__ TcMaps maps, int stride) {
     extern __shared__ __align__(1024) uint8_t smem_tc[];
     const int G = a.grid_per_net;
-    const bool policy = pair_nets ? ((blockIdx.x & 1) == 0) : ((int)blockIdx.x < G);
-    const int cta = pair_nets ? (int)(blockIdx.x >> 1) : ((int)blockIdx.x < G ? (int)blockIdx.x : (int)blockIdx.x - G);
+    const bool policy = (int)blockIdx.x < G;
+    const int cta = policy ? (int)blockIdx.x : (int)blockIdx.x - G;
     if (policy) tc_net_pass<true, NOUT, ACT, TMA>(a, maps, smem_tc, cta, G, stride);
     else tc_net_pass<false, 1, ACT, TMA>(a, maps, smem_tc, cta, G, stride);
 }
 
-using TcKernel = void (*)(const OrlPpoArgs, const TcMaps, int, int);
+using TcKernel = void (*)(const OrlPpoArgs, const TcMaps, int);
 template <int NOUT, int ACT>
 TcKernel pick_staging(bool tma) { return tma ? ppo_fwdbwd_tc_kernel<NOUT, ACT, true> : ppo_fwdbwd_tc_kernel<NOUT, ACT, false>; }
 template <int NOUT>
@@ -720,16 +726,15 @@ int launch_ppo_fwdbwd_tc(const OrlPpoArgs& a, cudaStream_t st) {
         static std::map<TcKernel, bool> prepared;
         std::lock_guard<std::mutex> lock(mu);
         if (!prepared.count(kern)) {
-            int e = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 116 * 1024), "cudaFuncSetAttribute(ppo_fwdbwd_tc)");
+            int e = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(8)), "cudaFuncSetAttribute(ppo_fwdbwd_tc)");
             if (e) return e;
             cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
             prepared[kern] = true;
         }
     }
-    static const int pair_nets = [] { const char* v = getenv("ORL_TC_PAIR_NETS"); return v ? atoi(v) : 0; }();
     TcMaps none;
     if (!maps) memset(&none, 0, sizeof(none));
-    kern<<<2 * a.grid_per_net, T_NT, smem, st>>>(a, maps ? *maps : none, stride, pair_nets && (a.grid_per_net % 2 == 0));
+    kern<<<2 * a.grid_per_net, T_NT, smem, st>>>(a, maps ? *maps : none, stride);
     return check_cuda(cudaGetLastError(), "ppo_fwdbwd_tc_kernel");
 }
 }  // namespace orl

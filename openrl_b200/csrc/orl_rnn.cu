@@ -606,8 +606,7 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
     const long long rows = a.n_chunks * a.chunk_length;
     const int rb = ws_row_blocks(rows);
     float* partials = a.tape + ws_tape_floats(rows);
-    // two chunks per warp: every weight read from shared memory feeds two rows (four per warp with 8 warps / CTA
-    // measured 12 % slower on B200: profiles/r1_gru_perf.md)
+    // two chunks per warp: every weight read from shared memory feeds two rows
     constexpr int C_R = 2;
     if ((e = orl::check_cuda(cudaFuncSetAttribute(tape_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TR_SMEM),
                              "smem attr (tape gemm)"))) return e;

@@ -17,7 +17,7 @@
 #define ORL_HD __host__ __device__ __forceinline__
 // The two step functions are real calls on the device (own stack frames): with everything inlined into the
 // per-chunk kernel nvcc 12.9 merged the stack slots of the caller's observation row and the callee's GRU
-// output (observed in SASS and as a corrupted tape, see profiles/r1_gru_debug.md), i.e. wrong gradients.
+// output (observed in SASS and as a corrupted tape), i.e. wrong gradients.
 #define ORL_HD_STEP __host__ __device__ __noinline__
 #else
 #define ORL_HD static inline

@@ -1,19 +1,20 @@
-// tcgen05 kind::f16 primitives for the "2 x fp16" split GEMMs of the PPO update (sm_100a), plus the
-// TMA / cp.async staging primitives.  Validated stand-alone by tools/tc_test2.cu on B200.
+// Split-fp16 operand primitives for the "2 x fp16" GEMMs of the PPO update and the forward passes (sm_90a wgmma),
+// plus the TMA / cp.async staging primitives.
 //
 // Split: x = hi + lo, hi = fp16(x), lo = fp16(x - hi)  (22 significand bits);  A.B ~= Al.Bh + Ah.Bl + Ah.Bh
-// accumulated in fp32 in TMEM — measured error on 64..256-long dot products: at or below the error of an
-// fp32 FFMA chain (tools/tc_test2.cu), i.e. the tensor-core path keeps the 1e-4 loss-parity bar.
+// accumulated in fp32: on 64..256-long dot products the error is at or below that of an fp32 FFMA chain, i.e. the
+// tensor-core path keeps the 1e-4 loss-parity bar.
 //
 // Operand buffer ("row-major panel buffer"): a matrix of R rows x F fp16 features is stored as F/8 panels;
 // panel p holds features [8p, 8p+8) of every row as R consecutive 16-byte units:
 //        element (row r, feature f) at  (f/8) * R*16 + r*16 + (f%8)*2.
 // A thread that owns a row writes 16-byte vectors (conflict-free: consecutive rows are consecutive units).
-// The SAME buffer is read by the tensor core in both majors, by descriptor only (no transposed copies):
+// The SAME buffer is read by the tensor core in both majors, by descriptor only (no transposed copies); every
+// 8 x 16-byte block is one core matrix of the no-swizzle layout:
 //   * K-major  (rows = M/N index, features = K): LBO = R*16 (next 8 features), SBO = 128 (next 8 rows);
-//     the k-slice of one MMA (K = 16) starts at panel k0/8.
+//     the k-slice of one MMA (K = 16) starts at panel k0/8, the 64-row block m0 at byte m0*16.
 //   * MN-major (rows = K index, features = M/N): SBO = R*16 (next 8 features along M/N), LBO = 128 (next 8
-//     rows along K); the k-slice of one MMA starts at row r0.
+//     rows along K); the k-slice of one MMA starts at row r0, the 64-feature block m0 at panel m0/8.
 #pragma once
 #include <cuda_fp16.h>
 
@@ -22,26 +23,9 @@
 namespace orl {
 namespace tc {
 
-// instruction descriptor, kind::f16: A, B = F16 (format 0), D = F32
-__host__ __device__ __forceinline__ uint32_t make_idesc_f16(int M, int N, bool a_mn_major, bool b_mn_major) {
-    uint32_t d = 0;
-    d |= 1u << 4;
-    d |= (a_mn_major ? 1u : 0u) << 15;
-    d |= (b_mn_major ? 1u : 0u) << 16;
-    d |= (uint32_t)(N >> 3) << 17;
-    d |= (uint32_t)(M >> 4) << 24;
-    return d;
-}
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// descriptor = constant part (LBO, SBO, version) | start address
+// wgmma descriptor = constant part (LBO, SBO; layout type 0 = no swizzle) | start address
 __device__ __forceinline__ uint64_t desc_const(uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | ((uint64_t)1 << 46);
+    return ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32);
 }
 __device__ __forceinline__ uint64_t desc_at(uint64_t dconst, uint32_t smem_addr) { return dconst | (uint64_t)((smem_addr >> 4) & 0x3FFF); }
 

@@ -54,7 +54,7 @@ def load(path=None):
     if not os.path.exists(p):
         raise OrlLibraryError(
             f"{p} not found: build it with `python -m openrl_b200.build` "
-            "(nvcc, sm_100a). There is no CPU fallback."
+            "(nvcc, sm_90a). There is no CPU fallback."
         )
     try:
         lib = ctypes.CDLL(p)

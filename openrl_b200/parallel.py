@@ -8,8 +8,7 @@ exchange steps of the path (SURVEY.md §8e):
   2. once per update: SUM of the folded gradient bucket `folded` (2*stride floats, 37 KB for CartPole) between the
      reduce and the optimiser step.
 For the feed-forward update both steps run INSIDE our kernels over NVLink peer memory (`PeerBucket` below,
-orl_ppo_reduce_peer / orl_ppo_apply_peer / orl_peer_sum_f64; DESIGN.md §4.5: 1.871 ms vs 1.956 ms per iteration with NCCL
-on 8 B200s); the NCCL all-reduce is the fallback (ORL_PEER_APPLY=0 or no peer mapping) and carries the recurrent and
+orl_ppo_reduce_peer / orl_ppo_apply_peer / orl_peer_sum_f64; DESIGN.md §4.5); the NCCL all-reduce is the fallback (ORL_PEER_APPLY=0 or no peer mapping) and carries the recurrent and
 shared-network buckets.
 
 Rollouts shard over envs: rank r owns global envs [r*N, (r+1)*N) and seeds them exactly as the
@@ -53,8 +52,7 @@ def allreduce_sum_(t):
 
 # ---- alternative for the fallback path: torch's symmetric-memory one-shot all-reduce -----------------------------------
 # ORL_SYMM_ALLREDUCE=1 (with ORL_PEER_APPLY=0): every rank reads all peers' buffers over NVLink and sums locally (signal-pad
-# barriers, graph-capturable) instead of NCCL.  Measured inside the captured iteration graph: 2 x B200 1.862 vs 1.866 ms,
-# 8 x B200 1.907 vs 1.956 ms per iteration; the fused PeerBucket path (1.871 ms) supersedes it.  Any failure to set the
+# barriers, graph-capturable) instead of NCCL; the fused PeerBucket path supersedes it.  Any failure to set the
 # symmetric path up falls back to NCCL.
 _SYMM = {}   # data_ptr -> (symmetric input tensor, output tensor, group name)
 

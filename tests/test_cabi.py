@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a, loads, and exports every symbol the header declares
+"""The C-ABI library builds for sm_90a, loads, and exports every symbol the header declares
 (no compute calls: this runs without a GPU)."""
 import ctypes
 

@@ -117,7 +117,7 @@ def test_update_flag_matrix_vs_oracle(cuda, flags):
 
 
 def test_fast_mode_multi_minibatch_and_odd_sizes(cuda):
-    """Fast mode (tcgen05) with num_mini_batch > 1, rows not a multiple of the 128-row tile, device randperm."""
+    """Fast mode (wgmma) with num_mini_batch > 1, rows not a multiple of the 128-row tile, device randperm."""
     from openrl_b200.configs.config import create_config_parser
     from openrl_b200.envs.common import make
     from openrl_b200.modules.common import PPONet
@@ -168,7 +168,7 @@ def test_save_load_roundtrip_and_lr_decay(cuda, tmp_path):
 
 @pytest.mark.parametrize("n_actions", [2, 3, 5, 8])
 def test_tensor_core_kernel_head_width_templates(cuda, n_actions):
-    """The tcgen05 kernel is instantiated for head widths 2, 5 and a generic (runtime n <= 8) variant:
+    """The wgmma kernel is instantiated for head widths 2, 5 and a generic (runtime n <= 8) variant:
     each must agree with the fp32 kernel on the same synthetic minibatch (incl. a partial last tile)."""
     import torch
 

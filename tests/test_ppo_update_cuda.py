@@ -183,7 +183,7 @@ def test_sharded_minibatch_buckets_sum_to_global_bucket(cuda, tf32):
 
 
 def test_tensor_core_update_matches_fp32_update(cuda):
-    """tcgen05 update (split-fp16 operands, fp32 accumulate) vs the fp32 FFMA update on the same shuffled minibatch
+    """wgmma update (split-fp16 operands, fp32 accumulate) vs the fp32 FFMA update on the same shuffled minibatch
     (gather staging): the six scalars within the 1e-4 parity bar, gradients to fp32-class accuracy."""
     import torch
 

@@ -1,5 +1,6 @@
 """GAE kernel micro-benchmark: CUDA-event timing of orl_gae at the BASELINE config shapes and
-at a >= 1 GB shape, reported against the measured HBM peak (MEASURED_PEAKS.json)."""
+at a >= 1 GB shape, reported against the HBM peak (MEASURED_PEAKS.json, else the H100 SXM data sheet).
+Prints one JSON line per shape; `python tools/gae_micro.py OUT.json` also writes the list to OUT.json."""
 import json
 import os
 import sys
@@ -15,7 +16,7 @@ def peak_hbm():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p))["hbm_gbs"], "measured"
-    return 6650.0, "fallback"
+    return 3350.0, "datasheet"
 
 
 def bench_shape(L, T, B, flags=5, adv=True, stats=True, iters=20, flush=None):
@@ -58,7 +59,7 @@ def bench_shape(L, T, B, flags=5, adv=True, stats=True, iters=20, flush=None):
 def main():
     L = lib.load()
     peak, how = peak_hbm()
-    flush = torch.empty(256 * 1024 * 1024 // 4, device="cuda:0")  # 256 MB > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device="cuda:0")  # 256 MB > 50 MB L2
     out = []
     for name, T, B in [("C2 cartpole 4096", 128, 4096), ("C3 mpe 2048x3", 25, 6144), ("C4 gridworld 4096x2", 128, 8192),
                        ("C5 cheetah 1024", 128, 1024), ("1GB+ T128 B2^21", 128, 1 << 21)]:
@@ -68,8 +69,8 @@ def main():
             r["frac_of_%s_hbm_peak" % how] = r["GBps_median"] / peak
             out.append(r)
             print(json.dumps(r))
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    json.dump(out, open(os.path.join(ROOT, "gpurun_out", "gae_micro.json"), "w"), indent=1)
+    if len(sys.argv) > 1:
+        json.dump(out, open(sys.argv[1], "w"), indent=1)
 
 
 if __name__ == "__main__":
