@@ -153,7 +153,7 @@ __device__ __forceinline__ void fwd_tile(const FwdCtx& c, const float (&x)[8], i
         }
         wgmma_commit();
         overlap();
-        wgmma_wait0();
+        wgmma_wait<0>();
         frag_store<64>(z, c.S + half * 64 * S_LD, S_LD);
     }
     __syncthreads();   // the staging tile is complete; the next tile's stores follow its CTA barrier in front of the MMAs
@@ -476,7 +476,7 @@ __global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlR
                         wgmma_f16_n32<0, 0>(z, desc_at(dK_A, aa + 2 * kk * FPANEL), desc_at(dK_W, bb + 2 * kk * FPANEL_W), (pass | kk) > 0);
                 }
                 wgmma_commit();
-                wgmma_wait0();
+                wgmma_wait<0>();
                 frag_store<32>(z, c.S + mb * 64 * S_LD + 32 * nb, S_LD);
             }
             Q_FWD_SYNC();   // the staging tile is complete; the next step's stores follow its forward barrier in front of the MMAs

@@ -3,17 +3,22 @@
 // (orl_ppo.cu) at fp32-class accuracy (orl_tc16.cuh).  Selected with ORL_PPO_TENSORCORE; categorical
 // heads, obs widths <= 8 (CartPole, GridWorld).  Reference: openrl/algorithms/ppo.py:46-361.
 //
-// CTA = 256 threads = 128 tile rows x 2 column halves = 2 warpgroups, one CTA per SM (~147 KB shared
-// memory): warps w and w+4 own the same 32 rows and 32 columns each, so every row-wise operation (fc1
-// with K = d <= 8, LayerNorm forward/backward, head, loss) is thread-local apart from three two-float
-// exchanges and one head exchange through shared memory (named barriers per row group).  The per-tile
-// GEMM results (Z3, dN1) arrive in the warpgroups' accumulator registers in the wgmma fragment layout
-// and reach the row-owning threads through an fp32 staging tile in shared memory.
+// CTA = 256 threads = 128 tile rows x 2 column halves = 2 warpgroups, one CTA per SM (~171 KB shared
+// memory): warp w owns rows [16w, +16), lane l row 16w + l % 16 and columns [32 (l / 16), +32), so every
+// row-wise operation (fc1 with K = d <= 8, LayerNorm forward/backward, head, loss) is thread-local apart
+// from four exchanges with lane l ^ 16 (shuffles).  The per-tile GEMM results (Z3, dN1) arrive in the
+// warpgroups' accumulator registers in the wgmma fragment layout, whose rows [16w, +16) sit in warp w, and
+// reach the row-owning lanes through an fp32 staging tile in shared memory within the warp.  GEMM1 and
+// GEMM2 read only the issuing warpgroup's rows (warpgroup barrier); GEMM3a / GEMM3b reduce over all 128
+// rows (CTA barrier).  GEMM3a / GEMM3b have no consumer inside the tile loop: they stay in flight under
+// the LayerNorm-1 backward and the next tile's staging wait, fc1 and activation, and are waited for just
+// before the next tile overwrites R1.
 //
 // All matrix operands live in row-major panel buffers (orl_tc16.cuh) as fp16 hi/lo pairs, written by
 // the row-owning threads with 16-byte stores and read K-major or MN-major by descriptor only:
-//   R1 = [ n1 (8 panels) | CST = (1, mu3, std3, 0..) | X ]   rows = tile rows       (dZ1 reuses the n1 panels)
+//   R1 = [ n1 (8 panels) | CST = (1, mu3, std3, 0..) | X ]   rows = tile rows
 //   R2 = [ dZ3 (8 panels) | U = dL * rstd3 ]                  rows = tile rows
+//   R3 = [ dZ1 (8 panels) ]                                   rows = tile rows       (GEMM3a may still read R1)
 //   W  = W3f [64 out rows][64 in features]
 // Four GEMMs per 128-row tile, each as three MMA passes (Al.Bh, Ah.Bl, Ah.Bh), issued by one thread:
 //   GEMM1  Z3 [128x64]  = n1 . W3f^T                 A = R1 K-major,  B = W K-major     (fwd fc3)
@@ -55,7 +60,7 @@ constexpr int T_M = 128, T_NT = 256;
 constexpr int CW = 32;                         // columns per thread
 constexpr uint32_t PANEL = T_M * 16;           // 8 fp16 features of 128 rows
 constexpr uint32_t PANEL_W = H * 16;
-constexpr int R1_PANELS = 10, R2_PANELS = 9;
+constexpr int R1_PANELS = 10, R2_PANELS = 9, R3_PANELS = 8;
 constexpr int P_CST = 8, P_X = 9, P_U = 8;
 constexpr int N_LOSS_TC = 8;
 // staging tile of the per-tile GEMM results: 128 rows x 64 fp32, row pitch 68 floats (conflict-free row reads);
@@ -64,10 +69,11 @@ constexpr int S_LD = 68, GA_LD = 84, GB_LD = 20;
 // shared-memory carve-up (bytes)
 constexpr uint32_t OFF_R1H = 0, OFF_R1L = OFF_R1H + R1_PANELS * PANEL, OFF_R2H = OFF_R1L + R1_PANELS * PANEL,
                    OFF_R2L = OFF_R2H + R2_PANELS * PANEL, OFF_WH = OFF_R2L + R2_PANELS * PANEL, OFF_WL = OFF_WH + 8 * PANEL_W,
-                   OFF_S = OFF_WL + 8 * PANEL_W, OFF_STAGE = OFF_S + T_M * S_LD * 4;
+                   OFF_R3H = OFF_WL + 8 * PANEL_W, OFF_R3L = OFF_R3H + R3_PANELS * PANEL,
+                   OFF_S = OFF_R3L + R3_PANELS * PANEL, OFF_STAGE = OFF_S + T_M * S_LD * 4;
 static_assert((T_M * GA_LD + 64 * GB_LD) * 4 <= OFF_WH, "the Ga / Gb staging fits in R1 + R2");
 static_assert(OFF_STAGE % 128 == 0, "TMA destination alignment");
-static_assert(OFF_R2L + 16 * PANEL <= OFF_STAGE + 4096, "the 16-panel A descriptors stay inside the allocation");
+static_assert(OFF_R2L + 16 * PANEL <= OFF_R3H, "the 16-panel A descriptors of GEMM3a stop short of R3 (written while they run)");
 constexpr int N_SCAL = 4;                      // scalar columns staged per row
 
 struct TcMaps {   // TMA descriptors of the flattened rollout buffers (built by the launcher)
@@ -77,22 +83,17 @@ struct TcMaps {   // TMA descriptors of the flattened rollout buffers (built by 
 struct AdvNormTc { float m0, s0, m1, s1; bool two; };
 
 #define FOR_OUT(j) _Pragma("unroll") for (int j = 0; j < NOUT; ++j) if (NOUT != 8 || j < n)
-// row-group barrier: the two warps that share rows [32g, 32g+32) (g = warp % 4)
-#define ROWGROUP_SYNC()                                                        \
-    do {                                                                       \
-        switch (warp & 3) {                                                    \
-            case 0: asm volatile("bar.sync 1, 64;" ::: "memory"); break;       \
-            case 1: asm volatile("bar.sync 2, 64;" ::: "memory"); break;       \
-            case 2: asm volatile("bar.sync 3, 64;" ::: "memory"); break;       \
-            default: asm volatile("bar.sync 4, 64;" ::: "memory"); break;      \
-        }                                                                      \
-    } while (0)
+// the two column halves of a row sit in lanes l and l ^ 16 of one warp
+__device__ __forceinline__ float other_half(float v) { return __shfl_xor_sync(0xffffffffu, v, 16); }
+// barrier of this thread's warpgroup (named barriers 1 and 2)
+__device__ __forceinline__ void warpgroup_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory"); }
 
 __host__ __device__ inline uint32_t tc_stage_bytes(int d) { return (uint32_t)((T_M * d * 4 + 127) & ~127) + N_SCAL * T_M * 4; }
 __host__ __device__ inline uint32_t tc_small_off(int d) { return OFF_STAGE + tc_stage_bytes(d); }
-// fp32 weights: w1t[8][64] b1[64] b3f[64] whf[8][64] bhf[8] swh[8]; exchange: xs[2][128][2] xh[8][2][128]; staging mbarrier
+// fp32 weights: w1t[8][64] b1[64] b3f[64] whf[8][64] bhf[8] swh[8]; flush scratch: Q[8][64] su smu sdl[3][8], loss
+// partials [3][8 warps]; staging mbarrier
 constexpr uint32_t SMALL_FLOATS = 8 * H + H + H + MAX_OUT * H + 2 * MAX_OUT;
-constexpr uint32_t XCH_FLOATS = 2 * T_M * 2 + 2 * T_M * 8;
+constexpr uint32_t XCH_FLOATS = MAX_OUT * H + 3 * MAX_OUT + 3 * 8;
 __host__ __device__ inline uint32_t tc_smem_bytes(int d) { return tc_small_off(d) + 4 * (SMALL_FLOATS + XCH_FLOATS) + 8; }
 
 // ACT == 1: ReLU (the reference's default activation_id) compiled in; ACT == -1: runtime activation_id (tanh / leaky / elu
@@ -108,14 +109,17 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     const int n = POLICY ? (NOUT == 8 ? a.n_actions : NOUT) : 1;
     const float* params = POLICY ? a.policy_params : a.critic_params;
     const float* obs = POLICY ? a.policy_obs : a.critic_obs;
-    const int tid = threadIdx.x, warp = tid >> 5;
-    const int row = tid & 127, half = tid >> 7;   // this thread: tile row, column half (= its warpgroup)
-    const int cb = CW * half;                     // first column of the half
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    // warp w owns tile rows [16w, +16): the rows of its wgmma accumulator fragment, so the per-tile GEMM results
+    // reach the row owners within the warp.  Warpgroup g (= w / 4) owns rows [64g, +64).
+    const int row = 16 * warp + (lane & 15), half = lane >> 4, wg = warp >> 2;   // this thread: tile row, column half, warpgroup
+    const int cb = CW * half;                                                    // first column of the half
     const NetOffsets po = net_offsets(d, n);
 
     uint8_t* R1h = smem + OFF_R1H; uint8_t* R1l = smem + OFF_R1L;
     uint8_t* R2h = smem + OFF_R2H; uint8_t* R2l = smem + OFF_R2L;
     uint8_t* Wh = smem + OFF_WH;   uint8_t* Wl = smem + OFF_WL;
+    uint8_t* R3h = smem + OFF_R3H; uint8_t* R3l = smem + OFF_R3L;
     float* S = reinterpret_cast<float*>(smem + OFF_S);                                  // [128][S_LD]
     float* st_obs = reinterpret_cast<float*>(smem + OFF_STAGE);                        // [128][d]
     float* st_sc = reinterpret_cast<float*>(smem + OFF_STAGE + ((T_M * d * 4 + 127) & ~127));   // [4][128]
@@ -125,9 +129,9 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     float* whf = b3f + H;                        // [8][64] folded head
     float* bhf = whf + MAX_OUT * H;
     float* swh = bhf + MAX_OUT;                  // [8] row sums of whf
-    float* xs = swh + MAX_OUT;                   // [2][128][2] statistics exchange
-    float* xh = xs + 2 * T_M * 2;                // [2][128][8] head exchange (flush scratch afterwards)
-    uint64_t* bar_st = reinterpret_cast<uint64_t*>(xh + 2 * T_M * 8);  // TMA staging
+    float* qs = swh + MAX_OUT;                   // flush: [8][64] Q rows, then su[8], smu[8], sdl[8]
+    float* red = qs + MAX_OUT * H + 3 * MAX_OUT; // flush: [3][8] per-warp loss sums
+    uint64_t* bar_st = reinterpret_cast<uint64_t*>(red + 3 * 8);  // TMA staging
 
     // ---- stage weights (folded); the fc3 matrix as split fp16 ----
     for (int i = tid; i < 8 * H; i += T_NT) { const int k = i / H, j = i % H; w1t[i] = (k < d) ? params[po.w1 + j * d + k] : 0.f; }
@@ -215,6 +219,7 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     const uint64_t dK_A = desc_const(PANEL, 128), dK_W = desc_const(PANEL_W, 128);      // K-major
     const uint64_t dMN_A = desc_const(128, PANEL), dMN_W = desc_const(128, PANEL_W);    // MN-major
     const uint32_t aR1h = smem_u32(R1h), aR1l = smem_u32(R1l), aR2h = smem_u32(R2h), aR2l = smem_u32(R2l), aWh = smem_u32(Wh), aWl = smem_u32(Wl);
+    const uint32_t aR3h = smem_u32(R3h), aR3l = smem_u32(R3l);
 
     // ---- staging of the minibatch rows, one tile ahead ----
     const long long n_tiles = (a.batch_rows + T_M - 1) / T_M;
@@ -269,7 +274,7 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         const uint32_t par = it & 1u;
         // ---- this tile's rows from the staging buffer ----
         if (TMA) mbar_wait(bar_st, par);
-        else { cp_async_wait_all(); __syncthreads(); }
+        else { cp_async_wait_all(); __syncwarp(); }   // a row's gathers are issued by its two lanes
         const bool valid = gi >= 0;
         float x[8];
 #pragma unroll
@@ -310,19 +315,19 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
             n1[i] = act_fwd_t<ACT>(n1[i], a.activation_id);
             s += n1[i]; sq = fmaf(n1[i], n1[i], sq);
         }
-        {   // exchange 1 (slot xs): LayerNorm-1 statistics
-            *reinterpret_cast<float2*>(xs + (half * T_M + row) * 2) = make_float2(s, sq);
-            ROWGROUP_SYNC();
-            const float2 o = *reinterpret_cast<const float2*>(xs + ((half ^ 1) * T_M + row) * 2);
-            s += o.x; sq += o.y;
-        }
+        // the previous tile's GEMM3a / GEMM3b have been in flight up to here.  They must complete before R1 is
+        // overwritten below; waiting here rather than there keeps ptxas from placing its own wait inside the divergent
+        // slow path of the square root, which would serialise every wgmma of the kernel.
+        wgmma_wait<0>();
+        s += other_half(s); sq += other_half(sq);   // LayerNorm-1 statistics of the whole row
         const float mu1 = s * (1.f / H);
         const float rstd1 = 1.0f / sqrtf(fmaxf(sq * (1.f / H) - mu1 * mu1, 0.f) + LN_EPS);
 #pragma unroll
         for (int i = 0; i < CW; ++i) n1[i] = (n1[i] - mu1) * rstd1;
 
-        // previous tile's GEMM3b (warpgroup 1) must have finished reading R1
-        if (it > 0) __syncthreads();
+        // GEMM3a / GEMM3b of both warpgroups read every row of R1, R2 and R3: all have completed past this barrier.
+        // It also means every thread has read its staged row, which the TMA issued after GEMM1 overwrites.
+        __syncthreads();
 #pragma unroll
         for (int q8 = 0; q8 < CW; q8 += 8) {
             const uint32_t off = (uint32_t)((cb + q8) >> 3) * PANEL + row * 16;
@@ -330,20 +335,20 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         }
         if (half == 0) split_store8(R1h + P_X * PANEL + row * 16, R1l + P_X * PANEL + row * 16, x, SX);
         fence_proxy_async();
-        __syncthreads();
-        float z[32];   // GEMM1: Z3 = n1 . W3f^T, rows [64 half, +64)
+        warpgroup_sync(wg);   // GEMM1 reads only this warpgroup's rows of R1
+        float z[32];   // GEMM1: Z3 = n1 . W3f^T, rows [64g, +64)
 #pragma unroll
         for (int i = 0; i < 32; ++i) z[i] = 0.f;
         wgmma_fence();
 #pragma unroll
         for (int pass = 0; pass < 3; ++pass) {
-            const uint32_t aa = (pass == 0 ? aR1l : aR1h) + half * 64 * 16, bb = pass == 1 ? aWl : aWh;
+            const uint32_t aa = (pass == 0 ? aR1l : aR1h) + wg * 64 * 16, bb = pass == 1 ? aWl : aWh;
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk)
                 wgmma_f16_n64<0, 0>(z, desc_at(dK_A, aa + 2 * kk * PANEL), desc_at(dK_W, bb + 2 * kk * PANEL_W), (pass | kk) > 0);
         }
-        wgmma_commit();
-        if (TMA && tid == 0 && tile + G < n_tiles) issue_tma(tile + G);   // the staging buffer was consumed before the barrier above
+        wgmma_commit();   // the only group in flight
+        if (TMA && tid == 0 && tile + G < n_tiles) issue_tma(tile + G);   // the staging buffer was consumed before the CTA barrier above
         long long gi_cur = gi;
         if (!TMA) {
             issue_gather(gi_next);
@@ -353,9 +358,9 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
             gi = row_index(tile + G);
         }
 
-        wgmma_wait0();
-        frag_store<64>(z, S + half * 64 * S_LD, S_LD);
-        __syncthreads();
+        wgmma_wait<0>();
+        frag_store<64>(z, S + wg * 64 * S_LD, S_LD);
+        __syncwarp();   // rows [16 warp, +16) of S: written and read by this warp
 
         // ---- Z3 (staging tile) + b3f -> LayerNorm-3 -> n3 (registers only) ----
         float n3[CW];
@@ -367,12 +372,7 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         float s3 = 0.f, q3 = 0.f;
 #pragma unroll
         for (int i = 0; i < CW; ++i) { n3[i] += b3f[cb + i]; s3 += n3[i]; q3 = fmaf(n3[i], n3[i], q3); }
-        {   // exchange 2 (slot xs; the barrier before GEMM1 separates it from exchange 1)
-            *reinterpret_cast<float2*>(xs + (half * T_M + row) * 2) = make_float2(s3, q3);
-            ROWGROUP_SYNC();
-            const float2 o = *reinterpret_cast<const float2*>(xs + ((half ^ 1) * T_M + row) * 2);
-            s3 += o.x; q3 += o.y;
-        }
+        s3 += other_half(s3); q3 += other_half(q3);
         const float mu3 = s3 * (1.f / H);
         const float var3 = fmaxf(q3 * (1.f / H) - mu3 * mu3, 0.f) + LN_EPS;
         const float rstd3 = 1.0f / sqrtf(var3);
@@ -388,11 +388,7 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
                 out[j] = fmaf(n3[q4], wv.x, fmaf(n3[q4 + 1], wv.y, fmaf(n3[q4 + 2], wv.z, fmaf(n3[q4 + 3], wv.w, out[j]))));
             }
         }
-        {   // exchange 3 (slot xh): partial head dots
-            FOR_OUT(j) xh[(j * 2 + half) * T_M + row] = out[j];   // [j][half][row]: lanes are consecutive words (conflict-free)
-            ROWGROUP_SYNC();
-            FOR_OUT(j) out[j] += xh[(j * 2 + (half ^ 1)) * T_M + row];
-        }
+        FOR_OUT(j) out[j] += other_half(out[j]);   // partial head dots of the two halves
         // dot[j] = sum_k Whf[j][k] n3[k] (needed by the LayerNorm-3 backward); logits add the folded bias
         float dot[MAX_OUT];
 #pragma unroll
@@ -485,30 +481,32 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
             split_store8(R1h + P_CST * PANEL + row * 16, R1l + P_CST * PANEL + row * 16, c8, 1.0f);
         }
         fence_proxy_async();
-        __syncthreads();
-        // GEMM2: dN1 = dZ3 . W3f (rows [64 half, +64)) ; GEMM3a: Ga += R2^T . R1 (rows [64 half, +64))
+        warpgroup_sync(wg);   // GEMM2 reads only this warpgroup's rows of R2
+        // GEMM2: dN1 = dZ3 . W3f (rows [64g, +64)) ; GEMM3a: Ga += R2^T . R1 (rows [64g, +64))
 #pragma unroll
         for (int i = 0; i < 32; ++i) z[i] = 0.f;
         wgmma_fence();
 #pragma unroll
         for (int pass = 0; pass < 3; ++pass) {
-            const uint32_t aa = (pass == 0 ? aR2l : aR2h) + half * 64 * 16, bb = pass == 1 ? aWl : aWh;
+            const uint32_t aa = (pass == 0 ? aR2l : aR2h) + wg * 64 * 16, bb = pass == 1 ? aWl : aWh;
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk)
                 wgmma_f16_n64<0, 1>(z, desc_at(dK_A, aa + 2 * kk * PANEL), desc_at(dMN_W, bb + kk * 256), (pass | kk) > 0);
         }
+        wgmma_commit();
+        __syncthreads();   // GEMM3a reduces over all 128 rows of R1 and R2
 #pragma unroll
         for (int pass = 0; pass < 3; ++pass) {
-            const uint32_t aa = (pass == 0 ? aR2l : aR2h) + half * 8 * PANEL, bb = pass == 1 ? aR1l : aR1h;
+            const uint32_t aa = (pass == 0 ? aR2l : aR2h) + wg * 8 * PANEL, bb = pass == 1 ? aR1l : aR1h;
 #pragma unroll
             for (int kk = 0; kk < 8; ++kk)
                 wgmma_f16_n80<1, 1>(ga, desc_at(dMN_A, aa + kk * 256), desc_at(dMN_A, bb + kk * 256), 1u);
         }
         wgmma_commit();
-        wgmma_wait0();
-        frag_store<64>(z, S + half * 64 * S_LD, S_LD);
-        __syncthreads();   // dN1 is staged, and both warpgroups' GEMM3a have finished reading n1 from R1
-        // ---- dN1 (staging tile) -> LayerNorm-1 backward -> activation backward -> dZ1 (into the n1 panels of R1) ----
+        wgmma_wait<1>();   // GEMM2 has completed; GEMM3a runs on under the row work below and the next tile's fc1
+        frag_store<64>(z, S + wg * 64 * S_LD, S_LD);
+        __syncwarp();
+        // ---- dN1 (staging tile) -> LayerNorm-1 backward -> activation backward -> dZ1 (R3) ----
         {
             float g[CW];
 #pragma unroll
@@ -519,12 +517,7 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
             float t1 = 0.f, t2 = 0.f;
 #pragma unroll
             for (int i = 0; i < CW; ++i) { t1 += g[i]; t2 = fmaf(g[i], n1[i], t2); }
-            {   // exchange 4 (slot xs; the barrier before GEMM2 separates it from exchange 2)
-                *reinterpret_cast<float2*>(xs + (half * T_M + row) * 2) = make_float2(t1, t2);
-                ROWGROUP_SYNC();
-                const float2 o = *reinterpret_cast<const float2*>(xs + ((half ^ 1) * T_M + row) * 2);
-                t1 += o.x; t2 += o.y;
-            }
+            t1 += other_half(t1); t2 += other_half(t2);
             t1 *= (1.f / H); t2 *= (1.f / H);
             const float std1 = 1.0f / rstd1;
 #pragma unroll
@@ -536,36 +529,38 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
 #pragma unroll
             for (int q8 = 0; q8 < CW; q8 += 8) {
                 const uint32_t off = (uint32_t)((cb + q8) >> 3) * PANEL + row * 16;
-                split_store8(R1h + off, R1l + off, g + q8, 1.0f);
+                split_store8(R3h + off, R3l + off, g + q8, 1.0f);
             }
         }
         fence_proxy_async();
-        __syncthreads();
-        if (half == 1) {   // GEMM3b: Gb += dZ1^T . [CST | X]
+        // GEMM3b (warpgroup 1) reduces dZ1 over all 128 rows: warpgroup 0 only signals that its rows are stored
+        if (wg == 1) {   // GEMM3b: Gb += dZ1^T . [CST | X], waited for before the next tile overwrites R1
+            asm volatile("bar.sync 3, 256;" ::: "memory");
             wgmma_fence();
 #pragma unroll
             for (int pass = 0; pass < 3; ++pass) {
-                const uint32_t aa = pass == 0 ? aR1l : aR1h, bb = (pass == 1 ? aR1l : aR1h) + P_CST * PANEL;
+                const uint32_t aa = pass == 0 ? aR3l : aR3h, bb = (pass == 1 ? aR1l : aR1h) + P_CST * PANEL;
 #pragma unroll
                 for (int kk = 0; kk < 8; ++kk)
                     wgmma_f16_n16<1, 1>(gb, desc_at(dMN_A, aa + kk * 256), desc_at(dMN_A, bb + kk * 256), 1u);
             }
             wgmma_commit();
-            wgmma_wait0();
+        } else {
+            asm volatile("bar.arrive 3, 256;" ::: "memory");
         }
     }
+    wgmma_wait<0>();   // the last tile's GEMM3a / GEMM3b
 
     // ---- flush: Ga / Gb (accumulator registers -> staging in R1 / R2) -> partial folded gradients ----
     float* part = a.partials + (size_t)((POLICY ? 0 : G) + cta) * stride;
     const FoldOffsets fo = fold_offsets(d, n);
-    float* qs = xh;              // [8][64] Q rows, then su[8], smu[8], sdl[8]
     float* qsu = qs + MAX_OUT * H;
     if (it > 0) {
         float* gas = reinterpret_cast<float*>(smem);   // [128][GA_LD]
         float* gbs = gas + T_M * GA_LD;                // [64][GB_LD]
         __syncthreads();   // every MMA has completed: R1 / R2 are free
-        frag_store<80>(ga, gas + half * 64 * GA_LD, GA_LD);
-        if (half == 1) frag_store<16>(gb, gbs, GB_LD);
+        frag_store<80>(ga, gas + wg * 64 * GA_LD, GA_LD);
+        if (wg == 1) frag_store<16>(gb, gbs, GB_LD);
         __syncthreads();
         {   // Ga columns [32*half, 32*half+32) of this row
             float v[32];
@@ -605,8 +600,6 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     }
     {
         float v[3] = {loss0, loss1, loss2};
-        float* red = xs;
-        const int lane = tid & 31;
         __syncthreads();
 #pragma unroll
         for (int k = 0; k < 3; ++k) { const float sv = warp_sum(v[k]); if (lane == 0) red[k * 8 + warp] = sv; }

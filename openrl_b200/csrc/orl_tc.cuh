@@ -30,11 +30,13 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 
 // ---- warpgroup MMA (all 128 threads of a warpgroup execute these together) ----
 // wgmma_fence orders this thread's register accesses to the accumulators before the MMAs that follow;
-// wgmma_commit closes the group of MMAs issued so far, wgmma_wait0 waits until every committed group has completed
-// (its accumulators are readable and its shared-memory operands may be overwritten).
+// wgmma_commit closes the group of MMAs issued so far, wgmma_wait<N> waits until at most the N most recently
+// committed groups are still pending: every older group has completed (its accumulators are readable and its
+// shared-memory operands may be overwritten).
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // D[64 x N] (+)= A[64 x 16] . B[16 x N], fp16 operands, fp32 accumulators.  TA / TB = 1: the operand is MN-major
 // (transposed) in shared memory, 0: K-major.  `accumulate` = 0 overwrites D.
