@@ -237,6 +237,8 @@ int orl_policy_eval(const float* policy_params, int obs_dim, int n_actions, int 
                                          staged by TMA when `indices` is NULL, by cp.async gathers otherwise.
                                          Without the flag everything is fp32 FFMA. */
 #define ORL_PPO_TF32 ORL_PPO_TENSORCORE /* round-1 name of the flag */
+#define ORL_PPO_JOINT_ACTION 1024     /* cfg.use_joint_action_loss (JRPO) on the recurrent update (OrlRnnArgs only, 3 agents):
+                                         see orl_rnn_fwdbwd */
 
 typedef struct OrlPpoArgs {
     int32_t obs_dim;         /* d  policy obs width  (<= 64) */
@@ -338,6 +340,12 @@ int orl_minibatch_stats(const int64_t* indices, int64_t batch_rows, const float*
  * CPU against the oracle); parameter gradients are reductions of a per-row tape, dW = sum P^T Q.
  * Parameter layout of a recurrent net (reference state_dict order):
  *   W1[64][d] b1 g1 be1 | W3[64][64] b3 g3 be3 | Wih[192][64] Whh[192][64] bih bhh | g_rnn be_rnn | Wh[n][64] bh[n]
+ * With ORL_PPO_JOINT_ACTION (JRPO, ppo.py:254-319 + recurrent_generator_v3, replay_data.py:425-551): a chunk c covers the
+ * samples f = n*T + t in [c*L, c*L + L), each carrying all A agents; the policy is evaluated on every agent row, the
+ * ratio is exp(sum_a logp - sum_a old_logp) per (chunk, step) group with agent 0's advantage, the critic runs on agent
+ * 0's rows only.  mb_stats then holds 6 doubles: the {sum ret, sum ret^2, sum active} moments of the agent-0 rows (value
+ * loss, ValueNorm, policy-loss weights) and of all agent rows (only the active sum [5] is read: entropy weights).
+ * norm_rows counts (chunk, step) groups.
  */
 typedef struct OrlRnnArgs {
     int32_t env_kind, n_envs, n_agents, episode_length;   /* N, A, T; rows B = N*A */
@@ -373,7 +381,7 @@ typedef struct OrlRnnArgs {
 } OrlRnnArgs;
 int orl_rnn_param_count(int obs_dim, int n_out);
 int orl_rnn_tape_width(void);
-/* floats of OrlRnnArgs.tape for a minibatch of `rows` = n_chunks * chunk_length row-steps */
+/* floats of OrlRnnArgs.tape for a minibatch of `rows` = n_chunks * chunk_length row-steps (times A with ORL_PPO_JOINT_ACTION) */
 long long orl_rnn_workspace_floats(long long rows, int grads_stride);
 /* policy GRU rollout for steps [t_begin, t_end) fused with the device env (simple_spread, CartPole, GridWorld) */
 int orl_rnn_rollout(const OrlRnnArgs* args, void* stream);

@@ -13,7 +13,7 @@ permutation is needed at all (a minibatch that is the whole buffer is a sum over
 import numpy as np
 import torch
 from .. import lib, parallel
-from ..buffers.replay_data import ReplayData, chunk_row_indices
+from ..buffers.replay_data import ReplayData, chunk_row_indices, v3_row_indices
 
 
 class PPOAlgorithm:
@@ -79,10 +79,17 @@ class PPOAlgorithm:
             self.share_grads = self.share_bucket[:(self.share_total + 3) & ~3]
             self.share_loss = self.share_bucket[(self.share_total + 3) & ~3:]
             self.share_ws = None
-        for name in ("use_joint_action_loss", "use_policy_vhead",
-                     "use_amp", "use_deepspeed"):
+        for name in ("use_policy_vhead", "use_amp", "use_deepspeed"):
             if getattr(cfg, name, False):
                 raise NotImplementedError(f"cfg.{name} is not built into the CUDA update yet (SURVEY.md §8f)")
+        # JRPO: joint ratio over the agents of a step, agent-0 critic, recurrent_generator_v3 chunks (ppo.py:254-371).  The
+        # reference takes it only with use_recurrent_policy; with the feed-forward / naive generators its reshape(-1, A)
+        # would group unrelated shuffled rows
+        self.joint_action = bool(getattr(cfg, "use_joint_action_loss", False))
+        if self.joint_action and (not cfg.use_recurrent_policy or self.share):
+            raise NotImplementedError("use_joint_action_loss (JRPO) is built for the chunked recurrent update: it needs "
+                                      "use_recurrent_policy and is not built with use_share_model or the feed-forward / "
+                                      "naive-recurrent generators")
         if self.recurrent:
             if self.head_kind != lib.HEAD_CATEGORICAL:
                 raise NotImplementedError("recurrent policies are built for Discrete action spaces")
@@ -96,6 +103,8 @@ class PPOAlgorithm:
             self.rnn_grads = self.rnn_bucket[:2 * self.rnn_stride].view(2, self.rnn_stride)
             self.loss_acc = self.rnn_bucket[2 * self.rnn_stride:]
             self.tape = None
+            if self.joint_action:   # minibatch moments of the agent-0 rows, then of all agent rows (OrlRnnArgs.mb_stats)
+                self.joint_stats = torch.zeros(6, dtype=torch.float64, device=dev)
         self.gpu_launches = 0
         self.h2d_bytes = 0
         self.d2h_bytes = 0
@@ -191,7 +200,7 @@ class PPOAlgorithm:
         a = lib.OrlRnnArgs()
         a.n_envs, a.n_agents, a.episode_length = buf.n_rollout_threads, buf.num_agents, buf.episode_length
         a.obs_dim, a.critic_obs_dim, a.n_actions, a.activation_id = self.d, self.dc, self.n, pol.activation_id
-        a.chunk_length, a.flags = self.chunk_length, self.flags
+        a.chunk_length, a.flags = self.chunk_length, self.flags | (lib.PPO_JOINT_ACTION if self._joint(buf) else 0)
         a.n_chunks, a.chunk_ids = int(chunk_ids.numel()), lib.ptr(chunk_ids)
         a.policy_params, a.critic_params = lib.ptr(pol.flat_params), lib.ptr(cri.flat_params)
         a.policy_obs, a.critic_obs = lib.ptr(buf.policy_obs), lib.ptr(buf.critic_obs)
@@ -217,23 +226,46 @@ class PPOAlgorithm:
         a.norm_rows = rows * self.world_size if self.world_size > 1 else 0
         return a
 
+    def _joint(self, buf):
+        """JRPO on the joint kernels.  With one agent the v3 chunks, the permutation draw and the joint loss are those of
+        recurrent_generator and the ordinary loss, so the ordinary kernels run."""
+        return self.joint_action and buf.num_agents > 1
+
+    def _joint_mb_stats(self, buf, ids):
+        """mb_stats of ORL_PPO_JOINT_ACTION: {sum ret, sum ret^2, sum active} over the agent-0 rows of the chunks (value
+        loss, ValueNorm, policy-loss weights), then over all their agent rows (entropy weights).  Always computed: the
+        whole-buffer moments gae_stats[5:8] cover every agent."""
+        T, A = buf.episode_length, buf.num_agents
+        s = lib.current_stream()
+        for k, every in ((0, False), (3, True)):
+            bi = v3_row_indices(ids, self.chunk_length, T, A, buf.n_rollout_threads * A, all_agents=every)
+            lib.check(self._lib.orl_minibatch_stats(lib.ptr(bi), int(bi.numel()), lib.ptr(buf.returns), lib.ptr(buf.active_masks),
+                                                    lib.ptr(self.joint_stats[k:k + 3]), s), "orl_minibatch_stats")
+        self.gpu_launches += 2
+        parallel.allreduce_sum_(self.joint_stats)
+        return self.joint_stats
+
     def _train_recurrent(self, buf):
         """train_ppo with ReplayData.recurrent_generator (replay_data.py:1062-1258): per epoch one permutation of
         the data chunks (L consecutive steps of the agent-major / time-minor flattening f = (n*A + a)*T + t);
-        a minibatch is a slice of chunk ids, gathered inside the kernels."""
+        a minibatch is a slice of chunk ids, gathered inside the kernels.  JRPO with A > 1 (recurrent_generator_v3,
+        replay_data.py:425-551): chunks of L consecutive samples of the env-major / time-minor flattening f = n*T + t,
+        each sample carrying all A agents."""
         cfg = self.cfg
         T, B = buf.episode_length, buf.n_rollout_threads * buf.num_agents
-        total, L = T * B, (T if self.naive else cfg.data_chunk_length)
+        joint = self._joint(buf)
+        total, L = (T * buf.n_rollout_threads if joint else T * B), (T if self.naive else cfg.data_chunk_length)
         if total < L:
             raise AssertionError(f"PPO requires the number of processes ({buf.n_rollout_threads}) * episode length ({T}) "
-                                 f"* agents to be greater than or equal to the data chunk length ({L}).")
+                                 f"{'' if joint else '* agents '}to be greater than or equal to the data chunk length ({L}).")
         data_chunks = total // L
         mbc = data_chunks // self.num_mini_batch
         rows = mbc * L
-        need = int(self._lib.orl_rnn_workspace_floats(rows, self.rnn_stride))   # tape rows + reduction partials
+        tape_rows = rows * buf.num_agents if joint else rows   # the joint policy tapes every agent row of a step
+        need = int(self._lib.orl_rnn_workspace_floats(tape_rows, self.rnn_stride))   # tape rows + reduction partials
         if self.tape is None or self.tape.numel() < need:
             self.tape = torch.empty(need, dtype=torch.float32, device=self.device)
-        whole = self.num_mini_batch == 1 and rows == total
+        whole = self.num_mini_batch == 1 and rows == total and not joint
         s, Lb = lib.current_stream(), self._lib
         for _ in range(self.ppo_epoch):
             if cfg.parity_mode:
@@ -243,7 +275,9 @@ class PPOAlgorithm:
                 perm = torch.randperm(data_chunks, device=self.device)
             for i in range(self.num_mini_batch):
                 ids = perm[i * mbc:(i + 1) * mbc].contiguous()
-                if whole:
+                if joint:
+                    mb_stats = self._joint_mb_stats(buf, ids)
+                elif whole:
                     mb_stats = buf.gae_stats[5:8]
                 else:
                     bi = chunk_row_indices(ids, L, T, B)

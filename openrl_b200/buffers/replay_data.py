@@ -29,6 +29,21 @@ def chunk_row_indices(chunk_ids, chunk_length, episode_length, rows):
     return ((f % episode_length) * rows + f // episode_length).contiguous()
 
 
+def v3_row_indices(chunk_ids, chunk_length, episode_length, n_agents, rows, all_agents=False):
+    """Buffer row index t*B + row of every step of the given `recurrent_generator_v3` chunks: agent 0's row of each step
+    (chunk-major / step-minor), or with `all_agents` every agent's row (chunk, step, agent order).
+
+    `recurrent_generator_v3` (replay_data.py:425-551) flattens (T, N, ...) env-major / time-minor (`_cast_v3`,
+    buffers/utils/util.py:100-101): sample f = n*T + t carries all A agents; chunk c holds f in [c*L, c*L + L) and does not
+    stop at env boundaries.  Agent a of sample f is buffer row (f % T)*B + (f // T)*A + a."""
+    lane = torch.arange(chunk_length, device=chunk_ids.device)
+    f = (chunk_ids[:, None] * chunk_length + lane[None, :]).reshape(-1)
+    r0 = (f % episode_length) * rows + (f // episode_length) * n_agents
+    if all_agents:
+        r0 = (r0[:, None] + torch.arange(n_agents, device=chunk_ids.device)[None, :]).reshape(-1)
+    return r0.contiguous()
+
+
 class ReplayData:
     def __init__(self, cfg, num_agents, obs_space, act_space, data_client=None, episode_length=None, device="cuda:0"):
         T = cfg.episode_length if episode_length is None else episode_length

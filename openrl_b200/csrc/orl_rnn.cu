@@ -5,6 +5,7 @@
 //   OnPolicyDriver.act / add2buffer       openrl/drivers/onpolicy_driver.py:80-152,236-279 (rnn-state carry,
 //                                         zeroing on dones_env)
 //   ReplayData.recurrent_generator        openrl/buffers/replay_data.py:1062-1258 (chunks of L over f=(n*A+a)*T+t)
+//   ReplayData.recurrent_generator_v3     openrl/buffers/replay_data.py:425-551 (JRPO: chunks of L over f=n*T+t, all agents)
 //   PPOAlgorithm.ppo_update (BPTT part)   openrl/algorithms/ppo.py:46-458
 //
 // Design (DESIGN.md "recurrent path"): ONE WARP per env (rollout), per row (critic) or per chunk (update) running
@@ -30,6 +31,7 @@ namespace rw = orl_rnnw;
 static_assert(rc::MAXN == MAX_OUT, "head width limits must agree");
 constexpr int LMAX = 32;     // data_chunk_length limit accepted by the host API (the chunk kernels loop over l; the tape is n_chunks * L rows)
 constexpr int RNN_NT = 64;   // threads per CTA of the sequential kernels
+constexpr int JOINT_A = 3;   // agents of the joint-action update (simple_spread, the multi-agent device env)
 
 __device__ __forceinline__ int pick_action(const OrlRnnArgs& a, const float (&pr)[MAX_OUT], int n, size_t grow, int row,
                                            int t, uint64_t rng_base) {
@@ -199,7 +201,9 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_critic_warp_kernel(const OrlRnnAr
 }
 
 // ---- update: one warp per C_R chunks; L forward steps (tape), per-step loss, L backward steps ----
-template <bool POLICY, int C_R, int C_NT>
+// AGENT0 (the critic under ORL_PPO_JOINT_ACTION): chunks are recurrent_generator_v3 chunks over f = n*T + t and the
+// critic sees agent 0's row of every step only (to_single_np, ppo.py:222-224, 254-262), buffer row t*B + n*A.
+template <bool POLICY, bool AGENT0, int C_R, int C_NT>
 __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArgs a) {
     constexpr int C_WPC = C_NT / 32;
     extern __shared__ __align__(16) float smem[];
@@ -238,7 +242,8 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
             valid[r] = grp * C_R + r < a.n_chunks;
             cpos[r] = valid[r] ? grp * C_R + r : grp * C_R;   // a tail slot recomputes chunk 0 of the group (same values, same addresses)
             f0[r] = a.chunk_ids[cpos[r]] * (long long)L;
-            h[r] = rw::ldv(states + ((size_t)(f0[r] % T) * B + (size_t)(f0[r] / T)) * rc::H, lane);
+            const size_t row0 = AGENT0 ? (size_t)(f0[r] / T) * a.n_agents : (size_t)(f0[r] / T);
+            h[r] = rw::ldv(states + ((size_t)(f0[r] % T) * B + row0) * rc::H, lane);
         }
         for (int l = 0; l < L; ++l) {
             rw::V2 x[C_R], h2[C_R];
@@ -247,7 +252,7 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
             size_t bi[C_R];
 #pragma unroll
             for (int r = 0; r < C_R; ++r) {
-                const long long f = f0[r] + l, row = f / T, t = f % T;
+                const long long f = f0[r] + l, row = AGENT0 ? f / T * a.n_agents : f / T, t = f % T;
                 bi[r] = (size_t)t * B + row;
                 const float* ob = obs + bi[r] * d;
                 x[r] = rw::V2{lane < d ? ob[lane] : 0.f, lane + 32 < d ? ob[lane + 32] : 0.f};
@@ -314,6 +319,111 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
         for (int w = 0; w < C_WPC; ++w) s += red[threadIdx.x][w];
         if (POLICY) atomicAdd(a.loss_acc + threadIdx.x, s);
         else if (threadIdx.x == 0) atomicAdd(a.loss_acc + 3, s);
+    }
+}
+
+// ---- joint-action policy update (ORL_PPO_JOINT_ACTION, JRPO): one warp per recurrent_generator_v3 chunk ----
+// A v3 sample is one (env, step) pair f = n*T + t carrying all A agents (replay_data.py:425-551); the warp advances
+// the A agent rows of its chunk together (step_forward<A> / step_backward<A>, the rollout's row grouping).  Per step
+// (one group): ratio = exp(sum_a logp_a - sum_a old_logp_a) with agent 0's advantage, weighted by agent 0's active
+// mask over the agent-0 active sum (mb_stats[2]) or 1/groups; every agent row receives the same dL/dlogp.  The
+// entropy stays per agent row, weighted by every agent's active mask over the all-agent active sum (mb_stats[5]) or
+// 1/(groups*A) (ppo.py:254-319).  Tape row of (chunk c, step l, agent ag): (c*L + l)*A + ag.
+template <int A, int C_NT>
+__global__ void __launch_bounds__(C_NT, 1) rnn_joint_policy_warp_kernel(const OrlRnnArgs a) {
+    constexpr int C_WPC = C_NT / 32;
+    extern __shared__ __align__(16) float smem[];
+    const int B = a.n_envs * A, T = a.episode_length, L = a.chunk_length;
+    const int d = a.obs_dim, n = a.n_actions;
+    const rc::Offsets o = rc::rnn_offsets(d, n);
+    const rw::SmemNet W = rw::load_net(smem, a.policy_params, o, threadIdx.x, C_NT);
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float* scr = smem + rw::smem_net_floats() + warp * A * rw::SCR;
+    float loss0 = 0.f, loss1 = 0.f, loss2 = 0.f;   // identical on every lane; lane 0's copy is reduced
+
+    const double groups_d = a.norm_rows > 0 ? (double)a.norm_rows : (double)a.n_chunks * L;
+    const float inv_groups = (float)(1.0 / groups_d), inv_rows = (float)(1.0 / (groups_d * A));
+    const float inv_act0 = (float)(1.0 / a.mb_stats[2]), inv_act_all = (float)(1.0 / a.mb_stats[5]);
+    const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS;
+    const AdvNorm advn = make_adv_norm(a.gae_stats, a.flags & ORL_PPO_ADV_NORMALIZE);
+
+    for (long long c = (long long)blockIdx.x * C_WPC + warp; c < a.n_chunks; c += (long long)gridDim.x * C_WPC) {
+        const long long f0 = a.chunk_ids[c] * (long long)L;
+        const size_t s0 = (size_t)(f0 % T) * B + (size_t)(f0 / T) * A;   // agent 0 of the chunk's first sample
+        rw::V2 h[A];
+#pragma unroll
+        for (int ag = 0; ag < A; ++ag) h[ag] = rw::ldv(a.rnn_states + (s0 + ag) * rc::H, lane);
+        for (int l = 0; l < L; ++l) {
+            const long long f = f0 + l;
+            const size_t base = (size_t)(f % T) * B + (size_t)(f / T) * A;
+            rw::V2 x[A], h2[A];
+            float mk[A], out[A][MAX_OUT];
+            float* tape[A];
+#pragma unroll
+            for (int ag = 0; ag < A; ++ag) {
+                const float* ob = a.policy_obs + (base + ag) * d;
+                x[ag] = rw::V2{lane < d ? ob[lane] : 0.f, lane + 32 < d ? ob[lane + 32] : 0.f};
+                mk[ag] = a.masks[base + ag];
+                tape[ag] = a.tape + (((size_t)c * L + l) * A + ag) * rw::TAPE_W;
+            }
+            rw::step_forward<A>(W, scr, d, n, a.activation_id, x, h, mk, h2, out, tape, lane);
+            float joint = 0.f, joint_old = 0.f;   // summed in agent order, like the reference's reshape(-1, A).sum
+#pragma unroll
+            for (int ag = 0; ag < A; ++ag) {
+                h[ag] = h2[ag];
+                float nl[MAX_OUT], pr[MAX_OUT];
+                log_softmax_n(out[ag], n, nl, pr);
+                const int act = (int)a.actions[base + ag];
+                float lp = nl[0];
+#pragma unroll
+                for (int j = 1; j < MAX_OUT; ++j) if (j == act) lp = nl[j];
+                joint += lp;
+                joint_old += a.action_log_probs[base + ag];
+            }
+            const float adv = apply_adv_norm(advn, a.advantages[base]);
+            const PgTerm pg = pg_term(joint, joint_old, adv, a.clip_param, a.flags, a.dual_clip_coeff);
+            const float wgrp = pol_masks ? a.active_masks[base] * inv_act0 : inv_groups;
+            loss0 += pg.loss * wgrp; loss2 += pg.ratio;
+            const float dlp = pg.dlogp * wgrp;
+#pragma unroll
+            for (int ag = 0; ag < A; ++ag) {
+                float nl[MAX_OUT], pr[MAX_OUT], dl[MAX_OUT];
+                log_softmax_n(out[ag], n, nl, pr);
+                const int act = (int)a.actions[base + ag];
+                const float went_w = pol_masks ? a.active_masks[base + ag] * inv_act_all : inv_rows;
+                float ent = 0.f;
+#pragma unroll
+                for (int j = 0; j < MAX_OUT; ++j) if (j < n) ent -= pr[j] * nl[j];
+                loss1 += ent * went_w;
+                const float went = a.entropy_coef * went_w;
+#pragma unroll
+                for (int j = 0; j < MAX_OUT; ++j)
+                    dl[j] = j < n ? dlp * ((j == act ? 1.f : 0.f) - pr[j]) + went * pr[j] * (nl[j] + ent) : 0.f;
+                float mine = 0.f;   // lane m < 8 stores dL/dout[m]
+#pragma unroll
+                for (int j = 0; j < MAX_OUT; ++j) if (lane == j) mine = dl[j];
+                if (lane < MAX_OUT) tape[ag][rc::TP_DLOG + lane] = mine;
+            }
+        }
+        __syncwarp();   // tape scalars (lane 0) and dL/dout (lanes < 8) are read by every lane below
+        rw::V2 dh[A];
+#pragma unroll
+        for (int ag = 0; ag < A; ++ag) dh[ag] = rw::V2{0.f, 0.f};
+        for (int l = L - 1; l >= 0; --l) {
+            float* tape[A];
+#pragma unroll
+            for (int ag = 0; ag < A; ++ag) tape[ag] = a.tape + (((size_t)c * L + l) * A + ag) * rw::TAPE_W;
+            rw::step_backward<A>(W, scr, n, a.activation_id, tape, dh, lane);
+        }
+    }
+    __shared__ float red[3][C_WPC];
+    if (lane == 0) { red[0][warp] = loss0; red[1][warp] = loss1; red[2][warp] = loss2; }
+    __syncthreads();
+    if (threadIdx.x < 3) {
+        float s = 0.f;
+        for (int w = 0; w < C_WPC; ++w) s += red[threadIdx.x][w];
+        atomicAdd(a.loss_acc + threadIdx.x, s);
     }
 }
 
@@ -600,23 +710,38 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
     ORL_CHECK_ARG(a.grads_stride >= rc::rnn_offsets(a.obs_dim, a.n_actions).total &&
                       a.grads_stride >= rc::rnn_offsets(a.critic_obs_dim, 1).total, "grads_stride");
     if (a.flags & ORL_PPO_VALUENORM) { ORL_CHECK_ARG(a.vn_state, "vn_state"); }
+    // ORL_PPO_JOINT_ACTION: v3 chunks; the policy tape holds A rows per chunk step, the critic's one (agent 0)
+    const bool joint = a.flags & ORL_PPO_JOINT_ACTION;
+    if (joint) {
+        ORL_CHECK_ARG(a.n_agents == JOINT_A, "ORL_PPO_JOINT_ACTION is built for 3 agents (simple_spread)");
+        ORL_CHECK_ARG(a.n_chunks * a.chunk_length <= (long long)a.n_envs * a.episode_length, "v3 chunks exceed the N*T samples");
+    }
     cudaStream_t st = (cudaStream_t)stream;
     int e = orl::check_cuda(cudaMemsetAsync(a.loss_acc, 0, 8 * sizeof(float), st), "memset loss_acc");
     if (e) return e;
-    const long long rows = a.n_chunks * a.chunk_length;
-    const int rb = ws_row_blocks(rows);
-    float* partials = a.tape + ws_tape_floats(rows);
+    const long long steps = a.n_chunks * a.chunk_length;
+    const long long net_rows[2] = {joint ? steps * JOINT_A : steps, steps};
+    float* partials = a.tape + ws_tape_floats(net_rows[0]);   // the policy's tape is the larger one
     // two chunks per warp: every weight read from shared memory feeds two rows
     constexpr int C_R = 2;
     if ((e = orl::check_cuda(cudaFuncSetAttribute(tape_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TR_SMEM),
                              "smem attr (tape gemm)"))) return e;
-    if ((e = warp_kernel_prepare(rnn_chunk_warp_kernel<true, C_R, W_NT>, w_smem(C_R), "smem attr (rnn chunk policy)"))) return e;
-    if ((e = warp_kernel_prepare(rnn_chunk_warp_kernel<false, C_R, W_NT>, w_smem(C_R), "smem attr (rnn chunk critic)"))) return e;
     const int cgrid = warp_grid((a.n_chunks + C_R - 1) / C_R);
+    if (joint) {
+        if ((e = warp_kernel_prepare(rnn_joint_policy_warp_kernel<JOINT_A, W_NT>, w_smem(JOINT_A), "smem attr (rnn joint policy)"))) return e;
+        if ((e = warp_kernel_prepare(rnn_chunk_warp_kernel<false, true, C_R, W_NT>, w_smem(C_R), "smem attr (rnn chunk critic, agent 0)"))) return e;
+    } else {
+        if ((e = warp_kernel_prepare(rnn_chunk_warp_kernel<true, false, C_R, W_NT>, w_smem(C_R), "smem attr (rnn chunk policy)"))) return e;
+        if ((e = warp_kernel_prepare(rnn_chunk_warp_kernel<false, false, C_R, W_NT>, w_smem(C_R), "smem attr (rnn chunk critic)"))) return e;
+    }
     for (int net = 0; net < 2; ++net) {
         const int d = net == 0 ? a.obs_dim : a.critic_obs_dim, n = net == 0 ? a.n_actions : 1;
-        if (net == 0) rnn_chunk_warp_kernel<true, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
-        else rnn_chunk_warp_kernel<false, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
+        if (net == 0 && joint) rnn_joint_policy_warp_kernel<JOINT_A, W_NT><<<warp_grid(a.n_chunks), W_NT, w_smem(JOINT_A), st>>>(a);
+        else if (net == 0) rnn_chunk_warp_kernel<true, false, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
+        else if (joint) rnn_chunk_warp_kernel<false, true, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
+        else rnn_chunk_warp_kernel<false, false, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
+        const long long rows = net_rows[net];
+        const int rb = ws_row_blocks(rows);
         const TapeJobs jobs = make_jobs(d, n);
         tape_gemm_kernel<<<dim3(rb, jobs.n_gemm), TR_NT, TR_SMEM, st>>>(a.tape, rows, jobs, partials, a.grads_stride);
         tape_colsum_kernel<<<dim3(rb, jobs.n_col), rc::G3, 0, st>>>(a.tape, rows, jobs, partials, a.grads_stride);
