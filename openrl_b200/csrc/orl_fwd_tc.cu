@@ -25,15 +25,21 @@ using namespace orl;
 using namespace orl::tc;
 
 constexpr int F_M = 128, F_NT = 256, FCW = 32;
-constexpr uint32_t FPANEL = F_M * 16, FPANEL_W = H * 16;
-// Z3 staging tile: 128 rows x 64 fp32, row pitch 68 floats (row-per-thread float4 reads are conflict-free)
+constexpr uint32_t FPANEL_W = H * 16;
+// Z3 staging tile: row pitch 68 floats (row-per-thread float4 reads are conflict-free)
 constexpr int S_LD = 68;
-constexpr uint32_t FOFF_R1H = 0, FOFF_R1L = 8 * FPANEL, FOFF_WH = 16 * FPANEL, FOFF_WL = FOFF_WH + 8 * FPANEL_W, FOFF_S = FOFF_WL + 8 * FPANEL_W,
-                   FOFF_SMALL = FOFF_S + F_M * S_LD * 4;
+// shared-memory carve of a forward kernel: n1 hi/lo panels of M1 rows | W3f hi/lo panels | staging tile of MS rows | small
+template <int M1, int MS>
+struct FwdLayout {
+    static constexpr uint32_t PANEL = M1 * 16, R1H = 0, R1L = 8 * PANEL, WH = 16 * PANEL, WL = WH + 8 * FPANEL_W, S = WL + 8 * FPANEL_W,
+                              SMALL = S + MS * S_LD * 4;
+};
+using FLay = FwdLayout<F_M, F_M>;
+constexpr uint32_t FPANEL = FLay::PANEL;
 // fp32: w1t[8][64] b1[64] b3f[64] whf[8][64] bhf[8] | xs[2][128][2] xh[8][2][128] xst[128][8]
 constexpr uint32_t F_SMALL_FLOATS = 8 * H + H + H + MAX_OUT * H + MAX_OUT;
 constexpr uint32_t F_XCH_FLOATS = 2 * F_M * 2 + 2 * F_M * 8 + F_M * 8;
-constexpr uint32_t F_SMEM = FOFF_SMALL + 4 * (F_SMALL_FLOATS + F_XCH_FLOATS);
+constexpr uint32_t F_SMEM = FLay::SMALL + 4 * (F_SMALL_FLOATS + F_XCH_FLOATS);
 
 #define F_FOR_OUT(j) _Pragma("unroll") for (int j = 0; j < NOUT; ++j) if (NOUT != 8 || j < n)
 #define F_ROWGROUP_SYNC()                                                      \
@@ -56,13 +62,14 @@ struct FwdCtx {
 };
 
 // carve shared memory, stage + fold the weights (fc3 matrix as split fp16); ends with a CTA barrier.
+template <typename L = FLay>
 __device__ __forceinline__ FwdCtx fwd_setup(uint8_t* smem, const float* __restrict__ params, int d, int n) {
     const int tid = threadIdx.x, nt = blockDim.x;
     FwdCtx c;
-    c.R1h = smem + FOFF_R1H; c.R1l = smem + FOFF_R1L;
-    uint8_t* Wh = smem + FOFF_WH; uint8_t* Wl = smem + FOFF_WL;
-    c.S = reinterpret_cast<float*>(smem + FOFF_S);
-    c.w1t = reinterpret_cast<float*>(smem + FOFF_SMALL);
+    c.R1h = smem + L::R1H; c.R1l = smem + L::R1L;
+    uint8_t* Wh = smem + L::WH; uint8_t* Wl = smem + L::WL;
+    c.S = reinterpret_cast<float*>(smem + L::S);
+    c.w1t = reinterpret_cast<float*>(smem + L::SMALL);
     c.b1s = c.w1t + 8 * H; c.b3f = c.b1s + H; c.whf = c.b3f + H; c.bhf = c.whf + MAX_OUT * H;
     c.xs = c.bhf + MAX_OUT; c.xh = c.xs + 2 * F_M * 2; c.xst = c.xh + 2 * F_M * 8;   // the 2-half layout of the exchange area
     const NetOffsets po = net_offsets(d, n);
@@ -311,57 +318,72 @@ __global__ void __launch_bounds__(F_NT, 1) rollout_tc_kernel(const OrlRolloutArg
 }
 
 
-// ---- CartPole rollout: 4 forward threads + 2 env threads per row -----------------------------------------------------
+// ---- CartPole rollout: R envs per CTA, 4 forward lanes + 2 env threads per env -------------------------------------
 // The rollout is a chain of T dependent steps whose length is one row's work.  The f64 CartPole physics (sin / cos and
 // three dependent divides: ~250 dependent instructions) is a large share of a step when it runs after sampling, the
-// policy forward most of the rest.  So:
-//   * CTA = 768 threads = 128 rows x 6 groups.  Groups 0-3 (warps w, w+4, w+8, w+12 share rows [32(w%4), +32)) are the
-//     column quarters of the policy forward: quarter qd owns hidden columns [16 qd, +16).  They are also the four
-//     warpgroups of the fc3 GEMM: warpgroup g computes rows [64 (g % 2), +64) x columns [32 (g / 2), +32) of Z3.
-//   * Groups 4 and 5 are the env.  As soon as the state of step t is known, group 4 advances the physics for action 0 and
-//     draws the reset state (PCG64), group 5 advances the physics for action 1 and draws the sampling noise of step t+1 -
-//     concurrently with the whole forward pass of step t - and publish the candidates through (parity double-buffered)
-//     shared memory.  Quarter 0 samples.
-// After sampling a step is: publish the action, one row-group barrier (192 threads), every thread picks the candidate.
-// Same functions and explicitly rounded f64 operations as env_step_single -> bit-identical trajectories.
-constexpr int Q_NT = 768, Q_FWD = 512, QCW = 16;
-// exchange area: xs[4][128][2] | xh[8][4][128] | qn[2 parity][8][128] | act[2][128] (int) | termf[2][2][128] (int) |
-//                f64: cand[2 parity][2 action][4][128]  sr[2 parity][4][128]
-constexpr uint32_t Q_XCH_FLOATS = 4 * F_M * 2 + MAX_OUT * 4 * F_M + 2 * MAX_OUT * F_M + 2 * F_M + 4 * F_M;
-constexpr uint32_t Q_F64 = 2 * (2 * 4 + 4) * F_M;
-constexpr uint32_t Q_XCH_BYTES = 4 * Q_XCH_FLOATS + 8 * Q_F64;
-constexpr uint32_t Q_SMEM = FOFF_SMALL + 4 * F_SMALL_FLOATS + Q_XCH_BYTES;
-static_assert((FOFF_SMALL + 4 * F_SMALL_FLOATS + 4 * Q_XCH_FLOATS) % 8 == 0, "f64 exchange area must be 8-byte aligned");
+// policy forward most of the rest.  A CTA owns R = 32 (or 64) envs, so 4096 envs spread over 128 CTAs, one per SM, and
+// each SM issues the forward of R rows instead of 128:
+//   * Forward: 4R threads = R rows x 4 column quarters, the 4 quarters of a row in one warp (lane = 4 row + quarter,
+//     quarter qd owns hidden columns [16 qd, +16)); the LayerNorm and head partials meet through shuffles, added in a
+//     fixed order.  The fc3 GEMM is one M = 64 tile over R1 rows [0, 64) (rows [R, 64) zero padding when R = 32):
+//     with R = 32 the one forward warpgroup computes both 32-column halves, with R = 64 warpgroup g computes columns
+//     [32 g, +32).  Each Z3 element is the same wgmma_f16_n32 chain (Al.Bh, Ah.Bl, Ah.Bh; kk = 0..3) as in the
+//     row-parallel kernels.
+//   * Env: 2R threads, lane = row.  As soon as the state of step t is known, the action-0 threads advance the physics
+//     for action 0 and draw the reset state (PCG64), the action-1 threads advance the physics for action 1 and draw the
+//     sampling noise of step t+1 - concurrently with the whole forward pass of step t - and publish the candidates
+//     through (parity double-buffered) shared memory.  Quarter 0 samples.
+// Per step: one forward barrier in front of the MMA issue, one after the staging tile is written, one CTA barrier
+// (publish the action, every thread picks the candidate).  Same functions and explicitly rounded f64 operations as
+// env_step_single -> bit-identical trajectories.
+constexpr int QCW = 16, RW_M = 64;
+template <int R>
+struct RowsCfg {
+    static_assert(R == 32 || R == 64, "R1 holds 64 rows; a warpgroup of forward threads owns 32 of them");
+    static constexpr int FWD = 4 * R, NT = 6 * R, NWG = R / 32, NB = 2 / NWG;   // NB: 32-column halves per warpgroup
+    // resident CTAs per SM the register budget is sized for: with R = 32, three (96 registers, no spills; four would
+    // spill), so up to 3 x 32 x #SMs envs run in one wave; R = 64 needs ~146 registers (one CTA per SM)
+    static constexpr int MIN_CTAS = R == 32 ? 3 : 1;
+    using L = FwdLayout<RW_M, R>;
+    // exchange area: qn[2 parity][8][R] | act[2][R] (int) | termf[2][2][R] (int) | f64: cand[2 parity][2 action][4][R]
+    // srs[2 parity][4][R]
+    static constexpr uint32_t XCH = L::SMALL + 4 * F_SMALL_FLOATS;
+    static constexpr uint32_t XCH_F64 = XCH + 4 * (2 * MAX_OUT * R + 2 * R + 4 * R);
+    static constexpr uint32_t SMEM = XCH_F64 + 8 * (2 * 2 * 4 * R + 2 * 4 * R);
+    static_assert(XCH_F64 % 8 == 0, "f64 exchange area must be 8-byte aligned");
+};
 
-// named barriers: 1-4 = the 4 forward warps of a row group (128 threads), 5-8 = those + the row group's two env warps
-// (192), 9 = all forward threads (the CTA barrier in front of the MMA issue)
-#define Q_BAR(id, count) asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory")
-#define Q_ROWGROUP_SYNC() Q_BAR(1 + (warp & 3), 128)
-#define Q_PUBLISH_SYNC() Q_BAR(5 + (warp & 3), 192)
-#define Q_FWD_SYNC() Q_BAR(9, Q_FWD)
+// named barriers: 1 = the forward threads (in front of the MMA issue, after the staging tile), 2 = the whole CTA
+#define RW_FWD_SYNC() asm volatile("bar.sync 1, %0;" ::"n"(C::FWD) : "memory")
+#define RW_PUBLISH_SYNC() asm volatile("bar.sync 2, %0;" ::"n"(C::NT) : "memory")
 
-template <int NOUT, int ACT>
-__global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlRolloutArgs a) {
+template <int R, int NOUT, int ACT>
+__global__ void __launch_bounds__(RowsCfg<R>::NT, RowsCfg<R>::MIN_CTAS) rollout_cartpole_rows_kernel(const OrlRolloutArgs a) {
+    using C = RowsCfg<R>;
     extern __shared__ __align__(1024) uint8_t smem_f[];
-    const int N = a.n_envs, B = N, d = 4;
+    const int N = a.n_envs, B = N;
     const int n = NOUT == 8 ? a.n_actions : NOUT;
-    const FwdCtx c = fwd_setup(smem_f, a.policy_params, d, n);
-    const int tid = threadIdx.x, warp = tid >> 5, row = tid & 127, qd = tid >> 7, cb = QCW * (qd & 3);
-    float* xs = c.xs;                                   // [4][128][2]
-    float* xh = xs + 4 * F_M * 2;                       // [8][4][128]
-    float* qn = xh + MAX_OUT * 4 * F_M;                 // [2][8][128]
-    int* act_slot = reinterpret_cast<int*>(qn + 2 * MAX_OUT * F_M);   // [2][128]
-    int* termf = act_slot + 2 * F_M;                    // [2][2][128]
-    double* cand = reinterpret_cast<double*>(termf + 4 * F_M);    // [2][2][4][128]
-    double* srs = cand + 2 * 2 * 4 * F_M;               // [2][4][128]
-    const int e = blockIdx.x * F_M + row;               // env == buffer row (single-agent env)
-    const bool valid = e < N;
+    const int tid = threadIdx.x;
+    if constexpr (R < RW_M) {   // the MMA tile's padding rows [R, 64) of the 16 n1 panels: zeroed once, never written again
+        for (int i = tid; i < 16 * (RW_M - R); i += C::NT) {
+            const int p = i / (RW_M - R), r = R + i % (RW_M - R);
+            *reinterpret_cast<uint4*>(smem_f + C::L::R1H + p * C::L::PANEL + r * 16) = make_uint4(0u, 0u, 0u, 0u);
+        }
+    }
+    const FwdCtx c = fwd_setup<typename C::L>(smem_f, a.policy_params, 4, n);
+    float* qn = reinterpret_cast<float*>(smem_f + C::XCH);            // [2][8][R]
+    int* act_slot = reinterpret_cast<int*>(qn + 2 * MAX_OUT * R);     // [2][R]
+    int* termf = act_slot + 2 * R;                                    // [2][2][R]
+    double* cand = reinterpret_cast<double*>(smem_f + C::XCH_F64);    // [2][2][4][R]
+    double* srs = cand + 2 * 2 * 4 * R;                               // [2][4][R]
     const uint64_t rng_base = a.rng_step_base + (a.rng_counter ? *a.rng_counter : 0ull);
-    int elapsed = valid ? a.env_i32[e] : 0;
     uint32_t it = 0;
-    if (qd >= 4) {
-        // ================= env groups: one action each, one step ahead of the sampling ==================================
-        const int my_act = qd - 4;
+    if (tid >= C::FWD) {
+        // ================= env threads: one action each, one step ahead of the sampling =================================
+        const int my_act = (tid - C::FWD) / R, row = (tid - C::FWD) % R;
+        const int e = blockIdx.x * R + row;
+        const bool valid = e < N;
+        int elapsed = valid ? a.env_i32[e] : 0;
         double s[4] = {0, 0, 0, 0};
         Pcg64 g; g.state = 0; g.inc = 0;
         if (valid) {
@@ -374,36 +396,36 @@ __global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlR
             float q[MAX_OUT];
             row_noise<NOUT>(a, n, (size_t)a.t_begin * B + e, rng_base + (uint64_t)a.t_begin, e, q);
 #pragma unroll
-            for (int j = 0; j < MAX_OUT; ++j) if (j < n) qn[j * F_M + row] = q[j];
+            for (int j = 0; j < MAX_OUT; ++j) if (j < n) qn[j * R + row] = q[j];
         }
-        Q_PUBLISH_SYNC();
+        RW_PUBLISH_SYNC();
         for (int t = a.t_begin; t < a.t_end; ++t, ++it) {
             const uint32_t pb = it & 1u;
             double cs[4] = {s[0], s[1], s[2], s[3]};
             const bool term = cartpole_dynamics(cs, my_act);
 #pragma unroll
-            for (int k = 0; k < 4; ++k) cand[((pb * 2 + my_act) * 4 + k) * F_M + row] = cs[k];
-            termf[(pb * 2 + my_act) * F_M + row] = term ? 1 : 0;
+            for (int k = 0; k < 4; ++k) cand[((pb * 2 + my_act) * 4 + k) * R + row] = cs[k];
+            termf[(pb * 2 + my_act) * R + row] = term ? 1 : 0;
             Pcg64 g2 = g;
             if (my_act == 0) {
                 double sr[4];
                 cartpole_reset(sr, g2);
 #pragma unroll
-                for (int k = 0; k < 4; ++k) srs[(pb * 4 + k) * F_M + row] = sr[k];
+                for (int k = 0; k < 4; ++k) srs[(pb * 4 + k) * R + row] = sr[k];
             } else if (draw && t + 1 < a.t_end) {   // noise of the next step, into the other parity
                 float q[MAX_OUT];
                 row_noise<NOUT>(a, n, (size_t)(t + 1) * B + e, rng_base + (uint64_t)(t + 1), e, q);
 #pragma unroll
-                for (int j = 0; j < MAX_OUT; ++j) if (j < n) qn[((pb ^ 1u) * MAX_OUT + j) * F_M + row] = q[j];
+                for (int j = 0; j < MAX_OUT; ++j) if (j < n) qn[((pb ^ 1u) * MAX_OUT + j) * R + row] = q[j];
             }
-            Q_PUBLISH_SYNC();   // candidates out, action in
-            const int act = act_slot[pb * F_M + row] & 1;
-            const bool terminated = termf[(pb * 2 + act) * F_M + row] != 0;
+            RW_PUBLISH_SYNC();   // candidates out, action in
+            const int act = act_slot[pb * R + row] & 1;
+            const bool terminated = termf[(pb * 2 + act) * R + row] != 0;
             elapsed += 1;
             const bool done = terminated || (elapsed >= 500);
-            const double* src = done ? srs + (size_t)pb * 4 * F_M : cand + (size_t)(pb * 2 + act) * 4 * F_M;
+            const double* src = done ? srs + (size_t)pb * 4 * R : cand + (size_t)(pb * 2 + act) * 4 * R;
 #pragma unroll
-            for (int k = 0; k < 4; ++k) s[k] = src[k * F_M + row];
+            for (int k = 0; k < 4; ++k) s[k] = src[k * R + row];
             if (done) { elapsed = 0; g = g2; }
         }
         if (valid && my_act == 0) {
@@ -414,13 +436,17 @@ __global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlR
         }
     } else {
         // ================= forward quarters =================================================================================
+        const int warp = tid >> 5, lane = tid & 31, row = tid >> 2, qd = tid & 3, cb = QCW * qd, qbase = lane & ~3;
+        const int e = blockIdx.x * R + row;
+        const bool valid = e < N;
+        int elapsed = valid ? a.env_i32[e] : 0;
         int len = 0;
         float ret = 0.f;
         if (valid && qd == 0) { ret = a.ep_return[e]; len = a.ep_length[e]; }
         float x[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) x[k] = valid ? a.policy_obs[((size_t)a.t_begin * B + e) * 4 + k] : 0.f;
-        Q_PUBLISH_SYNC();   // the first step's noise is in place
+        RW_PUBLISH_SYNC();   // the first step's noise is in place
         for (int t = a.t_begin; t < a.t_end; ++t, ++it) {
             const uint32_t pb = it & 1u;
             const size_t grow = (size_t)t * B + (valid ? e : 0);
@@ -443,12 +469,11 @@ __global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlR
             float sm = 0.f, sq = 0.f;
 #pragma unroll
             for (int i = 0; i < QCW; ++i) { n1[i] = f_act<ACT>(n1[i], a.activation_id); sm += n1[i]; sq = fmaf(n1[i], n1[i], sq); }
-            *reinterpret_cast<float2*>(xs + (qd * F_M + row) * 2) = make_float2(sm, sq);
-            Q_ROWGROUP_SYNC();
             {   // all quarters add the four partials in the same order -> identical statistics
-                sm = 0.f; sq = 0.f;
+                float ts = 0.f, tq = 0.f;
 #pragma unroll
-                for (int p = 0; p < 4; ++p) { const float2 o = *reinterpret_cast<const float2*>(xs + (p * F_M + row) * 2); sm += o.x; sq += o.y; }
+                for (int p = 0; p < 4; ++p) { ts += __shfl_sync(0xffffffffu, sm, qbase + p); tq += __shfl_sync(0xffffffffu, sq, qbase + p); }
+                sm = ts; sq = tq;
             }
             const float mu1 = sm * (1.f / H);
             const float rstd1 = 1.0f / sqrtf(fmaxf(sq * (1.f / H) - mu1 * mu1, 0.f) + LN_EPS);
@@ -456,30 +481,38 @@ __global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlR
             for (int i = 0; i < QCW; ++i) n1[i] = (n1[i] - mu1) * rstd1;
 #pragma unroll
             for (int q8 = 0; q8 < QCW; q8 += 8) {
-                const uint32_t off = (uint32_t)((cb + q8) >> 3) * FPANEL + row * 16;
+                const uint32_t off = (uint32_t)((cb + q8) >> 3) * C::L::PANEL + row * 16;
                 split_store8(c.R1h + off, c.R1l + off, n1 + q8, 1.0f);
             }
             fence_proxy_async();
-            Q_FWD_SYNC();
-            {   // Z3 = n1 . W3f^T: warpgroup qd computes rows [64 (qd & 1), +64) x columns [32 (qd >> 1), +32)
-                const uint64_t dK_A = desc_const(FPANEL, 128), dK_W = desc_const(FPANEL_W, 128);
-                const int mb = qd & 1, nb = qd >> 1;
-                float z[16];
+            RW_FWD_SYNC();
+            {   // Z3 = n1 . W3f^T over R1 rows [0, 64): warpgroup wg computes the column halves [nb0, nb0 + NB)
+                const uint64_t dK_A = desc_const(C::L::PANEL, 128), dK_W = desc_const(FPANEL_W, 128);
+                const int nb0 = (warp >> 2) * C::NB;
+                float z[C::NB][16];
 #pragma unroll
-                for (int i = 0; i < 16; ++i) z[i] = 0.f;
+                for (int b = 0; b < C::NB; ++b)
+#pragma unroll
+                    for (int i = 0; i < 16; ++i) z[b][i] = 0.f;
                 wgmma_fence();
 #pragma unroll
                 for (int pass = 0; pass < 3; ++pass) {
-                    const uint32_t aa = (pass == 0 ? c.aR1l : c.aR1h) + mb * 64 * 16, bb = (pass == 1 ? c.aWl : c.aWh) + nb * 32 * 16;
+                    const uint32_t aa = pass == 0 ? c.aR1l : c.aR1h, bb = pass == 1 ? c.aWl : c.aWh;
 #pragma unroll
                     for (int kk = 0; kk < 4; ++kk)
-                        wgmma_f16_n32<0, 0>(z, desc_at(dK_A, aa + 2 * kk * FPANEL), desc_at(dK_W, bb + 2 * kk * FPANEL_W), (pass | kk) > 0);
+#pragma unroll
+                        for (int b = 0; b < C::NB; ++b)
+                            wgmma_f16_n32<0, 0>(z[b], desc_at(dK_A, aa + 2 * kk * C::L::PANEL),
+                                                desc_at(dK_W, bb + (nb0 + b) * 32 * 16 + 2 * kk * FPANEL_W), (pass | kk) > 0);
                 }
                 wgmma_commit();
                 wgmma_wait<0>();
-                frag_store<32>(z, c.S + mb * 64 * S_LD + 32 * nb, S_LD);
+                if (16 * (warp & 3) < R) {   // fragment rows 16 (warp % 4) + [0, 16): only real rows go to the staging tile
+#pragma unroll
+                    for (int b = 0; b < C::NB; ++b) frag_store<32>(z[b], c.S + 32 * (nb0 + b), S_LD);
+                }
             }
-            Q_FWD_SYNC();   // the staging tile is complete; the next step's stores follow its forward barrier in front of the MMAs
+            RW_FWD_SYNC();   // the staging tile is complete; the next step's stores follow its forward barrier in front of the MMAs
             float n3[QCW];
 #pragma unroll
             for (int q4 = 0; q4 < QCW; q4 += 4) {
@@ -489,14 +522,11 @@ __global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlR
             float s3 = 0.f, q3 = 0.f;
 #pragma unroll
             for (int i = 0; i < QCW; ++i) { n3[i] += c.b3f[cb + i]; s3 += n3[i]; q3 = fmaf(n3[i], n3[i], q3); }
-            __syncwarp();
-            // slot xs is free again: every partner read of exchange 1 happened before the forward barrier above
-            *reinterpret_cast<float2*>(xs + (qd * F_M + row) * 2) = make_float2(s3, q3);
-            Q_ROWGROUP_SYNC();
             {
-                s3 = 0.f; q3 = 0.f;
+                float ts = 0.f, tq = 0.f;
 #pragma unroll
-                for (int p = 0; p < 4; ++p) { const float2 o = *reinterpret_cast<const float2*>(xs + (p * F_M + row) * 2); s3 += o.x; q3 += o.y; }
+                for (int p = 0; p < 4; ++p) { ts += __shfl_sync(0xffffffffu, s3, qbase + p); tq += __shfl_sync(0xffffffffu, q3, qbase + p); }
+                s3 = ts; q3 = tq;
             }
             const float mu3 = s3 * (1.f / H);
             const float rstd3 = 1.0f / sqrtf(fmaxf(q3 * (1.f / H) - mu3 * mu3, 0.f) + LN_EPS);
@@ -512,35 +542,38 @@ __global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlR
                     out[j] = fmaf(n3[q4], wv.x, fmaf(n3[q4 + 1], wv.y, fmaf(n3[q4 + 2], wv.z, fmaf(n3[q4 + 3], wv.w, out[j]))));
                 }
             }
-            F_FOR_OUT(j) xh[(j * 4 + qd) * F_M + row] = out[j];   // [j][quarter][row]: conflict-free
-            Q_ROWGROUP_SYNC();
-            // ---- quarter 0: logits, sampling, action outputs ----
+            float logit[MAX_OUT];
+#pragma unroll
+            for (int j = 0; j < MAX_OUT; ++j) logit[j] = 0.f;
+            F_FOR_OUT(j) {
+                const float p0 = __shfl_sync(0xffffffffu, out[j], qbase), p1 = __shfl_sync(0xffffffffu, out[j], qbase + 1);
+                const float p2 = __shfl_sync(0xffffffffu, out[j], qbase + 2), p3 = __shfl_sync(0xffffffffu, out[j], qbase + 3);
+                logit[j] = ((p0 + p1) + (p2 + p3)) + c.bhf[j];
+            }
+            // ---- quarter 0: sampling, action outputs ----
             if (qd == 0) {
                 int act = 0;
                 if (valid) {
-                    float logit[MAX_OUT], q[MAX_OUT];
+                    float q[MAX_OUT];
 #pragma unroll
-                    for (int j = 0; j < MAX_OUT; ++j) { logit[j] = 0.f; q[j] = 1.f; }
-                    F_FOR_OUT(j) {
-                        logit[j] = ((xh[(j * 4 + 0) * F_M + row] + xh[(j * 4 + 1) * F_M + row]) + (xh[(j * 4 + 2) * F_M + row] + xh[(j * 4 + 3) * F_M + row])) + c.bhf[j];
-                        if (!a.deterministic) q[j] = qn[(pb * MAX_OUT + j) * F_M + row];
-                    }
+                    for (int j = 0; j < MAX_OUT; ++j) q[j] = 1.f;
+                    if (!a.deterministic) { F_FOR_OUT(j) q[j] = qn[(pb * MAX_OUT + j) * R + row]; }
                     float lp;
                     act = sample_row<NOUT>(logit, n, q, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0, lp);
                     a.actions[grow] = (float)act;
                     a.action_log_probs[grow] = lp;
                 }
-                act_slot[pb * F_M + row] = act;
+                act_slot[pb * R + row] = act;
             }
-            Q_PUBLISH_SYNC();   // action out, candidates in; orders every exchange slot against the next step's writes
+            RW_PUBLISH_SYNC();   // action out, candidates in; orders every exchange slot against the next step's writes
             // ---- commit env.step (sync_venv.py:213-218 auto-reset): every thread of the row picks the same candidate ----
-            const int act = act_slot[pb * F_M + row] & 1;
-            const bool terminated = termf[(pb * 2 + act) * F_M + row] != 0;
+            const int act = act_slot[pb * R + row] & 1;
+            const bool terminated = termf[(pb * 2 + act) * R + row] != 0;
             elapsed += 1;
             const bool done = terminated || (elapsed >= 500);
-            const double* src = done ? srs + (size_t)pb * 4 * F_M : cand + (size_t)(pb * 2 + act) * 4 * F_M;
+            const double* src = done ? srs + (size_t)pb * 4 * R : cand + (size_t)(pb * 2 + act) * 4 * R;
 #pragma unroll
-            for (int k = 0; k < 4; ++k) x[k] = (float)src[k * F_M + row];
+            for (int k = 0; k < 4; ++k) x[k] = (float)src[k * R + row];
             if (done) elapsed = 0;
             if (qd == 0 && valid) {
                 ret += 1.0f; len += 1;
@@ -560,6 +593,8 @@ __global__ void __launch_bounds__(Q_NT, 1) rollout_cartpole_q5_kernel(const OrlR
         if (valid && qd == 0) { a.ep_return[e] = ret; a.ep_length[e] = len; }
     }
 }
+#undef RW_FWD_SYNC
+#undef RW_PUBLISH_SYNC
 
 template <typename K>
 int prepare_kernel(K kern, uint32_t smem_bytes = F_SMEM) {
@@ -573,6 +608,20 @@ int prepare_kernel(K kern, uint32_t smem_bytes = F_SMEM) {
         done[key] = true;
     }
     return 0;
+}
+
+template <int R>
+int launch_rollout_rows(const OrlRolloutArgs& a, cudaStream_t st) {
+    using C = RowsCfg<R>;
+    const int grid = (a.n_envs + R - 1) / R;
+    if (a.activation_id == 1) {
+        if (int e = prepare_kernel(rollout_cartpole_rows_kernel<R, 2, 1>, C::SMEM)) return e;
+        rollout_cartpole_rows_kernel<R, 2, 1><<<grid, C::NT, C::SMEM, st>>>(a);
+    } else {
+        if (int e = prepare_kernel(rollout_cartpole_rows_kernel<R, 2, -1>, C::SMEM)) return e;
+        rollout_cartpole_rows_kernel<R, 2, -1><<<grid, C::NT, C::SMEM, st>>>(a);
+    }
+    return check_cuda(cudaGetLastError(), "rollout_cartpole_rows_kernel");
 }
 
 }  // namespace
@@ -617,13 +666,10 @@ int launch_rollout_tc(const OrlRolloutArgs& a, cudaStream_t st) {
     } while (0)
     static const bool q5 = [] { const char* v = getenv("ORL_ROLLOUT_Q5"); return !(v && atoi(v) == 0); }();
     if (a.env_kind == ORL_ENV_CARTPOLE && q5) {
-        if (a.activation_id == 1) {
-            if (int e_ = prepare_kernel(rollout_cartpole_q5_kernel<2, 1>, Q_SMEM)) return e_;
-            rollout_cartpole_q5_kernel<2, 1><<<grid, Q_NT, Q_SMEM, st>>>(a);
-        } else {
-            if (int e_ = prepare_kernel(rollout_cartpole_q5_kernel<2, -1>, Q_SMEM)) return e_;
-            rollout_cartpole_q5_kernel<2, -1><<<grid, Q_NT, Q_SMEM, st>>>(a);
-        }
+        // R = 32 envs per CTA: the envs spread over the most SMs, and each SM issues the forward of the fewest rows per
+        // step (DESIGN.md §6 has R = 32 against R = 64).  ORL_ROLLOUT_ROWS=64 selects R = 64.
+        static const bool rows64 = [] { const char* v = getenv("ORL_ROLLOUT_ROWS"); return v && atoi(v) == 64; }();
+        return rows64 ? launch_rollout_rows<64>(a, st) : launch_rollout_rows<32>(a, st);
     } else if (a.env_kind == ORL_ENV_CARTPOLE) ORL_RTC(ORL_ENV_CARTPOLE, 2);
     else ORL_RTC(ORL_ENV_GRIDWORLD, 5);
 #undef ORL_RTC
