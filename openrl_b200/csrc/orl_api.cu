@@ -1,4 +1,4 @@
-// Library-level C-ABI entry points: version, error string, device query.
+// Library-level C-ABI entry points: version, error string, device query; the rollouts' noise-counter bump.
 #include <stdarg.h>
 #include <string.h>
 
@@ -30,6 +30,14 @@ int sm_count() {
         cached[dev] = n;
     }
     return cached[dev];
+}
+
+__global__ void bump_rng_counter_kernel(uint64_t* c, uint64_t by) { *c += by; }
+
+int bump_rng_counter(uint64_t* counter, int steps, cudaStream_t st) {
+    if (!counter) return 0;
+    bump_rng_counter_kernel<<<1, 1, 0, st>>>(counter, (uint64_t)steps);
+    return check_cuda(cudaGetLastError(), "bump_rng_counter_kernel");
 }
 }  // namespace orl
 

@@ -11,6 +11,9 @@ namespace orl {
 void set_last_error(const char* fmt, ...);
 int check_cuda(cudaError_t e, const char* what);
 int sm_count();
+// advances the device Philox step counter of the action noise by the `steps` steps a rollout launch consumed; no-op
+// when `counter` is null
+int bump_rng_counter(uint64_t* counter, int steps, cudaStream_t st);
 
 #define ORL_CHECK_ARG(cond, msg)                                   \
     do {                                                           \

@@ -1,5 +1,5 @@
-// Device-side env.step wrappers (auto-reset + episode statistics) and the categorical sampler shared by the
-// feed-forward rollout (orl_rollout.cu) and the recurrent rollout (orl_rnn.cu).
+// Device-side env.step wrappers (auto-reset + episode statistics) and the action sampler (noise, masking, sampling,
+// log-prob) shared by every rollout kernel.
 #pragma once
 #include "orl_envs.cuh"
 #include "orl_mlp.cuh"
@@ -99,14 +99,74 @@ __device__ __forceinline__ void env_step_mpe(const EnvPtrs& E, int e, int N, con
     for (int ag = 0; ag < 3; ++ag) mpe_obs(s, ag, ob[ag]);
 }
 
-__device__ __forceinline__ int sample_categorical(const float (&p)[MAX_OUT], int n, const float (&q)[MAX_OUT]) {
-    // torch.multinomial(probs, 1) == argmax(probs / q), first index wins ties
-    int best = 0;
-    float bv = p[0] / q[0];
+// ---- the action sampler of every rollout kernel ------------------------------------------------------------------------
+// Philox4x32-10 block `lane` of the action randomness of (step, row): key = seed, counter = (step lo, step hi, row, lane).
+// The row is the GLOBAL row (local row + rng_row_offset) wherever the kernel knows it, so an env-sharded run draws the
+// same noise as the unsharded one.
+__device__ __forceinline__ uint4 action_philox(uint64_t seed, uint64_t step, uint32_t row, uint32_t lane) {
+    const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+    return philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), row, lane), key);
+}
+
+// Exp(1) noise q[0..n) of (step, row): the reference-order table exp_noise[grow * n + j] when one is given (parity mode),
+// else -log U of the 8 draws of Philox lanes `lane`, `lane + 1`.
+__device__ __forceinline__ void action_noise(const float* exp_noise, size_t grow, int n, uint64_t seed, uint64_t step,
+                                             uint32_t row, float (&q)[MAX_OUT], uint32_t lane = 0u) {
+    if (exp_noise) {
 #pragma unroll
-    for (int j = 1; j < MAX_OUT; ++j)
-        if (j < n) { const float v = p[j] / q[j]; if (v > bv) { bv = v; best = j; } }
-    return best;
+        for (int j = 0; j < MAX_OUT; ++j) q[j] = (j < n) ? exp_noise[grow * n + j] : 1.f;
+    } else {
+        const uint4 r0 = action_philox(seed, step, row, lane), r1 = action_philox(seed, step, row, lane + 1u);
+        const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
+#pragma unroll
+        for (int j = 0; j < MAX_OUT; ++j) q[j] = -logf(u32_to_unit_open(rr[j]));
+    }
+}
+
+// log_softmax_n of a row's logits with the masked-out actions (mask row entry 0, nullable) at -6e4
+__device__ __forceinline__ void masked_log_softmax(float (&logit)[MAX_OUT], int n, const float* mask_row,
+                                                   float (&nl)[MAX_OUT], float (&pr)[MAX_OUT]) {
+    if (mask_row) {
+#pragma unroll
+        for (int j = 0; j < MAX_OUT; ++j)
+            if (j < n && mask_row[j] == 0.f) logit[j] = -6e4f;
+    }
+    log_softmax_n(logit, n, nl, pr);
+}
+
+// log-prob of action `act`; an action outside [0, n) gets nl[0]
+__device__ __forceinline__ float log_prob_of(const float (&nl)[MAX_OUT], int n, int act) {
+    float lp = nl[0];
+#pragma unroll
+    for (int j = 1; j < MAX_OUT; ++j) if (j < n && j == act) lp = nl[j];
+    return lp;
+}
+
+// Categorical action of one row and its log-prob: the first-max mode when deterministic, else torch.multinomial(probs, 1)
+// == argmax(probs / q) (first index wins ties) over the Exp(1) noise q that `noise(q)` writes.  The noise is asked for
+// only on the stochastic branch, after the log-softmax, so a kernel that draws it there keeps q short-lived.
+template <typename Noise>
+__device__ __forceinline__ int sample_action(float (&logit)[MAX_OUT], int n, const float* mask_row, bool deterministic,
+                                             Noise&& noise, float& lp) {
+    float nl[MAX_OUT], pr[MAX_OUT];
+    masked_log_softmax(logit, n, mask_row, nl, pr);
+    int act;
+    if (deterministic) {
+        act = 0;
+#pragma unroll
+        for (int j = 1; j < MAX_OUT; ++j) if (j < n && pr[j] > pr[act]) act = j;
+    } else {
+        float q[MAX_OUT];
+        noise(q);
+        int best = 0;
+        float bv = pr[0] / q[0];
+#pragma unroll
+        for (int j = 1; j < MAX_OUT; ++j)
+            if (j < n) { const float v = pr[j] / q[j]; if (v > bv) { bv = v; best = j; } }
+        act = best;
+    }
+    lp = log_prob_of(nl, n, act);
+    return act;
 }
 
 }  // namespace orl

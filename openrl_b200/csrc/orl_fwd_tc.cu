@@ -4,10 +4,13 @@
 //   critic_values_tc_kernel : ValueNetwork.forward over a flat batch of rows (value_network.py:113-136), the
 //                             (T+1)*B-row pass of OnPolicyDriver.compute_returns (onpolicy_driver.py:206-215).
 //   rollout_tc_kernel       : the fused rollout (policy forward + Categorical sampling + device env.step + in-place
-//                             buffer insert, onpolicy_driver.py:154-203,236-279) for single-agent device envs
-//                             (CartPole-v1, GridWorldEnv): a CTA owns 128 envs for all T steps, ONE launch.
+//                             buffer insert, onpolicy_driver.py:154-203,236-279) for GridWorldEnv: a CTA owns 128 envs
+//                             for all T steps, ONE launch.
+//   rollout_cartpole_rows_kernel : the same for CartPole-v1 with 32 envs per CTA and the physics one step ahead
+//                             (layout below, before the kernel).
 //
-// CTA = 256 threads = 128 rows x 2 column halves (warps w, w+4 share rows [32(w%4), +32)).
+// critic_values_tc_kernel and rollout_tc_kernel: CTA = 256 threads = 128 rows x 2 column halves (warps w, w+4 share rows
+// [32(w%4), +32)).
 // Per 128-row tile: fc1 (K = d <= 8, FFMA) + activation + LayerNorm-1 in registers -> n1 as fp16 hi/lo panels ->
 // Z3 = n1 . W3f^T as 12 wgmma (3 split passes x K/16; warpgroup g computes rows [64g, +64)) -> fp32 staging tile in
 // shared memory -> every thread reads its row's columns -> LayerNorm-3 + head in registers.  The rollout's
@@ -227,54 +230,11 @@ __global__ void __launch_bounds__(F_NT, 2) critic_values_tc_kernel(const float* 
     }
 }
 
-// Categorical sampling of one row from its logits (rollout tail, half 0): masks, log-softmax, argmax / multinomial rule
-template <int NOUT>
-__device__ __forceinline__ int sample_row(float (&logit)[MAX_OUT], int n, const float (&q)[MAX_OUT], const float* __restrict__ mask_row,
-                                          bool deterministic, float& lp) {
-    if (mask_row) {
-#pragma unroll
-        for (int j = 0; j < MAX_OUT; ++j)
-            if (j < n && mask_row[j] == 0.f) logit[j] = -6e4f;
-    }
-#pragma unroll
-    for (int j = 0; j < MAX_OUT; ++j) if (j >= n) logit[j] = 0.f;
-    float nl[MAX_OUT], pr[MAX_OUT];
-    log_softmax_n(logit, n, nl, pr);
-    int act;
-    if (deterministic) {
-        act = 0;
-#pragma unroll
-        for (int j = 1; j < MAX_OUT; ++j) if (j < n && pr[j] > pr[act]) act = j;
-    } else {
-        act = sample_categorical(pr, n, q);   // argmax(probs / q): torch.multinomial's rule, as in the FFMA kernel
-    }
-    lp = nl[0];
-#pragma unroll
-    for (int j = 1; j < MAX_OUT; ++j) if (j == act) lp = nl[j];
-    return act;
-}
-
-// Exp(1) noise of (step t, row): the supplied reference-order table, else Philox4x32-10 keyed by the seed
-template <int NOUT>
-__device__ __forceinline__ void row_noise(const OrlRolloutArgs& a, int n, size_t grow, uint64_t step, int e, float (&q)[MAX_OUT]) {
-    if (a.exp_noise) {
-#pragma unroll
-        for (int j = 0; j < MAX_OUT; ++j) q[j] = (j < n) ? a.exp_noise[grow * n + j] : 1.f;
-    } else {
-        const uint2 key = make_uint2((uint32_t)a.rng_seed, (uint32_t)(a.rng_seed >> 32));
-        const uint4 r0 = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)(e + a.rng_row_offset), 0u), key);
-        const uint4 r1 = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)(e + a.rng_row_offset), 1u), key);
-        const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-        for (int j = 0; j < MAX_OUT; ++j) q[j] = -logf(u32_to_unit_open(rr[j]));
-    }
-}
-
-template <int ENV, int NOUT, int ACT>
+template <int ACT>
 __global__ void __launch_bounds__(F_NT, 1) rollout_tc_kernel(const OrlRolloutArgs a) {
     extern __shared__ __align__(1024) uint8_t smem_f[];
-    const int N = a.n_envs, B = N, d = a.obs_dim;
-    const int n = NOUT == 8 ? a.n_actions : NOUT;
+    constexpr int NOUT = 5;   // GridWorldEnv's actions
+    const int N = a.n_envs, B = N, d = a.obs_dim, n = NOUT;
     const FwdCtx c = fwd_setup(smem_f, a.policy_params, d, n);
     const int tid = threadIdx.x, warp = tid >> 5, row = tid & 127, half = tid >> 7;
     const int e = blockIdx.x * F_M + row;          // env == buffer row (single-agent envs)
@@ -289,18 +249,20 @@ __global__ void __launch_bounds__(F_NT, 1) rollout_tc_kernel(const OrlRolloutArg
             float q[MAX_OUT];
             const size_t grow = (size_t)t * B + (valid ? e : 0);
             fwd_tile<NOUT, ACT>(c, x, d, n, a.activation_id, logit, [&] {
-                if (half == 0 && valid && !a.deterministic) row_noise<NOUT>(a, n, grow, rng_base + (uint64_t)t, e, q);
+                if (half == 0 && valid && !a.deterministic)
+                    action_noise(a.exp_noise, grow, n, a.rng_seed, rng_base + (uint64_t)t, (uint32_t)(e + a.rng_row_offset), q);
             });
             if (half == 0 && valid) {
                 float lp;
-                const int act = sample_row<NOUT>(logit, n, q, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0, lp);
+                const int act = sample_action(logit, n, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0,
+                                              [&](float (&qs)[MAX_OUT]) { for (int j = 0; j < MAX_OUT; ++j) qs[j] = q[j]; }, lp);
                 a.actions[grow] = (float)act;
                 a.action_log_probs[grow] = lp;
                 // ---- env.step of this thread's env, in-place insert into slot t / t+1 ----
                 EnvPtrs E{a.env_f64, a.env_u64, a.env_i32, a.env_table, a.env_table_len, a.rng_seed,
                           a.ep_return, a.ep_length, a.episode_stats, a.rng_row_offset};
                 float ob[4], fin[4], reward; bool done;
-                env_step_single(E, ENV, e, N, act, ob, reward, done, fin);
+                env_step_single(E, ORL_ENV_GRIDWORLD, e, N, act, ob, reward, done, fin);
                 const size_t o1 = (size_t)(t + 1) * B + e;
                 *reinterpret_cast<float4*>(a.policy_obs + o1 * 4) = make_float4(ob[0], ob[1], ob[2], ob[3]);
                 a.rewards[grow] = reward;
@@ -321,14 +283,13 @@ __global__ void __launch_bounds__(F_NT, 1) rollout_tc_kernel(const OrlRolloutArg
 // ---- CartPole rollout: R envs per CTA, 4 forward lanes + 2 env threads per env -------------------------------------
 // The rollout is a chain of T dependent steps whose length is one row's work.  The f64 CartPole physics (sin / cos and
 // three dependent divides: ~250 dependent instructions) is a large share of a step when it runs after sampling, the
-// policy forward most of the rest.  A CTA owns R = 32 (or 64) envs, so 4096 envs spread over 128 CTAs, one per SM, and
-// each SM issues the forward of R rows instead of 128:
+// policy forward most of the rest.  A CTA owns R = 32 envs, so 4096 envs spread over 128 CTAs, one per SM, and each SM
+// issues the forward of 32 rows instead of 128 (DESIGN.md §6 has R = 32 against the removed R = 64):
 //   * Forward: 4R threads = R rows x 4 column quarters, the 4 quarters of a row in one warp (lane = 4 row + quarter,
 //     quarter qd owns hidden columns [16 qd, +16)); the LayerNorm and head partials meet through shuffles, added in a
-//     fixed order.  The fc3 GEMM is one M = 64 tile over R1 rows [0, 64) (rows [R, 64) zero padding when R = 32):
-//     with R = 32 the one forward warpgroup computes both 32-column halves, with R = 64 warpgroup g computes columns
-//     [32 g, +32).  Each Z3 element is the same wgmma_f16_n32 chain (Al.Bh, Ah.Bl, Ah.Bh; kk = 0..3) as in the
-//     row-parallel kernels.
+//     fixed order.  The fc3 GEMM is one M = 64 tile over R1 rows [0, 64) (rows [R, 64) zero padding): the one forward
+//     warpgroup computes both 32-column halves.  Each Z3 element is the same wgmma_f16_n32 chain (Al.Bh, Ah.Bl, Ah.Bh;
+//     kk = 0..3) as in the row-parallel kernels.
 //   * Env: 2R threads, lane = row.  As soon as the state of step t is known, the action-0 threads advance the physics
 //     for action 0 and draw the reset state (PCG64), the action-1 threads advance the physics for action 1 and draw the
 //     sampling noise of step t+1 - concurrently with the whole forward pass of step t - and publish the candidates
@@ -337,13 +298,11 @@ __global__ void __launch_bounds__(F_NT, 1) rollout_tc_kernel(const OrlRolloutArg
 // (publish the action, every thread picks the candidate).  Same functions and explicitly rounded f64 operations as
 // env_step_single -> bit-identical trajectories.
 constexpr int QCW = 16, RW_M = 64;
-template <int R>
 struct RowsCfg {
-    static_assert(R == 32 || R == 64, "R1 holds 64 rows; a warpgroup of forward threads owns 32 of them");
-    static constexpr int FWD = 4 * R, NT = 6 * R, NWG = R / 32, NB = 2 / NWG;   // NB: 32-column halves per warpgroup
-    // resident CTAs per SM the register budget is sized for: with R = 32, three (96 registers, no spills; four would
-    // spill), so up to 3 x 32 x #SMs envs run in one wave; R = 64 needs ~146 registers (one CTA per SM)
-    static constexpr int MIN_CTAS = R == 32 ? 3 : 1;
+    static constexpr int R = 32, FWD = 4 * R, NT = 6 * R;
+    // resident CTAs per SM the register budget is sized for: three (96 registers, no spills; four would spill), so up
+    // to 3 x 32 x #SMs envs run in one wave
+    static constexpr int MIN_CTAS = 3;
     using L = FwdLayout<RW_M, R>;
     // exchange area: qn[2 parity][8][R] | act[2][R] (int) | termf[2][2][R] (int) | f64: cand[2 parity][2 action][4][R]
     // srs[2 parity][4][R]
@@ -357,18 +316,17 @@ struct RowsCfg {
 #define RW_FWD_SYNC() asm volatile("bar.sync 1, %0;" ::"n"(C::FWD) : "memory")
 #define RW_PUBLISH_SYNC() asm volatile("bar.sync 2, %0;" ::"n"(C::NT) : "memory")
 
-template <int R, int NOUT, int ACT>
-__global__ void __launch_bounds__(RowsCfg<R>::NT, RowsCfg<R>::MIN_CTAS) rollout_cartpole_rows_kernel(const OrlRolloutArgs a) {
-    using C = RowsCfg<R>;
+template <int ACT>
+__global__ void __launch_bounds__(RowsCfg::NT, RowsCfg::MIN_CTAS) rollout_cartpole_rows_kernel(const OrlRolloutArgs a) {
+    using C = RowsCfg;
+    constexpr int R = C::R, NOUT = 2;   // CartPole's actions
     extern __shared__ __align__(1024) uint8_t smem_f[];
-    const int N = a.n_envs, B = N;
-    const int n = NOUT == 8 ? a.n_actions : NOUT;
+    const int N = a.n_envs, B = N, n = NOUT;
     const int tid = threadIdx.x;
-    if constexpr (R < RW_M) {   // the MMA tile's padding rows [R, 64) of the 16 n1 panels: zeroed once, never written again
-        for (int i = tid; i < 16 * (RW_M - R); i += C::NT) {
-            const int p = i / (RW_M - R), r = R + i % (RW_M - R);
-            *reinterpret_cast<uint4*>(smem_f + C::L::R1H + p * C::L::PANEL + r * 16) = make_uint4(0u, 0u, 0u, 0u);
-        }
+    // the MMA tile's padding rows [R, 64) of the 16 n1 panels: zeroed once, never written again
+    for (int i = tid; i < 16 * (RW_M - R); i += C::NT) {
+        const int p = i / (RW_M - R), r = R + i % (RW_M - R);
+        *reinterpret_cast<uint4*>(smem_f + C::L::R1H + p * C::L::PANEL + r * 16) = make_uint4(0u, 0u, 0u, 0u);
     }
     const FwdCtx c = fwd_setup<typename C::L>(smem_f, a.policy_params, 4, n);
     float* qn = reinterpret_cast<float*>(smem_f + C::XCH);            // [2][8][R]
@@ -394,7 +352,7 @@ __global__ void __launch_bounds__(RowsCfg<R>::NT, RowsCfg<R>::MIN_CTAS) rollout_
         const bool draw = my_act == 1 && valid && !a.deterministic;
         if (draw) {   // noise of the first step
             float q[MAX_OUT];
-            row_noise<NOUT>(a, n, (size_t)a.t_begin * B + e, rng_base + (uint64_t)a.t_begin, e, q);
+            action_noise(a.exp_noise, (size_t)a.t_begin * B + e, n, a.rng_seed, rng_base + (uint64_t)a.t_begin, (uint32_t)(e + a.rng_row_offset), q);
 #pragma unroll
             for (int j = 0; j < MAX_OUT; ++j) if (j < n) qn[j * R + row] = q[j];
         }
@@ -414,7 +372,7 @@ __global__ void __launch_bounds__(RowsCfg<R>::NT, RowsCfg<R>::MIN_CTAS) rollout_
                 for (int k = 0; k < 4; ++k) srs[(pb * 4 + k) * R + row] = sr[k];
             } else if (draw && t + 1 < a.t_end) {   // noise of the next step, into the other parity
                 float q[MAX_OUT];
-                row_noise<NOUT>(a, n, (size_t)(t + 1) * B + e, rng_base + (uint64_t)(t + 1), e, q);
+                action_noise(a.exp_noise, (size_t)(t + 1) * B + e, n, a.rng_seed, rng_base + (uint64_t)(t + 1), (uint32_t)(e + a.rng_row_offset), q);
 #pragma unroll
                 for (int j = 0; j < MAX_OUT; ++j) if (j < n) qn[((pb ^ 1u) * MAX_OUT + j) * R + row] = q[j];
             }
@@ -486,12 +444,12 @@ __global__ void __launch_bounds__(RowsCfg<R>::NT, RowsCfg<R>::MIN_CTAS) rollout_
             }
             fence_proxy_async();
             RW_FWD_SYNC();
-            {   // Z3 = n1 . W3f^T over R1 rows [0, 64): warpgroup wg computes the column halves [nb0, nb0 + NB)
+            {   // Z3 = n1 . W3f^T over R1 rows [0, 64), both 32-column halves b
                 const uint64_t dK_A = desc_const(C::L::PANEL, 128), dK_W = desc_const(FPANEL_W, 128);
-                const int nb0 = (warp >> 2) * C::NB;
-                float z[C::NB][16];
+                const int nb0 = (warp >> 2) * 2;   // 0: the forward threads are one warpgroup
+                float z[2][16];
 #pragma unroll
-                for (int b = 0; b < C::NB; ++b)
+                for (int b = 0; b < 2; ++b)
 #pragma unroll
                     for (int i = 0; i < 16; ++i) z[b][i] = 0.f;
                 wgmma_fence();
@@ -501,7 +459,7 @@ __global__ void __launch_bounds__(RowsCfg<R>::NT, RowsCfg<R>::MIN_CTAS) rollout_
 #pragma unroll
                     for (int kk = 0; kk < 4; ++kk)
 #pragma unroll
-                        for (int b = 0; b < C::NB; ++b)
+                        for (int b = 0; b < 2; ++b)
                             wgmma_f16_n32<0, 0>(z[b], desc_at(dK_A, aa + 2 * kk * C::L::PANEL),
                                                 desc_at(dK_W, bb + (nb0 + b) * 32 * 16 + 2 * kk * FPANEL_W), (pass | kk) > 0);
                 }
@@ -509,7 +467,7 @@ __global__ void __launch_bounds__(RowsCfg<R>::NT, RowsCfg<R>::MIN_CTAS) rollout_
                 wgmma_wait<0>();
                 if (16 * (warp & 3) < R) {   // fragment rows 16 (warp % 4) + [0, 16): only real rows go to the staging tile
 #pragma unroll
-                    for (int b = 0; b < C::NB; ++b) frag_store<32>(z[b], c.S + 32 * (nb0 + b), S_LD);
+                    for (int b = 0; b < 2; ++b) frag_store<32>(z[b], c.S + 32 * (nb0 + b), S_LD);
                 }
             }
             RW_FWD_SYNC();   // the staging tile is complete; the next step's stores follow its forward barrier in front of the MMAs
@@ -559,7 +517,8 @@ __global__ void __launch_bounds__(RowsCfg<R>::NT, RowsCfg<R>::MIN_CTAS) rollout_
                     for (int j = 0; j < MAX_OUT; ++j) q[j] = 1.f;
                     if (!a.deterministic) { F_FOR_OUT(j) q[j] = qn[(pb * MAX_OUT + j) * R + row]; }
                     float lp;
-                    act = sample_row<NOUT>(logit, n, q, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0, lp);
+                    act = sample_action(logit, n, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0,
+                                        [&](float (&qs)[MAX_OUT]) { for (int j = 0; j < MAX_OUT; ++j) qs[j] = q[j]; }, lp);
                     a.actions[grow] = (float)act;
                     a.action_log_probs[grow] = lp;
                 }
@@ -610,20 +569,6 @@ int prepare_kernel(K kern, uint32_t smem_bytes = F_SMEM) {
     return 0;
 }
 
-template <int R>
-int launch_rollout_rows(const OrlRolloutArgs& a, cudaStream_t st) {
-    using C = RowsCfg<R>;
-    const int grid = (a.n_envs + R - 1) / R;
-    if (a.activation_id == 1) {
-        if (int e = prepare_kernel(rollout_cartpole_rows_kernel<R, 2, 1>, C::SMEM)) return e;
-        rollout_cartpole_rows_kernel<R, 2, 1><<<grid, C::NT, C::SMEM, st>>>(a);
-    } else {
-        if (int e = prepare_kernel(rollout_cartpole_rows_kernel<R, 2, -1>, C::SMEM)) return e;
-        rollout_cartpole_rows_kernel<R, 2, -1><<<grid, C::NT, C::SMEM, st>>>(a);
-    }
-    return check_cuda(cudaGetLastError(), "rollout_cartpole_rows_kernel");
-}
-
 }  // namespace
 
 namespace orl {
@@ -653,26 +598,16 @@ bool rollout_tc_eligible(const OrlRolloutArgs& a) {
 }
 
 int launch_rollout_tc(const OrlRolloutArgs& a, cudaStream_t st) {
-    const int grid = (a.n_envs + F_M - 1) / F_M;
-#define ORL_RTC(ENVK, NO)                                                                               \
-    do {                                                                                                \
-        if (a.activation_id == 1) {                                                                     \
-            if (int e_ = prepare_kernel(rollout_tc_kernel<ENVK, NO, 1>)) return e_;                     \
-            rollout_tc_kernel<ENVK, NO, 1><<<grid, F_NT, F_SMEM, st>>>(a);                              \
-        } else {                                                                                        \
-            if (int e_ = prepare_kernel(rollout_tc_kernel<ENVK, NO, -1>)) return e_;                    \
-            rollout_tc_kernel<ENVK, NO, -1><<<grid, F_NT, F_SMEM, st>>>(a);                             \
-        }                                                                                               \
-    } while (0)
-    static const bool q5 = [] { const char* v = getenv("ORL_ROLLOUT_Q5"); return !(v && atoi(v) == 0); }();
-    if (a.env_kind == ORL_ENV_CARTPOLE && q5) {
-        // R = 32 envs per CTA: the envs spread over the most SMs, and each SM issues the forward of the fewest rows per
-        // step (DESIGN.md §6 has R = 32 against R = 64).  ORL_ROLLOUT_ROWS=64 selects R = 64.
-        static const bool rows64 = [] { const char* v = getenv("ORL_ROLLOUT_ROWS"); return v && atoi(v) == 64; }();
-        return rows64 ? launch_rollout_rows<64>(a, st) : launch_rollout_rows<32>(a, st);
-    } else if (a.env_kind == ORL_ENV_CARTPOLE) ORL_RTC(ORL_ENV_CARTPOLE, 2);
-    else ORL_RTC(ORL_ENV_GRIDWORLD, 5);
-#undef ORL_RTC
+    const bool relu = a.activation_id == 1;
+    if (a.env_kind == ORL_ENV_CARTPOLE) {
+        const auto kern = relu ? rollout_cartpole_rows_kernel<1> : rollout_cartpole_rows_kernel<-1>;
+        if (int e = prepare_kernel(kern, RowsCfg::SMEM)) return e;
+        kern<<<(a.n_envs + RowsCfg::R - 1) / RowsCfg::R, RowsCfg::NT, RowsCfg::SMEM, st>>>(a);
+        return check_cuda(cudaGetLastError(), "rollout_cartpole_rows_kernel");
+    }
+    const auto kern = relu ? rollout_tc_kernel<1> : rollout_tc_kernel<-1>;
+    if (int e = prepare_kernel(kern)) return e;
+    kern<<<(a.n_envs + F_M - 1) / F_M, F_NT, F_SMEM, st>>>(a);
     return check_cuda(cudaGetLastError(), "rollout_tc_kernel");
 }
 

@@ -33,30 +33,6 @@ constexpr int LMAX = 32;     // data_chunk_length limit accepted by the host API
 constexpr int RNN_NT = 64;   // threads per CTA of the sequential kernels
 constexpr int JOINT_A = 3;   // agents of the joint-action update (simple_spread, the multi-agent device env)
 
-__device__ __forceinline__ int pick_action(const OrlRnnArgs& a, const float (&pr)[MAX_OUT], int n, size_t grow, int row,
-                                           int t, uint64_t rng_base) {
-    if (a.deterministic) {
-        int act = 0;
-#pragma unroll
-        for (int j = 1; j < MAX_OUT; ++j) if (j < n && pr[j] > pr[act]) act = j;
-        return act;
-    }
-    float q[MAX_OUT];
-    if (a.exp_noise) {
-#pragma unroll
-        for (int j = 0; j < MAX_OUT; ++j) q[j] = (j < n) ? a.exp_noise[grow * n + j] : 1.f;
-    } else {
-        const uint64_t step = rng_base + (uint64_t)t;
-        const uint2 key = make_uint2((uint32_t)a.rng_seed, (uint32_t)(a.rng_seed >> 32));
-        const uint4 r0 = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)row, 0u), key);
-        const uint4 r1 = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)row, 1u), key);
-        const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-        for (int j = 0; j < MAX_OUT; ++j) q[j] = -logf(u32_to_unit_open(rr[j]));
-    }
-    return sample_categorical(pr, n, q);
-}
-
 // ---- act only (PPOModule.act / PPONet.act): one thread per row runs the sequential core; the caller owns env.step ----
 __global__ void __launch_bounds__(RNN_NT) rnn_act_kernel(const OrlRnnArgs a) {
     const int B = a.n_envs, n = a.n_actions, d = a.obs_dim;
@@ -71,20 +47,15 @@ __global__ void __launch_bounds__(RNN_NT) rnn_act_kernel(const OrlRnnArgs a) {
         for (int j = 0; j < rc::H; ++j) h[j] = a.rnn_states[grow * rc::H + j];
         rc::rnn_step_forward(a.policy_params, o, a.activation_id, x, h, a.masks[grow], hn, logit, nullptr, nullptr);
         for (int j = 0; j < rc::H; ++j) a.rnn_states[((size_t)(t + 1) * B + row) * rc::H + j] = hn[j];
-#pragma unroll
-        for (int j = 0; j < MAX_OUT; ++j) if (j >= n) logit[j] = 0.f;
-        float nl[MAX_OUT], pr[MAX_OUT];
-        log_softmax_n(logit, n, nl, pr);
-        const int act = pick_action(a, pr, n, grow, row, t, rng_base);
-        float lp = nl[0];
-#pragma unroll
-        for (int j = 1; j < MAX_OUT; ++j) if (j == act) lp = nl[j];
+        // the recurrent kernels key the action noise by the local row: OrlRnnArgs has no rng_row_offset
+        float lp;
+        const int act = sample_action(logit, n, nullptr, a.deterministic != 0, [&](float (&q)[MAX_OUT]) {
+            action_noise(a.exp_noise, grow, n, a.rng_seed, rng_base + (uint64_t)t, (uint32_t)row, q);
+        }, lp);
         a.actions[grow] = (float)act;
         a.action_log_probs[grow] = lp;
     }
 }
-
-__global__ void rnn_bump_counter_kernel(uint64_t* c, uint64_t by) { *c += by; }
 
 constexpr int W_NT = 512, W_WPC = W_NT / 32;   // one persistent CTA per SM, 16 warps, weights of one net in smem
 
@@ -121,12 +92,10 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_rollout_warp_kernel(const OrlRnnA
             for (int ag = 0; ag < A; ++ag) {
                 const int row = e * A + ag;
                 const size_t grow = (size_t)t * B + row;
-                float nl[MAX_OUT], pr[MAX_OUT];
-                log_softmax_n(logit[ag], n, nl, pr);                 // identical on every lane
-                const int act = pick_action(a, pr, n, grow, row, t, rng_base);
-                float lp = nl[0];
-#pragma unroll
-                for (int j = 1; j < MAX_OUT; ++j) if (j == act) lp = nl[j];
+                float lp;
+                const int act = sample_action(logit[ag], n, nullptr, a.deterministic != 0, [&](float (&q)[MAX_OUT]) {   // identical on every lane
+                    action_noise(a.exp_noise, grow, n, a.rng_seed, rng_base + (uint64_t)t, (uint32_t)row, q);
+                }, lp);
                 if (lane == 0) { a.actions[grow] = (float)act; a.action_log_probs[grow] = lp; }
                 acts[ag] = act;
             }
@@ -654,8 +623,8 @@ int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
     if (a.env_kind == ORL_ENV_NONE) {   // policy step(s) only: rows = n_envs, slot t -> actions[t], rnn_states[t+1]
         ORL_CHECK_ARG(a.n_agents == 1, "ENV_NONE rows are passed as n_envs with n_agents == 1");
         if (a.t_end > a.t_begin) rnn_act_kernel<<<grid, RNN_NT, 0, st>>>(a);
-        if (a.rng_counter) rnn_bump_counter_kernel<<<1, 1, 0, st>>>(a.rng_counter, (uint64_t)(a.t_end - a.t_begin));
-        return orl::check_cuda(cudaGetLastError(), "rnn_act_kernel launch");
+        if (int e = orl::check_cuda(cudaGetLastError(), "rnn_act_kernel launch")) return e;
+        return orl::bump_rng_counter(a.rng_counter, a.t_end - a.t_begin, st);
     }
     ORL_CHECK_ARG(a.critic_obs && a.rewards && a.active_masks, "null rollout buffer");
     ORL_CHECK_ARG(a.env_kind == ORL_ENV_MPE_SPREAD || a.env_kind == ORL_ENV_CARTPOLE || a.env_kind == ORL_ENV_GRIDWORLD,
@@ -682,8 +651,8 @@ int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
                 rnn_rollout_warp_kernel<ORL_ENV_GRIDWORLD><<<wg, W_NT, w_smem(1), st>>>(a); break;
         }
     }
-    if (a.rng_counter) rnn_bump_counter_kernel<<<1, 1, 0, st>>>(a.rng_counter, (uint64_t)(a.t_end - a.t_begin));
-    return orl::check_cuda(cudaGetLastError(), "rnn_rollout_warp_kernel launch");
+    if (int e = orl::check_cuda(cudaGetLastError(), "rnn_rollout_warp_kernel launch")) return e;
+    return orl::bump_rng_counter(a.rng_counter, a.t_end - a.t_begin, st);
 }
 
 int orl_rnn_critic(const OrlRnnArgs* ap, void* stream) {

@@ -97,11 +97,9 @@ __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
             uint32_t rr[8];
             if (!a.exp_noise && !a.deterministic) {
                 const uint64_t step = rng_base + (uint64_t)t;
-                const uint2 key = make_uint2((uint32_t)a.rng_seed, (uint32_t)(a.rng_seed >> 32));
-                const uint4 r0 = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)(row0 + hrow + a.rng_row_offset), 2u), key);
-                const uint4 r1 = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)(row0 + hrow + a.rng_row_offset), 3u), key);
-                const uint4 r2 = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)(row0 + hrow + a.rng_row_offset), 4u), key);
-                const uint4 r3 = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)(row0 + hrow + a.rng_row_offset), 5u), key);
+                const uint32_t crow = (uint32_t)(row0 + hrow + a.rng_row_offset);
+                const uint4 r0 = action_philox(a.rng_seed, step, crow, 2u), r1 = action_philox(a.rng_seed, step, crow, 3u);
+                const uint4 r2 = action_philox(a.rng_seed, step, crow, 4u), r3 = action_philox(a.rng_seed, step, crow, 5u);
                 // Box-Muller: 8 normals from 16 uniforms (pairs (r0,r1) and (r2,r3))
                 const uint32_t u1[8] = {r0.x, r0.y, r0.z, r0.w, r2.x, r2.y, r2.z, r2.w};
                 const uint32_t u2[8] = {r1.x, r1.y, r1.z, r1.w, r3.x, r3.y, r3.z, r3.w};
@@ -130,37 +128,12 @@ __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
         }
         if (hpart == 0 && hrow < rows_here && a.head_kind != ORL_HEAD_GAUSSIAN) {
             const size_t grow = (size_t)t * B + row0 + hrow;
-            if (a.action_masks) {
-#pragma unroll
-                for (int j = 0; j < MAX_OUT; ++j)
-                    if (j < n && a.action_masks[grow * n + j] == 0.f) logit[j] = -6e4f;
-            }
-            float nl[MAX_OUT], pr[MAX_OUT];
-            log_softmax_n(logit, n, nl, pr);
-            int act;
-            if (a.deterministic) {
-                act = 0;
-#pragma unroll
-                for (int j = 1; j < MAX_OUT; ++j) if (j < n && pr[j] > pr[act]) act = j;
-            } else {
-                float q[MAX_OUT];
-                if (a.exp_noise) {
-#pragma unroll
-                    for (int j = 0; j < MAX_OUT; ++j) q[j] = (j < n) ? a.exp_noise[grow * n + j] : 1.f;
-                } else {
-                    const uint64_t step = rng_base + (uint64_t)t;
-                    const uint2 key = make_uint2((uint32_t)a.rng_seed, (uint32_t)(a.rng_seed >> 32));
-                    const uint4 r0 = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)(row0 + hrow + a.rng_row_offset), 0u), key);
-                    const uint4 r1 = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)(row0 + hrow + a.rng_row_offset), 1u), key);
-                    const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-                    for (int j = 0; j < MAX_OUT; ++j) q[j] = -logf(u32_to_unit_open(rr[j]));
-                }
-                act = sample_categorical(pr, n, q);
-            }
-            float lp = nl[0];
-#pragma unroll
-            for (int j = 1; j < MAX_OUT; ++j) if (j == act) lp = nl[j];
+            float lp;
+            const int act = sample_action(logit, n, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0,
+                                          [&](float (&q)[MAX_OUT]) {
+                                              action_noise(a.exp_noise, grow, n, a.rng_seed, rng_base + (uint64_t)t,
+                                                           (uint32_t)(row0 + hrow + a.rng_row_offset), q);
+                                          }, lp);
             a.actions[grow] = (float)act;
             a.action_log_probs[grow] = lp;
             act_s[hrow] = act;
@@ -209,8 +182,6 @@ __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
         __syncthreads();
     }
 }
-
-__global__ void bump_counter_kernel(uint64_t* c, uint64_t by) { *c += by; }
 
 __global__ void env_reset_kernel(int env_kind, int N, double* env_f64, uint64_t* env_u64, int32_t* env_i32,
                                  const int32_t* env_table, int env_table_len, uint64_t seed, float* obs_out,
@@ -349,16 +320,12 @@ __global__ void __launch_bounds__(C_NT) policy_eval_kernel(const float* __restri
                     entropy_out[g * n + j] = 1.4189385332046727f + ls;
                 }
             } else {
-                if (action_masks) {
-#pragma unroll
-                    for (int j = 0; j < MAX_OUT; ++j) if (j < n && action_masks[g * n + j] == 0.f) out[j] = -6e4f;
-                }
                 float nl[MAX_OUT], pr[MAX_OUT];
-                log_softmax_n(out, n, nl, pr);
-                const int act = (int)actions[g];
-                float lp = nl[0], ent = 0.f;
+                masked_log_softmax(out, n, action_masks ? action_masks + g * n : nullptr, nl, pr);
+                const float lp = log_prob_of(nl, n, (int)actions[g]);
+                float ent = 0.f;
 #pragma unroll
-                for (int j = 0; j < MAX_OUT; ++j) if (j < n) { if (j == act) lp = nl[j]; ent -= pr[j] * nl[j]; }
+                for (int j = 0; j < MAX_OUT; ++j) if (j < n) ent -= pr[j] * nl[j];
                 logp_out[g] = lp;
                 entropy_out[g] = ent;
             }
@@ -448,13 +415,10 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
         orl::set_last_error("orl_rollout: unsupported env_kind %d", a.env_kind);
         return ORL_ERR_UNSUPPORTED;
     }
-    if (orl::rollout_tc_eligible(a)) {   // single-agent device envs: the tensor-core rollout (orl_fwd_tc.cu), one CTA per 128 envs
-        if (int e = orl::launch_rollout_tc(a, reinterpret_cast<cudaStream_t>(stream))) return e;
-        if (a.rng_counter) {
-            bump_counter_kernel<<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream)>>>(a.rng_counter, (uint64_t)(a.t_end - a.t_begin));
-            ORL_LAUNCH_CHECK("bump_counter_kernel");
-        }
-        return 0;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (orl::rollout_tc_eligible(a)) {   // single-agent device envs: the tensor-core rollouts (orl_fwd_tc.cu)
+        if (int e = orl::launch_rollout_tc(a, st)) return e;
+        return orl::bump_rng_counter(a.rng_counter, a.t_end - a.t_begin, st);
     }
     // rows per CTA: the step chain is latency-bound, so prefer many small CTAs (>= ~4 per SM) and
     // only grow the tile when there are enough rows to keep that many CTAs anyway
@@ -468,7 +432,6 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
     const int grid = (a.n_envs + envs_per_cta - 1) / envs_per_cta;
     const int ldx = orl::pad4(a.obs_dim) + 4;
     const size_t smem = sizeof(float) * (orl::smem_weights_floats(a.obs_dim, false) + rm * ldx + 2 * rm * orl::LDA + rm);
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
 #define ORL_LAUNCH_ROLLOUT(RM, EK)                                                                                   \
     do {                                                                                                             \
         static bool attr_done = false;                                                                               \
@@ -492,11 +455,7 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
         default: ORL_LAUNCH_ROLLOUT_RM(ORL_ENV_MPE_SPREAD); break;
     }
     ORL_LAUNCH_CHECK("rollout_kernel");
-    if (a.rng_counter) {
-        bump_counter_kernel<<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream)>>>(a.rng_counter, (uint64_t)(a.t_end - a.t_begin));
-        ORL_LAUNCH_CHECK("bump_counter_kernel");
-    }
-    return 0;
+    return orl::bump_rng_counter(a.rng_counter, a.t_end - a.t_begin, st);
 }
 
 extern "C" int orl_critic_values(const float* critic_params, int obs_dim, int activation_id, const float* obs,

@@ -100,35 +100,6 @@ __device__ __forceinline__ int sp_pick_opponent(int strategy, int pool_count, in
     return (int)(((uint64_t)r.x * (uint64_t)avail) >> 32);                                // random.randint(0, len - 1), random_opponent.py:25-28
 }
 
-__device__ __forceinline__ int sp_sample(const float* logits, int n, int deterministic, uint32_t c0, uint32_t c1, uint32_t row, uint32_t lane,
-                                         uint64_t seed, float* logp_out) {
-    float lg[MAX_OUT], nl[MAX_OUT], pr[MAX_OUT];
-#pragma unroll
-    for (int j = 0; j < MAX_OUT; ++j) lg[j] = j < n ? logits[j] : 0.f;
-    log_softmax_n(lg, n, nl, pr);
-    int act = 0;
-    if (deterministic) {
-#pragma unroll
-        for (int j = 1; j < MAX_OUT; ++j) if (j < n && pr[j] > pr[act]) act = j;
-    } else {
-        const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
-        const uint4 r0 = philox4x32_10(make_uint4(c0, c1, row, lane), key);
-        const uint4 r1 = philox4x32_10(make_uint4(c0, c1, row, lane + 1u), key);
-        const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-        float q[MAX_OUT];
-#pragma unroll
-        for (int j = 0; j < MAX_OUT; ++j) q[j] = -logf(u32_to_unit_open(rr[j]));
-        act = sample_categorical(pr, n, q);
-    }
-    if (logp_out) {
-        float lp = nl[0];
-#pragma unroll
-        for (int j = 1; j < MAX_OUT; ++j) if (j == act) lp = nl[j];
-        *logp_out = lp;
-    }
-    return act;
-}
-
 // env_i32 layout [8][N]: x0, y0, x1, y1, steps, nreset, opponent index, (unused)
 __global__ void __launch_bounds__(SP_NT) selfplay_reset_kernel(const OrlSelfPlayArgs s, float* __restrict__ obs_out) {
     const OrlRolloutArgs& a = s.rollout;
@@ -160,19 +131,18 @@ __global__ void __launch_bounds__(SP_NT) selfplay_rollout_kernel(const OrlSelfPl
         const uint64_t step = rng_base + (uint64_t)t;
         const size_t grow = (size_t)t * N + e;
         // ---- learner: forward + sample (deterministic bit 1: greedy, bit 2: scripted from exp_noise) ----
+        // Philox lanes of (step, env_key): 0/1 learner, 2/3 opponent policy, 4 random opponent
         const float xl[4] = {(float)x0, (float)y0, (float)x1, (float)y1};
-        float logits[MAX_OUT], lp = 0.f;
+        float logits[MAX_OUT], lp;
         sp_policy_logits(a.policy_params, n, a.activation_id, xl, logits);
-        int act0 = sp_sample(logits, n, a.deterministic & 1, (uint32_t)step, (uint32_t)(step >> 32), (uint32_t)env_key, 0u, a.rng_seed, &lp);
+        int act0 = sample_action(logits, n, nullptr, a.deterministic & 1, [&](float (&q)[MAX_OUT]) {
+            action_noise(nullptr, 0, n, a.rng_seed, step, (uint32_t)env_key, q);
+        }, lp);
         if ((a.deterministic & 2) && a.exp_noise) {   // scripted learner action (vec-env step API, tests): log-prob of THAT action
             act0 = (int)a.exp_noise[grow * 2 + 0];
-            float lg[MAX_OUT], nl[MAX_OUT], pr[MAX_OUT];
-#pragma unroll
-            for (int j = 0; j < MAX_OUT; ++j) lg[j] = j < n ? logits[j] : 0.f;
-            log_softmax_n(lg, n, nl, pr);
-            lp = nl[0];
-#pragma unroll
-            for (int j = 1; j < MAX_OUT; ++j) if (j == act0) lp = nl[j];
+            float nl[MAX_OUT], pr[MAX_OUT];
+            masked_log_softmax(logits, n, nullptr, nl, pr);
+            lp = log_prob_of(nl, n, act0);
         }
         // ---- opponent: its snapshot's policy on the mirrored observation, or a uniformly random action ----
         int act1;
@@ -180,13 +150,13 @@ __global__ void __launch_bounds__(SP_NT) selfplay_rollout_kernel(const OrlSelfPl
             act1 = (int)a.exp_noise[grow * 2 + 1];
         } else if (opp >= 0) {
             const float xo[4] = {(float)x1, (float)y1, (float)x0, (float)y0};
-            float lo[MAX_OUT];
+            float lo[MAX_OUT], lpo;
             sp_policy_logits(s.pool_params + (size_t)opp * s.pool_stride, n, a.activation_id, xo, lo);
-            act1 = sp_sample(lo, n, 0, (uint32_t)step, (uint32_t)(step >> 32), (uint32_t)env_key, 2u, a.rng_seed, nullptr);
+            act1 = sample_action(lo, n, nullptr, false, [&](float (&q)[MAX_OUT]) {
+                action_noise(nullptr, 0, n, a.rng_seed, step, (uint32_t)env_key, q, 2u);
+            }, lpo);
         } else {
-            const uint2 key = make_uint2((uint32_t)a.rng_seed, (uint32_t)(a.rng_seed >> 32));
-            const uint4 r = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)env_key, 4u), key);
-            act1 = (int)(((uint64_t)r.x * (uint64_t)n) >> 32);
+            act1 = (int)(((uint64_t)action_philox(a.rng_seed, step, (uint32_t)env_key, 4u).x * (uint64_t)n) >> 32);
         }
         a.actions[grow] = (float)act0;
         a.action_log_probs[grow] = lp;
@@ -226,8 +196,6 @@ __global__ void __launch_bounds__(SP_NT) selfplay_rollout_kernel(const OrlSelfPl
     a.ep_return[e] = ep_ret; a.ep_length[e] = ep_len;
 }
 
-__global__ void selfplay_bump_counter_kernel(uint64_t* c, uint64_t by) { *c += by; }
-
 int check_selfplay(const OrlSelfPlayArgs& s) {
     const OrlRolloutArgs& a = s.rollout;
     ORL_CHECK_ARG(a.n_envs > 0 && a.n_agents == 1 && a.obs_dim == 4 && a.n_actions == 5, "the 2-player GridWorld has obs (x0,y0,x1,y1) and 5 actions");
@@ -258,9 +226,5 @@ extern "C" int orl_selfplay_rollout(const OrlSelfPlayArgs* sp, void* stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     selfplay_rollout_kernel<<<(a.n_envs + SP_NT - 1) / SP_NT, SP_NT, 0, st>>>(*sp);
     ORL_LAUNCH_CHECK("selfplay_rollout_kernel");
-    if (a.rng_counter) {
-        selfplay_bump_counter_kernel<<<1, 1, 0, st>>>(a.rng_counter, (uint64_t)(a.t_end - a.t_begin));
-        ORL_LAUNCH_CHECK("selfplay_bump_counter_kernel");
-    }
-    return 0;
+    return orl::bump_rng_counter(a.rng_counter, a.t_end - a.t_begin, st);
 }

@@ -37,36 +37,11 @@ __global__ void __launch_bounds__(S_NT) share_rollout_kernel(const OrlRolloutArg
         for (int j = 0; j < MAX_OUT; ++j) logit[j] = 0.f;
         dc::deep_forward(a.policy_params, o, a.activation_id, x, nullptr, logit, nullptr, nullptr);
         const size_t grow = (size_t)t * B + e;
-        if (a.action_masks) {
-#pragma unroll
-            for (int j = 0; j < MAX_OUT; ++j) if (j < n && a.action_masks[grow * n + j] == 0.f) logit[j] = -6e4f;
-        }
-        float nl[MAX_OUT], pr[MAX_OUT];
-        log_softmax_n(logit, n, nl, pr);
-        int act;
-        if (a.deterministic) {
-            act = 0;
-#pragma unroll
-            for (int j = 1; j < MAX_OUT; ++j) if (j < n && pr[j] > pr[act]) act = j;
-        } else {
-            float q[MAX_OUT];
-            if (a.exp_noise) {
-#pragma unroll
-                for (int j = 0; j < MAX_OUT; ++j) q[j] = (j < n) ? a.exp_noise[grow * n + j] : 1.f;
-            } else {
-                const uint64_t step = rng_base + (uint64_t)t;
-                const uint2 key = make_uint2((uint32_t)a.rng_seed, (uint32_t)(a.rng_seed >> 32));
-                const uint4 r0 = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)(e + a.rng_row_offset), 0u), key);
-                const uint4 r1 = philox4x32_10(make_uint4((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)(e + a.rng_row_offset), 1u), key);
-                const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-#pragma unroll
-                for (int j = 0; j < MAX_OUT; ++j) q[j] = -logf(u32_to_unit_open(rr[j]));
-            }
-            act = sample_categorical(pr, n, q);
-        }
-        float lp = nl[0];
-#pragma unroll
-        for (int j = 1; j < MAX_OUT; ++j) if (j == act) lp = nl[j];
+        float lp;
+        const int act = sample_action(logit, n, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0,
+                                      [&](float (&q)[MAX_OUT]) {
+                                          action_noise(a.exp_noise, grow, n, a.rng_seed, rng_base + (uint64_t)t, (uint32_t)(e + a.rng_row_offset), q);
+                                      }, lp);
         a.actions[grow] = (float)act;
         a.action_log_probs[grow] = lp;
         if (ENV != ORL_ENV_NONE) {
@@ -85,8 +60,6 @@ __global__ void __launch_bounds__(S_NT) share_rollout_kernel(const OrlRolloutArg
         }
     }
 }
-
-__global__ void share_bump_counter_kernel(uint64_t* c, uint64_t by) { *c += by; }
 
 __global__ void __launch_bounds__(S_NT) share_values_kernel(const float* __restrict__ params, int d, int n, int activation_id,
                                                             const float* __restrict__ obs, float* __restrict__ values, long long rows) {
@@ -343,11 +316,7 @@ int orl_share_rollout(const OrlRolloutArgs* ap, void* stream) {
         return ORL_ERR_UNSUPPORTED;
     }
     ORL_LAUNCH_CHECK("share_rollout_kernel");
-    if (a.rng_counter) {
-        share_bump_counter_kernel<<<1, 1, 0, st>>>(a.rng_counter, (uint64_t)(a.t_end - a.t_begin));
-        ORL_LAUNCH_CHECK("share_bump_counter_kernel");
-    }
-    return 0;
+    return orl::bump_rng_counter(a.rng_counter, a.t_end - a.t_begin, st);
 }
 
 int orl_share_values(const float* params, int obs_dim, int n_actions, int activation_id, const float* obs, float* values, long long rows,

@@ -5,8 +5,7 @@ bench.py's C2 workload (CartPole-v1, T = 128, MLP 64x64, device sampling) at eac
 the latency of one CTA's step chain, and the full grid).  CUDA events around each of `--launches` launches after
 `--warmup` launches; the env state simply carries on from launch to launch.  Reports microseconds per step (median and
 range over launches), SM cycles per step at the SM clock read right after the timed launches, and the card's name, power
-limit, maximum SM clock and active clock-event (throttle) reasons, read in the same run.  `ORL_ROLLOUT_ROWS=32 / 64`
-pins the envs per CTA of the CartPole kernel.  Prints one JSON line.
+limit, maximum SM clock and active clock-event (throttle) reasons, read in the same run.  Prints one JSON line.
 
     python tools/rollout_bench.py [--envs 128,4096 --launches 50 --warmup 10]
 """
@@ -46,7 +45,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("rollout_bench needs a CUDA device")
     out = {"card": torch.cuda.get_device_name(), "name,power_limit,max_sm_clock": smi("name,power.limit,clocks.max.sm"),
-           "rows_per_cta": os.environ.get("ORL_ROLLOUT_ROWS", "default"), "T": bench.T, "results": {}}
+           "T": bench.T, "results": {}}
     for n in (int(x) for x in args.envs.split(",")):
         cfg, env, net, agent = bench.build_agent(0, 1, "c2", n)
         drv = bench.make_driver(cfg, env, net, agent, 0, 1)
