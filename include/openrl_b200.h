@@ -378,6 +378,10 @@ typedef struct OrlRnnArgs {
     double vn_beta;
     float* train_info;
     int64_t norm_rows;                                    /* row-steps of the GLOBAL minibatch (see OrlPpoArgs.norm_rows); 0 = n_chunks*L */
+    /* orl_rnn_act_rows only: */
+    int32_t rng_row_offset;                               /* added to the buffer row in the action-noise key (first GLOBAL row of this buffer) */
+    int32_t row_begin, row_end;                           /* buffer rows [row_begin, row_end) of slot t_begin */
+    int32_t reserved2;
 } OrlRnnArgs;
 int orl_rnn_param_count(int obs_dim, int n_out);
 int orl_rnn_tape_width(void);
@@ -385,6 +389,18 @@ int orl_rnn_tape_width(void);
 long long orl_rnn_workspace_floats(long long rows, int grads_stride);
 /* policy GRU rollout for steps [t_begin, t_end) fused with the device env (simple_spread, CartPole, GridWorld) */
 int orl_rnn_rollout(const OrlRnnArgs* args, void* stream);
+/* policy GRU act for a HOST-stepped env: one step t = t_begin over buffer rows [row_begin, row_end) (B = n_envs *
+ * n_agents rows per slot).  Reads policy_obs[t], rnn_states[t], masks[t]; writes actions[t], action_log_probs[t] and
+ * rnn_states[t+1] (orl_host_insert_rnn zeroes the rows of the envs that finish at step t).  The action noise of row r is
+ * keyed by (rng_seed, rng_step_base + *rng_counter, r + rng_row_offset) — the slot index is not added — and rng_counter
+ * (nullable) advances by one per call; exp_noise (parity mode, nullable) is the (B, n) Exp(1) table of this slot,
+ * indexed by buffer row. */
+int orl_rnn_act_rows(const OrlRnnArgs* args, void* stream);
+/* orl_host_insert for a recurrent policy: additionally zeroes the 64-float rnn_states_next row of every agent of an env
+ * whose agents are all done (rnn_states[dones_env] = 0, onpolicy_driver.py:262-269).  rnn_states_next addresses slot
+ * t+1 at the same first row as the other pointers. */
+int orl_host_insert_rnn(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
+                        float* masks_next, float* active_masks_next, float* rnn_states_next, void* stream);
 /* recurrent critic over slots 0..T: value_preds[t] and rnn_states_critic[t+1] */
 int orl_rnn_critic(const OrlRnnArgs* args, void* stream);
 /* chunked BPTT forward + loss + backward of both nets over the minibatch chunks -> grads, loss_acc */

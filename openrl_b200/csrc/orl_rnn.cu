@@ -3,7 +3,8 @@
 // Replaces, for cfg.use_recurrent_policy:
 //   RNNLayer.forward                      openrl/modules/networks/utils/rnn.py:39-99
 //   OnPolicyDriver.act / add2buffer       openrl/drivers/onpolicy_driver.py:80-152,236-279 (rnn-state carry,
-//                                         zeroing on dones_env)
+//                                         zeroing on dones_env; for host-stepped envs the act is orl_rnn_act_rows
+//                                         and the zeroing orl_host_insert_rnn)
 //   ReplayData.recurrent_generator        openrl/buffers/replay_data.py:1062-1258 (chunks of L over f=(n*A+a)*T+t)
 //   ReplayData.recurrent_generator_v3     openrl/buffers/replay_data.py:425-551 (JRPO: chunks of L over f=n*T+t, all agents)
 //   PPOAlgorithm.ppo_update (BPTT part)   openrl/algorithms/ppo.py:46-458
@@ -47,7 +48,7 @@ __global__ void __launch_bounds__(RNN_NT) rnn_act_kernel(const OrlRnnArgs a) {
         for (int j = 0; j < rc::H; ++j) h[j] = a.rnn_states[grow * rc::H + j];
         rc::rnn_step_forward(a.policy_params, o, a.activation_id, x, h, a.masks[grow], hn, logit, nullptr, nullptr);
         for (int j = 0; j < rc::H; ++j) a.rnn_states[((size_t)(t + 1) * B + row) * rc::H + j] = hn[j];
-        // the recurrent kernels key the action noise by the local row: OrlRnnArgs has no rng_row_offset
+        // keyed by the local row (rng_row_offset is read by orl_rnn_act_rows only)
         float lp;
         const int act = sample_action(logit, n, nullptr, a.deterministic != 0, [&](float (&q)[MAX_OUT]) {
             action_noise(a.exp_noise, grow, n, a.rng_seed, rng_base + (uint64_t)t, (uint32_t)row, q);
@@ -136,6 +137,51 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_rollout_warp_kernel(const OrlRnnA
                 rw::stv(a.rnn_states + r1 * rc::H, lane, done_i ? rw::V2{0.f, 0.f} : hn[ag]);
             }
             __syncwarp();   // lane 0's observation / mask writes are read by the whole warp in the next step
+        }
+    }
+}
+
+// ---- act over host-stepped rows: rows [row_begin, row_end) of slot t = t_begin, R rows per warp ----
+// The host steps the env between two launches; this kernel writes actions[t], action_log_probs[t] and rnn_states[t+1]
+// (orl_host_insert_rnn zeroes the rows of the envs that finish at step t).  Same staged weights, step_forward and
+// sampler as rnn_rollout_warp_kernel: a row's state, logits and action depend neither on R nor on the warp that runs it.
+template <int R>
+__global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnnArgs a) {
+    extern __shared__ __align__(16) float smem[];
+    const int B = a.n_envs * a.n_agents, d = a.obs_dim, n = a.n_actions, t = a.t_begin;
+    const rc::Offsets o = rc::rnn_offsets(d, n);
+    const rw::SmemNet W = rw::load_net(smem, a.policy_params, o, threadIdx.x, W_NT);
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float* scr = smem + rw::smem_net_floats() + warp * R * rw::SCR;
+    const uint64_t step = a.rng_step_base + (a.rng_counter ? *a.rng_counter : 0ull);
+    float* const no_tape[R] = {};
+    const int rows = a.row_end - a.row_begin, groups = (rows + R - 1) / R;
+    for (int g = blockIdx.x * W_WPC + warp; g < groups; g += gridDim.x * W_WPC) {
+        rw::V2 x[R], h[R], hn[R];
+        float mk[R], logit[R][MAX_OUT];
+        int row[R];
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            row[r] = a.row_begin + min(g * R + r, rows - 1);   // a ragged tail recomputes the last row; its stores are skipped
+            const size_t grow = (size_t)t * B + row[r];
+            const float* ob = a.policy_obs + grow * d;
+            x[r] = rw::V2{lane < d ? ob[lane] : 0.f, lane + 32 < d ? ob[lane + 32] : 0.f};
+            h[r] = rw::ldv(a.rnn_states + grow * rc::H, lane);
+            mk[r] = a.masks[grow];
+        }
+        rw::step_forward<R>(W, scr, d, n, a.activation_id, x, h, mk, hn, logit, no_tape, lane);
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            if (g * R + r < rows) {
+                const size_t grow = (size_t)t * B + row[r];
+                float lp;
+                const int act = sample_action(logit[r], n, nullptr, a.deterministic != 0, [&](float (&q)[MAX_OUT]) {   // identical on every lane
+                    action_noise(a.exp_noise, (size_t)row[r], n, a.rng_seed, step, (uint32_t)(row[r] + a.rng_row_offset), q);
+                }, lp);
+                if (lane == 0) { a.actions[grow] = (float)act; a.action_log_probs[grow] = lp; }
+                rw::stv(a.rnn_states + (grow + B) * rc::H, lane, hn[r]);
+            }
         }
     }
 }
@@ -653,6 +699,30 @@ int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
     }
     if (int e = orl::check_cuda(cudaGetLastError(), "rnn_rollout_warp_kernel launch")) return e;
     return orl::bump_rng_counter(a.rng_counter, a.t_end - a.t_begin, st);
+}
+
+int orl_rnn_act_rows(const OrlRnnArgs* ap, void* stream) {
+    ORL_CHECK_ARG(ap, "args");
+    const OrlRnnArgs& a = *ap;
+    if (int e = check_common(a)) return e;
+    ORL_CHECK_ARG(a.policy_params && a.policy_obs && a.rnn_states && a.actions && a.action_log_probs && a.masks, "null act buffer");
+    ORL_CHECK_ARG(a.t_begin >= 0 && a.t_begin < a.episode_length, "slot t_begin");
+    ORL_CHECK_ARG(a.row_begin >= 0 && a.row_begin <= a.row_end && (long long)a.row_end <= (long long)a.n_envs * a.n_agents, "row range");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int rows = a.row_end - a.row_begin;
+    if (rows > 0) {
+        // one row per warp while the rows leave warps of the persistent grid idle, two (every weight read feeds both) beyond
+        int e = 0;
+        if (rows <= orl::sm_count() * W_WPC) {
+            if ((e = warp_kernel_prepare(rnn_act_rows_warp_kernel<1>, w_smem(1), "smem attr (rnn act rows)"))) return e;
+            rnn_act_rows_warp_kernel<1><<<warp_grid(rows), W_NT, w_smem(1), st>>>(a);
+        } else {
+            if ((e = warp_kernel_prepare(rnn_act_rows_warp_kernel<2>, w_smem(2), "smem attr (rnn act rows)"))) return e;
+            rnn_act_rows_warp_kernel<2><<<warp_grid((rows + 1) / 2), W_NT, w_smem(2), st>>>(a);
+        }
+        if ((e = orl::check_cuda(cudaGetLastError(), "rnn_act_rows_warp_kernel launch"))) return e;
+    }
+    return orl::bump_rng_counter(a.rng_counter, 1, st);
 }
 
 int orl_rnn_critic(const OrlRnnArgs* ap, void* stream) {

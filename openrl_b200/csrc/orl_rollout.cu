@@ -260,11 +260,11 @@ __global__ void __launch_bounds__(C_NT) critic_values_kernel(const float* __rest
 
 // ---- insert of one host env.step into the rollout buffer (OnPolicyDriver.add2buffer, onpolicy_driver.py:80-152) -----------
 // staged = [obs (B*d) | rewards (B) | dones (B)] as uploaded from the host in ONE copy; one thread per row.
-__global__ void host_insert_kernel(const float* __restrict__ staged, int n_envs, int n_agents, int d, float* __restrict__ obs_next,
-                                   float* __restrict__ rewards, float* __restrict__ masks_next, float* __restrict__ active_next) {
+// Row r of the insert; returns whether every agent of the row's env is done.
+__device__ __forceinline__ bool host_insert_row(const float* __restrict__ staged, int n_envs, int n_agents, int d, int r,
+                                                float* __restrict__ obs_next, float* __restrict__ rewards,
+                                                float* __restrict__ masks_next, float* __restrict__ active_next) {
     const int B = n_envs * n_agents;
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= B) return;
     const float* so = staged;
     const float* sr = staged + (size_t)B * d;
     const float* sd = sr + B;
@@ -276,6 +276,28 @@ __global__ void host_insert_kernel(const float* __restrict__ staged, int n_envs,
     const bool done = sd[r] != 0.f;
     masks_next[r] = all_done ? 0.f : 1.f;                    // masks[dones_env] = 0
     active_next[r] = (done && !all_done) ? 0.f : 1.f;        // active[dones] = 0, active[dones_env] = 1
+    return all_done;
+}
+
+__global__ void host_insert_kernel(const float* __restrict__ staged, int n_envs, int n_agents, int d, float* __restrict__ obs_next,
+                                   float* __restrict__ rewards, float* __restrict__ masks_next, float* __restrict__ active_next) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_envs * n_agents) return;
+    host_insert_row(staged, n_envs, n_agents, d, r, obs_next, rewards, masks_next, active_next);
+}
+
+// the same insert for a recurrent policy: rnn_states[t+1] of every agent of a finished env is zeroed (onpolicy_driver.py:262-269)
+constexpr int RNN_HIDDEN = 64;   // OrlRnnArgs.rnn_states rows
+__global__ void host_insert_rnn_kernel(const float* __restrict__ staged, int n_envs, int n_agents, int d, float* __restrict__ obs_next,
+                                       float* __restrict__ rewards, float* __restrict__ masks_next, float* __restrict__ active_next,
+                                       float* __restrict__ rnn_next) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_envs * n_agents) return;
+    if (host_insert_row(staged, n_envs, n_agents, d, r, obs_next, rewards, masks_next, active_next)) {
+        float4* h = reinterpret_cast<float4*>(rnn_next + (size_t)r * RNN_HIDDEN);
+#pragma unroll
+        for (int k = 0; k < RNN_HIDDEN / 4; ++k) h[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
 }
 
 // ---- PolicyNetwork.eval_actions over a flat batch (policy_network.py:164-203, act.py:160-168 / 150-158) ----------------
@@ -515,5 +537,17 @@ extern "C" int orl_host_insert(const float* staged, int n_envs, int n_agents, in
     host_insert_kernel<<<(B + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(staged, n_envs, n_agents, obs_dim, policy_obs_next,
                                                                                          rewards, masks_next, active_masks_next);
     ORL_LAUNCH_CHECK("host_insert_kernel");
+    return 0;
+}
+
+extern "C" int orl_host_insert_rnn(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
+                                   float* masks_next, float* active_masks_next, float* rnn_states_next, void* stream) {
+    ORL_CHECK_ARG(staged && policy_obs_next && rewards && masks_next && active_masks_next && rnn_states_next, "null buffer");
+    ORL_CHECK_ARG(n_envs > 0 && n_agents > 0 && obs_dim > 0, "shapes");
+    ORL_CHECK_ARG(reinterpret_cast<uintptr_t>(rnn_states_next) % 16 == 0, "rnn_states_next must be 16-byte aligned");
+    const int B = n_envs * n_agents;
+    host_insert_rnn_kernel<<<(B + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        staged, n_envs, n_agents, obs_dim, policy_obs_next, rewards, masks_next, active_masks_next, rnn_states_next);
+    ORL_LAUNCH_CHECK("host_insert_rnn_kernel");
     return 0;
 }

@@ -44,8 +44,9 @@ class OnPolicyDriver:
         self.d2h_bytes = 0
         self.phase_events = None  # set to a list by bench.py to collect (name, start, end) CUDA events
         self.recurrent = bool(cfg.use_recurrent_policy or getattr(cfg, "use_naive_recurrent_policy", False))
-        if self.recurrent and self.envs.kind == lib.ENV_NONE:
-            raise NotImplementedError("recurrent policies need a device env (CartPole-v1, GridWorldEnv, simple_spread)")
+        if self.recurrent and self.envs.kind == lib.ENV_NONE and getattr(cfg, "use_joint_action_loss", False):
+            raise NotImplementedError("use_joint_action_loss (JRPO) is built for simple_spread on the device (3 agents, agent-0 "
+                                      "critic); host-stepped envs take the per-agent recurrent update")
 
     # -- reference surface -------------------------------------------------------------------
     def run(self):
@@ -268,10 +269,37 @@ class OnPolicyDriver:
         a.masks, a.active_masks, a.value_preds = lib.ptr(d.masks), lib.ptr(d.active_masks), lib.ptr(d.value_preds)
         a.exp_noise = lib.ptr(noise)
         a.rng_seed, a.rng_step_base, a.rng_counter = int(self.cfg.seed) + 0x9E3779B9 * (self.rank + 1), 0, lib.ptr(self.rng_counter)
-        a.env_f64, a.env_u64, a.env_i32 = lib.ptr(env.env_f64), lib.ptr(env.env_u64), lib.ptr(env.env_i32)
-        a.env_table = lib.ptr(env.env_table)
-        a.ep_return, a.ep_length, a.episode_stats = lib.ptr(env.ep_return), lib.ptr(env.ep_length), lib.ptr(env.episode_stats)
+        state = lambda name: lib.ptr(getattr(env, name, None))   # a host-stepped env has no device state
+        a.env_f64, a.env_u64, a.env_i32, a.env_table = state("env_f64"), state("env_u64"), state("env_i32"), state("env_table")
+        a.ep_return, a.ep_length, a.episode_stats = state("ep_return"), state("ep_length"), state("episode_stats")
         return a
+
+    def _rnn_act_rows(self, step, lo, hi, noise, rng_step_base=None):
+        """Recurrent policy act for envs [lo, hi) of slot `step` of a host-stepped rollout (orl_rnn_act_rows): actions,
+        log-probs and rnn_states[step + 1] of their rows.  The noise step is the device counter (advanced by one per call)
+        or, when given, `rng_step_base`."""
+        A = self.envs.agent_num
+        a = self._rnn_args(step, step + 1, noise)
+        a.row_begin, a.row_end = lo * A, hi * A
+        a.rng_row_offset = int(getattr(self.envs, "env_index_offset", 0)) * A
+        if rng_step_base is not None:
+            a.rng_step_base, a.rng_counter = rng_step_base, None
+        lib.check(self._lib.orl_rnn_act_rows(a, lib.current_stream()), "orl_rnn_act_rows")
+
+    def _host_insert(self, staged, step, lo, hi):
+        """One host env.step of envs [lo, hi) into slot step + 1 (rewards: slot step): orl_host_insert, or
+        orl_host_insert_rnn, which also zeroes rnn_states[step + 1] of the envs that finished."""
+        d, A = self.buffer.data, self.envs.agent_num
+        r0, r1 = lo * A, hi * A
+        args = (lib.ptr(staged), hi - lo, A, d.obs_dim, lib.ptr(d.policy_obs[step + 1].view(-1, d.obs_dim)[r0:r1]),
+                lib.ptr(d.rewards[step].view(-1)[r0:r1]), lib.ptr(d.masks[step + 1].view(-1)[r0:r1]),
+                lib.ptr(d.active_masks[step + 1].view(-1)[r0:r1]))
+        if self.recurrent:
+            states = d.rnn_states[step + 1].view(d.n_rollout_threads * A, -1)[r0:r1]
+            lib.check(self._lib.orl_host_insert_rnn(*args, lib.ptr(states), lib.current_stream()), "orl_host_insert_rnn")
+        else:
+            lib.check(self._lib.orl_host_insert(*args, lib.current_stream()), "orl_host_insert")
+        self.gpu_launches += 1
 
     def _launch_steps(self, t_begin, t_end, noise):
         """Policy + env for steps [t_begin, t_end): feed-forward (orl_rollout) or recurrent (orl_rnn_rollout)."""
@@ -370,25 +398,26 @@ class OnPolicyDriver:
                 noise.normal_() if pol.head_kind == lib.HEAD_GAUSSIAN else noise.exponential_(1)
                 noise = noise.to(self.device)
                 self.h2d_bytes += noise.numel() * 4
-            a = lib.OrlRolloutArgs()
-            a.env_kind, a.n_envs, a.n_agents, a.episode_length = lib.ENV_NONE, B, 1, 1
-            a.t_begin, a.t_end = 0, 1
-            a.obs_dim, a.critic_obs_dim, a.n_actions = d.obs_dim, 0, d.n_actions
-            a.activation_id, a.deterministic, a.head_kind = pol.activation_id, 0, pol.head_kind
-            a.policy_params = lib.ptr(pol.flat_params)
-            a.policy_obs = lib.ptr(d.policy_obs[step])
-            a.actions, a.action_log_probs = lib.ptr(d.actions[step]), lib.ptr(d.action_log_probs[step])
-            a.exp_noise = lib.ptr(noise)
-            a.rng_seed, a.rng_step_base, a.rng_counter = int(self.cfg.seed) + 0x9E3779B9 * (self.rank + 1), 0, lib.ptr(self.rng_counter)
-            with self._phase("rollout"):
-                act_fn = self._lib.orl_share_rollout if getattr(self.trainer, "share", False) else self._lib.orl_rollout
-                lib.check(act_fn(a, lib.current_stream()), "orl_rollout(act)")
+            if self.recurrent:
+                with self._phase("rollout"):
+                    self._rnn_act_rows(step, 0, N, noise)
+            else:
+                a = lib.OrlRolloutArgs()
+                a.env_kind, a.n_envs, a.n_agents, a.episode_length = lib.ENV_NONE, B, 1, 1
+                a.t_begin, a.t_end = 0, 1
+                a.obs_dim, a.critic_obs_dim, a.n_actions = d.obs_dim, 0, d.n_actions
+                a.activation_id, a.deterministic, a.head_kind = pol.activation_id, 0, pol.head_kind
+                a.policy_params = lib.ptr(pol.flat_params)
+                a.policy_obs = lib.ptr(d.policy_obs[step])
+                a.actions, a.action_log_probs = lib.ptr(d.actions[step]), lib.ptr(d.action_log_probs[step])
+                a.exp_noise = lib.ptr(noise)
+                a.rng_seed, a.rng_step_base, a.rng_counter = int(self.cfg.seed) + 0x9E3779B9 * (self.rank + 1), 0, lib.ptr(self.rng_counter)
+                with self._phase("rollout"):
+                    act_fn = self._lib.orl_share_rollout if getattr(self.trainer, "share", False) else self._lib.orl_rollout
+                    lib.check(act_fn(a, lib.current_stream()), "orl_rollout(act)")
             self.gpu_launches += 2
             staged, obs, rewards, dones, infos = env.step_staged(d.actions[step].view(B, w))
-            lib.check(self._lib.orl_host_insert(lib.ptr(staged), N, A, d.obs_dim, lib.ptr(d.policy_obs[step + 1]), lib.ptr(d.rewards[step]),
-                                                lib.ptr(d.masks[step + 1]), lib.ptr(d.active_masks[step + 1]), lib.current_stream()),
-                      "orl_host_insert")
-            self.gpu_launches += 1
+            self._host_insert(staged, step, 0, N)
             self.agent.num_time_steps += N
             if cb is not None:
                 actions = d.actions[step].cpu().numpy()  # noqa: F841
@@ -398,7 +427,8 @@ class OnPolicyDriver:
         return True
 
     def _act_rows(self, step, lo, hi):
-        """Policy forward + sampling for buffer rows [lo, hi) of slot `step` (orl_rollout, ORL_ENV_NONE)."""
+        """Policy forward + sampling for the rows of envs [lo, hi) of slot `step` (orl_rollout, ORL_ENV_NONE; a recurrent
+        policy: orl_rnn_act_rows)."""
         d = self.buffer.data
         pol = self.trainer.algo_module.models["policy"]
         A = self.envs.agent_num
@@ -406,6 +436,10 @@ class OnPolicyDriver:
         obs = d.policy_obs[step].view(-1, d.obs_dim)
         w = d.actions.shape[-1]
         acts, logp = d.actions[step].view(-1, w), d.action_log_probs[step].view(-1, w)
+        if self.recurrent:
+            self._rnn_act_rows(step, lo, hi, None, rng_step_base=self._host_steps_base + step)
+            self.gpu_launches += 1
+            return acts[r0:r1]
         a = lib.OrlRolloutArgs()
         a.env_kind, a.n_envs, a.n_agents, a.episode_length = lib.ENV_NONE, r1 - r0, 1, 1
         a.t_begin, a.t_end = 0, 1
@@ -426,8 +460,8 @@ class OnPolicyDriver:
         group g, the device inserts the other group's results and runs its policy forward for the next step; a group's
         actions travel D2H asynchronously and are awaited (CUDA event) only when the host is ready to step that group.
         Same per-step semantics as `_host_rollout` (add2buffer, onpolicy_driver.py:80-152)."""
-        d, env = self.buffer.data, self.envs
-        T, N, A = self.episode_length, env.parallel_env_num, env.agent_num
+        env = self.envs
+        T, N = self.episode_length, env.parallel_env_num
         groups = env.group_bounds(2)
         self._host_steps_base = getattr(self, "_host_steps_base", 0)   # Philox step of slot 0 of this rollout
         with self._phase("rollout"):
@@ -436,12 +470,7 @@ class OnPolicyDriver:
             for step in range(T):
                 for g, (lo, hi) in enumerate(groups):
                     staged, *_ = env.group_step(g, lo, hi)     # host env.step of this group (device busy with the other)
-                    r0, r1 = lo * A, hi * A
-                    lib.check(self._lib.orl_host_insert(
-                        lib.ptr(staged), hi - lo, A, d.obs_dim, lib.ptr(d.policy_obs[step + 1].view(-1, d.obs_dim)[r0:r1]),
-                        lib.ptr(d.rewards[step].view(-1)[r0:r1]), lib.ptr(d.masks[step + 1].view(-1)[r0:r1]),
-                        lib.ptr(d.active_masks[step + 1].view(-1)[r0:r1]), lib.current_stream()), "orl_host_insert")
-                    self.gpu_launches += 1
+                    self._host_insert(staged, step, lo, hi)
                     if step + 1 < T:
                         env.group_fetch_actions(g, lo, hi, self._act_rows(step + 1, lo, hi))
                 self.agent.num_time_steps += N

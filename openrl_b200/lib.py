@@ -209,10 +209,13 @@ class OrlRnnArgs(ctypes.Structure):
         ("vn_beta", _D),
         ("train_info", _P),
         ("norm_rows", _c.c_int64),
+        ("rng_row_offset", _c.c_int32), ("row_begin", _c.c_int32), ("row_end", _c.c_int32), ("reserved2", _c.c_int32),
     ]
 
 
 _SIGNATURES.update({
+    "orl_rnn_act_rows": [_c.POINTER(OrlRnnArgs), _P],
+    "orl_host_insert_rnn": [_P, _I, _I, _I, _P, _P, _P, _P, _P, _P],
     "orl_rnn_param_count": [_I, _I],
     "orl_rnn_tape_width": [],
     "orl_rnn_workspace_floats": [_c.c_int64, _I],
