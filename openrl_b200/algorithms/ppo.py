@@ -116,29 +116,14 @@ class PPOAlgorithm:
     def prep_training(self):
         pass
 
-    def _args(self, buf, batch_rows, indices, row_begin):
+    def _common_args(self, a, rows):
+        """Fill the fields OrlPpoArgs and OrlRnnArgs share: shapes, loss and Adam coefficients, ValueNorm, the parameter /
+        Adam / lr / step pointers, train_info and the global row count of a minibatch of `rows` rows on this rank."""
         m = self.algo_module
         pol, cri = m.models["policy"], m.models["critic"]
         op, oc = m.optimizers["policy"], m.optimizers["critic"]
         cfg = self.cfg
-        a = lib.OrlPpoArgs()
         a.obs_dim, a.critic_obs_dim, a.n_actions, a.activation_id = self.d, self.dc, self.n, pol.activation_id
-        a.flags, a.grid_per_net = self.flags, self.grid_per_net
-        a.head_kind = self.head_kind
-        a.dual_clip_coeff = float(getattr(self.cfg, "dual_clip_coeff", 3.0))
-        total = buf.episode_length * buf.n_rollout_threads * buf.num_agents
-        a.batch_rows, a.row_begin, a.total_rows = int(batch_rows), int(row_begin), int(total)
-        # every rank holds an equal shard of the global minibatch: weights / batch moments refer to the global row count
-        a.norm_rows = int(batch_rows) * self.world_size if self.world_size > 1 else 0
-        a.indices = lib.ptr(indices)
-        a.policy_obs, a.critic_obs = lib.ptr(buf.policy_obs), lib.ptr(buf.critic_obs)
-        a.actions, a.old_log_probs = lib.ptr(buf.actions), lib.ptr(buf.action_log_probs)
-        a.advantages, a.value_preds, a.returns = lib.ptr(buf.advantages), lib.ptr(buf.value_preds), lib.ptr(buf.returns)
-        a.active_masks = lib.ptr(buf.active_masks)
-        a.action_masks = None if (buf.action_masks_trivial or buf.continuous) else lib.ptr(buf.action_masks)
-        a.gae_stats = lib.ptr(buf.gae_stats)
-        vn = cri.value_normalizer
-        a.vn_state = None if vn is None else lib.ptr(vn.state)
         a.policy_params, a.critic_params = lib.ptr(pol.flat_params), lib.ptr(cri.flat_params)
         a.policy_adam_m, a.policy_adam_v = lib.ptr(op.exp_avg), lib.ptr(op.exp_avg_sq)
         a.critic_adam_m, a.critic_adam_v = lib.ptr(oc.exp_avg), lib.ptr(oc.exp_avg_sq)
@@ -147,9 +132,29 @@ class PPOAlgorithm:
         a.huber_delta, a.max_grad_norm = cfg.huber_delta, cfg.max_grad_norm
         g = op.param_groups[0]
         a.adam_beta1, a.adam_beta2, a.adam_eps, a.weight_decay = g["betas"][0], g["betas"][1], g["eps"], g["weight_decay"]
+        a.dual_clip_coeff = float(getattr(cfg, "dual_clip_coeff", 3.0))
+        vn = cri.value_normalizer
+        a.vn_state = None if vn is None else lib.ptr(vn.state)
         a.vn_beta = 0.99999 if vn is None else vn.beta
-        a.partials, a.folded, a.grads, a.train_info = (lib.ptr(self.partials), lib.ptr(self.folded),
-                                                        lib.ptr(self.grads), lib.ptr(self.train_info))
+        a.train_info = lib.ptr(self.train_info)
+        # every rank holds an equal shard of the global minibatch: weights / batch moments refer to the global row count
+        a.norm_rows = int(rows) * self.world_size if self.world_size > 1 else 0
+        return a
+
+    def _args(self, buf, batch_rows, indices, row_begin):
+        a = self._common_args(lib.OrlPpoArgs(), batch_rows)
+        a.flags, a.grid_per_net = self.flags, self.grid_per_net
+        a.head_kind = self.head_kind
+        total = buf.episode_length * buf.n_rollout_threads * buf.num_agents
+        a.batch_rows, a.row_begin, a.total_rows = int(batch_rows), int(row_begin), int(total)
+        a.indices = lib.ptr(indices)
+        a.policy_obs, a.critic_obs = lib.ptr(buf.policy_obs), lib.ptr(buf.critic_obs)
+        a.actions, a.old_log_probs = lib.ptr(buf.actions), lib.ptr(buf.action_log_probs)
+        a.advantages, a.value_preds, a.returns = lib.ptr(buf.advantages), lib.ptr(buf.value_preds), lib.ptr(buf.returns)
+        a.active_masks = lib.ptr(buf.active_masks)
+        a.action_masks = None if (buf.action_masks_trivial or buf.continuous) else lib.ptr(buf.action_masks)
+        a.gae_stats = lib.ptr(buf.gae_stats)
+        a.partials, a.folded, a.grads = lib.ptr(self.partials), lib.ptr(self.folded), lib.ptr(self.grads)
         return a
 
     def _share_update(self, buf, batch_rows, indices, row_begin, mb_stats):
@@ -193,37 +198,17 @@ class PPOAlgorithm:
         self.gpu_launches += 3
 
     def _rnn_args(self, buf, chunk_ids, mb_stats):
-        m = self.algo_module
-        pol, cri = m.models["policy"], m.models["critic"]
-        op, oc = m.optimizers["policy"], m.optimizers["critic"]
-        cfg = self.cfg
-        a = lib.OrlRnnArgs()
+        a = self._common_args(lib.OrlRnnArgs(), int(chunk_ids.numel()) * self.chunk_length)
         a.n_envs, a.n_agents, a.episode_length = buf.n_rollout_threads, buf.num_agents, buf.episode_length
-        a.obs_dim, a.critic_obs_dim, a.n_actions, a.activation_id = self.d, self.dc, self.n, pol.activation_id
         a.chunk_length, a.flags = self.chunk_length, self.flags | (lib.PPO_JOINT_ACTION if self._joint(buf) else 0)
         a.n_chunks, a.chunk_ids = int(chunk_ids.numel()), lib.ptr(chunk_ids)
-        a.policy_params, a.critic_params = lib.ptr(pol.flat_params), lib.ptr(cri.flat_params)
         a.policy_obs, a.critic_obs = lib.ptr(buf.policy_obs), lib.ptr(buf.critic_obs)
         a.rnn_states, a.rnn_states_critic = lib.ptr(buf.rnn_states), lib.ptr(buf.rnn_states_critic)
         a.actions, a.action_log_probs = lib.ptr(buf.actions), lib.ptr(buf.action_log_probs)
         a.masks, a.active_masks = lib.ptr(buf.masks), lib.ptr(buf.active_masks)
         a.value_preds, a.returns, a.advantages = lib.ptr(buf.value_preds), lib.ptr(buf.returns), lib.ptr(buf.advantages)
         a.gae_stats, a.mb_stats = lib.ptr(buf.gae_stats), lib.ptr(mb_stats)
-        vn = cri.value_normalizer
-        a.vn_state = None if vn is None else lib.ptr(vn.state)
         a.tape, a.grads, a.grads_stride, a.loss_acc = lib.ptr(self.tape), lib.ptr(self.rnn_grads), self.rnn_stride, lib.ptr(self.loss_acc)
-        a.policy_adam_m, a.policy_adam_v = lib.ptr(op.exp_avg), lib.ptr(op.exp_avg_sq)
-        a.critic_adam_m, a.critic_adam_v = lib.ptr(oc.exp_avg), lib.ptr(oc.exp_avg_sq)
-        a.adam_steps, a.lrs = lib.ptr(m.adam_steps), lib.ptr(self.lrs)
-        a.clip_param, a.entropy_coef, a.value_loss_coef = cfg.clip_param, cfg.entropy_coef, cfg.value_loss_coef
-        a.huber_delta, a.max_grad_norm = cfg.huber_delta, cfg.max_grad_norm
-        g = op.param_groups[0]
-        a.adam_beta1, a.adam_beta2, a.adam_eps, a.weight_decay = g["betas"][0], g["betas"][1], g["eps"], g["weight_decay"]
-        a.dual_clip_coeff = float(getattr(cfg, "dual_clip_coeff", 3.0))
-        a.vn_beta = 0.99999 if vn is None else vn.beta
-        a.train_info = lib.ptr(self.train_info)
-        rows = int(chunk_ids.numel()) * self.chunk_length
-        a.norm_rows = rows * self.world_size if self.world_size > 1 else 0
         return a
 
     def _joint(self, buf):

@@ -14,6 +14,9 @@ int sm_count();
 // advances the device Philox step counter of the action noise by the `steps` steps a rollout launch consumed; no-op
 // when `counter` is null
 int bump_rng_counter(uint64_t* counter, int steps, cudaStream_t st);
+// out[i] = sum over rb < row_blocks of partials[rb * stride + i] for i < total, in row-block order (deterministic): the
+// second stage of the tape-gradient reductions of the recurrent and shared-model updates
+int sum_row_blocks(const float* partials, int row_blocks, int stride, int total, float* out, cudaStream_t st);
 
 #define ORL_CHECK_ARG(cond, msg)                                   \
     do {                                                           \

@@ -2,7 +2,7 @@
 // log-prob) shared by every rollout kernel.
 #pragma once
 #include "orl_envs.cuh"
-#include "orl_mlp.cuh"
+#include "orl_loss.cuh"
 
 namespace orl {
 
@@ -121,25 +121,6 @@ __device__ __forceinline__ void action_noise(const float* exp_noise, size_t grow
 #pragma unroll
         for (int j = 0; j < MAX_OUT; ++j) q[j] = -logf(u32_to_unit_open(rr[j]));
     }
-}
-
-// log_softmax_n of a row's logits with the masked-out actions (mask row entry 0, nullable) at -6e4
-__device__ __forceinline__ void masked_log_softmax(float (&logit)[MAX_OUT], int n, const float* mask_row,
-                                                   float (&nl)[MAX_OUT], float (&pr)[MAX_OUT]) {
-    if (mask_row) {
-#pragma unroll
-        for (int j = 0; j < MAX_OUT; ++j)
-            if (j < n && mask_row[j] == 0.f) logit[j] = -6e4f;
-    }
-    log_softmax_n(logit, n, nl, pr);
-}
-
-// log-prob of action `act`; an action outside [0, n) gets nl[0]
-__device__ __forceinline__ float log_prob_of(const float (&nl)[MAX_OUT], int n, int act) {
-    float lp = nl[0];
-#pragma unroll
-    for (int j = 1; j < MAX_OUT; ++j) if (j < n && j == act) lp = nl[j];
-    return lp;
 }
 
 // Categorical action of one row and its log-prob: the first-max mode when deterministic, else torch.multinomial(probs, 1)

@@ -1,8 +1,76 @@
-// Loss-side scalar helpers shared by the feed-forward (orl_ppo.cu) and recurrent (orl_rnn.cu) PPO updates.
+// The PPO loss maths, in one place: the categorical log-softmax and log-prob that the rollout sampler (orl_envstep.cuh)
+// shares with the updates, and the per-minibatch constants, categorical row loss and value row loss of every update
+// kernel (ppo_net_pass in orl_ppo.cu, tc_net_pass in orl_ppo_tc.cu, the chunk and JRPO kernels of orl_rnn.cu,
+// share_fwdbwd_kernel in orl_share.cu).  The FFMA Gaussian head loss has one user and stays in ppo_net_pass.
 #pragma once
 #include "orl_mlp.cuh"
 
 namespace orl {
+
+// torch.distributions.Categorical(logits=x): normalised logits nl = x - logsumexp(x), probs =
+// softmax(nl).  Masked entries were set to -6e4 by the caller (distributions.py:71).
+__device__ __forceinline__ void log_softmax_n(const float (&x)[MAX_OUT], int n, float (&nl)[MAX_OUT],
+                                              float (&p)[MAX_OUT]) {
+    float mx = x[0];
+#pragma unroll
+    for (int j = 1; j < MAX_OUT; ++j) if (j < n) mx = fmaxf(mx, x[j]);
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < MAX_OUT; ++j) if (j < n) s += expf(x[j] - mx);
+    const float lse = mx + logf(s);
+    float mx2 = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < MAX_OUT; ++j) if (j < n) { nl[j] = x[j] - lse; mx2 = fmaxf(mx2, nl[j]); }
+    float s2 = 0.f;
+#pragma unroll
+    for (int j = 0; j < MAX_OUT; ++j) if (j < n) { p[j] = expf(nl[j] - mx2); s2 += p[j]; }
+#pragma unroll
+    for (int j = 0; j < MAX_OUT; ++j) if (j < n) p[j] = p[j] / s2;
+}
+
+// log_softmax_n of a row's logits with the masked-out actions (mask row entry 0, nullable) at -6e4; returns the
+// masked-out actions as a bit set
+__device__ __forceinline__ unsigned masked_log_softmax(float (&logit)[MAX_OUT], int n, const float* mask_row,
+                                                       float (&nl)[MAX_OUT], float (&pr)[MAX_OUT]) {
+    unsigned masked = 0;
+    if (mask_row) {
+#pragma unroll
+        for (int j = 0; j < MAX_OUT; ++j)
+            if (j < n && mask_row[j] == 0.f) { logit[j] = -6e4f; masked |= 1u << j; }
+    }
+    log_softmax_n(logit, n, nl, pr);
+    return masked;
+}
+
+// log-prob of action `act`; an action outside [0, n) gets nl[0]
+__device__ __forceinline__ float log_prob_of(const float (&nl)[MAX_OUT], int n, int act) {
+    float lp = nl[0];
+#pragma unroll
+    for (int j = 1; j < MAX_OUT; ++j) if (j < n && j == act) lp = nl[j];
+    return lp;
+}
+
+// Policy-gradient term of one (row, action-dimension): PPO clipped surrogate (ppo.py:300-319, with the
+// optional dual clip :304-305) or the A2C loss -adv*logp (a2c.py:88).  Returns the loss contribution
+// (to be weighted by the row weight) and d(loss)/d(logp); `ratio` comes back as the reported ratio.
+struct PgTerm { float loss, dlogp, ratio; };
+__device__ __forceinline__ PgTerm pg_term(float lp, float old_lp, float adv, float clip, int flags, float dual_coeff) {
+    PgTerm o;
+    if (flags & ORL_PPO_A2C) { o.loss = -adv * lp; o.dlogp = -adv; o.ratio = 0.f; return o; }
+    const float raw = expf(lp - old_lp);
+    float ratio = raw, dr = 1.f;                       // dr = d(ratio)/d(raw)
+    if (flags & ORL_PPO_DUAL_CLIP) {                   // torch.min(ratio, coeff): ties split the gradient
+        if (raw > dual_coeff) { ratio = dual_coeff; dr = 0.f; } else if (raw == dual_coeff) dr = 0.5f;
+    }
+    const float lo = 1.0f - clip, hi = 1.0f + clip;
+    const float surr1 = ratio * adv, surr2 = fminf(fmaxf(ratio, lo), hi) * adv;
+    const bool inside = ratio >= lo && ratio <= hi;
+    const float sel = surr1 < surr2 ? 1.f : (surr1 > surr2 ? 0.f : (inside ? 1.f : 0.5f));
+    o.loss = -fminf(surr1, surr2);
+    o.dlogp = -sel * adv * dr * raw;
+    o.ratio = ratio;
+    return o;
+}
 
 struct AdvNorm { float m0, s0, m1, s1; bool two_stage; };
 __device__ __forceinline__ AdvNorm make_adv_norm(const double* __restrict__ gs, bool use_adv_normalize) {
@@ -42,6 +110,75 @@ __device__ __forceinline__ void vn_updated(const float* __restrict__ vn_state, c
     out[0] = __fadd_rn(__fmul_rn(vn_state[0], beta), __fmul_rn(bm, omw));
     out[1] = __fadd_rn(__fmul_rn(vn_state[1], beta), __fmul_rn(bsq, omw));
     out[2] = __fadd_rn(__fmul_rn(vn_state[2], beta), __fmul_rn(1.0f, omw));
+}
+
+// Rows behind the 1/rows loss weights, the reported ratio mean and the ValueNorm batch moments: the global minibatch
+// (norm_rows) when ranks share the update, else this call's rows (feed-forward) or chunk steps (recurrent).
+__device__ __forceinline__ double loss_rows(const OrlPpoArgs& a) { return (double)(a.norm_rows > 0 ? a.norm_rows : a.batch_rows); }
+__device__ __forceinline__ double loss_rows(const OrlRnnArgs& a) {
+    return a.norm_rows > 0 ? (double)a.norm_rows : (double)a.n_chunks * a.chunk_length;
+}
+
+// Per-minibatch constants of an update kernel, built once per kernel: the row weights 1/rows and 1/sum(active), the
+// advantage normalisation, and the ValueNorm mean / std after this minibatch's update (0 / 1 without ORL_PPO_VALUENORM).
+struct MbConsts {
+    float inv_rows, inv_act;
+    AdvNorm adv;
+    float vn_mean, vn_std;
+    // loss weight of a row: active / sum(active) with the active-mask option, else 1 / rows
+    __device__ __forceinline__ float weight(bool use_active_masks, float active) const {
+        return use_active_masks ? active * inv_act : inv_rows;
+    }
+};
+template <class Args>
+__device__ __forceinline__ MbConsts mb_consts(const Args& a) {
+    MbConsts c;
+    const double rows = loss_rows(a);
+    c.inv_rows = (float)(1.0 / rows);
+    c.inv_act = (float)(1.0 / a.mb_stats[2]);
+    c.adv = make_adv_norm(a.gae_stats, a.flags & ORL_PPO_ADV_NORMALIZE);
+    c.vn_mean = 0.f; c.vn_std = 1.f;
+    if (a.flags & ORL_PPO_VALUENORM) {
+        float st[3];
+        vn_updated(a.vn_state, a.mb_stats, rows, a.vn_beta, st);
+        const VnScalars s = vn_mean_std(st);
+        c.vn_mean = s.mean; c.vn_std = s.std;
+    }
+    return c;
+}
+
+// entropy of a categorical row (act.py:160-168)
+template <int NOUT = MAX_OUT>
+__device__ __forceinline__ float categorical_entropy(const float (&nl)[MAX_OUT], const float (&pr)[MAX_OUT], int n) {
+    float ent = 0.f;
+#pragma unroll
+    for (int j = 0; j < NOUT; ++j) if (j < n) ent -= pr[j] * nl[j];
+    return ent;
+}
+
+// dL/dlogits of a categorical row from d(loss)/d(logp) `dlp` and the entropy weight `went` (entropy_coef x row
+// weight).  Writes the unmasked entries j < n only; the masked-out actions (bits of `masked`) get no gradient.
+template <int NOUT = MAX_OUT>
+__device__ __forceinline__ void categorical_dlogits(float dlp, float went, int act, int n, unsigned masked,
+                                                    const float (&nl)[MAX_OUT], const float (&pr)[MAX_OUT], float ent,
+                                                    float (&dl)[MAX_OUT]) {
+#pragma unroll
+    for (int j = 0; j < NOUT; ++j)
+        if (j < n && !((masked >> j) & 1u)) dl[j] = dlp * ((j == act ? 1.f : 0.f) - pr[j]) + went * pr[j] * (nl[j] + ent);
+}
+
+// Policy loss of one categorical row (ppo.py:300-319, entropy act.py:160-168): masks the logits in place, writes
+// dL/dlogits (entries as categorical_dlogits) and returns the unweighted policy loss and entropy and the ratio.
+struct CatRow { float loss, ent, ratio; };
+template <int NOUT = MAX_OUT, class Args>
+__device__ __forceinline__ CatRow categorical_row(const Args& a, float (&logit)[MAX_OUT], int n, const float* mask_row,
+                                                  int act, float old_lp, float adv, float wrow, float (&dl)[MAX_OUT]) {
+    float nl[MAX_OUT], pr[MAX_OUT];
+    const unsigned masked = masked_log_softmax(logit, n, mask_row, nl, pr);
+    const PgTerm pg = pg_term(log_prob_of(nl, n, act), old_lp, adv, a.clip_param, a.flags, a.dual_clip_coeff);
+    const float ent = categorical_entropy<NOUT>(nl, pr, n);
+    categorical_dlogits<NOUT>(pg.dlogp * wrow, a.entropy_coef * wrow, act, n, masked, nl, pr, ent, dl);
+    return CatRow{pg.loss, ent, pg.ratio};
 }
 
 __device__ __forceinline__ float huber(float e, float d) { return fabsf(e) <= d ? 0.5f * e * e : d * (fabsf(e) - 0.5f * d); }

@@ -291,48 +291,4 @@ __device__ __forceinline__ void head_dots(const SmemWeights& w, const float* __r
     }
 }
 
-// torch.distributions.Categorical(logits=x): normalised logits nl = x - logsumexp(x), probs =
-// softmax(nl).  Masked entries were set to -6e4 by the caller (distributions.py:71).
-__device__ __forceinline__ void log_softmax_n(const float (&x)[MAX_OUT], int n, float (&nl)[MAX_OUT],
-                                              float (&p)[MAX_OUT]) {
-    float mx = x[0];
-#pragma unroll
-    for (int j = 1; j < MAX_OUT; ++j) if (j < n) mx = fmaxf(mx, x[j]);
-    float s = 0.f;
-#pragma unroll
-    for (int j = 0; j < MAX_OUT; ++j) if (j < n) s += expf(x[j] - mx);
-    const float lse = mx + logf(s);
-    float mx2 = -INFINITY;
-#pragma unroll
-    for (int j = 0; j < MAX_OUT; ++j) if (j < n) { nl[j] = x[j] - lse; mx2 = fmaxf(mx2, nl[j]); }
-    float s2 = 0.f;
-#pragma unroll
-    for (int j = 0; j < MAX_OUT; ++j) if (j < n) { p[j] = expf(nl[j] - mx2); s2 += p[j]; }
-#pragma unroll
-    for (int j = 0; j < MAX_OUT; ++j) if (j < n) p[j] = p[j] / s2;
-}
-
-
-// Policy-gradient term of one (row, action-dimension): PPO clipped surrogate (ppo.py:300-319, with the
-// optional dual clip :304-305) or the A2C loss -adv*logp (a2c.py:88).  Returns the loss contribution
-// (to be weighted by the row weight) and d(loss)/d(logp); `ratio` comes back as the reported ratio.
-struct PgTerm { float loss, dlogp, ratio; };
-__device__ __forceinline__ PgTerm pg_term(float lp, float old_lp, float adv, float clip, int flags, float dual_coeff) {
-    PgTerm o;
-    if (flags & ORL_PPO_A2C) { o.loss = -adv * lp; o.dlogp = -adv; o.ratio = 0.f; return o; }
-    const float raw = expf(lp - old_lp);
-    float ratio = raw, dr = 1.f;                       // dr = d(ratio)/d(raw)
-    if (flags & ORL_PPO_DUAL_CLIP) {                   // torch.min(ratio, coeff): ties split the gradient
-        if (raw > dual_coeff) { ratio = dual_coeff; dr = 0.f; } else if (raw == dual_coeff) dr = 0.5f;
-    }
-    const float lo = 1.0f - clip, hi = 1.0f + clip;
-    const float surr1 = ratio * adv, surr2 = fminf(fmaxf(ratio, lo), hi) * adv;
-    const bool inside = ratio >= lo && ratio <= hi;
-    const float sel = surr1 < surr2 ? 1.f : (surr1 > surr2 ? 0.f : (inside ? 1.f : 0.5f));
-    o.loss = -fminf(surr1, surr2);
-    o.dlogp = -sel * adv * dr * raw;
-    o.ratio = ratio;
-    return o;
-}
-
 }  // namespace orl

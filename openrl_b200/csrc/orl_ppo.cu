@@ -13,7 +13,7 @@
 // Arithmetic per row (d=4, n=2, both nets): ~53 kFLOP; bytes per row: ~60 B  => fp32-pipe bound.
 #include <algorithm>
 
-#include "orl_loss.cuh"
+#include "orl_adam.cuh"
 
 namespace {
 using namespace orl;
@@ -125,19 +125,7 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
     load_weights_folded<P_NT>(w, params, d, n, true);
 
     const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS, val_masks = a.flags & ORL_PPO_VALUE_ACTIVE_MASKS;
-    const double rows_d = (double)(a.norm_rows > 0 ? a.norm_rows : a.batch_rows);
-    const float inv_rows = (float)(1.0 / rows_d);
-    const float inv_act = (float)(1.0 / a.mb_stats[2]);
-    AdvNorm advn;
-    float vn_mean = 0.f, vn_std = 1.f;
-    if (POLICY) {
-        advn = make_adv_norm(a.gae_stats, a.flags & ORL_PPO_ADV_NORMALIZE);
-    } else if (a.flags & ORL_PPO_VALUENORM) {
-        float st[3];
-        vn_updated(a.vn_state, a.mb_stats, rows_d, a.vn_beta, st);
-        const VnScalars s = vn_mean_std(st);
-        vn_mean = s.mean; vn_std = s.std;
-    }
+    const MbConsts mb = mb_consts(a);
 
     const WgMap map3 = wg_map(16, 16);
     const WgMap map1 = wg_map(16, dp / 4);
@@ -192,9 +180,9 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
                         // surrogate summed over the action dimension (ppo.py:307-319)
                         const long long gi = row_idx[row];
                         const float* logstd = params + net_offsets(d, n, 1).ls;
-                        const float adv = apply_adv_norm(advn, row_c[row]);
-                        const float wrow = pol_masks ? active * inv_act : inv_rows;
-                        const float went_row = pol_masks ? active * inv_act : inv_rows / (float)n;
+                        const float adv = apply_adv_norm(mb.adv, row_c[row]);
+                        const float wrow = mb.weight(pol_masks, active);
+                        const float went_row = pol_masks ? active * mb.inv_act : mb.inv_rows / (float)n;
 #pragma unroll
                         for (int j = 0; j < MAX_OUT; ++j) {
                             if (j < n) {
@@ -212,58 +200,19 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
                         }
                     } else if (POLICY) {
                         const long long gi = row_idx[row];
-                        unsigned masked = 0;
-                        if (a.action_masks) {
-#pragma unroll
-                            for (int j = 0; j < MAX_OUT; ++j)
-                                if (j < n && a.action_masks[gi * n + j] == 0.f) { out[j] = -6e4f; masked |= 1u << j; }
-                        }
-                        float nl[MAX_OUT], pr[MAX_OUT];
-                        log_softmax_n(out, n, nl, pr);
-                        const int act = (int)row_a[row];
-                        float lp = nl[0];
-#pragma unroll
-                        for (int j = 1; j < MAX_OUT; ++j) if (j == act) lp = nl[j];
-                        const float adv = apply_adv_norm(advn, row_c[row]);
-                        const PgTerm pg = pg_term(lp, row_b[row], adv, a.clip_param, a.flags, a.dual_clip_coeff);
-                        const float wrow = pol_masks ? active * inv_act : inv_rows;
-                        float ent = 0.f;
-#pragma unroll
-                        for (int j = 0; j < MAX_OUT; ++j) if (j < n) ent -= pr[j] * nl[j];
-                        loss0 += pg.loss * wrow;
-                        loss1 += ent * wrow;
-                        loss2 += pg.ratio;
-                        const float dlp = pg.dlogp * wrow;
-                        const float went = a.entropy_coef * wrow;
-#pragma unroll
-                        for (int j = 0; j < MAX_OUT; ++j) {
-                            if (j < n && !((masked >> j) & 1u)) {
-                                const float onehot = (j == act) ? 1.f : 0.f;
-                                dl[j] = dlp * (onehot - pr[j]) + went * pr[j] * (nl[j] + ent);
-                            }
-                        }
+                        const float wrow = mb.weight(pol_masks, active);
+                        const CatRow c = categorical_row(a, out, n, a.action_masks ? a.action_masks + gi * n : nullptr, (int)row_a[row],
+                                                         row_b[row], apply_adv_norm(mb.adv, row_c[row]), wrow, dl);
+                        loss0 += c.loss * wrow;
+                        loss1 += c.ent * wrow;
+                        loss2 += c.ratio;
                     } else {
-                        const float v = out[0], vp = row_a[row], ret = row_b[row];
-                        const float target = (a.flags & ORL_PPO_VALUENORM) ? (ret - vn_mean) / vn_std : ret;
-                        const float diff = v - vp;
-                        const float clipped = vp + fminf(fmaxf(diff, -a.clip_param), a.clip_param);
-                        const float e_c = target - clipped, e_o = target - v;
-                        const bool hub = a.flags & ORL_PPO_HUBER;
-                        const float l_c = hub ? huber(e_c, a.huber_delta) : 0.5f * e_c * e_c;
-                        const float l_o = hub ? huber(e_o, a.huber_delta) : 0.5f * e_o * e_o;
-                        const float gc = hub ? huber_grad(e_c, a.huber_delta) : e_c;
-                        const float go = hub ? huber_grad(e_o, a.huber_delta) : e_o;
-                        float l = l_o, dv = -go;
-                        if (a.flags & ORL_PPO_CLIP_VALUE) {
-                            const bool inrange = diff >= -a.clip_param && diff <= a.clip_param;
-                            const float dc = inrange ? -gc : 0.f;
-                            if (l_o > l_c) { l = l_o; dv = -go; }
-                            else if (l_c > l_o) { l = l_c; dv = dc; }
-                            else { l = l_o; dv = 0.5f * (-go) + 0.5f * dc; }
-                        }
-                        const float wrow = val_masks ? active * inv_act : inv_rows;
-                        loss0 += l * wrow;
-                        dl[0] = a.value_loss_coef * wrow * dv;
+                        const float ret = row_b[row];
+                        const float target = (a.flags & ORL_PPO_VALUENORM) ? (ret - mb.vn_mean) / mb.vn_std : ret;
+                        const ValueTerm vt = value_term(out[0], row_a[row], target, a.clip_param, a.huber_delta, a.flags);
+                        const float wrow = mb.weight(val_masks, active);
+                        loss0 += vt.loss * wrow;
+                        dl[0] = a.value_loss_coef * wrow * vt.dv;
                     }
                 }
                 *reinterpret_cast<float4*>(DLs + row * DLW) = make_float4(dl[0], dl[1], dl[2], dl[3]);
@@ -525,8 +474,6 @@ __global__ void __launch_bounds__(1024) ppo_apply_kernel(const OrlPpoArgs a, con
     float* am = net == 0 ? a.policy_adam_m : a.critic_adam_m;
     float* av = net == 0 ? a.policy_adam_v : a.critic_adam_v;
     float* grads = a.grads + (size_t)net * ppo_grads_stride(a.obs_dim, a.critic_obs_dim, a.n_actions);
-    __shared__ float red[32];
-    __shared__ float s_norm;
     const int tid = threadIdx.x;
     const float* f = PEER ? peer_gather(pa, net, stride) : a.folded + (size_t)net * stride;
 
@@ -563,63 +510,17 @@ __global__ void __launch_bounds__(1024) ppo_apply_kernel(const OrlPpoArgs a, con
         grads[i] = g;
         sq = fmaf(g, g, sq);
     }
-    {
-        const float s = warp_sum(sq);
-        if ((tid & 31) == 0) red[tid >> 5] = s;
-        __syncthreads();
-        if (tid < 32) {
-            float v = (tid < (int)(blockDim.x >> 5)) ? red[tid] : 0.f;
-            v = warp_sum(v);
-            if (tid == 0) s_norm = sqrtf(v);
-        }
-        __syncthreads();
-    }
-    const float norm = s_norm;
-    float clip = 1.f;
-    if (a.flags & ORL_PPO_MAX_GRAD_NORM) clip = fminf(a.max_grad_norm / (norm + 1e-6f), 1.0f);
-
-    const int step = a.adam_steps[net] + 1;
-    __shared__ float s_adam[2];
-    if (tid == (int)blockDim.x - 1) {   // the two double-precision pow() once per CTA (f64 is slow here), not once per thread
-        const double bc1 = 1.0 - pow((double)a.adam_beta1, (double)step);
-        const double bc2 = 1.0 - pow((double)a.adam_beta2, (double)step);
-        s_adam[0] = (float)((double)a.lrs[net] / bc1);
-        s_adam[1] = (float)sqrt(bc2);
-    }
-    __syncthreads();  // every thread has read the parameters it needs for unfolding; the step constants are in place
-    const float step_size = s_adam[0], bc2_sqrt = s_adam[1];
-    for (int i = tid; i < po.total; i += blockDim.x) {
-        float g = grads[i] * clip;
-        float pv = params[i];
-        if (a.weight_decay != 0.f) g = fmaf(a.weight_decay, pv, g);
-        const float m = am[i] + (g - am[i]) * (1.f - a.adam_beta1);          // exp_avg.lerp_(grad, 1-beta1)
-        const float v = fmaf(av[i], a.adam_beta2, (g * g) * (1.f - a.adam_beta2));  // mul_(beta2).addcmul_(g,g,1-beta2)
-        am[i] = m; av[i] = v;
-        const float denom = sqrtf(v) / bc2_sqrt + a.adam_eps;
-        params[i] = pv - step_size * (m / denom);
-    }
+    const float norm = block_l2_norm(sq);
+    adam_step(a, net, params, am, av, grads, po.total, clip_factor(a, norm));   // after every thread's unfolding reads of params
     if (tid == 0) {
-        a.adam_steps[net] = step;
         if (PEER) {
             pa.epochs[net] += 1u;
             // a peer timed out: poison the logged scalars so that the host's one read-back sees it (it then reads error_flag)
             if (*reinterpret_cast<volatile int32_t*>(pa.error_flag) != 0) a.train_info[net == 0 ? 2 : 0] = __int_as_float(0x7fc00000);
         }
         const float* ls = f + stride - N_LOSS;
-        if (net == 0) {
-            a.train_info[2] += ls[0];
-            a.train_info[3] += ls[1];
-            a.train_info[4] += norm;
-            a.train_info[5] += ls[2] / (float)(a.norm_rows > 0 ? a.norm_rows : a.batch_rows);
-        } else {
-            a.train_info[0] += ls[0];
-            a.train_info[1] += norm;
-            if (a.flags & ORL_PPO_VALUENORM) {
-                float st[3];
-                vn_updated(a.vn_state, a.mb_stats, (double)(a.norm_rows > 0 ? a.norm_rows : a.batch_rows), a.vn_beta, st);
-                a.vn_state[0] = st[0]; a.vn_state[1] = st[1]; a.vn_state[2] = st[2];
-            }
-        }
+        if (net == 0) add_policy_info(a, ls, norm);
+        else add_value_info(a, ls[0], norm);
     }
 }
 

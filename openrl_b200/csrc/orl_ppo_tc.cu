@@ -45,7 +45,7 @@
 #include <map>
 #include <mutex>
 
-#include "orl_mlp.cuh"
+#include "orl_loss.cuh"
 #include "orl_tc16.cuh"
 
 namespace orl {
@@ -79,8 +79,6 @@ constexpr int N_SCAL = 4;                      // scalar columns staged per row
 struct TcMaps {   // TMA descriptors of the flattened rollout buffers (built by the launcher)
     CUtensorMap obs_p, obs_c, actions, old_logp, adv, value_preds, returns, active;
 };
-
-struct AdvNormTc { float m0, s0, m1, s1; bool two; };
 
 #define FOR_OUT(j) _Pragma("unroll") for (int j = 0; j < NOUT; ++j) if (NOUT != 8 || j < n)
 // the two column halves of a row sit in lanes l and l ^ 16 of one warp
@@ -177,9 +175,8 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
 
     // ---- minibatch constants ----
     const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS, val_masks = a.flags & ORL_PPO_VALUE_ACTIVE_MASKS;
-    const double rows_d = (double)(a.norm_rows > 0 ? a.norm_rows : a.batch_rows);
-    const float inv_rows = (float)(1.0 / rows_d), inv_act = (float)(1.0 / a.mb_stats[2]);
-    // operand scale of the backward GEMMs: 2^e ~ rows / 16 (row weights are ~ 1/rows)
+    const MbConsts mb = mb_consts(a);
+    const double rows_d = loss_rows(a);
     // operand scales of the backward GEMMs (powers of two; see the header comment)
     float wmax = 0.f;
     for (int i = 0; i < MAX_OUT * H; ++i) wmax = fmaxf(wmax, fabsf(whf[i]));   // smem broadcast reads, once per kernel
@@ -189,31 +186,6 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     const float Sz = exp2f((float)e_z), Su = exp2f((float)e_u);
     constexpr float SX = 16.f, K1 = 0.25f;          // observations x 16; dZ1 is stored as S_z / 4
     const float invSz = exp2f(-(float)e_z), invSu = exp2f(-(float)e_u), invS1 = invSz * (1.f / K1);
-    AdvNormTc an = {0.f, 1.f, 0.f, 1.f, false};
-    float vn_mean = 0.f, vn_std = 1.f;
-    if (POLICY) {  // ppo.py:402-409
-        const double* gs = a.gae_stats;
-        const double n_all = gs[ORL_GS_COUNT], n_act = gs[ORL_GS_ACT_COUNT];
-        const double mean_all = gs[ORL_GS_ADV_SUM] / n_all;
-        const double var_all = fmax(gs[ORL_GS_ADV_SQSUM] / n_all - mean_all * mean_all, 0.0);
-        double mean_act = gs[ORL_GS_ADV_ACT_SUM] / n_act;
-        double std_act = sqrt(fmax(gs[ORL_GS_ADV_ACT_SQSUM] / n_act - mean_act * mean_act, 0.0));
-        if (a.flags & ORL_PPO_ADV_NORMALIZE) {
-            const double s0 = (double)((float)sqrt(var_all)) + 1e-5;
-            an.two = true; an.m0 = (float)mean_all; an.s0 = (float)s0;
-            mean_act = (mean_act - mean_all) / s0; std_act = std_act / s0;
-        }
-        an.m1 = (float)mean_act; an.s1 = (float)((double)((float)std_act) + 1e-5);
-    } else if (a.flags & ORL_PPO_VALUENORM) {
-        const float bm = (float)(a.mb_stats[0] / rows_d), bsq = (float)(a.mb_stats[1] / rows_d);
-        const float beta = (float)a.vn_beta, omw = (float)(1.0 - a.vn_beta);
-        float st[3];
-        st[0] = __fadd_rn(__fmul_rn(a.vn_state[0], beta), __fmul_rn(bm, omw));
-        st[1] = __fadd_rn(__fmul_rn(a.vn_state[1], beta), __fmul_rn(bsq, omw));
-        st[2] = __fadd_rn(__fmul_rn(a.vn_state[2], beta), __fmul_rn(1.0f, omw));
-        const VnScalars s = vn_mean_std(st);
-        vn_mean = s.mean; vn_std = s.std;
-    }
 
     // ---- MMA descriptors (constant parts) ----
     const uint64_t dK_A = desc_const(PANEL, 128), dK_W = desc_const(PANEL_W, 128);      // K-major
@@ -400,51 +372,16 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         for (int j = 0; j < MAX_OUT; ++j) dl[j] = 0.f;
         if (valid) {
             if (POLICY) {
-                unsigned masked = 0;
-                if (a.action_masks) {
-#pragma unroll
-                    for (int j = 0; j < MAX_OUT; ++j)
-                        if (j < n && a.action_masks[gi_cur * n + j] == 0.f) { out[j] = -6e4f; masked |= 1u << j; }
-                }
-                float nl[MAX_OUT], pr[MAX_OUT];
-                log_softmax_n(out, n, nl, pr);
-                const int act = (int)row_a;
-                float lp = nl[0];
-#pragma unroll
-                for (int j = 1; j < MAX_OUT; ++j) if (j == act) lp = nl[j];
-                float adv = row_c;
-                if (an.two) adv = (adv - an.m0) / an.s0;
-                adv = (adv - an.m1) / an.s1;
-                const PgTerm pg = pg_term(lp, row_b, adv, a.clip_param, a.flags, a.dual_clip_coeff);
-                const float wrow = pol_masks ? active * inv_act : inv_rows;
-                float ent = 0.f;
-#pragma unroll
-                for (int j = 0; j < MAX_OUT; ++j) if (j < n) ent -= pr[j] * nl[j];
-                if (half == 0) { loss0 += pg.loss * wrow; loss1 += ent * wrow; loss2 += pg.ratio; }
-                const float dlp = pg.dlogp * wrow, went = a.entropy_coef * wrow;
-#pragma unroll
-                for (int j = 0; j < MAX_OUT; ++j)
-                    if (j < n && !((masked >> j) & 1u)) dl[j] = dlp * ((j == act ? 1.f : 0.f) - pr[j]) + went * pr[j] * (nl[j] + ent);
+                const float wrow = mb.weight(pol_masks, active);
+                const CatRow c = categorical_row<NOUT>(a, out, n, a.action_masks ? a.action_masks + gi_cur * n : nullptr, (int)row_a, row_b,
+                                                       apply_adv_norm(mb.adv, row_c), wrow, dl);
+                if (half == 0) { loss0 += c.loss * wrow; loss1 += c.ent * wrow; loss2 += c.ratio; }
             } else {
-                const float v = out[0], vp = row_a, ret = row_b;
-                const float target = (a.flags & ORL_PPO_VALUENORM) ? (ret - vn_mean) / vn_std : ret;
-                const float diff = v - vp;
-                const float clipped = vp + fminf(fmaxf(diff, -a.clip_param), a.clip_param);
-                const float e_c = target - clipped, e_o = target - v, dlt = a.huber_delta;
-                const bool hub = a.flags & ORL_PPO_HUBER;
-                const float l_c = hub ? (fabsf(e_c) <= dlt ? 0.5f * e_c * e_c : dlt * (fabsf(e_c) - 0.5f * dlt)) : 0.5f * e_c * e_c;
-                const float l_o = hub ? (fabsf(e_o) <= dlt ? 0.5f * e_o * e_o : dlt * (fabsf(e_o) - 0.5f * dlt)) : 0.5f * e_o * e_o;
-                const float gc = hub ? (fabsf(e_c) <= dlt ? e_c : (e_c > 0.f ? dlt : -dlt)) : e_c;
-                const float go = hub ? (fabsf(e_o) <= dlt ? e_o : (e_o > 0.f ? dlt : -dlt)) : e_o;
-                float l = l_o, dv = -go;
-                if (a.flags & ORL_PPO_CLIP_VALUE) {
-                    const bool inrange = diff >= -a.clip_param && diff <= a.clip_param;
-                    const float dc = inrange ? -gc : 0.f;
-                    if (l_o > l_c) { l = l_o; dv = -go; } else if (l_c > l_o) { l = l_c; dv = dc; } else { l = l_o; dv = 0.5f * (-go) + 0.5f * dc; }
-                }
-                const float wrow = val_masks ? active * inv_act : inv_rows;
-                if (half == 0) loss0 += l * wrow;
-                dl[0] = a.value_loss_coef * wrow * dv;
+                const float target = (a.flags & ORL_PPO_VALUENORM) ? (row_b - mb.vn_mean) / mb.vn_std : row_b;
+                const ValueTerm vt = value_term(out[0], row_a, target, a.clip_param, a.huber_delta, a.flags);
+                const float wrow = mb.weight(val_masks, active);
+                if (half == 0) loss0 += vt.loss * wrow;
+                dl[0] = a.value_loss_coef * wrow * vt.dv;
             }
         }
         // ---- dn3 = dL . Whf ; LayerNorm-3 backward -> dZ3 (single pass: the two row means are

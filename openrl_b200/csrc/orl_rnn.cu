@@ -19,8 +19,8 @@
 // (tests/debug_gru.py).
 #include <algorithm>
 
+#include "orl_adam.cuh"
 #include "orl_envstep.cuh"
-#include "orl_loss.cuh"
 #include "orl_rnn_core.h"
 #include "orl_rnn_warp.cuh"
 
@@ -233,19 +233,8 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
     float* scr = smem + rw::smem_net_floats() + warp * C_R * rw::SCR;
     float loss0 = 0.f, loss1 = 0.f, loss2 = 0.f;   // identical on every lane; lane 0's copy is reduced
 
-    const double rows_d = a.norm_rows > 0 ? (double)a.norm_rows : (double)a.n_chunks * L;
-    const float inv_rows = (float)(1.0 / rows_d);
-    const float inv_act = (float)(1.0 / a.mb_stats[2]);
+    const MbConsts mb = mb_consts(a);
     const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS, val_masks = a.flags & ORL_PPO_VALUE_ACTIVE_MASKS;
-    AdvNorm advn;
-    float vn_mean = 0.f, vn_std = 1.f;
-    if (POLICY) advn = make_adv_norm(a.gae_stats, a.flags & ORL_PPO_ADV_NORMALIZE);
-    else if (a.flags & ORL_PPO_VALUENORM) {
-        float st[3];
-        vn_updated(a.vn_state, a.mb_stats, rows_d, a.vn_beta, st);
-        const VnScalars s = vn_mean_std(st);
-        vn_mean = s.mean; vn_std = s.std;
-    }
 
     const long long n_groups = (a.n_chunks + C_R - 1) / C_R;
     for (long long grp = (long long)blockIdx.x * C_WPC + warp; grp < n_groups; grp += (long long)gridDim.x * C_WPC) {
@@ -284,28 +273,15 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
                 const float active = a.active_masks[bi[r]];
                 const float keep = valid[r] ? 1.f : 0.f;
                 if (POLICY) {
-                    float nl[MAX_OUT], pr[MAX_OUT];
-                    log_softmax_n(out[r], n, nl, pr);
-                    const int act = (int)a.actions[bi[r]];
-                    float lp = nl[0];
-#pragma unroll
-                    for (int j = 1; j < MAX_OUT; ++j) if (j == act) lp = nl[j];
-                    const float adv = apply_adv_norm(advn, a.advantages[bi[r]]);
-                    const PgTerm pg = pg_term(lp, a.action_log_probs[bi[r]], adv, a.clip_param, a.flags, a.dual_clip_coeff);
-                    const float wrow = pol_masks ? active * inv_act : inv_rows;
-                    float ent = 0.f;
-#pragma unroll
-                    for (int j = 0; j < MAX_OUT; ++j) if (j < n) ent -= pr[j] * nl[j];
-                    loss0 += keep * pg.loss * wrow; loss1 += keep * ent * wrow; loss2 += keep * pg.ratio;
-                    const float dlp = pg.dlogp * wrow, went = a.entropy_coef * wrow;
-#pragma unroll
-                    for (int j = 0; j < MAX_OUT; ++j)
-                        if (j < n) dl[j] = dlp * ((j == act ? 1.f : 0.f) - pr[j]) + went * pr[j] * (nl[j] + ent);
+                    const float wrow = mb.weight(pol_masks, active);
+                    const CatRow c = categorical_row(a, out[r], n, nullptr, (int)a.actions[bi[r]], a.action_log_probs[bi[r]],
+                                                     apply_adv_norm(mb.adv, a.advantages[bi[r]]), wrow, dl);
+                    loss0 += keep * c.loss * wrow; loss1 += keep * c.ent * wrow; loss2 += keep * c.ratio;
                 } else {
                     const float ret = a.returns[bi[r]];
-                    const float target = (a.flags & ORL_PPO_VALUENORM) ? (ret - vn_mean) / vn_std : ret;
+                    const float target = (a.flags & ORL_PPO_VALUENORM) ? (ret - mb.vn_mean) / mb.vn_std : ret;
                     const ValueTerm vt = value_term(out[r][0], a.value_preds[bi[r]], target, a.clip_param, a.huber_delta, a.flags);
-                    const float wrow = val_masks ? active * inv_act : inv_rows;
+                    const float wrow = mb.weight(val_masks, active);
                     loss0 += keep * vt.loss * wrow;
                     dl[0] = a.value_loss_coef * wrow * vt.dv;
                 }
@@ -357,7 +333,7 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_joint_policy_warp_kernel(const Or
     float* scr = smem + rw::smem_net_floats() + warp * A * rw::SCR;
     float loss0 = 0.f, loss1 = 0.f, loss2 = 0.f;   // identical on every lane; lane 0's copy is reduced
 
-    const double groups_d = a.norm_rows > 0 ? (double)a.norm_rows : (double)a.n_chunks * L;
+    const double groups_d = loss_rows(a);
     const float inv_groups = (float)(1.0 / groups_d), inv_rows = (float)(1.0 / (groups_d * A));
     const float inv_act0 = (float)(1.0 / a.mb_stats[2]), inv_act_all = (float)(1.0 / a.mb_stats[5]);
     const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS;
@@ -389,11 +365,7 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_joint_policy_warp_kernel(const Or
                 h[ag] = h2[ag];
                 float nl[MAX_OUT], pr[MAX_OUT];
                 log_softmax_n(out[ag], n, nl, pr);
-                const int act = (int)a.actions[base + ag];
-                float lp = nl[0];
-#pragma unroll
-                for (int j = 1; j < MAX_OUT; ++j) if (j == act) lp = nl[j];
-                joint += lp;
+                joint += log_prob_of(nl, n, (int)a.actions[base + ag]);
                 joint_old += a.action_log_probs[base + ag];
             }
             const float adv = apply_adv_norm(advn, a.advantages[base]);
@@ -403,18 +375,12 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_joint_policy_warp_kernel(const Or
             const float dlp = pg.dlogp * wgrp;
 #pragma unroll
             for (int ag = 0; ag < A; ++ag) {
-                float nl[MAX_OUT], pr[MAX_OUT], dl[MAX_OUT];
+                float nl[MAX_OUT], pr[MAX_OUT], dl[MAX_OUT] = {};
                 log_softmax_n(out[ag], n, nl, pr);
-                const int act = (int)a.actions[base + ag];
                 const float went_w = pol_masks ? a.active_masks[base + ag] * inv_act_all : inv_rows;
-                float ent = 0.f;
-#pragma unroll
-                for (int j = 0; j < MAX_OUT; ++j) if (j < n) ent -= pr[j] * nl[j];
+                const float ent = categorical_entropy(nl, pr, n);
                 loss1 += ent * went_w;
-                const float went = a.entropy_coef * went_w;
-#pragma unroll
-                for (int j = 0; j < MAX_OUT; ++j)
-                    dl[j] = j < n ? dlp * ((j == act ? 1.f : 0.f) - pr[j]) + went * pr[j] * (nl[j] + ent) : 0.f;
+                categorical_dlogits(dlp, a.entropy_coef * went_w, (int)a.actions[base + ag], n, 0u, nl, pr, ent, dl);
                 float mine = 0.f;   // lane m < 8 stores dL/dout[m]
 #pragma unroll
                 for (int j = 0; j < MAX_OUT; ++j) if (lane == j) mine = dl[j];
@@ -538,15 +504,6 @@ __global__ void __launch_bounds__(rc::G3) tape_colsum_kernel(const float* __rest
     partials[(size_t)blockIdx.x * stride + jb.out_off + m] = (s0 + s1) + (s2 + s3);
 }
 
-__global__ void tape_partial_sum_kernel(const float* __restrict__ partials, int row_blocks, int stride, int total,
-                                        float* __restrict__ grads) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return;
-    float s = 0.f;
-    for (int rb = 0; rb < row_blocks; ++rb) s += partials[(size_t)rb * stride + i];
-    grads[i] = s;
-}
-
 TapeJobs make_jobs(int d, int n) {
     const rc::Offsets o = rc::rnn_offsets(d, n);
     TapeJobs t; int g = 0, c = 0;
@@ -572,59 +529,15 @@ int ws_row_blocks(long long rows) { return (int)((rows + TR_ROWS - 1) / TR_ROWS)
 __global__ void __launch_bounds__(1024) rnn_apply_kernel(const OrlRnnArgs a) {
     const int net = blockIdx.x;
     const int total = net == 0 ? rc::rnn_offsets(a.obs_dim, a.n_actions).total : rc::rnn_offsets(a.critic_obs_dim, 1).total;
-    float* params = net == 0 ? a.policy_params : a.critic_params;
-    float* am = net == 0 ? a.policy_adam_m : a.critic_adam_m;
-    float* av = net == 0 ? a.policy_adam_v : a.critic_adam_v;
     const float* grads = a.grads + (size_t)net * a.grads_stride;
-    __shared__ float red[32];
-    __shared__ float s_norm;
-    const int tid = threadIdx.x;
     float sq = 0.f;
-    for (int i = tid; i < total; i += blockDim.x) { const float g = grads[i]; sq = fmaf(g, g, sq); }
-    {
-        const float s = warp_sum(sq);
-        if ((tid & 31) == 0) red[tid >> 5] = s;
-        __syncthreads();
-        if (tid < 32) {
-            float v = (tid < (int)(blockDim.x >> 5)) ? red[tid] : 0.f;
-            v = warp_sum(v);
-            if (tid == 0) s_norm = sqrtf(v);
-        }
-        __syncthreads();
-    }
-    const float norm = s_norm;
-    float clip = 1.f;
-    if (a.flags & ORL_PPO_MAX_GRAD_NORM) clip = fminf(a.max_grad_norm / (norm + 1e-6f), 1.0f);
-    const int step = a.adam_steps[net] + 1;
-    const double bc1 = 1.0 - pow((double)a.adam_beta1, (double)step);
-    const double bc2 = 1.0 - pow((double)a.adam_beta2, (double)step);
-    const float step_size = (float)((double)a.lrs[net] / bc1);
-    const float bc2_sqrt = (float)sqrt(bc2);
-    for (int i = tid; i < total; i += blockDim.x) {
-        float g = grads[i] * clip;
-        const float pv = params[i];
-        if (a.weight_decay != 0.f) g = fmaf(a.weight_decay, pv, g);
-        const float m = am[i] + (g - am[i]) * (1.f - a.adam_beta1);
-        const float v = fmaf(av[i], a.adam_beta2, (g * g) * (1.f - a.adam_beta2));
-        am[i] = m; av[i] = v;
-        params[i] = pv - step_size * (m / (sqrtf(v) / bc2_sqrt + a.adam_eps));
-    }
-    if (tid == 0) {
-        a.adam_steps[net] = step;
-        if (net == 0) {
-            a.train_info[2] += a.loss_acc[0];
-            a.train_info[3] += a.loss_acc[1];
-            a.train_info[4] += norm;
-            a.train_info[5] += a.loss_acc[2] / (float)(a.norm_rows > 0 ? (double)a.norm_rows : (double)a.n_chunks * a.chunk_length);
-        } else {
-            a.train_info[0] += a.loss_acc[3];
-            a.train_info[1] += norm;
-            if (a.flags & ORL_PPO_VALUENORM) {
-                float st[3];
-                vn_updated(a.vn_state, a.mb_stats, a.norm_rows > 0 ? (double)a.norm_rows : (double)a.n_chunks * a.chunk_length, a.vn_beta, st);
-                a.vn_state[0] = st[0]; a.vn_state[1] = st[1]; a.vn_state[2] = st[2];
-            }
-        }
+    for (int i = threadIdx.x; i < total; i += blockDim.x) sq = fmaf(grads[i], grads[i], sq);
+    const float norm = block_l2_norm(sq);
+    adam_step(a, net, net == 0 ? a.policy_params : a.critic_params, net == 0 ? a.policy_adam_m : a.critic_adam_m,
+              net == 0 ? a.policy_adam_v : a.critic_adam_v, grads, total, clip_factor(a, norm));
+    if (threadIdx.x == 0) {
+        if (net == 0) add_policy_info(a, a.loss_acc, norm);
+        else add_value_info(a, a.loss_acc[3], norm);
     }
 }
 
@@ -785,8 +698,7 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
         tape_gemm_kernel<<<dim3(rb, jobs.n_gemm), TR_NT, TR_SMEM, st>>>(a.tape, rows, jobs, partials, a.grads_stride);
         tape_colsum_kernel<<<dim3(rb, jobs.n_col), rc::G3, 0, st>>>(a.tape, rows, jobs, partials, a.grads_stride);
         const int total = rc::rnn_offsets(d, n).total;
-        tape_partial_sum_kernel<<<(total + 255) / 256, 256, 0, st>>>(partials, rb, a.grads_stride, total,
-                                                                     a.grads + (size_t)net * a.grads_stride);
+        if ((e = orl::sum_row_blocks(partials, rb, a.grads_stride, total, a.grads + (size_t)net * a.grads_stride, st))) return e;
     }
     return orl::check_cuda(cudaGetLastError(), "rnn update launches");
 }

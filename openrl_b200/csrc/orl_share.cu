@@ -7,9 +7,9 @@
 // the update writes a per-row tape and the parameter gradients are deterministic tape reductions dW = sum_rows P^T Q.
 #include <algorithm>
 
+#include "orl_adam.cuh"
 #include "orl_deep_core.h"
 #include "orl_envstep.cuh"
-#include "orl_loss.cuh"
 
 namespace {
 using namespace orl;
@@ -82,16 +82,7 @@ __global__ void __launch_bounds__(S_NT) share_fwdbwd_kernel(const OrlPpoArgs a, 
     if (r < a.batch_rows) {
         const long long gi = a.indices ? a.indices[r] : a.row_begin + r;
         const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS, val_masks = a.flags & ORL_PPO_VALUE_ACTIVE_MASKS;
-        const double rows_d = (double)(a.norm_rows > 0 ? a.norm_rows : a.batch_rows);
-        const float inv_rows = (float)(1.0 / rows_d), inv_act = (float)(1.0 / a.mb_stats[2]);
-        const AdvNorm advn = make_adv_norm(a.gae_stats, a.flags & ORL_PPO_ADV_NORMALIZE);
-        float vn_mean = 0.f, vn_std = 1.f;
-        if (a.flags & ORL_PPO_VALUENORM) {
-            float st[3];
-            vn_updated(a.vn_state, a.mb_stats, rows_d, a.vn_beta, st);
-            const VnScalars s = vn_mean_std(st);
-            vn_mean = s.mean; vn_std = s.std;
-        }
+        const MbConsts mb = mb_consts(a);
         float x[dc::MAXD];
         load_obs_row(a.policy_obs, (size_t)gi, d, x);
         dc::Save sv;
@@ -102,36 +93,16 @@ __global__ void __launch_bounds__(S_NT) share_fwdbwd_kernel(const OrlPpoArgs a, 
         dc::deep_forward(a.policy_params, o, a.activation_id, x, &value, logit, &sv, tp);
         const float active = a.active_masks[gi];
         // policy loss (ppo.py:300-319) + entropy (act.py:160-168)
-        unsigned masked = 0;
-        if (a.action_masks) {
-#pragma unroll
-            for (int j = 0; j < MAX_OUT; ++j) if (j < n && a.action_masks[gi * n + j] == 0.f) { logit[j] = -6e4f; masked |= 1u << j; }
-        }
-        float nl[MAX_OUT], pr[MAX_OUT];
-        log_softmax_n(logit, n, nl, pr);
-        const int act = (int)a.actions[gi];
-        float lp = nl[0];
-#pragma unroll
-        for (int j = 1; j < MAX_OUT; ++j) if (j == act) lp = nl[j];
-        const float adv = apply_adv_norm(advn, a.advantages[gi]);
-        const PgTerm pg = pg_term(lp, a.old_log_probs[gi], adv, a.clip_param, a.flags, a.dual_clip_coeff);
-        const float wrow = pol_masks ? active * inv_act : inv_rows;
-        float ent = 0.f;
-#pragma unroll
-        for (int j = 0; j < MAX_OUT; ++j) if (j < n) ent -= pr[j] * nl[j];
-        l_pol = pg.loss * wrow; l_ent = ent * wrow; l_ratio = pg.ratio;
-        const float dlp = pg.dlogp * wrow, went = a.entropy_coef * wrow;
-        float dl[MAX_OUT];
-#pragma unroll
-        for (int j = 0; j < MAX_OUT; ++j) {
-            dl[j] = 0.f;
-            if (j < n && !((masked >> j) & 1u)) dl[j] = dlp * ((j == act ? 1.f : 0.f) - pr[j]) + went * pr[j] * (nl[j] + ent);
-        }
+        const float wrow = mb.weight(pol_masks, active);
+        float dl[MAX_OUT] = {};
+        const CatRow c = categorical_row(a, logit, n, a.action_masks ? a.action_masks + gi * n : nullptr, (int)a.actions[gi],
+                                         a.old_log_probs[gi], apply_adv_norm(mb.adv, a.advantages[gi]), wrow, dl);
+        l_pol = c.loss * wrow; l_ent = c.ent * wrow; l_ratio = c.ratio;
         // value loss (ppo.py:178-220)
         const float ret = a.returns[gi];
-        const float target = (a.flags & ORL_PPO_VALUENORM) ? (ret - vn_mean) / vn_std : ret;
+        const float target = (a.flags & ORL_PPO_VALUENORM) ? (ret - mb.vn_mean) / mb.vn_std : ret;
         const ValueTerm vt = value_term(value, a.value_preds[gi], target, a.clip_param, a.huber_delta, a.flags);
-        const float wv = val_masks ? active * inv_act : inv_rows;
+        const float wv = mb.weight(val_masks, active);
         l_val = vt.loss * wv;
         dc::deep_backward(a.policy_params, o, a.activation_id, sv, a.value_loss_coef * wv * vt.dv, dl, tp);
     }
@@ -195,14 +166,6 @@ __global__ void __launch_bounds__(256) share_tape_reduce_kernel(const float* __r
     }
 }
 
-__global__ void share_partial_sum_kernel(const float* __restrict__ partials, int row_blocks, int stride, int total, float* __restrict__ grads) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return;
-    float s = 0.f;
-    for (int rb = 0; rb < row_blocks; ++rb) s += partials[(size_t)rb * stride + i];   // fixed order: deterministic
-    grads[i] = s;
-}
-
 SJobs make_share_jobs(int d, int n) {
     const dc::Offsets o = dc::deep_offsets(d, n);
     SJobs t; int g = 0;
@@ -221,62 +184,15 @@ SJobs make_share_jobs(int d, int n) {
 // ---- optimiser: ppo.py:120-158 with a shared model — clip_grad_norm_(all) twice, one Adam step (lr = lrs[0]) ----
 __global__ void __launch_bounds__(1024) share_apply_kernel(const OrlPpoArgs a, const float* __restrict__ loss_acc) {
     const int total = dc::deep_offsets(a.obs_dim, a.n_actions).total;
-    float* params = a.policy_params;
-    float* am = a.policy_adam_m;
-    float* av = a.policy_adam_v;
-    const float* grads = a.grads;
-    __shared__ float red[32];
-    __shared__ float s_norm;
-    const int tid = threadIdx.x;
     float sq = 0.f;
-    for (int i = tid; i < total; i += blockDim.x) { const float g = grads[i]; sq = fmaf(g, g, sq); }
-    {
-        const float s = warp_sum(sq);
-        if ((tid & 31) == 0) red[tid >> 5] = s;
-        __syncthreads();
-        if (tid < 32) {
-            float v = (tid < (int)(blockDim.x >> 5)) ? red[tid] : 0.f;
-            v = warp_sum(v);
-            if (tid == 0) s_norm = sqrtf(v);
-        }
-        __syncthreads();
-    }
-    const float norm1 = s_norm;                       // actor_grad_norm: norm before the first clip
-    float c1 = 1.f, norm2 = norm1, c2 = 1.f;
-    if (a.flags & ORL_PPO_MAX_GRAD_NORM) {
-        c1 = fminf(a.max_grad_norm / (norm1 + 1e-6f), 1.0f);
-        norm2 = norm1 * c1;                           // critic_grad_norm: what the second clip_grad_norm_ measures
-        c2 = fminf(a.max_grad_norm / (norm2 + 1e-6f), 1.0f);
-    }
-    const float clip = c1 * c2;
-    const int step = a.adam_steps[0] + 1;
-    const double bc1 = 1.0 - pow((double)a.adam_beta1, (double)step);
-    const double bc2 = 1.0 - pow((double)a.adam_beta2, (double)step);
-    const float step_size = (float)((double)a.lrs[0] / bc1);
-    const float bc2_sqrt = (float)sqrt(bc2);
-    for (int i = tid; i < total; i += blockDim.x) {
-        float g = grads[i] * clip;
-        const float pv = params[i];
-        if (a.weight_decay != 0.f) g = fmaf(a.weight_decay, pv, g);
-        const float m = am[i] + (g - am[i]) * (1.f - a.adam_beta1);
-        const float v = fmaf(av[i], a.adam_beta2, (g * g) * (1.f - a.adam_beta2));
-        am[i] = m; av[i] = v;
-        params[i] = pv - step_size * (m / (sqrtf(v) / bc2_sqrt + a.adam_eps));
-    }
-    if (tid == 0) {
-        a.adam_steps[0] = step;
-        const double rows_d = (double)(a.norm_rows > 0 ? a.norm_rows : a.batch_rows);
-        a.train_info[0] += loss_acc[3];
-        a.train_info[1] += norm2;
-        a.train_info[2] += loss_acc[0];
-        a.train_info[3] += loss_acc[1];
-        a.train_info[4] += norm1;
-        a.train_info[5] += loss_acc[2] / (float)rows_d;
-        if (a.flags & ORL_PPO_VALUENORM) {
-            float st[3];
-            vn_updated(a.vn_state, a.mb_stats, rows_d, a.vn_beta, st);
-            a.vn_state[0] = st[0]; a.vn_state[1] = st[1]; a.vn_state[2] = st[2];
-        }
+    for (int i = threadIdx.x; i < total; i += blockDim.x) sq = fmaf(a.grads[i], a.grads[i], sq);
+    const float norm1 = block_l2_norm(sq);   // actor_grad_norm: norm before the first clip
+    const float c1 = clip_factor(a, norm1);
+    const float norm2 = norm1 * c1;          // critic_grad_norm: what the second clip_grad_norm_ measures
+    adam_step(a, 0, a.policy_params, a.policy_adam_m, a.policy_adam_v, a.grads, total, c1 * clip_factor(a, norm2));
+    if (threadIdx.x == 0) {
+        add_value_info(a, loss_acc[3], norm2);
+        add_policy_info(a, loss_acc, norm1);
     }
 }
 
@@ -351,9 +267,7 @@ int orl_share_fwdbwd(const OrlPpoArgs* ap, void* stream) {
     const SJobs jobs = make_share_jobs(a.obs_dim, a.n_actions);
     share_tape_reduce_kernel<<<dim3(rb, jobs.n), 256, 0, st>>>(tape, rows, jobs, partials, stride);
     ORL_LAUNCH_CHECK("share_tape_reduce_kernel");
-    share_partial_sum_kernel<<<(total + 255) / 256, 256, 0, st>>>(partials, rb, stride, total, a.grads);
-    ORL_LAUNCH_CHECK("share_partial_sum_kernel");
-    return 0;
+    return orl::sum_row_blocks(partials, rb, stride, total, a.grads, st);
 }
 
 int orl_share_apply(const OrlPpoArgs* ap, void* stream) {

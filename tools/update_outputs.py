@@ -1,0 +1,145 @@
+"""Save what K = 3 device iterations leave behind on every PPO update path, and compare two such saves.
+
+    python tools/update_outputs.py --out DIR            # needs a GPU; about a minute
+    python tools/update_outputs.py --compare DIR_A DIR_B
+
+`bench.py --dump-outputs` covers the C2 tensor-core update only.  This tool runs, from the seed, each update kernel
+family at a small shape: C2 on tensor cores, on FFMA, with the shared model and with dual clip / plain MSE value loss;
+C4 (GridWorld self-play, 5 actions); C3 GRU and C3 JRPO; C5 (Gaussian head, host-stepped synthetic env).  Per path it
+saves the policy and critic (or shared model) `flat_params`, their Adam moment buffers, `adam_steps`, the ValueNorm state and `train_info`
+as DIR/<path>/<name>.npy.  `--compare` prints the largest distance in units in the last place per array, so a refactor
+that must not change results can be checked bit for bit (distance 0) against its parent commit.
+"""
+import argparse
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+K = 3
+ENVS = 64
+PATHS = {
+    "c2_tc": ("c2", []),
+    "c2_ffma": ("c2", ["--use_tensor_cores", "false"]),
+    "c2_share": ("c2", ["--use_share_model", "true"]),
+    "c2_dualclip_mse": ("c2", ["--dual_clip_ppo", "true", "--use_huber_loss", "false", "--use_clipped_value_loss", "false"]),
+    "c4": ("c4", []),
+    "c3_gru": ("c3", []),
+    "c3_jrpo": ("c3", ["--use_joint_action_loss", "true"]),
+    "c5_gaussian_host": (None, []),
+}
+
+
+def state_arrays(trainer):
+    m = trainer.algo_module
+    out = {"adam_steps": m.adam_steps, "train_info": trainer.train_info}
+    for net in ("policy", "critic", "model"):   # "model": the shared policy-value network (use_share_model)
+        model, opt = m.models.get(net), m.optimizers.get(net)
+        if model is not None:
+            out[f"{net}_params"] = model.flat_params
+            vn = getattr(model, "value_normalizer", None)
+            if vn is not None:
+                out["valuenorm_state"] = vn.state
+        if opt is not None:
+            out[f"{net}_exp_avg"], out[f"{net}_exp_avg_sq"] = opt.exp_avg, opt.exp_avg_sq
+    return {k: v.detach().cpu().numpy() for k, v in out.items()}
+
+
+def run_device(workload, flags):
+    import bench
+
+    cfg, env, net, agent = bench.build_agent(0, 1, workload, ENVS, flags)
+    drv = bench.make_driver(cfg, env, net, agent, 0, 1)
+    for _ in range(K):
+        drv.device_iteration()
+    return state_arrays(drv.trainer)
+
+
+def run_host_gaussian():
+    import torch
+
+    import bench
+    from openrl_b200.configs.config import create_config_parser
+    from openrl_b200.envs.vec_env import HostVecEnv
+    from openrl_b200.modules.common import PPONet
+    from openrl_b200.runners.common import PPOAgent
+    from openrl_b200.utils.logger import Logger
+
+    cfg = create_config_parser().parse_args(list(bench.FLAGS))
+    cfg.quiet = True
+    env = HostVecEnv(bench.SyntheticHostEnv(ENVS, seed=0))
+    agent = PPOAgent(PPONet(env, cfg=cfg, device=f"cuda:{torch.cuda.current_device()}"))
+    agent.train(total_time_steps=ENVS * cfg.episode_length * K, logger=Logger(quiet=True))
+    return state_arrays(agent.driver.trainer)
+
+
+def save(out_dir):
+    import torch
+
+    assert torch.cuda.is_available(), "update_outputs.py --out needs a CUDA device"
+    for name, (workload, flags) in PATHS.items():
+        arrays = run_host_gaussian() if workload is None else run_device(workload, flags)
+        d = os.path.join(out_dir, name)
+        os.makedirs(d, exist_ok=True)
+        for k, a in arrays.items():
+            np.save(os.path.join(d, k + ".npy"), a)
+        print(f"{name}: {', '.join(sorted(arrays))}", flush=True)
+
+
+def ulp_distance(a, b):
+    """Largest distance in units in the last place between two float arrays of one dtype (integers: largest |a - b|);
+    two NaNs are at distance 0."""
+    if a.size == 0:
+        return 0
+    if a.dtype.kind != "f":
+        return int(np.max(np.abs(a.astype(np.int64) - b.astype(np.int64))))
+    it = {4: np.int32, 8: np.int64}[a.dtype.itemsize]
+
+    def ordered(x):   # IEEE bit patterns mapped onto a monotone integer line
+        i = x.view(it).astype(np.int64)
+        return np.where(i < 0, np.iinfo(it).min - i, i)
+
+    with np.errstate(over="ignore"):
+        d = np.abs(ordered(a) - ordered(b))
+    return int(np.max(np.where(np.isnan(a) & np.isnan(b), 0, d)))
+
+
+def compare(dir_a, dir_b):
+    worst = 0
+    for name in sorted(os.listdir(dir_a)):
+        pa, pb = os.path.join(dir_a, name), os.path.join(dir_b, name)
+        if not os.path.isdir(pa):
+            continue
+        for f in sorted(os.listdir(pa)):
+            if not os.path.exists(os.path.join(pb, f)):
+                print(f"{name}/{f[:-4]}: missing in {dir_b}")
+                worst = max(worst, 1)
+                continue
+            a, b = np.load(os.path.join(pa, f)), np.load(os.path.join(pb, f))
+            if a.shape != b.shape or a.dtype != b.dtype:
+                print(f"{name}/{f[:-4]}: shape/dtype {a.shape} {a.dtype} vs {b.shape} {b.dtype}")
+                worst = max(worst, 1)
+                continue
+            u = ulp_distance(a, b)
+            worst = max(worst, u)
+            print(f"{name}/{f[:-4]}: max ulp {u}" + ("" if u == 0 else f"  ({int(np.sum(a != b))} of {a.size} differ)"))
+    return worst
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    g = ap.add_mutually_exclusive_group(required=True)
+    g.add_argument("--out", metavar="DIR")
+    g.add_argument("--compare", nargs=2, metavar=("DIR_A", "DIR_B"))
+    args = ap.parse_args()
+    if args.out:
+        save(args.out)
+    else:
+        print("largest ulp distance:", compare(*args.compare))
+
+
+if __name__ == "__main__":
+    main()
