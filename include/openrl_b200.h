@@ -335,9 +335,9 @@ int orl_minibatch_stats(const int64_t* indices, int64_t batch_rows, const float*
  * (onpolicy_driver.py:80-152,236-279), ReplayData.recurrent_generator (replay_data.py:1062-1258:
  * chunks of L = data_chunk_length over the agent-major / time-minor flattening f = (n*A + a)*T + t,
  * initial hidden state rnn_states[f = c*L], chunks ignore trajectory boundaries) and the BPTT part of
- * PPOAlgorithm.ppo_update.  First, correctness-first implementation: one thread per row (rollout,
- * critic) or per chunk (update) running the sequential core of csrc/orl_rnn_core.h (verified on the
- * CPU against the oracle); parameter gradients are reductions of a per-row tape, dW = sum P^T Q.
+ * PPOAlgorithm.ppo_update.  One warp per env (rollout), row (act, critic) or chunk (update) runs the
+ * warp-cooperative step of csrc/orl_rnn_warp.cuh (checked against the sequential core csrc/orl_rnn_core.h,
+ * which is pinned to the oracle on the CPU); parameter gradients are reductions of a per-row tape, dW = sum P^T Q.
  * Parameter layout of a recurrent net (reference state_dict order):
  *   W1[64][d] b1 g1 be1 | W3[64][64] b3 g3 be3 | Wih[192][64] Whh[192][64] bih bhh | g_rnn be_rnn | Wh[n][64] bh[n]
  * With ORL_PPO_JOINT_ACTION (JRPO, ppo.py:254-319 + recurrent_generator_v3, replay_data.py:425-551): a chunk c covers the
@@ -387,7 +387,8 @@ int orl_rnn_param_count(int obs_dim, int n_out);
 int orl_rnn_tape_width(void);
 /* floats of OrlRnnArgs.tape for a minibatch of `rows` = n_chunks * chunk_length row-steps (times A with ORL_PPO_JOINT_ACTION) */
 long long orl_rnn_workspace_floats(long long rows, int grads_stride);
-/* policy GRU rollout for steps [t_begin, t_end) fused with the device env (simple_spread, CartPole, GridWorld) */
+/* policy GRU rollout for steps [t_begin, t_end) fused with the device env (simple_spread, CartPole, GridWorld); device
+ * envs only: ORL_ENV_NONE is rejected (the policy step of host-stepped rows is orl_rnn_act_rows) */
 int orl_rnn_rollout(const OrlRnnArgs* args, void* stream);
 /* policy GRU act for a HOST-stepped env: one step t = t_begin over buffer rows [row_begin, row_end) (B = n_envs *
  * n_agents rows per slot).  Reads policy_obs[t], rnn_states[t], masks[t]; writes actions[t], action_log_probs[t] and

@@ -1,5 +1,4 @@
-// Library-level C-ABI entry points: version, error string, device query; the rollouts' noise-counter bump and the
-// row-block sum of the tape-gradient reductions.
+// Library-level C-ABI entry points: version, error string, device query; the rollouts' noise-counter bump.
 #include <stdarg.h>
 #include <string.h>
 
@@ -39,20 +38,6 @@ int bump_rng_counter(uint64_t* counter, int steps, cudaStream_t st) {
     if (!counter) return 0;
     bump_rng_counter_kernel<<<1, 1, 0, st>>>(counter, (uint64_t)steps);
     return check_cuda(cudaGetLastError(), "bump_rng_counter_kernel");
-}
-
-__global__ void row_block_sum_kernel(const float* __restrict__ partials, int row_blocks, int stride, int total,
-                                     float* __restrict__ out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return;
-    float s = 0.f;
-    for (int rb = 0; rb < row_blocks; ++rb) s += partials[(size_t)rb * stride + i];   // fixed order: deterministic
-    out[i] = s;
-}
-
-int sum_row_blocks(const float* partials, int row_blocks, int stride, int total, float* out, cudaStream_t st) {
-    row_block_sum_kernel<<<(total + 255) / 256, 256, 0, st>>>(partials, row_blocks, stride, total, out);
-    return check_cuda(cudaGetLastError(), "row_block_sum_kernel");
 }
 }  // namespace orl
 

@@ -14,9 +14,20 @@ int sm_count();
 // advances the device Philox step counter of the action noise by the `steps` steps a rollout launch consumed; no-op
 // when `counter` is null
 int bump_rng_counter(uint64_t* counter, int steps, cudaStream_t st);
-// out[i] = sum over rb < row_blocks of partials[rb * stride + i] for i < total, in row-block order (deterministic): the
-// second stage of the tape-gradient reductions of the recurrent and shared-model updates
-int sum_row_blocks(const float* partials, int row_blocks, int stride, int total, float* out, cudaStream_t st);
+
+// ---- tape-gradient reductions of the recurrent and shared-model updates (orl_tape.cu) ----
+// A job reads columns of the `tape_width`-float tape rows: a gemm job writes sum_rows tape[p_off + m] * tape[q_off + k]
+// (m < M, k < N) to grads[out_off + m*N + k], a column job sum_rows tape[p_off + m] (m < M) to grads[out_off + m].
+struct TapeJob { int p_off, M, q_off, N, out_off; };
+constexpr int TAPE_MAX_GEMM_JOBS = 6, TAPE_MAX_COL_JOBS = 14;   // the shared model's tables (the GRU's: 5 and 11)
+struct TapeJobs { TapeJob gemm[TAPE_MAX_GEMM_JOBS]; TapeJob col[TAPE_MAX_COL_JOBS]; int n_gemm, n_col; };
+constexpr int TAPE_ROW_BLOCK = 1024;   // tape rows per partial result: partials hold ceil(rows / TAPE_ROW_BLOCK) x stride floats
+// grads[0, total) = the jobs over tape rows [0, rows), summed per row block into partials and then over the row blocks
+// in a fixed order (deterministic).  ORL_ERR_BAD_ARG when a gemm job's tiles are not 16-byte aligned (tape_width, p_off,
+// q_off multiples of 4) or leave the tape row (q_off + 64, p_off + 16*ceil(M/16)), or M > 192, N > 64, or tape_width
+// is neither the GRU's nor the shared model's.
+int reduce_tape(const float* tape, int tape_width, long long rows, const TapeJobs& jobs, float* partials, int stride, int total,
+                float* grads, cudaStream_t st);
 
 #define ORL_CHECK_ARG(cond, msg)                                   \
     do {                                                           \

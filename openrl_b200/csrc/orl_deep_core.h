@@ -9,28 +9,35 @@
 // Flat parameter layout (named_parameters order of the reference; `critic_obs_prep` aliases `obs_prep`):
 //   W1[64][d] b1 g1 be1 | W3[64][64] b3 g3 be3 | W5[64][64] b5 g5 be5 | W7[64][64] b7 g7 be7 | Wv[1][64] bv | Wa[n][64] ba
 // The backward writes a per-row "tape" of local gradients and forward activations; the parameter gradients are tape
-// reductions dW = sum_rows P^T Q / column sums, done by the generic tape kernels of orl_rnn.cu.
+// reductions dW = sum_rows P^T Q / column sums, done by orl::reduce_tape (orl_tape.cu).
+// The widths, activations and LayerNorm are those of the recurrent core (orl_rnn_core.h).
 #pragma once
-#include <math.h>
+#include "orl_rnn_core.h"
 
 #ifdef __CUDACC__
-#define ORLD_HD __host__ __device__ __forceinline__
-#define ORLD_STEP __host__ __device__ __noinline__   // real calls: see the note in orl_rnn_core.h
+// Real calls on the device (own stack frames): with a whole sequential step inlined into its kernel, nvcc 12.9 once
+// merged the stack slots of the caller's observation row and the callee's outputs (observed in SASS as a corrupted
+// tape of the recurrent core), i.e. wrong gradients.  `inline`: one definition however many files include this header.
+#define ORLD_STEP inline __host__ __device__ __noinline__
 #else
-#define ORLD_HD static inline
 #define ORLD_STEP static inline
 #endif
 
 namespace orl_deep {
 
-constexpr int H = 64, MAXN = 8, MAXD = 64;
-constexpr float LN_EPS = 1e-5f;
+using orl_rnn::H;
+using orl_rnn::MAXN;
+using orl_rnn::MAXD;
+using orl_rnn::act_fwd;
+using orl_rnn::act_bwd_from_out;
+using orl_rnn::layernorm64;
+using orl_rnn::layernorm64_bwd;
 
 struct Offsets {
     int d, n;
     int w1, b1, g1, be1, w3, b3, g3, be3, w5, b5, g5, be5, w7, b7, g7, be7, wv, bv, wa, ba, total;
 };
-ORLD_HD Offsets deep_offsets(int d, int n) {
+ORL_HD Offsets deep_offsets(int d, int n) {
     Offsets o; o.d = d; o.n = n; int p = 0;
     o.w1 = p; p += H * d; o.b1 = p; p += H; o.g1 = p; p += H; o.be1 = p; p += H;
     o.w3 = p; p += H * H; o.b3 = p; p += H; o.g3 = p; p += H; o.be3 = p; p += H;
@@ -48,30 +55,8 @@ constexpr int TQ_X = 272, TQ_Y1 = 336, TQ_Y3 = 400, TQ_Y5 = 464, TQ_Y7 = 528;
 constexpr int TS_DY1N1 = 592, TS_DY1 = 656, TS_DY3N3 = 720, TS_DY3 = 784, TS_DY5N5 = 848, TS_DY5 = 912, TS_DY7N7 = 976, TS_DY7 = 1040;
 constexpr int TAPE = 1104;
 
-ORLD_HD float act_fwd(float z, int id) {
-    switch (id) { case 0: return tanhf(z); case 1: return z > 0.f ? z : 0.f; case 2: return z > 0.f ? z : 0.01f * z; default: return z > 0.f ? z : expm1f(z); }
-}
-ORLD_HD float act_bwd_from_out(float a, int id) {
-    switch (id) { case 0: return 1.f - a * a; case 1: return a > 0.f ? 1.f : 0.f; case 2: return a > 0.f ? 1.f : 0.01f; default: return a > 0.f ? 1.f : a + 1.f; }
-}
-ORLD_HD float layernorm64(const float* v, float* n_out) {
-    float s = 0.f;
-    for (int i = 0; i < H; ++i) s += v[i];
-    const float m = s * (1.f / H);
-    float q = 0.f;
-    for (int i = 0; i < H; ++i) { const float dlt = v[i] - m; n_out[i] = dlt; q += dlt * dlt; }
-    const float r = 1.f / sqrtf(q * (1.f / H) + LN_EPS);
-    for (int i = 0; i < H; ++i) n_out[i] *= r;
-    return r;
-}
-ORLD_HD void layernorm64_bwd(const float* dn, const float* n, float rstd, float* dv) {
-    float s1 = 0.f, s2 = 0.f;
-    for (int i = 0; i < H; ++i) { s1 += dn[i]; s2 += dn[i] * n[i]; }
-    s1 *= (1.f / H); s2 *= (1.f / H);
-    for (int i = 0; i < H; ++i) dv[i] = rstd * (dn[i] - s1 - n[i] * s2);
-}
 // y[j] = b[j] + sum_k W[j][k] x[k]   (64 x K, row-major)
-ORLD_HD void linear64(const float* W, const float* b, const float* x, int K, float* y) {
+ORL_HD void linear64(const float* W, const float* b, const float* x, int K, float* y) {
     for (int j = 0; j < H; ++j) {
         float s = b[j];
         for (int k = 0; k < K; ++k) s = fmaf(W[j * K + k], x[k], s);
@@ -79,7 +64,7 @@ ORLD_HD void linear64(const float* W, const float* b, const float* x, int K, flo
     }
 }
 // dx[k] = sum_j W[j][k] dz[j]
-ORLD_HD void linear64_bwd_data(const float* W, const float* dz, float* dx) {
+ORL_HD void linear64_bwd_data(const float* W, const float* dz, float* dx) {
     for (int k = 0; k < H; ++k) dx[k] = 0.f;
     for (int j = 0; j < H; ++j) {
         const float g = dz[j];

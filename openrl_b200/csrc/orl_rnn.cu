@@ -13,9 +13,9 @@
 // the warp-cooperative step of orl_rnn_warp.cuh — 64-vectors as two registers per lane, the net's weights staged
 // once per persistent CTA in 136 KB of shared memory, mat-vecs by shuffle broadcast (shared-memory-bandwidth
 // bound: one LDS per FMA).  The update writes a per-row-step tape (forward activations, local gradients);
-// parameter gradients are reductions of the tape, dW = sum_rows P^T Q, by a staged-GEMM kernel with float atomics
-// into the true-layout gradient buffer.  The sequential restatement of the same step (orl_rnn_core.h, pinned to
-// the torch oracle on the CPU) serves PPOModule.act and is the element-wise checker of the warp path
+// parameter gradients are reductions of the tape, dW = sum_rows P^T Q, by the deterministic two-stage reduction of
+// orl_tape.cu.  The sequential restatement of the same step (orl_rnn_core.h, pinned to the torch oracle on the CPU)
+// is compiled for the host only: the g++ reference of the CPU tests and the element-wise checker of the warp path
 // (tests/debug_gru.py).
 #include <algorithm>
 
@@ -31,32 +31,7 @@ namespace rw = orl_rnnw;
 
 static_assert(rc::MAXN == MAX_OUT, "head width limits must agree");
 constexpr int LMAX = 32;     // data_chunk_length limit accepted by the host API (the chunk kernels loop over l; the tape is n_chunks * L rows)
-constexpr int RNN_NT = 64;   // threads per CTA of the sequential kernels
 constexpr int JOINT_A = 3;   // agents of the joint-action update (simple_spread, the multi-agent device env)
-
-// ---- act only (PPOModule.act / PPONet.act): one thread per row runs the sequential core; the caller owns env.step ----
-__global__ void __launch_bounds__(RNN_NT) rnn_act_kernel(const OrlRnnArgs a) {
-    const int B = a.n_envs, n = a.n_actions, d = a.obs_dim;
-    const int row = blockIdx.x * blockDim.x + threadIdx.x;
-    if (row >= B) return;
-    const rc::Offsets o = rc::rnn_offsets(d, n);
-    const uint64_t rng_base = a.rng_step_base + (a.rng_counter ? *a.rng_counter : 0ull);
-    for (int t = a.t_begin; t < a.t_end; ++t) {
-        const size_t grow = (size_t)t * B + row;
-        float x[rc::MAXD], h[rc::H], hn[rc::H], logit[MAX_OUT];
-        for (int k = 0; k < rc::MAXD; ++k) x[k] = k < d ? a.policy_obs[grow * d + k] : 0.f;
-        for (int j = 0; j < rc::H; ++j) h[j] = a.rnn_states[grow * rc::H + j];
-        rc::rnn_step_forward(a.policy_params, o, a.activation_id, x, h, a.masks[grow], hn, logit, nullptr, nullptr);
-        for (int j = 0; j < rc::H; ++j) a.rnn_states[((size_t)(t + 1) * B + row) * rc::H + j] = hn[j];
-        // keyed by the local row (rng_row_offset is read by orl_rnn_act_rows only)
-        float lp;
-        const int act = sample_action(logit, n, nullptr, a.deterministic != 0, [&](float (&q)[MAX_OUT]) {
-            action_noise(a.exp_noise, grow, n, a.rng_seed, rng_base + (uint64_t)t, (uint32_t)row, q);
-        }, lp);
-        a.actions[grow] = (float)act;
-        a.action_log_probs[grow] = lp;
-    }
-}
 
 constexpr int W_NT = 512, W_WPC = W_NT / 32;   // one persistent CTA per SM, 16 warps, weights of one net in smem
 
@@ -408,102 +383,7 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_joint_policy_warp_kernel(const Or
     }
 }
 
-// ---- tape reductions (deterministic, two stages) ----
-// Stage 1: every CTA owns TR_ROWS tape rows and one job and writes its partial result to partials[row_block][...]:
-//   gemm job   part[out_off + m*N + k] = sum_rows tape[r][p_off+m] * tape[r][q_off+k]     (register-tiled, 12x4 per thread)
-//   column job part[out_off + m]       = sum_rows tape[r][p_off+m]
-// Stage 2: grads[i] = sum over row blocks of partials[rb][i], fixed order.
-struct TapeJob { int p_off, M, q_off, N, out_off; };
-constexpr int MAX_GEMM_JOBS = 5, MAX_COL_JOBS = 11;
-struct TapeJobs { TapeJob gemm[MAX_GEMM_JOBS]; TapeJob col[MAX_COL_JOBS]; int n_gemm, n_col; };
-constexpr int TR_NT = 256, TR_ROWS = 1024, TR_SUB = 32, TR_MI = rc::G3 / 16;   // 16 x 16 threads; thread tile (M/16) x 4
-
-__device__ __forceinline__ void cp_async16(float* smem_dst, const float* gmem_src, bool valid) {
-    const unsigned dst = (unsigned)__cvta_generic_to_shared(smem_dst);
-    const int src_size = valid ? 16 : 0;   // 0: the 16 bytes are zero-filled
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(gmem_src), "r"(src_size));
-}
-constexpr size_t TR_SMEM = 2 * (size_t)TR_SUB * (rc::G3 + rc::H) * sizeof(float);   // two stages of P and Q tiles
-
-__global__ void __launch_bounds__(TR_NT) tape_gemm_kernel(const float* __restrict__ tape, long long rows, TapeJobs jobs,
-                                                          float* __restrict__ partials, int stride) {
-    extern __shared__ __align__(16) float tsm[];
-    const TapeJob jb = jobs.gemm[blockIdx.y];
-    const long long r_begin = (long long)blockIdx.x * TR_ROWS;
-    const int rows_here = (int)min((long long)TR_ROWS, rows - r_begin);
-    auto Ps = [&](int buf) { return tsm + buf * (TR_SUB * rc::G3); };
-    auto Qs = [&](int buf) { return tsm + 2 * TR_SUB * rc::G3 + buf * (TR_SUB * rc::H); };
-    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const int MI = (jb.M + 15) >> 4, Mq = MI * 4;   // P columns are read in whole float4 up to 16*MI (fields are zero / foreign beyond M: discarded)
-    // stage loader: rows beyond the block's tail are zero-filled
-    auto load_stage = [&](int buf, int s0) {
-        const int sub = min(TR_SUB, rows_here - s0);
-        const float* base = tape + (size_t)(r_begin + s0) * rw::TAPE_W;
-        for (int i = tid; i < TR_SUB * Mq; i += TR_NT) {
-            const int r = i / Mq, c = i % Mq;
-            cp_async16(Ps(buf) + r * rc::G3 + 4 * c, base + (size_t)(r < sub ? r : 0) * rw::TAPE_W + jb.p_off + 4 * c, r < sub);
-        }
-        for (int i = tid; i < TR_SUB * (rc::H / 4); i += TR_NT) {
-            const int r = i >> 4, c = i & 15;
-            cp_async16(Qs(buf) + r * rc::H + 4 * c, base + (size_t)(r < sub ? r : 0) * rw::TAPE_W + jb.q_off + 4 * c, r < sub);
-        }
-        asm volatile("cp.async.commit_group;\n" ::);
-    };
-    float acc[TR_MI][4];
-#pragma unroll
-    for (int i = 0; i < TR_MI; ++i) { acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f; }
-    const int n_sub = (rows_here + TR_SUB - 1) / TR_SUB;
-    load_stage(0, 0);
-    for (int s = 0; s < n_sub; ++s) {
-        const int buf = s & 1;
-        if (s + 1 < n_sub) { load_stage(buf ^ 1, (s + 1) * TR_SUB); asm volatile("cp.async.wait_group 1;\n" ::); }
-        else asm volatile("cp.async.wait_group 0;\n" ::);
-        __syncthreads();
-        const float* P = Ps(buf);
-        const float* Q = Qs(buf);
-#pragma unroll 4
-        for (int r = 0; r < TR_SUB; ++r) {
-            const float4 q = *reinterpret_cast<const float4*>(Q + r * rc::H + 4 * tx);
-#pragma unroll
-            for (int i = 0; i < TR_MI; ++i) {
-                if (i < MI) {
-                    const float p = P[r * rc::G3 + ty + 16 * i];
-                    acc[i][0] = fmaf(p, q.x, acc[i][0]); acc[i][1] = fmaf(p, q.y, acc[i][1]);
-                    acc[i][2] = fmaf(p, q.z, acc[i][2]); acc[i][3] = fmaf(p, q.w, acc[i][3]);
-                }
-            }
-        }
-        __syncthreads();   // the stage just read is refilled by the next iteration's load
-    }
-    float* part = partials + (size_t)blockIdx.x * stride + jb.out_off;
-#pragma unroll
-    for (int i = 0; i < TR_MI; ++i) {
-        const int m = ty + 16 * i;
-        if (i < MI && m < jb.M) {
-#pragma unroll
-            for (int c = 0; c < 4; ++c) { const int k = 4 * tx + c; if (k < jb.N) part[m * jb.N + k] = acc[i][c]; }
-        }
-    }
-}
-
-__global__ void __launch_bounds__(rc::G3) tape_colsum_kernel(const float* __restrict__ tape, long long rows, TapeJobs jobs,
-                                                             float* __restrict__ partials, int stride) {
-    const TapeJob jb = jobs.col[blockIdx.y];
-    const long long r_begin = (long long)blockIdx.x * TR_ROWS;
-    const int rows_here = (int)min((long long)TR_ROWS, rows - r_begin);
-    const int m = threadIdx.x;
-    if (m >= jb.M) return;
-    const float* p = tape + (size_t)r_begin * rw::TAPE_W + jb.p_off + m;
-    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-    int r = 0;
-    for (; r + 4 <= rows_here; r += 4) {
-        s0 += p[(size_t)r * rw::TAPE_W]; s1 += p[(size_t)(r + 1) * rw::TAPE_W];
-        s2 += p[(size_t)(r + 2) * rw::TAPE_W]; s3 += p[(size_t)(r + 3) * rw::TAPE_W];
-    }
-    for (; r < rows_here; ++r) s0 += p[(size_t)r * rw::TAPE_W];
-    partials[(size_t)blockIdx.x * stride + jb.out_off + m] = (s0 + s1) + (s2 + s3);
-}
-
+// ---- parameter gradients of one net from its tape (orl::reduce_tape); every job fits the gemm tiles: TQ_X + 64 <= TAPE_W ----
 TapeJobs make_jobs(int d, int n) {
     const rc::Offsets o = rc::rnn_offsets(d, n);
     TapeJobs t; int g = 0, c = 0;
@@ -523,7 +403,6 @@ TapeJobs make_jobs(int d, int n) {
 
 // workspace = tape (rows x TAPE_W) followed by the reduction partials (row blocks x grads_stride)
 long long ws_tape_floats(long long rows) { return rows * rw::TAPE_W; }
-int ws_row_blocks(long long rows) { return (int)((rows + TR_ROWS - 1) / TR_ROWS); }
 
 // ---- optimizer: per-net global-norm clip + Adam on the true-layout gradients (one CTA per net) ----
 __global__ void __launch_bounds__(1024) rnn_apply_kernel(const OrlRnnArgs a) {
@@ -568,23 +447,16 @@ extern "C" {
 int orl_rnn_param_count(int obs_dim, int n_out) { return rc::rnn_offsets(obs_dim, n_out).total; }
 int orl_rnn_tape_width(void) { return rw::TAPE_W; }
 long long orl_rnn_workspace_floats(long long rows, int grads_stride) {
-    return ws_tape_floats(rows) + (long long)ws_row_blocks(rows) * grads_stride;
+    return ws_tape_floats(rows) + (rows + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK * grads_stride;
 }
 
 int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
     ORL_CHECK_ARG(ap, "args");
     const OrlRnnArgs& a = *ap;
     if (int e = check_common(a)) return e;
+    ORL_CHECK_ARG(a.env_kind != ORL_ENV_NONE, "ORL_ENV_NONE: the act of host-stepped rows is orl_rnn_act_rows");
     ORL_CHECK_ARG(a.policy_params && a.policy_obs && a.rnn_states && a.actions && a.action_log_probs && a.masks, "null rollout buffer");
     ORL_CHECK_ARG(a.t_begin >= 0 && a.t_end <= a.episode_length && a.t_begin <= a.t_end, "t range");
-    cudaStream_t st = (cudaStream_t)stream;
-    const int grid = (a.n_envs + RNN_NT - 1) / RNN_NT;
-    if (a.env_kind == ORL_ENV_NONE) {   // policy step(s) only: rows = n_envs, slot t -> actions[t], rnn_states[t+1]
-        ORL_CHECK_ARG(a.n_agents == 1, "ENV_NONE rows are passed as n_envs with n_agents == 1");
-        if (a.t_end > a.t_begin) rnn_act_kernel<<<grid, RNN_NT, 0, st>>>(a);
-        if (int e = orl::check_cuda(cudaGetLastError(), "rnn_act_kernel launch")) return e;
-        return orl::bump_rng_counter(a.rng_counter, a.t_end - a.t_begin, st);
-    }
     ORL_CHECK_ARG(a.critic_obs && a.rewards && a.active_masks, "null rollout buffer");
     ORL_CHECK_ARG(a.env_kind == ORL_ENV_MPE_SPREAD || a.env_kind == ORL_ENV_CARTPOLE || a.env_kind == ORL_ENV_GRIDWORLD,
                   "unknown env kind");
@@ -595,6 +467,7 @@ int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
     } else {
         ORL_CHECK_ARG(a.n_agents == 1 && a.obs_dim == 4, "single-agent env shapes");
     }
+    cudaStream_t st = (cudaStream_t)stream;
     if (a.t_end > a.t_begin) {
         const int wg = warp_grid(a.n_envs);
         int e = 0;
@@ -676,8 +549,6 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
     float* partials = a.tape + ws_tape_floats(net_rows[0]);   // the policy's tape is the larger one
     // two chunks per warp: every weight read from shared memory feeds two rows
     constexpr int C_R = 2;
-    if ((e = orl::check_cuda(cudaFuncSetAttribute(tape_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TR_SMEM),
-                             "smem attr (tape gemm)"))) return e;
     const int cgrid = warp_grid((a.n_chunks + C_R - 1) / C_R);
     if (joint) {
         if ((e = warp_kernel_prepare(rnn_joint_policy_warp_kernel<JOINT_A, W_NT>, w_smem(JOINT_A), "smem attr (rnn joint policy)"))) return e;
@@ -692,13 +563,8 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
         else if (net == 0) rnn_chunk_warp_kernel<true, false, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
         else if (joint) rnn_chunk_warp_kernel<false, true, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
         else rnn_chunk_warp_kernel<false, false, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
-        const long long rows = net_rows[net];
-        const int rb = ws_row_blocks(rows);
-        const TapeJobs jobs = make_jobs(d, n);
-        tape_gemm_kernel<<<dim3(rb, jobs.n_gemm), TR_NT, TR_SMEM, st>>>(a.tape, rows, jobs, partials, a.grads_stride);
-        tape_colsum_kernel<<<dim3(rb, jobs.n_col), rc::G3, 0, st>>>(a.tape, rows, jobs, partials, a.grads_stride);
-        const int total = rc::rnn_offsets(d, n).total;
-        if ((e = orl::sum_row_blocks(partials, rb, a.grads_stride, total, a.grads + (size_t)net * a.grads_stride, st))) return e;
+        if ((e = orl::reduce_tape(a.tape, rw::TAPE_W, net_rows[net], make_jobs(d, n), partials, a.grads_stride,
+                                  rc::rnn_offsets(d, n).total, a.grads + (size_t)net * a.grads_stride, st))) return e;
     }
     return orl::check_cuda(cudaGetLastError(), "rnn update launches");
 }

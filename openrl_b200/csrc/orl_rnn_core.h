@@ -1,7 +1,9 @@
 // Sequential (one row at a time) restatement of the recurrent policy / value network of the PPO hot
-// path, compiled BOTH by nvcc (device functions used by orl_rnn.cu, one thread per row / chunk) and by
-// g++ (tests/test_rnn_core_cpu.py drives it through a tiny C shim and checks it against the torch
-// oracle) — so the numerics of the GRU path are verified without a GPU.
+// path.  The step functions are host code: g++ compiles them for the CPU tests (tests/test_rnn_core_cpu.py
+// drives them through a tiny C shim and checks them against the torch oracle) and they are the element-wise
+// reference of the warp-cooperative step of orl_rnn_warp.cuh — so the numerics of the GRU path are verified
+// without a GPU.  The parameter offsets, the tape layout and the helpers are __host__ __device__: the warp path
+// and the shared-model core (orl_deep_core.h) use them.
 //
 // Network (reference: MLPBase mlp.py:100-176 -> RNNLayer rnn.py:5-99 (nn.GRU 64->64, 1 layer, then
 // LayerNorm) -> head: Categorical.linear act.py / v_out value_network.py:106-109):
@@ -15,13 +17,8 @@
 
 #ifdef __CUDACC__
 #define ORL_HD __host__ __device__ __forceinline__
-// The two step functions are real calls on the device (own stack frames): with everything inlined into the
-// per-chunk kernel nvcc 12.9 merged the stack slots of the caller's observation row and the callee's GRU
-// output (observed in SASS and as a corrupted tape), i.e. wrong gradients.
-#define ORL_HD_STEP __host__ __device__ __noinline__
 #else
 #define ORL_HD static inline
-#define ORL_HD_STEP static inline
 #endif
 
 namespace orl_rnn {
@@ -85,7 +82,7 @@ struct StepSave {
 
 // One forward step of a recurrent net.  x[d], h_in[64], mask -> h_out[64], head out[n].
 // `sv` may be NULL (rollout).  Also returns y1 / o through the tape pointer when given.
-ORL_HD_STEP void rnn_step_forward(const float* P, const Offsets& o, int act_id, const float* x, const float* h_in, float mask,
+static inline void rnn_step_forward(const float* P, const Offsets& o, int act_id, const float* x, const float* h_in, float mask,
                              float* h_out, float* out, StepSave* sv, float* tape) {
     float a1[H], n1[H], y1[H], z3[H], n3[H], y3[H];
     if (tape) for (int k = 0; k < MAXD; ++k) tape[TQ_X + k] = k < o.d ? x[k] : 0.f;
@@ -147,7 +144,7 @@ ORL_HD_STEP void rnn_step_forward(const float* P, const Offsets& o, int act_id, 
 // Backward of one row-step.  dlogit[n]: dL/d head output; dh_from_next[64]: dL/d h_out arriving from the
 // following step of the chunk (zero for the last step).  Writes the P / S parts of the tape and returns
 // dL/d h_in (already multiplied by the mask) in dh_prev.
-ORL_HD_STEP void rnn_step_backward(const float* P, const Offsets& o, int act_id, const StepSave& sv, float mask, const float* dlogit,
+static inline void rnn_step_backward(const float* P, const Offsets& o, int act_id, const StepSave& sv, float mask, const float* dlogit,
                               const float* dh_from_next, float* dh_prev, float* tape) {
     float dov[H], dno[H], dh[H];
     for (int k = 0; k < H; ++k) {

@@ -120,64 +120,20 @@ __global__ void __launch_bounds__(S_NT) share_fwdbwd_kernel(const OrlPpoArgs a, 
     }
 }
 
-// ---- tape reductions: out[m*N + k] = sum_rows tape[r][p_off + m] * tape[r][q_off + k]  (q_off < 0: column sum, N = 1) ----
-struct SJob { int p_off, M, q_off, N, out_off; };
-constexpr int S_MAX_JOBS = 24, SR_ROWS = 512, SR_SUB = 32;
-struct SJobs { SJob job[S_MAX_JOBS]; int n; };
-
-__global__ void __launch_bounds__(256) share_tape_reduce_kernel(const float* __restrict__ tape, long long rows, SJobs jobs,
-                                                                float* __restrict__ partials, int stride) {
-    __shared__ float Ps[SR_SUB][64 + 1], Qs[SR_SUB][64 + 1];
-    const SJob jb = jobs.job[blockIdx.y];
-    const long long r_begin = (long long)blockIdx.x * SR_ROWS;
-    const int rows_here = (int)min((long long)SR_ROWS, rows - r_begin);
-    const int tid = threadIdx.x, tk = tid & 15, tm = tid >> 4;   // outputs m = tm + 16 i (i < 4), k = 4 tk + c (c < 4)
-    float acc[4][4] = {};
-    for (int s0 = 0; s0 < rows_here; s0 += SR_SUB) {
-        const int sub = min(SR_SUB, rows_here - s0);
-        for (int i = tid; i < SR_SUB * 64; i += 256) {
-            const int r = i >> 6, c = i & 63;
-            const float* row = tape + (size_t)(r_begin + s0 + (r < sub ? r : 0)) * dc::TAPE;
-            Ps[r][c] = (r < sub && c < jb.M) ? row[jb.p_off + c] : 0.f;
-            Qs[r][c] = (r < sub && c < jb.N) ? (jb.q_off >= 0 ? row[jb.q_off + c] : 1.f) : 0.f;
-        }
-        __syncthreads();
-        for (int r = 0; r < SR_SUB; ++r) {
-            float q[4], p[4];
-#pragma unroll
-            for (int c = 0; c < 4; ++c) q[c] = Qs[r][4 * tk + c];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) p[i] = Ps[r][tm + 16 * i];
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int c = 0; c < 4; ++c) acc[i][c] = fmaf(p[i], q[c], acc[i][c]);
-        }
-        __syncthreads();
-    }
-    float* part = partials + (size_t)blockIdx.x * stride + jb.out_off;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int m = tm + 16 * i;
-        if (m < jb.M) {
-#pragma unroll
-            for (int c = 0; c < 4; ++c) { const int k = 4 * tk + c; if (k < jb.N) part[m * jb.N + k] = acc[i][c]; }
-        }
-    }
-}
-
-SJobs make_share_jobs(int d, int n) {
+// ---- parameter gradients from the tape (orl::reduce_tape).  Every gemm job fits its tiles: the Q tiles end by TQ_Y7 + 64
+// <= TAPE, the P tile of the M = 1 value head is TP_DV + 16 <= TAPE ----
+TapeJobs make_share_jobs(int d, int n) {
     const dc::Offsets o = dc::deep_offsets(d, n);
-    SJobs t; int g = 0;
-    auto gemm = [&](int p, int M, int q, int N, int out) { t.job[g++] = SJob{p, M, q, N, out}; };
-    auto col = [&](int p, int M, int out) { t.job[g++] = SJob{p, M, -1, 1, out}; };
+    TapeJobs t; int g = 0, c = 0;
+    auto gemm = [&](int p, int M, int q, int N, int out) { t.gemm[g++] = TapeJob{p, M, q, N, out}; };
+    auto col = [&](int p, int M, int out) { t.col[c++] = TapeJob{p, M, -1, 1, out}; };
     gemm(dc::TP_DZ1, dc::H, dc::TQ_X, d, o.w1);       col(dc::TP_DZ1, dc::H, o.b1);  col(dc::TS_DY1N1, dc::H, o.g1); col(dc::TS_DY1, dc::H, o.be1);
     gemm(dc::TP_DZ3, dc::H, dc::TQ_Y1, dc::H, o.w3);  col(dc::TP_DZ3, dc::H, o.b3);  col(dc::TS_DY3N3, dc::H, o.g3); col(dc::TS_DY3, dc::H, o.be3);
     gemm(dc::TP_DZ5, dc::H, dc::TQ_Y3, dc::H, o.w5);  col(dc::TP_DZ5, dc::H, o.b5);  col(dc::TS_DY5N5, dc::H, o.g5); col(dc::TS_DY5, dc::H, o.be5);
     gemm(dc::TP_DZ7, dc::H, dc::TQ_Y5, dc::H, o.w7);  col(dc::TP_DZ7, dc::H, o.b7);  col(dc::TS_DY7N7, dc::H, o.g7); col(dc::TS_DY7, dc::H, o.be7);
     gemm(dc::TP_DV, 1, dc::TQ_Y7, dc::H, o.wv);       col(dc::TP_DV, 1, o.bv);
     gemm(dc::TP_DLOG, n, dc::TQ_Y7, dc::H, o.wa);     col(dc::TP_DLOG, n, o.ba);
-    t.n = g;
+    t.n_gemm = g; t.n_col = c;
     return t;
 }
 
@@ -204,7 +160,7 @@ int orl_share_param_count(int obs_dim, int n_actions) { return dc::deep_offsets(
 int orl_share_tape_width(void) { return dc::TAPE; }
 /* floats of the update workspace for a minibatch of `rows` rows: tape rows, then reduction partials */
 long long orl_share_workspace_floats(long long rows, int obs_dim, int n_actions) {
-    const long long rb = (rows + SR_ROWS - 1) / SR_ROWS;
+    const long long rb = (rows + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK;
     return rows * dc::TAPE + rb * (long long)((dc::deep_offsets(obs_dim, n_actions).total + 3) & ~3);
 }
 
@@ -257,17 +213,13 @@ int orl_share_fwdbwd(const OrlPpoArgs* ap, void* stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     float* tape = a.partials;
     const long long rows = a.batch_rows;
-    const int rb = (int)((rows + SR_ROWS - 1) / SR_ROWS);
     const int total = dc::deep_offsets(a.obs_dim, a.n_actions).total, stride = (total + 3) & ~3;
     float* partials = tape + (size_t)rows * dc::TAPE;
     int e = orl::check_cuda(cudaMemsetAsync(a.folded, 0, 8 * sizeof(float), st), "memset loss sums");
     if (e) return e;
     share_fwdbwd_kernel<<<(unsigned)((rows + S_NT - 1) / S_NT), S_NT, 0, st>>>(a, tape, a.folded);
     ORL_LAUNCH_CHECK("share_fwdbwd_kernel");
-    const SJobs jobs = make_share_jobs(a.obs_dim, a.n_actions);
-    share_tape_reduce_kernel<<<dim3(rb, jobs.n), 256, 0, st>>>(tape, rows, jobs, partials, stride);
-    ORL_LAUNCH_CHECK("share_tape_reduce_kernel");
-    return orl::sum_row_blocks(partials, rb, stride, total, a.grads, st);
+    return orl::reduce_tape(tape, dc::TAPE, rows, make_share_jobs(a.obs_dim, a.n_actions), partials, stride, total, a.grads, st);
 }
 
 int orl_share_apply(const OrlPpoArgs* ap, void* stream) {

@@ -183,7 +183,8 @@ class PPOModule:
 
     def _act_recurrent(self, pol, obs, rnn_states_actor, masks, deterministic, exp_noise, rng_seed, rng_step):
         """One GRU policy step on a (rows, d) batch: returns (actions, log-probs, new rnn states (rows, 1, H))
-        (policy_network.py:130-162 with RNNLayer; orl_rnn_rollout with ENV_NONE)."""
+        (policy_network.py:130-162 with RNNLayer; orl_rnn_act_rows, the act of the host-stepped rollout, on slot 0 of
+        a one-step buffer: the noise of row r is keyed by (rng_seed, rng_step, r))."""
         rows, H = obs.shape[0], pol.hidden_size
         states = torch.zeros(2, rows, H, dtype=torch.float32, device=self.device)
         if rnn_states_actor is not None:
@@ -196,15 +197,15 @@ class PPOModule:
         noise = None if exp_noise is None else torch.as_tensor(exp_noise, dtype=torch.float32).to(self.device).contiguous()
         a = lib.OrlRnnArgs()
         a.env_kind, a.n_envs, a.n_agents, a.episode_length = lib.ENV_NONE, rows, 1, 1
-        a.t_begin, a.t_end = 0, 1
+        a.t_begin, a.t_end, a.row_begin, a.row_end = 0, 1, 0, rows
         a.obs_dim, a.critic_obs_dim, a.n_actions = pol.obs_dim, pol.obs_dim, pol.n_actions
         a.activation_id, a.deterministic = pol.activation_id, int(bool(deterministic))
         a.policy_params, a.policy_obs = lib.ptr(pol.flat_params), lib.ptr(obs)
         a.rnn_states, a.masks = lib.ptr(states), lib.ptr(mk)
         a.actions, a.action_log_probs = lib.ptr(actions), lib.ptr(logp)
         a.exp_noise = lib.ptr(noise)
-        a.rng_seed, a.rng_step_base = int(rng_seed), int(rng_step)
-        lib.check(self._lib.orl_rnn_rollout(a, lib.current_stream()), "orl_rnn_rollout(act)")
+        a.rng_seed, a.rng_step_base, a.rng_counter, a.rng_row_offset = int(rng_seed), int(rng_step), None, 0
+        lib.check(self._lib.orl_rnn_act_rows(a, lib.current_stream()), "orl_rnn_act_rows(act)")
         return actions, logp, states[1].view(rows, 1, H)
 
     @staticmethod

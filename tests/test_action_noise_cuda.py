@@ -134,7 +134,7 @@ def test_act_feed_forward_noise_key(device, share):
 
 
 def test_act_recurrent_noise_key(device):
-    """The recurrent act keys by the local row (OrlRnnArgs has no row offset)."""
+    """The recurrent act (orl_rnn_act_rows on rows [0, rows), rng_row_offset 0) keys by the local row."""
     import torch
 
     n, rows = 5, 20_000

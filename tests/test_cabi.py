@@ -24,3 +24,11 @@ def test_bad_arguments_are_reported_not_crashed(orl_lib):
     rc = orl_lib.orl_gae(None, None, None, None, None, None, None, None, None, None, 4, 4, 0.99, 0.95, 1, None)
     assert rc == 10001
     assert b"orl_gae" in orl_lib.orl_last_error()
+    # the recurrent rollout steps device envs only; a policy-only step goes to orl_rnn_act_rows
+    from openrl_b200 import lib
+
+    a = lib.OrlRnnArgs()
+    a.env_kind, a.n_envs, a.n_agents, a.episode_length, a.t_end = lib.ENV_NONE, 4, 1, 1, 1
+    a.obs_dim, a.critic_obs_dim, a.n_actions = 4, 4, 2
+    assert orl_lib.orl_rnn_rollout(a, None) == 10001
+    assert b"orl_rnn_act_rows" in orl_lib.orl_last_error()

@@ -4,13 +4,14 @@ between two host env.step calls, and `orl_host_insert_rnn`, which zeroes the hid
 Bars: the reference's CartPole-GRU trace (tests/golden/trace_cartpole_gru.npz) reproduced with the numpy CartPole stepped
 on the host, with the bars of `check_recurrent_trace`; the host-stepped rollout bit-identical to the device-env rollout of
 the same seed, in both host loops, and parameters within 1e-6 after one update; on a multi-agent host env every recorded
-hidden state within 2e-6 of the sequential core (`PPOModule.act`) and exactly zero where the env finished."""
+hidden state within 2e-6 of the sequential core (orl_rnn_core.h compiled by g++) and exactly zero where the env finished."""
 import os
 
 import numpy as np
 import pytest
 
 from conftest import GOLDEN
+from test_rnn_core_cpu import _ptr, shim  # noqa: F401  (pytest fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -244,7 +245,7 @@ def test_host_recurrent_rollout_is_bit_identical_to_device_rollout(cuda, env_id,
 
 @pytest.mark.parametrize("grouped", [False, True])
 @pytest.mark.parametrize("mode", ["use_recurrent_policy", "use_naive_recurrent_policy"])
-def test_host_recurrent_multi_agent_states_match_sequential_core(cuda, mode, grouped):
+def test_host_recurrent_multi_agent_states_match_sequential_core(cuda, shim, mode, grouped):  # noqa: F811
     """3 agents per env, ragged minibatches (chunked: 11*3*20/3 = 220 chunks in 3 minibatches; naive: 33 rows in 2), three
     iterations: every recorded rnn_states[t+1] is the sequential core's step from (obs[t], rnn_states[t], masks[t]),
     zero exactly where the env finished, and the metrics are finite."""
@@ -263,6 +264,7 @@ def test_host_recurrent_multi_agent_states_match_sequential_core(cuda, mode, gro
     drv = agent.driver
     b = drv.buffer.data
     rows = N * A
+    pol = net.module.models["policy"]
     for it in range(3):
         drv.episode = it
         host.finished_table()
@@ -272,9 +274,13 @@ def test_host_recurrent_multi_agent_states_match_sequential_core(cuda, mode, gro
         fin = np.repeat(host.finished_table(), A, axis=1)              # (T, rows)
         assert fin.shape == (T, rows) and fin.any()
         assert np.array_equal(mk[1:, :, 0].cpu().numpy() == 0, fin)
+        P = pol.flat_params.cpu().numpy()
         for t in range(T):
-            _, _, h1 = net.module.act(obs[t], hs[t], mk[t], deterministic=True)
-            got, want = hs[t + 1].cpu().numpy(), h1.cpu().numpy()
+            X, H0, m = (np.ascontiguousarray(v.cpu().numpy().reshape(rows, -1)) for v in (obs[t], hs[t], mk[t]))
+            want, out = np.zeros((rows, 64), np.float32), np.zeros((rows, pol.n_actions), np.float32)
+            shim.shim_forward_rows(_ptr(P), pol.obs_dim, pol.n_actions, pol.activation_id, rows, _ptr(X), _ptr(H0), _ptr(m),
+                                   _ptr(want), _ptr(out))
+            got = hs[t + 1].cpu().numpy().reshape(rows, 64)
             assert (got[fin[t]] == 0).all(), t
             np.testing.assert_allclose(got[~fin[t]], want[~fin[t]], rtol=0, atol=2e-6, err_msg=f"it{it} t{t}")
         drv.compute_returns()
