@@ -146,8 +146,10 @@ typedef struct OrlRolloutArgs {
     int32_t deterministic;
     int32_t env_table_len;
     const float* policy_params; /* flat net parameters, layout in orl_mlp.cuh / DESIGN.md */
-    float* policy_obs;          /* (T+1, B, d)   slot t read at t_begin, slots t+1 written */
-    float* critic_obs;          /* (T+1, B, dc)  or NULL */
+    float* policy_obs;          /* (T+1, B, d)   slot t read at t_begin, slots t+1 written; 16-byte aligned for
+                                   CartPole and GridWorld (one float4 per observation), else ORL_ERR_BAD_ARG */
+    float* critic_obs;          /* (T+1, B, dc)  or NULL; a separate one is written like policy_obs (and must be aligned
+                                   alike), except by orl_rollout on CartPole, which leaves it untouched */
     float* actions;             /* (T, B, 1)  sampled index stored as float32 (replay_data.py:163-166) */
     float* action_log_probs;    /* (T, B, 1) */
     float* rewards;             /* (T, B, 1) */
@@ -388,7 +390,8 @@ int orl_rnn_tape_width(void);
 /* floats of OrlRnnArgs.tape for a minibatch of `rows` = n_chunks * chunk_length row-steps (times A with ORL_PPO_JOINT_ACTION) */
 long long orl_rnn_workspace_floats(long long rows, int grads_stride);
 /* policy GRU rollout for steps [t_begin, t_end) fused with the device env (simple_spread, CartPole, GridWorld); device
- * envs only: ORL_ENV_NONE is rejected (the policy step of host-stepped rows is orl_rnn_act_rows) */
+ * envs only: ORL_ENV_NONE is rejected (the policy step of host-stepped rows is orl_rnn_act_rows).  CartPole and
+ * GridWorld need 16-byte aligned policy_obs and critic_obs (ORL_ERR_BAD_ARG otherwise). */
 int orl_rnn_rollout(const OrlRnnArgs* args, void* stream);
 /* policy GRU act for a HOST-stepped env: one step t = t_begin over buffer rows [row_begin, row_end) (B = n_envs *
  * n_agents rows per slot).  Reads policy_obs[t], rnn_states[t], masks[t]; writes actions[t], action_log_probs[t] and

@@ -1,6 +1,10 @@
-// Library-level C-ABI entry points: version, error string, device query; the rollouts' noise-counter bump.
+// Library-level C-ABI entry points: version, error string, device query; the rollouts' noise-counter bump; the kernels'
+// dynamic shared-memory opt-in.
 #include <stdarg.h>
 #include <string.h>
+
+#include <map>
+#include <mutex>
 
 #include "orl_common.cuh"
 
@@ -38,6 +42,23 @@ int bump_rng_counter(uint64_t* counter, int steps, cudaStream_t st) {
     if (!counter) return 0;
     bump_rng_counter_kernel<<<1, 1, 0, st>>>(counter, (uint64_t)steps);
     return check_cuda(cudaGetLastError(), "bump_rng_counter_kernel");
+}
+
+// the attribute belongs to the (kernel, device) pair: a process that launches on several devices opts in on each
+int allow_dynamic_smem(const void* kernel, size_t smem_bytes, bool max_carveout) {
+    static std::mutex mu;
+    static std::map<std::pair<const void*, int>, size_t> allowed;
+    int dev = 0;
+    if (int e = check_cuda(cudaGetDevice(&dev), "cudaGetDevice")) return e;
+    std::lock_guard<std::mutex> lock(mu);
+    size_t& have = allowed[{kernel, dev}];
+    if (have >= smem_bytes) return 0;
+    if (int e = check_cuda(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes),
+                           "cudaFuncSetAttribute(MaxDynamicSharedMemorySize)"))
+        return e;
+    if (max_carveout) cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    have = smem_bytes;
+    return 0;
 }
 }  // namespace orl
 

@@ -14,6 +14,13 @@ int sm_count();
 // advances the device Philox step counter of the action noise by the `steps` steps a rollout launch consumed; no-op
 // when `counter` is null
 int bump_rng_counter(uint64_t* counter, int steps, cudaStream_t st);
+// lets `kernel` take up to `smem_bytes` of dynamic shared memory on the current device, once per (kernel, device);
+// `max_carveout` also asks for the largest shared-memory carveout (best effort).  Thread-safe.
+int allow_dynamic_smem(const void* kernel, size_t smem_bytes, bool max_carveout = false);
+template <typename K>
+int allow_dynamic_smem(K* kernel, size_t smem_bytes, bool max_carveout = false) {
+    return allow_dynamic_smem(reinterpret_cast<const void*>(kernel), smem_bytes, max_carveout);
+}
 
 // ---- tape-gradient reductions of the recurrent and shared-model updates (orl_tape.cu) ----
 // A job reads columns of the `tape_width`-float tape rows: a gemm job writes sum_rows tape[p_off + m] * tape[q_off + k]

@@ -1,5 +1,5 @@
-// Device-side env.step wrappers (auto-reset + episode statistics) and the action sampler (noise, masking, sampling,
-// log-prob) shared by every rollout kernel.
+// Device-side env.step wrappers (auto-reset + episode statistics), the env step-and-insert of the device rollouts and the
+// action sampler (noise, masking, sampling, log-prob) shared by every rollout kernel.
 #pragma once
 #include "orl_envs.cuh"
 #include "orl_loss.cuh"
@@ -97,6 +97,81 @@ __device__ __forceinline__ void env_step_mpe(const EnvPtrs& E, int e, int N, con
     mpe_store(E.f64, e, N, s);
 #pragma unroll
     for (int ag = 0; ag < 3; ++ag) mpe_obs(s, ag, ob[ag]);
+}
+
+// ---- env.step + in-place buffer insert of the device rollouts (onpolicy_driver.py:80-152 for device envs) ---------------
+// EnvPtrs of an OrlRolloutArgs or an OrlRnnArgs (the two share the field names)
+template <typename Args>
+__device__ __forceinline__ EnvPtrs env_ptrs(const Args& a, int env_offset) {
+    return EnvPtrs{a.env_f64, a.env_u64, a.env_i32, a.env_table, a.env_table_len, a.rng_seed,
+                   a.ep_return, a.ep_length, a.episode_stats, env_offset};
+}
+
+// agent ag's observation of a simple_spread env whose agent 0 is buffer row r0: to its policy row and, when critic_obs is
+// given, to columns [18 ag, +18) of all three agents' 54-wide critic rows (the concatenated observation)
+__device__ __forceinline__ void mpe_insert_obs(const float (&o)[18], int ag, size_t r0, float* policy_obs, float* critic_obs) {
+#pragma unroll
+    for (int k = 0; k < 18; ++k) {
+        policy_obs[(r0 + ag) * 18 + k] = o[k];
+        if (critic_obs) {
+#pragma unroll
+            for (int dst = 0; dst < 3; ++dst) critic_obs[(r0 + dst) * 54 + ag * 18 + k] = o[k];
+        }
+    }
+}
+
+// step_insert_single stores an observation as one float4: policy_obs and a separate critic_obs must be 16-byte aligned
+template <typename Args>
+inline bool single_obs_aligned(const Args& a) {
+    return ((reinterpret_cast<uintptr_t>(a.policy_obs) | reinterpret_cast<uintptr_t>(a.critic_obs)) & 15) == 0;
+}
+
+// env.step of single-agent env e (CartPole-v1 / GridWorldEnv) on the action of slot t, then the insert: obs[t+1] (and a
+// separate critic_obs[t+1]), rewards[t], masks[t+1] and active_masks[t+1] = 1 (onpolicy_driver.py:118-124 with one
+// agent).  Returns obs[t+1]; `done` tells whether the env finished and was reset.
+template <typename Args>
+__device__ __forceinline__ float4 step_insert_single(const Args& a, const EnvPtrs& E, int kind, int e, int t, int act, bool& done) {
+    const int N = a.n_envs;
+    float ob[4], fin[4], reward;
+    env_step_single(E, kind, e, N, act, ob, reward, done, fin);
+    const float4 o = make_float4(ob[0], ob[1], ob[2], ob[3]);
+    const size_t o1 = (size_t)(t + 1) * N + e;
+    reinterpret_cast<float4*>(a.policy_obs)[o1] = o;
+    if (a.critic_obs && a.critic_obs != a.policy_obs) reinterpret_cast<float4*>(a.critic_obs)[o1] = o;
+    a.rewards[(size_t)t * N + e] = reward;
+    a.masks[o1] = done ? 0.f : 1.f;
+    a.active_masks[o1] = 1.f;
+    return o;
+}
+
+// no copy of the observations besides the buffers (the default `keep` of step_insert_mpe)
+struct NoKeep {
+    __device__ __forceinline__ void operator()(int, int, float) const {}
+};
+
+// the same for a simple_spread env: its three agent rows, which finish together.  keep(ag, k, v) receives obs[t+1] for a
+// kernel's own shared-memory copy, ahead of every buffer store: so the compiler can merge those shared stores into
+// vector stores (it cannot move them across the global ones), and the FFMA rollout stays within its registers without
+// spilling.  Returns done.
+template <typename Args, typename Keep = NoKeep>
+__device__ __forceinline__ bool step_insert_mpe(const Args& a, const EnvPtrs& E, int e, int t, const int (&acts)[3],
+                                                Keep keep = {}) {
+    const int N = a.n_envs, B = N * a.n_agents;   // n_agents == 3
+    float ob[3][18], reward; bool done;
+    env_step_mpe(E, e, N, acts, ob, reward, done);
+#pragma unroll
+    for (int ag = 0; ag < 3; ++ag)
+#pragma unroll
+        for (int k = 0; k < 18; ++k) keep(ag, k, ob[ag][k]);
+    const size_t r1 = (size_t)(t + 1) * B + (size_t)e * 3;
+#pragma unroll
+    for (int ag = 0; ag < 3; ++ag) {
+        mpe_insert_obs(ob[ag], ag, r1, a.policy_obs, a.critic_obs);
+        a.rewards[(size_t)t * B + (size_t)e * 3 + ag] = reward;
+        a.masks[r1 + ag] = done ? 0.f : 1.f;
+        a.active_masks[r1 + ag] = 1.f;
+    }
+    return done;
 }
 
 // ---- the action sampler of every rollout kernel ------------------------------------------------------------------------

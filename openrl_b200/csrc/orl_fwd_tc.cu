@@ -16,9 +16,6 @@
 // shared memory -> every thread reads its row's columns -> LayerNorm-3 + head in registers.  The rollout's
 // per-step critical path is one row's work (no shared-memory GEMM, no cross-row shuffles): ~1/3 of the FFMA kernel's.
 #include <algorithm>
-#include <cstdlib>
-#include <map>
-#include <mutex>
 
 #include "orl_envstep.cuh"
 #include "orl_tc16.cuh"
@@ -259,16 +256,9 @@ __global__ void __launch_bounds__(F_NT, 1) rollout_tc_kernel(const OrlRolloutArg
                 a.actions[grow] = (float)act;
                 a.action_log_probs[grow] = lp;
                 // ---- env.step of this thread's env, in-place insert into slot t / t+1 ----
-                EnvPtrs E{a.env_f64, a.env_u64, a.env_i32, a.env_table, a.env_table_len, a.rng_seed,
-                          a.ep_return, a.ep_length, a.episode_stats, a.rng_row_offset};
-                float ob[4], fin[4], reward; bool done;
-                env_step_single(E, ORL_ENV_GRIDWORLD, e, N, act, ob, reward, done, fin);
-                const size_t o1 = (size_t)(t + 1) * B + e;
-                *reinterpret_cast<float4*>(a.policy_obs + o1 * 4) = make_float4(ob[0], ob[1], ob[2], ob[3]);
-                a.rewards[grow] = reward;
-                a.masks[o1] = done ? 0.f : 1.f;
-                a.active_masks[o1] = 1.f;   // onpolicy_driver.py:118-124 with one agent
-                *reinterpret_cast<float4*>(c.xst + row * 8) = make_float4(ob[0], ob[1], ob[2], ob[3]);
+                bool done;
+                *reinterpret_cast<float4*>(c.xst + row * 8) =
+                    step_insert_single(a, env_ptrs(a, a.rng_row_offset / a.n_agents), ORL_ENV_GRIDWORLD, e, t, act, done);
             }
             F_ROWGROUP_SYNC();   // publishes the next observation to the row's other half; orders the exchange slots
             if (valid) {
@@ -555,58 +545,30 @@ __global__ void __launch_bounds__(RowsCfg::NT, RowsCfg::MIN_CTAS) rollout_cartpo
 #undef RW_FWD_SYNC
 #undef RW_PUBLISH_SYNC
 
-template <typename K>
-int prepare_kernel(K kern, uint32_t smem_bytes = F_SMEM) {
-    static std::mutex mu;
-    static std::map<const void*, bool> done;
-    std::lock_guard<std::mutex> lock(mu);
-    const void* key = reinterpret_cast<const void*>(kern);
-    if (!done.count(key)) {
-        int e = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes), "cudaFuncSetAttribute(fwd_tc)");
-        if (e) return e;
-        done[key] = true;
-    }
-    return 0;
-}
-
 }  // namespace
 
 namespace orl {
-
-bool fwd_tc_enabled() {
-    static const bool on = [] { const char* v = getenv("ORL_FWD_FFMA"); return !(v && atoi(v) != 0); }();
-    return on;
-}
 
 // ValueNetwork.forward over `rows` rows on the tensor cores; obs widths <= 8
 int launch_critic_values_tc(const float* params, int d, int activation_id, const float* obs, float* values, long long rows, cudaStream_t st) {
     const long long n_tiles = (rows + F_M - 1) / F_M;
     const int grid = (int)std::min<long long>(n_tiles, 2LL * sm_count());
-    if (activation_id == 1) {
-        if (int e = prepare_kernel(critic_values_tc_kernel<1>)) return e;
-        critic_values_tc_kernel<1><<<grid, F_NT, F_SMEM, st>>>(params, d, activation_id, obs, values, rows);
-    } else {
-        if (int e = prepare_kernel(critic_values_tc_kernel<-1>)) return e;
-        critic_values_tc_kernel<-1><<<grid, F_NT, F_SMEM, st>>>(params, d, activation_id, obs, values, rows);
-    }
+    const auto kern = activation_id == 1 ? critic_values_tc_kernel<1> : critic_values_tc_kernel<-1>;
+    if (int e = allow_dynamic_smem(kern, F_SMEM)) return e;
+    kern<<<grid, F_NT, F_SMEM, st>>>(params, d, activation_id, obs, values, rows);
     return check_cuda(cudaGetLastError(), "critic_values_tc_kernel");
-}
-
-bool rollout_tc_eligible(const OrlRolloutArgs& a) {
-    return fwd_tc_enabled() && (a.env_kind == ORL_ENV_CARTPOLE || a.env_kind == ORL_ENV_GRIDWORLD) && a.n_agents == 1 && a.obs_dim == 4 &&
-           a.head_kind == ORL_HEAD_CATEGORICAL && (reinterpret_cast<uintptr_t>(a.policy_obs) & 15) == 0;
 }
 
 int launch_rollout_tc(const OrlRolloutArgs& a, cudaStream_t st) {
     const bool relu = a.activation_id == 1;
     if (a.env_kind == ORL_ENV_CARTPOLE) {
         const auto kern = relu ? rollout_cartpole_rows_kernel<1> : rollout_cartpole_rows_kernel<-1>;
-        if (int e = prepare_kernel(kern, RowsCfg::SMEM)) return e;
+        if (int e = allow_dynamic_smem(kern, RowsCfg::SMEM)) return e;
         kern<<<(a.n_envs + RowsCfg::R - 1) / RowsCfg::R, RowsCfg::NT, RowsCfg::SMEM, st>>>(a);
         return check_cuda(cudaGetLastError(), "rollout_cartpole_rows_kernel");
     }
     const auto kern = relu ? rollout_tc_kernel<1> : rollout_tc_kernel<-1>;
-    if (int e = prepare_kernel(kern)) return e;
+    if (int e = allow_dynamic_smem(kern, F_SMEM)) return e;
     kern<<<(a.n_envs + F_M - 1) / F_M, F_NT, F_SMEM, st>>>(a);
     return check_cuda(cudaGetLastError(), "rollout_tc_kernel");
 }

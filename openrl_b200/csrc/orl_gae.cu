@@ -306,20 +306,10 @@ int launch_gae_tile(const GaeParams& p, cudaStream_t st) {
         int e = orl::check_cuda(cudaMemsetAsync(p.stats, 0, sizeof(double) * ORL_GAE_NSTATS, st), "memset stats");
         if (e) return e;
     }
-#define ORL_GAE_TILE(A_, S_)                                                                                          \
-    do {                                                                                                              \
-        static bool attr_done = false;                                                                                \
-        if (!attr_done) {                                                                                             \
-            int e_ = orl::check_cuda(cudaFuncSetAttribute(gae_tile_kernel<DENORM, A_, S_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024), "attr"); \
-            if (e_) return e_;                                                                                        \
-            attr_done = true;                                                                                         \
-        }                                                                                                             \
-        gae_tile_kernel<DENORM, A_, S_><<<grid, TILE_THREADS, smem, st>>>(p);                                         \
-    } while (0)
-    if (adv && stats) ORL_GAE_TILE(true, true);
-    else if (adv) ORL_GAE_TILE(true, false);
-    else if (stats) ORL_GAE_TILE(false, true);
-    else ORL_GAE_TILE(false, false);
+    const auto kern = adv ? (stats ? gae_tile_kernel<DENORM, true, true> : gae_tile_kernel<DENORM, true, false>)
+                          : (stats ? gae_tile_kernel<DENORM, false, true> : gae_tile_kernel<DENORM, false, false>);
+    if (int e = orl::allow_dynamic_smem(kern, 200 * 1024)) return e;
+    kern<<<grid, TILE_THREADS, smem, st>>>(p);
     ORL_LAUNCH_CHECK("gae_tile_kernel");
     return 0;
 }

@@ -596,13 +596,7 @@ extern "C" int orl_ppo_fwdbwd(const OrlPpoArgs* args, void* stream) {
         return orl::launch_ppo_fwdbwd_tc(a, reinterpret_cast<cudaStream_t>(stream));
     }
     const size_t smem = fwdbwd_smem_bytes(a.obs_dim, a.critic_obs_dim);
-    static bool attr_set = false;
-    if (!attr_set) {
-        int e = orl::check_cuda(cudaFuncSetAttribute(ppo_fwdbwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024),
-                                "cudaFuncSetAttribute(ppo_fwdbwd)");
-        if (e) return e;
-        attr_set = true;
-    }
+    if (int e = orl::allow_dynamic_smem(ppo_fwdbwd_kernel, 227 * 1024)) return e;
     ppo_fwdbwd_kernel<<<2 * a.grid_per_net, P_NT, smem, reinterpret_cast<cudaStream_t>(stream)>>>(a);
     ORL_LAUNCH_CHECK("ppo_fwdbwd_kernel");
     return 0;

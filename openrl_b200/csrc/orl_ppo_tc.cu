@@ -651,17 +651,7 @@ int launch_ppo_fwdbwd_tc(const OrlPpoArgs& a, cudaStream_t st) {
                         a.row_begin + (((a.batch_rows + T_M - 1) / T_M) * T_M) < (1ll << 31);
     const TcMaps* maps = tma_ok ? maps_for(a) : nullptr;
     TcKernel kern = pick_kernel(a.n_actions, a.activation_id, maps != nullptr);
-    {
-        static std::mutex mu;
-        static std::map<TcKernel, bool> prepared;
-        std::lock_guard<std::mutex> lock(mu);
-        if (!prepared.count(kern)) {
-            int e = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(8)), "cudaFuncSetAttribute(ppo_fwdbwd_tc)");
-            if (e) return e;
-            cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-            prepared[kern] = true;
-        }
-    }
+    if (int e = allow_dynamic_smem(kern, tc_smem_bytes(8), true)) return e;
     TcMaps none;
     if (!maps) memset(&none, 0, sizeof(none));
     kern<<<2 * a.grid_per_net, T_NT, smem, st>>>(a, maps ? *maps : none, stride);

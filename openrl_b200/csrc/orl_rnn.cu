@@ -47,7 +47,7 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_rollout_warp_kernel(const OrlRnnA
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     float* scr = smem + rw::smem_net_floats() + warp * A * rw::SCR;
-    EnvPtrs E{a.env_f64, a.env_u64, a.env_i32, a.env_table, a.env_table_len, a.rng_seed, a.ep_return, a.ep_length, a.episode_stats};
+    const EnvPtrs E = env_ptrs(a, 0);   // the env randomness is keyed by the launch's env index, like the action noise
     const uint64_t rng_base = a.rng_step_base + (a.rng_counter ? *a.rng_counter : 0ull);
     float* const no_tape[A] = {};
     for (int e = blockIdx.x * W_WPC + warp; e < N; e += gridDim.x * W_WPC) {
@@ -77,31 +77,11 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_rollout_warp_kernel(const OrlRnnA
             }
             int done_i = 0;
             if (lane == 0) {
-                bool done = false; float reward = 0.f;
+                bool done;
                 if constexpr (ENV == ORL_ENV_MPE_SPREAD) {
-                    float ob[3][18];
-                    const int acts3[3] = {acts[0], acts[A > 1 ? 1 : 0], acts[A > 2 ? 2 : 0]};
-                    env_step_mpe(E, e, N, acts3, ob, reward, done);
-                    const size_t r1 = (size_t)(t + 1) * B + (size_t)e * 3;
-                    for (int ag = 0; ag < 3; ++ag)
-                        for (int k = 0; k < 18; ++k) {
-                            a.policy_obs[(r1 + ag) * 18 + k] = ob[ag][k];
-                            for (int dst = 0; dst < 3; ++dst) a.critic_obs[(r1 + dst) * 54 + ag * 18 + k] = ob[ag][k];
-                        }
+                    done = step_insert_mpe(a, E, e, t, acts);
                 } else {
-                    float ob[4], fin[4];
-                    env_step_single(E, ENV, e, N, acts[0], ob, reward, done, fin);
-                    const size_t o1 = (size_t)(t + 1) * B + e;
-                    for (int k = 0; k < 4; ++k) {
-                        a.policy_obs[o1 * 4 + k] = ob[k];
-                        if (a.critic_obs != a.policy_obs) a.critic_obs[o1 * 4 + k] = ob[k];
-                    }
-                }
-                for (int ag = 0; ag < A; ++ag) {
-                    const size_t r1 = (size_t)(t + 1) * B + (size_t)e * A + ag;
-                    a.rewards[(size_t)t * B + (size_t)e * A + ag] = reward;
-                    a.masks[r1] = done ? 0.f : 1.f;
-                    a.active_masks[r1] = 1.f;
+                    step_insert_single(a, E, ENV, e, t, acts[0], done);
                 }
                 done_i = done ? 1 : 0;
             }
@@ -423,10 +403,6 @@ __global__ void __launch_bounds__(1024) rnn_apply_kernel(const OrlRnnArgs a) {
 constexpr size_t w_smem(int rows_per_warp) {   // weights of one net + the per-warp mat-vec scratch
     return (size_t)(rw::smem_net_floats() + rw::smem_scratch_floats(W_WPC, rows_per_warp)) * sizeof(float);
 }
-template <typename K>
-int warp_kernel_prepare(K kernel, size_t smem, const char* what) {
-    return orl::check_cuda(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), what);
-}
 int warp_grid(long long units) {   // persistent CTAs: one per SM, never more than the work needs
     const long long need = (units + W_WPC - 1) / W_WPC;
     return (int)std::max(1LL, std::min<long long>(need, orl::sm_count()));
@@ -466,6 +442,7 @@ int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
                       "simple_spread shapes / state");
     } else {
         ORL_CHECK_ARG(a.n_agents == 1 && a.obs_dim == 4, "single-agent env shapes");
+        ORL_CHECK_ARG(single_obs_aligned(a), "policy_obs and critic_obs must be 16-byte aligned");
     }
     cudaStream_t st = (cudaStream_t)stream;
     if (a.t_end > a.t_begin) {
@@ -473,13 +450,13 @@ int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
         int e = 0;
         switch (a.env_kind) {
             case ORL_ENV_MPE_SPREAD:
-                if ((e = warp_kernel_prepare(rnn_rollout_warp_kernel<ORL_ENV_MPE_SPREAD>, w_smem(3), "smem attr (rnn rollout)"))) return e;
+                if ((e = orl::allow_dynamic_smem(rnn_rollout_warp_kernel<ORL_ENV_MPE_SPREAD>, w_smem(3)))) return e;
                 rnn_rollout_warp_kernel<ORL_ENV_MPE_SPREAD><<<wg, W_NT, w_smem(3), st>>>(a); break;
             case ORL_ENV_CARTPOLE:
-                if ((e = warp_kernel_prepare(rnn_rollout_warp_kernel<ORL_ENV_CARTPOLE>, w_smem(1), "smem attr (rnn rollout)"))) return e;
+                if ((e = orl::allow_dynamic_smem(rnn_rollout_warp_kernel<ORL_ENV_CARTPOLE>, w_smem(1)))) return e;
                 rnn_rollout_warp_kernel<ORL_ENV_CARTPOLE><<<wg, W_NT, w_smem(1), st>>>(a); break;
             default:
-                if ((e = warp_kernel_prepare(rnn_rollout_warp_kernel<ORL_ENV_GRIDWORLD>, w_smem(1), "smem attr (rnn rollout)"))) return e;
+                if ((e = orl::allow_dynamic_smem(rnn_rollout_warp_kernel<ORL_ENV_GRIDWORLD>, w_smem(1)))) return e;
                 rnn_rollout_warp_kernel<ORL_ENV_GRIDWORLD><<<wg, W_NT, w_smem(1), st>>>(a); break;
         }
     }
@@ -500,10 +477,10 @@ int orl_rnn_act_rows(const OrlRnnArgs* ap, void* stream) {
         // one row per warp while the rows leave warps of the persistent grid idle, two (every weight read feeds both) beyond
         int e = 0;
         if (rows <= orl::sm_count() * W_WPC) {
-            if ((e = warp_kernel_prepare(rnn_act_rows_warp_kernel<1>, w_smem(1), "smem attr (rnn act rows)"))) return e;
+            if ((e = orl::allow_dynamic_smem(rnn_act_rows_warp_kernel<1>, w_smem(1)))) return e;
             rnn_act_rows_warp_kernel<1><<<warp_grid(rows), W_NT, w_smem(1), st>>>(a);
         } else {
-            if ((e = warp_kernel_prepare(rnn_act_rows_warp_kernel<2>, w_smem(2), "smem attr (rnn act rows)"))) return e;
+            if ((e = orl::allow_dynamic_smem(rnn_act_rows_warp_kernel<2>, w_smem(2)))) return e;
             rnn_act_rows_warp_kernel<2><<<warp_grid((rows + 1) / 2), W_NT, w_smem(2), st>>>(a);
         }
         if ((e = orl::check_cuda(cudaGetLastError(), "rnn_act_rows_warp_kernel launch"))) return e;
@@ -517,7 +494,7 @@ int orl_rnn_critic(const OrlRnnArgs* ap, void* stream) {
     if (int e = check_common(a)) return e;
     ORL_CHECK_ARG(a.critic_params && a.critic_obs && a.rnn_states_critic && a.masks && a.value_preds, "null critic buffer");
     const int B = a.n_envs * a.n_agents;
-    if (int e = warp_kernel_prepare(rnn_critic_warp_kernel, w_smem(1), "smem attr (rnn critic)")) return e;
+    if (int e = orl::allow_dynamic_smem(rnn_critic_warp_kernel, w_smem(1))) return e;
     rnn_critic_warp_kernel<<<warp_grid(B), W_NT, w_smem(1), (cudaStream_t)stream>>>(a);
     return orl::check_cuda(cudaGetLastError(), "rnn_critic_warp_kernel launch");
 }
@@ -551,11 +528,11 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
     constexpr int C_R = 2;
     const int cgrid = warp_grid((a.n_chunks + C_R - 1) / C_R);
     if (joint) {
-        if ((e = warp_kernel_prepare(rnn_joint_policy_warp_kernel<JOINT_A, W_NT>, w_smem(JOINT_A), "smem attr (rnn joint policy)"))) return e;
-        if ((e = warp_kernel_prepare(rnn_chunk_warp_kernel<false, true, C_R, W_NT>, w_smem(C_R), "smem attr (rnn chunk critic, agent 0)"))) return e;
+        if ((e = orl::allow_dynamic_smem(rnn_joint_policy_warp_kernel<JOINT_A, W_NT>, w_smem(JOINT_A)))) return e;
+        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<false, true, C_R, W_NT>, w_smem(C_R)))) return e;
     } else {
-        if ((e = warp_kernel_prepare(rnn_chunk_warp_kernel<true, false, C_R, W_NT>, w_smem(C_R), "smem attr (rnn chunk policy)"))) return e;
-        if ((e = warp_kernel_prepare(rnn_chunk_warp_kernel<false, false, C_R, W_NT>, w_smem(C_R), "smem attr (rnn chunk critic)"))) return e;
+        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<true, false, C_R, W_NT>, w_smem(C_R)))) return e;
+        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<false, false, C_R, W_NT>, w_smem(C_R)))) return e;
     }
     for (int net = 0; net < 2; ++net) {
         const int d = net == 0 ? a.obs_dim : a.critic_obs_dim, n = net == 0 ? a.n_actions : 1;

@@ -1,6 +1,8 @@
 // Fused rollout kernel: policy MLP forward + categorical sampling + device env.step + in-place
-// buffer insert, for steps [t_begin, t_end) of one rollout, plus env reset and the batched critic
-// forward.  See include/openrl_b200.h for the reference functions this replaces.
+// buffer insert, for steps [t_begin, t_end) of one rollout of simple_spread or of host-stepped envs
+// (ORL_ENV_NONE: act only; CartPole and GridWorld run the tensor-core rollouts of orl_fwd_tc.cu), plus
+// env reset and the batched critic forward.  See include/openrl_b200.h for the reference functions
+// this replaces.
 //
 // Mapping: a CTA of 128 threads owns ROWS = 32 consecutive rows (env, agent) for the whole step
 // range — envs never interact, so there is no grid-wide dependency and ONE launch covers all T
@@ -25,10 +27,7 @@ __global__ void env_step_mpe_kernel(int N, EnvPtrs E, const float* __restrict__ 
     float ob[3][18], reward; bool done;
     env_step_mpe(E, e, N, acts, ob, reward, done);
     for (int ag = 0; ag < 3; ++ag) {
-        for (int k = 0; k < 18; ++k) {
-            obs_out[((size_t)e * 3 + ag) * 18 + k] = ob[ag][k];
-            if (critic_obs_out) for (int dst = 0; dst < 3; ++dst) critic_obs_out[((size_t)e * 3 + dst) * 54 + ag * 18 + k] = ob[ag][k];
-        }
+        mpe_insert_obs(ob[ag], ag, (size_t)e * 3, obs_out, critic_obs_out);
         rewards_out[e * 3 + ag] = reward;
         dones_out[e * 3 + ag] = done ? 1.f : 0.f;
     }
@@ -141,43 +140,12 @@ __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
         __syncthreads();
 
         // ---- env.step for the envs of this CTA (one thread per env) ----
-        if (ENV == ORL_ENV_MPE_SPREAD && tid < n_env_here) {
-          if constexpr (ENV == ORL_ENV_MPE_SPREAD) {
-            const int e = env0 + tid;
-            EnvPtrs E{a.env_f64, a.env_u64, a.env_i32, a.env_table, a.env_table_len, a.rng_seed,
-                      a.ep_return, a.ep_length, a.episode_stats};
-            const int acts[3] = {act_s[tid * 3], act_s[tid * 3 + 1], act_s[tid * 3 + 2]};
-            float ob[3][18], reward; bool done;
-            env_step_mpe(E, e, N, acts, ob, reward, done);
-            const size_t r1 = (size_t)(t + 1) * B + (size_t)e * 3;
-#pragma unroll
-            for (int ag = 0; ag < 3; ++ag) {
-#pragma unroll
-                for (int k = 0; k < 18; ++k) {
-                    Xs[(tid * 3 + ag) * ldx + k] = ob[ag][k];
-                    a.policy_obs[(r1 + ag) * 18 + k] = ob[ag][k];
-#pragma unroll
-                    for (int dst = 0; dst < 3; ++dst) a.critic_obs[(r1 + dst) * 54 + ag * 18 + k] = ob[ag][k];
-                }
-                a.rewards[(size_t)t * B + (size_t)e * 3 + ag] = reward;
-                a.masks[r1 + ag] = done ? 0.f : 1.f;
-                a.active_masks[r1 + ag] = 1.f;  // all agents finish together (onpolicy_driver.py:118-124)
+        if constexpr (ENV == ORL_ENV_MPE_SPREAD) {
+            if (tid < n_env_here) {
+                const int acts[3] = {act_s[tid * 3], act_s[tid * 3 + 1], act_s[tid * 3 + 2]};
+                step_insert_mpe(a, env_ptrs(a, a.rng_row_offset / A), env0 + tid, t, acts,
+                                [&](int ag, int k, float v) { Xs[(tid * 3 + ag) * ldx + k] = v; });
             }
-          }
-        } else if (ENV != ORL_ENV_NONE && ENV != ORL_ENV_MPE_SPREAD && tid < n_env_here) {
-          if constexpr (ENV == ORL_ENV_CARTPOLE || ENV == ORL_ENV_GRIDWORLD) {
-            const int e = env0 + tid;
-            EnvPtrs E{a.env_f64, a.env_u64, a.env_i32, a.env_table, a.env_table_len, a.rng_seed,
-                      a.ep_return, a.ep_length, a.episode_stats, a.rng_row_offset / max(a.n_agents, 1)};
-            float ob[4], fin[4], reward; bool done;
-            env_step_single(E, ENV, e, N, act_s[tid], ob, reward, done, fin);
-            const size_t o1 = ((size_t)(t + 1) * B + e);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) { Xs[tid * ldx + k] = ob[k]; a.policy_obs[o1 * 4 + k] = ob[k]; }
-            a.rewards[(size_t)t * B + e] = reward;
-            a.masks[o1] = done ? 0.f : 1.f;
-            a.active_masks[o1] = 1.f;  // onpolicy_driver.py:118-124 with A == 1
-          }
         }
         __syncthreads();
     }
@@ -198,10 +166,7 @@ __global__ void env_reset_kernel(int env_kind, int N, double* env_f64, uint64_t*
         for (int ag = 0; ag < 3; ++ag) {
             float o[18];
             mpe_obs(s, ag, o);
-            for (int k = 0; k < 18; ++k) {
-                obs_out[((size_t)e * 3 + ag) * 18 + k] = o[k];
-                if (critic_obs_out) for (int dst = 0; dst < 3; ++dst) critic_obs_out[((size_t)e * 3 + dst) * 54 + ag * 18 + k] = o[k];
-            }
+            mpe_insert_obs(o, ag, (size_t)e * 3, obs_out, critic_obs_out);
         }
         return;
     }
@@ -359,8 +324,6 @@ __global__ void __launch_bounds__(C_NT) policy_eval_kernel(const float* __restri
 }  // namespace
 
 namespace orl {
-bool fwd_tc_enabled();
-bool rollout_tc_eligible(const OrlRolloutArgs& a);
 int launch_rollout_tc(const OrlRolloutArgs& a, cudaStream_t st);
 int launch_critic_values_tc(const float* params, int d, int activation_id, const float* obs, float* values, long long rows, cudaStream_t st);
 }  // namespace orl
@@ -438,7 +401,10 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
         return ORL_ERR_UNSUPPORTED;
     }
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (orl::rollout_tc_eligible(a)) {   // single-agent device envs: the tensor-core rollouts (orl_fwd_tc.cu)
+    if (a.env_kind == ORL_ENV_CARTPOLE || a.env_kind == ORL_ENV_GRIDWORLD) {   // the tensor-core rollouts (orl_fwd_tc.cu)
+        // both store each observation as one float4; only rollout_tc_kernel (GridWorld) writes a separate critic_obs
+        ORL_CHECK_ARG(a.env_kind == ORL_ENV_CARTPOLE ? (reinterpret_cast<uintptr_t>(a.policy_obs) & 15) == 0 : orl::single_obs_aligned(a),
+                      "CartPole / GridWorld: policy_obs (and GridWorld's separate critic_obs) must be 16-byte aligned");
         if (int e = orl::launch_rollout_tc(a, st)) return e;
         return orl::bump_rng_counter(a.rng_counter, a.t_end - a.t_begin, st);
     }
@@ -454,28 +420,13 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
     const int grid = (a.n_envs + envs_per_cta - 1) / envs_per_cta;
     const int ldx = orl::pad4(a.obs_dim) + 4;
     const size_t smem = sizeof(float) * (orl::smem_weights_floats(a.obs_dim, false) + rm * ldx + 2 * rm * orl::LDA + rm);
-#define ORL_LAUNCH_ROLLOUT(RM, EK)                                                                                   \
-    do {                                                                                                             \
-        static bool attr_done = false;                                                                               \
-        if (!attr_done) {                                                                                            \
-            int e_ = orl::check_cuda(cudaFuncSetAttribute(rollout_kernel<RM, EK>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024), "attr"); \
-            if (e_) return e_;                                                                                       \
-            attr_done = true;                                                                                        \
-        }                                                                                                            \
-        rollout_kernel<RM, EK><<<grid, R_NT, smem, st>>>(a);                                                         \
-    } while (0)
-#define ORL_LAUNCH_ROLLOUT_RM(EK)                                                        \
-    do {                                                                                 \
-        if (rm == 8) ORL_LAUNCH_ROLLOUT(8, EK);                                          \
-        else if (rm == 16) ORL_LAUNCH_ROLLOUT(16, EK);                                   \
-        else ORL_LAUNCH_ROLLOUT(32, EK);                                                 \
-    } while (0)
-    switch (a.env_kind) {
-        case ORL_ENV_NONE: ORL_LAUNCH_ROLLOUT_RM(ORL_ENV_NONE); break;
-        case ORL_ENV_CARTPOLE: ORL_LAUNCH_ROLLOUT_RM(ORL_ENV_CARTPOLE); break;
-        case ORL_ENV_GRIDWORLD: ORL_LAUNCH_ROLLOUT_RM(ORL_ENV_GRIDWORLD); break;
-        default: ORL_LAUNCH_ROLLOUT_RM(ORL_ENV_MPE_SPREAD); break;
-    }
+    const bool mpe = a.env_kind == ORL_ENV_MPE_SPREAD;
+    void (*const kern)(OrlRolloutArgs) =
+        rm == 8 ? (mpe ? rollout_kernel<8, ORL_ENV_MPE_SPREAD> : rollout_kernel<8, ORL_ENV_NONE>)
+        : rm == 16 ? (mpe ? rollout_kernel<16, ORL_ENV_MPE_SPREAD> : rollout_kernel<16, ORL_ENV_NONE>)
+                   : (mpe ? rollout_kernel<32, ORL_ENV_MPE_SPREAD> : rollout_kernel<32, ORL_ENV_NONE>);
+    if (int e = orl::allow_dynamic_smem(kern, 200 * 1024)) return e;
+    kern<<<grid, R_NT, smem, st>>>(a);
     ORL_LAUNCH_CHECK("rollout_kernel");
     return orl::bump_rng_counter(a.rng_counter, a.t_end - a.t_begin, st);
 }
@@ -486,17 +437,11 @@ extern "C" int orl_critic_values(const float* critic_params, int obs_dim, int ac
     ORL_CHECK_ARG(obs_dim > 0 && obs_dim <= 64, "obs_dim must be in 1..64");
     ORL_CHECK_ARG(rows > 0, "rows");
     ORL_CHECK_ARG(activation_id >= 0 && activation_id <= 3, "activation_id");
-    if (orl::fwd_tc_enabled() && obs_dim <= 8)   // tensor-core forward (orl_fwd_tc.cu)
+    if (obs_dim <= 8)   // tensor-core forward (orl_fwd_tc.cu)
         return orl::launch_critic_values_tc(critic_params, obs_dim, activation_id, obs, values, rows, reinterpret_cast<cudaStream_t>(stream));
     const int ldx = orl::pad4(obs_dim) + 4;
     const size_t smem = sizeof(float) * (orl::smem_weights_floats(obs_dim, false) + C_M * ldx + 2 * C_M * orl::LDA);
-    static bool attr_set = false;
-    if (!attr_set) {
-        int e = orl::check_cuda(cudaFuncSetAttribute(critic_values_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024),
-                                "cudaFuncSetAttribute(critic_values)");
-        if (e) return e;
-        attr_set = true;
-    }
+    if (int e = orl::allow_dynamic_smem(critic_values_kernel, 200 * 1024)) return e;
     const long long n_tiles = (rows + C_M - 1) / C_M;
     const int grid = (int)std::min<long long>(n_tiles, 2LL * orl::sm_count());
     critic_values_kernel<<<grid, C_NT, smem, reinterpret_cast<cudaStream_t>(stream)>>>(critic_params, obs_dim, activation_id,
@@ -514,13 +459,7 @@ extern "C" int orl_policy_eval(const float* policy_params, int obs_dim, int n_ac
     ORL_CHECK_ARG(head_kind == ORL_HEAD_CATEGORICAL || head_kind == ORL_HEAD_GAUSSIAN, "head_kind");
     const int ldx = orl::pad4(obs_dim) + 4;
     const size_t smem = sizeof(float) * (orl::smem_weights_floats(obs_dim, false) + C_M * ldx + 2 * C_M * orl::LDA);
-    static bool attr_set = false;
-    if (!attr_set) {
-        int e = orl::check_cuda(cudaFuncSetAttribute(policy_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024),
-                                "cudaFuncSetAttribute(policy_eval)");
-        if (e) return e;
-        attr_set = true;
-    }
+    if (int e = orl::allow_dynamic_smem(policy_eval_kernel, 200 * 1024)) return e;
     const long long n_tiles = (rows + C_M - 1) / C_M;
     const int grid = (int)std::min<long long>(n_tiles, 2LL * orl::sm_count());
     policy_eval_kernel<<<grid, C_NT, smem, reinterpret_cast<cudaStream_t>(stream)>>>(policy_params, obs_dim, n_actions, activation_id, head_kind,

@@ -44,19 +44,10 @@ __global__ void __launch_bounds__(S_NT) share_rollout_kernel(const OrlRolloutArg
                                       }, lp);
         a.actions[grow] = (float)act;
         a.action_log_probs[grow] = lp;
-        if (ENV != ORL_ENV_NONE) {
-            if constexpr (ENV == ORL_ENV_CARTPOLE || ENV == ORL_ENV_GRIDWORLD) {
-                EnvPtrs E{a.env_f64, a.env_u64, a.env_i32, a.env_table, a.env_table_len, a.rng_seed,
-                          a.ep_return, a.ep_length, a.episode_stats, a.rng_row_offset};
-                float ob[4], fin[4], reward; bool done;
-                env_step_single(E, ENV, e, N, act, ob, reward, done, fin);
-                const size_t o1 = (size_t)(t + 1) * B + e;
-#pragma unroll
-                for (int k = 0; k < 4; ++k) { x[k] = ob[k]; a.policy_obs[o1 * 4 + k] = ob[k]; }
-                a.rewards[grow] = reward;
-                a.masks[o1] = done ? 0.f : 1.f;
-                a.active_masks[o1] = 1.f;
-            }
+        if constexpr (ENV != ORL_ENV_NONE) {
+            bool done;
+            const float4 o = step_insert_single(a, env_ptrs(a, a.rng_row_offset / a.n_agents), ENV, e, t, act, done);
+            x[0] = o.x; x[1] = o.y; x[2] = o.z; x[3] = o.w;
         }
     }
 }
@@ -174,14 +165,17 @@ int orl_share_rollout(const OrlRolloutArgs* ap, void* stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const int B = a.n_envs * a.n_agents;
     const int grid = (B + S_NT - 1) / S_NT;
+    const char* aligned = "policy_obs (and a separate critic_obs) must be 16-byte aligned";
     if (a.env_kind == ORL_ENV_NONE) {
         ORL_CHECK_ARG(a.t_end == a.t_begin + 1, "ORL_ENV_NONE acts for one step per call");
         share_rollout_kernel<ORL_ENV_NONE><<<grid, S_NT, 0, st>>>(a);
     } else if (a.env_kind == ORL_ENV_CARTPOLE) {
         ORL_CHECK_ARG(a.n_agents == 1 && a.obs_dim == 4 && a.n_actions == 2 && a.env_f64 && a.env_u64 && a.env_i32, "CartPole shapes / state");
+        ORL_CHECK_ARG(single_obs_aligned(a), aligned);
         share_rollout_kernel<ORL_ENV_CARTPOLE><<<grid, S_NT, 0, st>>>(a);
     } else if (a.env_kind == ORL_ENV_GRIDWORLD) {
         ORL_CHECK_ARG(a.n_agents == 1 && a.obs_dim == 4 && a.n_actions == 5 && a.env_i32, "GridWorld shapes / state");
+        ORL_CHECK_ARG(single_obs_aligned(a), aligned);
         share_rollout_kernel<ORL_ENV_GRIDWORLD><<<grid, S_NT, 0, st>>>(a);
     } else {
         orl::set_last_error("orl_share_rollout: env_kind %d is not built for the shared model (single-agent device envs and ORL_ENV_NONE are)", a.env_kind);

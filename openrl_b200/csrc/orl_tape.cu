@@ -128,8 +128,7 @@ bool jobs_fit(const TapeJobs& jobs, int tape_width) {
 
 template <int TAPE_W>
 int launch_jobs(const float* tape, long long rows, const TapeJobs& jobs, float* partials, int stride, int rb, cudaStream_t st) {
-    if (int e = check_cuda(cudaFuncSetAttribute(tape_gemm_kernel<TAPE_W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TR_SMEM),
-                           "smem attr (tape gemm)")) return e;
+    if (int e = allow_dynamic_smem(tape_gemm_kernel<TAPE_W>, TR_SMEM)) return e;
     tape_gemm_kernel<TAPE_W><<<dim3(rb, jobs.n_gemm), TR_NT, TR_SMEM, st>>>(tape, rows, jobs, partials, stride);
     tape_colsum_kernel<TAPE_W><<<dim3(rb, jobs.n_col), TR_MAX_M, 0, st>>>(tape, rows, jobs, partials, stride);
     return 0;

@@ -32,3 +32,31 @@ def test_bad_arguments_are_reported_not_crashed(orl_lib):
     a.obs_dim, a.critic_obs_dim, a.n_actions = 4, 4, 2
     assert orl_lib.orl_rnn_rollout(a, None) == 10001
     assert b"orl_rnn_act_rows" in orl_lib.orl_last_error()
+    # the single-agent device rollouts store each observation as one float4: an observation buffer 4 bytes off a 16-byte
+    # boundary is rejected before anything is launched or dereferenced
+    fake = 1 << 20   # never dereferenced
+    buffers = ("policy_params", "policy_obs", "actions", "action_log_probs", "rewards", "masks", "active_masks", "env_f64",
+               "env_u64", "env_i32", "ep_return", "ep_length", "episode_stats")
+
+    def rollout_args(kind, n_actions, **misaligned):
+        r = lib.OrlRolloutArgs()
+        r.env_kind, r.n_envs, r.n_agents, r.episode_length, r.t_end = kind, 4, 1, 1, 1
+        r.obs_dim, r.n_actions, r.head_kind = 4, n_actions, lib.HEAD_CATEGORICAL
+        for name in buffers:
+            setattr(r, name, fake)
+        for name in misaligned:
+            setattr(r, name, fake + 4)
+        return r
+
+    for fn, args in ((orl_lib.orl_rollout, rollout_args(lib.ENV_CARTPOLE, 2, policy_obs=1)),
+                     (orl_lib.orl_rollout, rollout_args(lib.ENV_GRIDWORLD, 5, critic_obs=1)),
+                     (orl_lib.orl_share_rollout, rollout_args(lib.ENV_CARTPOLE, 2, policy_obs=1)),
+                     (orl_lib.orl_share_rollout, rollout_args(lib.ENV_GRIDWORLD, 5, critic_obs=1))):
+        assert fn(args, None) == 10001
+        assert b"16-byte aligned" in orl_lib.orl_last_error()
+    a.env_kind = lib.ENV_CARTPOLE
+    for name in buffers + ("rnn_states",):
+        setattr(a, name, fake)
+    a.critic_obs = fake + 4
+    assert orl_lib.orl_rnn_rollout(a, None) == 10001
+    assert b"16-byte aligned" in orl_lib.orl_last_error()

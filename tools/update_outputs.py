@@ -4,10 +4,12 @@
     python tools/update_outputs.py --compare DIR_A DIR_B
 
 `bench.py --dump-outputs` covers the C2 tensor-core update only.  This tool runs, from the seed, each update kernel
-family at a small shape: C2 on tensor cores, on FFMA, with the shared model and with dual clip / plain MSE value loss;
-C4 (GridWorld self-play, 5 actions); C3 GRU and C3 JRPO; C5 (Gaussian head, host-stepped synthetic env).  Per path it
-saves the policy and critic (or shared model) `flat_params`, their Adam moment buffers, `adam_steps`, the ValueNorm state and `train_info`
-as DIR/<path>/<name>.npy.  `--compare` prints the largest distance in units in the last place per array, so a refactor
+family and each rollout kernel at a small shape: C2 on tensor cores, on FFMA, with the shared model and with dual clip /
+plain MSE value loss; C2's flags on GridWorldEnv (rollout_tc_kernel) and with a GRU policy; C4 (GridWorld self-play,
+5 actions); C3 GRU, C3 JRPO and C3 with MLP nets (the simple_spread FFMA rollout); C5 (Gaussian head, host-stepped
+synthetic env).  Per path it saves the policy and critic (or shared model) `flat_params`, their Adam moment buffers,
+`adam_steps`, the ValueNorm state, `train_info` and the rollout buffer the last iteration leaves (`buffer_<name>`) as
+DIR/<path>/<name>.npy.  `--compare` prints the largest distance in units in the last place per array, so a refactor
 that must not change results can be checked bit for bit (distance 0) against its parent commit.
 """
 import argparse
@@ -26,16 +28,27 @@ PATHS = {
     "c2_ffma": ("c2", ["--use_tensor_cores", "false"]),
     "c2_share": ("c2", ["--use_share_model", "true"]),
     "c2_dualclip_mse": ("c2", ["--dual_clip_ppo", "true", "--use_huber_loss", "false", "--use_clipped_value_loss", "false"]),
+    "c2_gridworld": ("gridworld", []),
+    "c2_gru": ("c2", ["--use_recurrent_policy", "true"]),
     "c4": ("c4", []),
     "c3_gru": ("c3", []),
     "c3_jrpo": ("c3", ["--use_joint_action_loss", "true"]),
+    "c3_mlp": ("c3", ["--use_recurrent_policy", "false"]),
     "c5_gaussian_host": (None, []),
 }
 
 
-def state_arrays(trainer):
+BUFFER = ("actions", "action_log_probs", "policy_obs", "critic_obs", "rewards", "masks", "active_masks", "rnn_states",
+          "rnn_states_critic")
+
+
+def state_arrays(driver):
+    trainer, data = driver.trainer, driver.buffer.data
     m = trainer.algo_module
     out = {"adam_steps": m.adam_steps, "train_info": trainer.train_info}
+    for name in BUFFER:   # rnn_states* are None for MLP policies
+        if getattr(data, name, None) is not None:
+            out[f"buffer_{name}"] = getattr(data, name)
     for net in ("policy", "critic", "model"):   # "model": the shared policy-value network (use_share_model)
         model, opt = m.models.get(net), m.optimizers.get(net)
         if model is not None:
@@ -51,11 +64,13 @@ def state_arrays(trainer):
 def run_device(workload, flags):
     import bench
 
+    # GridWorldEnv is on no bench workload: C2's flags on it
+    bench.WORKLOADS.setdefault("gridworld", dict(bench.WORKLOADS["c2"], env="GridWorldEnv"))
     cfg, env, net, agent = bench.build_agent(0, 1, workload, ENVS, flags)
     drv = bench.make_driver(cfg, env, net, agent, 0, 1)
     for _ in range(K):
         drv.device_iteration()
-    return state_arrays(drv.trainer)
+    return state_arrays(drv)
 
 
 def run_host_gaussian():
@@ -73,7 +88,7 @@ def run_host_gaussian():
     env = HostVecEnv(bench.SyntheticHostEnv(ENVS, seed=0))
     agent = PPOAgent(PPONet(env, cfg=cfg, device=f"cuda:{torch.cuda.current_device()}"))
     agent.train(total_time_steps=ENVS * cfg.episode_length * K, logger=Logger(quiet=True))
-    return state_arrays(agent.driver.trainer)
+    return state_arrays(agent.driver)
 
 
 def save(out_dir):
