@@ -1,7 +1,9 @@
 // The PPO loss maths, in one place: the categorical log-softmax and log-prob that the rollout sampler (orl_envstep.cuh)
-// shares with the updates, and the per-minibatch constants, categorical row loss and value row loss of every update
-// kernel (ppo_net_pass in orl_ppo.cu, tc_net_pass in orl_ppo_tc.cu, the chunk and JRPO kernels of orl_rnn.cu,
-// share_fwdbwd_kernel in orl_share.cu).  The FFMA Gaussian head loss has one user and stays in ppo_net_pass.
+// and policy_eval_kernel share with the updates, the DiagGaussian log-prob and entropy of policy_eval_kernel and the
+// FFMA update, and the per-minibatch constants, categorical row loss and value row loss of every update kernel
+// (ppo_net_pass in orl_ppo.cu, tc_net_pass in orl_ppo_tc.cu, the chunk and JRPO kernels of orl_rnn.cu,
+// share_fwdbwd_kernel in orl_share.cu).  The DiagGaussian row loss is ppo_net_pass's alone: Box action spaces run the
+// FFMA update only.
 #pragma once
 #include "orl_mlp.cuh"
 
@@ -179,6 +181,37 @@ __device__ __forceinline__ CatRow categorical_row(const Args& a, float (&logit)[
     const float ent = categorical_entropy<NOUT>(nl, pr, n);
     categorical_dlogits<NOUT>(pg.dlogp * wrow, a.entropy_coef * wrow, act, n, masked, nl, pr, ent, dl);
     return CatRow{pg.loss, ent, pg.ratio};
+}
+
+// DiagGaussian head (distributions.py:34-47, 75-98): Normal.log_prob of one dimension at distance diff = x - mean,
+// -diff^2 / (2 var) - log(std) - log(sqrt(2 pi)), and Normal.entropy of one dimension, 0.5 + 0.5 log(2 pi) + log(std)
+__device__ __forceinline__ float gaussian_log_prob(float diff, float std, float logstd) {
+    return -(diff * diff) / (2.0f * (std * std)) - logstd - 0.9189385332046727f;
+}
+__device__ __forceinline__ float gaussian_entropy(float logstd) { return 1.4189385332046727f + logstd; }
+
+// Policy loss of one DiagGaussian row (act.py:150-158; ppo.py:307-319: a ratio per dimension, the surrogate summed over
+// the dimensions).  act / old_lp are the row's n entries; wrow weights the loss, went the entropy.  Adds each
+// dimension's weighted loss, weighted entropy and ratio / n to loss / ent / ratio in dimension order, so the caller's
+// running sums round as one loop over its rows' dimensions; writes dL/dmean to dl[j] and adds dL/dlogstd to dls[j].
+template <class Args>
+__device__ __forceinline__ void gaussian_row(const Args& a, const float (&mean)[MAX_OUT], int n, const float* logstd,
+                                             const float* act, const float* old_lp, float adv, float wrow, float went,
+                                             float (&dl)[MAX_OUT], float (&dls)[MAX_OUT], float& loss, float& ent,
+                                             float& ratio) {
+#pragma unroll
+    for (int j = 0; j < MAX_OUT; ++j) {
+        if (j < n) {
+            const float ls = logstd[j], std = expf(ls), var = std * std, diff = act[j] - mean[j];
+            const PgTerm pg = pg_term(gaussian_log_prob(diff, std, ls), old_lp[j], adv, a.clip_param, a.flags, a.dual_clip_coeff);
+            loss += pg.loss * wrow;
+            ent += gaussian_entropy(ls) * went;
+            ratio += pg.ratio / (float)n;
+            const float dlp = pg.dlogp * wrow;
+            dl[j] = dlp * diff / var;
+            dls[j] += dlp * (diff * diff / var - 1.0f) - a.entropy_coef * went;
+        }
+    }
 }
 
 __device__ __forceinline__ float huber(float e, float d) { return fabsf(e) <= d ? 0.5f * e * e : d * (fabsf(e) - 0.5f * d); }

@@ -176,28 +176,11 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
                 if (row < rows_here) {
                     const float active = row_act[row];
                     if (POLICY && gaussian) {
-                        // DiagGaussian head (act.py:150-158, distributions.py:34-47): per-dimension ratios,
-                        // surrogate summed over the action dimension (ppo.py:307-319)
                         const long long gi = row_idx[row];
-                        const float* logstd = params + net_offsets(d, n, 1).ls;
-                        const float adv = apply_adv_norm(mb.adv, row_c[row]);
-                        const float wrow = mb.weight(pol_masks, active);
                         const float went_row = pol_masks ? active * mb.inv_act : mb.inv_rows / (float)n;
-#pragma unroll
-                        for (int j = 0; j < MAX_OUT; ++j) {
-                            if (j < n) {
-                                const float mean = out[j], ls = logstd[j], std = expf(ls), var = std * std;
-                                const float act = a.actions[gi * n + j], diff = act - mean;
-                                const float lp = -(diff * diff) / (2.0f * var) - ls - 0.9189385332046727f;
-                                const PgTerm pg = pg_term(lp, a.old_log_probs[gi * n + j], adv, a.clip_param, a.flags, a.dual_clip_coeff);
-                                loss0 += pg.loss * wrow;
-                                loss1 += (1.4189385332046727f + ls) * went_row;   // 0.5 + 0.5 log(2 pi) + log(std)
-                                loss2 += pg.ratio / (float)n;
-                                const float dlp = pg.dlogp * wrow;
-                                dl[j] = dlp * diff / var;                                               // dL/dmean
-                                dls_acc[j] += dlp * (diff * diff / var - 1.0f) - a.entropy_coef * went_row;   // dL/dlogstd
-                            }
-                        }
+                        gaussian_row(a, out, n, params + net_offsets(d, n, 1).ls, a.actions + gi * n, a.old_log_probs + gi * n,
+                                     apply_adv_norm(mb.adv, row_c[row]), mb.weight(pol_masks, active), went_row, dl, dls_acc,
+                                     loss0, loss1, loss2);
                     } else if (POLICY) {
                         const long long gi = row_idx[row];
                         const float wrow = mb.weight(pol_masks, active);

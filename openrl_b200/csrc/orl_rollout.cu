@@ -1,8 +1,8 @@
-// Fused rollout kernel: policy MLP forward + categorical sampling + device env.step + in-place
-// buffer insert, for steps [t_begin, t_end) of one rollout of simple_spread or of host-stepped envs
-// (ORL_ENV_NONE: act only; CartPole and GridWorld run the tensor-core rollouts of orl_fwd_tc.cu), plus
-// env reset and the batched critic forward.  See include/openrl_b200.h for the reference functions
-// this replaces.
+// Fused rollout kernel: policy MLP forward + action sampling (categorical, or DiagGaussian on host-stepped envs) +
+// device env.step + in-place buffer insert, for steps [t_begin, t_end) of one rollout of simple_spread or of host-stepped
+// envs (ORL_ENV_NONE: act only; CartPole and GridWorld run the tensor-core rollouts of orl_fwd_tc.cu), plus env reset and
+// the FFMA row-batch forward of the critic values (obs_dim > 8) and the policy eval.  See include/openrl_b200.h for the
+// reference functions this replaces.
 //
 // Mapping: a CTA of 128 threads owns ROWS = 32 consecutive rows (env, agent) for the whole step
 // range — envs never interact, so there is no grid-wide dependency and ONE launch covers all T
@@ -187,12 +187,14 @@ __global__ void env_reset_kernel(int env_kind, int N, double* env_f64, uint64_t*
     }
 }
 
-// ---- batched critic forward --------------------------------------------------------------------
+// ---- FFMA row-batch forward: the MLP of one net over a flat batch of rows ------------------------------------------------
+// Persistent CTAs of C_NT threads walk tiles of C_M rows (grid-stride); per tile the trunk and the n head dots, then
+// epilogue(g, out) on the thread that owns row g, with out[0..n) the head outputs of that row.
 constexpr int C_M = 128, C_NT = 256;
 
-__global__ void __launch_bounds__(C_NT) critic_values_kernel(const float* __restrict__ params, int d, int activation_id,
-                                                             const float* __restrict__ obs, float* __restrict__ values,
-                                                             long long rows) {
+template <typename Epilogue>
+__device__ __forceinline__ void rows_forward(const float* __restrict__ params, int d, int n, int activation_id,
+                                             const float* __restrict__ obs, long long rows, Epilogue&& epilogue) {
     extern __shared__ __align__(16) float smem[];
     const int ldx = pad4(d) + 4;
     float* p = smem;
@@ -201,7 +203,7 @@ __global__ void __launch_bounds__(C_NT) critic_values_kernel(const float* __rest
     float* N1s = p; p += C_M * LDA;
     float* N3s = p; p += C_M * LDA;
     const int tid = threadIdx.x;
-    load_weights_folded<C_NT>(w, params, d, 1, false);
+    load_weights_folded<C_NT>(w, params, d, n, false);
     const long long n_tiles = (rows + C_M - 1) / C_M;
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const long long r0 = tile * C_M;
@@ -216,11 +218,41 @@ __global__ void __launch_bounds__(C_NT) critic_values_kernel(const float* __rest
         trunk_forward<C_M, C_NT, false>(w, Xs, ldx, d, activation_id, N1s, N3s, mu1, rstd1, rstd3, pm);
         __syncthreads();
         float out[MAX_OUT];
-        head_dots<C_M, C_NT>(w, N3s, 1, out);
+        head_dots<C_M, C_NT>(w, N3s, n, out);
         constexpr int PPR = C_NT / C_M;
-        if (tid % PPR == 0 && tid / PPR < rows_here) values[r0 + tid / PPR] = out[0];
+        if (tid % PPR == 0 && tid / PPR < rows_here) epilogue(r0 + tid / PPR, out);
         __syncthreads();
     }
+}
+
+// ValueNetwork.forward (value_network.py:113-136)
+__global__ void __launch_bounds__(C_NT) critic_values_kernel(const float* __restrict__ params, int d, int activation_id,
+                                                             const float* __restrict__ obs, float* __restrict__ values,
+                                                             long long rows) {
+    rows_forward(params, d, 1, activation_id, obs, rows, [&](long long g, float (&out)[MAX_OUT]) { values[g] = out[0]; });
+}
+
+// PolicyNetwork.eval_actions (policy_network.py:164-203, act.py:160-168 / 150-158): the log-prob of the given action and
+// the entropy of the action distribution per row (the caller takes the masked mean); per dimension for a Gaussian head.
+__global__ void __launch_bounds__(C_NT) policy_eval_kernel(const float* __restrict__ params, int d, int n, int activation_id, int head_kind,
+                                                           const float* __restrict__ obs, const float* __restrict__ actions,
+                                                           const float* __restrict__ action_masks, float* __restrict__ logp_out,
+                                                           float* __restrict__ entropy_out, long long rows) {
+    const float* logstd = params + net_offsets(d, n, 1).ls;
+    rows_forward(params, d, n, activation_id, obs, rows, [&](long long g, float (&out)[MAX_OUT]) {
+        if (head_kind == ORL_HEAD_GAUSSIAN) {
+            for (int j = 0; j < n; ++j) {
+                const float ls = logstd[j];
+                logp_out[g * n + j] = gaussian_log_prob(actions[g * n + j] - out[j], expf(ls), ls);
+                entropy_out[g * n + j] = gaussian_entropy(ls);
+            }
+        } else {
+            float nl[MAX_OUT], pr[MAX_OUT];
+            masked_log_softmax(out, n, action_masks ? action_masks + g * n : nullptr, nl, pr);
+            logp_out[g] = log_prob_of(nl, n, (int)actions[g]);
+            entropy_out[g] = categorical_entropy(nl, pr, n);
+        }
+    });
 }
 
 // ---- insert of one host env.step into the rollout buffer (OnPolicyDriver.add2buffer, onpolicy_driver.py:80-152) -----------
@@ -265,60 +297,17 @@ __global__ void host_insert_rnn_kernel(const float* __restrict__ staged, int n_e
     }
 }
 
-// ---- PolicyNetwork.eval_actions over a flat batch (policy_network.py:164-203, act.py:160-168 / 150-158) ----------------
-// log-prob of the given action and the entropy of the action distribution per row (the caller takes the masked mean).
-__global__ void __launch_bounds__(C_NT) policy_eval_kernel(const float* __restrict__ params, int d, int n, int activation_id, int head_kind,
-                                                           const float* __restrict__ obs, const float* __restrict__ actions,
-                                                           const float* __restrict__ action_masks, float* __restrict__ logp_out,
-                                                           float* __restrict__ entropy_out, long long rows) {
-    extern __shared__ __align__(16) float smem[];
+// launch of a row-batch forward kernel over `rows` rows of obs_dim d: grid = min(tiles, 2 x SMs)
+template <typename... Params, typename... Args>
+int launch_rows_forward(void (*kern)(Params...), const char* name, int d, long long rows, cudaStream_t st, Args... args) {
     const int ldx = pad4(d) + 4;
-    float* p = smem;
-    SmemWeights w = carve_weights(p, d, false);
-    float* Xs = p;  p += C_M * ldx;
-    float* N1s = p; p += C_M * LDA;
-    float* N3s = p; p += C_M * LDA;
-    const int tid = threadIdx.x;
-    load_weights_folded<C_NT>(w, params, d, n, false);
-    const bool gaussian = head_kind == ORL_HEAD_GAUSSIAN;
-    const float* logstd = params + net_offsets(d, n, 1).ls;
+    const size_t smem = sizeof(float) * (smem_weights_floats(d, false) + C_M * ldx + 2 * C_M * LDA);
+    if (int e = allow_dynamic_smem(kern, 200 * 1024)) return e;
     const long long n_tiles = (rows + C_M - 1) / C_M;
-    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const long long r0 = tile * C_M;
-        const int rows_here = (int)min((long long)C_M, rows - r0);
-        for (int i = tid; i < C_M * ldx; i += C_NT) {
-            const int r = i / ldx, k = i % ldx;
-            Xs[i] = (r < rows_here && k < d) ? obs[(r0 + r) * d + k] : 0.f;
-        }
-        __syncthreads();
-        float mu1[C_M / (C_NT / 16)], rstd1[C_M / (C_NT / 16)], rstd3[C_M / (C_NT / 16)];
-        unsigned pm;
-        trunk_forward<C_M, C_NT, false>(w, Xs, ldx, d, activation_id, N1s, N3s, mu1, rstd1, rstd3, pm);
-        __syncthreads();
-        float out[MAX_OUT];
-        head_dots<C_M, C_NT>(w, N3s, n, out);
-        constexpr int PPR = C_NT / C_M;
-        if (tid % PPR == 0 && tid / PPR < rows_here) {
-            const long long g = r0 + tid / PPR;
-            if (gaussian) {   // per-dimension log-probs and entropies (distributions.py:34-47)
-                for (int j = 0; j < n; ++j) {
-                    const float ls = logstd[j], std = expf(ls), diff = actions[g * n + j] - out[j];
-                    logp_out[g * n + j] = -(diff * diff) / (2.0f * (std * std)) - ls - 0.9189385332046727f;
-                    entropy_out[g * n + j] = 1.4189385332046727f + ls;
-                }
-            } else {
-                float nl[MAX_OUT], pr[MAX_OUT];
-                masked_log_softmax(out, n, action_masks ? action_masks + g * n : nullptr, nl, pr);
-                const float lp = log_prob_of(nl, n, (int)actions[g]);
-                float ent = 0.f;
-#pragma unroll
-                for (int j = 0; j < MAX_OUT; ++j) if (j < n) ent -= pr[j] * nl[j];
-                logp_out[g] = lp;
-                entropy_out[g] = ent;
-            }
-        }
-        __syncthreads();
-    }
+    const int grid = (int)std::min<long long>(n_tiles, 2LL * sm_count());
+    kern<<<grid, C_NT, smem, st>>>(args...);
+    ORL_LAUNCH_CHECK(name);
+    return 0;
 }
 
 }  // namespace
@@ -437,17 +426,11 @@ extern "C" int orl_critic_values(const float* critic_params, int obs_dim, int ac
     ORL_CHECK_ARG(obs_dim > 0 && obs_dim <= 64, "obs_dim must be in 1..64");
     ORL_CHECK_ARG(rows > 0, "rows");
     ORL_CHECK_ARG(activation_id >= 0 && activation_id <= 3, "activation_id");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (obs_dim <= 8)   // tensor-core forward (orl_fwd_tc.cu)
-        return orl::launch_critic_values_tc(critic_params, obs_dim, activation_id, obs, values, rows, reinterpret_cast<cudaStream_t>(stream));
-    const int ldx = orl::pad4(obs_dim) + 4;
-    const size_t smem = sizeof(float) * (orl::smem_weights_floats(obs_dim, false) + C_M * ldx + 2 * C_M * orl::LDA);
-    if (int e = orl::allow_dynamic_smem(critic_values_kernel, 200 * 1024)) return e;
-    const long long n_tiles = (rows + C_M - 1) / C_M;
-    const int grid = (int)std::min<long long>(n_tiles, 2LL * orl::sm_count());
-    critic_values_kernel<<<grid, C_NT, smem, reinterpret_cast<cudaStream_t>(stream)>>>(critic_params, obs_dim, activation_id,
-                                                                                      obs, values, rows);
-    ORL_LAUNCH_CHECK("critic_values_kernel");
-    return 0;
+        return orl::launch_critic_values_tc(critic_params, obs_dim, activation_id, obs, values, rows, st);
+    return launch_rows_forward(critic_values_kernel, "critic_values_kernel", obs_dim, rows, st, critic_params, obs_dim,
+                               activation_id, obs, values, rows);
 }
 
 extern "C" int orl_policy_eval(const float* policy_params, int obs_dim, int n_actions, int activation_id, int head_kind,
@@ -457,15 +440,9 @@ extern "C" int orl_policy_eval(const float* policy_params, int obs_dim, int n_ac
     ORL_CHECK_ARG(obs_dim > 0 && obs_dim <= 64 && n_actions > 0 && n_actions <= orl::MAX_OUT, "shapes");
     ORL_CHECK_ARG(rows > 0 && activation_id >= 0 && activation_id <= 3, "rows / activation_id");
     ORL_CHECK_ARG(head_kind == ORL_HEAD_CATEGORICAL || head_kind == ORL_HEAD_GAUSSIAN, "head_kind");
-    const int ldx = orl::pad4(obs_dim) + 4;
-    const size_t smem = sizeof(float) * (orl::smem_weights_floats(obs_dim, false) + C_M * ldx + 2 * C_M * orl::LDA);
-    if (int e = orl::allow_dynamic_smem(policy_eval_kernel, 200 * 1024)) return e;
-    const long long n_tiles = (rows + C_M - 1) / C_M;
-    const int grid = (int)std::min<long long>(n_tiles, 2LL * orl::sm_count());
-    policy_eval_kernel<<<grid, C_NT, smem, reinterpret_cast<cudaStream_t>(stream)>>>(policy_params, obs_dim, n_actions, activation_id, head_kind,
-                                                                                    obs, actions, action_masks, log_probs, entropy, rows);
-    ORL_LAUNCH_CHECK("policy_eval_kernel");
-    return 0;
+    return launch_rows_forward(policy_eval_kernel, "policy_eval_kernel", obs_dim, rows, reinterpret_cast<cudaStream_t>(stream),
+                               policy_params, obs_dim, n_actions, activation_id, head_kind, obs, actions, action_masks,
+                               log_probs, entropy, rows);
 }
 
 extern "C" int orl_host_insert(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,

@@ -29,16 +29,21 @@ def philox4x32_10(c0, c1, c2, c3, seed):
     return c
 
 
-def noise_table(T, rows, n, seed, step_base, row_offset):
-    """(T, rows, n) float32 Exp(1) noise exactly as the device keys it: step = step_base + t, row = row + row_offset."""
+def philox_units(T, rows, seed, step_base, row_offset, lanes):
+    """(T, rows, 4 * len(lanes)) float32 uniforms in (0, 1): the four words of each Philox lane in `lanes`, keyed as the
+    device's action_philox keys them (step = step_base + t, row = row + row_offset) and mapped by u32_to_unit_open."""
     step = np.uint64(step_base) + np.arange(T, dtype=np.uint64)[:, None]
     row = np.uint64(row_offset) + np.arange(rows, dtype=np.uint64)[None, :]
     words = []
-    for lane in (0, 1):
+    for lane in lanes:
         words += philox4x32_10(step & M32, step >> np.uint64(32), row, np.uint64(lane), seed)
-    u = np.stack(words, -1)[..., :n]
-    unit = ((u >> np.uint64(8)).astype(np.float32) + np.float32(0.5)) * np.float32(1.0 / 16777216.0)
-    return (-np.log(unit)).astype(np.float32)
+    u = np.stack(words, -1)
+    return ((u >> np.uint64(8)).astype(np.float32) + np.float32(0.5)) * np.float32(1.0 / 16777216.0)
+
+
+def noise_table(T, rows, n, seed, step_base, row_offset):
+    """(T, rows, n) float32 Exp(1) noise exactly as the device keys it: step = step_base + t, row = row + row_offset."""
+    return (-np.log(philox_units(T, rows, seed, step_base, row_offset, (0, 1))[..., :n])).astype(np.float32)
 
 
 def assert_same_draws(act_a, lp_a, act_b, lp_b, q, per_env_trajectory=False, valid=None):
