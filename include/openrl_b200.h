@@ -191,9 +191,13 @@ int orl_critic_values(const float* critic_params, int obs_dim, int activation_id
  * host-stepped envs: `staged` is the step's result as ONE uploaded block [obs (B*d) | rewards (B) | dones (B)]
  * (B = n_envs * n_agents rows); writes slot t+1 of policy_obs / masks / active_masks and slot t of rewards with the
  * reference's mask rules (masks = 0 where all agents of the env are done, active_masks = 0 for a done agent of a
- * running env).  Pointers address the given slot / row range (rows of a group are contiguous). */
+ * running env).  Pointers address the given slot / row range (rows of a group are contiguous).
+ * action_masks_next (nullable): when the envs reported legal-move masks (`info["action_masks"]`, prepare_action_masks,
+ * envs/vec_env/utils/util.py:54-88) for this step, the staged block carries them after the dones, [... | action masks
+ * (B*n_actions)], and they are written to slot t+1 of action_masks (replay_data.py:282-283); NULL writes nothing there,
+ * so the slot keeps what it held, as in the reference. */
 int orl_host_insert(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
-                    float* masks_next, float* active_masks_next, void* stream);
+                    float* masks_next, float* active_masks_next, float* action_masks_next, int n_actions, void* stream);
 
 /* ---- policy evaluation of given actions over a flat batch of rows ------------------------
  * Replaces PolicyNetwork.eval_actions (policy_network.py:164-203) -> ACTLayer.evaluate_actions (act.py:130-172), the
@@ -384,6 +388,11 @@ typedef struct OrlRnnArgs {
     int32_t rng_row_offset;                               /* added to the buffer row in the action-noise key (first GLOBAL row of this buffer) */
     int32_t row_begin, row_end;                           /* buffer rows [row_begin, row_end) of slot t_begin */
     int32_t reserved2;
+    /* (T+1, B, n) legal-move masks (0 = illegal: logit -6e4, no gradient; distributions.py:71) or NULL (every action
+     * legal).  Read by orl_rnn_act_rows (slot t_begin) and by the policy pass of orl_rnn_fwdbwd; when the
+     * ORL_PPO_JOINT_ACTION flag is set, orl_rnn_fwdbwd rejects it (ORL_ERR_BAD_ARG); orl_rnn_rollout (device envs, which
+     * report no masks) ignores it. */
+    const float* action_masks;
 } OrlRnnArgs;
 int orl_rnn_param_count(int obs_dim, int n_out);
 int orl_rnn_tape_width(void);
@@ -402,9 +411,10 @@ int orl_rnn_rollout(const OrlRnnArgs* args, void* stream);
 int orl_rnn_act_rows(const OrlRnnArgs* args, void* stream);
 /* orl_host_insert for a recurrent policy: additionally zeroes the 64-float rnn_states_next row of every agent of an env
  * whose agents are all done (rnn_states[dones_env] = 0, onpolicy_driver.py:262-269).  rnn_states_next addresses slot
- * t+1 at the same first row as the other pointers. */
+ * t+1 at the same first row as the other pointers; action_masks_next / n_actions as in orl_host_insert. */
 int orl_host_insert_rnn(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
-                        float* masks_next, float* active_masks_next, float* rnn_states_next, void* stream);
+                        float* masks_next, float* active_masks_next, float* rnn_states_next, float* action_masks_next,
+                        int n_actions, void* stream);
 /* recurrent critic over slots 0..T: value_preds[t] and rnn_states_critic[t+1] */
 int orl_rnn_critic(const OrlRnnArgs* args, void* stream);
 /* chunked BPTT forward + loss + backward of both nets over the minibatch chunks -> grads, loss_acc */

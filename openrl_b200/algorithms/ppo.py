@@ -206,6 +206,7 @@ class PPOAlgorithm:
         a.rnn_states, a.rnn_states_critic = lib.ptr(buf.rnn_states), lib.ptr(buf.rnn_states_critic)
         a.actions, a.action_log_probs = lib.ptr(buf.actions), lib.ptr(buf.action_log_probs)
         a.masks, a.active_masks = lib.ptr(buf.masks), lib.ptr(buf.active_masks)
+        a.action_masks = None if (buf.action_masks_trivial or buf.continuous) else lib.ptr(buf.action_masks)
         a.value_preds, a.returns, a.advantages = lib.ptr(buf.value_preds), lib.ptr(buf.returns), lib.ptr(buf.advantages)
         a.gae_stats, a.mb_stats = lib.ptr(buf.gae_stats), lib.ptr(mb_stats)
         a.tape, a.grads, a.grads_stride, a.loss_acc = lib.ptr(self.tape), lib.ptr(self.rnn_grads), self.rnn_stride, lib.ptr(self.loss_acc)

@@ -131,7 +131,8 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnn
             if (g * R + r < rows) {
                 const size_t grow = (size_t)t * B + row[r];
                 float lp;
-                const int act = sample_action(logit[r], n, nullptr, a.deterministic != 0, [&](float (&q)[MAX_OUT]) {   // identical on every lane
+                const int act = sample_action(logit[r], n, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0,
+                                              [&](float (&q)[MAX_OUT]) {   // identical on every lane
                     action_noise(a.exp_noise, (size_t)row[r], n, a.rng_seed, step, (uint32_t)(row[r] + a.rng_row_offset), q);
                 }, lp);
                 if (lane == 0) { a.actions[grow] = (float)act; a.action_log_probs[grow] = lp; }
@@ -229,7 +230,8 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
                 const float keep = valid[r] ? 1.f : 0.f;
                 if (POLICY) {
                     const float wrow = mb.weight(pol_masks, active);
-                    const CatRow c = categorical_row(a, out[r], n, nullptr, (int)a.actions[bi[r]], a.action_log_probs[bi[r]],
+                    const CatRow c = categorical_row(a, out[r], n, a.action_masks ? a.action_masks + bi[r] * n : nullptr,
+                                                     (int)a.actions[bi[r]], a.action_log_probs[bi[r]],
                                                      apply_adv_norm(mb.adv, a.advantages[bi[r]]), wrow, dl);
                     loss0 += keep * c.loss * wrow; loss1 += keep * c.ent * wrow; loss2 += keep * c.ratio;
                 } else {
@@ -517,6 +519,7 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
     if (joint) {
         ORL_CHECK_ARG(a.n_agents == JOINT_A, "ORL_PPO_JOINT_ACTION is built for 3 agents (simple_spread)");
         ORL_CHECK_ARG(a.n_chunks * a.chunk_length <= (long long)a.n_envs * a.episode_length, "v3 chunks exceed the N*T samples");
+        ORL_CHECK_ARG(!a.action_masks, "ORL_PPO_JOINT_ACTION takes no action_masks (simple_spread reports none)");
     }
     cudaStream_t st = (cudaStream_t)stream;
     int e = orl::check_cuda(cudaMemsetAsync(a.loss_acc, 0, 8 * sizeof(float), st), "memset loss_acc");

@@ -256,16 +256,22 @@ __global__ void __launch_bounds__(C_NT) policy_eval_kernel(const float* __restri
 }
 
 // ---- insert of one host env.step into the rollout buffer (OnPolicyDriver.add2buffer, onpolicy_driver.py:80-152) -----------
-// staged = [obs (B*d) | rewards (B) | dones (B)] as uploaded from the host in ONE copy; one thread per row.
-// Row r of the insert; returns whether every agent of the row's env is done.
+// staged = [obs (B*d) | rewards (B) | dones (B) (| action masks (B*n))] as uploaded from the host in ONE copy; one thread
+// per row.  Row r of the insert; returns whether every agent of the row's env is done.  The masks block is present (and
+// action_masks_next non-null) only when the envs reported masks for this step; otherwise slot t+1 keeps what it held.
 __device__ __forceinline__ bool host_insert_row(const float* __restrict__ staged, int n_envs, int n_agents, int d, int r,
                                                 float* __restrict__ obs_next, float* __restrict__ rewards,
-                                                float* __restrict__ masks_next, float* __restrict__ active_next) {
+                                                float* __restrict__ masks_next, float* __restrict__ active_next,
+                                                float* __restrict__ action_masks_next, int n) {
     const int B = n_envs * n_agents;
     const float* so = staged;
     const float* sr = staged + (size_t)B * d;
     const float* sd = sr + B;
     for (int k = 0; k < d; ++k) obs_next[(size_t)r * d + k] = so[(size_t)r * d + k];
+    if (action_masks_next) {
+        const float* sm = sd + B;
+        for (int k = 0; k < n; ++k) action_masks_next[(size_t)r * n + k] = sm[(size_t)r * n + k];
+    }
     rewards[r] = sr[r];
     const int e = r / n_agents;
     bool all_done = true;
@@ -277,20 +283,21 @@ __device__ __forceinline__ bool host_insert_row(const float* __restrict__ staged
 }
 
 __global__ void host_insert_kernel(const float* __restrict__ staged, int n_envs, int n_agents, int d, float* __restrict__ obs_next,
-                                   float* __restrict__ rewards, float* __restrict__ masks_next, float* __restrict__ active_next) {
+                                   float* __restrict__ rewards, float* __restrict__ masks_next, float* __restrict__ active_next,
+                                   float* __restrict__ action_masks_next, int n) {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n_envs * n_agents) return;
-    host_insert_row(staged, n_envs, n_agents, d, r, obs_next, rewards, masks_next, active_next);
+    host_insert_row(staged, n_envs, n_agents, d, r, obs_next, rewards, masks_next, active_next, action_masks_next, n);
 }
 
 // the same insert for a recurrent policy: rnn_states[t+1] of every agent of a finished env is zeroed (onpolicy_driver.py:262-269)
 constexpr int RNN_HIDDEN = 64;   // OrlRnnArgs.rnn_states rows
 __global__ void host_insert_rnn_kernel(const float* __restrict__ staged, int n_envs, int n_agents, int d, float* __restrict__ obs_next,
                                        float* __restrict__ rewards, float* __restrict__ masks_next, float* __restrict__ active_next,
-                                       float* __restrict__ rnn_next) {
+                                       float* __restrict__ rnn_next, float* __restrict__ action_masks_next, int n) {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= n_envs * n_agents) return;
-    if (host_insert_row(staged, n_envs, n_agents, d, r, obs_next, rewards, masks_next, active_next)) {
+    if (host_insert_row(staged, n_envs, n_agents, d, r, obs_next, rewards, masks_next, active_next, action_masks_next, n)) {
         float4* h = reinterpret_cast<float4*>(rnn_next + (size_t)r * RNN_HIDDEN);
 #pragma unroll
         for (int k = 0; k < RNN_HIDDEN / 4; ++k) h[k] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -446,24 +453,29 @@ extern "C" int orl_policy_eval(const float* policy_params, int obs_dim, int n_ac
 }
 
 extern "C" int orl_host_insert(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
-                               float* masks_next, float* active_masks_next, void* stream) {
+                               float* masks_next, float* active_masks_next, float* action_masks_next, int n_actions, void* stream) {
     ORL_CHECK_ARG(staged && policy_obs_next && rewards && masks_next && active_masks_next, "null buffer");
     ORL_CHECK_ARG(n_envs > 0 && n_agents > 0 && obs_dim > 0, "shapes");
+    ORL_CHECK_ARG(!action_masks_next || (n_actions > 0 && n_actions <= orl::MAX_OUT), "n_actions must be in 1..8");
     const int B = n_envs * n_agents;
     host_insert_kernel<<<(B + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(staged, n_envs, n_agents, obs_dim, policy_obs_next,
-                                                                                         rewards, masks_next, active_masks_next);
+                                                                                         rewards, masks_next, active_masks_next,
+                                                                                         action_masks_next, n_actions);
     ORL_LAUNCH_CHECK("host_insert_kernel");
     return 0;
 }
 
 extern "C" int orl_host_insert_rnn(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
-                                   float* masks_next, float* active_masks_next, float* rnn_states_next, void* stream) {
+                                   float* masks_next, float* active_masks_next, float* rnn_states_next, float* action_masks_next,
+                                   int n_actions, void* stream) {
     ORL_CHECK_ARG(staged && policy_obs_next && rewards && masks_next && active_masks_next && rnn_states_next, "null buffer");
     ORL_CHECK_ARG(n_envs > 0 && n_agents > 0 && obs_dim > 0, "shapes");
+    ORL_CHECK_ARG(!action_masks_next || (n_actions > 0 && n_actions <= orl::MAX_OUT), "n_actions must be in 1..8");
     ORL_CHECK_ARG(reinterpret_cast<uintptr_t>(rnn_states_next) % 16 == 0, "rnn_states_next must be 16-byte aligned");
     const int B = n_envs * n_agents;
     host_insert_rnn_kernel<<<(B + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        staged, n_envs, n_agents, obs_dim, policy_obs_next, rewards, masks_next, active_masks_next, rnn_states_next);
+        staged, n_envs, n_agents, obs_dim, policy_obs_next, rewards, masks_next, active_masks_next, rnn_states_next,
+        action_masks_next, n_actions);
     ORL_LAUNCH_CHECK("host_insert_rnn_kernel");
     return 0;
 }

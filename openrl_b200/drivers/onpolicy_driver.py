@@ -63,7 +63,12 @@ class OnPolicyDriver:
     def reset_and_buffer_init(self):
         d = self.buffer.data
         cri = None if d.critic_obs is d.policy_obs else d.critic_obs[0].view(-1, d.critic_obs_dim)
-        self.envs.reset_into(d.policy_obs[0].view(-1, d.obs_dim), cri)  # rl_driver.py:118-131, no host copy
+        if self.envs.kind == lib.ENV_NONE and not d.continuous:
+            # rl_driver.py:118-131: the reset infos' action masks go to slot 0 (init_buffer, replay_data.py:286-298)
+            if self.envs.reset_into(d.policy_obs[0].view(-1, d.obs_dim), cri, d.action_masks[0].view(-1, d.n_actions)):
+                d.action_masks_trivial = False
+        else:
+            self.envs.reset_into(d.policy_obs[0].view(-1, d.obs_dim), cri)  # rl_driver.py:118-131, no host copy
         d.masks[0].fill_(1.0)
         d.active_masks[0].fill_(1.0)
 
@@ -268,6 +273,7 @@ class OnPolicyDriver:
         a.actions, a.action_log_probs, a.rewards = lib.ptr(d.actions), lib.ptr(d.action_log_probs), lib.ptr(d.rewards)
         a.masks, a.active_masks, a.value_preds = lib.ptr(d.masks), lib.ptr(d.active_masks), lib.ptr(d.value_preds)
         a.exp_noise = lib.ptr(noise)
+        a.action_masks = None if d.action_masks_trivial else lib.ptr(d.action_masks)
         a.rng_seed, a.rng_step_base, a.rng_counter = int(self.cfg.seed) + 0x9E3779B9 * (self.rank + 1), 0, lib.ptr(self.rng_counter)
         state = lambda name: lib.ptr(getattr(env, name, None))   # a host-stepped env has no device state
         a.env_f64, a.env_u64, a.env_i32, a.env_table = state("env_f64"), state("env_u64"), state("env_i32"), state("env_table")
@@ -286,19 +292,26 @@ class OnPolicyDriver:
             a.rng_step_base, a.rng_counter = rng_step_base, None
         lib.check(self._lib.orl_rnn_act_rows(a, lib.current_stream()), "orl_rnn_act_rows")
 
-    def _host_insert(self, staged, step, lo, hi):
+    def _host_insert(self, staged, step, lo, hi, has_masks=False):
         """One host env.step of envs [lo, hi) into slot step + 1 (rewards: slot step): orl_host_insert, or
-        orl_host_insert_rnn, which also zeroes rnn_states[step + 1] of the envs that finished."""
+        orl_host_insert_rnn, which also zeroes rnn_states[step + 1] of the envs that finished.  With `has_masks` the
+        staged block carries the envs' action masks, written to action_masks[step + 1] (replay_data.py:282-283); the
+        buffer's masks stop being trivial for good."""
         d, A = self.buffer.data, self.envs.agent_num
         r0, r1 = lo * A, hi * A
         args = (lib.ptr(staged), hi - lo, A, d.obs_dim, lib.ptr(d.policy_obs[step + 1].view(-1, d.obs_dim)[r0:r1]),
                 lib.ptr(d.rewards[step].view(-1)[r0:r1]), lib.ptr(d.masks[step + 1].view(-1)[r0:r1]),
                 lib.ptr(d.active_masks[step + 1].view(-1)[r0:r1]))
+        am = None
+        if has_masks:
+            d.action_masks_trivial = False
+            am = d.action_masks[step + 1].view(-1, d.n_actions)[r0:r1]
         if self.recurrent:
             states = d.rnn_states[step + 1].view(d.n_rollout_threads * A, -1)[r0:r1]
-            lib.check(self._lib.orl_host_insert_rnn(*args, lib.ptr(states), lib.current_stream()), "orl_host_insert_rnn")
+            lib.check(self._lib.orl_host_insert_rnn(*args, lib.ptr(states), lib.ptr(am), d.n_actions, lib.current_stream()),
+                      "orl_host_insert_rnn")
         else:
-            lib.check(self._lib.orl_host_insert(*args, lib.current_stream()), "orl_host_insert")
+            lib.check(self._lib.orl_host_insert(*args, lib.ptr(am), d.n_actions, lib.current_stream()), "orl_host_insert")
         self.gpu_launches += 1
 
     def _launch_steps(self, t_begin, t_end, noise):
@@ -410,14 +423,15 @@ class OnPolicyDriver:
                 a.policy_params = lib.ptr(pol.flat_params)
                 a.policy_obs = lib.ptr(d.policy_obs[step])
                 a.actions, a.action_log_probs = lib.ptr(d.actions[step]), lib.ptr(d.action_log_probs[step])
+                a.action_masks = None if d.action_masks_trivial else lib.ptr(d.action_masks[step])
                 a.exp_noise = lib.ptr(noise)
                 a.rng_seed, a.rng_step_base, a.rng_counter = int(self.cfg.seed) + 0x9E3779B9 * (self.rank + 1), 0, lib.ptr(self.rng_counter)
                 with self._phase("rollout"):
                     act_fn = self._lib.orl_share_rollout if getattr(self.trainer, "share", False) else self._lib.orl_rollout
                     lib.check(act_fn(a, lib.current_stream()), "orl_rollout(act)")
             self.gpu_launches += 2
-            staged, obs, rewards, dones, infos = env.step_staged(d.actions[step].view(B, w))
-            self._host_insert(staged, step, 0, N)
+            staged, obs, rewards, dones, infos, has_masks = env.step_staged(d.actions[step].view(B, w))
+            self._host_insert(staged, step, 0, N, has_masks)
             self.agent.num_time_steps += N
             if cb is not None:
                 actions = d.actions[step].cpu().numpy()  # noqa: F841
@@ -448,6 +462,7 @@ class OnPolicyDriver:
         a.policy_params = lib.ptr(pol.flat_params)
         a.policy_obs = lib.ptr(obs[r0:r1])
         a.actions, a.action_log_probs = lib.ptr(acts[r0:r1]), lib.ptr(logp[r0:r1])
+        a.action_masks = None if d.action_masks_trivial else lib.ptr(d.action_masks[step].view(-1, d.n_actions)[r0:r1])
         a.rng_seed, a.rng_step_base, a.rng_counter = int(self.cfg.seed) + 0x9E3779B9 * (self.rank + 1), self._host_steps_base + step, None
         a.rng_row_offset = r0
         act_fn = self._lib.orl_share_rollout if getattr(self.trainer, "share", False) else self._lib.orl_rollout
@@ -469,8 +484,8 @@ class OnPolicyDriver:
                 env.group_fetch_actions(g, lo, hi, self._act_rows(0, lo, hi))
             for step in range(T):
                 for g, (lo, hi) in enumerate(groups):
-                    staged, *_ = env.group_step(g, lo, hi)     # host env.step of this group (device busy with the other)
-                    self._host_insert(staged, step, lo, hi)
+                    staged, *_, has_masks = env.group_step(g, lo, hi)   # host env.step of this group (device busy with the other)
+                    self._host_insert(staged, step, lo, hi, has_masks)
                     if step + 1 < T:
                         env.group_fetch_actions(g, lo, hi, self._act_rows(step + 1, lo, hi))
                 self.agent.num_time_steps += N

@@ -159,7 +159,7 @@ class PPOModule:
         obs = torch.as_tensor(obs, dtype=torch.float32).to(self.device).contiguous().view(-1, pol.obs_dim)
         rows = obs.shape[0]
         if getattr(pol, "recurrent", False):
-            return self._act_recurrent(pol, obs, rnn_states_actor, masks, deterministic, exp_noise, rng_seed, rng_step)
+            return self._act_recurrent(pol, obs, rnn_states_actor, masks, action_masks, deterministic, exp_noise, rng_seed, rng_step)
         act_w = pol.n_actions if pol.head_kind == lib.HEAD_GAUSSIAN else 1
         actions = torch.empty(rows, act_w, dtype=torch.float32, device=self.device)
         logp = torch.empty(rows, act_w, dtype=torch.float32, device=self.device)
@@ -181,10 +181,10 @@ class PPOModule:
             lib.check(self._lib.orl_rollout(a, lib.current_stream()), "orl_rollout(act)")
         return actions, logp
 
-    def _act_recurrent(self, pol, obs, rnn_states_actor, masks, deterministic, exp_noise, rng_seed, rng_step):
+    def _act_recurrent(self, pol, obs, rnn_states_actor, masks, action_masks, deterministic, exp_noise, rng_seed, rng_step):
         """One GRU policy step on a (rows, d) batch: returns (actions, log-probs, new rnn states (rows, 1, H))
         (policy_network.py:130-162 with RNNLayer; orl_rnn_act_rows, the act of the host-stepped rollout, on slot 0 of
-        a one-step buffer: the noise of row r is keyed by (rng_seed, rng_step, r))."""
+        a one-step buffer: the noise of row r is keyed by (rng_seed, rng_step, r)).  action_masks (rows, n) or None."""
         rows, H = obs.shape[0], pol.hidden_size
         states = torch.zeros(2, rows, H, dtype=torch.float32, device=self.device)
         if rnn_states_actor is not None:
@@ -195,6 +195,7 @@ class PPOModule:
         actions = torch.empty(rows, 1, dtype=torch.float32, device=self.device)
         logp = torch.empty(rows, 1, dtype=torch.float32, device=self.device)
         noise = None if exp_noise is None else torch.as_tensor(exp_noise, dtype=torch.float32).to(self.device).contiguous()
+        am = None if action_masks is None else torch.as_tensor(action_masks, dtype=torch.float32).to(self.device).contiguous()
         a = lib.OrlRnnArgs()
         a.env_kind, a.n_envs, a.n_agents, a.episode_length = lib.ENV_NONE, rows, 1, 1
         a.t_begin, a.t_end, a.row_begin, a.row_end = 0, 1, 0, rows
@@ -203,7 +204,7 @@ class PPOModule:
         a.policy_params, a.policy_obs = lib.ptr(pol.flat_params), lib.ptr(obs)
         a.rnn_states, a.masks = lib.ptr(states), lib.ptr(mk)
         a.actions, a.action_log_probs = lib.ptr(actions), lib.ptr(logp)
-        a.exp_noise = lib.ptr(noise)
+        a.exp_noise, a.action_masks = lib.ptr(noise), lib.ptr(am)
         a.rng_seed, a.rng_step_base, a.rng_counter, a.rng_row_offset = int(rng_seed), int(rng_step), None, 0
         lib.check(self._lib.orl_rnn_act_rows(a, lib.current_stream()), "orl_rnn_act_rows(act)")
         return actions, logp, states[1].view(rows, 1, H)

@@ -9,29 +9,10 @@ import torch
 from ...algorithms.ppo import PPOAlgorithm
 from ...buffers import NormalReplayBuffer
 from ...drivers.onpolicy_driver import OnPolicyDriver
+from ...envs.vec_env.host_venv import prepare_action_masks
 from ...utils.callbacks import BaseCallback, CallbackList
 from ...utils.logger import Logger
 from ... import lib
-
-
-def prepare_action_masks(info, agent_num=1):
-    """openrl/envs/vec_env/utils/util.py:54-88: per-env `info["action_masks"]` ((n,) or (A, n)) -> (N*A, n);
-    None when any env carries no mask (all actions available)."""
-    if info is None:
-        return None
-    rows = []
-    for env_info in info:
-        for a in range(agent_num):
-            if env_info is None or "action_masks" not in env_info:
-                return None
-            m = np.asarray(env_info["action_masks"])
-            if m.ndim == 2:
-                rows.append(m[a])
-            elif m.ndim == 1:
-                rows.append(m)
-            else:
-                raise ValueError(m.ndim)
-    return np.asarray(rows, dtype=np.float32)
 
 
 class PPOAgent:

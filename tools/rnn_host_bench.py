@@ -7,9 +7,11 @@ sampling, data_chunk_length 16, the default epochs / minibatches.  Per mode: CUD
 (orl_rnn_act_rows, or orl_rollout with ORL_ENV_NONE for the MLP), around the critic and update phases and around the
 whole iteration (rollout -> returns -> update -> after_update); the numpy env alone is timed over T steps with uniform
 random actions.  An act event pair also spans the Python that fills the launch arguments.  Modes are timed alternately: `--rounds` rounds of `--iters` iterations each, after `--warmup` iterations of
-each.  Prints the card name, power limit and clocks read in the same run, and one JSON line.
+each.  Prints the card name, power limit and clocks read in the same run, and one JSON line.  `--masked`: every env
+reports `info["action_masks"]` on every step (a fixed random row per env, action 0 always legal), so the iteration also
+stages, uploads, inserts and applies the masks: the per-step cost of mask ingest is the difference to a run without.
 
-    python tools/rnn_host_bench.py [--envs 1024 --T 128 --iters 3 --rounds 2 --warmup 2]
+    python tools/rnn_host_bench.py [--envs 1024 --T 128 --iters 3 --rounds 2 --warmup 2 --masked]
 """
 import argparse
 import copy
@@ -42,11 +44,15 @@ def card():
 class CartPoleHost:
     """The numpy CartPole vec-env with the reference's duck type; `step_range` steps envs [lo, hi) (two-group loop)."""
 
-    def __init__(self, n):
+    def __init__(self, n, masked=False):
         from openrl_b200 import spaces
         from oracle.envs import CartPoleVec
 
         self.inner = CartPoleVec(n)
+        self.mask_rows = None
+        if masked:
+            self.mask_rows = (np.random.default_rng(1).random((n, 2)) < 0.5).astype(np.int8)
+            self.mask_rows[:, 0] = 1
         self.parallel_env_num, self.agent_num = n, 1
         self.observation_space = spaces.Box(-np.inf, np.inf, (4,), np.float32)
         self.action_space = spaces.Discrete(2)
@@ -61,10 +67,12 @@ class CartPoleHost:
         sub = copy.copy(self.inner)
         sub.N, sub.rng, sub.state, sub.elapsed = hi - lo, self.inner.rng[lo:hi], self.inner.state[lo:hi], self.inner.elapsed[lo:hi]
         o, r, d, _ = sub.step(actions)
+        if self.mask_rows is not None:
+            return o, r, d, [{"action_masks": m} for m in self.mask_rows[lo:hi]]
         return o, r, d, [{} for _ in range(hi - lo)]
 
 
-def build(n, T, recurrent, grouped):
+def build(n, T, recurrent, grouped, masked=False):
     from openrl_b200.configs.config import create_config_parser
     from openrl_b200.envs.vec_env import HostVecEnv
     from openrl_b200.modules.common import PPONet
@@ -75,7 +83,7 @@ def build(n, T, recurrent, grouped):
                                              "--use_recurrent_policy", "true" if recurrent else "false",
                                              "--host_env_groups", "true" if grouped else "false"])
     cfg.quiet = True
-    agent = PPOAgent(PPONet(HostVecEnv(CartPoleHost(n)), cfg=cfg, device="cuda:0"))
+    agent = PPOAgent(PPONet(HostVecEnv(CartPoleHost(n, masked)), cfg=cfg, device="cuda:0"))
     agent.train(total_time_steps=0, logger=Logger(quiet=True))   # trainer / buffer / driver, envs reset
     drv = agent.driver
     assert drv.recurrent == recurrent
@@ -133,6 +141,7 @@ def main():
     ap.add_argument("--iters", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--masked", action="store_true", help="the envs report action masks on every step")
     args = ap.parse_args()
 
     import torch
@@ -142,7 +151,7 @@ def main():
     modes = {}
     for recurrent in (True, False):
         for grouped in (False, True):
-            drv, acts = build(args.envs, args.T, recurrent, grouped)
+            drv, acts = build(args.envs, args.T, recurrent, grouped, args.masked)
             for _ in range(args.warmup):
                 iteration(drv, acts)
             modes[("gru" if recurrent else "mlp") + ("_grouped" if grouped else "_sync")] = (drv, acts)
@@ -160,7 +169,8 @@ def main():
         host.step(acts_host[t])
     env_ms = (time.perf_counter() - t0) * 1e3
     name, q = card()
-    res = {"workload": f"CartPole host-stepped (numpy env), {args.envs} envs, T={args.T}, Philox sampling, data_chunk_length 16",
+    res = {"workload": f"CartPole host-stepped (numpy env), {args.envs} envs, T={args.T}, Philox sampling, data_chunk_length 16"
+                       + (", action masks reported on every step" if args.masked else ""),
            "card": name, "power_limit,clocks.sm,clocks.max.sm": q, "host_env_only_ms_per_iteration": round(env_ms, 2),
            "iterations_per_mode": args.rounds * args.iters, "modes": {}}
     for m, s in samples.items():
