@@ -78,7 +78,8 @@ class OnPolicyDriver:
         pool = getattr(self.envs, "opponent_pool", None)
         freq = int(getattr(self.cfg, "selfplay_save_freq", 5))
         if pool is not None and freq > 0 and (self.episode + 1) % freq == 0:
-            pool.add(self.trainer.algo_module.models["policy"].flat_params, self.agent.num_time_steps)
+            pol = self.trainer.algo_module.models["policy"]
+            pool.add(pol.flat_params, self.agent.num_time_steps, activation_id=pol.activation_id)
 
     # -- one captured CUDA graph per iteration -------------------------------------------------
     def _graph_ok(self):

@@ -143,8 +143,9 @@ class DeviceVecEnv:
         return s
 
     def _selfplay_step(self, actions):
-        """vec-env step API for the 2-player grid: the learner's actions are given, the opponent acts from the pool.  Runs the
-        rollout kernel for one step on a two-slot scratch buffer (policy parameters are not needed: actions are scripted)."""
+        """vec-env step API for the 2-player grid: the learner's actions are given, the opponent acts from the pool with the
+        snapshots' activation.  Runs the rollout kernel for one step on a two-slot scratch buffer (policy parameters are not
+        needed: actions are scripted)."""
         N = self.parallel_env_num
         dev = self.device
         if getattr(self, "_sp_scratch", None) is None:
@@ -157,7 +158,8 @@ class DeviceVecEnv:
         sc["scripted"][0, :, 0].copy_(torch.as_tensor(np.asarray(actions, dtype=np.float32).reshape(N)).to(dev))
         a = lib.OrlRolloutArgs()
         a.env_kind, a.n_envs, a.n_agents, a.episode_length = self.kind, N, 1, 1
-        a.t_begin, a.t_end, a.obs_dim, a.n_actions, a.activation_id, a.deterministic = 0, 1, 4, self.n_actions, 1, 2
+        a.t_begin, a.t_end, a.obs_dim, a.n_actions, a.deterministic = 0, 1, 4, self.n_actions, 2
+        a.activation_id = self.opponent_pool.activation_id   # the kernel evaluates the pool's snapshots with this activation
         a.policy_params, a.policy_obs = lib.ptr(sc["params"]), lib.ptr(sc["obs"])
         a.actions, a.action_log_probs, a.rewards = lib.ptr(sc["act"]), lib.ptr(sc["logp"]), lib.ptr(sc["rew"])
         a.masks, a.active_masks, a.exp_noise = lib.ptr(sc["masks"]), lib.ptr(sc["active"]), lib.ptr(sc["scripted"])

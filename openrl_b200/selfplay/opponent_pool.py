@@ -27,9 +27,14 @@ class OpponentPool:
         self.stats = torch.zeros(self.capacity + 1, 3, dtype=torch.int32, device=self.device)   # wins / losses / draws per slot; last row: random opponent
         self.count = 0          # host mirror of count_dev
         self.steps_of_slot = [None] * self.capacity
+        self.activation_id = 1  # hidden activation of the snapshots' policy (cfg.activation_id): the step API evaluates them with it
 
-    def add(self, flat_params, num_time_steps=None):
-        """SelfplayCallback.save_opponent: the learner's current parameters become the newest opponent."""
+    def add(self, flat_params, num_time_steps=None, activation_id=1):
+        """SelfplayCallback.save_opponent: the learner's current parameters become the newest opponent.  `activation_id` is
+        the policy's hidden activation; every snapshot of one pool shares it."""
+        if self.count > 0 and activation_id != self.activation_id:
+            raise ValueError(f"the pool holds snapshots of activation_id {self.activation_id}, not {activation_id}")
+        self.activation_id = int(activation_id)
         if self.capacity == 0:
             return
         slot = self.count % self.capacity

@@ -10,8 +10,9 @@ y+1}, -1 per step, +10 on the goal, -10 extra on the 100-step time-out) to two s
   * otherwise reward -1; when the episode has already taken 100 steps it ends as a draw with reward -1 - 10;
   * on episode end both players restart from the next entry of the start-cell table.
 
-The opponent-selection rules (RandomOpponent / LastOpponent, openrl/selfplay/sample_strategy/*.py) are restated by
-`pick_opponent_counts` for the statistical test."""
+The opponent-selection rules (RandomOpponent / LastOpponent, openrl/selfplay/sample_strategy/*.py), the Philox start
+cells and the policy-driven opponent are restated by the float64 replay of the whole rollout, tests/selfplay_ref64.py
+(`pick_opponent`, `reset_cells`, `SelfPlayReplay`), which takes its game rules from `_move` and the constants here."""
 import numpy as np
 
 ROWS = COLS = 10

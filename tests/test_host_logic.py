@@ -82,6 +82,22 @@ def test_missing_library_fails_loudly(tmp_path):
         lib.load(str(tmp_path / "nope.so"))
 
 
+def test_opponent_pool_records_the_snapshots_activation():
+    """The vec-env step API evaluates the pool with the activation its snapshots were trained with; one pool holds one."""
+    import torch
+
+    from openrl_b200.selfplay import OpponentPool
+
+    pool = OpponentPool(2, 10, device="cpu")
+    assert pool.activation_id == 1
+    for k in range(3):
+        pool.add(torch.full((10,), float(k)), activation_id=0)
+    assert pool.activation_id == 0 and pool.count == 3 and pool.params[0, 0] == 2.0
+    with pytest.raises(ValueError, match="activation_id"):
+        pool.add(torch.zeros(10), activation_id=3)
+    assert pool.count == 3
+
+
 def test_cpu_device_is_refused():
     """There is no CPU fallback: PPONet refuses non-CUDA devices before touching any kernel."""
     from openrl_b200 import spaces

@@ -227,10 +227,12 @@ def test_train_matches_reference_flag_variants(cuda, tag):
     np.testing.assert_allclose(b.returns.cpu().numpy()[:-1], d[f"it{iters - 1}/returns"][:-1], rtol=1e-5, atol=1e-5)
 
 
-@pytest.mark.parametrize("env_id,extra", [("CartPole-v1", []), ("GridWorldEnv", ["--num_mini_batch", "2"])])
+@pytest.mark.parametrize("env_id,extra", [("CartPole-v1", []), ("GridWorldEnv", ["--num_mini_batch", "2"]),
+                                          ("GridWorldSelfPlay", ["--selfplay_save_freq", "2"])])
 def test_cuda_graph_iterations_equal_eager_iterations(cuda, env_id, extra):
     """cfg.use_cuda_graph replays ONE captured graph per iteration (rollout + critic + GAE + updates + slot shift):
-    same launches, same device RNG counters -> bit-identical parameters, buffers and logged metrics."""
+    same launches, same device RNG counters -> bit-identical parameters, buffers and logged metrics.  Self-play: the
+    snapshots added to the opponent pool between iterations reach the graph's rollout as they reach the eager one."""
     import torch
 
     from openrl_b200.configs.config import create_config_parser
