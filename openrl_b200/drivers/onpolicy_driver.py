@@ -39,6 +39,7 @@ class OnPolicyDriver:
         self._lib = lib.load()
         self._global_step = 0
         self.rng_counter = torch.zeros(1, dtype=torch.int64, device=self.device)
+        self.host_act_steps = 0     # slots acted on by host-stepped rollouts: the Philox step of slot t is this + t
         self.gpu_launches = 0
         self.h2d_bytes = 0
         self.d2h_bytes = 0
@@ -281,18 +282,6 @@ class OnPolicyDriver:
         a.ep_return, a.ep_length, a.episode_stats = state("ep_return"), state("ep_length"), state("episode_stats")
         return a
 
-    def _rnn_act_rows(self, step, lo, hi, noise, rng_step_base=None):
-        """Recurrent policy act for envs [lo, hi) of slot `step` of a host-stepped rollout (orl_rnn_act_rows): actions,
-        log-probs and rnn_states[step + 1] of their rows.  The noise step is the device counter (advanced by one per call)
-        or, when given, `rng_step_base`."""
-        A = self.envs.agent_num
-        a = self._rnn_args(step, step + 1, noise)
-        a.row_begin, a.row_end = lo * A, hi * A
-        a.rng_row_offset = int(getattr(self.envs, "env_index_offset", 0)) * A
-        if rng_step_base is not None:
-            a.rng_step_base, a.rng_counter = rng_step_base, None
-        lib.check(self._lib.orl_rnn_act_rows(a, lib.current_stream()), "orl_rnn_act_rows")
-
     def _host_insert(self, staged, step, lo, hi, has_masks=False):
         """One host env.step of envs [lo, hi) into slot step + 1 (rewards: slot step): orl_host_insert, or
         orl_host_insert_rnn, which also zeroes rnn_states[step + 1] of the envs that finished.  With `has_masks` the
@@ -395,103 +384,63 @@ class OnPolicyDriver:
         return batch_rew_infos, cont
 
     def _host_rollout(self, cb):
-        """Per-step loop for host-stepped envs (onpolicy_driver.py:154-203): device act -> D2H actions
-        -> host env.step -> one pinned H2D copy -> in-place insert with the reference's mask rules
-        (add2buffer, onpolicy_driver.py:80-152)."""
+        """Per-step loop for host-stepped envs (onpolicy_driver.py:154-203): device act -> D2H actions -> host env.step
+        -> one pinned H2D copy -> in-place insert with the reference's mask rules (add2buffer, onpolicy_driver.py:80-152).
+        With `host_env_groups` (and no callback or parity noise) the envs run as two groups in ping-pong: while the host
+        steps one group, the device inserts the other group's results and acts on them for the next step; a group's
+        actions travel D2H asynchronously and are awaited (CUDA event) only when the host is ready to step that group."""
         d, env = self.buffer.data, self.envs
-        T, N, A = self.episode_length, env.parallel_env_num, env.agent_num
-        B = N * A
-        pol = self.trainer.algo_module.models["policy"]
-        w = d.actions.shape[-1]
-        if getattr(env, "supports_groups", False) and cb is None and not self.cfg.parity_mode and bool(getattr(self.cfg, "host_env_groups", True)):
-            return self._host_rollout_grouped()
-        for step in range(T):
-            noise = None
-            if self.cfg.parity_mode:
-                noise = torch.empty(B, d.n_actions, dtype=torch.float32)
-                noise.normal_() if pol.head_kind == lib.HEAD_GAUSSIAN else noise.exponential_(1)
-                noise = noise.to(self.device)
-                self.h2d_bytes += noise.numel() * 4
-            if self.recurrent:
-                with self._phase("rollout"):
-                    self._rnn_act_rows(step, 0, N, noise)
-            else:
-                a = lib.OrlRolloutArgs()
-                a.env_kind, a.n_envs, a.n_agents, a.episode_length = lib.ENV_NONE, B, 1, 1
-                a.t_begin, a.t_end = 0, 1
-                a.obs_dim, a.critic_obs_dim, a.n_actions = d.obs_dim, 0, d.n_actions
-                a.activation_id, a.deterministic, a.head_kind = pol.activation_id, 0, pol.head_kind
-                a.policy_params = lib.ptr(pol.flat_params)
-                a.policy_obs = lib.ptr(d.policy_obs[step])
-                a.actions, a.action_log_probs = lib.ptr(d.actions[step]), lib.ptr(d.action_log_probs[step])
-                a.action_masks = None if d.action_masks_trivial else lib.ptr(d.action_masks[step])
-                a.exp_noise = lib.ptr(noise)
-                a.rng_seed, a.rng_step_base, a.rng_counter = int(self.cfg.seed) + 0x9E3779B9 * (self.rank + 1), 0, lib.ptr(self.rng_counter)
-                with self._phase("rollout"):
-                    act_fn = self._lib.orl_share_rollout if getattr(self.trainer, "share", False) else self._lib.orl_rollout
-                    lib.check(act_fn(a, lib.current_stream()), "orl_rollout(act)")
-            self.gpu_launches += 2
-            staged, obs, rewards, dones, infos, has_masks = env.step_staged(d.actions[step].view(B, w))
-            self._host_insert(staged, step, 0, N, has_masks)
-            self.agent.num_time_steps += N
-            if cb is not None:
-                actions = d.actions[step].cpu().numpy()  # noqa: F841
-                cb.update_locals(locals())
-                if cb.on_step() is False:
-                    return False
-        return True
-
-    def _act_rows(self, step, lo, hi):
-        """Policy forward + sampling for the rows of envs [lo, hi) of slot `step` (orl_rollout, ORL_ENV_NONE; a recurrent
-        policy: orl_rnn_act_rows)."""
-        d = self.buffer.data
-        pol = self.trainer.algo_module.models["policy"]
-        A = self.envs.agent_num
-        r0, r1 = lo * A, hi * A
-        obs = d.policy_obs[step].view(-1, d.obs_dim)
-        w = d.actions.shape[-1]
-        acts, logp = d.actions[step].view(-1, w), d.action_log_probs[step].view(-1, w)
-        if self.recurrent:
-            self._rnn_act_rows(step, lo, hi, None, rng_step_base=self._host_steps_base + step)
-            self.gpu_launches += 1
-            return acts[r0:r1]
-        a = lib.OrlRolloutArgs()
-        a.env_kind, a.n_envs, a.n_agents, a.episode_length = lib.ENV_NONE, r1 - r0, 1, 1
-        a.t_begin, a.t_end = 0, 1
-        a.obs_dim, a.critic_obs_dim, a.n_actions = d.obs_dim, 0, d.n_actions
-        a.activation_id, a.deterministic, a.head_kind = pol.activation_id, 0, pol.head_kind
-        a.policy_params = lib.ptr(pol.flat_params)
-        a.policy_obs = lib.ptr(obs[r0:r1])
-        a.actions, a.action_log_probs = lib.ptr(acts[r0:r1]), lib.ptr(logp[r0:r1])
-        a.action_masks = None if d.action_masks_trivial else lib.ptr(d.action_masks[step].view(-1, d.n_actions)[r0:r1])
-        a.rng_seed, a.rng_step_base, a.rng_counter = int(self.cfg.seed) + 0x9E3779B9 * (self.rank + 1), self._host_steps_base + step, None
-        a.rng_row_offset = r0
-        act_fn = self._lib.orl_share_rollout if getattr(self.trainer, "share", False) else self._lib.orl_rollout
-        lib.check(act_fn(a, lib.current_stream()), "orl_rollout(act rows)")
-        self.gpu_launches += 1
-        return acts[r0:r1]
-
-    def _host_rollout_grouped(self):
-        """Host-stepped rollout with two env groups in ping-pong (double-buffered pinned staging): while the host steps
-        group g, the device inserts the other group's results and runs its policy forward for the next step; a group's
-        actions travel D2H asynchronously and are awaited (CUDA event) only when the host is ready to step that group.
-        Same per-step semantics as `_host_rollout` (add2buffer, onpolicy_driver.py:80-152)."""
-        env = self.envs
         T, N = self.episode_length, env.parallel_env_num
-        groups = env.group_bounds(2)
-        self._host_steps_base = getattr(self, "_host_steps_base", 0)   # Philox step of slot 0 of this rollout
+        grouped = getattr(env, "supports_groups", False) and cb is None and not self.cfg.parity_mode and bool(getattr(self.cfg, "host_env_groups", True))
+        groups = env.group_bounds(2) if grouped else [(0, N)]
         with self._phase("rollout"):
-            for g, (lo, hi) in enumerate(groups):       # prime: actions of step 0 for both groups
-                env.group_fetch_actions(g, lo, hi, self._act_rows(0, lo, hi))
+            noise = self._host_noise()
+            for lo, hi in groups:                       # prime: actions of step 0 for every group
+                env.fetch_actions(lo, hi, self._act(0, lo, hi, noise))
             for step in range(T):
                 for g, (lo, hi) in enumerate(groups):
-                    staged, *_, has_masks = env.group_step(g, lo, hi)   # host env.step of this group (device busy with the other)
+                    staged, obs, rewards, dones, infos, has_masks = env.step_staged(lo, hi)
                     self._host_insert(staged, step, lo, hi, has_masks)
+                    self.agent.num_time_steps += hi - lo
+                    if cb is not None:
+                        actions = d.actions[step].cpu().numpy()  # noqa: F841
+                        cb.update_locals(locals())
+                        if cb.on_step() is False:
+                            self.host_act_steps += step + 1
+                            return False
                     if step + 1 < T:
-                        env.group_fetch_actions(g, lo, hi, self._act_rows(step + 1, lo, hi))
-                self.agent.num_time_steps += N
-        self._host_steps_base += T
+                        if g == 0:
+                            noise = self._host_noise()
+                        env.fetch_actions(lo, hi, self._act(step + 1, lo, hi, noise))
+        self.host_act_steps += T
         return True
+
+    def _host_noise(self):
+        """cfg.parity_mode: one step's (B, n) noise from the global CPU generator, drawn as `_draw_noise` draws each step;
+        else None (Philox on the device)."""
+        if not self.cfg.parity_mode:
+            return None
+        d = self.buffer.data
+        noise = torch.empty(d.n_rollout_threads * d.num_agents, d.n_actions, dtype=torch.float32)
+        noise.normal_() if self.trainer.algo_module.models["policy"].head_kind == lib.HEAD_GAUSSIAN else noise.exponential_(1)
+        self.h2d_bytes += noise.numel() * 4
+        return noise.to(self.device)
+
+    def _act(self, step, lo, hi, noise):
+        """The policy act for envs [lo, hi) of slot `step` of a host-stepped rollout (PPOModule.act_rows): actions and
+        log-probs of their rows and, for a GRU policy, their rnn_states[step + 1].  The noise of a row is keyed by
+        (per-rank seed, host_act_steps + step, buffer row + env_index_offset * A).  Returns the actions of the rows."""
+        d, A = self.buffer.data, self.envs.agent_num
+        B, w = d.n_rollout_threads * A, d.actions.shape[-1]
+        acts = d.actions[step].view(B, w)
+        self.trainer.algo_module.act_rows(
+            d.policy_obs[step].view(B, d.obs_dim), acts, d.action_log_probs[step].view(B, w), lo * A, hi * A,
+            int(self.cfg.seed) + 0x9E3779B9 * (self.rank + 1), self.host_act_steps + step,
+            rng_row_offset=int(getattr(self.envs, "env_index_offset", 0)) * A,
+            action_masks=None if d.action_masks_trivial else d.action_masks[step].view(B, d.n_actions), noise=noise,
+            masks=d.masks[step], rnn_states=d.rnn_states[step:step + 2] if self.recurrent else None)
+        self.gpu_launches += 1
+        return acts[lo * A:hi * A]
 
     @torch.no_grad()
     def compute_returns(self):

@@ -46,15 +46,12 @@ class HostVecEnv:
         self.env_table, self.env_table_len = None, 0
         self.h2d_bytes = 0
         self.d2h_bytes = 0
-        N, A = self.parallel_env_num, self.agent_num
         if not hasattr(self.observation_space, "shape") or self.observation_space.shape is None:
             raise NotImplementedError("HostVecEnv stages flat Box observations; Dict observation spaces are not supported")
-        d = self.observation_space.shape[0]
-        self.obs_dim = d
+        self.obs_dim = self.observation_space.shape[0]
         self._discrete = hasattr(self.action_space, "n")
         # masks of Box action spaces are ignored, like the reference's buffer (replay_data.py:148-159)
         self.n_mask = int(self.action_space.n) if self._discrete else 0
-        self._stage = torch.empty(N * A * (d + 2 + self.n_mask), dtype=torch.float32, pin_memory=torch.cuda.is_available())
 
     def reset(self, seed=None, options=None):
         out = self.env.reset(seed=seed) if seed is not None else self.env.reset()
@@ -101,22 +98,7 @@ class HostVecEnv:
     def step(self, actions, extra_data=None):
         return self.env.step(actions)
 
-    def step_staged(self, actions_dev):
-        """actions (B, w) device tensor -> host env.step -> the device block [obs | rewards | dones (| masks)] (one pinned
-        H2D copy, the layout orl_host_insert reads) plus the host-side step outputs and whether the block carries the
-        envs' action masks (every env's info has `action_masks`): a 6-tuple (dev, obs, rewards, dones, infos, has_masks)."""
-        N, A = self.parallel_env_num, self.agent_num
-        a = actions_dev.cpu().numpy().reshape(N, A, -1)          # D2H (synchronises the stream)
-        self.d2h_bytes += a.nbytes
-        if self._discrete:                                       # the reference hands integer indices to env.step
-            a = a.astype(np.int64)
-        obs, rewards, dones, infos = self.env.step(a)
-        n, has_masks = self._stage_step(self._stage.numpy(), obs, rewards, dones, infos, N)
-        dev = self._stage[:n].to(self.device, non_blocking=True)      # one H2D copy
-        self.h2d_bytes += n * 4
-        return dev, obs, rewards, dones, infos, has_masks
-
-    # -- two-group ping-pong (double-buffered ingest) ---------------------------------------------
+    # -- staged stepping of an env range: the whole range, or one of the groups of the ping-pong loop ---------------
     @property
     def supports_groups(self):
         """True when the wrapped vec-env can step a sub-range of its envs (`step_range(lo, hi, actions)`)."""
@@ -127,46 +109,53 @@ class HostVecEnv:
         cuts = [N * g // n_groups for g in range(n_groups + 1)]
         return [(cuts[g], cuts[g + 1]) for g in range(n_groups)]
 
-    def _group_stage(self, g, lo, hi):
-        key = (g, lo, hi)
-        if getattr(self, "_gstages", None) is None:
-            self._gstages = {}
-        if key not in self._gstages:
+    def _range_stage(self, lo, hi):
+        """The staging of envs [lo, hi): pinned action and step buffers, the device block and the actions' event (a
+        CPU device copies synchronously and needs neither pinning nor events)."""
+        if getattr(self, "_stages", None) is None:
+            self._stages = {}
+        if (lo, hi) not in self._stages:
             n, A, w = hi - lo, self.agent_num, self.obs_dim + 2 + self.n_mask
-            pin = torch.cuda.is_available()
-            self._gstages[key] = dict(
-                inp=torch.empty(n * A * w, dtype=torch.float32, pin_memory=pin),     # obs | rewards | dones (| masks)
+            cuda = self.device.type == "cuda"
+            self._stages[lo, hi] = dict(
+                inp=torch.empty(n * A * w, dtype=torch.float32, pin_memory=cuda),     # obs | rewards | dones (| masks)
                 act=None, dev=torch.empty(n * A * w, dtype=torch.float32, device=self.device),
-                ev=torch.cuda.Event() if pin else None)
-        return self._gstages[key]
+                ev=torch.cuda.Event() if cuda else None)
+        return self._stages[lo, hi]
 
-    def group_fetch_actions(self, g, lo, hi, actions_dev):
-        """Enqueue the D2H copy of this group's actions into its pinned buffer and mark it with an event."""
-        st = self._group_stage(g, lo, hi)
+    def fetch_actions(self, lo, hi, actions_dev):
+        """Enqueue the D2H copy of the actions (rows, w) of envs [lo, hi) into their pinned buffer and mark it with an
+        event."""
+        st = self._range_stage(lo, hi)
         if st["act"] is None or st["act"].shape != actions_dev.shape:
-            st["act"] = torch.empty(actions_dev.shape, dtype=torch.float32, pin_memory=torch.cuda.is_available())
+            st["act"] = torch.empty(actions_dev.shape, dtype=torch.float32, pin_memory=st["ev"] is not None)
         st["act"].copy_(actions_dev, non_blocking=True)
         if st["ev"] is not None:
             st["ev"].record()
         self.d2h_bytes += actions_dev.numel() * 4
 
-    def group_step(self, g, lo, hi):
-        """Wait for the group's actions, step its envs on the host, stage the results in pinned memory and enqueue ONE
-        H2D copy; returns the device block [obs | rewards | dones (| masks)] (the layout orl_host_insert reads) plus the
-        host-side step outputs and whether the block carries masks (every env of the group reported them): a 6-tuple
+    def step_staged(self, lo, hi):
+        """Wait for the actions of envs [lo, hi) (`fetch_actions`), step them on the host (`env.step` for every env,
+        `env.step_range` for a sub-range), stage the results in pinned memory and enqueue ONE H2D copy.  Returns the device
+        block [obs | rewards | dones (| masks)] (the layout orl_host_insert reads), the host-side step outputs and whether
+        the block carries the envs' action masks (every stepped env's info has `action_masks`): a 6-tuple
         (dev, obs, rewards, dones, infos, has_masks)."""
-        st = self._group_stage(g, lo, hi)
+        st = self._range_stage(lo, hi)
         if st["ev"] is not None:
             st["ev"].synchronize()
-        n_envs, A = hi - lo, self.agent_num
-        a = st["act"].numpy().reshape(n_envs, A, -1)
-        if self._discrete:
+        n_envs = hi - lo
+        a = st["act"].numpy().reshape(n_envs, self.agent_num, -1)
+        if self._discrete:                                       # the reference hands integer indices to env.step
             a = a.astype(np.int64)
-        obs, rewards, dones, infos = self.env.step_range(lo, hi, a)
+        if n_envs == self.parallel_env_num:
+            obs, rewards, dones, infos = self.env.step(a)
+        else:
+            obs, rewards, dones, infos = self.env.step_range(lo, hi, a)
         n, has_masks = self._stage_step(st["inp"].numpy(), obs, rewards, dones, infos, n_envs)
-        st["dev"][:n].copy_(st["inp"][:n], non_blocking=True)
+        dev = st["dev"][:n]
+        dev.copy_(st["inp"][:n], non_blocking=True)
         self.h2d_bytes += n * 4
-        return st["dev"], obs, rewards, dones, infos, has_masks
+        return dev, obs, rewards, dones, infos, has_masks
 
     def random_action(self, infos=None):
         return np.array([[self.action_space.sample() for _ in range(self.agent_num)] for _ in range(self.parallel_env_num)])

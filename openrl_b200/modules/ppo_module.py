@@ -147,8 +147,9 @@ class PPOModule:
     def act(self, obs, rnn_states_actor=None, masks=None, action_masks=None, deterministic=False, exp_noise=None,
             rng_seed=None, rng_step=None):
         """PolicyNetwork.forward_original on a (rows, d) batch (ppo_module.py:195-210):
-        returns (actions (rows,1) float CUDA tensor, log-probs (rows,1)).
-        Stochastic calls draw Philox noise keyed by (cfg.seed, call counter): every call sees fresh noise
+        returns (actions (rows,1) float CUDA tensor, log-probs (rows,1)) and, for a GRU policy, the new rnn states
+        (rows, 1, H).  action_masks (rows, n) or None.
+        Stochastic calls draw Philox noise keyed by (cfg.seed, call counter, row): every call sees fresh noise
         (the reference samples from torch's advancing global generator)."""
         pol = self.models["policy"]
         if rng_seed is None:
@@ -156,58 +157,59 @@ class PPOModule:
         if rng_step is None:
             rng_step = self._act_calls
             self._act_calls += 1
-        obs = torch.as_tensor(obs, dtype=torch.float32).to(self.device).contiguous().view(-1, pol.obs_dim)
+        dev = lambda x: None if x is None else torch.as_tensor(x, dtype=torch.float32).to(self.device).contiguous()  # noqa: E731
+        obs = dev(obs).view(-1, pol.obs_dim)
         rows = obs.shape[0]
-        if getattr(pol, "recurrent", False):
-            return self._act_recurrent(pol, obs, rnn_states_actor, masks, action_masks, deterministic, exp_noise, rng_seed, rng_step)
         act_w = pol.n_actions if pol.head_kind == lib.HEAD_GAUSSIAN else 1
         actions = torch.empty(rows, act_w, dtype=torch.float32, device=self.device)
         logp = torch.empty(rows, act_w, dtype=torch.float32, device=self.device)
-        am = None if action_masks is None else torch.as_tensor(action_masks, dtype=torch.float32).to(self.device).contiguous()
-        noise = None if exp_noise is None else torch.as_tensor(exp_noise, dtype=torch.float32).to(self.device).contiguous()
-        a = lib.OrlRolloutArgs()
-        a.env_kind, a.n_envs, a.n_agents, a.episode_length = lib.ENV_NONE, rows, 1, 1
-        a.t_begin, a.t_end = 0, 1
-        a.obs_dim, a.critic_obs_dim, a.n_actions = pol.obs_dim, 0, pol.n_actions
-        a.activation_id, a.deterministic = pol.activation_id, int(bool(deterministic))
-        a.policy_params, a.policy_obs = lib.ptr(pol.flat_params), lib.ptr(obs)
-        a.actions, a.action_log_probs = lib.ptr(actions), lib.ptr(logp)
-        a.action_masks, a.exp_noise = lib.ptr(am), lib.ptr(noise)
-        a.rng_seed, a.rng_step_base = int(rng_seed), int(rng_step)
-        a.head_kind = pol.head_kind
-        if self.share_model:
-            lib.check(self._lib.orl_share_rollout(a, lib.current_stream()), "orl_share_rollout(act)")
-        else:
-            lib.check(self._lib.orl_rollout(a, lib.current_stream()), "orl_rollout(act)")
-        return actions, logp
-
-    def _act_recurrent(self, pol, obs, rnn_states_actor, masks, action_masks, deterministic, exp_noise, rng_seed, rng_step):
-        """One GRU policy step on a (rows, d) batch: returns (actions, log-probs, new rnn states (rows, 1, H))
-        (policy_network.py:130-162 with RNNLayer; orl_rnn_act_rows, the act of the host-stepped rollout, on slot 0 of
-        a one-step buffer: the noise of row r is keyed by (rng_seed, rng_step, r)).  action_masks (rows, n) or None."""
-        rows, H = obs.shape[0], pol.hidden_size
+        if not getattr(pol, "recurrent", False):
+            self.act_rows(obs, actions, logp, 0, rows, rng_seed, rng_step, action_masks=dev(action_masks), noise=dev(exp_noise),
+                          deterministic=deterministic)
+            return actions, logp
+        # one GRU step (policy_network.py:130-162 with RNNLayer) on a one-slot buffer: the new states land in slot 1
+        H = pol.hidden_size
         states = torch.zeros(2, rows, H, dtype=torch.float32, device=self.device)
         if rnn_states_actor is not None:
-            states[0].copy_(torch.as_tensor(rnn_states_actor, dtype=torch.float32).to(self.device).reshape(rows, H))
+            states[0].copy_(dev(rnn_states_actor).reshape(rows, H))
         mk = torch.ones(rows, dtype=torch.float32, device=self.device)
         if masks is not None:
-            mk.copy_(torch.as_tensor(masks, dtype=torch.float32).to(self.device).reshape(rows))
-        actions = torch.empty(rows, 1, dtype=torch.float32, device=self.device)
-        logp = torch.empty(rows, 1, dtype=torch.float32, device=self.device)
-        noise = None if exp_noise is None else torch.as_tensor(exp_noise, dtype=torch.float32).to(self.device).contiguous()
-        am = None if action_masks is None else torch.as_tensor(action_masks, dtype=torch.float32).to(self.device).contiguous()
-        a = lib.OrlRnnArgs()
-        a.env_kind, a.n_envs, a.n_agents, a.episode_length = lib.ENV_NONE, rows, 1, 1
-        a.t_begin, a.t_end, a.row_begin, a.row_end = 0, 1, 0, rows
-        a.obs_dim, a.critic_obs_dim, a.n_actions = pol.obs_dim, pol.obs_dim, pol.n_actions
+            mk.copy_(dev(masks).reshape(rows))
+        self.act_rows(obs, actions, logp, 0, rows, rng_seed, rng_step, action_masks=dev(action_masks), noise=dev(exp_noise),
+                      masks=mk, rnn_states=states, deterministic=deterministic)
+        return actions, logp, states[1].view(rows, 1, H)
+
+    def act_rows(self, obs, actions, log_probs, r0, r1, rng_seed, rng_step, rng_row_offset=0, action_masks=None, noise=None,
+                 masks=None, rnn_states=None, deterministic=False):
+        """The policy act on rows [r0, r1) of one slot, with no env step: orl_rollout / orl_share_rollout with
+        ORL_ENV_NONE, or orl_rnn_act_rows for a GRU policy.  obs (B, d), actions and log_probs (B, w), action_masks and
+        the noise table (B, n) or None are the slot's rows; a GRU policy also reads masks (B,) and rnn_states (2, B, H),
+        this slot's states and the next slot's, which it writes.  The noise of row r is keyed by
+        (rng_seed, rng_step, r + rng_row_offset)."""
+        pol = self.models["policy"]
+        recurrent = getattr(pol, "recurrent", False)
+        if not recurrent:   # the feed-forward act runs over every row it is handed
+            obs, actions, log_probs = obs[r0:r1], actions[r0:r1], log_probs[r0:r1]
+            action_masks = None if action_masks is None else action_masks[r0:r1]
+            noise = None if noise is None else noise[r0:r1]
+            rng_row_offset += r0
+        a = lib.OrlRnnArgs() if recurrent else lib.OrlRolloutArgs()
+        a.env_kind, a.n_envs, a.n_agents, a.episode_length, a.t_begin, a.t_end = lib.ENV_NONE, obs.shape[0], 1, 1, 0, 1
+        a.obs_dim, a.n_actions = pol.obs_dim, pol.n_actions
         a.activation_id, a.deterministic = pol.activation_id, int(bool(deterministic))
         a.policy_params, a.policy_obs = lib.ptr(pol.flat_params), lib.ptr(obs)
-        a.rnn_states, a.masks = lib.ptr(states), lib.ptr(mk)
-        a.actions, a.action_log_probs = lib.ptr(actions), lib.ptr(logp)
-        a.exp_noise, a.action_masks = lib.ptr(noise), lib.ptr(am)
-        a.rng_seed, a.rng_step_base, a.rng_counter, a.rng_row_offset = int(rng_seed), int(rng_step), None, 0
-        lib.check(self._lib.orl_rnn_act_rows(a, lib.current_stream()), "orl_rnn_act_rows(act)")
-        return actions, logp, states[1].view(rows, 1, H)
+        a.actions, a.action_log_probs = lib.ptr(actions), lib.ptr(log_probs)
+        a.action_masks, a.exp_noise = lib.ptr(action_masks), lib.ptr(noise)
+        a.rng_seed, a.rng_step_base, a.rng_counter, a.rng_row_offset = int(rng_seed), int(rng_step), None, int(rng_row_offset)
+        s = lib.current_stream()
+        if recurrent:   # reads the noise table by buffer row
+            a.critic_obs_dim, a.row_begin, a.row_end = pol.obs_dim, r0, r1
+            a.rnn_states, a.masks = lib.ptr(rnn_states), lib.ptr(masks)
+            lib.check(self._lib.orl_rnn_act_rows(a, s), "orl_rnn_act_rows")
+        else:
+            a.head_kind = pol.head_kind
+            act_fn = self._lib.orl_share_rollout if self.share_model else self._lib.orl_rollout
+            lib.check(act_fn(a, s), "orl_rollout(act)")
 
     @staticmethod
     def init_rnn_states(rollout_num, agent_num, rnn_layers, hidden_size):

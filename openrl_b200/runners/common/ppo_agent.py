@@ -63,6 +63,7 @@ class PPOAgent:
                               rank=self.rank, world_size=self.world_size, logger=logger, callback=callback)
         if prev is not None and prev.trainer is trainer:
             driver.rng_counter = prev.rng_counter  # keep the device noise stream moving forward
+            driver.host_act_steps = prev.host_act_steps   # and that of host-stepped rollouts
         self.driver = driver
         if callback is not None:
             callback.on_training_start(locals(), globals())

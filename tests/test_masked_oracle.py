@@ -95,9 +95,10 @@ def test_prepare_action_masks_rule():
     assert np.array_equal(prepare_action_masks([{"action_masks": [True, False, 2.5]}]), [[1, 0, 2]])
 
 
-def test_host_env_stages_masks_of_auto_reset_infos():
-    """HostVecEnv stages [obs | rewards | dones | masks] when every env reported masks, the auto-reset info's masks
-    for a finished env (the new episode's first observation), and reports their absence otherwise."""
+def test_host_env_stages_masks_of_auto_reset_infos_over_env_range():
+    """HostVecEnv's staged step of the whole env range stages [obs | rewards | dones | masks] when every env reported
+    masks, the auto-reset info's masks for a finished env (the new episode's first observation), and reports their
+    absence otherwise."""
     from masked_oracle import MaskedTargetVec
     from openrl_b200 import spaces
     from openrl_b200.envs.vec_env.host_venv import HostVecEnv
@@ -123,7 +124,8 @@ def test_host_env_stages_masks_of_auto_reset_infos():
     assert np.array_equal(am0.numpy(), np.stack([i["action_masks"] for i in inner.last_infos]))
     for t in range(6):
         acts = torch.tensor([[float(e.target)] for e in inner.envs])
-        dev, obs, rewards, dones, infos, has = env.step_staged(acts)
+        env.fetch_actions(0, N, acts)
+        dev, obs, rewards, dones, infos, has = env.step_staged(0, N)
         blk = dev.numpy()
         assert has == (t != 2)
         if not has:

@@ -88,20 +88,19 @@ def build(n, T, recurrent, grouped, masked=False):
     drv = agent.driver
     assert drv.recurrent == recurrent
     acts = []
-    if grouped:   # the act launches of the two-group loop: one per group and step
+    inner = drv._act   # the act launches: one per group and step
+
+    def timed(*a, **k):
         import torch
 
-        inner = drv._act_rows
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        out = inner(*a, **k)
+        e1.record()
+        acts.append((e0, e1))
+        return out
 
-        def timed(*a, **k):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            out = inner(*a, **k)
-            e1.record()
-            acts.append((e0, e1))
-            return out
-
-        drv._act_rows = timed
+    drv._act = timed
     return drv, acts
 
 
@@ -123,9 +122,6 @@ def iteration(drv, acts):
     for name, a, b in drv.phase_events:
         if name in ("critic", "update"):
             out[name] += a.elapsed_time(b)
-        elif name == "rollout" and not acts:   # the synchronous loop: the phase is the act launch
-            out["act"] += a.elapsed_time(b)
-            n_act += 1
     for a, b in acts:
         out["act"] += a.elapsed_time(b)
         n_act += 1
