@@ -10,7 +10,7 @@
 //   W1[64][d] b1 g1 be1 | W3[64][64] b3 g3 be3 | W5[64][64] b5 g5 be5 | W7[64][64] b7 g7 be7 | Wv[1][64] bv | Wa[n][64] ba
 // The backward writes a per-row "tape" of local gradients and forward activations; the parameter gradients are tape
 // reductions dW = sum_rows P^T Q / column sums, done by orl::reduce_tape (orl_tape.cu).
-// The widths, activations and LayerNorm are those of the recurrent core (orl_rnn_core.h).
+// The widths, activations, LayerNorm and the obs_prep trunk are those of the recurrent core (orl_rnn_core.h).
 #pragma once
 #include "orl_rnn_core.h"
 
@@ -32,6 +32,8 @@ using orl_rnn::act_fwd;
 using orl_rnn::act_bwd_from_out;
 using orl_rnn::layernorm64;
 using orl_rnn::layernorm64_bwd;
+using orl_rnn::linear64;
+using orl_rnn::linear64_bwd_data;
 
 struct Offsets {
     int d, n;
@@ -55,23 +57,6 @@ constexpr int TQ_X = 272, TQ_Y1 = 336, TQ_Y3 = 400, TQ_Y5 = 464, TQ_Y7 = 528;
 constexpr int TS_DY1N1 = 592, TS_DY1 = 656, TS_DY3N3 = 720, TS_DY3 = 784, TS_DY5N5 = 848, TS_DY5 = 912, TS_DY7N7 = 976, TS_DY7 = 1040;
 constexpr int TAPE = 1104;
 
-// y[j] = b[j] + sum_k W[j][k] x[k]   (64 x K, row-major)
-ORL_HD void linear64(const float* W, const float* b, const float* x, int K, float* y) {
-    for (int j = 0; j < H; ++j) {
-        float s = b[j];
-        for (int k = 0; k < K; ++k) s = fmaf(W[j * K + k], x[k], s);
-        y[j] = s;
-    }
-}
-// dx[k] = sum_j W[j][k] dz[j]
-ORL_HD void linear64_bwd_data(const float* W, const float* dz, float* dx) {
-    for (int k = 0; k < H; ++k) dx[k] = 0.f;
-    for (int j = 0; j < H; ++j) {
-        const float g = dz[j];
-        for (int k = 0; k < H; ++k) dx[k] = fmaf(W[j * H + k], g, dx[k]);
-    }
-}
-
 // what the backward needs from the forward of one row
 struct Save {
     float a1[H], n1[H], n3[H], a5[H], n5[H], n7[H];
@@ -82,26 +67,14 @@ struct Save {
 ORLD_STEP void deep_forward(const float* P, const Offsets& o, int act_id, const float* x, float* value, float* logits, Save* sv,
                             float* tape) {
     float a[H], nrm[H], y[H], z[H];
-    // obs_prep.fc1 -> act -> LN1
-    for (int j = 0; j < H; ++j) {
-        float s = P[o.b1 + j];
-        for (int k = 0; k < o.d; ++k) s = fmaf(P[o.w1 + j * o.d + k], x[k], s);
-        a[j] = act_fwd(s, act_id);
-    }
-    float r = layernorm64(a, nrm);
-    if (sv) { for (int j = 0; j < H; ++j) { sv->a1[j] = a[j]; sv->n1[j] = nrm[j]; } sv->rstd1 = r; }
-    for (int j = 0; j < H; ++j) y[j] = nrm[j] * P[o.g1 + j] + P[o.be1 + j];
-    if (tape) { for (int k = 0; k < MAXD; ++k) tape[TQ_X + k] = k < o.d ? x[k] : 0.f; for (int j = 0; j < H; ++j) tape[TQ_Y1 + j] = y[j]; }
-    // obs_prep.fc3 -> LN3
-    linear64(P + o.w3, P + o.b3, y, H, z);
-    r = layernorm64(z, nrm);
-    if (sv) { for (int j = 0; j < H; ++j) sv->n3[j] = nrm[j]; sv->rstd3 = r; }
-    for (int j = 0; j < H; ++j) y[j] = nrm[j] * P[o.g3 + j] + P[o.be3 + j];
-    if (tape) for (int j = 0; j < H; ++j) tape[TQ_Y3 + j] = y[j];
+    // obs_prep
+    orl_rnn::trunk_forward(P, o, act_id, x, y, sv ? sv->a1 : nullptr, sv ? sv->n1 : nullptr, tape ? tape + TQ_Y1 : nullptr,
+                           sv ? sv->n3 : nullptr, sv ? &sv->rstd1 : nullptr, sv ? &sv->rstd3 : nullptr);
+    if (tape) { for (int k = 0; k < MAXD; ++k) tape[TQ_X + k] = k < o.d ? x[k] : 0.f; for (int j = 0; j < H; ++j) tape[TQ_Y3 + j] = y[j]; }
     // common.fc1 -> act -> LN5
     linear64(P + o.w5, P + o.b5, y, H, z);
     for (int j = 0; j < H; ++j) a[j] = act_fwd(z[j], act_id);
-    r = layernorm64(a, nrm);
+    float r = layernorm64(a, nrm);
     if (sv) { for (int j = 0; j < H; ++j) { sv->a5[j] = a[j]; sv->n5[j] = nrm[j]; } sv->rstd5 = r; }
     for (int j = 0; j < H; ++j) y[j] = nrm[j] * P[o.g5 + j] + P[o.be5 + j];
     if (tape) for (int j = 0; j < H; ++j) tape[TQ_Y5 + j] = y[j];
@@ -147,16 +120,9 @@ ORLD_STEP void deep_backward(const float* P, const Offsets& o, int act_id, const
     for (int j = 0; j < H; ++j) { tape[TS_DY5N5 + j] = dy[j] * sv.n5[j]; tape[TS_DY5 + j] = dy[j]; dn[j] = dy[j] * P[o.g5 + j]; }
     layernorm64_bwd(dn, sv.n5, sv.rstd5, dz);
     for (int j = 0; j < H; ++j) { dz[j] *= act_bwd_from_out(sv.a5[j], act_id); tape[TP_DZ5 + j] = dz[j]; }
-    // fc5 -> y3 -> LN3
+    // fc5 -> y3 -> obs_prep
     linear64_bwd_data(P + o.w5, dz, dy);
-    for (int j = 0; j < H; ++j) { tape[TS_DY3N3 + j] = dy[j] * sv.n3[j]; tape[TS_DY3 + j] = dy[j]; dn[j] = dy[j] * P[o.g3 + j]; }
-    layernorm64_bwd(dn, sv.n3, sv.rstd3, dz);
-    for (int j = 0; j < H; ++j) tape[TP_DZ3 + j] = dz[j];
-    // fc3 -> y1 -> LN1 -> act
-    linear64_bwd_data(P + o.w3, dz, dy);
-    for (int j = 0; j < H; ++j) { tape[TS_DY1N1 + j] = dy[j] * sv.n1[j]; tape[TS_DY1 + j] = dy[j]; dn[j] = dy[j] * P[o.g1 + j]; }
-    layernorm64_bwd(dn, sv.n1, sv.rstd1, dz);
-    for (int j = 0; j < H; ++j) tape[TP_DZ1 + j] = dz[j] * act_bwd_from_out(sv.a1[j], act_id);
+    orl_rnn::trunk_backward<TP_DZ1, TP_DZ3, TS_DY1N1, TS_DY1, TS_DY3N3, TS_DY3>(P, o, act_id, sv, dy, tape);
 }
 
 }  // namespace orl_deep

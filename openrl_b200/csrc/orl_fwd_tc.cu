@@ -25,13 +25,12 @@ using namespace orl;
 using namespace orl::tc;
 
 constexpr int F_M = 128, F_NT = 256, FCW = 32;
-constexpr uint32_t FPANEL_W = H * 16;
 // Z3 staging tile: row pitch 68 floats (row-per-thread float4 reads are conflict-free)
 constexpr int S_LD = 68;
 // shared-memory carve of a forward kernel: n1 hi/lo panels of M1 rows | W3f hi/lo panels | staging tile of MS rows | small
 template <int M1, int MS>
 struct FwdLayout {
-    static constexpr uint32_t PANEL = M1 * 16, R1H = 0, R1L = 8 * PANEL, WH = 16 * PANEL, WL = WH + 8 * FPANEL_W, S = WL + 8 * FPANEL_W,
+    static constexpr uint32_t PANEL = M1 * 16, R1H = 0, R1L = 8 * PANEL, WH = 16 * PANEL, WL = WH + 8 * W_PANEL, S = WL + 8 * W_PANEL,
                               SMALL = S + MS * S_LD * 4;
 };
 using FLay = FwdLayout<F_M, F_M>;
@@ -64,7 +63,6 @@ struct FwdCtx {
 // carve shared memory, stage + fold the weights (fc3 matrix as split fp16); ends with a CTA barrier.
 template <typename L = FLay>
 __device__ __forceinline__ FwdCtx fwd_setup(uint8_t* smem, const float* __restrict__ params, int d, int n) {
-    const int tid = threadIdx.x, nt = blockDim.x;
     FwdCtx c;
     c.R1h = smem + L::R1H; c.R1l = smem + L::R1L;
     uint8_t* Wh = smem + L::WH; uint8_t* Wl = smem + L::WL;
@@ -72,28 +70,7 @@ __device__ __forceinline__ FwdCtx fwd_setup(uint8_t* smem, const float* __restri
     c.w1t = reinterpret_cast<float*>(smem + L::SMALL);
     c.b1s = c.w1t + 8 * H; c.b3f = c.b1s + H; c.whf = c.b3f + H; c.bhf = c.whf + MAX_OUT * H;
     c.xs = c.bhf + MAX_OUT; c.xh = c.xs + 2 * F_M * 2; c.xst = c.xh + 2 * F_M * 8;   // the 2-half layout of the exchange area
-    const NetOffsets po = net_offsets(d, n);
-    for (int i = tid; i < 8 * H; i += nt) { const int k = i / H, j = i % H; c.w1t[i] = (k < d) ? params[po.w1 + j * d + k] : 0.f; }
-    for (int i = tid; i < H; i += nt) c.b1s[i] = params[po.b1 + i];
-    for (int i = tid; i < H * 8; i += nt) {   // item = (panel p, row j): lanes own consecutive rows -> conflict-free 16-byte stores
-        const int pnl = i / H, j = i % H;
-        float w8[8];
-#pragma unroll
-        for (int c = 0; c < 8; ++c) w8[c] = params[po.w3 + j * H + 8 * pnl + c] * params[po.g1 + 8 * pnl + c];
-        const uint32_t off = (uint32_t)pnl * FPANEL_W + j * 16;
-        split_store8(Wh + off, Wl + off, w8, 1.0f);
-    }
-    for (int i = tid; i < MAX_OUT * H; i += nt) { const int j = i / H, k = i % H; c.whf[i] = (j < n) ? params[po.wh + j * H + k] * params[po.g3 + k] : 0.f; }
-    for (int j = tid; j < H; j += nt) {
-        float s = params[po.b3 + j];
-        for (int k = 0; k < H; ++k) s = fmaf(params[po.w3 + j * H + k], params[po.be1 + k], s);
-        c.b3f[j] = s;
-    }
-    for (int j = tid; j < MAX_OUT; j += nt) {
-        float s = 0.f;
-        if (j < n) { s = params[po.bh + j]; for (int k = 0; k < H; ++k) s = fmaf(params[po.wh + j * H + k], params[po.be3 + k], s); }
-        c.bhf[j] = s;
-    }
+    stage_weights_tc(c.w1t, Wh, Wl, params, d, n, blockDim.x);
     fence_proxy_async();
     __syncthreads();
     c.aR1h = smem_u32(c.R1h); c.aR1l = smem_u32(c.R1l); c.aWh = smem_u32(Wh); c.aWl = smem_u32(Wl);
@@ -146,7 +123,7 @@ __device__ __forceinline__ void fwd_tile(const FwdCtx& c, const float (&x)[8], i
     fence_proxy_async();
     __syncthreads();
     {   // Z3 = n1 . W3f^T: warpgroup `half` computes rows [64 half, +64)
-        const uint64_t dK_A = desc_const(FPANEL, 128), dK_W = desc_const(FPANEL_W, 128);
+        const uint64_t dK_A = desc_const(FPANEL, 128), dK_W = desc_const(W_PANEL, 128);
         float z[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) z[i] = 0.f;
@@ -156,7 +133,7 @@ __device__ __forceinline__ void fwd_tile(const FwdCtx& c, const float (&x)[8], i
             const uint32_t aa = (pass == 0 ? c.aR1l : c.aR1h) + half * 64 * 16, bb = pass == 1 ? c.aWl : c.aWh;
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk)
-                wgmma_f16_n64<0, 0>(z, desc_at(dK_A, aa + 2 * kk * FPANEL), desc_at(dK_W, bb + 2 * kk * FPANEL_W), (pass | kk) > 0);
+                wgmma_f16_n64<0, 0>(z, desc_at(dK_A, aa + 2 * kk * FPANEL), desc_at(dK_W, bb + 2 * kk * W_PANEL), (pass | kk) > 0);
         }
         wgmma_commit();
         overlap();
@@ -435,7 +412,7 @@ __global__ void __launch_bounds__(RowsCfg::NT, RowsCfg::MIN_CTAS) rollout_cartpo
             fence_proxy_async();
             RW_FWD_SYNC();
             {   // Z3 = n1 . W3f^T over R1 rows [0, 64), both 32-column halves b
-                const uint64_t dK_A = desc_const(C::L::PANEL, 128), dK_W = desc_const(FPANEL_W, 128);
+                const uint64_t dK_A = desc_const(C::L::PANEL, 128), dK_W = desc_const(W_PANEL, 128);
                 const int nb0 = (warp >> 2) * 2;   // 0: the forward threads are one warpgroup
                 float z[2][16];
 #pragma unroll
@@ -451,7 +428,7 @@ __global__ void __launch_bounds__(RowsCfg::NT, RowsCfg::MIN_CTAS) rollout_cartpo
 #pragma unroll
                         for (int b = 0; b < 2; ++b)
                             wgmma_f16_n32<0, 0>(z[b], desc_at(dK_A, aa + 2 * kk * C::L::PANEL),
-                                                desc_at(dK_W, bb + (nb0 + b) * 32 * 16 + 2 * kk * FPANEL_W), (pass | kk) > 0);
+                                                desc_at(dK_W, bb + (nb0 + b) * 32 * 16 + 2 * kk * W_PANEL), (pass | kk) > 0);
                 }
                 wgmma_commit();
                 wgmma_wait<0>();

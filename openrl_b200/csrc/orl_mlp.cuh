@@ -13,7 +13,8 @@
 // shared memory (W3f = W3*g1, b3f = b3 + W3.be1; Whf = Wh*g3, bhf = bh + Wh.be3), so tiles only
 // carry the normalised activations n1, n3.  The backward pass therefore produces "folded"
 // gradients (G1 = dZ1^T X, G3 = dZ3^T n1, GH = dL^T n3 and the bias sums); the finalize kernel
-// (orl_ppo.cu) unfolds them into the true parameter gradients.
+// (orl_ppo.cu) unfolds them into the true parameter gradients.  The fold and its inverse are written once,
+// below fold_offsets (folded_w3 ... folded_bh, unfolded_grad).
 //
 // A tile is M rows x 64 columns, activations row-major in shared memory with leading dimension
 // LDA = 68 floats.  Thread t of the NT-thread CTA owns columns 4*tx..4*tx+3 (tx = t % 16) of rows
@@ -50,6 +51,63 @@ __host__ __device__ inline FoldOffsets fold_offsets(int d, int n) {
     o.g1 = p; p += H * d;  o.db1 = p; p += H;  o.g3 = p; p += H * H;  o.db3 = p; p += H;
     o.gh = p; p += n * H;  o.dbh = p; p += n;  o.dls = p; p += n;  o.total = p;
     return o;
+}
+
+// The LayerNorm fold, one element of net `o` at a time: W3f[j][k] = W3[j][k] g1[k], b3f[j] = b3[j] + W3[j] . be1,
+// Whf[j][k] = Wh[j][k] g3[k] and bhf[j] = bh[j] + Wh[j] . be3 (both 0 for rows j >= n).  Every staging of folded
+// weights calls these, so every kernel sees the same bits.
+__device__ __forceinline__ float folded_w3(const float* P, const NetOffsets& o, int j, int k) { return P[o.w3 + j * H + k] * P[o.g1 + k]; }
+__device__ __forceinline__ float folded_b3(const float* P, const NetOffsets& o, int j) {
+    float s = P[o.b3 + j];
+    for (int k = 0; k < H; ++k) s = fmaf(P[o.w3 + j * H + k], P[o.be1 + k], s);
+    return s;
+}
+__device__ __forceinline__ float folded_wh(const float* P, const NetOffsets& o, int j, int k) {
+    return j < o.n ? P[o.wh + j * H + k] * P[o.g3 + k] : 0.f;
+}
+__device__ __forceinline__ float folded_bh(const float* P, const NetOffsets& o, int j) {
+    float s = 0.f;
+    if (j < o.n) {
+        s = P[o.bh + j];
+        for (int k = 0; k < H; ++k) s = fmaf(P[o.wh + j * H + k], P[o.be3 + k], s);
+    }
+    return s;
+}
+// The inverse: the true gradient of parameter i (net_offsets order) from the net's folded gradient vector f.
+__device__ __forceinline__ float unfolded_grad(const float* P, const NetOffsets& po, const FoldOffsets& fo, const float* f, int i) {
+    if (i < po.b1) return f[fo.g1 + (i - po.w1)];
+    if (i < po.g1) return f[fo.db1 + (i - po.b1)];
+    if (i < po.be1) {  // dg1[k] = sum_j W3[j][k] * G3[j][k]
+        const int k = i - po.g1; float s = 0.f;
+        for (int j = 0; j < H; ++j) s = fmaf(P[po.w3 + j * H + k], f[fo.g3 + j * H + k], s);
+        return s;
+    }
+    if (i < po.w3) {  // dbe1[k] = sum_j W3[j][k] * db3[j]
+        const int k = i - po.be1; float s = 0.f;
+        for (int j = 0; j < H; ++j) s = fmaf(P[po.w3 + j * H + k], f[fo.db3 + j], s);
+        return s;
+    }
+    if (i < po.b3) {  // dW3[j][k] = G3[j][k]*g1[k] + db3[j]*be1[k]
+        const int j = (i - po.w3) / H, k = (i - po.w3) % H;
+        return fmaf(f[fo.g3 + j * H + k], P[po.g1 + k], f[fo.db3 + j] * P[po.be1 + k]);
+    }
+    if (i < po.g3) return f[fo.db3 + (i - po.b3)];
+    if (i < po.be3) {
+        const int k = i - po.g3; float s = 0.f;
+        for (int j = 0; j < po.n; ++j) s = fmaf(P[po.wh + j * H + k], f[fo.gh + j * H + k], s);
+        return s;
+    }
+    if (i < po.wh) {
+        const int k = i - po.be3; float s = 0.f;
+        for (int j = 0; j < po.n; ++j) s = fmaf(P[po.wh + j * H + k], f[fo.dbh + j], s);
+        return s;
+    }
+    if (i < po.bh) {
+        const int j = (i - po.wh) / H, k = (i - po.wh) % H;
+        return fmaf(f[fo.gh + j * H + k], P[po.g3 + k], f[fo.dbh + j] * P[po.be3 + k]);
+    }
+    if (i < po.ls) return f[fo.dbh + (i - po.bh)];
+    return f[fo.dls + (i - po.ls)];
 }
 
 __host__ __device__ inline int pad4(int x) { return (x + 3) & ~3; }
@@ -93,28 +151,14 @@ __device__ inline void load_weights_folded(const SmemWeights& w, const float* __
     for (int i = tid; i < H; i += NT) w.b1[i] = params[o.b1 + i];
     for (int i = tid; i < H * H; i += NT) {
         const int j = i / H, k = i % H;  // coalesced read of W3[j][k]
-        const float v = params[o.w3 + i] * params[o.g1 + k];
+        const float v = folded_w3(params, o, j, k);
         w.w3t[k * H + j] = v;
         if (backward) w.w3n[i] = v;
     }
-    for (int i = tid; i < MAX_OUT * H; i += NT) {
-        const int j = i / H, k = i % H;
-        w.whf[i] = (j < n) ? params[o.wh + j * H + k] * params[o.g3 + k] : 0.f;
-    }
+    for (int i = tid; i < MAX_OUT * H; i += NT) w.whf[i] = folded_wh(params, o, i / H, i % H);
     // folded biases: one warp-sized group of threads per output
-    for (int j = tid; j < H; j += NT) {
-        float s = params[o.b3 + j];
-        for (int k = 0; k < H; ++k) s = fmaf(params[o.w3 + j * H + k], params[o.be1 + k], s);
-        w.b3f[j] = s;
-    }
-    for (int j = tid; j < MAX_OUT; j += NT) {
-        float s = 0.f;
-        if (j < n) {
-            s = params[o.bh + j];
-            for (int k = 0; k < H; ++k) s = fmaf(params[o.wh + j * H + k], params[o.be3 + k], s);
-        }
-        w.bhf[j] = s;
-    }
+    for (int j = tid; j < H; j += NT) w.b3f[j] = folded_b3(params, o, j);
+    for (int j = tid; j < MAX_OUT; j += NT) w.bhf[j] = folded_bh(params, o, j);
     __syncthreads();
 }
 

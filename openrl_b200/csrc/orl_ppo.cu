@@ -462,34 +462,7 @@ __global__ void __launch_bounds__(1024) ppo_apply_kernel(const OrlPpoArgs a, con
 
     float sq = 0.f;
     for (int i = tid; i < po.total; i += blockDim.x) {
-        float g;
-        if (i < po.b1) g = f[fo.g1 + (i - po.w1)];
-        else if (i < po.g1) g = f[fo.db1 + (i - po.b1)];
-        else if (i < po.be1) {  // dg1[k] = sum_j W3[j][k] * G3[j][k]
-            const int k = i - po.g1; float s = 0.f;
-            for (int j = 0; j < H; ++j) s = fmaf(params[po.w3 + j * H + k], f[fo.g3 + j * H + k], s);
-            g = s;
-        } else if (i < po.w3) {  // dbe1[k] = sum_j W3[j][k] * db3[j]
-            const int k = i - po.be1; float s = 0.f;
-            for (int j = 0; j < H; ++j) s = fmaf(params[po.w3 + j * H + k], f[fo.db3 + j], s);
-            g = s;
-        } else if (i < po.b3) {  // dW3[j][k] = G3[j][k]*g1[k] + db3[j]*be1[k]
-            const int j = (i - po.w3) / H, k = (i - po.w3) % H;
-            g = fmaf(f[fo.g3 + j * H + k], params[po.g1 + k], f[fo.db3 + j] * params[po.be1 + k]);
-        } else if (i < po.g3) g = f[fo.db3 + (i - po.b3)];
-        else if (i < po.be3) {
-            const int k = i - po.g3; float s = 0.f;
-            for (int j = 0; j < n; ++j) s = fmaf(params[po.wh + j * H + k], f[fo.gh + j * H + k], s);
-            g = s;
-        } else if (i < po.wh) {
-            const int k = i - po.be3; float s = 0.f;
-            for (int j = 0; j < n; ++j) s = fmaf(params[po.wh + j * H + k], f[fo.dbh + j], s);
-            g = s;
-        } else if (i < po.bh) {
-            const int j = (i - po.wh) / H, k = (i - po.wh) % H;
-            g = fmaf(f[fo.gh + j * H + k], params[po.g3 + k], f[fo.dbh + j] * params[po.be3 + k]);
-        } else if (i < po.ls) g = f[fo.dbh + (i - po.bh)];
-        else g = f[fo.dls + (i - po.ls)];
+        const float g = unfolded_grad(params, po, fo, f, i);
         grads[i] = g;
         sq = fmaf(g, g, sq);
     }

@@ -59,7 +59,6 @@ using namespace orl::tc;
 constexpr int T_M = 128, T_NT = 256;
 constexpr int CW = 32;                         // columns per thread
 constexpr uint32_t PANEL = T_M * 16;           // 8 fp16 features of 128 rows
-constexpr uint32_t PANEL_W = H * 16;
 constexpr int R1_PANELS = 10, R2_PANELS = 9, R3_PANELS = 8;
 constexpr int P_CST = 8, P_X = 9, P_U = 8;
 constexpr int N_LOSS_TC = 8;
@@ -68,8 +67,8 @@ constexpr int N_LOSS_TC = 8;
 constexpr int S_LD = 68, GA_LD = 84, GB_LD = 20;
 // shared-memory carve-up (bytes)
 constexpr uint32_t OFF_R1H = 0, OFF_R1L = OFF_R1H + R1_PANELS * PANEL, OFF_R2H = OFF_R1L + R1_PANELS * PANEL,
-                   OFF_R2L = OFF_R2H + R2_PANELS * PANEL, OFF_WH = OFF_R2L + R2_PANELS * PANEL, OFF_WL = OFF_WH + 8 * PANEL_W,
-                   OFF_R3H = OFF_WL + 8 * PANEL_W, OFF_R3L = OFF_R3H + R3_PANELS * PANEL,
+                   OFF_R2L = OFF_R2H + R2_PANELS * PANEL, OFF_WH = OFF_R2L + R2_PANELS * PANEL, OFF_WL = OFF_WH + 8 * W_PANEL,
+                   OFF_R3H = OFF_WL + 8 * W_PANEL, OFF_R3L = OFF_R3H + R3_PANELS * PANEL,
                    OFF_S = OFF_R3L + R3_PANELS * PANEL, OFF_STAGE = OFF_S + T_M * S_LD * 4;
 static_assert((T_M * GA_LD + 64 * GB_LD) * 4 <= OFF_WH, "the Ga / Gb staging fits in R1 + R2");
 static_assert(OFF_STAGE % 128 == 0, "TMA destination alignment");
@@ -132,28 +131,10 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     uint64_t* bar_st = reinterpret_cast<uint64_t*>(red + 3 * 8);  // TMA staging
 
     // ---- stage weights (folded); the fc3 matrix as split fp16 ----
-    for (int i = tid; i < 8 * H; i += T_NT) { const int k = i / H, j = i % H; w1t[i] = (k < d) ? params[po.w1 + j * d + k] : 0.f; }
-    for (int i = tid; i < H; i += T_NT) b1s[i] = params[po.b1 + i];
-    for (int i = tid; i < H * 8; i += T_NT) {   // item = (panel p, row j): lanes own consecutive rows -> conflict-free 16-byte stores
-        const int pnl = i / H, j = i % H;
-        float w8[8];
-#pragma unroll
-        for (int c = 0; c < 8; ++c) w8[c] = params[po.w3 + j * H + 8 * pnl + c] * params[po.g1 + 8 * pnl + c];
-        const uint32_t off = (uint32_t)pnl * PANEL_W + j * 16;
-        split_store8(Wh + off, Wl + off, w8, 1.0f);
-    }
-    for (int i = tid; i < MAX_OUT * H; i += T_NT) { const int j = i / H, k = i % H; whf[i] = (j < n) ? params[po.wh + j * H + k] * params[po.g3 + k] : 0.f; }
-    for (int j = tid; j < H; j += T_NT) {
-        float s = params[po.b3 + j];
-        for (int k = 0; k < H; ++k) s = fmaf(params[po.w3 + j * H + k], params[po.be1 + k], s);
-        b3f[j] = s;
-    }
-    for (int j = tid; j < MAX_OUT; j += T_NT) {
-        float s = 0.f;
-        if (j < n) { s = params[po.bh + j]; for (int k = 0; k < H; ++k) s = fmaf(params[po.wh + j * H + k], params[po.be3 + k], s); }
-        bhf[j] = s;
+    stage_weights_tc(w1t, Wh, Wl, params, d, n, T_NT);
+    for (int j = tid; j < MAX_OUT; j += T_NT) {   // from the parameters, not from the rounded whf
         float rs = 0.f;
-        if (j < n) for (int k = 0; k < H; ++k) rs += params[po.wh + j * H + k] * params[po.g3 + k];
+        if (j < n) for (int k = 0; k < H; ++k) rs += folded_wh(params, po, j, k);
         swh[j] = rs;
     }
     // panels that are read before their first per-tile write: zero them (U of lanes beyond n, X beyond d are rewritten per tile)
@@ -188,8 +169,8 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     const float invSz = exp2f(-(float)e_z), invSu = exp2f(-(float)e_u), invS1 = invSz * (1.f / K1);
 
     // ---- MMA descriptors (constant parts) ----
-    const uint64_t dK_A = desc_const(PANEL, 128), dK_W = desc_const(PANEL_W, 128);      // K-major
-    const uint64_t dMN_A = desc_const(128, PANEL), dMN_W = desc_const(128, PANEL_W);    // MN-major
+    const uint64_t dK_A = desc_const(PANEL, 128), dK_W = desc_const(W_PANEL, 128);      // K-major
+    const uint64_t dMN_A = desc_const(128, PANEL), dMN_W = desc_const(128, W_PANEL);    // MN-major
     const uint32_t aR1h = smem_u32(R1h), aR1l = smem_u32(R1l), aR2h = smem_u32(R2h), aR2l = smem_u32(R2l), aWh = smem_u32(Wh), aWl = smem_u32(Wl);
     const uint32_t aR3h = smem_u32(R3h), aR3l = smem_u32(R3l);
 
@@ -317,7 +298,7 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
             const uint32_t aa = (pass == 0 ? aR1l : aR1h) + wg * 64 * 16, bb = pass == 1 ? aWl : aWh;
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk)
-                wgmma_f16_n64<0, 0>(z, desc_at(dK_A, aa + 2 * kk * PANEL), desc_at(dK_W, bb + 2 * kk * PANEL_W), (pass | kk) > 0);
+                wgmma_f16_n64<0, 0>(z, desc_at(dK_A, aa + 2 * kk * PANEL), desc_at(dK_W, bb + 2 * kk * W_PANEL), (pass | kk) > 0);
         }
         wgmma_commit();   // the only group in flight
         if (TMA && tid == 0 && tile + G < n_tiles) issue_tma(tile + G);   // the staging buffer was consumed before the CTA barrier above
@@ -527,7 +508,7 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         for (int o = tid; o < n * H; o += T_NT) {
             const int j = o >> 6, k = o & 63;
             float acc = 0.f;
-            for (int i = 0; i < H; ++i) acc = fmaf(qs[j * H + i], params[po.w3 + k * H + i] * params[po.g1 + i], acc);
+            for (int i = 0; i < H; ++i) acc = fmaf(qs[j * H + i], folded_w3(params, po, k, i), acc);
             acc = fmaf(b3f[k], qsu[j], acc) - qsu[8 + j];
             part[fo.gh + o] = acc * invSu;
             if (k == 0) { part[fo.dbh + j] = qsu[16 + j] * invSu; part[fo.dls + j] = 0.f; }

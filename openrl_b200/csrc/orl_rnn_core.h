@@ -3,7 +3,8 @@
 // drives them through a tiny C shim and checks them against the torch oracle) and they are the element-wise
 // reference of the warp-cooperative step of orl_rnn_warp.cuh — so the numerics of the GRU path are verified
 // without a GPU.  The parameter offsets, the tape layout and the helpers are __host__ __device__: the warp path
-// and the shared-model core (orl_deep_core.h) use them.
+// and the shared-model core (orl_deep_core.h) use them, and the MLPBase trunk (trunk_forward / trunk_backward) is
+// also that of the shared-model core and of the self-play forward (orl_selfplay.cu).
 //
 // Network (reference: MLPBase mlp.py:100-176 -> RNNLayer rnn.py:5-99 (nn.GRU 64->64, 1 layer, then
 // LayerNorm) -> head: Categorical.linear act.py / v_out value_network.py:106-109):
@@ -73,6 +74,62 @@ ORL_HD void layernorm64_bwd(const float* dn, const float* n, float rstd, float* 
     s1 *= (1.f / H); s2 *= (1.f / H);
     for (int i = 0; i < H; ++i) dv[i] = rstd * (dn[i] - s1 - n[i] * s2);
 }
+// y[j] = b[j] + sum_k W[j][k] x[k]   (64 x K, row-major)
+ORL_HD void linear64(const float* W, const float* b, const float* x, int K, float* y) {
+    for (int j = 0; j < H; ++j) {
+        float s = b[j];
+        for (int k = 0; k < K; ++k) s = fmaf(W[j * K + k], x[k], s);
+        y[j] = s;
+    }
+}
+// dx[k] = sum_j W[j][k] dz[j]
+ORL_HD void linear64_bwd_data(const float* W, const float* dz, float* dx) {
+    for (int k = 0; k < H; ++k) dx[k] = 0.f;
+    for (int j = 0; j < H; ++j) {
+        const float g = dz[j];
+        for (int k = 0; k < H; ++k) dx[k] = fmaf(W[j * H + k], g, dx[k]);
+    }
+}
+
+// The MLPBase trunk of one row, x(d) -> fc1 -> act -> LN1 -> fc3 -> LN3 -> y3[64], of every sequential core and of the
+// self-play forward.  O: any offsets struct with d, w1, b1, g1, be1, w3, b3, g3, be3.  Writes a1 (the activation), n1,
+// y1 (= LN1 with affine), n3, rstd1 and rstd3 where the caller passes them.
+template <class O>
+ORL_HD void trunk_forward(const float* P, const O& o, int act_id, const float* x, float* y3, float* a1 = nullptr,
+                          float* n1 = nullptr, float* y1 = nullptr, float* n3 = nullptr, float* rstd1 = nullptr,
+                          float* rstd3 = nullptr) {
+    float a[H], nrm[H];
+    for (int j = 0; j < H; ++j) {
+        float s = P[o.b1 + j];
+        for (int k = 0; k < o.d; ++k) s = fmaf(P[o.w1 + j * o.d + k], x[k], s);
+        a[j] = act_fwd(s, act_id);
+    }
+    const float r1 = layernorm64(a, nrm);
+    if (a1) for (int j = 0; j < H; ++j) a1[j] = a[j];
+    if (n1) for (int j = 0; j < H; ++j) n1[j] = nrm[j];
+    if (rstd1) *rstd1 = r1;
+    for (int j = 0; j < H; ++j) y3[j] = nrm[j] * P[o.g1 + j] + P[o.be1 + j];   // y1, until fc3 has read it
+    if (y1) for (int j = 0; j < H; ++j) y1[j] = y3[j];
+    linear64(P + o.w3, P + o.b3, y3, H, a);
+    const float r3 = layernorm64(a, nrm);
+    if (n3) for (int j = 0; j < H; ++j) n3[j] = nrm[j];
+    if (rstd3) *rstd3 = r3;
+    for (int j = 0; j < H; ++j) y3[j] = nrm[j] * P[o.g3 + j] + P[o.be3 + j];
+}
+
+// Backward of the trunk from dy3 = dL/dy3, given the forward's saved a1, n1, n3, rstd1, rstd3 (fields of S).  Writes the
+// trunk's tape fields, whose offsets each core passes at compile time.
+template <int DZ1, int DZ3, int DY1N1, int DY1, int DY3N3, int DY3, class O, class S>
+ORL_HD void trunk_backward(const float* P, const O& o, int act_id, const S& sv, const float* dy3, float* tape) {
+    float dn[H], dz[H], dy[H];
+    for (int j = 0; j < H; ++j) { tape[DY3N3 + j] = dy3[j] * sv.n3[j]; tape[DY3 + j] = dy3[j]; dn[j] = dy3[j] * P[o.g3 + j]; }
+    layernorm64_bwd(dn, sv.n3, sv.rstd3, dz);
+    for (int j = 0; j < H; ++j) tape[DZ3 + j] = dz[j];
+    linear64_bwd_data(P + o.w3, dz, dy);
+    for (int j = 0; j < H; ++j) { tape[DY1N1 + j] = dy[j] * sv.n1[j]; tape[DY1 + j] = dy[j]; dn[j] = dy[j] * P[o.g1 + j]; }
+    layernorm64_bwd(dn, sv.n1, sv.rstd1, dz);
+    for (int j = 0; j < H; ++j) tape[DZ1 + j] = dz[j] * act_bwd_from_out(sv.a1[j], act_id);
+}
 
 // Saved forward state of one row-step (what the backward needs)
 struct StepSave {
@@ -84,22 +141,9 @@ struct StepSave {
 // `sv` may be NULL (rollout).  Also returns y1 / o through the tape pointer when given.
 static inline void rnn_step_forward(const float* P, const Offsets& o, int act_id, const float* x, const float* h_in, float mask,
                              float* h_out, float* out, StepSave* sv, float* tape) {
-    float a1[H], n1[H], y1[H], z3[H], n3[H], y3[H];
+    float a1[H], n1[H], y1[H], n3[H], y3[H], rstd1, rstd3;
     if (tape) for (int k = 0; k < MAXD; ++k) tape[TQ_X + k] = k < o.d ? x[k] : 0.f;
-    for (int j = 0; j < H; ++j) {
-        float s = P[o.b1 + j];
-        for (int k = 0; k < o.d; ++k) s = fmaf(P[o.w1 + j * o.d + k], x[k], s);
-        a1[j] = act_fwd(s, act_id);
-    }
-    const float rstd1 = layernorm64(a1, n1);
-    for (int j = 0; j < H; ++j) y1[j] = n1[j] * P[o.g1 + j] + P[o.be1 + j];
-    for (int j = 0; j < H; ++j) {
-        float s = P[o.b3 + j];
-        for (int k = 0; k < H; ++k) s = fmaf(P[o.w3 + j * H + k], y1[k], s);
-        z3[j] = s;
-    }
-    const float rstd3 = layernorm64(z3, n3);
-    for (int j = 0; j < H; ++j) y3[j] = n3[j] * P[o.g3 + j] + P[o.be3 + j];
+    trunk_forward(P, o, act_id, x, y3, a1, n1, y1, n3, &rstd1, &rstd3);
     float hm[H];
     for (int j = 0; j < H; ++j) hm[j] = h_in[j] * mask;
     float hraw[H], rr[H], zz[H], nn[H], ghn[H];
@@ -176,21 +220,7 @@ static inline void rnn_step_backward(const float* P, const Offsets& o, int act_i
         dh_prev[k] = (dhm[k] + t) * mask;
     }
     for (int g = 0; g < G3; ++g) { tape[TP_DGI + g] = dgi[g]; tape[TP_DGH + g] = dgh[g]; }
-    float dn3[H], dz3[H];
-    for (int k = 0; k < H; ++k) { dn3[k] = dy3[k] * P[o.g3 + k]; tape[TS_DY3N3 + k] = dy3[k] * sv.n3[k]; tape[TS_DY3 + k] = dy3[k]; }
-    layernorm64_bwd(dn3, sv.n3, sv.rstd3, dz3);
-    float dy1[H], dn1[H], da1[H];
-    for (int k = 0; k < H; ++k) {
-        float s = 0.f;
-        for (int j = 0; j < H; ++j) s = fmaf(P[o.w3 + j * H + k], dz3[j], s);
-        dy1[k] = s;
-        dn1[k] = s * P[o.g1 + k];
-        tape[TS_DY1N1 + k] = s * sv.n1[k];
-        tape[TS_DY1 + k] = s;
-        tape[TP_DZ3 + k] = dz3[k];
-    }
-    layernorm64_bwd(dn1, sv.n1, sv.rstd1, da1);
-    for (int k = 0; k < H; ++k) tape[TP_DZ1 + k] = da1[k] * act_bwd_from_out(sv.a1[k], act_id);
+    trunk_backward<TP_DZ1, TP_DZ3, TS_DY1N1, TS_DY1, TS_DY3N3, TS_DY3>(P, o, act_id, sv, dy3, tape);
     for (int j = 0; j < MAXN; ++j) tape[TP_DLOG + j] = j < o.n ? dlogit[j] : 0.f;
 }
 

@@ -21,41 +21,19 @@
 // episode start the env draws its opponent: uniform over the pool (RandomOpponent) or the newest snapshot (LastOpponent);
 // with an empty pool the opponent acts uniformly at random (opponent_pool_wrapper.py:70-81).
 #include "orl_envstep.cuh"
+#include "orl_rnn_core.h"
 
 namespace {
 using namespace orl;
 
 constexpr int SP_NT = 128, SP_ROWS = 10, SP_COLS = 10, SP_MAX_STEPS = 100;
 
-// 64-wide 2-layer MLP policy forward of one row from the flat parameter layout (net_offsets): logits[n]
-__device__ __noinline__ void sp_policy_logits(const float* __restrict__ P, int n, int activation_id, const float (&x)[4], float* logits) {
+// policy forward of one row (net_offsets layout): logits[n].  A real call: the kernel keeps one call frame instead of
+// inlining both forwards.
+__device__ __noinline__ void sp_forward(const float* __restrict__ P, int n, int activation_id, const float (&x)[4], float* logits) {
     const NetOffsets o = net_offsets(4, n);
-    float a[H], y[H];
-    for (int j = 0; j < H; ++j) {
-        float s = P[o.b1 + j];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) s = fmaf(P[o.w1 + j * 4 + k], x[k], s);
-        a[j] = act_fwd(s, activation_id);
-    }
-    float m = 0.f;
-    for (int j = 0; j < H; ++j) m += a[j];
-    m *= (1.f / H);
-    float q = 0.f;
-    for (int j = 0; j < H; ++j) { const float d = a[j] - m; q += d * d; }
-    float r = 1.f / sqrtf(q * (1.f / H) + LN_EPS);
-    for (int j = 0; j < H; ++j) y[j] = (a[j] - m) * r * P[o.g1 + j] + P[o.be1 + j];
-    for (int j = 0; j < H; ++j) {
-        float s = P[o.b3 + j];
-        for (int k = 0; k < H; ++k) s = fmaf(P[o.w3 + j * H + k], y[k], s);
-        a[j] = s;
-    }
-    m = 0.f;
-    for (int j = 0; j < H; ++j) m += a[j];
-    m *= (1.f / H);
-    q = 0.f;
-    for (int j = 0; j < H; ++j) { const float d = a[j] - m; q += d * d; }
-    r = 1.f / sqrtf(q * (1.f / H) + LN_EPS);
-    for (int j = 0; j < H; ++j) y[j] = (a[j] - m) * r * P[o.g3 + j] + P[o.be3 + j];
+    float y[H];
+    orl_rnn::trunk_forward(P, o, activation_id, x, y);
     for (int j = 0; j < n; ++j) {
         float s = P[o.bh + j];
         for (int k = 0; k < H; ++k) s = fmaf(P[o.wh + j * H + k], y[k], s);
@@ -134,7 +112,7 @@ __global__ void __launch_bounds__(SP_NT) selfplay_rollout_kernel(const OrlSelfPl
         // Philox lanes of (step, env_key): 0/1 learner, 2/3 opponent policy, 4 random opponent
         const float xl[4] = {(float)x0, (float)y0, (float)x1, (float)y1};
         float logits[MAX_OUT], lp;
-        sp_policy_logits(a.policy_params, n, a.activation_id, xl, logits);
+        sp_forward(a.policy_params, n, a.activation_id, xl, logits);
         int act0 = sample_action(logits, n, nullptr, a.deterministic & 1, [&](float (&q)[MAX_OUT]) {
             action_noise(nullptr, 0, n, a.rng_seed, step, (uint32_t)env_key, q);
         }, lp);
@@ -151,7 +129,7 @@ __global__ void __launch_bounds__(SP_NT) selfplay_rollout_kernel(const OrlSelfPl
         } else if (opp >= 0) {
             const float xo[4] = {(float)x1, (float)y1, (float)x0, (float)y0};
             float lo[MAX_OUT], lpo;
-            sp_policy_logits(s.pool_params + (size_t)opp * s.pool_stride, n, a.activation_id, xo, lo);
+            sp_forward(s.pool_params + (size_t)opp * s.pool_stride, n, a.activation_id, xo, lo);
             act1 = sample_action(lo, n, nullptr, false, [&](float (&q)[MAX_OUT]) {
                 action_noise(nullptr, 0, n, a.rng_seed, step, (uint32_t)env_key, q, 2u);
             }, lpo);

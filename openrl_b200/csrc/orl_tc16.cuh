@@ -18,10 +18,13 @@
 #pragma once
 #include <cuda_fp16.h>
 
+#include "orl_mlp.cuh"
 #include "orl_tc.cuh"
 
 namespace orl {
 namespace tc {
+
+constexpr uint32_t W_PANEL = H * 16;   // one panel of the W3f hi / lo buffers: 8 features of the 64 fc3 output rows
 
 // wgmma descriptor = constant part (LBO, SBO; layout type 0 = no swizzle) | start address
 __device__ __forceinline__ uint64_t desc_const(uint32_t lbo_bytes, uint32_t sbo_bytes) {
@@ -45,6 +48,29 @@ __device__ __forceinline__ void split_store8(uint8_t* hi_unit, uint8_t* lo_unit,
     split2(v[6] * scale, v[7] * scale, h.w, l.w);
     *reinterpret_cast<uint4*>(hi_unit) = h;
     *reinterpret_cast<uint4*>(lo_unit) = l;
+}
+
+// Stage one net's folded weights for the tensor-core kernels; all nt threads of the CTA call it, no barrier.  Writes the
+// fp32 block w1t[8][64] (k-major, zero padded) b1[64] b3f[64] whf[8][64] bhf[8] at `small`, and W3f as 8 split-fp16
+// panels of 64 rows at Wh / Wl.
+__device__ __forceinline__ void stage_weights_tc(float* small, uint8_t* Wh, uint8_t* Wl, const float* __restrict__ params, int d, int n,
+                                                 int nt) {
+    const int tid = threadIdx.x;
+    const NetOffsets po = net_offsets(d, n);
+    float* w1t = small; float* b1 = w1t + 8 * H; float* b3f = b1 + H; float* whf = b3f + H; float* bhf = whf + MAX_OUT * H;
+    for (int i = tid; i < 8 * H; i += nt) { const int k = i / H, j = i % H; w1t[i] = (k < d) ? params[po.w1 + j * d + k] : 0.f; }
+    for (int i = tid; i < H; i += nt) b1[i] = params[po.b1 + i];
+    for (int i = tid; i < H * 8; i += nt) {   // item = (panel p, row j): lanes own consecutive rows -> conflict-free 16-byte stores
+        const int pnl = i / H, j = i % H;
+        float w8[8];
+#pragma unroll
+        for (int c = 0; c < 8; ++c) w8[c] = folded_w3(params, po, j, 8 * pnl + c);
+        const uint32_t off = (uint32_t)pnl * W_PANEL + j * 16;
+        split_store8(Wh + off, Wl + off, w8, 1.0f);
+    }
+    for (int i = tid; i < MAX_OUT * H; i += nt) whf[i] = folded_wh(params, po, i / H, i % H);
+    for (int j = tid; j < H; j += nt) b3f[j] = folded_b3(params, po, j);
+    for (int j = tid; j < MAX_OUT; j += nt) bhf[j] = folded_bh(params, po, j);
 }
 
 // ---- TMA (cp.async.bulk.tensor) + mbarrier transaction accounting ----
