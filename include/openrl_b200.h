@@ -456,14 +456,21 @@ int orl_selfplay_rollout(const OrlSelfPlayArgs* args, void* stream);
  * gradients, clip_grad_norm_ over all parameters twice, ONE Adam step with lr = cfg.lr).
  * Parameter layout (named_parameters order of the reference):
  *   W1[64][d] b1 g1 be1 | W3[64][64] b3 g3 be3 | W5[64][64] b5 g5 be5 | W7[64][64] b7 g7 be7 | Wv[1][64] bv | Wa[n][64] ba
- * Discrete heads, single-agent device envs (or ORL_ENV_NONE).  OrlRolloutArgs.policy_params = the shared model.
+ *   then, for a DiagGaussian head, logstd[n] (act.action_out.logstd._bias).
+ * head_kind ORL_HEAD_CATEGORICAL: Discrete(n) actions, single-agent device envs or ORL_ENV_NONE.  ORL_HEAD_GAUSSIAN:
+ * Box(n <= 8) actions, ORL_ENV_NONE only (host-stepped envs); actions / log-probs are (rows, n), no action masks.
+ * OrlRolloutArgs.policy_params = the shared model.
  * OrlPpoArgs for the shared model: policy_params / policy_adam_* / lrs[0] / adam_steps[0] = the shared model and its
  * optimiser, partials = workspace of orl_share_workspace_floats() floats, grads = true gradients (>= parameter count),
  * folded = 8 floats of loss sums; critic_* fields are ignored.  With > 1 GPU the caller SUM-all-reduces `grads` and
- * `folded[0..3]` between orl_share_fwdbwd and orl_share_apply. */
+ * `folded[0..3]` between orl_share_fwdbwd and orl_share_apply.
+ * orl_share_param_count / orl_share_tape_width / orl_share_workspace_floats are the Categorical head's; the _head
+ * variants take the head kind. */
 int orl_share_param_count(int obs_dim, int n_actions);
+int orl_share_param_count_head(int obs_dim, int n_actions, int head_kind);
 int orl_share_tape_width(void);
 long long orl_share_workspace_floats(long long rows, int obs_dim, int n_actions);
+long long orl_share_workspace_floats_head(long long rows, int obs_dim, int n_actions, int head_kind);
 int orl_share_rollout(const OrlRolloutArgs* args, void* stream);
 int orl_share_values(const float* params, int obs_dim, int n_actions, int activation_id, const float* obs, float* values,
                      long long rows, void* stream);

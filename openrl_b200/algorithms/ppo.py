@@ -74,7 +74,7 @@ class PPOAlgorithm:
                 raise NotImplementedError("use_share_model with recurrent policies is not built")
             self.use_tensor_cores = False
             self.flags &= ~lib.PPO_TENSORCORE
-            self.share_total = int(self._lib.orl_share_param_count(self.d, self.n))
+            self.share_total = int(self._lib.orl_share_param_count_head(self.d, self.n, self.head_kind))
             self.share_bucket = torch.zeros(((self.share_total + 3) & ~3) + 8, dtype=torch.float32, device=dev)
             self.share_grads = self.share_bucket[:(self.share_total + 3) & ~3]
             self.share_loss = self.share_bucket[(self.share_total + 3) & ~3:]
@@ -160,7 +160,7 @@ class PPOAlgorithm:
     def _share_update(self, buf, batch_rows, indices, row_begin, mb_stats):
         """One minibatch update of the shared policy-value network (ppo.py:46-176 with `_use_share_model`)."""
         L, s = self._lib, lib.current_stream()
-        need = int(L.orl_share_workspace_floats(int(batch_rows), self.d, self.n))
+        need = int(L.orl_share_workspace_floats_head(int(batch_rows), self.d, self.n, self.head_kind))
         if self.share_ws is None or self.share_ws.numel() < need:
             self.share_ws = torch.empty(need, dtype=torch.float32, device=self.device)
         a = self._args(buf, batch_rows, indices, row_begin)

@@ -26,7 +26,7 @@ int allow_dynamic_smem(K* kernel, size_t smem_bytes, bool max_carveout = false) 
 // A job reads columns of the `tape_width`-float tape rows: a gemm job writes sum_rows tape[p_off + m] * tape[q_off + k]
 // (m < M, k < N) to grads[out_off + m*N + k], a column job sum_rows tape[p_off + m] (m < M) to grads[out_off + m].
 struct TapeJob { int p_off, M, q_off, N, out_off; };
-constexpr int TAPE_MAX_GEMM_JOBS = 6, TAPE_MAX_COL_JOBS = 14;   // the shared model's tables (the GRU's: 5 and 11)
+constexpr int TAPE_MAX_GEMM_JOBS = 6, TAPE_MAX_COL_JOBS = 15;   // the shared model's tables with a Gaussian head (the GRU's: 5 and 11)
 struct TapeJobs { TapeJob gemm[TAPE_MAX_GEMM_JOBS]; TapeJob col[TAPE_MAX_COL_JOBS]; int n_gemm, n_col; };
 constexpr int TAPE_ROW_BLOCK = 1024;   // tape rows per partial result: partials hold ceil(rows / TAPE_ROW_BLOCK) x stride floats
 // grads[0, total) = the jobs over tape rows [0, rows), summed per row block into partials and then over the row blocks

@@ -5,9 +5,12 @@
 //
 // Network:  x(d) -> obs_prep = MLPBase: fc1 -> act -> LN1 -> fc3 -> LN3          (mlp.py:100-176, layer_N = 1)
 //                -> common   = MLPLayer(64, 64, layer_N = 0): fc5 -> act -> LN5 -> fc7 -> LN7   (mlp.py:8-46)
-//                -> { v_out: Linear(64, 1),  act.action_out.linear: Linear(64, n) }
+//                -> { v_out: Linear(64, 1),  act: Categorical linear / DiagGaussian fc_mean Linear(64, n) }
 // Flat parameter layout (named_parameters order of the reference; `critic_obs_prep` aliases `obs_prep`):
 //   W1[64][d] b1 g1 be1 | W3[64][64] b3 g3 be3 | W5[64][64] b5 g5 be5 | W7[64][64] b7 g7 be7 | Wv[1][64] bv | Wa[n][64] ba
+//   and, for a DiagGaussian head (Box(n) actions), logstd[n] (act.action_out.logstd._bias, shape (n, 1)) after ba.
+// The head output is the logits of a Categorical head and the mean of a DiagGaussian one; the dL/dlogstd of a row is
+// the loss's business (orl_loss.cuh gaussian_row), kept in the tape field TS_DLS of the Gaussian tape.
 // The backward writes a per-row "tape" of local gradients and forward activations; the parameter gradients are tape
 // reductions dW = sum_rows P^T Q / column sums, done by orl::reduce_tape (orl_tape.cu).
 // The widths, activations, LayerNorm and the obs_prep trunk are those of the recurrent core (orl_rnn_core.h).
@@ -39,7 +42,7 @@ struct Offsets {
     int d, n;
     int w1, b1, g1, be1, w3, b3, g3, be3, w5, b5, g5, be5, w7, b7, g7, be7, wv, bv, wa, ba, total;
 };
-ORL_HD Offsets deep_offsets(int d, int n) {
+ORL_HD Offsets deep_offsets(int d, int n, bool gaussian = false) {
     Offsets o; o.d = d; o.n = n; int p = 0;
     o.w1 = p; p += H * d; o.b1 = p; p += H; o.g1 = p; p += H; o.be1 = p; p += H;
     o.w3 = p; p += H * H; o.b3 = p; p += H; o.g3 = p; p += H; o.be3 = p; p += H;
@@ -47,15 +50,21 @@ ORL_HD Offsets deep_offsets(int d, int n) {
     o.w7 = p; p += H * H; o.b7 = p; p += H; o.g7 = p; p += H; o.be7 = p; p += H;
     o.wv = p; p += H; o.bv = p; p += 1;
     o.wa = p; p += n * H; o.ba = p; p += n;
+    if (gaussian) p += n;   // logstd
     o.total = p;
     return o;
 }
+// logstd[n] of a DiagGaussian head: right after ba
+ORL_HD int logstd_offset(const Offsets& o) { return o.ba + o.n; }
 
 // tape layout of one row (floats).  P operands (local gradients), Q operands (layer inputs), S column-sum fields.
 constexpr int TP_DZ1 = 0, TP_DZ3 = 64, TP_DZ5 = 128, TP_DZ7 = 192, TP_DLOG = 256, TP_DV = 264;
 constexpr int TQ_X = 272, TQ_Y1 = 336, TQ_Y3 = 400, TQ_Y5 = 464, TQ_Y7 = 528;
 constexpr int TS_DY1N1 = 592, TS_DY1 = 656, TS_DY3N3 = 720, TS_DY3 = 784, TS_DY5N5 = 848, TS_DY5 = 912, TS_DY7N7 = 976, TS_DY7 = 1040;
 constexpr int TAPE = 1104;
+// DiagGaussian head: the same fields, then the row's dL/dlogstd[8] (zero beyond n), column-summed into logstd
+constexpr int TS_DLS = 1104, TAPE_GAUSSIAN = 1112;
+ORL_HD constexpr int tape_width(bool gaussian) { return gaussian ? TAPE_GAUSSIAN : TAPE; }
 
 // what the backward needs from the forward of one row
 struct Save {

@@ -225,4 +225,38 @@ __device__ __forceinline__ int sample_action(float (&logit)[MAX_OUT], int n, con
     return act;
 }
 
+// DiagGaussian act of one row (distributions.py:75-98): action = noise * std + mean (the mean when deterministic) and
+// the per-dimension log-probs, written to actions / log_probs [grow * n + j].  The N(0, 1) noise is the reference-order
+// table noise_table[grow * n + j] when one is given (parity mode), else Box-Muller over Philox lanes 2..5 of
+// (step, row): 8 normals from the 16 uniforms of the lane pairs (2, 3) and (4, 5).
+__device__ __forceinline__ void gaussian_act(const float (&mean)[MAX_OUT], int n, const float* logstd, bool deterministic,
+                                             const float* noise_table, uint64_t seed, uint64_t step, uint32_t row, size_t grow,
+                                             float* actions, float* log_probs) {
+    uint32_t rr[8];
+    if (!noise_table && !deterministic) {
+        const uint4 r0 = action_philox(seed, step, row, 2u), r1 = action_philox(seed, step, row, 3u);
+        const uint4 r2 = action_philox(seed, step, row, 4u), r3 = action_philox(seed, step, row, 5u);
+        const uint32_t u1[8] = {r0.x, r0.y, r0.z, r0.w, r2.x, r2.y, r2.z, r2.w};
+        const uint32_t u2[8] = {r1.x, r1.y, r1.z, r1.w, r3.x, r3.y, r3.z, r3.w};
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float rad = sqrtf(-2.0f * logf(u32_to_unit_open(u1[j])));
+            rr[j] = __float_as_uint(rad * cospif(2.0f * u32_to_unit_open(u2[j])));
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < MAX_OUT; ++j) {
+        if (j < n) {
+            const float ls = logstd[j], std = expf(ls);
+            float act = mean[j];
+            if (!deterministic) {
+                const float eps = noise_table ? noise_table[grow * n + j] : __uint_as_float(rr[j]);
+                act = __fadd_rn(__fmul_rn(eps, std), mean[j]);
+            }
+            actions[grow * n + j] = act;
+            log_probs[grow * n + j] = gaussian_log_prob(act - mean[j], std, ls);
+        }
+    }
+}
+
 }  // namespace orl

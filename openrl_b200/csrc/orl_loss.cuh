@@ -2,8 +2,8 @@
 // and policy_eval_kernel share with the updates, the DiagGaussian log-prob and entropy of policy_eval_kernel and the
 // FFMA update, and the per-minibatch constants, categorical row loss and value row loss of every update kernel
 // (ppo_net_pass in orl_ppo.cu, tc_net_pass in orl_ppo_tc.cu, the chunk and JRPO kernels of orl_rnn.cu,
-// share_fwdbwd_kernel in orl_share.cu).  The DiagGaussian row loss is ppo_net_pass's alone: Box action spaces run the
-// FFMA update only.
+// share_fwdbwd_kernel in orl_share.cu).  The DiagGaussian row loss serves ppo_net_pass (the FFMA update) and the
+// shared model's share_fwdbwd_kernel: Box action spaces run those two updates.
 #pragma once
 #include "orl_mlp.cuh"
 

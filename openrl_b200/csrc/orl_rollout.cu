@@ -89,42 +89,10 @@ __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
         __syncthreads();
         float logit[MAX_OUT];
         head_dots<R_M, R_NT>(w, N3s, n, logit);
-        if (hpart == 0 && hrow < rows_here && a.head_kind == ORL_HEAD_GAUSSIAN) {
-            // DiagGaussian (distributions.py:75-98): action = noise*std + mean, per-dimension log-probs
-            const size_t grow = (size_t)t * B + row0 + hrow;
-            const float* logstd = a.policy_params + net_offsets(d, n, 1).ls;
-            uint32_t rr[8];
-            if (!a.exp_noise && !a.deterministic) {
-                const uint64_t step = rng_base + (uint64_t)t;
-                const uint32_t crow = (uint32_t)(row0 + hrow + a.rng_row_offset);
-                const uint4 r0 = action_philox(a.rng_seed, step, crow, 2u), r1 = action_philox(a.rng_seed, step, crow, 3u);
-                const uint4 r2 = action_philox(a.rng_seed, step, crow, 4u), r3 = action_philox(a.rng_seed, step, crow, 5u);
-                // Box-Muller: 8 normals from 16 uniforms (pairs (r0,r1) and (r2,r3))
-                const uint32_t u1[8] = {r0.x, r0.y, r0.z, r0.w, r2.x, r2.y, r2.z, r2.w};
-                const uint32_t u2[8] = {r1.x, r1.y, r1.z, r1.w, r3.x, r3.y, r3.z, r3.w};
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const float rad = sqrtf(-2.0f * logf(u32_to_unit_open(u1[j])));
-                    rr[j] = __float_as_uint(rad * cospif(2.0f * u32_to_unit_open(u2[j])));
-                }
-            }
-#pragma unroll
-            for (int j = 0; j < MAX_OUT; ++j) {
-                if (j < n) {
-                    const float mean = logit[j], ls = logstd[j], std = expf(ls);
-                    float act = mean;
-                    if (!a.deterministic) {
-                        const float eps = a.exp_noise ? a.exp_noise[grow * n + j] : __uint_as_float(rr[j]);
-                        act = __fadd_rn(__fmul_rn(eps, std), mean);
-                    }
-                    const float diff = act - mean;
-                    // Normal.log_prob: -((x-mu)^2)/(2 var) - log(std) - log(sqrt(2 pi))
-                    const float lp = -(diff * diff) / (2.0f * (std * std)) - ls - 0.9189385332046727f;
-                    a.actions[grow * n + j] = act;
-                    a.action_log_probs[grow * n + j] = lp;
-                }
-            }
-        }
+        if (hpart == 0 && hrow < rows_here && a.head_kind == ORL_HEAD_GAUSSIAN)
+            gaussian_act(logit, n, a.policy_params + net_offsets(d, n, 1).ls, a.deterministic != 0, a.exp_noise, a.rng_seed,
+                         rng_base + (uint64_t)t, (uint32_t)(row0 + hrow + a.rng_row_offset), (size_t)t * B + row0 + hrow, a.actions,
+                         a.action_log_probs);
         if (hpart == 0 && hrow < rows_here && a.head_kind != ORL_HEAD_GAUSSIAN) {
             const size_t grow = (size_t)t * B + row0 + hrow;
             float lp;

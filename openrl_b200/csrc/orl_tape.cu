@@ -147,7 +147,8 @@ int reduce_tape(const float* tape, int tape_width, long long rows, const TapeJob
     switch (tape_width) {
         case orl_rnnw::TAPE_W: e = launch_jobs<orl_rnnw::TAPE_W>(tape, rows, jobs, partials, stride, rb, st); break;
         case orl_deep::TAPE: e = launch_jobs<orl_deep::TAPE>(tape, rows, jobs, partials, stride, rb, st); break;
-        default: ORL_CHECK_ARG(false, "tape_width (the GRU's or the shared model's tape)");
+        case orl_deep::TAPE_GAUSSIAN: e = launch_jobs<orl_deep::TAPE_GAUSSIAN>(tape, rows, jobs, partials, stride, rb, st); break;
+        default: ORL_CHECK_ARG(false, "tape_width (the GRU's or one of the shared model's tapes)");
     }
     if (e) return e;
     row_block_sum_kernel<<<(total + 255) / 256, 256, 0, st>>>(partials, rb, stride, total, grads);

@@ -71,6 +71,7 @@ def load(path=None):
     lib.orl_last_error.argtypes = []
     lib.orl_rnn_workspace_floats.restype = _c.c_int64
     lib.orl_share_workspace_floats.restype = _c.c_int64
+    lib.orl_share_workspace_floats_head.restype = _c.c_int64
     lib.orl_ppo_peer_bucket_bytes.restype = _c.c_int64
     if lib.orl_abi_version() != 1:
         raise OrlLibraryError("ABI version mismatch")
@@ -163,6 +164,8 @@ _SIGNATURES.update({
     "orl_share_param_count": [_I, _I],
     "orl_share_tape_width": [],
     "orl_share_workspace_floats": [_L, _I, _I],
+    "orl_share_param_count_head": [_I, _I, _I],
+    "orl_share_workspace_floats_head": [_L, _I, _I, _I],
     "orl_share_rollout": [_c.POINTER(OrlRolloutArgs), _P],
     "orl_share_values": [_P, _I, _I, _I, _P, _P, _L, _P],
     "orl_share_fwdbwd": [_c.POINTER(OrlPpoArgs), _P],

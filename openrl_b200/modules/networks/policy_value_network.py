@@ -1,7 +1,8 @@
 """PolicyValueNetwork for cfg.use_share_model (reference: openrl/modules/networks/policy_value_network.py:33-174):
 obs_prep (MLPBase) -> common (MLPLayer(H, H, layer_N=0)) -> {v_out, act}, `critic_obs_prep` aliasing `obs_prep`.
 Parameter tree / state_dict names and the initialisation sequence are the reference's; the numeric path is
-csrc/orl_share.cu (flat layout = named_parameters order, see orl_deep_core.h)."""
+csrc/orl_share.cu (flat layout = named_parameters order, see orl_deep_core.h).  Discrete action spaces take a
+Categorical head, Box spaces of width <= 8 a DiagGaussian head (fc_mean + logstd, as in PolicyNetwork)."""
 import torch
 import torch.nn as nn
 
@@ -38,10 +39,8 @@ class PolicyValueNetwork(nn.Module):
         self.common = CommonLayer(cfg.hidden_size, cfg.hidden_size, cfg.use_orthogonal, cfg.activation_id)
         self.v_out = _init(nn.Linear(cfg.hidden_size, 1), 1.0, cfg.use_orthogonal)
         self.act = ACTLayer(action_space, cfg.hidden_size, cfg.use_orthogonal, cfg.gain)
-        if self.act.continuous_action:
-            raise NotImplementedError("the shared-model kernels are built for Discrete action spaces")
-        self.head_kind = 0
-        self.n_actions = action_space.n
+        self.head_kind = 1 if self.act.continuous_action else 0          # lib.HEAD_GAUSSIAN / HEAD_CATEGORICAL
+        self.n_actions = action_space.shape[0] if self.act.continuous_action else action_space.n  # head width
         if self.n_actions > 8:
             raise NotImplementedError("head widths up to 8 are built")
         self.device = torch.device(device)
