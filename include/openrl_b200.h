@@ -195,9 +195,15 @@ int orl_critic_values(const float* critic_params, int obs_dim, int activation_id
  * action_masks_next (nullable): when the envs reported legal-move masks (`info["action_masks"]`, prepare_action_masks,
  * envs/vec_env/utils/util.py:54-88) for this step, the staged block carries them after the dones, [... | action masks
  * (B*n_actions)], and they are written to slot t+1 of action_masks (replay_data.py:282-283); NULL writes nothing there,
- * so the slot keeps what it held, as in the reference. */
+ * so the slot keeps what it held, as in the reference.
+ * critic_obs_next (nullable): for an env whose observation space is Dict {"policy", "critic"} (a separate critic
+ * observation, as the reference's MAPPO envs give it: get_critic_obs, buffers/utils/util.py:22-55) the block carries the
+ * critic observations right after the policy observations, [obs (B*d) | critic obs (B*critic_obs_dim) | rewards | ...],
+ * and they are written to slot t+1 of critic_obs at the same first row; critic_obs_dim must be in 1..64
+ * (ORL_ERR_BAD_ARG otherwise).  NULL: the block has no critic section. */
 int orl_host_insert(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
-                    float* masks_next, float* active_masks_next, float* action_masks_next, int n_actions, void* stream);
+                    float* masks_next, float* active_masks_next, float* action_masks_next, int n_actions,
+                    float* critic_obs_next, int critic_obs_dim, void* stream);
 
 /* ---- policy evaluation of given actions over a flat batch of rows ------------------------
  * Replaces PolicyNetwork.eval_actions (policy_network.py:164-203) -> ACTLayer.evaluate_actions (act.py:130-172), the
@@ -411,10 +417,11 @@ int orl_rnn_rollout(const OrlRnnArgs* args, void* stream);
 int orl_rnn_act_rows(const OrlRnnArgs* args, void* stream);
 /* orl_host_insert for a recurrent policy: additionally zeroes the 64-float rnn_states_next row of every agent of an env
  * whose agents are all done (rnn_states[dones_env] = 0, onpolicy_driver.py:262-269).  rnn_states_next addresses slot
- * t+1 at the same first row as the other pointers; action_masks_next / n_actions as in orl_host_insert. */
+ * t+1 at the same first row as the other pointers; action_masks_next / n_actions and critic_obs_next / critic_obs_dim
+ * as in orl_host_insert. */
 int orl_host_insert_rnn(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
                         float* masks_next, float* active_masks_next, float* rnn_states_next, float* action_masks_next,
-                        int n_actions, void* stream);
+                        int n_actions, float* critic_obs_next, int critic_obs_dim, void* stream);
 /* recurrent critic over slots 0..T: value_preds[t] and rnn_states_critic[t+1] */
 int orl_rnn_critic(const OrlRnnArgs* args, void* stream);
 /* chunked BPTT forward + loss + backward of both nets over the minibatch chunks -> grads, loss_acc */

@@ -48,6 +48,10 @@ class OnPolicyDriver:
         if self.recurrent and self.envs.kind == lib.ENV_NONE and getattr(cfg, "use_joint_action_loss", False):
             raise NotImplementedError("use_joint_action_loss (JRPO) is built for simple_spread on the device (3 agents, agent-0 "
                                       "critic); host-stepped envs take the per-agent recurrent update")
+        if self.envs.kind == lib.ENV_NONE and getattr(trainer, "share", False) and getattr(self.envs, "dict_obs", False):
+            # the shared net's update computes the value from policy_obs (critic_obs_prep is obs_prep, policy_value_network.py:75)
+            raise NotImplementedError("use_share_model computes the value from the policy observation; a host env with a "
+                                      "Dict {'policy', 'critic'} observation space needs the two-net policy and critic")
 
     # -- reference surface -------------------------------------------------------------------
     def run(self):
@@ -286,9 +290,11 @@ class OnPolicyDriver:
         """One host env.step of envs [lo, hi) into slot step + 1 (rewards: slot step): orl_host_insert, or
         orl_host_insert_rnn, which also zeroes rnn_states[step + 1] of the envs that finished.  With `has_masks` the
         staged block carries the envs' action masks, written to action_masks[step + 1] (replay_data.py:282-283); the
-        buffer's masks stop being trivial for good."""
+        buffer's masks stop being trivial for good.  A buffer with its own critic_obs (Dict observations) takes the
+        block's critic section into critic_obs[step + 1]."""
         d, A = self.buffer.data, self.envs.agent_num
         r0, r1 = lo * A, hi * A
+        cri = None if d.critic_obs is d.policy_obs else d.critic_obs[step + 1].view(-1, d.critic_obs_dim)[r0:r1]
         args = (lib.ptr(staged), hi - lo, A, d.obs_dim, lib.ptr(d.policy_obs[step + 1].view(-1, d.obs_dim)[r0:r1]),
                 lib.ptr(d.rewards[step].view(-1)[r0:r1]), lib.ptr(d.masks[step + 1].view(-1)[r0:r1]),
                 lib.ptr(d.active_masks[step + 1].view(-1)[r0:r1]))
@@ -298,10 +304,11 @@ class OnPolicyDriver:
             am = d.action_masks[step + 1].view(-1, d.n_actions)[r0:r1]
         if self.recurrent:
             states = d.rnn_states[step + 1].view(d.n_rollout_threads * A, -1)[r0:r1]
-            lib.check(self._lib.orl_host_insert_rnn(*args, lib.ptr(states), lib.ptr(am), d.n_actions, lib.current_stream()),
-                      "orl_host_insert_rnn")
+            lib.check(self._lib.orl_host_insert_rnn(*args, lib.ptr(states), lib.ptr(am), d.n_actions, lib.ptr(cri), d.critic_obs_dim,
+                                                    lib.current_stream()), "orl_host_insert_rnn")
         else:
-            lib.check(self._lib.orl_host_insert(*args, lib.ptr(am), d.n_actions, lib.current_stream()), "orl_host_insert")
+            lib.check(self._lib.orl_host_insert(*args, lib.ptr(am), d.n_actions, lib.ptr(cri), d.critic_obs_dim,
+                                                lib.current_stream()), "orl_host_insert")
         self.gpu_launches += 1
 
     def _launch_steps(self, t_begin, t_end, noise):

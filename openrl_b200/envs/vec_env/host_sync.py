@@ -1,8 +1,8 @@
 """Host-side synchronous vector env over per-env thunks (reference: SyncVectorEnv,
 openrl/envs/vec_env/sync_venv.py:129-247, with the single-agent wrapping of
 envs/wrappers/multiagent_wrapper.py:33-79): steps N Python envs in a loop and returns the
-reference's batched 4-tuple — obs (N, A, d), rewards (N, A, 1), dones (N, A), infos (list of N dicts) —
-auto-resetting finished envs with `final_observation` / `final_info` stashed in the info
+reference's batched 4-tuple — obs (N, A, d) (a dict of such arrays for Dict observations), rewards (N, A, 1),
+dones (N, A), infos (list of N dicts) — auto-resetting finished envs with `final_observation` / `final_info` stashed in the info
 (sync_venv.py:213-218).  This is the env side of host-stepped workloads (MuJoCo-class simulators,
 BASELINE configs[4]); `HostVecEnv` adds the pinned staging that feeds the device path.
 
@@ -29,8 +29,12 @@ class SyncHostVecEnv:
 
     # -- reference surface -------------------------------------------------------------------
     def _obs(self, obs_list):
+        """Stack the envs' observations to float32 (N, A, d); Dict observations (`{"policy": ..., "critic": ...}`, each
+        (d,) for a single agent or (A, d)) stack per key, as the reference's concatenate of a Dict space does."""
+        if isinstance(obs_list[0], dict):
+            return {k: self._obs([x[k] for x in obs_list]) for k in obs_list[0]}
         o = np.stack([np.asarray(x, dtype=np.float32) for x in obs_list])
-        return o.reshape(self.parallel_env_num, self.agent_num, -1)
+        return o.reshape(len(obs_list), self.agent_num, -1)
 
     def reset(self, seed=None, options=None):
         obs, infos = [], []
@@ -79,8 +83,7 @@ class SyncHostVecEnv:
                 info["final_info"] = old_info
             obs.append(o)
             infos.append(info)
-        o = np.stack([np.asarray(x, dtype=np.float32) for x in obs]).reshape(N, A, -1)
-        return o, rewards, dones, infos
+        return self._obs(obs), rewards, dones, infos
 
     def random_action(self, infos=None):
         return np.array([[self.action_space.sample() for _ in range(self.agent_num)] for _ in range(self.parallel_env_num)])

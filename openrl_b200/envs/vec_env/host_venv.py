@@ -6,7 +6,9 @@ Wraps any object with the reference's BaseVecEnv duck type — `reset(seed=) -> 
 `step(actions) -> (obs (N,A,d), rewards (N,A,1), dones (N,A), infos)`, `parallel_env_num`,
 `agent_num`, `observation_space`, `action_space` — and adds pinned staging buffers so that each step
 costs one D2H copy (actions) and one H2D copy (obs, rewards, dones and, for Discrete actions, the legal-move masks the
-envs report in `info["action_masks"]`).  `kind = ORL_ENV_NONE` tells
+envs report in `info["action_masks"]`).  An env whose observation space is Dict {"policy", "critic"} gives the critic
+its own observation (the reference's MAPPO envs: get_policy_obs / get_critic_obs, buffers/utils/util.py:22-55); both
+ride in the same copy.  `kind = ORL_ENV_NONE` tells
 the driver to run the per-step loop (onpolicy_driver.py:154-203 semantics)."""
 import numpy as np
 import torch
@@ -32,6 +34,25 @@ def prepare_action_masks(info, agent_num=1):
     return np.asarray(rows, dtype=np.int8).reshape(len(rows), -1)
 
 
+def dict_obs_dims(space):
+    """(policy width, critic width) of a Dict observation space with exactly the keys "policy" and "critic", each a flat
+    Box of width 1..64 (the widths the device networks take); NotImplementedError naming the cause otherwise."""
+    keys = sorted(space.keys())
+    if keys != ["critic", "policy"]:
+        raise NotImplementedError(f"HostVecEnv stages Dict observation spaces with exactly the keys 'policy' and 'critic'; "
+                                  f"this one has {keys}")
+    dims = []
+    for k in ("policy", "critic"):
+        sub = space[k]
+        shape = getattr(sub, "shape", None)
+        if sub.__class__.__name__ != "Box" or shape is None or len(shape) != 1:
+            raise NotImplementedError(f"HostVecEnv stages flat Box entries of a Dict observation space; '{k}' is {sub}")
+        if not 1 <= shape[0] <= 64:
+            raise NotImplementedError(f"the '{k}' observation has width {shape[0]}; the device networks take widths 1..64")
+        dims.append(int(shape[0]))
+    return tuple(dims)
+
+
 class HostVecEnv:
     def __init__(self, env, device="cuda:0"):
         self.env = env
@@ -46,9 +67,15 @@ class HostVecEnv:
         self.env_table, self.env_table_len = None, 0
         self.h2d_bytes = 0
         self.d2h_bytes = 0
-        if not hasattr(self.observation_space, "shape") or self.observation_space.shape is None:
-            raise NotImplementedError("HostVecEnv stages flat Box observations; Dict observation spaces are not supported")
-        self.obs_dim = self.observation_space.shape[0]
+        self.dict_obs = self.observation_space.__class__.__name__ == "Dict"
+        if self.dict_obs:
+            self.obs_dim, self.critic_obs_dim = dict_obs_dims(self.observation_space)
+        else:
+            if not hasattr(self.observation_space, "shape") or self.observation_space.shape is None:
+                raise NotImplementedError(f"HostVecEnv stages flat Box or Dict {{'policy', 'critic'}} observations; "
+                                          f"got {self.observation_space}")
+            self.obs_dim = self.critic_obs_dim = self.observation_space.shape[0]
+        self._staged_dc = self.critic_obs_dim if self.dict_obs else 0    # width of the block's critic section
         self._discrete = hasattr(self.action_space, "n")
         # masks of Box action spaces are ignored, like the reference's buffer (replay_data.py:148-159)
         self.n_mask = int(self.action_space.n) if self._discrete else 0
@@ -60,10 +87,14 @@ class HostVecEnv:
         return out, [{} for _ in range(self.parallel_env_num)]
 
     def reset_into(self, obs_out, critic_obs_out=None, action_masks_out=None):
-        """Slot 0 of the buffer from env.reset(): the observations and, when every env's reset info carries
-        `action_masks` and `action_masks_out` is given, the masks (init_buffer, replay_data.py:286-298).  Returns whether
-        masks were written."""
+        """Slot 0 of the buffer from env.reset(): the observations (with Dict observations the "policy" entry, and the
+        "critic" entry into `critic_obs_out` when it is given) and, when every env's reset info carries `action_masks` and
+        `action_masks_out` is given, the masks (init_buffer, replay_data.py:286-298).  Returns whether masks were written."""
         obs, infos = self.reset()
+        if self.dict_obs:
+            if critic_obs_out is not None:
+                critic_obs_out.copy_(torch.as_tensor(np.asarray(obs["critic"], dtype=np.float32)).view_as(critic_obs_out))
+            obs = obs["policy"]
         obs_out.copy_(torch.as_tensor(np.asarray(obs, dtype=np.float32)).view_as(obs_out), non_blocking=False)
         am = self._masks(infos, self.parallel_env_num)
         if am is None or action_masks_out is None:
@@ -83,10 +114,14 @@ class HostVecEnv:
         return am
 
     def _stage_step(self, buf, obs, rewards, dones, infos, n_envs):
-        """Write one step into the pinned block [obs | rewards | dones (| masks)]; returns the floats to upload and
-        whether masks were staged."""
-        B, d = n_envs * self.agent_num, self.obs_dim
-        buf[:B * d] = np.asarray(obs, dtype=np.float32).reshape(-1)
+        """Write one step into the pinned block [obs (| critic obs) | rewards | dones (| masks)]; returns the floats to
+        upload and whether masks were staged."""
+        B, d = n_envs * self.agent_num, self.obs_dim + self._staged_dc
+        if self.dict_obs:
+            buf[:B * self.obs_dim] = np.asarray(obs["policy"], dtype=np.float32).reshape(-1)
+            buf[B * self.obs_dim:B * d] = np.asarray(obs["critic"], dtype=np.float32).reshape(-1)
+        else:
+            buf[:B * d] = np.asarray(obs, dtype=np.float32).reshape(-1)
         buf[B * d:B * d + B] = np.asarray(rewards, dtype=np.float32).reshape(-1)
         buf[B * d + B:B * (d + 2)] = np.asarray(dones, dtype=np.float32).reshape(-1)
         am = self._masks(infos, n_envs)
@@ -115,10 +150,10 @@ class HostVecEnv:
         if getattr(self, "_stages", None) is None:
             self._stages = {}
         if (lo, hi) not in self._stages:
-            n, A, w = hi - lo, self.agent_num, self.obs_dim + 2 + self.n_mask
+            n, A, w = hi - lo, self.agent_num, self.obs_dim + self._staged_dc + 2 + self.n_mask
             cuda = self.device.type == "cuda"
             self._stages[lo, hi] = dict(
-                inp=torch.empty(n * A * w, dtype=torch.float32, pin_memory=cuda),     # obs | rewards | dones (| masks)
+                inp=torch.empty(n * A * w, dtype=torch.float32, pin_memory=cuda),     # obs (| critic obs) | rewards | dones (| masks)
                 act=None, dev=torch.empty(n * A * w, dtype=torch.float32, device=self.device),
                 ev=torch.cuda.Event() if cuda else None)
         return self._stages[lo, hi]
@@ -137,7 +172,7 @@ class HostVecEnv:
     def step_staged(self, lo, hi):
         """Wait for the actions of envs [lo, hi) (`fetch_actions`), step them on the host (`env.step` for every env,
         `env.step_range` for a sub-range), stage the results in pinned memory and enqueue ONE H2D copy.  Returns the device
-        block [obs | rewards | dones (| masks)] (the layout orl_host_insert reads), the host-side step outputs and whether
+        block [obs (| critic obs) | rewards | dones (| masks)] (the layout orl_host_insert reads), the host-side step outputs and whether
         the block carries the envs' action masks (every stepped env's info has `action_masks`): a 6-tuple
         (dev, obs, rewards, dones, infos, has_masks)."""
         st = self._range_stage(lo, hi)

@@ -170,7 +170,7 @@ _SIGNATURES.update({
     "orl_share_values": [_P, _I, _I, _I, _P, _P, _L, _P],
     "orl_share_fwdbwd": [_c.POINTER(OrlPpoArgs), _P],
     "orl_share_apply": [_c.POINTER(OrlPpoArgs), _P],
-    "orl_host_insert": [_P, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P],
+    "orl_host_insert": [_P, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _I, _P],
     "orl_policy_eval": [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _L, _P],
     "orl_ppo_stride": [_I, _I, _I],
     "orl_ppo_grads_stride": [_I, _I, _I],
@@ -219,7 +219,7 @@ class OrlRnnArgs(ctypes.Structure):
 
 _SIGNATURES.update({
     "orl_rnn_act_rows": [_c.POINTER(OrlRnnArgs), _P],
-    "orl_host_insert_rnn": [_P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _I, _P],
+    "orl_host_insert_rnn": [_P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _I, _P, _I, _P],
     "orl_rnn_param_count": [_I, _I],
     "orl_rnn_tape_width": [],
     "orl_rnn_workspace_floats": [_c.c_int64, _I],

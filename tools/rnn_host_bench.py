@@ -10,8 +10,12 @@ random actions.  An act event pair also spans the Python that fills the launch a
 each.  Prints the card name, power limit and clocks read in the same run, and one JSON line.  `--masked`: every env
 reports `info["action_masks"]` on every step (a fixed random row per env, action 0 always legal), so the iteration also
 stages, uploads, inserts and applies the masks: the per-step cost of mask ingest is the difference to a run without.
+`--dict-obs`: instead, a SMAC-3m-shaped GRU MAPPO workload (3 agents, policy obs 30, 8 actions, per-agent masks every
+step, an env ends every 20 steps, staggered) whose host env replays a fixed pool of observations, timed with a flat
+Box(30) observation and with Dict {"policy": Box(30), "critic": Box(48)}: the cost of the critic section (staged,
+uploaded, inserted, and read by the critic and the update) is the difference between the two.
 
-    python tools/rnn_host_bench.py [--envs 1024 --T 128 --iters 3 --rounds 2 --warmup 2 --masked]
+    python tools/rnn_host_bench.py [--envs 1024 --T 128 --iters 3 --rounds 2 --warmup 2 --masked | --dict-obs]
 """
 import argparse
 import copy
@@ -72,7 +76,47 @@ class CartPoleHost:
         return o, r, d, [{} for _ in range(hi - lo)]
 
 
-def build(n, T, recurrent, grouped, masked=False):
+class Smac3mHost:
+    """SMAC-3m-shaped host vec-env: A = 3 agents, policy obs 30 and, with `critic`, a Dict space with a 48-wide critic
+    obs; Discrete(8) with per-agent (A, 8) masks on every step; env e ends at steps where (t + e) % 20 == 19.  The
+    observations replay a fixed random pool, so the host side costs little beyond the staging."""
+    A, D, DC, N_ACT, POOL = 3, 30, 48, 8, 8
+
+    def __init__(self, n, critic=False):
+        from openrl_b200 import spaces
+
+        g = np.random.default_rng(0)
+        box = lambda w: spaces.Box(-np.inf, np.inf, (w,), np.float32)  # noqa: E731
+        self.parallel_env_num, self.agent_num, self.critic = n, self.A, critic
+        self.observation_space = spaces.Dict({"policy": box(self.D), "critic": box(self.DC)}) if critic else box(self.D)
+        self.action_space = spaces.Discrete(self.N_ACT)
+        self.pol = g.standard_normal((self.POOL, n, self.A, self.D)).astype(np.float32)
+        self.cri = g.standard_normal((self.POOL, n, self.A, self.DC)).astype(np.float32)
+        m = (g.random((n, self.A, self.N_ACT)) < 0.6).astype(np.int8)
+        m[..., 0] = 1
+        self.infos = [{"action_masks": m[e]} for e in range(n)]
+        self.rewards = g.standard_normal((n, self.A, 1))
+        self.t = 0
+
+    def _obs(self, lo, hi):
+        k = self.t % self.POOL
+        return {"policy": self.pol[k, lo:hi], "critic": self.cri[k, lo:hi]} if self.critic else self.pol[k, lo:hi]
+
+    def reset(self, seed=None):
+        self.t = 0
+        return self._obs(0, self.parallel_env_num), self.infos
+
+    def step(self, actions):
+        return self.step_range(0, self.parallel_env_num, actions)
+
+    def step_range(self, lo, hi, actions):
+        if hi == self.parallel_env_num:
+            self.t += 1
+        dones = np.repeat(((self.t + np.arange(lo, hi)) % 20 == 19)[:, None], self.A, axis=1)
+        return self._obs(lo, hi), self.rewards[lo:hi], dones, self.infos[lo:hi]
+
+
+def build(n, T, recurrent, grouped, masked=False, dict_obs=None):
     from openrl_b200.configs.config import create_config_parser
     from openrl_b200.envs.vec_env import HostVecEnv
     from openrl_b200.modules.common import PPONet
@@ -83,7 +127,8 @@ def build(n, T, recurrent, grouped, masked=False):
                                              "--use_recurrent_policy", "true" if recurrent else "false",
                                              "--host_env_groups", "true" if grouped else "false"])
     cfg.quiet = True
-    agent = PPOAgent(PPONet(HostVecEnv(CartPoleHost(n, masked)), cfg=cfg, device="cuda:0"))
+    host = CartPoleHost(n, masked) if dict_obs is None else Smac3mHost(n, critic=dict_obs)
+    agent = PPOAgent(PPONet(HostVecEnv(host), cfg=cfg, device="cuda:0"))
     agent.train(total_time_steps=0, logger=Logger(quiet=True))   # trainer / buffer / driver, envs reset
     drv = agent.driver
     assert drv.recurrent == recurrent
@@ -138,6 +183,8 @@ def main():
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--masked", action="store_true", help="the envs report action masks on every step")
+    ap.add_argument("--dict-obs", action="store_true",
+                    help="a SMAC-3m-shaped GRU workload, with and without a 48-wide critic observation")
     args = ap.parse_args()
 
     import torch
@@ -145,27 +192,34 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("rnn_host_bench needs a CUDA device")
     modes = {}
-    for recurrent in (True, False):
+    variants = [(True, None), (False, None)] if not args.dict_obs else [(True, False), (True, True)]
+    for recurrent, dict_obs in variants:
         for grouped in (False, True):
-            drv, acts = build(args.envs, args.T, recurrent, grouped, args.masked)
+            drv, acts = build(args.envs, args.T, recurrent, grouped, args.masked, dict_obs)
             for _ in range(args.warmup):
                 iteration(drv, acts)
-            modes[("gru" if recurrent else "mlp") + ("_grouped" if grouped else "_sync")] = (drv, acts)
+            tag = "gru" if recurrent else "mlp"
+            if dict_obs is not None:
+                tag += "_critic48" if dict_obs else "_box"
+            modes[tag + ("_grouped" if grouped else "_sync")] = (drv, acts)
     samples = {m: [] for m in modes}
     for _ in range(args.rounds):
         for m, (drv, acts) in modes.items():
             for _ in range(args.iters):
                 samples[m].append(iteration(drv, acts))
     # the host env alone: T steps of the numpy CartPole with uniform random actions (what an untrained policy takes)
-    host = CartPoleHost(args.envs)
+    host = CartPoleHost(args.envs) if not args.dict_obs else Smac3mHost(args.envs, critic=True)
     host.reset(seed=0)
-    acts_host = np.random.default_rng(0).integers(0, 2, size=(args.T, args.envs, 1, 1))
+    acts_host = np.random.default_rng(0).integers(0, 2, size=(args.T, args.envs, host.agent_num, 1))
     t0 = time.perf_counter()
     for t in range(args.T):
         host.step(acts_host[t])
     env_ms = (time.perf_counter() - t0) * 1e3
     name, q = card()
-    res = {"workload": f"CartPole host-stepped (numpy env), {args.envs} envs, T={args.T}, Philox sampling, data_chunk_length 16"
+    workload = (f"CartPole host-stepped (numpy env), {args.envs} envs" if not args.dict_obs else
+                f"SMAC-3m-shaped host env (3 agents, obs 30, 8 actions, masks every step; critic obs 48 in the critic48 "
+                f"modes), {args.envs} envs")
+    res = {"workload": workload + f", T={args.T}, Philox sampling, data_chunk_length 16"
                        + (", action masks reported on every step" if args.masked else ""),
            "card": name, "power_limit,clocks.sm,clocks.max.sm": q, "host_env_only_ms_per_iteration": round(env_ms, 2),
            "iterations_per_mode": args.rounds * args.iters, "modes": {}}
