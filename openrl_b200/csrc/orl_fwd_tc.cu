@@ -9,12 +9,13 @@
 //   rollout_cartpole_rows_kernel : the same for CartPole-v1 with 32 envs per CTA and the physics one step ahead
 //                             (layout below, before the kernel).
 //
-// critic_values_tc_kernel and rollout_tc_kernel: CTA = 256 threads = 128 rows x 2 column halves (warps w, w+4 share rows
-// [32(w%4), +32)).
+// critic_values_tc_kernel and rollout_tc_kernel: CTA = 256 threads = 128 rows x 2 column halves, in the update kernel's
+// layout (orl_tc16.cuh): warp w owns rows [16w, +16), the two halves of a row are lanes l and l ^ 16.
 // Per 128-row tile: fc1 (K = d <= 8, FFMA) + activation + LayerNorm-1 in registers -> n1 as fp16 hi/lo panels ->
 // Z3 = n1 . W3f^T as 12 wgmma (3 split passes x K/16; warpgroup g computes rows [64g, +64)) -> fp32 staging tile in
-// shared memory -> every thread reads its row's columns -> LayerNorm-3 + head in registers.  The rollout's
-// per-step critical path is one row's work (no shared-memory GEMM, no cross-row shuffles): ~1/3 of the FFMA kernel's.
+// shared memory, read back by the warp that owns the rows -> LayerNorm-3 + head in registers.  Both pass through the
+// row functions of orl_tc16.cuh, which the update and the CartPole rollout use as well.  The rollout's per-step critical
+// path is one row's work (no shared-memory GEMM, no cross-row shuffles): ~1/3 of the FFMA kernel's.
 #include <algorithm>
 
 #include "orl_envstep.cuh"
@@ -25,8 +26,6 @@ using namespace orl;
 using namespace orl::tc;
 
 constexpr int F_M = 128, F_NT = 256, FCW = 32;
-// Z3 staging tile: row pitch 68 floats (row-per-thread float4 reads are conflict-free)
-constexpr int S_LD = 68;
 // shared-memory carve of a forward kernel: n1 hi/lo panels of M1 rows | W3f hi/lo panels | staging tile of MS rows | small
 template <int M1, int MS>
 struct FwdLayout {
@@ -35,28 +34,13 @@ struct FwdLayout {
 };
 using FLay = FwdLayout<F_M, F_M>;
 constexpr uint32_t FPANEL = FLay::PANEL;
-// fp32: w1t[8][64] b1[64] b3f[64] whf[8][64] bhf[8] | xs[2][128][2] xh[8][2][128] xst[128][8]
+// fp32: w1t[8][64] b1[64] b3f[64] whf[8][64] bhf[8]
 constexpr uint32_t F_SMALL_FLOATS = 8 * H + H + H + MAX_OUT * H + MAX_OUT;
-constexpr uint32_t F_XCH_FLOATS = 2 * F_M * 2 + 2 * F_M * 8 + F_M * 8;
-constexpr uint32_t F_SMEM = FLay::SMALL + 4 * (F_SMALL_FLOATS + F_XCH_FLOATS);
-
-#define F_FOR_OUT(j) _Pragma("unroll") for (int j = 0; j < NOUT; ++j) if (NOUT != 8 || j < n)
-#define F_ROWGROUP_SYNC()                                                      \
-    do {                                                                       \
-        switch (warp & 3) {                                                    \
-            case 0: asm volatile("bar.sync 1, 64;" ::: "memory"); break;       \
-            case 1: asm volatile("bar.sync 2, 64;" ::: "memory"); break;       \
-            case 2: asm volatile("bar.sync 3, 64;" ::: "memory"); break;       \
-            default: asm volatile("bar.sync 4, 64;" ::: "memory"); break;      \
-        }                                                                      \
-    } while (0)
-
-template <int ACT>
-__device__ __forceinline__ float f_act(float z, int activation_id) { return ACT == 1 ? fmaxf(z, 0.f) : act_fwd(z, activation_id); }
+constexpr uint32_t F_SMEM = FLay::SMALL + 4 * F_SMALL_FLOATS;
 
 struct FwdCtx {
     uint8_t *R1h, *R1l;
-    float *S, *w1t, *b1s, *b3f, *whf, *bhf, *xs, *xh, *xst;
+    float *S, *w1t, *b1s, *b3f, *whf, *bhf;
     uint32_t aR1h, aR1l, aWh, aWl;
 };
 
@@ -69,7 +53,6 @@ __device__ __forceinline__ FwdCtx fwd_setup(uint8_t* smem, const float* __restri
     c.S = reinterpret_cast<float*>(smem + L::S);
     c.w1t = reinterpret_cast<float*>(smem + L::SMALL);
     c.b1s = c.w1t + 8 * H; c.b3f = c.b1s + H; c.whf = c.b3f + H; c.bhf = c.whf + MAX_OUT * H;
-    c.xs = c.bhf + MAX_OUT; c.xh = c.xs + 2 * F_M * 2; c.xst = c.xh + 2 * F_M * 8;   // the 2-half layout of the exchange area
     stage_weights_tc(c.w1t, Wh, Wl, params, d, n, blockDim.x);
     fence_proxy_async();
     __syncthreads();
@@ -78,51 +61,22 @@ __device__ __forceinline__ FwdCtx fwd_setup(uint8_t* smem, const float* __restri
 }
 
 // One 128-row tile forward: x (this thread's row, zero padded) -> out[j] = head(j) incl. the folded bias, valid in
-// BOTH column halves of the row.
+// BOTH column halves of the row.  Every hand-off is inside the warp or the warpgroup: the n1 rows a warpgroup's MMA
+// reads are its own, and the staging-tile rows a warp reads are those of its own accumulator fragment.  A warp
+// rewrites its n1 rows (next tile) only after its wgmma_wait has seen the MMA that read them complete.
 // `overlap()` runs between the MMA issue and the wait for its completion: work that does not depend on this tile's
 // result (the rollout's sampling noise) hides in the tensor-core latency.
 template <int NOUT, int ACT, typename Overlap>
 __device__ __forceinline__ void fwd_tile(const FwdCtx& c, const float (&x)[8], int d, int n, int activation_id,
                                          float (&out)[MAX_OUT], Overlap&& overlap) {
-    const int tid = threadIdx.x, warp = tid >> 5, row = tid & 127, half = tid >> 7, cb = FCW * half;
-    float n1[FCW];
-#pragma unroll
-    for (int q4 = 0; q4 < FCW; q4 += 4) {
-        const float4 b = *reinterpret_cast<const float4*>(c.b1s + cb + q4);
-        n1[q4] = b.x; n1[q4 + 1] = b.y; n1[q4 + 2] = b.z; n1[q4 + 3] = b.w;
-    }
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-        if (k < d) {
-#pragma unroll
-            for (int q4 = 0; q4 < FCW; q4 += 4) {
-                const float4 wv = *reinterpret_cast<const float4*>(c.w1t + k * H + cb + q4);
-                n1[q4] = fmaf(x[k], wv.x, n1[q4]); n1[q4 + 1] = fmaf(x[k], wv.y, n1[q4 + 1]);
-                n1[q4 + 2] = fmaf(x[k], wv.z, n1[q4 + 2]); n1[q4 + 3] = fmaf(x[k], wv.w, n1[q4 + 3]);
-            }
-        }
-    }
-    float s = 0.f, sq = 0.f;
-#pragma unroll
-    for (int i = 0; i < FCW; ++i) { n1[i] = f_act<ACT>(n1[i], activation_id); s += n1[i]; sq = fmaf(n1[i], n1[i], sq); }
-    {
-        *reinterpret_cast<float2*>(c.xs + (half * F_M + row) * 2) = make_float2(s, sq);
-        F_ROWGROUP_SYNC();
-        const float2 o = *reinterpret_cast<const float2*>(c.xs + ((half ^ 1) * F_M + row) * 2);
-        s += o.x; sq += o.y;
-    }
-    const float mu1 = s * (1.f / H);
-    const float rstd1 = 1.0f / sqrtf(fmaxf(sq * (1.f / H) - mu1 * mu1, 0.f) + LN_EPS);
-#pragma unroll
-    for (int i = 0; i < FCW; ++i) n1[i] = (n1[i] - mu1) * rstd1;
-#pragma unroll
-    for (int q8 = 0; q8 < FCW; q8 += 8) {
-        const uint32_t off = (uint32_t)((cb + q8) >> 3) * FPANEL + row * 16;
-        split_store8(c.R1h + off, c.R1l + off, n1 + q8, 1.0f);
-    }
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, row = 16 * warp + (lane & 15), wg = warp >> 2, cb = FCW * (lane >> 4);
+    float n1[FCW], s, sq;
+    row_fc1<FCW, ACT>(x, d, c.w1t, c.b1s, cb, activation_id, n1, s, sq);
+    row_sum_stats<FCW>(s, sq);
+    row_ln1_store<FCW>(n1, ln_stats(s, sq), c.R1h, c.R1l, FPANEL, row, cb);
     fence_proxy_async();
-    __syncthreads();
-    {   // Z3 = n1 . W3f^T: warpgroup `half` computes rows [64 half, +64)
+    warpgroup_sync(wg);   // the MMA reads this warpgroup's rows of n1
+    {   // Z3 = n1 . W3f^T: warpgroup wg computes rows [64 wg, +64)
         const uint64_t dK_A = desc_const(FPANEL, 128), dK_W = desc_const(W_PANEL, 128);
         float z[32];
 #pragma unroll
@@ -130,7 +84,7 @@ __device__ __forceinline__ void fwd_tile(const FwdCtx& c, const float (&x)[8], i
         wgmma_fence();
 #pragma unroll
         for (int pass = 0; pass < 3; ++pass) {
-            const uint32_t aa = (pass == 0 ? c.aR1l : c.aR1h) + half * 64 * 16, bb = pass == 1 ? c.aWl : c.aWh;
+            const uint32_t aa = (pass == 0 ? c.aR1l : c.aR1h) + wg * 64 * 16, bb = pass == 1 ? c.aWl : c.aWh;
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk)
                 wgmma_f16_n64<0, 0>(z, desc_at(dK_A, aa + 2 * kk * FPANEL), desc_at(dK_W, bb + 2 * kk * W_PANEL), (pass | kk) > 0);
@@ -138,48 +92,15 @@ __device__ __forceinline__ void fwd_tile(const FwdCtx& c, const float (&x)[8], i
         wgmma_commit();
         overlap();
         wgmma_wait<0>();
-        frag_store<64>(z, c.S + half * 64 * S_LD, S_LD);
+        frag_store<64>(z, c.S + wg * 64 * S_LD, S_LD);
     }
-    __syncthreads();   // the staging tile is complete; the next tile's stores follow its CTA barrier in front of the MMAs
-    float n3[FCW];
-#pragma unroll
-    for (int q4 = 0; q4 < FCW; q4 += 4) {
-        const float4 v = *reinterpret_cast<const float4*>(c.S + row * S_LD + cb + q4);
-        n3[q4] = v.x; n3[q4 + 1] = v.y; n3[q4 + 2] = v.z; n3[q4 + 3] = v.w;
-    }
-    float s3 = 0.f, q3 = 0.f;
-#pragma unroll
-    for (int i = 0; i < FCW; ++i) { n3[i] += c.b3f[cb + i]; s3 += n3[i]; q3 = fmaf(n3[i], n3[i], q3); }
-    {
-        __syncwarp();
-        // slot xs is free again: every partner read of exchange 1 happened before the CTA barrier above
-        *reinterpret_cast<float2*>(c.xs + (half * F_M + row) * 2) = make_float2(s3, q3);
-        F_ROWGROUP_SYNC();
-        const float2 o = *reinterpret_cast<const float2*>(c.xs + ((half ^ 1) * F_M + row) * 2);
-        s3 += o.x; q3 += o.y;
-    }
-    const float mu3 = s3 * (1.f / H);
-    const float rstd3 = 1.0f / sqrtf(fmaxf(q3 * (1.f / H) - mu3 * mu3, 0.f) + LN_EPS);
-#pragma unroll
-    for (int j = 0; j < MAX_OUT; ++j) out[j] = 0.f;
-#pragma unroll
-    for (int q4 = 0; q4 < FCW; q4 += 4) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) n3[q4 + i] = (n3[q4 + i] - mu3) * rstd3;
-        F_FOR_OUT(j) {
-            const float4 wv = *reinterpret_cast<const float4*>(c.whf + j * H + cb + q4);
-            out[j] = fmaf(n3[q4], wv.x, fmaf(n3[q4 + 1], wv.y, fmaf(n3[q4 + 2], wv.z, fmaf(n3[q4 + 3], wv.w, out[j]))));
-        }
-    }
-    {
-        F_FOR_OUT(j) c.xh[(j * 2 + half) * F_M + row] = out[j];   // [j][half][row]: conflict-free
-        F_ROWGROUP_SYNC();
-        // both halves add the two partial dots in the SAME order (half 0 first), so they hold identical logits
-        F_FOR_OUT(j) {
-            const float p0 = c.xh[(j * 2 + 0) * F_M + row], p1 = c.xh[(j * 2 + 1) * F_M + row];
-            out[j] = (p0 + p1) + c.bhf[j];
-        }
-    }
+    __syncwarp();   // rows [16 warp, +16) of the staging tile: written and read by this warp
+    float n3[FCW], s3, q3;
+    row_z3<FCW>(c.S, row, cb, c.b3f, n3, s3, q3);
+    row_sum_stats<FCW>(s3, q3);
+    row_head<FCW, NOUT>(n3, ln_stats(s3, q3), c.whf, cb, n, out);
+    row_sum_head<FCW, NOUT>(out, n);
+    FOR_OUT(j) out[j] += c.bhf[j];
 }
 
 template <int ACT>
@@ -188,7 +109,7 @@ __global__ void __launch_bounds__(F_NT, 2) critic_values_tc_kernel(const float* 
                                                                    long long rows) {
     extern __shared__ __align__(1024) uint8_t smem_f[];
     const FwdCtx c = fwd_setup(smem_f, params, d, 1);
-    const int tid = threadIdx.x, warp = tid >> 5, row = tid & 127, half = tid >> 7;
+    const int lane = threadIdx.x & 31, row = 16 * (threadIdx.x >> 5) + (lane & 15), half = lane >> 4;
     const long long n_tiles = (rows + F_M - 1) / F_M;
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const long long r = tile * F_M + row;
@@ -198,9 +119,6 @@ __global__ void __launch_bounds__(F_NT, 2) critic_values_tc_kernel(const float* 
         float out[MAX_OUT];
         fwd_tile<1, ACT>(c, x, d, 1, activation_id, out, [] {});
         if (half == 0 && r < rows) values[r] = out[0];
-        // the exchange slots are reused by the next tile: its first write follows this row group's last read only
-        // through the barriers inside fwd_tile of the NEXT tile -> order them here
-        F_ROWGROUP_SYNC();
     }
 }
 
@@ -210,42 +128,38 @@ __global__ void __launch_bounds__(F_NT, 1) rollout_tc_kernel(const OrlRolloutArg
     constexpr int NOUT = 5;   // GridWorldEnv's actions
     const int N = a.n_envs, B = N, d = a.obs_dim, n = NOUT;
     const FwdCtx c = fwd_setup(smem_f, a.policy_params, d, n);
-    const int tid = threadIdx.x, warp = tid >> 5, row = tid & 127, half = tid >> 7;
+    const int lane = threadIdx.x & 31, row = 16 * (threadIdx.x >> 5) + (lane & 15), half = lane >> 4;
     const int e = blockIdx.x * F_M + row;          // env == buffer row (single-agent envs)
     const bool valid = e < N;
     const uint64_t rng_base = a.rng_step_base + (a.rng_counter ? *a.rng_counter : 0ull);
     float x[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) x[k] = (valid && k < d) ? a.policy_obs[((size_t)a.t_begin * B + e) * d + k] : 0.f;
-    {
-        for (int t = a.t_begin; t < a.t_end; ++t) {
-            float logit[MAX_OUT];
-            float q[MAX_OUT];
-            const size_t grow = (size_t)t * B + (valid ? e : 0);
-            fwd_tile<NOUT, ACT>(c, x, d, n, a.activation_id, logit, [&] {
-                if (half == 0 && valid && !a.deterministic)
-                    action_noise(a.exp_noise, grow, n, a.rng_seed, rng_base + (uint64_t)t, (uint32_t)(e + a.rng_row_offset), q);
-            });
-            if (half == 0 && valid) {
-                float lp;
-                const int act = sample_action(logit, n, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0,
-                                              [&](float (&qs)[MAX_OUT]) { for (int j = 0; j < MAX_OUT; ++j) qs[j] = q[j]; }, lp);
-                a.actions[grow] = (float)act;
-                a.action_log_probs[grow] = lp;
-                // ---- env.step of this thread's env, in-place insert into slot t / t+1 ----
-                bool done;
-                *reinterpret_cast<float4*>(c.xst + row * 8) =
-                    step_insert_single(a, env_ptrs(a, a.rng_row_offset / a.n_agents), ORL_ENV_GRIDWORLD, e, t, act, done);
-            }
-            F_ROWGROUP_SYNC();   // publishes the next observation to the row's other half; orders the exchange slots
-            if (valid) {
-                const float4 o = *reinterpret_cast<const float4*>(c.xst + row * 8);
-                x[0] = o.x; x[1] = o.y; x[2] = o.z; x[3] = o.w;
-            }
+    for (int t = a.t_begin; t < a.t_end; ++t) {
+        float logit[MAX_OUT];
+        float q[MAX_OUT];
+        const size_t grow = (size_t)t * B + (valid ? e : 0);
+        fwd_tile<NOUT, ACT>(c, x, d, n, a.activation_id, logit, [&] {
+            if (half == 0 && valid && !a.deterministic)
+                action_noise(a.exp_noise, grow, n, a.rng_seed, rng_base + (uint64_t)t, (uint32_t)(e + a.rng_row_offset), q);
+        });
+        float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (half == 0 && valid) {
+            float lp;
+            const int act = sample_action(logit, n, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0,
+                                          [&](float (&qs)[MAX_OUT]) { for (int j = 0; j < MAX_OUT; ++j) qs[j] = q[j]; }, lp);
+            a.actions[grow] = (float)act;
+            a.action_log_probs[grow] = lp;
+            // ---- env.step of this thread's env, in-place insert into slot t / t+1 ----
+            bool done;
+            o = step_insert_single(a, env_ptrs(a, a.rng_row_offset / a.n_agents), ORL_ENV_GRIDWORLD, e, t, act, done);
         }
+        // the next observation, from half 0 (lane l % 16) to both halves of the row
+        o.x = __shfl_sync(0xffffffffu, o.x, lane & 15); o.y = __shfl_sync(0xffffffffu, o.y, lane & 15);
+        o.z = __shfl_sync(0xffffffffu, o.z, lane & 15); o.w = __shfl_sync(0xffffffffu, o.w, lane & 15);
+        if (valid) { x[0] = o.x; x[1] = o.y; x[2] = o.z; x[3] = o.w; }
     }
 }
-
 
 // ---- CartPole rollout: R envs per CTA, 4 forward lanes + 2 env threads per env -------------------------------------
 // The rollout is a chain of T dependent steps whose length is one row's work.  The f64 CartPole physics (sin / cos and
@@ -253,8 +167,8 @@ __global__ void __launch_bounds__(F_NT, 1) rollout_tc_kernel(const OrlRolloutArg
 // policy forward most of the rest.  A CTA owns R = 32 envs, so 4096 envs spread over 128 CTAs, one per SM, and each SM
 // issues the forward of 32 rows instead of 128 (DESIGN.md §6 has R = 32 against the removed R = 64):
 //   * Forward: 4R threads = R rows x 4 column quarters, the 4 quarters of a row in one warp (lane = 4 row + quarter,
-//     quarter qd owns hidden columns [16 qd, +16)); the LayerNorm and head partials meet through shuffles, added in a
-//     fixed order.  The fc3 GEMM is one M = 64 tile over R1 rows [0, 64) (rows [R, 64) zero padding): the one forward
+//     quarter qd owns hidden columns [16 qd, +16)); the row functions of orl_tc16.cuh with CW = 16, whose LayerNorm
+//     and head partials meet through shuffles, added in a fixed order.  The fc3 GEMM is one M = 64 tile over R1 rows [0, 64) (rows [R, 64) zero padding): the one forward
 //     warpgroup computes both 32-column halves.  Each Z3 element is the same wgmma_f16_n32 chain (Al.Bh, Ah.Bl, Ah.Bh;
 //     kk = 0..3) as in the row-parallel kernels.
 //   * Env: 2R threads, lane = row.  As soon as the state of step t is known, the action-0 threads advance the physics
@@ -361,14 +275,14 @@ __global__ void __launch_bounds__(RowsCfg::NT, RowsCfg::MIN_CTAS) rollout_cartpo
         }
     } else {
         // ================= forward quarters =================================================================================
-        const int warp = tid >> 5, lane = tid & 31, row = tid >> 2, qd = tid & 3, cb = QCW * qd, qbase = lane & ~3;
+        const int warp = tid >> 5, row = tid >> 2, qd = tid & 3, cb = QCW * qd;
         const int e = blockIdx.x * R + row;
         const bool valid = e < N;
         int elapsed = valid ? a.env_i32[e] : 0;
         int len = 0;
         float ret = 0.f;
         if (valid && qd == 0) { ret = a.ep_return[e]; len = a.ep_length[e]; }
-        float x[4];
+        float x[8];   // fc1 reads x[0, 4)
 #pragma unroll
         for (int k = 0; k < 4; ++k) x[k] = valid ? a.policy_obs[((size_t)a.t_begin * B + e) * 4 + k] : 0.f;
         RW_PUBLISH_SYNC();   // the first step's noise is in place
@@ -376,39 +290,10 @@ __global__ void __launch_bounds__(RowsCfg::NT, RowsCfg::MIN_CTAS) rollout_cartpo
             const uint32_t pb = it & 1u;
             const size_t grow = (size_t)t * B + (valid ? e : 0);
             // ---- fc1 + activation + LayerNorm-1 over this quarter's 16 columns ----
-            float n1[QCW];
-#pragma unroll
-            for (int q4 = 0; q4 < QCW; q4 += 4) {
-                const float4 b = *reinterpret_cast<const float4*>(c.b1s + cb + q4);
-                n1[q4] = b.x; n1[q4 + 1] = b.y; n1[q4 + 2] = b.z; n1[q4 + 3] = b.w;
-            }
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-#pragma unroll
-                for (int q4 = 0; q4 < QCW; q4 += 4) {
-                    const float4 wv = *reinterpret_cast<const float4*>(c.w1t + k * H + cb + q4);
-                    n1[q4] = fmaf(x[k], wv.x, n1[q4]); n1[q4 + 1] = fmaf(x[k], wv.y, n1[q4 + 1]);
-                    n1[q4 + 2] = fmaf(x[k], wv.z, n1[q4 + 2]); n1[q4 + 3] = fmaf(x[k], wv.w, n1[q4 + 3]);
-                }
-            }
-            float sm = 0.f, sq = 0.f;
-#pragma unroll
-            for (int i = 0; i < QCW; ++i) { n1[i] = f_act<ACT>(n1[i], a.activation_id); sm += n1[i]; sq = fmaf(n1[i], n1[i], sq); }
-            {   // all quarters add the four partials in the same order -> identical statistics
-                float ts = 0.f, tq = 0.f;
-#pragma unroll
-                for (int p = 0; p < 4; ++p) { ts += __shfl_sync(0xffffffffu, sm, qbase + p); tq += __shfl_sync(0xffffffffu, sq, qbase + p); }
-                sm = ts; sq = tq;
-            }
-            const float mu1 = sm * (1.f / H);
-            const float rstd1 = 1.0f / sqrtf(fmaxf(sq * (1.f / H) - mu1 * mu1, 0.f) + LN_EPS);
-#pragma unroll
-            for (int i = 0; i < QCW; ++i) n1[i] = (n1[i] - mu1) * rstd1;
-#pragma unroll
-            for (int q8 = 0; q8 < QCW; q8 += 8) {
-                const uint32_t off = (uint32_t)((cb + q8) >> 3) * C::L::PANEL + row * 16;
-                split_store8(c.R1h + off, c.R1l + off, n1 + q8, 1.0f);
-            }
+            float n1[QCW], sm, sq;
+            row_fc1<QCW, ACT>(x, 4, c.w1t, c.b1s, cb, a.activation_id, n1, sm, sq);
+            row_sum_stats<QCW>(sm, sq);
+            row_ln1_store<QCW>(n1, ln_stats(sm, sq), c.R1h, c.R1l, C::L::PANEL, row, cb);
             fence_proxy_async();
             RW_FWD_SYNC();
             {   // Z3 = n1 . W3f^T over R1 rows [0, 64), both 32-column halves b
@@ -438,43 +323,13 @@ __global__ void __launch_bounds__(RowsCfg::NT, RowsCfg::MIN_CTAS) rollout_cartpo
                 }
             }
             RW_FWD_SYNC();   // the staging tile is complete; the next step's stores follow its forward barrier in front of the MMAs
-            float n3[QCW];
-#pragma unroll
-            for (int q4 = 0; q4 < QCW; q4 += 4) {
-                const float4 v = *reinterpret_cast<const float4*>(c.S + row * S_LD + cb + q4);
-                n3[q4] = v.x; n3[q4 + 1] = v.y; n3[q4 + 2] = v.z; n3[q4 + 3] = v.w;
-            }
-            float s3 = 0.f, q3 = 0.f;
-#pragma unroll
-            for (int i = 0; i < QCW; ++i) { n3[i] += c.b3f[cb + i]; s3 += n3[i]; q3 = fmaf(n3[i], n3[i], q3); }
-            {
-                float ts = 0.f, tq = 0.f;
-#pragma unroll
-                for (int p = 0; p < 4; ++p) { ts += __shfl_sync(0xffffffffu, s3, qbase + p); tq += __shfl_sync(0xffffffffu, q3, qbase + p); }
-                s3 = ts; q3 = tq;
-            }
-            const float mu3 = s3 * (1.f / H);
-            const float rstd3 = 1.0f / sqrtf(fmaxf(q3 * (1.f / H) - mu3 * mu3, 0.f) + LN_EPS);
-            float out[MAX_OUT];
-#pragma unroll
-            for (int j = 0; j < MAX_OUT; ++j) out[j] = 0.f;
-#pragma unroll
-            for (int q4 = 0; q4 < QCW; q4 += 4) {
-#pragma unroll
-                for (int i = 0; i < 4; ++i) n3[q4 + i] = (n3[q4 + i] - mu3) * rstd3;
-                F_FOR_OUT(j) {
-                    const float4 wv = *reinterpret_cast<const float4*>(c.whf + j * H + cb + q4);
-                    out[j] = fmaf(n3[q4], wv.x, fmaf(n3[q4 + 1], wv.y, fmaf(n3[q4 + 2], wv.z, fmaf(n3[q4 + 3], wv.w, out[j]))));
-                }
-            }
+            float n3[QCW], s3, q3;
+            row_z3<QCW>(c.S, row, cb, c.b3f, n3, s3, q3);
+            row_sum_stats<QCW>(s3, q3);
             float logit[MAX_OUT];
-#pragma unroll
-            for (int j = 0; j < MAX_OUT; ++j) logit[j] = 0.f;
-            F_FOR_OUT(j) {
-                const float p0 = __shfl_sync(0xffffffffu, out[j], qbase), p1 = __shfl_sync(0xffffffffu, out[j], qbase + 1);
-                const float p2 = __shfl_sync(0xffffffffu, out[j], qbase + 2), p3 = __shfl_sync(0xffffffffu, out[j], qbase + 3);
-                logit[j] = ((p0 + p1) + (p2 + p3)) + c.bhf[j];
-            }
+            row_head<QCW, NOUT>(n3, ln_stats(s3, q3), c.whf, cb, n, logit);
+            row_sum_head<QCW, NOUT>(logit, n);
+            FOR_OUT(j) logit[j] += c.bhf[j];
             // ---- quarter 0: sampling, action outputs ----
             if (qd == 0) {
                 int act = 0;
@@ -482,7 +337,7 @@ __global__ void __launch_bounds__(RowsCfg::NT, RowsCfg::MIN_CTAS) rollout_cartpo
                     float q[MAX_OUT];
 #pragma unroll
                     for (int j = 0; j < MAX_OUT; ++j) q[j] = 1.f;
-                    if (!a.deterministic) { F_FOR_OUT(j) q[j] = qn[(pb * MAX_OUT + j) * R + row]; }
+                    if (!a.deterministic) { FOR_OUT(j) q[j] = qn[(pb * MAX_OUT + j) * R + row]; }
                     float lp;
                     act = sample_action(logit, n, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0,
                                         [&](float (&qs)[MAX_OUT]) { for (int j = 0; j < MAX_OUT; ++j) qs[j] = q[j]; }, lp);

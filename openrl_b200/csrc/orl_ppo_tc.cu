@@ -62,9 +62,9 @@ constexpr uint32_t PANEL = T_M * 16;           // 8 fp16 features of 128 rows
 constexpr int R1_PANELS = 10, R2_PANELS = 9, R3_PANELS = 8;
 constexpr int P_CST = 8, P_X = 9, P_U = 8;
 constexpr int N_LOSS_TC = 8;
-// staging tile of the per-tile GEMM results: 128 rows x 64 fp32, row pitch 68 floats (conflict-free row reads);
+// staging tile of the per-tile GEMM results: 128 rows x 64 fp32 at row pitch S_LD (orl_tc16.cuh);
 // the final Ga [128][GA_LD] / Gb [64][GB_LD] staging reuses R1 / R2
-constexpr int S_LD = 68, GA_LD = 84, GB_LD = 20;
+constexpr int GA_LD = 84, GB_LD = 20;
 // shared-memory carve-up (bytes)
 constexpr uint32_t OFF_R1H = 0, OFF_R1L = OFF_R1H + R1_PANELS * PANEL, OFF_R2H = OFF_R1L + R1_PANELS * PANEL,
                    OFF_R2L = OFF_R2H + R2_PANELS * PANEL, OFF_WH = OFF_R2L + R2_PANELS * PANEL, OFF_WL = OFF_WH + 8 * W_PANEL,
@@ -79,12 +79,6 @@ struct TcMaps {   // TMA descriptors of the flattened rollout buffers (built by 
     CUtensorMap obs_p, obs_c, actions, old_logp, adv, value_preds, returns, active;
 };
 
-#define FOR_OUT(j) _Pragma("unroll") for (int j = 0; j < NOUT; ++j) if (NOUT != 8 || j < n)
-// the two column halves of a row sit in lanes l and l ^ 16 of one warp
-__device__ __forceinline__ float other_half(float v) { return __shfl_xor_sync(0xffffffffu, v, 16); }
-// barrier of this thread's warpgroup (named barriers 1 and 2)
-__device__ __forceinline__ void warpgroup_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory"); }
-
 __host__ __device__ inline uint32_t tc_stage_bytes(int d) { return (uint32_t)((T_M * d * 4 + 127) & ~127) + N_SCAL * T_M * 4; }
 __host__ __device__ inline uint32_t tc_small_off(int d) { return OFF_STAGE + tc_stage_bytes(d); }
 // fp32 weights: w1t[8][64] b1[64] b3f[64] whf[8][64] bhf[8] swh[8]; flush scratch: Q[8][64] su smu sdl[3][8], loss
@@ -93,10 +87,7 @@ constexpr uint32_t SMALL_FLOATS = 8 * H + H + H + MAX_OUT * H + 2 * MAX_OUT;
 constexpr uint32_t XCH_FLOATS = MAX_OUT * H + 3 * MAX_OUT + 3 * 8;
 __host__ __device__ inline uint32_t tc_smem_bytes(int d) { return tc_small_off(d) + 4 * (SMALL_FLOATS + XCH_FLOATS) + 8; }
 
-// ACT == 1: ReLU (the reference's default activation_id) compiled in; ACT == -1: runtime activation_id (tanh / leaky / elu
-// expand to ~60 instructions per element, which the fully unrolled row code cannot afford in the instruction cache)
-template <int ACT>
-__device__ __forceinline__ float act_fwd_t(float z, int activation_id) { return ACT == 1 ? fmaxf(z, 0.f) : act_fwd(z, activation_id); }
+// the activation's derivative; ACT as for act_tc (orl_tc16.cuh)
 template <int ACT>
 __device__ __forceinline__ float act_bwd_t(float a, bool pos, int activation_id) { return ACT == 1 ? (pos ? 1.f : 0.f) : act_bwd(a, pos, activation_id); }
 
@@ -243,49 +234,19 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         const float row_c = POLICY ? st_sc[2 * T_M + row] : 0.f, active = st_sc[3 * T_M + row];
 
         // ---- fc1 + activation + LayerNorm-1 (this thread: columns [cb, cb+32) of its row) ----
-        float n1[CW];
-#pragma unroll
-        for (int q4 = 0; q4 < CW; q4 += 4) {
-            const float4 b = *reinterpret_cast<const float4*>(b1s + cb + q4);
-            n1[q4] = b.x; n1[q4 + 1] = b.y; n1[q4 + 2] = b.z; n1[q4 + 3] = b.w;
-        }
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            if (k < d) {
-#pragma unroll
-                for (int q4 = 0; q4 < CW; q4 += 4) {
-                    const float4 wv = *reinterpret_cast<const float4*>(w1t + k * H + cb + q4);
-                    n1[q4] = fmaf(x[k], wv.x, n1[q4]); n1[q4 + 1] = fmaf(x[k], wv.y, n1[q4 + 1]);
-                    n1[q4 + 2] = fmaf(x[k], wv.z, n1[q4 + 2]); n1[q4 + 3] = fmaf(x[k], wv.w, n1[q4 + 3]);
-                }
-            }
-        }
-        unsigned posmask = 0u;   // sign bits of this thread's pre-activations
-        float s = 0.f, sq = 0.f;
-#pragma unroll
-        for (int i = 0; i < CW; ++i) {
-            if (n1[i] > 0.f) posmask |= 1u << i;
-            n1[i] = act_fwd_t<ACT>(n1[i], a.activation_id);
-            s += n1[i]; sq = fmaf(n1[i], n1[i], sq);
-        }
+        float n1[CW], s, sq;
+        const unsigned posmask = row_fc1<CW, ACT>(x, d, w1t, b1s, cb, a.activation_id, n1, s, sq);
         // the previous tile's GEMM3a / GEMM3b have been in flight up to here.  They must complete before R1 is
         // overwritten below; waiting here rather than there keeps ptxas from placing its own wait inside the divergent
         // slow path of the square root, which would serialise every wgmma of the kernel.
         wgmma_wait<0>();
-        s += other_half(s); sq += other_half(sq);   // LayerNorm-1 statistics of the whole row
-        const float mu1 = s * (1.f / H);
-        const float rstd1 = 1.0f / sqrtf(fmaxf(sq * (1.f / H) - mu1 * mu1, 0.f) + LN_EPS);
-#pragma unroll
-        for (int i = 0; i < CW; ++i) n1[i] = (n1[i] - mu1) * rstd1;
+        row_sum_stats<CW>(s, sq);
+        const LnStats l1 = ln_stats(s, sq);
 
         // GEMM3a / GEMM3b of both warpgroups read every row of R1, R2 and R3: all have completed past this barrier.
         // It also means every thread has read its staged row, which the TMA issued after GEMM1 overwrites.
         __syncthreads();
-#pragma unroll
-        for (int q8 = 0; q8 < CW; q8 += 8) {
-            const uint32_t off = (uint32_t)((cb + q8) >> 3) * PANEL + row * 16;
-            split_store8(R1h + off, R1l + off, n1 + q8, 1.0f);
-        }
+        row_ln1_store<CW>(n1, l1, R1h, R1l, PANEL, row, cb);
         if (half == 0) split_store8(R1h + P_X * PANEL + row * 16, R1l + P_X * PANEL + row * 16, x, SX);
         fence_proxy_async();
         warpgroup_sync(wg);   // GEMM1 reads only this warpgroup's rows of R1
@@ -315,33 +276,14 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         frag_store<64>(z, S + wg * 64 * S_LD, S_LD);
         __syncwarp();   // rows [16 warp, +16) of S: written and read by this warp
 
-        // ---- Z3 (staging tile) + b3f -> LayerNorm-3 -> n3 (registers only) ----
-        float n3[CW];
-#pragma unroll
-        for (int q4 = 0; q4 < CW; q4 += 4) {
-            const float4 v = *reinterpret_cast<const float4*>(S + row * S_LD + cb + q4);
-            n3[q4] = v.x; n3[q4 + 1] = v.y; n3[q4 + 2] = v.z; n3[q4 + 3] = v.w;
-        }
-        float s3 = 0.f, q3 = 0.f;
-#pragma unroll
-        for (int i = 0; i < CW; ++i) { n3[i] += b3f[cb + i]; s3 += n3[i]; q3 = fmaf(n3[i], n3[i], q3); }
-        s3 += other_half(s3); q3 += other_half(q3);
-        const float mu3 = s3 * (1.f / H);
-        const float var3 = fmaxf(q3 * (1.f / H) - mu3 * mu3, 0.f) + LN_EPS;
-        const float rstd3 = 1.0f / sqrtf(var3);
+        // ---- Z3 (staging tile) + b3f -> LayerNorm-3 -> n3 (registers only) -> head ----
+        float n3[CW], s3, q3;
+        row_z3<CW>(S, row, cb, b3f, n3, s3, q3);
+        row_sum_stats<CW>(s3, q3);
+        const LnStats l3 = ln_stats(s3, q3);
         float out[MAX_OUT];
-#pragma unroll
-        for (int j = 0; j < MAX_OUT; ++j) out[j] = 0.f;
-#pragma unroll
-        for (int q4 = 0; q4 < CW; q4 += 4) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) n3[q4 + i] = (n3[q4 + i] - mu3) * rstd3;
-            FOR_OUT(j) {
-                const float4 wv = *reinterpret_cast<const float4*>(whf + j * H + cb + q4);
-                out[j] = fmaf(n3[q4], wv.x, fmaf(n3[q4 + 1], wv.y, fmaf(n3[q4 + 2], wv.z, fmaf(n3[q4 + 3], wv.w, out[j]))));
-            }
-        }
-        FOR_OUT(j) out[j] += other_half(out[j]);   // partial head dots of the two halves
+        row_head<CW, NOUT>(n3, l3, whf, cb, n, out);
+        row_sum_head<CW, NOUT>(out, n);
         // dot[j] = sum_k Whf[j][k] n3[k] (needed by the LayerNorm-3 backward); logits add the folded bias
         float dot[MAX_OUT];
 #pragma unroll
@@ -386,15 +328,15 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
                 }
             }
 #pragma unroll
-            for (int i = 0; i < 8; ++i) g8[i] = rstd3 * (g8[i] - m1 - n3[q8 + i] * m2);
+            for (int i = 0; i < 8; ++i) g8[i] = l3.rstd * (g8[i] - m1 - n3[q8 + i] * m2);
             const uint32_t off = (uint32_t)((cb + q8) >> 3) * PANEL + row * 16;
             split_store8(R2h + off, R2l + off, g8, 1.0f);   // dZ3 row slice
         }
         if (half == 0) {
             float u8[8], c8[8];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) { u8[j] = dl[j] * (rstd3 * (Su * invSz)); c8[j] = 0.f; }
-            c8[0] = 1.0f; c8[1] = mu3; c8[2] = var3 * rstd3;   // std3 = var3 / sqrt(var3)
+            for (int j = 0; j < 8; ++j) { u8[j] = dl[j] * (l3.rstd * (Su * invSz)); c8[j] = 0.f; }
+            c8[0] = 1.0f; c8[1] = l3.mu; c8[2] = l3.var * l3.rstd;   // std3 = var3 / sqrt(var3)
             split_store8(R2h + P_U * PANEL + row * 16, R2l + P_U * PANEL + row * 16, u8, 1.0f);
             split_store8(R1h + P_CST * PANEL + row * 16, R1l + P_CST * PANEL + row * 16, c8, 1.0f);
         }
@@ -435,13 +377,13 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
             float t1 = 0.f, t2 = 0.f;
 #pragma unroll
             for (int i = 0; i < CW; ++i) { t1 += g[i]; t2 = fmaf(g[i], n1[i], t2); }
-            t1 += other_half(t1); t2 += other_half(t2);
+            row_sum_stats<CW>(t1, t2);
             t1 *= (1.f / H); t2 *= (1.f / H);
-            const float std1 = 1.0f / rstd1;
+            const float std1 = 1.0f / l1.rstd;
 #pragma unroll
             for (int i = 0; i < CW; ++i) {
-                const float da = rstd1 * (g[i] - t1 - n1[i] * t2);
-                const float aval = fmaf(n1[i], std1, mu1);                          // activation output
+                const float da = l1.rstd * (g[i] - t1 - n1[i] * t2);
+                const float aval = fmaf(n1[i], std1, l1.mu);                       // activation output
                 g[i] = da * (K1 * act_bwd_t<ACT>(aval, (posmask >> i) & 1u, a.activation_id));
             }
 #pragma unroll

@@ -1,13 +1,14 @@
 #!/usr/bin/env python
-"""Time of the fused CartPole rollout (`orl_rollout`, one launch over T steps) alone, at the C2 shape.
+"""Time of the fused device rollout (`orl_rollout`, one launch over T steps) alone, at the C2 shape.
 
-bench.py's C2 workload (CartPole-v1, T = 128, MLP 64x64, device sampling) at each of `--envs` (default 128 and 4096:
-the latency of one CTA's step chain, and the full grid).  CUDA events around each of `--launches` launches after
+bench.py's C2 workload (T = 128, MLP 64x64, device sampling) on `--env` (default CartPole-v1; GridWorldEnv runs
+rollout_tc_kernel, which no bench workload times) at each of `--envs` (default 128 and 4096: the latency of one CTA's
+step chain, and the full grid).  CUDA events around each of `--launches` launches after
 `--warmup` launches; the env state simply carries on from launch to launch.  Reports microseconds per step (median and
 range over launches), SM cycles per step at the SM clock read right after the timed launches, and the card's name, power
 limit, maximum SM clock and active clock-event (throttle) reasons, read in the same run.  Prints one JSON line.
 
-    python tools/rollout_bench.py [--envs 128,4096 --launches 50 --warmup 10]
+    python tools/rollout_bench.py [--env CartPole-v1 --envs 128,4096 --launches 50 --warmup 10]
 """
 import argparse
 import json
@@ -32,6 +33,7 @@ def smi(fields):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--env", default="CartPole-v1")
     ap.add_argument("--envs", default="128,4096")
     ap.add_argument("--launches", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
@@ -44,10 +46,12 @@ def main():
 
     if not torch.cuda.is_available():
         raise SystemExit("rollout_bench needs a CUDA device")
+    workload = "c2" if args.env == bench.WORKLOADS["c2"]["env"] else "c2_" + args.env
+    bench.WORKLOADS.setdefault(workload, dict(bench.WORKLOADS["c2"], env=args.env))
     out = {"card": torch.cuda.get_device_name(), "name,power_limit,max_sm_clock": smi("name,power.limit,clocks.max.sm"),
-           "T": bench.T, "results": {}}
+           "env": args.env, "T": bench.T, "results": {}}
     for n in (int(x) for x in args.envs.split(",")):
-        cfg, env, net, agent = bench.build_agent(0, 1, "c2", n)
+        cfg, env, net, agent = bench.build_agent(0, 1, workload, n)
         drv = bench.make_driver(cfg, env, net, agent, 0, 1)
         drv.trainer.prep_rollout()
         L, s, T = lib.load(), lib.current_stream(), drv.episode_length

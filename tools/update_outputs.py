@@ -38,8 +38,8 @@ PATHS = {
 }
 
 
-BUFFER = ("actions", "action_log_probs", "policy_obs", "critic_obs", "rewards", "masks", "active_masks", "rnn_states",
-          "rnn_states_critic")
+BUFFER = ("actions", "action_log_probs", "policy_obs", "critic_obs", "rewards", "masks", "active_masks", "value_preds", "returns",
+          "rnn_states", "rnn_states_critic")
 
 
 def state_arrays(driver):
