@@ -13,17 +13,19 @@ from . import nets
 
 
 class ValueNormState:
-    """ValueNorm with norm_axes=1, beta=0.99999 (valuenorm.py:6-106) as three float32 scalars."""
+    """ValueNorm with norm_axes=1, beta=0.99999 (valuenorm.py:6-106) as three scalars: float32 like the reference, or
+    float64 (`dtype`) for a high-precision reference of the update; `device` is where the returns it sees live."""
 
-    def __init__(self, state=None, beta=0.99999):
+    def __init__(self, state=None, beta=0.99999, dtype=torch.float32, device=None):
         self.beta = beta
         s = [0.0, 0.0, 0.0] if state is None else [float(x) for x in state]
-        self.running_mean = torch.tensor([s[0]], dtype=torch.float32)
-        self.running_mean_sq = torch.tensor([s[1]], dtype=torch.float32)
-        self.debiasing_term = torch.tensor(s[2], dtype=torch.float32)
+        self.running_mean = torch.tensor([s[0]], dtype=dtype, device=device)
+        self.running_mean_sq = torch.tensor([s[1]], dtype=dtype, device=device)
+        self.debiasing_term = torch.tensor(s[2], dtype=dtype, device=device)
 
     def state(self):
-        return np.array([self.running_mean.item(), self.running_mean_sq.item(), self.debiasing_term.item()], np.float32)
+        dt = np.float64 if self.running_mean.dtype == torch.float64 else np.float32
+        return np.array([self.running_mean.item(), self.running_mean_sq.item(), self.debiasing_term.item()], dt)
 
     def mean_var(self):
         m = self.running_mean / self.debiasing_term.clamp(min=1e-5)
@@ -85,10 +87,12 @@ def value_loss_fn(cfg, vn, values, value_preds, returns, active):
     return loss.mean()
 
 
-def ppo_update(cfg, pol, cri, opt_p, opt_c, vn, batch):
+def ppo_update(cfg, pol, cri, opt_p, opt_c, vn, batch, record=None):
     """One minibatch update.  batch: dict of torch tensors (critic_obs, policy_obs, actions,
     value_preds, returns, masks, active_masks, old_logp, adv, action_masks[, rnn...]).
-    Returns (value_loss, critic_grad_norm, policy_loss, dist_entropy, actor_grad_norm, ratio_mean)."""
+    Returns (value_loss, critic_grad_norm, policy_loss, dist_entropy, actor_grad_norm, ratio_mean).
+    record: a dict that receives what a kernel's intermediate results are compared with: `grads_policy` /
+    `grads_critic` ({name: gradient before the clip}), the detached `surr` and `ratio` tensors and the losses."""
     opt_p.zero_grad()
     opt_c.zero_grad()
     active = batch["active_masks"]
@@ -119,6 +123,10 @@ def ppo_update(cfg, pol, cri, opt_p, opt_c, vn, batch):
     # 58-62: the second one acts on the already clipped gradients) and the single optimiser steps once
     (policy_loss - ent * cfg.entropy_coef).backward(retain_graph=pol is cri)
     (value_loss * cfg.value_loss_coef).backward()
+    if record is not None:
+        record.update(grads_policy={k: v.grad.detach().clone() for k, v in pol.items()},
+                      grads_critic={k: v.grad.detach().clone() for k, v in cri.items()}, surr=surr.detach(),
+                      ratio=ratio.detach(), policy_loss=policy_loss.detach(), entropy=ent.detach(), value_loss=value_loss.detach())
     if cfg.use_max_grad_norm:
         agn = torch.nn.utils.clip_grad_norm_(list(pol.values()), cfg.max_grad_norm)
         cgn = torch.nn.utils.clip_grad_norm_(list(cri.values()), cfg.max_grad_norm)

@@ -52,12 +52,15 @@ def _rel(x, ref, scale=None):
 class Checker:
     """Collects kernel-vs-float64 errors against the self-calibrated bar; fails with every violation listed."""
 
-    def __init__(self, case):
-        self.case, self.bad, self.worst = case, [], (0.0, "")
+    def __init__(self, case, floor=FLOOR):
+        self.case, self.bad, self.worst, self.floor = case, [], (0.0, ""), floor
+
+    def bar(self, e32):
+        return min(max(RATIO * e32, self.floor), CEIL)
 
     def __call__(self, what, got, r64, r32, scale=None):
         ek, e32 = _rel(got, r64, scale), _rel(r32, r64, scale)
-        bar = min(max(RATIO * e32, FLOOR), CEIL)
+        bar = self.bar(e32)
         ratio = ek / e32 if e32 > 0 else (0.0 if ek == 0 else float("inf"))
         if ratio > self.worst[0]:
             self.worst = (ratio, what)
