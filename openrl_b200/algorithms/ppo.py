@@ -169,7 +169,7 @@ class PPOAlgorithm:
         lib.check(L.orl_share_fwdbwd(a, s), "orl_share_fwdbwd")
         parallel.allreduce_sum_(self.share_bucket)   # gradients + loss sums (no-op on one GPU)
         lib.check(L.orl_share_apply(a, s), "orl_share_apply")
-        self.gpu_launches += 5
+        self.gpu_launches += 6   # fwdbwd, loss sums, tape gemm, tape colsum, row-block sum, apply
 
     def ppo_update(self, buf, batch_rows, indices=None, row_begin=0, mb_stats=None):
         """One minibatch update (ppo.py:46-176) — asynchronous."""

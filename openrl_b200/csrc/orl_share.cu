@@ -79,7 +79,7 @@ __global__ void __launch_bounds__(S_NT) share_values_kernel(const float* __restr
 // HEAD = ORL_HEAD_GAUSSIAN: gaussian_row's per-dimension loss, dL/dmean into the backward and the row's dL/dlogstd into
 // the tape field TS_DLS of the wider Gaussian tape.
 template <int HEAD>
-__global__ void __launch_bounds__(S_NT) share_fwdbwd_kernel(const OrlPpoArgs a, float* __restrict__ tape, float* __restrict__ loss_acc) {
+__global__ void __launch_bounds__(S_NT) share_fwdbwd_kernel(const OrlPpoArgs a, float* __restrict__ tape, float* __restrict__ loss_part) {
     constexpr bool GAUSS = HEAD == ORL_HEAD_GAUSSIAN;
     const long long r = (long long)blockIdx.x * S_NT + threadIdx.x;
     const int d = a.obs_dim, n = a.n_actions;
@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(S_NT) share_fwdbwd_kernel(const OrlPpoArgs a, 
         l_val = vt.loss * wv;
         dc::deep_backward(a.policy_params, o, a.activation_id, sv, a.value_loss_coef * wv * vt.dv, dl, tp);
     }
-    // block sums -> one atomicAdd per block and slot (order across blocks is not fixed: last-ulp noise on the logged sums only)
+    // block sums -> loss_part[block][slot], summed over the blocks by share_loss_sum_kernel
     __shared__ float red[4][S_NT / 32];
     float v[4] = {l_pol, l_ent, l_ratio, l_val};
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -133,8 +133,25 @@ __global__ void __launch_bounds__(S_NT) share_fwdbwd_kernel(const OrlPpoArgs a, 
     if (threadIdx.x < 4) {
         float s = 0.f;
         for (int w = 0; w < S_NT / 32; ++w) s += red[threadIdx.x][w];
-        atomicAdd(loss_acc + threadIdx.x, s);
+        loss_part[(size_t)blockIdx.x * 4 + threadIdx.x] = s;
     }
+}
+
+// The four loss sums over the update's blocks, in double and in a fixed order (deterministic).  One float atomic per
+// block and slot drifted by up to 2e-5 relative at C2's 4096 blocks: the entropy's nearly equal block sums round alike
+// against the growing total.  One CTA of S_NT threads per slot.
+__global__ void __launch_bounds__(S_NT) share_loss_sum_kernel(const float* __restrict__ loss_part, int blocks, float* __restrict__ out) {
+    const int k = blockIdx.x;
+    double s = 0.0;
+    for (int b = threadIdx.x; b < blocks; b += S_NT) s += (double)loss_part[(size_t)b * 4 + k];
+    __shared__ double red[S_NT];
+    red[threadIdx.x] = s;
+    __syncthreads();
+    for (int w = S_NT / 2; w > 0; w >>= 1) {
+        if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) out[k] = (float)red[0];
 }
 
 // ---- parameter gradients from the tape (orl::reduce_tape).  Every gemm job fits its tiles: the Q tiles end by TQ_Y7 + 64
@@ -180,11 +197,13 @@ int orl_share_param_count_head(int obs_dim, int n_actions, int head_kind) {
     return dc::deep_offsets(obs_dim, n_actions, head_kind == ORL_HEAD_GAUSSIAN).total;
 }
 int orl_share_tape_width(void) { return dc::TAPE; }
-/* floats of the update workspace for a minibatch of `rows` rows: tape rows, then reduction partials */
+/* floats of the update workspace for a minibatch of `rows` rows: tape rows, then reduction partials, then the loss sums
+ * of each share_fwdbwd_kernel block */
 long long orl_share_workspace_floats_head(long long rows, int obs_dim, int n_actions, int head_kind) {
     const bool g = head_kind == ORL_HEAD_GAUSSIAN;
     const long long rb = (rows + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK;
-    return rows * dc::tape_width(g) + rb * (long long)((dc::deep_offsets(obs_dim, n_actions, g).total + 3) & ~3);
+    return rows * dc::tape_width(g) + rb * (long long)((dc::deep_offsets(obs_dim, n_actions, g).total + 3) & ~3) +
+           4 * ((rows + S_NT - 1) / S_NT);
 }
 long long orl_share_workspace_floats(long long rows, int obs_dim, int n_actions) {
     return orl_share_workspace_floats_head(rows, obs_dim, n_actions, ORL_HEAD_CATEGORICAL);
@@ -241,6 +260,8 @@ int orl_share_fwdbwd(const OrlPpoArgs* ap, void* stream) {
     ORL_CHECK_ARG(a.policy_params && a.partials && a.folded && a.grads && a.policy_obs && a.actions && a.old_log_probs && a.advantages &&
                       a.value_preds && a.returns && a.active_masks && a.gae_stats && a.mb_stats, "null buffer");
     ORL_CHECK_ARG(a.head_kind == ORL_HEAD_CATEGORICAL || a.head_kind == ORL_HEAD_GAUSSIAN, "head_kind");
+    ORL_CHECK_ARG(!(a.flags & ORL_PPO_VALUENORM) || a.vn_state, "vn_state required with VALUENORM");   // read by mb_consts
+    ORL_CHECK_ARG(a.indices || (a.row_begin >= 0 && a.row_begin + a.batch_rows <= a.total_rows), "row range");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const bool g = a.head_kind == ORL_HEAD_GAUSSIAN;
     const int width = dc::tape_width(g);
@@ -248,12 +269,15 @@ int orl_share_fwdbwd(const OrlPpoArgs* ap, void* stream) {
     const long long rows = a.batch_rows;
     const int total = dc::deep_offsets(a.obs_dim, a.n_actions, g).total, stride = (total + 3) & ~3;
     float* partials = tape + (size_t)rows * width;
+    const unsigned grid = (unsigned)((rows + S_NT - 1) / S_NT);
+    float* loss_part = partials + (size_t)((rows + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK) * stride;
     int e = orl::check_cuda(cudaMemsetAsync(a.folded, 0, 8 * sizeof(float), st), "memset loss sums");
     if (e) return e;
-    const unsigned grid = (unsigned)((rows + S_NT - 1) / S_NT);
-    if (g) share_fwdbwd_kernel<ORL_HEAD_GAUSSIAN><<<grid, S_NT, 0, st>>>(a, tape, a.folded);
-    else share_fwdbwd_kernel<ORL_HEAD_CATEGORICAL><<<grid, S_NT, 0, st>>>(a, tape, a.folded);
+    if (g) share_fwdbwd_kernel<ORL_HEAD_GAUSSIAN><<<grid, S_NT, 0, st>>>(a, tape, loss_part);
+    else share_fwdbwd_kernel<ORL_HEAD_CATEGORICAL><<<grid, S_NT, 0, st>>>(a, tape, loss_part);
     ORL_LAUNCH_CHECK("share_fwdbwd_kernel");
+    share_loss_sum_kernel<<<4, S_NT, 0, st>>>(loss_part, (int)grid, a.folded);
+    ORL_LAUNCH_CHECK("share_loss_sum_kernel");
     return orl::reduce_tape(tape, width, rows, make_share_jobs(a.obs_dim, a.n_actions, g), partials, stride, total, a.grads, st);
 }
 
@@ -263,6 +287,7 @@ int orl_share_apply(const OrlPpoArgs* ap, void* stream) {
     ORL_CHECK_ARG(a.policy_params && a.policy_adam_m && a.policy_adam_v && a.adam_steps && a.lrs && a.grads && a.folded && a.train_info && a.mb_stats,
                   "null buffer");
     ORL_CHECK_ARG(a.head_kind == ORL_HEAD_CATEGORICAL || a.head_kind == ORL_HEAD_GAUSSIAN, "head_kind");
+    ORL_CHECK_ARG(!(a.flags & ORL_PPO_VALUENORM) || a.vn_state, "vn_state required with VALUENORM");   // written by add_value_info
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (a.head_kind == ORL_HEAD_GAUSSIAN) share_apply_kernel<ORL_HEAD_GAUSSIAN><<<1, 1024, 0, st>>>(a, a.folded);
     else share_apply_kernel<ORL_HEAD_CATEGORICAL><<<1, 1024, 0, st>>>(a, a.folded);

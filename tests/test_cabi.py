@@ -60,3 +60,27 @@ def test_bad_arguments_are_reported_not_crashed(orl_lib):
     a.critic_obs = fake + 4
     assert orl_lib.orl_rnn_rollout(a, None) == 10001
     assert b"16-byte aligned" in orl_lib.orl_last_error()
+
+
+def test_share_update_refuses_what_the_ffma_update_refuses(orl_lib):
+    """orl_share_fwdbwd / orl_share_apply refuse, before any launch, ValueNorm without a vn_state (the update reads it
+    for the value targets, the optimiser step writes it back) and a contiguous row range past the buffer's end."""
+    from openrl_b200 import lib
+
+    fake = 1 << 20   # never dereferenced
+    a = lib.OrlPpoArgs()
+    a.obs_dim, a.critic_obs_dim, a.n_actions, a.activation_id, a.head_kind = 4, 4, 2, 1, lib.HEAD_CATEGORICAL
+    a.grid_per_net, a.batch_rows, a.row_begin, a.total_rows = 1, 1024, 0, 1024
+    for name in ("policy_params", "critic_params", "partials", "folded", "grads", "policy_obs", "critic_obs", "actions",
+                 "old_log_probs", "advantages", "value_preds", "returns", "active_masks", "gae_stats", "mb_stats",
+                 "policy_adam_m", "policy_adam_v", "critic_adam_m", "critic_adam_v", "adam_steps", "lrs", "train_info"):
+        setattr(a, name, fake)
+    a.flags, a.vn_state = lib.PPO_VALUENORM, None
+    for fn in (orl_lib.orl_share_fwdbwd, orl_lib.orl_share_apply):
+        assert fn(a, None) == 10001
+        assert b"vn_state" in orl_lib.orl_last_error()
+    a.vn_state = fake
+    for begin, rows in ((1, 1024), (0, 1025), (-1, 4)):
+        a.row_begin, a.batch_rows = begin, rows
+        assert orl_lib.orl_share_fwdbwd(a, None) == 10001
+        assert b"row range" in orl_lib.orl_last_error()
