@@ -32,7 +32,10 @@
 // fp16 carries 22 significand bits as hi + lo only while hi >= 2^-3 (below, lo is subnormal), so every backward
 // operand is scaled by a power of two chosen per minibatch to put its TYPICAL magnitude near 2^4: dZ3 / dZ1 by
 // S_z ~ 8 rows / max|Whf| (head weights are tiny: gain 0.01), U by S_u ~ 8 rows, observations by 16; the accumulators
-// are multiplied by the exact inverse when flushed, conversions saturate instead of overflowing.
+// are multiplied by the exact inverse when flushed, conversions saturate instead of overflowing.  `rows` is the count
+// the row weights divide by: sum(active) of the minibatch when the net's active-mask option is on (a live row then
+// weighs active / sum(active)), else the row count.  Headroom: a scaled operand reaches 65504 at ~2^12 times its
+// typical size, i.e. when |dL/dlogit| x rstd3 of a row is ~4000 times that of a unit-advantage row.
 //
 // Minibatch tiles are staged in shared memory one tile ahead: TMA (cp.async.bulk.tensor: the 128 x d
 // observation tile and the scalar columns, zero-filled past the end) when the minibatch is a contiguous
@@ -152,7 +155,9 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     // operand scales of the backward GEMMs (powers of two; see the header comment)
     float wmax = 0.f;
     for (int i = 0; i < MAX_OUT * H; ++i) wmax = fmaxf(wmax, fabsf(whf[i]));   // smem broadcast reads, once per kernel
-    const int e_rows = (int)ceil(log2(fmax(rows_d, 1.0)));
+    // with active masks a live row weighs active / sum(active), not 1 / rows: scale by the rows that carry the weight
+    const double live_d = (POLICY ? pol_masks : val_masks) ? fmin(rows_d, a.mb_stats[2]) : rows_d;
+    const int e_rows = (int)ceil(log2(fmax(live_d, 1.0)));
     const int e_u = min(e_rows + 3, 60);
     const int e_z = min(max(e_rows + 3 - (int)floorf(log2f(fmaxf(wmax, 1e-12f))), 0), 60);
     const float Sz = exp2f((float)e_z), Su = exp2f((float)e_u);
@@ -229,6 +234,13 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         } else {
 #pragma unroll
             for (int k = 0; k < 8; ++k) if (k < d) x[k] = st_obs[row * d + k];
+        }
+        // rows past the minibatch's end: the gather zero-fills them, TMA loads whatever the buffer holds there (the
+        // partial last tile of a range that ends inside the buffer).  Their dL is 0, but a NaN or inf in x would still
+        // reach GEMM3a / GEMM3b through n1 and the X panel (0 x NaN), so they run on x = 0 on both paths.
+        if (!valid) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] = 0.f;
         }
         const float row_a = st_sc[0 * T_M + row], row_b = st_sc[1 * T_M + row];
         const float row_c = POLICY ? st_sc[2 * T_M + row] : 0.f, active = st_sc[3 * T_M + row];
