@@ -14,12 +14,12 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 def main():
     from oracle import loop_ma
     from openrl_b200.utils.logger import Logger
-    from test_rollout_cuda import _product
+    from helpers import product
 
     d = np.load(os.path.join(ROOT, "tests", "golden", "trace_mpe_gru.npz"), allow_pickle=True)
     N = int(d["meta/env_num"])
     flags = str(d["meta/flags"]).split()
-    cfg, env, net, agent = _product("simple_spread", N, flags, golden=d)
+    cfg, env, net, agent = product("simple_spread", N, flags, golden=d)
     agent.train(total_time_steps=0, logger=Logger(quiet=True))
     drv = agent.driver
     b = drv.buffer.data

@@ -14,45 +14,31 @@ norms, the reported ratio mean, and the parameters, Adam moments, step counts an
 Adam step.
 """
 import contextlib
-import math
 import types
 from unittest import mock
 
 import numpy as np
 import torch
 
+import param_layout as layout
 import rnn_ref64
 from oracle import nets, ppo as oppo
 
-H = 64
+H = layout.H
 
 
 def param_shapes(d, n, head):
     """(state_dict name, shape) in the order of the flat parameter buffer; head: "gaussian", "categorical" or "critic"."""
-    out = [("base.mlp.fc1.0.weight", (H, d)), ("base.mlp.fc1.0.bias", (H,)),
-           ("base.mlp.fc1.2.weight", (H,)), ("base.mlp.fc1.2.bias", (H,)),
-           ("base.mlp.fc3.0.weight", (H, H)), ("base.mlp.fc3.0.bias", (H,)),
-           ("base.mlp.fc3.1.weight", (H,)), ("base.mlp.fc3.1.bias", (H,))]
-    if head == "critic":
-        return out + [("v_out.weight", (1, H)), ("v_out.bias", (1,))]
-    if head == "gaussian":
-        return out + [("act.action_out.fc_mean.weight", (n, H)), ("act.action_out.fc_mean.bias", (n,)),
-                      ("act.action_out.logstd._bias", (n, 1))]
-    return out + [("act.action_out.linear.weight", (n, H)), ("act.action_out.linear.bias", (n,))]
+    return layout.mlp_trunk(d) + layout.head(n, head)
 
 
 def blocks(d, n, head):
     """{name: slice of the flat buffer} in flat order."""
-    out, off = {}, 0
-    for name, shp in param_shapes(d, n, head):
-        k = math.prod(shp)
-        out[name] = slice(off, off + k)
-        off += k
-    return out
+    return layout.blocks(param_shapes(d, n, head))
 
 
 def unflatten(flat, d, n, head):
-    return {name: flat[s].reshape(shp).clone() for (name, shp), s in zip(param_shapes(d, n, head), blocks(d, n, head).values())}
+    return layout.unflatten(flat, param_shapes(d, n, head))
 
 
 def f32(x):
@@ -125,7 +111,8 @@ def _mutant_eval(kind):
     return f
 
 
-def update(cfg, buf, state, rows, dims, head, dtype=torch.float64, vn_beta=0.99999, mutant=None, dropped_rows=None):
+def update(cfg, buf, state, rows, dims, head, dtype=torch.float64, vn_beta=0.99999, mutant=None, dropped_rows=None,
+           functional=None):
     """One minibatch update in `dtype` on the buffer rows `rows`.
 
     cfg: the project's option names (clip_param, entropy_coef, ..., use_valuenorm, use_adv_normalize, a2c).
@@ -134,7 +121,9 @@ def update(cfg, buf, state, rows, dims, head, dtype=torch.float64, vn_beta=0.999
     state: flat parameters pol / cri, Adam moments pol_m, pol_v, cri_m, cri_v, step counts steps = (pol, cri), ValueNorm
       state vn (3,).  dims: (d, n, dc); head: "gaussian" or "categorical".
     mutant: a key of MUTANTS; "cta-last-tile-dropped" leaves out `dropped_rows` (a subset of `rows`) while keeping
-      the minibatch's loss weights."""
+      the minibatch's loss weights.
+    functional: None, or functional(pol, cri) -> the stand-in for torch.nn.functional that oracle/nets.py runs the
+      update under, given the two nets' parameter dicts (tests/tc_ref64.py records the layer calls with it)."""
     d, n, dc = dims
     dev = rows.device
     cast = lambda x: torch.as_tensor(x).to(device=dev, dtype=dtype)   # noqa: E731
@@ -159,13 +148,14 @@ def update(cfg, buf, state, rows, dims, head, dtype=torch.float64, vn_beta=0.999
                  value_preds=g("value_preds"), returns=g("returns"), active_masks=g("active_masks"), adv=adv[rows])
     if "action_masks" in buf:
         batch["action_masks"] = g("action_masks")
-    patch = contextlib.nullcontext()
-    if mutant in ("entropy-weight-1/rows", "one-ratio-per-row", "logstd-grad-without-entropy"):
-        patch = mock.patch.object(nets, "policy_eval_gaussian", _mutant_eval(mutant))
-        if mutant == "one-ratio-per-row":
-            batch["old_logp"] = batch["old_logp"].sum(-1, keepdim=True)
     rec = {}
-    with patch:
+    with contextlib.ExitStack() as patches:
+        if mutant in ("entropy-weight-1/rows", "one-ratio-per-row", "logstd-grad-without-entropy"):
+            patches.enter_context(mock.patch.object(nets, "policy_eval_gaussian", _mutant_eval(mutant)))
+            if mutant == "one-ratio-per-row":
+                batch["old_logp"] = batch["old_logp"].sum(-1, keepdim=True)
+        if functional is not None:
+            patches.enter_context(mock.patch.object(nets, "F", functional(pol, cri)))
         oppo.ppo_update(ocfg, pol, cri, opt_p, opt_c, vn, batch, record=rec)
 
     gp = torch.cat([x.reshape(-1) for x in rec["grads_policy"].values()])

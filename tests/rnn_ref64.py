@@ -20,39 +20,29 @@ import types
 
 import torch
 
+import param_layout as layout
 from oracle import nets
 
-H = 64
+H = layout.H
 
 
 def param_shapes(d, n, critic):
     """(state_dict name, shape) of a recurrent policy (head width n) or critic net on d-wide observations, in the
     order of the flat parameter buffer (orl_rnn_core.h rnn_offsets)."""
-    head = ([("v_out.weight", (1, H)), ("v_out.bias", (1,))] if critic else
-            [("act.action_out.linear.weight", (n, H)), ("act.action_out.linear.bias", (n,))])
-    return [("base.mlp.fc1.0.weight", (H, d)), ("base.mlp.fc1.0.bias", (H,)),
-            ("base.mlp.fc1.2.weight", (H,)), ("base.mlp.fc1.2.bias", (H,)),
-            ("base.mlp.fc3.0.weight", (H, H)), ("base.mlp.fc3.0.bias", (H,)),
-            ("base.mlp.fc3.1.weight", (H,)), ("base.mlp.fc3.1.bias", (H,)),
-            ("rnn.rnn.weight_ih_l0", (3 * H, H)), ("rnn.rnn.weight_hh_l0", (3 * H, H)),
-            ("rnn.rnn.bias_ih_l0", (3 * H,)), ("rnn.rnn.bias_hh_l0", (3 * H,)),
-            ("rnn.norm.weight", (H,)), ("rnn.norm.bias", (H,))] + head
+    return (layout.mlp_trunk(d) + [("rnn.rnn.weight_ih_l0", (3 * H, H)), ("rnn.rnn.weight_hh_l0", (3 * H, H)),
+                                   ("rnn.rnn.bias_ih_l0", (3 * H,)), ("rnn.rnn.bias_hh_l0", (3 * H,)),
+                                   ("rnn.norm.weight", (H,)), ("rnn.norm.bias", (H,))]
+            + layout.head(n, "critic" if critic else "categorical"))
 
 
 def blocks(d, n, critic):
     """{name: slice of the flat buffer} in flat order."""
-    out, off = {}, 0
-    for name, shp in param_shapes(d, n, critic):
-        k = math.prod(shp)
-        out[name] = slice(off, off + k)
-        off += k
-    return out
+    return layout.blocks(param_shapes(d, n, critic))
 
 
 def unflatten(flat, d, n, critic):
     """Leaf tensors (requires_grad) viewing copies of the flat buffer, keyed by state_dict name."""
-    return {name: flat[s].clone().view(shp).requires_grad_(True)
-            for (name, shp), s in zip(param_shapes(d, n, critic), blocks(d, n, critic).values())}
+    return {name: x.requires_grad_(True) for name, x in layout.unflatten(flat, param_shapes(d, n, critic)).items()}
 
 
 def rows(x):

@@ -24,10 +24,11 @@ import types
 
 import numpy as np
 
+import param_layout as layout
 from oracle.selfplay import COLS, GOAL, MAX_STEPS, ROWS, _move
-from test_action_noise_cuda import philox4x32_10, philox_units
+from helpers import philox4x32_10, philox_units
 
-H = 64
+H = layout.H
 N_ACTIONS = 5
 LN_EPS = 1e-5
 TIE_RTOL = 1e-5
@@ -43,11 +44,7 @@ _MOVE = np.array([[[_move(x, y, a) for a in range(N_ACTIONS)] for y in range(COL
 
 def param_shapes(n=N_ACTIONS, d=4):
     """(state_dict name, shape) of the policy in the order of its flat parameter buffer (orl_mlp.cuh net_offsets)."""
-    return [("base.mlp.fc1.0.weight", (H, d)), ("base.mlp.fc1.0.bias", (H,)),
-            ("base.mlp.fc1.2.weight", (H,)), ("base.mlp.fc1.2.bias", (H,)),
-            ("base.mlp.fc3.0.weight", (H, H)), ("base.mlp.fc3.0.bias", (H,)),
-            ("base.mlp.fc3.1.weight", (H,)), ("base.mlp.fc3.1.bias", (H,)),
-            ("act.action_out.linear.weight", (n, H)), ("act.action_out.linear.bias", (n,))]
+    return layout.mlp_trunk(d) + layout.head(n, "categorical")
 
 
 def param_count(n=N_ACTIONS, d=4):

@@ -18,46 +18,32 @@ PolicyValueNetwork, logstd last):
 - the parameters, exp_avg, exp_avg_sq and step count after the clip-twice-then-Adam step, and the ValueNorm state.
 """
 import contextlib
-import math
 from unittest import mock
 
 import torch
 import torch.nn.functional as F
 
 import ffma_ref64
+import param_layout as layout
 import rnn_ref64
 from oracle import nets, ppo as oppo
 
-H = 64
+H = layout.H
 TAPE_ROW_BLOCK = 1024   # rows per partial sum of the tape reduction (orl_tape.cu)
 
 
 def param_shapes(d, n, head):
     """(state_dict name, shape) in the order of the flat parameter buffer; head: "gaussian" or "categorical"."""
-    out = []
-    for pre, width in (("obs_prep.mlp.", d), ("common.", H)):
-        out += [(pre + "fc1.0.weight", (H, width)), (pre + "fc1.0.bias", (H,)), (pre + "fc1.2.weight", (H,)),
-                (pre + "fc1.2.bias", (H,)), (pre + "fc3.0.weight", (H, H)), (pre + "fc3.0.bias", (H,)),
-                (pre + "fc3.1.weight", (H,)), (pre + "fc3.1.bias", (H,))]
-    out += [("v_out.weight", (1, H)), ("v_out.bias", (1,))]
-    if head == "gaussian":
-        return out + [("act.action_out.fc_mean.weight", (n, H)), ("act.action_out.fc_mean.bias", (n,)),
-                      ("act.action_out.logstd._bias", (n, 1))]
-    return out + [("act.action_out.linear.weight", (n, H)), ("act.action_out.linear.bias", (n,))]
+    return layout.mlp_trunk(d, "obs_prep.mlp.") + layout.mlp_trunk(H, "common.") + layout.head(1, "critic") + layout.head(n, head)
 
 
 def blocks(d, n, head):
     """{state_dict name: slice of the flat buffer} in flat order."""
-    out, off = {}, 0
-    for name, shp in param_shapes(d, n, head):
-        k = math.prod(shp)
-        out[name] = slice(off, off + k)
-        off += k
-    return out
+    return layout.blocks(param_shapes(d, n, head))
 
 
 def unflatten(flat, d, n, head):
-    return {name: flat[s].reshape(shp).clone() for (name, shp), s in zip(param_shapes(d, n, head), blocks(d, n, head).values())}
+    return layout.unflatten(flat, param_shapes(d, n, head))
 
 
 class _BatchReturnsValueNorm(oppo.ValueNormState):

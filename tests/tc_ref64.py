@@ -16,13 +16,11 @@ and, per net, the peaks of the backward operands the kernel converts to split fp
 fc1 output, U = dL/dhead * rstd3) before its per-minibatch power-of-two scales are applied (`operand_scales`).
 """
 import math
-from unittest import mock
 
 import torch
 import torch.nn.functional as F
 
 import ffma_ref64 as ref
-from oracle import nets
 
 H = ref.H
 FP16_MAX = 65504.0   # the largest finite fp16: split conversions saturate here (cvt.rn.satfinite)
@@ -128,31 +126,15 @@ def update(cfg, buf, state, rows, dims, dtype=torch.float64, vn_beta=0.99999, cl
     """ffma_ref64.update with a Categorical head, plus `terms_pol` / `terms_cri` ({block: (signed row-term sum, sum of the
     absolute row terms)}, both flattened in the kernel's order; S_block is the norm of the second)
     and `peaks` ({"pol" | "cri": operand peaks}).  clamp_dz3: {"pol" | "cri": limit} clamps dL/d fc3-output of that net."""
-    caps = {}
-    real_unflatten = ref.unflatten
-
-    def unflatten(flat, d, n, head):   # the two nets' parameter dicts, as ffma_ref64.update builds them
-        p = real_unflatten(flat, d, n, head)
-        caps.setdefault("cri" if head == "critic" else "pol", p)   # the parameters come first, then the Adam moments
-        return p
-
     captures = []
 
-    class _Both(_Capture):
-        def __init__(self):
-            names = {**caps["pol"], **{"cri." + k: v for k, v in caps["cri"].items()}}
-            lim = {("cri." if k == "cri" else "") + "base.mlp.fc3.0.weight": v for k, v in (clamp_dz3 or {}).items()}
-            super().__init__(names, lim)
-            captures.append(self)
+    def functional(pol, cri):
+        names = {**pol, **{"cri." + k: v for k, v in cri.items()}}
+        lim = {("cri." if k == "cri" else "") + "base.mlp.fc3.0.weight": v for k, v in (clamp_dz3 or {}).items()}
+        captures.append(_Capture(names, lim))
+        return captures[-1]
 
-    real_ppo_update = ref.oppo.ppo_update
-
-    def ppo_update(*a, **kw):
-        with mock.patch.object(nets, "F", _Both()):
-            return real_ppo_update(*a, **kw)
-
-    with mock.patch.object(ref, "unflatten", unflatten), mock.patch.object(ref.oppo, "ppo_update", ppo_update):
-        out = ref.update(cfg, buf, state, rows, dims, "categorical", dtype, vn_beta=vn_beta)
+    out = ref.update(cfg, buf, state, rows, dims, "categorical", dtype, vn_beta=vn_beta, functional=functional)
     calls = captures[0].calls
     pol_calls = [c for c in calls if not c[1].startswith("cri.")]
     cri_calls = [(k, w[4:], b[4:] if b else b, x, y) for k, w, b, x, y in calls if w.startswith("cri.")]

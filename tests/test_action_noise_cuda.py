@@ -10,35 +10,13 @@ is compared up to its first such tie (the trajectories part there)."""
 import numpy as np
 import pytest
 
+from helpers import philox_units
+
 pytestmark = pytest.mark.gpu
 
 SEED = 0x1234_5678_9ABC
 STEP_BASE = (1 << 32) + 77      # the high step word must reach the counter
 ROW_OFFSET = 1000               # and so must rng_row_offset
-M32 = np.uint64(0xFFFFFFFF)
-
-
-def philox4x32_10(c0, c1, c2, c3, seed):
-    """Philox4x32-10 on uint64 arrays holding 32-bit words (the device's philox4x32_10)."""
-    c = [np.asarray(x, np.uint64) & M32 for x in np.broadcast_arrays(c0, c1, c2, c3)]
-    k0, k1 = np.uint64(seed & 0xFFFFFFFF), np.uint64((seed >> 32) & 0xFFFFFFFF)
-    for _ in range(10):
-        p0, p1 = np.uint64(0xD2511F53) * c[0], np.uint64(0xCD9E8D57) * c[2]
-        c = [(p1 >> np.uint64(32)) ^ c[1] ^ k0, p1 & M32, (p0 >> np.uint64(32)) ^ c[3] ^ k1, p0 & M32]
-        k0, k1 = (k0 + np.uint64(0x9E3779B9)) & M32, (k1 + np.uint64(0xBB67AE85)) & M32
-    return c
-
-
-def philox_units(T, rows, seed, step_base, row_offset, lanes):
-    """(T, rows, 4 * len(lanes)) float32 uniforms in (0, 1): the four words of each Philox lane in `lanes`, keyed as the
-    device's action_philox keys them (step = step_base + t, row = row + row_offset) and mapped by u32_to_unit_open."""
-    step = np.uint64(step_base) + np.arange(T, dtype=np.uint64)[:, None]
-    row = np.uint64(row_offset) + np.arange(rows, dtype=np.uint64)[None, :]
-    words = []
-    for lane in lanes:
-        words += philox4x32_10(step & M32, step >> np.uint64(32), row, np.uint64(lane), seed)
-    u = np.stack(words, -1)
-    return ((u >> np.uint64(8)).astype(np.float32) + np.float32(0.5)) * np.float32(1.0 / 16777216.0)
 
 
 def noise_table(T, rows, n, seed, step_base, row_offset):

@@ -2,58 +2,20 @@
 (openrl_b200/csrc/orl_deep_core.h) compiled with g++ and checked on the CPU against torch autograd of the oracle
 (oracle/nets.py: PolicyValueNetwork restatement, pinned to the reference trace tests/golden/trace_share_model.npz):
 forward heads, and every parameter gradient obtained from the per-row tape as dW = sum_rows P^T Q / column sums."""
-import ctypes
-import os
-import subprocess
-
 import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT
+from helpers import grads_from_tape, gxx_shim, ptr
 from oracle import loop, nets
 
 
 @pytest.fixture(scope="module")
 def shim(tmp_path_factory):
-    out = tmp_path_factory.mktemp("deep") / "libdeepshim.so"
-    subprocess.run(["g++", "-O2", "-shared", "-fPIC", "-I", os.path.join(ROOT, "openrl_b200", "csrc"),
-                    os.path.join(ROOT, "tests", "deep_core_shim.cpp"), "-o", str(out)], check=True)
-    return ctypes.CDLL(str(out))
-
-
-def _ptr(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
+    return gxx_shim(tmp_path_factory, "deep", "deep_core_shim.cpp")
 
 
 # tape field offsets (orl_deep_core.h)
-TP_DZ1, TP_DZ3, TP_DZ5, TP_DZ7, TP_DLOG, TP_DV = 0, 64, 128, 192, 256, 264
-TQ_X, TQ_Y1, TQ_Y3, TQ_Y5, TQ_Y7 = 272, 336, 400, 464, 528
-TS = dict(DY1N1=592, DY1=656, DY3N3=720, DY3=784, DY5N5=848, DY5=912, DY7N7=976, DY7=1040)
-
-
-def grads_from_tape(tape, d, n):
-    g = {}
-    P = lambda off, m: tape[:, off:off + m]   # noqa: E731
-    g["obs_prep.mlp.fc1.0.weight"] = P(TP_DZ1, 64).T @ P(TQ_X, d)
-    g["obs_prep.mlp.fc1.0.bias"] = P(TP_DZ1, 64).sum(0)
-    g["obs_prep.mlp.fc1.2.weight"], g["obs_prep.mlp.fc1.2.bias"] = P(TS["DY1N1"], 64).sum(0), P(TS["DY1"], 64).sum(0)
-    g["obs_prep.mlp.fc3.0.weight"] = P(TP_DZ3, 64).T @ P(TQ_Y1, 64)
-    g["obs_prep.mlp.fc3.0.bias"] = P(TP_DZ3, 64).sum(0)
-    g["obs_prep.mlp.fc3.1.weight"], g["obs_prep.mlp.fc3.1.bias"] = P(TS["DY3N3"], 64).sum(0), P(TS["DY3"], 64).sum(0)
-    g["common.fc1.0.weight"] = P(TP_DZ5, 64).T @ P(TQ_Y3, 64)
-    g["common.fc1.0.bias"] = P(TP_DZ5, 64).sum(0)
-    g["common.fc1.2.weight"], g["common.fc1.2.bias"] = P(TS["DY5N5"], 64).sum(0), P(TS["DY5"], 64).sum(0)
-    g["common.fc3.0.weight"] = P(TP_DZ7, 64).T @ P(TQ_Y5, 64)
-    g["common.fc3.0.bias"] = P(TP_DZ7, 64).sum(0)
-    g["common.fc3.1.weight"], g["common.fc3.1.bias"] = P(TS["DY7N7"], 64).sum(0), P(TS["DY7"], 64).sum(0)
-    g["v_out.weight"] = P(TP_DV, 1).T @ P(TQ_Y7, 64)
-    g["v_out.bias"] = P(TP_DV, 1).sum(0)
-    g["act.action_out.linear.weight"] = P(TP_DLOG, n).T @ P(TQ_Y7, 64)
-    g["act.action_out.linear.bias"] = P(TP_DLOG, n).sum(0)
-    return g
-
-
 @pytest.mark.parametrize("d,n,act", [(4, 2, 1), (7, 5, 0), (18, 3, 3), (4, 8, 2)])
 def test_deep_core_forward_backward_matches_torch(shim, d, n, act):
     torch.manual_seed(0)
@@ -77,7 +39,7 @@ def test_deep_core_forward_backward_matches_torch(shim, d, n, act):
     tape = np.zeros((rows, T), np.float32)
     v_out, l_out = np.zeros(rows, np.float32), np.zeros((rows, n), np.float32)
     Xn, dvn, dln = X.numpy().copy(), dv.numpy().reshape(-1).copy(), dlog.numpy().copy()
-    shim.shim_deep_rows(_ptr(P), d, n, act, rows, _ptr(Xn), _ptr(v_out), _ptr(l_out), _ptr(dvn), _ptr(dln), _ptr(tape))
+    shim.shim_deep_rows(ptr(P), d, n, act, rows, ptr(Xn), ptr(v_out), ptr(l_out), ptr(dvn), ptr(dln), ptr(tape))
     np.testing.assert_allclose(v_out, values.detach().numpy().reshape(-1), rtol=1e-5, atol=5e-6)
     np.testing.assert_allclose(l_out, logits.detach().numpy(), rtol=1e-5, atol=5e-6)
     got = grads_from_tape(tape.astype(np.float64), d, n)

@@ -10,17 +10,8 @@ import pytest
 import torch
 
 from conftest import GOLDEN
+from helpers import trace_threads  # noqa: F401  (autouse fixture)
 from oracle import loop
-
-TRACE_THREADS = 8   # the recording thread count (tests/test_oracle_loop.py)
-
-
-@pytest.fixture(autouse=True)
-def _trace_threads():
-    before = torch.get_num_threads()
-    torch.set_num_threads(TRACE_THREADS)
-    yield
-    torch.set_num_threads(before)
 
 
 @pytest.mark.parametrize("tag", ["dict_obs_ff", "dict_obs_gru"])

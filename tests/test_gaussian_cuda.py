@@ -8,6 +8,8 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN
+from helpers import SyntheticHost, make_agent
+from openrl_b200.envs.vec_env import HostVecEnv
 
 pytestmark = pytest.mark.gpu
 
@@ -32,60 +34,14 @@ class _IdentityHost:
         return o, r, d, [{} for _ in range(self.parallel_env_num)]
 
 
-class _SyntheticHost:
-    """BASELINE.md config 5 stand-in (mujoco is absent): obs ~ N(0,1) (N,1,17), reward ~ N(0,1),
-    done ~ Bernoulli(1/1000), Box(6) actions."""
-
-    def __init__(self, n, obs_dim=17, act_dim=6, seed=0):
-        from openrl_b200 import spaces
-
-        self.parallel_env_num, self.agent_num = n, 1
-        self.observation_space = spaces.Box(-np.inf, np.inf, (obs_dim,), np.float32)
-        self.action_space = spaces.Box(-1, 1, (act_dim,), np.float32)
-        self.rng = np.random.default_rng(seed)
-        self.obs_dim = obs_dim
-
-    def reset(self, seed=None):
-        if seed is not None:
-            self.rng = np.random.default_rng(seed)
-        return self.rng.standard_normal((self.parallel_env_num, 1, self.obs_dim)).astype(np.float32)
-
-    def step(self, actions):
-        assert actions.shape == (self.parallel_env_num, 1, 6) and np.isfinite(actions).all()
-        n = self.parallel_env_num
-        return (self.rng.standard_normal((n, 1, self.obs_dim)).astype(np.float32), self.rng.standard_normal((n, 1, 1)),
-                self.rng.random((n, 1)) < 1e-3, [{} for _ in range(n)])
-
-
-def _agent(host_env, flags, golden=None):
-    import torch
-
-    from openrl_b200.configs.config import create_config_parser
-    from openrl_b200.envs.vec_env import HostVecEnv
-    from openrl_b200.modules.common import PPONet
-    from openrl_b200.runners.common import PPOAgent
-
-    cfg = create_config_parser().parse_args(flags)
-    cfg.quiet = True
-    env = HostVecEnv(host_env)
-    net = PPONet(env, cfg=cfg, device="cuda:0")
-    if golden is not None:
-        for mk in ("policy", "critic"):
-            sd = net.module.models[mk].state_dict()
-            for k in list(sd.keys()):
-                gk = f"init/{mk}.{k}"
-                if gk in golden:
-                    sd[k].copy_(torch.from_numpy(golden[gk]))
-    return cfg, env, net, PPOAgent(net)
-
-
 def test_gaussian_head_host_env_matches_reference_trace(cuda):
     from openrl_b200.utils.logger import Logger
 
     d = np.load(os.path.join(GOLDEN, "trace_identity_continuous.npz"), allow_pickle=True)
     iters, N = int(d["meta/iters"]), int(d["meta/env_num"])
     flags = str(d["meta/flags"]).split() + ["--parity_mode", "true", "--log_interval", "1"]
-    cfg, env, net, agent = _agent(_IdentityHost(N), flags, golden=d)
+    env = HostVecEnv(_IdentityHost(N))
+    cfg, net, agent = make_agent(env, flags, golden=d, start=False)
     # same parameter tree as the reference (incl. act.action_out.logstd._bias)
     keys = [k for k, _ in net.module.models["policy"].named_parameters()]
     assert keys[-3:] == ["act.action_out.fc_mean.weight", "act.action_out.fc_mean.bias", "act.action_out.logstd._bias"]
@@ -113,7 +69,8 @@ def test_config5_shape_runs(cuda):
     from openrl_b200.utils.logger import Logger
 
     flags = ["--seed", "1", "--episode_length", "16", "--ppo_epoch", "2", "--log_interval", "1"]
-    cfg, env, net, agent = _agent(_SyntheticHost(1024), flags)
+    env = HostVecEnv(SyntheticHost(1024))
+    cfg, net, agent = make_agent(env, flags, start=False)
     logger = Logger(quiet=True)
     agent.train(total_time_steps=16 * 1024 * 2, logger=logger)
     logs = [h[1] for h in logger.history if "value_loss" in h[1]]
@@ -133,7 +90,7 @@ def test_host_rollout_grouped_and_synchronous_fill_the_buffer_identically(cuda, 
     from openrl_b200.modules.common import PPONet
     from openrl_b200.runners.common import PPOAgent
     from openrl_b200.utils.logger import Logger
-    from test_host_sync_env import CountEnv
+    from helpers import CountEnv
 
     T, N, H = 12, 10, 5
     cfg = create_config_parser().parse_args(["--seed", "0", "--episode_length", str(T), "--ppo_epoch", "1", "--host_env_groups", grouped,

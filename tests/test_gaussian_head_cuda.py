@@ -12,7 +12,7 @@ bit for bit against their float32 closed forms."""
 import numpy as np
 import pytest
 
-from test_action_noise_cuda import philox_units
+from helpers import philox_units
 
 pytestmark = pytest.mark.gpu
 

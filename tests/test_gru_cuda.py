@@ -12,10 +12,9 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN
+from helpers import check_recurrent_trace
 
 pytestmark = pytest.mark.gpu
-
-KEYS = ["value_loss", "critic_grad_norm", "policy_loss", "dist_entropy", "actor_grad_norm", "ratio"]
 
 
 def _oracle_params(model):
@@ -38,9 +37,9 @@ def test_recurrent_act_matches_oracle(cuda):
     import torch
 
     from oracle import nets
-    from test_rollout_cuda import _product
+    from helpers import product
 
-    cfg, env, net, agent = _product("simple_spread", 4, ["--use_recurrent_policy", "true"])
+    cfg, env, net, agent = product("simple_spread", 4, ["--use_recurrent_policy", "true"])
     pol = net.module.models["policy"]
     p = _oracle_params(pol)
     g = torch.Generator().manual_seed(3)
@@ -54,48 +53,6 @@ def test_recurrent_act_matches_oracle(cuda):
         a2, lp2, h2 = nets.policy_act(p, cfg, obs, None, h, masks, deterministic=det, exp_noise=noise)
         _compare_act(a1.cpu().numpy(), lp1.cpu().numpy(), a2.numpy(), lp2.numpy(), rows)
         np.testing.assert_allclose(h1.cpu().numpy(), h2.numpy(), rtol=0, atol=2e-6)
-
-
-def check_recurrent_trace(tag, env_id):
-    """Drive rollout -> returns -> update by hand for every recorded iteration and compare each stage with the
-    unmodified reference's trace."""
-    from openrl_b200.utils.logger import Logger
-    from test_rollout_cuda import _product
-
-    d = np.load(os.path.join(GOLDEN, f"trace_{tag}.npz"), allow_pickle=True)
-    iters, N = int(d["meta/iters"]), int(d["meta/env_num"])
-    cfg, env, net, agent = _product(env_id, N, str(d["meta/flags"]).split(), golden=d)
-    agent.train(total_time_steps=0, logger=Logger(quiet=True))   # builds trainer / buffer / driver, resets the envs
-    drv = agent.driver
-    b = drv.buffer.data
-    assert b.rnn_states.shape == d["it0/rnn_states"].shape
-    for it in range(iters):
-        tag_i = f"it{it}"
-        drv.episode = it
-        drv.actor_rollout()
-        assert np.array_equal(b.actions.cpu().numpy(), d[f"{tag_i}/actions"]), tag_i
-        np.testing.assert_allclose(b.action_log_probs.cpu().numpy(), d[f"{tag_i}/action_log_probs"], rtol=0, atol=2e-5)
-        np.testing.assert_allclose(b.rnn_states.cpu().numpy(), d[f"{tag_i}/rnn_states"], rtol=0, atol=2e-5)
-        assert np.array_equal(b.masks.cpu().numpy(), d[f"{tag_i}/masks"])
-        np.testing.assert_allclose(b.policy_obs.cpu().numpy(), d[f"{tag_i}/policy_obs"], rtol=0, atol=2e-6)
-        np.testing.assert_allclose(b.rewards.cpu().numpy(), d[f"{tag_i}/rewards"], rtol=1e-6, atol=1e-5)
-        drv.compute_returns()
-        np.testing.assert_allclose(b.rnn_states_critic.cpu().numpy(), d[f"{tag_i}/rnn_states_critic"], rtol=0, atol=2e-5)
-        np.testing.assert_allclose(b.value_preds.cpu().numpy()[:-1], d[f"{tag_i}/value_preds"][:-1], rtol=0, atol=2e-5)
-        np.testing.assert_allclose(b.returns.cpu().numpy()[:-1], d[f"{tag_i}/returns"][:-1], rtol=1e-4, atol=2e-4)
-        info = drv.trainer.train(b)
-        want = d[f"{tag_i}/updates"].mean(axis=0)
-        for col, name in enumerate(KEYS):
-            np.testing.assert_allclose(info[name], want[col], rtol=2e-4, atol=1e-5, err_msg=f"{tag_i} {name}")
-        for mk in ("policy", "critic"):
-            for k, v in net.module.models[mk].state_dict().items():
-                gk = f"{tag_i}/params/{mk}.{k}"
-                if gk in d and "value_normalizer" not in k:
-                    np.testing.assert_allclose(v.cpu().numpy(), d[gk], rtol=2e-3, atol=2e-5, err_msg=gk)
-        vn = net.module.models["critic"].value_normalizer
-        if vn is not None:
-            np.testing.assert_allclose(vn.state.cpu().numpy(), d[f"{tag_i}/vn_after_update"], rtol=1e-5, atol=1e-7)
-        b.after_update()
 
 
 def test_recurrent_mappo_matches_reference_trace(cuda):
@@ -180,10 +137,10 @@ def test_recurrent_sharded_buckets_sum_to_global_bucket(cuda):
 
     from openrl_b200 import lib
     from openrl_b200.utils.logger import Logger
-    from test_rollout_cuda import _product
+    from helpers import product
 
     d = np.load(os.path.join(GOLDEN, "trace_mpe_gru.npz"), allow_pickle=True)
-    cfg, env, net, agent = _product("simple_spread", int(d["meta/env_num"]), str(d["meta/flags"]).split(), golden=d)
+    cfg, env, net, agent = product("simple_spread", int(d["meta/env_num"]), str(d["meta/flags"]).split(), golden=d)
     agent.train(total_time_steps=0, logger=Logger(quiet=True))
     drv = agent.driver
     drv.actor_rollout()

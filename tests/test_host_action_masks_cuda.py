@@ -14,8 +14,8 @@ import pytest
 
 from conftest import GOLDEN
 from masked_oracle import MaskedTargetVec
-from test_rnn_host_cuda import KEYS, _agent
-from test_rnn_scale_cuda import no_tf32  # noqa: F401  (pytest fixture)
+from helpers import KEYS, make_agent
+from scale_harness import no_tf32  # noqa: F401  (pytest fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -62,7 +62,7 @@ def test_host_masks_reproduce_reference_trace(cuda, tag):
     iters, N = int(d["meta/iters"]), int(d["meta/env_num"])
     flags = str(d["meta/flags"]).split() + ["--parity_mode", "true", "--log_interval", "1"]
     env = _host(N)
-    cfg, net, agent = _agent(env, flags, golden=d)
+    cfg, net, agent = make_agent(env, flags, golden=d)
     drv = agent.driver
     b = drv.buffer.data
     assert not b.action_masks_trivial      # the reset infos carried masks
@@ -108,7 +108,7 @@ def test_host_masks_at_scale_no_illegal_action_and_loops_agree(cuda, recurrent):
     for grouped in (False, True):
         env = _host(N)
         assert env.supports_groups
-        cfg, net, agent = _agent(env, flags + ["--host_env_groups", "true" if grouped else "false"], like=init)
+        cfg, net, agent = make_agent(env, flags + ["--host_env_groups", "true" if grouped else "false"], like=init)
         if init is None:
             init = {mk: {k: v.clone() for k, v in net.module.models[mk].state_dict().items()} for mk in ("policy", "critic")}
         drv, b = agent.driver, agent.driver.buffer.data
@@ -144,7 +144,7 @@ def test_slots_without_masks_keep_their_content(cuda):
     flags = ["--seed", "1", "--episode_length", str(T), "--ppo_epoch", "1", "--log_interval", "1"]
     for grouped in ("false", "true"):
         env = _host(N, report)
-        cfg, net, agent = _agent(env, flags + ["--host_env_groups", grouped])
+        cfg, net, agent = make_agent(env, flags + ["--host_env_groups", grouped])
         drv, b = agent.driver, agent.driver.buffer.data
         prev = b.action_masks.cpu().numpy().copy()
         for it in range(2):
@@ -196,7 +196,7 @@ def test_single_legal_action_and_all_masked_rows(cuda, recurrent):
     if recurrent:
         flags += ["--use_recurrent_policy", "true", "--data_chunk_length", "4"]
     env = _host(N, cls=_OneLegal)
-    cfg, net, agent = _agent(env, flags)
+    cfg, net, agent = make_agent(env, flags)
     drv, b = agent.driver, agent.driver.buffer.data
     drv.actor_rollout()
     acts, obs = b.actions.cpu().numpy()[..., 0], b.policy_obs.cpu().numpy()
@@ -213,7 +213,7 @@ def test_single_legal_action_and_all_masked_rows(cuda, recurrent):
         none = True
 
     env = _host(N, cls=_NoneLegal)
-    cfg, net, agent = _agent(env, flags)
+    cfg, net, agent = make_agent(env, flags)
     drv, b = agent.driver, agent.driver.buffer.data
     drv.actor_rollout()
     assert not b.action_masks_trivial and (b.action_masks.cpu().numpy() == 0).all()
@@ -236,7 +236,7 @@ def test_recurrent_agent_act_applies_masks(cuda):
     N = 32
     flags = ["--seed", "2", "--episode_length", "8", "--use_recurrent_policy", "true", "--data_chunk_length", "4"]
     env = _host(N)
-    cfg, net, agent = _agent(env, flags)
+    cfg, net, agent = make_agent(env, flags)
     rng = np.random.default_rng(0)
     obs = rng.standard_normal((N, 1, 5)).astype(np.float32)
     m = (rng.random((N, 5)) < 0.5).astype(np.int8)
@@ -316,13 +316,13 @@ def test_multi_agent_masked_gru_update_matches_float64(cuda, no_tf32):
     import rnn_ref64_masked
     from oracle import nets
     from openrl_b200.envs.vec_env import HostVecEnv
-    from test_rnn_scale_cuda import _c3_buf, _compare, _drive
+    from scale_harness import c3_buf, drive, rnn_compare
 
     N, A, T, L = 64, 3, 16, 4
     host = _MaskedMultiAgent(N)
     flags = ["--seed", "6", "--use_recurrent_policy", "true", "--episode_length", str(T), "--data_chunk_length", str(L),
              "--ppo_epoch", "1", "--num_mini_batch", "1", "--use_valuenorm", "true", "--host_env_groups", "false"]
-    cfg, net, agent = _agent(HostVecEnv(host), flags)
+    cfg, net, agent = make_agent(HostVecEnv(host), flags)
     drv, tr, b = agent.driver, agent.driver.trainer, agent.driver.buffer.data
     drv.actor_rollout()
     drv.compute_returns()
@@ -355,16 +355,16 @@ def test_multi_agent_masked_gru_update_matches_float64(cuda, no_tf32):
     tr.sync_lrs()
     a = tr._rnn_args(b, ids, b.gae_stats[5:8])
     assert a.action_masks == b.action_masks.data_ptr()
-    grads, la, after = _drive(a, tr.rnn_grads, tr.loss_acc, live)
+    grads, la, after = drive(a, tr.rnn_grads, tr.loss_acc, live)
     tr.tape = None
     np_, nc = int(pol.flat_params.numel()), int(cri.flat_params.numel())
     k = dict(grad_pol=grads[0, :np_], grad_cri=grads[1, :nc], losses=la, steps=[int(x) for x in m.adam_steps], **after)
     rcfg = types.SimpleNamespace(**vars(cfg), vn_beta=vn.beta)
     dims = (tr.d, tr.n, tr.dc)
-    buf = _c3_buf(b)
+    buf = c3_buf(b)
     r64, r32 = (rnn_ref64_masked.update(rcfg, buf, state, ids, L, dims, b.action_masks, dtype=dt)
                 for dt in (torch.float64, torch.float32))
-    _compare("masked-A3-L4-768chunks-3072rows", dims, k, r64, r32, check_vn=True)
+    rnn_compare("masked-A3-L4-768chunks-3072rows", dims, k, r64, r32, check_vn=True)
     # the masks matter: without them the float64 policy gradient is another one
     plain = rnn_ref64.update(rcfg, buf, state, ids, L, dims, joint=False, dtype=torch.float64)
     assert float((plain["grad_pol"] - r64["grad_pol"]).norm()) > 1e-3 * float(r64["grad_pol"].norm())

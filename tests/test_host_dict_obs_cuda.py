@@ -11,8 +11,8 @@ import types
 import numpy as np
 import pytest
 
-from test_rnn_host_cuda import KEYS, _agent
-from test_rnn_scale_cuda import no_tf32  # noqa: F401  (pytest fixture)
+from helpers import KEYS, make_agent
+from scale_harness import no_tf32  # noqa: F401  (pytest fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -91,7 +91,7 @@ def test_dict_obs_host_env_reproduces_reference_trace(cuda, tag):
     flags = str(d["meta/flags"]).split() + ["--parity_mode", "true", "--log_interval", "1"]
     env = _make(N)
     assert env.dict_obs and (env.obs_dim, env.critic_obs_dim) == (3, 7)
-    cfg, net, agent = _agent(env, flags, golden=d)
+    cfg, net, agent = make_agent(env, flags, golden=d)
     drv, tr = agent.driver, agent.driver.trainer
     b = drv.buffer.data
     assert b.critic_obs is not b.policy_obs and b.critic_obs.shape[-1] == 7
@@ -144,7 +144,7 @@ def test_dict_obs_loops_agree_and_critic_rows_are_the_envs(cuda, recurrent):
         host = _DictHost(N, A)
         env = HostVecEnv(host)
         assert env.supports_groups
-        cfg, net, agent = _agent(env, flags + ["--host_env_groups", "true" if grouped else "false"], like=init)
+        cfg, net, agent = make_agent(env, flags + ["--host_env_groups", "true" if grouped else "false"], like=init)
         if init is None:
             init = {mk: {k: v.clone() for k, v in net.module.models[mk].state_dict().items()} for mk in ("policy", "critic")}
         drv, b = agent.driver, agent.driver.buffer.data
@@ -190,7 +190,7 @@ def test_wide_critic_feed_forward_update_matches_float64(cuda):
     flags = ["--seed", "5", "--episode_length", str(T), "--ppo_epoch", "1", "--num_mini_batch", "1",
              "--use_valuenorm", "false", "--host_env_groups", "false"]
     host = _DictHost(N, A, masks=False)
-    cfg, net, agent = _agent(HostVecEnv(host), flags)
+    cfg, net, agent = make_agent(HostVecEnv(host), flags)
     drv, tr, b = agent.driver, agent.driver.trainer, agent.driver.buffer.data
     assert (tr.d, tr.dc) == (6, 40) and not tr.use_tensor_cores
     drv.actor_rollout()
@@ -237,12 +237,12 @@ def test_wide_critic_gru_update_matches_float64(cuda, no_tf32):
 
     import rnn_ref64
     from openrl_b200.envs.vec_env import HostVecEnv
-    from test_rnn_scale_cuda import _c3_buf, _compare, _drive
+    from scale_harness import c3_buf, drive, rnn_compare
 
     N, A, T, L = 64, 3, 16, 4
     flags = ["--seed", "6", "--use_recurrent_policy", "true", "--episode_length", str(T), "--data_chunk_length", str(L),
              "--ppo_epoch", "1", "--num_mini_batch", "1", "--use_valuenorm", "true", "--host_env_groups", "false"]
-    cfg, net, agent = _agent(HostVecEnv(_DictHost(N, A, masks=False)), flags)
+    cfg, net, agent = make_agent(HostVecEnv(_DictHost(N, A, masks=False)), flags)
     drv, tr, b = agent.driver, agent.driver.trainer, agent.driver.buffer.data
     assert (tr.d, tr.n, tr.dc) == (6, 5, 40)
     drv.actor_rollout()
@@ -263,15 +263,15 @@ def test_wide_critic_gru_update_matches_float64(cuda, no_tf32):
     tr.sync_lrs()
     a = tr._rnn_args(b, ids, b.gae_stats[5:8])
     assert (a.critic_obs, a.critic_obs_dim) == (b.critic_obs.data_ptr(), 40)
-    grads, la, after = _drive(a, tr.rnn_grads, tr.loss_acc, live)
+    grads, la, after = drive(a, tr.rnn_grads, tr.loss_acc, live)
     tr.tape = None
     np_, nc = int(pol.flat_params.numel()), int(cri.flat_params.numel())
     k = dict(grad_pol=grads[0, :np_], grad_cri=grads[1, :nc], losses=la, steps=[int(x) for x in m.adam_steps], **after)
     rcfg = types.SimpleNamespace(**vars(cfg), vn_beta=vn.beta)
     dims = (tr.d, tr.n, tr.dc)
-    buf = _c3_buf(b)
+    buf = c3_buf(b)
     r64, r32 = (rnn_ref64.update(rcfg, buf, state, ids, L, dims, joint=False, dtype=dt) for dt in (torch.float64, torch.float32))
-    _compare("dict-obs-d6-dc40-A3-L4-768chunks-3072rows", dims, k, r64, r32, check_vn=True)
+    rnn_compare("dict-obs-d6-dc40-A3-L4-768chunks-3072rows", dims, k, r64, r32, check_vn=True)
 
 
 def _staged_block(rng, B, d, dc, n, with_critic, with_masks, n_agents):

@@ -8,7 +8,7 @@ second call on.  CPU: the staged step of the whole range goes through `env.step`
 import numpy as np
 import pytest
 
-from test_host_sync_env import CountEnv
+from helpers import CountEnv
 
 
 def _train_twice(recurrent, grouped, T, N):

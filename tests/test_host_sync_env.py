@@ -4,30 +4,8 @@ checks: tests/test_env/test_sync_env.py)."""
 import numpy as np
 import pytest
 
-from openrl_b200 import spaces
+from helpers import CountEnv
 from openrl_b200.envs.vec_env.host_sync import SyncHostVecEnv
-
-
-class CountEnv:
-    """5-tuple API, episode ends after `horizon` steps; obs = [t, id]."""
-
-    def __init__(self, ident, horizon=3):
-        self.observation_space = spaces.Box(-np.inf, np.inf, (2,), np.float32)
-        self.action_space = spaces.Discrete(3)
-        self.ident, self.horizon, self.t, self.seed_seen, self.tag = ident, horizon, 0, None, "x"
-        self.actions = []
-
-    def reset(self, seed=None, options=None):
-        self.t = 0
-        if seed is not None:
-            self.seed_seen = seed
-        return np.array([0, self.ident], np.float32), {"reset": True}
-
-    def step(self, a):
-        assert isinstance(a, (int, np.integer)) or np.asarray(a).shape == ()
-        self.actions.append(int(a))
-        self.t += 1
-        return np.array([self.t, self.ident], np.float32), float(a), self.t >= self.horizon, False, {"t": self.t}
 
 
 def test_sync_host_vec_env_matches_reference_semantics():

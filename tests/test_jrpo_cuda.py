@@ -17,20 +17,19 @@ pytestmark = pytest.mark.gpu
 
 @pytest.mark.parametrize("tag", ["mpe_jrpo", "mpe_jrpo_mb"])
 def test_jrpo_matches_reference_trace(cuda, tag):
-    from test_gru_cuda import check_recurrent_trace
+    from helpers import check_recurrent_trace
 
     check_recurrent_trace(tag, "simple_spread")
 
 
-def test_jrpo_single_agent_reproduces_cartpole_gru_trace(cuda, tmp_path, monkeypatch):
-    import test_gru_cuda
+def test_jrpo_single_agent_reproduces_cartpole_gru_trace(cuda, tmp_path):
+    from helpers import check_recurrent_trace
 
     with np.load(os.path.join(GOLDEN, "trace_cartpole_gru.npz"), allow_pickle=True) as d:
         rec = {k: d[k] for k in d.files}
     rec["meta/flags"] = np.array(str(rec["meta/flags"]) + " --use_joint_action_loss true")
     np.savez(tmp_path / "trace_cartpole_gru.npz", **rec)
-    monkeypatch.setattr(test_gru_cuda, "GOLDEN", str(tmp_path))
-    test_gru_cuda.check_recurrent_trace("cartpole_gru", "CartPole-v1")
+    check_recurrent_trace("cartpole_gru", "CartPole-v1", golden_dir=str(tmp_path))
 
 
 def _mpe_jrpo_cfg(extra=()):
@@ -97,10 +96,10 @@ def test_jrpo_sharded_buckets_sum_to_global_bucket(cuda):
 
     from openrl_b200 import lib
     from openrl_b200.utils.logger import Logger
-    from test_rollout_cuda import _product
+    from helpers import product
 
     d = np.load(os.path.join(GOLDEN, "trace_mpe_jrpo.npz"), allow_pickle=True)
-    cfg, env, net, agent = _product("simple_spread", int(d["meta/env_num"]), str(d["meta/flags"]).split(), golden=d)
+    cfg, env, net, agent = product("simple_spread", int(d["meta/env_num"]), str(d["meta/flags"]).split(), golden=d)
     agent.train(total_time_steps=0, logger=Logger(quiet=True))
     drv = agent.driver
     drv.actor_rollout()
@@ -135,7 +134,7 @@ def test_jrpo_limits_are_loud(cuda):
     from openrl_b200.modules.common import PPONet
     from openrl_b200.runners.common import PPOAgent
     from openrl_b200.utils.logger import Logger
-    from test_rollout_cuda import _product
+    from helpers import product
 
     for flags in (["--use_joint_action_loss", "true"],
                   ["--use_joint_action_loss", "true", "--use_naive_recurrent_policy", "true", "--episode_length", "25"]):
@@ -145,7 +144,7 @@ def test_jrpo_limits_are_loud(cuda):
         with pytest.raises(NotImplementedError, match="use_joint_action_loss"):
             agent.train(total_time_steps=25 * 2 * 2)
     # the kernel entry point refuses the flag with a number of agents it was not built for
-    cfg, env, net, agent = _product("CartPole-v1", 4, ["--use_recurrent_policy", "true", "--episode_length", "8"])
+    cfg, env, net, agent = product("CartPole-v1", 4, ["--use_recurrent_policy", "true", "--episode_length", "8"])
     agent.train(total_time_steps=0, logger=Logger(quiet=True))
     drv = agent.driver
     drv.actor_rollout()

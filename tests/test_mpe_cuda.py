@@ -37,11 +37,11 @@ def test_simple_spread_env_matches_oracle(cuda):
 
 def test_mpe_mappo_train_matches_reference_trace(cuda):
     from openrl_b200.utils.logger import Logger
-    from test_rollout_cuda import _product
+    from helpers import product
 
     d = np.load(os.path.join(GOLDEN, "trace_mpe_mlp.npz"), allow_pickle=True)
     iters, N = int(d["meta/iters"]), int(d["meta/env_num"])
-    cfg, env, net, agent = _product("simple_spread", N, str(d["meta/flags"]).split(), golden=d)
+    cfg, env, net, agent = product("simple_spread", N, str(d["meta/flags"]).split(), golden=d)
     logger = Logger(quiet=True)
     agent.train(total_time_steps=cfg.episode_length * N * iters, logger=logger)
     train_logs = [h[1] for h in logger.history if "value_loss" in h[1]]

@@ -8,22 +8,8 @@ import pytest
 import torch
 
 from conftest import GOLDEN
+from helpers import trace_threads  # noqa: F401  (autouse fixture)
 from oracle import loop
-
-# The reference traces were recorded on an 8-core host with torch's default of 8 intra-op threads, and the oracle
-# reproduces them bit for bit only under comparable threading: with 1 thread the QR of the orthogonal init differs
-# (init parameters off by up to ~2e-7); on a 16-core host running 16 threads the first update's CPU reductions differ
-# in their last bits, which moves a continuous action of iteration 1 by one ulp.  Running the oracle with the
-# recording count makes these bit-exact checks independent of the host.
-TRACE_THREADS = 8
-
-
-@pytest.fixture(autouse=True)
-def _trace_threads():
-    before = torch.get_num_threads()
-    torch.set_num_threads(TRACE_THREADS)
-    yield
-    torch.set_num_threads(before)
 
 
 def _params(tr):

@@ -19,11 +19,11 @@ def test_reduce_peer_pushes_the_sums_of_reduce_into_every_ranks_slot(cuda, rank,
     import torch
 
     from openrl_b200 import lib
-    from test_ppo_update_cuda import _load_buffer, _setup
+    from helpers import load_buffer, ppo_update_setup
 
     d = np.load(os.path.join(GOLDEN, "trace_cartpole.npz"), allow_pickle=True)
-    cfg, net, trainer, buf = _setup(d)
-    _load_buffer(buf, d, 0)
+    cfg, net, trainer, buf = ppo_update_setup(d)
+    load_buffer(buf, d, 0)
     L, s = lib.load(), lib.current_stream()
     stride, G, W = trainer.stride, trainer.grid_per_net, 2
     gen = torch.Generator(device="cuda").manual_seed(3)

@@ -4,27 +4,9 @@ CUDA update vs the torch-CPU oracle on the same synthetic minibatch with NON-tri
 import numpy as np
 import pytest
 
-pytestmark = pytest.mark.gpu
+from scale_harness import CASES
 
-CASES = [
-    [],
-    ["--use_huber_loss", "false"],
-    ["--use_clipped_value_loss", "false"],
-    ["--use_valuenorm", "false"],
-    ["--use_value_active_masks", "false", "--use_policy_active_masks", "false"],
-    ["--use_adv_normalize", "true"],
-    ["--use_max_grad_norm", "false"],
-    ["--weight_decay", "0.01", "--lr", "1e-3", "--critic_lr", "2e-3"],
-    ["--activation_id", "0"],
-    ["--activation_id", "2"],
-    ["--activation_id", "3"],
-    ["--clip_param", "0.05", "--entropy_coef", "0.05", "--value_loss_coef", "1.0", "--huber_delta", "0.5"],
-    ["--max_grad_norm", "0.5"],
-    ["--use_proper_time_limits", "true"],
-    ["--use_gae", "false"],
-    ["--dual_clip_ppo", "true", "--dual_clip_coeff", "1.05"],
-    ["A2C"],
-]
+pytestmark = pytest.mark.gpu
 
 
 def _build(flags, env_id="GridWorldEnv", N=24, T=20, seed=3):

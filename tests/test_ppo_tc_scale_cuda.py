@@ -20,15 +20,14 @@ compared in units of lr: an element whose float64 gradient is outside the bar's 
 it may move by up to one Adam step, and such elements must be few.  Adam moments are bounded through the same gradient
 bar; the ValueNorm state and the ratio mean use the self-calibrated bar of tests/test_rnn_scale_cuda.py."""
 import types
-from unittest import mock
 
 import pytest
 import torch
 
 import ffma_ref64
+import scale_harness as h
 import tc_ref64 as ref
-import test_ppo_ffma_scale_cuda as fscale
-from test_rnn_scale_cuda import Checker, _mb_stats, _rel, no_tf32  # noqa: F401  (no_tf32: pytest fixture)
+from scale_harness import BASE, PPO_FLOOR, Checker, no_tf32  # noqa: F401  (no_tf32: pytest fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -50,11 +49,6 @@ def _needs_cuda(cuda):
     pass
 
 
-def _lib():
-    from openrl_b200 import lib
-    return lib, lib.load()
-
-
 def _sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
@@ -68,8 +62,8 @@ class TauChecker:
     def __call__(self, what, got, r64, scale, r32=None):
         err = float((got.double() - r64.double()).norm())
         es = err / float(scale) if float(scale) > 0 else (0.0 if err == 0 else float("inf"))
-        rk = _rel(got, r64)
-        r32s = f"fp32 {_rel(r32, r64):9.2e}" if r32 is not None else " " * 14
+        rk = h.rel(got, r64)
+        r32s = f"fp32 {h.rel(r32, r64):9.2e}" if r32 is not None else " " * 14
         if es > self.worst[0]:
             self.worst = (es, what)
         print(f"  {self.case:44s} {what:42s} rel kernel {rk:9.2e} {r32s}  err/S {es:9.2e}  bar {TAU:.1e}")
@@ -88,7 +82,7 @@ def _clip(r64, j, cfg):
 
 def compare(case, dims, k, r64, r32, state, cfg, check_vn=True):
     """Every quantity of one update: gradients and loss sums against TAU x S, train_info, Adam state, ValueNorm."""
-    chk, calib = TauChecker(case), Checker(case, floor=fscale.FLOOR)
+    chk, calib = TauChecker(case), Checker(case, PPO_FLOOR)
     s_tot = {}
     for net in ("pol", "cri"):
         tot = 0.0
@@ -138,22 +132,18 @@ def compare(case, dims, k, r64, r32, state, cfg, check_vn=True):
     return chk.worst[0]
 
 
-def _loss_sums(folded, stride):
-    return fscale._loss_sums(folded, stride)
-
-
 # ---------------------------------------------------------------- the real C2 buffer ----------------------------------
 
 @pytest.fixture(scope="module")
 def c2():
     """The bench's C2 agent (CartPole-v1, 4096 device envs), one rollout and its returns."""
     from openrl_b200.envs.common import make
-    from test_rnn_host_cuda import _agent
+    from helpers import make_agent
 
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     torch.manual_seed(0)
-    cfg, net, agent = _agent(make("CartPole-v1", env_num=4096), C2_FLAGS)
+    cfg, net, agent = make_agent(make("CartPole-v1", env_num=4096), C2_FLAGS)
     drv = agent.driver
     drv.actor_rollout()
     drv.compute_returns()
@@ -189,33 +179,33 @@ def _refs(c, state, rows_idx):
 def test_c2_four_epochs_contiguous(c2, no_tf32):
     """C2's four updates (4 epochs over the whole buffer, indices == NULL: TMA staging, the GAE moments as minibatch
     moments), each teacher-forced from the device's own state before it.  Epoch 1 has every ratio at 1."""
-    snap = fscale._snapshot(c2)
+    snap = h.snapshot(c2)
     rows = torch.arange(c2.rows, device="cuda")
     try:
         for epoch in range(4):
-            state = fscale._state(c2)
-            k = fscale._kernel_update(c2, None, c2.b.gae_stats[5:8], c2.rows)
+            state = h.state(c2)
+            k = h.kernel_update(c2, None, c2.b.gae_stats[5:8], c2.rows)
             r64, r32 = _refs(c2, state, rows)
             compare(f"c2-epoch{epoch + 1}-contiguous-{c2.rows}rows", (4, 2, 4), k, r64, r32, state, c2.cfg)
             spread = float(r64["ratio_spread"])
             assert (spread > 1e-4) if epoch else (spread < 1e-4), spread
     finally:
-        fscale._restore(c2, snap)
+        h.restore(c2, snap)
 
 
 def test_c2_shuffled_quarter(c2, no_tf32):
     """num_mini_batch 4 on the same buffer: a shuffled quarter (gather staging, two tiles ahead), orl_minibatch_stats."""
-    snap = fscale._snapshot(c2)
+    snap = h.snapshot(c2)
     g = torch.Generator(device="cuda").manual_seed(4)
     idx = torch.randperm(c2.rows, device="cuda", generator=g)[:c2.rows // 4].contiguous()
     assert idx.numel() // T_M // c2.tr.grid_per_net >= 7
     try:
-        state = fscale._state(c2)
-        k = fscale._kernel_update(c2, idx, _mb_stats(idx, c2.b.returns, c2.b.active_masks), idx.numel())
+        state = h.state(c2)
+        k = h.kernel_update(c2, idx, h.mb_stats(idx, c2.b.returns, c2.b.active_masks), idx.numel())
         r64, r32 = _refs(c2, state, idx)
         compare(f"c2-mb4-shuffled-{idx.numel()}rows", (4, 2, 4), k, r64, r32, state, c2.cfg)
     finally:
-        fscale._restore(c2, snap)
+        h.restore(c2, snap)
 
 
 # ---------------------------------------------------------------- deliberate mistakes ---------------------------------
@@ -236,13 +226,13 @@ def test_c2_mutants_are_detected(c2, no_tf32, mutant):
     what, block = ref.TC_MUTANTS[mutant]
     rows_n = c2.rows - 127 if mutant == "partial-tail-counted" else c2.rows
     rows = torch.arange(rows_n, device="cuda")
-    snap = fscale._snapshot(c2)
+    snap = h.snapshot(c2)
     try:
-        state = fscale._state(c2)
-        stats = c2.b.gae_stats[5:8] if rows_n == c2.rows else _mb_stats(rows, c2.b.returns, c2.b.active_masks)
-        k = fscale._kernel_update(c2, None, stats, rows_n)
+        state = h.state(c2)
+        stats = c2.b.gae_stats[5:8] if rows_n == c2.rows else h.mb_stats(rows, c2.b.returns, c2.b.active_masks)
+        k = h.kernel_update(c2, None, stats, rows_n)
     finally:
-        fscale._restore(c2, snap)
+        h.restore(c2, snap)
     G, tiles = c2.tr.grid_per_net, -(-rows_n // T_M)
     mine = _cta_tiles(tiles, G)
     kw = {}
@@ -268,12 +258,9 @@ def test_c2_mutants_are_detected(c2, no_tf32, mutant):
 
 # ---------------------------------------------------------------- synthetic buffers -----------------------------------
 
-BASE = fscale.BASE
-
-
 def _launch(cfg, dims, buf, state, batch_rows, idx, row_begin, total, gae_stats, mb_stats, G=None):
     """OrlPpoArgs built by hand with ORL_PPO_TENSORCORE: fwdbwd, reduce, apply; what the comparison reads back."""
-    lib, L = _lib()
+    lb, L = h.lib()
     d, n, dc = dims
     G = G or _sms()
     stride, gstride = L.orl_ppo_stride(d, dc, n), L.orl_ppo_grads_stride(d, dc, n)
@@ -284,51 +271,24 @@ def _launch(cfg, dims, buf, state, batch_rows, idx, row_begin, total, gae_stats,
     steps = torch.tensor(state["steps"], dtype=torch.int32, device="cuda")
     lrs = torch.tensor([cfg.lr, cfg.critic_lr], dtype=torch.float32, device="cuda")
     train_info = torch.zeros(6, device="cuda")
-    a = lib.OrlPpoArgs()
-    a.obs_dim, a.critic_obs_dim, a.n_actions, a.activation_id = d, dc, n, cfg.activation_id
-    a.flags, a.grid_per_net, a.head_kind = fscale._flags(cfg) | lib.PPO_TENSORCORE, G, lib.HEAD_CATEGORICAL
-    a.batch_rows, a.row_begin, a.total_rows = batch_rows, row_begin, total
-    a.indices = None if idx is None else lib.ptr(idx)
-    for k, key in (("policy_obs", "policy_obs"), ("critic_obs", "critic_obs"), ("actions", "actions"),
-                   ("old_log_probs", "action_log_probs"), ("advantages", "advantages"), ("value_preds", "value_preds"),
-                   ("returns", "returns"), ("active_masks", "active_masks")):
-        setattr(a, k, lib.ptr(buf[key]))
-    a.action_masks = lib.ptr(buf["action_masks"]) if "action_masks" in buf else None
-    a.gae_stats, a.mb_stats, a.vn_state = lib.ptr(gae_stats), lib.ptr(mb_stats), lib.ptr(dev["vn"])
-    a.policy_params, a.critic_params = lib.ptr(dev["pol"]), lib.ptr(dev["cri"])
-    a.policy_adam_m, a.policy_adam_v = lib.ptr(dev["pol_m"]), lib.ptr(dev["pol_v"])
-    a.critic_adam_m, a.critic_adam_v = lib.ptr(dev["cri_m"]), lib.ptr(dev["cri_v"])
-    a.adam_steps, a.lrs, a.train_info = lib.ptr(steps), lib.ptr(lrs), lib.ptr(train_info)
-    a.clip_param, a.entropy_coef, a.value_loss_coef = cfg.clip_param, cfg.entropy_coef, cfg.value_loss_coef
-    a.huber_delta, a.max_grad_norm, a.dual_clip_coeff = cfg.huber_delta, cfg.max_grad_norm, cfg.dual_clip_coeff
-    a.adam_beta1, a.adam_beta2, a.adam_eps, a.weight_decay = 0.9, 0.999, cfg.opti_eps, cfg.weight_decay
-    a.vn_beta, a.norm_rows = cfg.vn_beta, 0
-    a.partials, a.folded, a.grads = lib.ptr(partials), lib.ptr(folded), lib.ptr(grads)
-    s = lib.current_stream()
-    lib.check(L.orl_ppo_fwdbwd(a, s), "orl_ppo_fwdbwd")
-    lib.check(L.orl_ppo_reduce(a, s), "orl_ppo_reduce")
-    lib.check(L.orl_ppo_apply(a, s), "orl_ppo_apply")
+    a = h.ppo_args(cfg, dims, lb.HEAD_CATEGORICAL, h.ppo_flags(cfg) | lb.PPO_TENSORCORE, G, buf, batch_rows, total, idx, row_begin,
+                   (gae_stats, mb_stats), dev, steps, lrs, train_info, partials, folded, grads)
+    s = lb.current_stream()
+    lb.check(L.orl_ppo_fwdbwd(a, s), "orl_ppo_fwdbwd")
+    lb.check(L.orl_ppo_reduce(a, s), "orl_ppo_reduce")
+    lb.check(L.orl_ppo_apply(a, s), "orl_ppo_apply")
     torch.cuda.synchronize()
-    return dict(grad_pol=grads[0, :dev["pol"].numel()], grad_cri=grads[1, :dev["cri"].numel()], losses=_loss_sums(folded, stride),
+    return dict(grad_pol=grads[0, :dev["pol"].numel()], grad_cri=grads[1, :dev["cri"].numel()], losses=h.loss_sums(folded, stride),
                 folded_losses=folded[:, stride - 8:].clone(), info=train_info, steps=[int(x) for x in steps], **dev)
 
 
 def _setup(cfg, dims, batch_rows, contiguous_from=None, total=None, seed=0, net_edit=None):
-    """A synthetic buffer (tests/test_ppo_ffma_scale_cuda.py `_synthetic`, Categorical head with action masks and active
-    masks with zeros) and the minibatch: a shuffled index list, or a contiguous range from `contiguous_from`.
-    net_edit(state) edits the random nets before the buffer's log-probs and values are drawn from them."""
+    """A synthetic buffer (scale_harness.ppo_synthetic, Categorical head with action masks and active masks with zeros)
+    and the minibatch: a shuffled index list, or a contiguous range from `contiguous_from`.
+    net_edit(head, flat) edits the random nets before the buffer's log-probs and values are drawn from them."""
     total = total or batch_rows + 301
-    g = torch.Generator(device="cuda").manual_seed(seed + 1)
-    if contiguous_from is None:
-        idx = torch.randperm(total, device="cuda", generator=g)[:batch_rows].contiguous()
-        rows_idx = idx
-    else:
-        idx = None
-        rows_idx = torch.arange(contiguous_from, contiguous_from + batch_rows, device="cuda")
-    real = fscale._random_net
-    edit = (lambda *a: net_edit(a[3], real(*a))) if net_edit else real
-    with mock.patch.object(fscale, "_random_net", edit):
-        buf, state = fscale._synthetic(cfg, dims, "categorical", total, rows_idx, seed)
+    idx, rows_idx = h.minibatch(total, batch_rows, contiguous_from, seed)
+    buf, state = h.ppo_synthetic(cfg, dims, "categorical", total, rows_idx, seed, net_edit)
     return buf, state, idx, rows_idx, total
 
 
@@ -337,8 +297,8 @@ def _run(case, cfg, dims, batch_rows, contiguous_from=None, total=None, seed=0, 
     if buf_edit:
         buf_edit(buf, rows_idx)
     G = _sms()
-    k = _launch(cfg, dims, buf, state, batch_rows, idx, contiguous_from or 0, total, fscale._gae_stats(buf),
-                _mb_stats(rows_idx.contiguous(), buf["returns"], buf["active_masks"]))
+    k = _launch(cfg, dims, buf, state, batch_rows, idx, contiguous_from or 0, total, h.gae_stats(buf),
+                h.mb_stats(rows_idx.contiguous(), buf["returns"], buf["active_masks"]))
     r64 = ref.update(cfg, buf, state, rows_idx, dims, vn_beta=cfg.vn_beta)
     r32 = ffma_ref64.update(cfg, buf, state, rows_idx, dims, "categorical", torch.float32, vn_beta=cfg.vn_beta)
     tiles = -(-batch_rows // T_M)
@@ -366,7 +326,7 @@ SYN_CASES = [(f"{name}-{rk}rows", dims, act, rk) for name, dims, act, rks in SYN
 @pytest.mark.parametrize("case,dims,act,rows_kind", SYN_CASES, ids=[c[0] for c in SYN_CASES])
 def test_update_synthetic_edges(no_tf32, case, dims, act, rows_kind):
     """Shuffled minibatches (an index list into a larger buffer: gather staging) at every template and row-count edge."""
-    cfg = types.SimpleNamespace(**{**BASE, "activation_id": act}, vn_beta=0.99999)
+    cfg = types.SimpleNamespace(**{**BASE, "activation_id": act})
     _run(case, cfg, dims, _rows(rows_kind), seed=len(case) * 7 + dims[0])
 
 
@@ -375,15 +335,15 @@ def test_update_contiguous_range_not_at_row_zero(no_tf32, dims, act):
     """A contiguous range (indices == NULL) starting at row 1000 of a larger buffer, 3 G tiles + 37 rows: the TMA path
     for d % 4 == 0, the contiguous gather for d = 7."""
     rows = 3 * _sms() * T_M + 37
-    cfg = types.SimpleNamespace(**{**BASE, "activation_id": act}, vn_beta=0.99999)
+    cfg = types.SimpleNamespace(**{**BASE, "activation_id": act})
     _run(f"contiguous-from-1000-d{dims[0]}-n{dims[1]}-{rows}rows", cfg, dims, rows, contiguous_from=1000, total=rows + 1500,
          seed=dims[0])
 
 
 # ---------------------------------------------------------------- staging paths and rows outside the minibatch --------
 
-KEYS = ("policy_obs", "critic_obs", "actions", "action_log_probs", "advantages", "value_preds", "returns", "active_masks",
-        "action_masks")
+BUF_KEYS = ("policy_obs", "critic_obs", "actions", "action_log_probs", "advantages", "value_preds", "returns",
+            "active_masks", "action_masks")
 
 
 def _exact(case, dims, cfg, buf, state, rows, row_begin, total, gae, mb, idx):
@@ -399,9 +359,9 @@ def _staging_setup(dims):
     G = _sms()
     rows = 30 * G * T_M + 37
     begin, total = 1000, rows + 1500
-    cfg = types.SimpleNamespace(**{**BASE, "activation_id": 1}, vn_beta=0.99999)
+    cfg = types.SimpleNamespace(**{**BASE, "activation_id": 1})
     buf, state, _, rows_idx, _ = _setup(cfg, dims, rows, contiguous_from=begin, total=total, seed=11 + dims[0])
-    gae, mb = fscale._gae_stats(buf), _mb_stats(rows_idx.contiguous(), buf["returns"], buf["active_masks"])
+    gae, mb = h.gae_stats(buf), h.mb_stats(rows_idx.contiguous(), buf["returns"], buf["active_masks"])
     return cfg, buf, state, rows, begin, total, gae, mb, rows_idx.contiguous()
 
 
@@ -433,7 +393,7 @@ def test_rows_outside_the_minibatch_never_matter(dims, poison):
     clean = {p: _exact(p, dims, cfg, buf, state, rows, begin, total, gae, mb, i) for p, i in (("tma", None), ("gather", ar))}
     outside = torch.ones(total, dtype=torch.bool, device="cuda")
     outside[begin:begin + rows] = False
-    for key in KEYS:
+    for key in BUF_KEYS:
         if key in buf:
             x = buf[key]
             v = torch.full_like(x[:x.shape[0]], float("nan")) if poison == "nan" else \
@@ -509,7 +469,7 @@ def _scaled_peaks(r64, state, live):
 
 def _scale_case(case):
     rows = 3 * _sms() * T_M + 37
-    cfg = types.SimpleNamespace(**BASE, vn_beta=0.99999)
+    cfg = types.SimpleNamespace(**BASE)
     kw = SCALE_CASES[case]
     buf, state, idx, rows_idx, total = _setup(cfg, SCALE_DIMS, rows, seed=5, net_edit=kw.get("net_edit"))
     if kw.get("buf_edit"):
@@ -524,8 +484,8 @@ def _scale_case(case):
         print(f"\n  scale-{case} {net}: scaled peaks dZ3 {p['dz3']:.3e}  dZ1 {p['dz1']:.3e}  U {p['u']:.3e}  (limit {ref.FP16_MAX:.0f}; "
               f"scaled by the row count instead: dZ3 {q['dz3']:.3e}  U {q['u']:.3e}); max rstd3 {p['rstd3']:.2e}, "
               f"{live:.0f} of {rows} rows active")
-    k = _launch(cfg, SCALE_DIMS, buf, state, rows, idx, 0, total, fscale._gae_stats(buf),
-                _mb_stats(rows_idx.contiguous(), buf["returns"], buf["active_masks"]))
+    k = _launch(cfg, SCALE_DIMS, buf, state, rows, idx, 0, total, h.gae_stats(buf),
+                h.mb_stats(rows_idx.contiguous(), buf["returns"], buf["active_masks"]))
     return cfg, buf, state, rows_idx, r64, k, peaks, by_rows
 
 

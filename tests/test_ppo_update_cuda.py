@@ -7,36 +7,9 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN
+from helpers import load_buffer, ppo_update_setup
 
 pytestmark = pytest.mark.gpu
-
-
-def _setup(d, flags_extra=()):
-    import torch
-
-    from openrl_b200.algorithms.ppo import PPOAlgorithm
-    from openrl_b200.buffers import NormalReplayBuffer
-    from test_rollout_cuda import _product
-
-    flags = str(d["meta/flags"]).split() + list(flags_extra)
-    cfg, env, net, agent = _product("CartPole-v1", int(d["meta/env_num"]), flags, golden=d)
-    trainer = PPOAlgorithm(cfg, net.module, agent_num=1, device=net.device)
-    buf = NormalReplayBuffer(cfg, 1, env.observation_space, env.action_space, device=net.device)
-    return cfg, net, trainer, buf
-
-
-def _load_buffer(buf, d, it):
-    import torch
-
-    b = buf.data
-    g = lambda k: torch.from_numpy(d[f"it{it}/{k}"]).cuda()
-    b.policy_obs.copy_(g("policy_obs"))
-    b.actions.copy_(g("actions"))
-    b.action_log_probs.copy_(g("action_log_probs"))
-    b.rewards.copy_(g("rewards"))
-    b.masks.copy_(g("masks"))
-    b.active_masks.copy_(g("active_masks"))
-    b.value_preds.copy_(g("value_preds"))
 
 
 @pytest.mark.parametrize("tag", ["cartpole", "cartpole_c1"])
@@ -47,8 +20,8 @@ def test_first_iteration_updates_match_reference(cuda, tag):
     import torch
 
     d = np.load(os.path.join(GOLDEN, f"trace_{tag}.npz"), allow_pickle=True)
-    cfg, net, trainer, buf = _setup(d)
-    _load_buffer(buf, d, 0)
+    cfg, net, trainer, buf = ppo_update_setup(d)
+    load_buffer(buf, d, 0)
     vn = net.module.get_critic_value_normalizer()
     buf.data.compute_returns(buf.data.value_preds[-1].clone(), vn)
     torch.cuda.synchronize()
@@ -87,8 +60,8 @@ def test_gradients_match_oracle_autograd(cuda):
     from oracle import loop, nets, ppo as oppo
 
     d = np.load(os.path.join(GOLDEN, "trace_cartpole.npz"), allow_pickle=True)
-    cfg, net, trainer, buf = _setup(d)
-    _load_buffer(buf, d, 0)
+    cfg, net, trainer, buf = ppo_update_setup(d)
+    load_buffer(buf, d, 0)
     vn = net.module.get_critic_value_normalizer()
     buf.data.compute_returns(buf.data.value_preds[-1].clone(), vn)
     total = cfg.episode_length * int(d["meta/env_num"])
@@ -132,8 +105,8 @@ def test_whole_buffer_minibatch_equals_permuted_minibatch(cuda):
     d = np.load(os.path.join(GOLDEN, "trace_cartpole_c1.npz"), allow_pickle=True)
     res = []
     for use_perm in (False, True):
-        cfg, net, trainer, buf = _setup(d)
-        _load_buffer(buf, d, 0)
+        cfg, net, trainer, buf = ppo_update_setup(d)
+        load_buffer(buf, d, 0)
         vn = net.module.get_critic_value_normalizer()
         buf.data.compute_returns(buf.data.value_preds[-1].clone(), vn)
         total = cfg.episode_length * int(d["meta/env_num"])
@@ -158,9 +131,9 @@ def test_sharded_minibatch_buckets_sum_to_global_bucket(cuda, tf32):
     from openrl_b200 import lib
 
     d = np.load(os.path.join(GOLDEN, "trace_cartpole_c1.npz"), allow_pickle=True)
-    cfg, net, trainer, buf = _setup(d)
+    cfg, net, trainer, buf = ppo_update_setup(d)
     trainer.flags = (trainer.flags | lib.PPO_TENSORCORE) if tf32 else (trainer.flags & ~lib.PPO_TENSORCORE)
-    _load_buffer(buf, d, 0)
+    load_buffer(buf, d, 0)
     vn = net.module.get_critic_value_normalizer()
     buf.data.compute_returns(buf.data.value_preds[-1].clone(), vn)
     total = cfg.episode_length * int(d["meta/env_num"])
@@ -192,9 +165,9 @@ def test_tensor_core_update_matches_fp32_update(cuda):
     d = np.load(os.path.join(GOLDEN, "trace_cartpole_c1.npz"), allow_pickle=True)
     res = []
     for tf32 in (False, True):
-        cfg, net, trainer, buf = _setup(d)
+        cfg, net, trainer, buf = ppo_update_setup(d)
         trainer.flags = (trainer.flags | lib.PPO_TENSORCORE) if tf32 else (trainer.flags & ~lib.PPO_TENSORCORE)
-        _load_buffer(buf, d, 0)
+        load_buffer(buf, d, 0)
         vn = net.module.get_critic_value_normalizer()
         buf.data.compute_returns(buf.data.value_preds[-1].clone(), vn)
         total = cfg.episode_length * int(d["meta/env_num"])
@@ -221,9 +194,9 @@ def test_tensor_core_partial_tile_and_idle_ctas(cuda):
     d = np.load(os.path.join(GOLDEN, "trace_cartpole.npz"), allow_pickle=True)
     res = []
     for tf32 in (False, True):
-        cfg, net, trainer, buf = _setup(d)
+        cfg, net, trainer, buf = ppo_update_setup(d)
         trainer.flags = (trainer.flags | lib.PPO_TENSORCORE) if tf32 else (trainer.flags & ~lib.PPO_TENSORCORE)
-        _load_buffer(buf, d, 0)
+        load_buffer(buf, d, 0)
         vn = net.module.get_critic_value_normalizer()
         buf.data.compute_returns(buf.data.value_preds[-1].clone(), vn)
         trainer.lrs.copy_(torch.tensor([cfg.lr, cfg.critic_lr]))
@@ -245,7 +218,7 @@ def test_algorithm_train_accepts_host_numpy_replay_data(cuda, monkeypatch):
     import torch
 
     d = np.load(os.path.join(GOLDEN, "trace_cartpole.npz"), allow_pickle=True)
-    cfg, net, trainer, buf = _setup(d)
+    cfg, net, trainer, buf = ppo_update_setup(d)
     host = types.SimpleNamespace(**{k: d[f"it0/{k}"].copy() for k in
                                     ("policy_obs", "critic_obs", "value_preds", "returns", "masks", "bad_masks", "active_masks",
                                      "actions", "action_log_probs", "rewards", "action_masks")})

@@ -2,32 +2,21 @@
 compiled with g++ and checked on the CPU against the torch oracle (oracle/nets.py: MLPBase -> RNNLayer ->
 head; reference mlp.py / rnn.py): forward step, chunked BPTT (L steps with masked hidden-state carry) and
 every parameter gradient obtained from the per-row tape as dW = sum_rows P^T Q."""
-import ctypes
-import os
-import subprocess
-
 import numpy as np
 import pytest
 import torch
 
-from conftest import ROOT
+from helpers import gxx_shim, ptr
 from oracle import loop, nets
 
 
 @pytest.fixture(scope="module")
 def shim(tmp_path_factory):
-    out = tmp_path_factory.mktemp("rnn") / "librnnshim.so"
-    subprocess.run(["g++", "-O2", "-shared", "-fPIC", "-I", os.path.join(ROOT, "openrl_b200", "csrc"),
-                    os.path.join(ROOT, "tests", "rnn_core_shim.cpp"), "-o", str(out)], check=True)
-    return ctypes.CDLL(str(out))
+    return gxx_shim(tmp_path_factory, "rnn", "rnn_core_shim.cpp")
 
 
 def _flat(params):
     return np.concatenate([v.detach().numpy().reshape(-1) for v in params.values()]).astype(np.float32)
-
-
-def _ptr(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
 
 
 @pytest.mark.parametrize("kind,d,n,act", [("policy", 18, 5, 1), ("critic", 54, 1, 1), ("policy", 7, 3, 0), ("policy", 4, 2, 3)])
@@ -60,7 +49,7 @@ def test_chunk_forward_backward_matches_torch(shim, kind, d, n, act):
     tape = np.zeros((L * C, T), np.float32)
     Out = np.zeros((L * C, n), np.float32)
     Xn, H0n, mn, dn = (np.ascontiguousarray(a.numpy(), dtype=np.float32) for a in (X, H0.reshape(C, 64), masks.reshape(-1), dlog))
-    shim.shim_chunk_fwdbwd(_ptr(P), d, n, act, L, C, _ptr(Xn), _ptr(H0n), _ptr(mn), _ptr(dn), _ptr(Out), _ptr(tape))
+    shim.shim_chunk_fwdbwd(ptr(P), d, n, act, L, C, ptr(Xn), ptr(H0n), ptr(mn), ptr(dn), ptr(Out), ptr(tape))
     np.testing.assert_allclose(Out, out.detach().numpy(), rtol=1e-4, atol=2e-5)
     t = tape.astype(np.float64)
     dz1, dz3, dgi, dgh, dlg = t[:, 0:64], t[:, 64:128], t[:, 128:320], t[:, 320:512], t[:, 512:512 + n]
@@ -97,6 +86,6 @@ def test_single_step_matches_torch(shim):
     P = _flat(params)
     Hout, Out = np.zeros((rows, 64), np.float32), np.zeros((rows, 5), np.float32)
     Xn, Hn, mn = (np.ascontiguousarray(a.numpy(), dtype=np.float32) for a in (X, Hin.reshape(rows, 64), masks.reshape(-1)))
-    shim.shim_forward_rows(_ptr(P), 18, 5, 1, rows, _ptr(Xn), _ptr(Hn), _ptr(mn), _ptr(Hout), _ptr(Out))
+    shim.shim_forward_rows(ptr(P), 18, 5, 1, rows, ptr(Xn), ptr(Hn), ptr(mn), ptr(Hout), ptr(Out))
     np.testing.assert_allclose(Out, out.numpy(), rtol=1e-4, atol=1e-6)
     np.testing.assert_allclose(Hout, hout.numpy().reshape(rows, 64), rtol=1e-4, atol=1e-6)

@@ -11,11 +11,14 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN
-from test_rnn_core_cpu import _ptr, shim  # noqa: F401  (pytest fixture)
+from helpers import KEYS, gxx_shim, make_agent, ptr
 
 pytestmark = pytest.mark.gpu
 
-KEYS = ["value_loss", "critic_grad_norm", "policy_loss", "dist_entropy", "actor_grad_norm", "ratio"]
+
+@pytest.fixture(scope="module")
+def shim(tmp_path_factory):
+    return gxx_shim(tmp_path_factory, "rnn", "rnn_core_shim.cpp")
 
 
 class _OracleHost:
@@ -129,30 +132,6 @@ class _SyntheticMultiAgentRanges(_SyntheticMultiAgent):
         return self._step(lo, hi, actions)
 
 
-def _agent(env, flags, golden=None, like=None):
-    """golden: the reference's initial weights (init/<net>.<key>); like: {net: state_dict} of weights to start from."""
-    import torch
-
-    from openrl_b200.configs.config import create_config_parser
-    from openrl_b200.modules.common import PPONet
-    from openrl_b200.runners.common import PPOAgent
-    from openrl_b200.utils.logger import Logger
-
-    cfg = create_config_parser().parse_args(flags)
-    cfg.quiet = True
-    net = PPONet(env, cfg=cfg, device="cuda:0")
-    for mk in ("policy", "critic"):
-        sd = net.module.models[mk].state_dict()
-        for k in list(sd.keys()):
-            if golden is not None and f"init/{mk}.{k}" in golden:
-                sd[k].copy_(torch.from_numpy(golden[f"init/{mk}.{k}"]))
-            elif like is not None:
-                sd[k].copy_(like[mk][k])
-    agent = PPOAgent(net)
-    agent.train(total_time_steps=0, logger=Logger(quiet=True))   # builds trainer / buffer / driver, resets the envs
-    return cfg, net, agent
-
-
 def test_host_recurrent_cartpole_matches_reference_trace(cuda):
     """The executed reference's CartPole GRU run (8 envs, T = 32, episodes ending inside chunks, L = 4, two minibatches)
     with the numpy CartPole stepped on the host in parity mode."""
@@ -162,7 +141,7 @@ def test_host_recurrent_cartpole_matches_reference_trace(cuda):
     iters, N = int(d["meta/iters"]), int(d["meta/env_num"])
     flags = str(d["meta/flags"]).split() + ["--parity_mode", "true", "--log_interval", "1"]
     env = HostVecEnv(_cartpole_host(N))
-    cfg, net, agent = _agent(env, flags, golden=d)
+    cfg, net, agent = make_agent(env, flags, golden=d)
     drv = agent.driver
     assert drv.recurrent and env.kind == 0
     b = drv.buffer.data
@@ -217,7 +196,7 @@ def test_host_recurrent_rollout_is_bit_identical_to_device_rollout(cuda, env_id,
     assert host_env.supports_groups
     runs, init = [], None
     for env in (dev_env, host_env):
-        cfg, net, agent = _agent(env, flags, like=init)   # the host run starts from the device run's initial weights
+        cfg, net, agent = make_agent(env, flags, like=init)   # the host run starts from the device run's initial weights
         if init is None:
             init = {mk: {k: v.clone() for k, v in net.module.models[mk].state_dict().items()} for mk in ("policy", "critic")}
         drv = agent.driver
@@ -260,7 +239,7 @@ def test_host_recurrent_multi_agent_states_match_sequential_core(cuda, shim, mod
     host = (_SyntheticMultiAgentRanges if grouped else _SyntheticMultiAgent)(N, A)
     env = HostVecEnv(host)
     assert env.supports_groups == grouped
-    cfg, net, agent = _agent(env, flags)
+    cfg, net, agent = make_agent(env, flags)
     drv = agent.driver
     b = drv.buffer.data
     rows = N * A
@@ -278,8 +257,8 @@ def test_host_recurrent_multi_agent_states_match_sequential_core(cuda, shim, mod
         for t in range(T):
             X, H0, m = (np.ascontiguousarray(v.cpu().numpy().reshape(rows, -1)) for v in (obs[t], hs[t], mk[t]))
             want, out = np.zeros((rows, 64), np.float32), np.zeros((rows, pol.n_actions), np.float32)
-            shim.shim_forward_rows(_ptr(P), pol.obs_dim, pol.n_actions, pol.activation_id, rows, _ptr(X), _ptr(H0), _ptr(m),
-                                   _ptr(want), _ptr(out))
+            shim.shim_forward_rows(ptr(P), pol.obs_dim, pol.n_actions, pol.activation_id, rows, ptr(X), ptr(H0), ptr(m),
+                                   ptr(want), ptr(out))
             got = hs[t + 1].cpu().numpy().reshape(rows, 64)
             assert (got[fin[t]] == 0).all(), t
             np.testing.assert_allclose(got[~fin[t]], want[~fin[t]], rtol=0, atol=2e-6, err_msg=f"it{it} t{t}")
@@ -296,7 +275,7 @@ def test_make_custom_envs_trains_a_recurrent_policy(cuda):
     from openrl_b200.modules.common import PPONet
     from openrl_b200.runners.common import PPOAgent
     from openrl_b200.utils.logger import Logger
-    from test_host_sync_env import CountEnv
+    from helpers import CountEnv
 
     T, N = 16, 6
     for grouped in ("false", "true"):

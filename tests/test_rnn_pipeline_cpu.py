@@ -14,14 +14,21 @@ and the six scalars of every update plus the parameters after the iteration must
 import os
 
 import numpy as np
+import pytest
 import torch
 
 from conftest import GOLDEN
 from oracle import loop, nets, ppo
 import rnn_pipeline_helpers as hp
-from test_rnn_core_cpu import shim  # noqa: F401  (pytest fixture)
+from helpers import gxx_shim
 
-def test_device_recurrent_pipeline_on_cpu_matches_reference_trace(shim):  # noqa: F811
+
+@pytest.fixture(scope="module")
+def shim(tmp_path_factory):
+    return gxx_shim(tmp_path_factory, "rnn", "rnn_core_shim.cpp")
+
+
+def test_device_recurrent_pipeline_on_cpu_matches_reference_trace(shim):
     d = np.load(os.path.join(GOLDEN, "trace_cartpole_gru.npz"), allow_pickle=True)
     cfg = loop.cfg_from_flags(str(d["meta/flags"]))
     N, T, L, dim, n = int(d["meta/env_num"]), cfg.episode_length, cfg.data_chunk_length, 4, 2

@@ -9,10 +9,10 @@ crossings, and active masks with zeros.
 
 The reference is tests/rnn_ref64.py (pinned to the unmodified reference's traces by tests/test_rnn_ref64_cpu.py).
 
-Bars of the update (gradients per parameter block, loss sums per scalar, parameters / Adam moments / ValueNorm state
+Bars of the update (tests/scale_harness.py; gradients per parameter block, loss sums per scalar, parameters / Adam moments / ValueNorm state
 after the optimizer step) are self-calibrating: the reference runs once in float64 and once in float32 (TF32 off
 for matmul and cuDNN), and the kernel's error against float64 may be at most RATIO x the float32 reference's error
-against float64, never less than FLOOR and never more than CEIL (relative L2 norm per block; relative error per scalar,
+against float64, never less than RNN_FLOOR and never more than CEIL (relative L2 norm per block; relative error per scalar,
 against the sum of the absolute loss terms).  Rollout and critic quantities are compared element-wise at the 2e-5
 absolute bar of tests/test_gru_cuda.py, teacher-forced: every float64 step starts from the device's own hidden state.
 Every case prints its observed kernel / float32 error ratios (`pytest -s`)."""
@@ -23,97 +23,12 @@ import pytest
 import torch
 
 import rnn_ref64
+import scale_harness as h
+from scale_harness import ATOL, BASE, no_tf32  # noqa: F401  (no_tf32: pytest fixture)
 
 pytestmark = pytest.mark.gpu
 
-# FLOOR: the C3 entropy sum (153 600 terms added per lane, per CTA and by float atomics) is 1.1e-6 off float64, where
-# torch's pairwise float32 sum is 1.6e-9 off: a long float32 sum in a fixed kernel order legitimately reaches ~1e-6.
-RATIO, FLOOR, CEIL = 4.0, 2e-6, 1e-3
-ATOL = 2e-5
 T, H = 25, 64
-KINK = 5e-3   # synthetic rows keep at least this distance from every branch point of the loss
-
-
-@pytest.fixture
-def no_tf32():
-    before = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = False
-    torch.backends.cudnn.allow_tf32 = False
-    yield
-    torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = before
-
-
-def _rel(x, ref, scale=None):
-    den = float(ref.double().norm()) if scale is None else float(scale)
-    num = float((x.double() - ref.double()).norm())
-    return num / den if den > 0 else num
-
-
-class Checker:
-    """Collects kernel-vs-float64 errors against the self-calibrated bar; fails with every violation listed."""
-
-    def __init__(self, case, floor=FLOOR):
-        self.case, self.bad, self.worst, self.floor = case, [], (0.0, ""), floor
-
-    def bar(self, e32):
-        return min(max(RATIO * e32, self.floor), CEIL)
-
-    def __call__(self, what, got, r64, r32, scale=None):
-        ek, e32 = _rel(got, r64, scale), _rel(r32, r64, scale)
-        bar = self.bar(e32)
-        ratio = ek / e32 if e32 > 0 else (0.0 if ek == 0 else float("inf"))
-        if ratio > self.worst[0]:
-            self.worst = (ratio, what)
-        print(f"  {self.case:48s} {what:44s} kernel {ek:9.2e}  fp32 {e32:9.2e}  ratio {ratio:7.2f}")
-        if not ek <= bar:
-            self.bad.append(f"{what}: kernel {ek:.3e} > bar {bar:.3e} (fp32 {e32:.3e})")
-
-    def done(self):
-        print(f"  {self.case}: worst kernel/fp32 error ratio {self.worst[0]:.2f} ({self.worst[1]})")
-        assert not self.bad, f"{self.case}:\n" + "\n".join(self.bad)
-
-
-def _compare(case, dims, k, r64, r32, check_vn):
-    d, n, dc = dims
-    chk = Checker(case)
-    for net, dd, nn, critic in (("pol", d, n, False), ("cri", dc, 1, True)):
-        for name, s in rnn_ref64.blocks(dd, nn, critic).items():
-            chk(f"grad {net}.{name}", k["grad_" + net][s], r64["grad_" + net][s], r32["grad_" + net][s])
-    for i, name in enumerate(("policy loss", "entropy", "ratio sum", "value loss")):
-        chk(f"loss_acc[{i}] {name}", k["losses"][i:i + 1], r64["losses"][i:i + 1], r32["losses"][i:i + 1],
-            scale=r64["loss_scales"][i])
-    for net, dd, nn, critic in (("pol", d, n, False), ("cri", dc, 1, True)):
-        for key in ("", "_m", "_v"):
-            for name, s in rnn_ref64.blocks(dd, nn, critic).items():
-                chk(f"{net}{key or '_param'} {name}", k[net + key][s], r64[net + key][s], r32[net + key][s])
-    if check_vn:
-        chk("vn_state", k["vn"], r64["vn"], r32["vn"])
-    assert k["steps"] == [r64["pol_step"], r64["cri_step"]]
-    chk.done()
-
-
-def _lib():
-    from openrl_b200 import lib
-    return lib, lib.load()
-
-
-def _drive(a, grads, loss_acc, outs):
-    """orl_rnn_fwdbwd (gradients, loss sums), then orl_rnn_apply; `outs` names the device tensors read back after."""
-    lib, L = _lib()
-    s = lib.current_stream()
-    lib.check(L.orl_rnn_fwdbwd(a, s), "orl_rnn_fwdbwd")
-    g, la = grads.clone(), loss_acc[:4].clone()
-    lib.check(L.orl_rnn_apply(a, s), "orl_rnn_apply")
-    torch.cuda.synchronize()
-    return g, la, {k: v.clone() for k, v in outs.items()}
-
-
-def _mb_stats(rows_idx, buf_returns, buf_active):
-    lib, L = _lib()
-    out = torch.zeros(3, dtype=torch.float64, device="cuda")
-    lib.check(L.orl_minibatch_stats(lib.ptr(rows_idx), int(rows_idx.numel()), lib.ptr(buf_returns), lib.ptr(buf_active),
-                                    lib.ptr(out), lib.current_stream()), "orl_minibatch_stats")
-    return out
 
 
 def _refs(cfg, buf, state, ids, L, dims, joint):
@@ -131,20 +46,13 @@ C3_FLAGS = ["--episode_length", "25", "--lr", "7e-4", "--critic_lr", "7e-4", "--
 @pytest.fixture(scope="module")
 def c3():
     """One fast-mode device rollout of C3 (orl_rnn_rollout), its critic pass (orl_rnn_critic) and returns (orl_gae)."""
-    from openrl_b200.configs.config import create_config_parser
     from openrl_b200.envs.common import make
-    from openrl_b200.modules.common import PPONet
-    from openrl_b200.runners.common import PPOAgent
-    from openrl_b200.utils.logger import Logger
+    from helpers import make_agent
 
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     torch.manual_seed(0)
-    cfg = create_config_parser().parse_args(C3_FLAGS)
-    cfg.quiet = True
-    env = make("simple_spread", env_num=2048)
-    agent = PPOAgent(PPONet(env, cfg=cfg, device="cuda:0"))
-    agent.train(total_time_steps=0, logger=Logger(quiet=True))
+    cfg, _, agent = make_agent(make("simple_spread", env_num=2048), C3_FLAGS)
     drv = agent.driver
     drv.actor_rollout()
     drv.compute_returns()
@@ -154,11 +62,6 @@ def c3():
     yield types.SimpleNamespace(cfg=cfg, agent=agent, drv=drv, tr=tr, b=b)
     tr.tape = None
     torch.cuda.empty_cache()
-
-
-def _c3_buf(b):
-    return {k: getattr(b, k) for k in ("policy_obs", "critic_obs", "rnn_states", "rnn_states_critic", "masks", "active_masks",
-                                       "actions", "action_log_probs", "value_preds", "returns", "advantages")}
 
 
 @pytest.mark.parametrize("mode,mini", [("ordinary", 1), ("ordinary", 7), ("jrpo", 1), ("jrpo", 7)],
@@ -183,11 +86,11 @@ def test_update_on_c3_buffer(c3, no_tf32, mode, mini):
     g = torch.Generator(device="cuda").manual_seed(11 + mini + 100 * joint)
     ids = torch.randperm(total, device="cuda", generator=g)[:total // mini].contiguous()
     if joint:
-        stats = torch.cat([_mb_stats(v3_row_indices(ids, L, T, A, B, all_agents=ev), b.returns, b.active_masks) for ev in (False, True)])
+        stats = torch.cat([h.mb_stats(v3_row_indices(ids, L, T, A, B, all_agents=ev), b.returns, b.active_masks) for ev in (False, True)])
     elif mini == 1:
         stats = b.gae_stats[5:8]
     else:
-        stats = _mb_stats(chunk_row_indices(ids, L, T, B), b.returns, b.active_masks)
+        stats = h.mb_stats(chunk_row_indices(ids, L, T, B), b.returns, b.active_masks)
     tape_rows = ids.numel() * L * (A if joint else 1)
     tr.tape = torch.empty(int(tr._lib.orl_rnn_workspace_floats(tape_rows, tr.rnn_stride)), dtype=torch.float32, device="cuda")
     tr.sync_lrs()
@@ -197,7 +100,7 @@ def test_update_on_c3_buffer(c3, no_tf32, mode, mini):
         a = tr._rnn_args(b, ids, stats)
         if joint:
             a.flags |= lib.PPO_JOINT_ACTION
-        grads, la, after = _drive(a, tr.rnn_grads, tr.loss_acc, live)
+        grads, la, after = h.drive(a, tr.rnn_grads, tr.loss_acc, live)
         steps = [int(x) for x in m.adam_steps]
     finally:
         tr.tape = None
@@ -208,8 +111,8 @@ def test_update_on_c3_buffer(c3, no_tf32, mode, mini):
     dims = (tr.d, tr.n, tr.dc)
     np_, nc = int(pol.flat_params.numel()), int(cri.flat_params.numel())
     k = dict(grad_pol=grads[0, :np_], grad_cri=grads[1, :nc], losses=la, steps=steps, **after)
-    r64, r32 = _refs(rcfg, _c3_buf(b), state, ids, L, dims, joint)
-    _compare(f"c3-{mode}-mb{mini}", dims, k, r64, r32, check_vn=True)
+    r64, r32 = _refs(rcfg, h.c3_buf(b), state, ids, L, dims, joint)
+    h.rnn_compare(f"c3-{mode}-mb{mini}", dims, k, r64, r32, check_vn=True)
 
 
 def test_critic_pass_at_c3(c3):
@@ -217,23 +120,23 @@ def test_critic_pass_at_c3(c3):
     rnn_states_critic[t+1] (zero where masks[t+1] == 0) from the device's own rnn_states_critic[t]."""
     from oracle import nets
 
-    lib, Lb = _lib()
+    lb, Lb = h.lib()
     drv, b, cri = c3.drv, c3.b, c3.tr.algo_module.models["critic"]
-    lib.check(Lb.orl_rnn_critic(drv._rnn_args(0, T, None), lib.current_stream()), "orl_rnn_critic")
+    lb.check(Lb.orl_rnn_critic(drv._rnn_args(0, T, None), lb.current_stream()), "orl_rnn_critic")
     torch.cuda.synchronize()
     dc = c3.tr.dc
     p = {k: v.detach().double() for k, v in rnn_ref64.unflatten(cri.flat_params.double(), dc, 1, True).items()}
     ncfg = rnn_ref64.net_cfg(c3.cfg.activation_id, True)
-    h = rnn_ref64.rows(b.rnn_states_critic).double()
+    hid = rnn_ref64.rows(b.rnn_states_critic).double()
     masks = rnn_ref64.rows(b.masks).double()
     with torch.no_grad():
-        v, hn = nets.critic_forward(p, ncfg, rnn_ref64.rows(b.critic_obs).double(), h.unsqueeze(1), masks)
+        v, hn = nets.critic_forward(p, ncfg, rnn_ref64.rows(b.critic_obs).double(), hid.unsqueeze(1), masks)
     B = b.n_rollout_threads * b.num_agents
     np.testing.assert_allclose(rnn_ref64.rows(b.value_preds).cpu().numpy(), v.cpu().numpy(), rtol=0, atol=ATOL)
     want = hn[:T * B, 0] * (masks[B:] != 0)
-    np.testing.assert_allclose(h[B:].cpu().numpy(), want.cpu().numpy(), rtol=0, atol=ATOL)
+    np.testing.assert_allclose(hid[B:].cpu().numpy(), want.cpu().numpy(), rtol=0, atol=ATOL)
     reset = masks[B:, 0] == 0
-    assert int(reset.sum()) > 0 and bool((h[B:][reset] == 0).all()) and bool((h[B:][~reset].abs().amax(1) > 0).all())
+    assert int(reset.sum()) > 0 and bool((hid[B:][reset] == 0).all()) and bool((hid[B:][~reset].abs().amax(1) > 0).all())
 
 
 def test_rollout_at_c3(c3):
@@ -245,16 +148,16 @@ def test_rollout_at_c3(c3):
     B = b.n_rollout_threads * b.num_agents
     p = {k: v.detach().double() for k, v in rnn_ref64.unflatten(pol.flat_params.double(), c3.tr.d, c3.tr.n, False).items()}
     ncfg = rnn_ref64.net_cfg(c3.cfg.activation_id, True)
-    h = rnn_ref64.rows(b.rnn_states).double()
+    hid = rnn_ref64.rows(b.rnn_states).double()
     masks = rnn_ref64.rows(b.masks).double()
     with torch.no_grad():
-        feat, hn = nets.policy_features(p, ncfg, rnn_ref64.rows(b.policy_obs).double()[:T * B], h[:T * B].unsqueeze(1), masks[:T * B])
+        feat, hn = nets.policy_features(p, ncfg, rnn_ref64.rows(b.policy_obs).double()[:T * B], hid[:T * B].unsqueeze(1), masks[:T * B])
         lp = nets.categorical_logits(p, feat).gather(-1, rnn_ref64.rows(b.actions).long())
     np.testing.assert_allclose(rnn_ref64.rows(b.action_log_probs).cpu().numpy(), lp.cpu().numpy(), rtol=0, atol=ATOL)
     want = hn[:, 0] * (masks[B:] != 0)
-    np.testing.assert_allclose(h[B:].cpu().numpy(), want.cpu().numpy(), rtol=0, atol=ATOL)
+    np.testing.assert_allclose(hid[B:].cpu().numpy(), want.cpu().numpy(), rtol=0, atol=ATOL)
     reset = masks[B:, 0] == 0
-    assert int(reset.sum()) > 0 and bool((h[B:][reset] == 0).all())
+    assert int(reset.sum()) > 0 and bool((hid[B:][reset] == 0).all())
 
 
 @pytest.mark.parametrize("mini", [1, 7])
@@ -270,7 +173,7 @@ def test_minibatch_stats_at_c3(c3, mini):
     for idx in (chunk_row_indices(torch.randperm(T * B // L, device="cuda", generator=g)[:T * B // L // mini], L, T, B),
                 v3_row_indices(torch.randperm(T * N // L, device="cuda", generator=g)[:T * N // L // mini], L, T, A, B),
                 v3_row_indices(torch.randperm(T * N // L, device="cuda", generator=g)[:T * N // L // mini], L, T, A, B, all_agents=True)):
-        got = _mb_stats(idx, b.returns, b.active_masks)
+        got = h.mb_stats(idx, b.returns, b.active_masks)
         r, a = ret[idx], act[idx]
         want = torch.stack([r.sum(), (r * r).sum(), a.sum()])
         np.testing.assert_allclose(got.cpu().numpy(), want.cpu().numpy(), rtol=1e-12, atol=0)
@@ -278,39 +181,6 @@ def test_minibatch_stats_at_c3(c3, mini):
 
 
 # ---------------------------------------------------------------- synthetic buffers -----------------------------------
-
-BASE = dict(use_huber_loss=True, use_clipped_value_loss=True, use_value_active_masks=True, use_policy_active_masks=True,
-            use_valuenorm=True, use_adv_normalize=False, use_max_grad_norm=True, dual_clip_ppo=False, activation_id=1,
-            clip_param=0.2, entropy_coef=0.01, value_loss_coef=0.5, huber_delta=1.0, max_grad_norm=1e3, dual_clip_coeff=3.0,
-            lr=7e-4, critic_lr=5e-4, opti_eps=1e-5, weight_decay=0.0, vn_beta=0.99999)
-
-
-def _flags(c):
-    from openrl_b200 import lib
-    return ((lib.PPO_HUBER if c.use_huber_loss else 0) | (lib.PPO_CLIP_VALUE if c.use_clipped_value_loss else 0)
-            | (lib.PPO_VALUE_ACTIVE_MASKS if c.use_value_active_masks else 0)
-            | (lib.PPO_POLICY_ACTIVE_MASKS if c.use_policy_active_masks else 0) | (lib.PPO_VALUENORM if c.use_valuenorm else 0)
-            | (lib.PPO_ADV_NORMALIZE if c.use_adv_normalize else 0) | (lib.PPO_MAX_GRAD_NORM if c.use_max_grad_norm else 0)
-            | (lib.PPO_DUAL_CLIP if c.dual_clip_ppo else 0))
-
-
-def _random_net(g, d, n, critic):
-    parts = []
-    for name, shp in rnn_ref64.param_shapes(d, n, critic):
-        x = torch.randn(shp, generator=g, device="cuda")
-        if len(shp) == 2:
-            x *= (0.3 if name.startswith(("act.", "v_out")) else 1.0) / shp[1] ** 0.5
-        elif name.endswith("weight"):   # LayerNorm gains
-            x = 1.0 + 0.2 * x
-        else:
-            x *= 0.1
-        parts.append(x.reshape(-1))
-    return torch.cat(parts)
-
-
-def _redraw(bad, draw, x):
-    return torch.where(bad, draw(x.shape), x)
-
 
 def _synthetic(cfg, dims, L, B, n_chunks, seed):
     """A (T, B) buffer of random observations / hidden states / masks, nets with random weights, Adam moments mid-run,
@@ -339,8 +209,8 @@ def _synthetic(cfg, dims, L, B, n_chunks, seed):
     if len(cross):
         m[rp[cross[0, 0], cross[0, 1]]] = 0.0                    # trajectory-row crossing
     assert L == 1 or len(cross) or n_chunks < 3
-    state = dict(pol=_random_net(g, d, n, False), cri=_random_net(g, dc, 1, True), vn=torch.tensor([0.3, 1.5, 0.8], device="cuda"),
-                 steps=[3, 3])
+    state = dict(pol=h.random_net(g, rnn_ref64.param_shapes(d, n, False)), cri=h.random_net(g, rnn_ref64.param_shapes(dc, 1, True)),
+                 vn=torch.tensor([0.3, 1.5, 0.8], device="cuda"), steps=[3, 3])
     for k in ("pol", "cri"):
         state[k + "_m"] = 1e-3 * r(state[k].numel())
         state[k + "_v"] = 1e-6 * u(state[k].numel()) + 1e-8
@@ -350,63 +220,15 @@ def _synthetic(cfg, dims, L, B, n_chunks, seed):
     with torch.no_grad():
         rp, rc, logp, _, v = rnn_ref64.forward(types.SimpleNamespace(**cfg.__dict__), buf, pol, cri, ids, L, False, torch.float64)
     rp, rc = rp.reshape(-1), rc.reshape(-1)
-    kinks = torch.tensor([1 - cfg.clip_param, 1 + cfg.clip_param, cfg.dual_clip_coeff], device="cuda", dtype=torch.float64)
-
-    def draw_ratio(shape):
-        near = torch.exp(0.25 * torch.randn(shape, generator=g, device="cuda", dtype=torch.float64))
-        far = 2.5 + 1.5 * torch.rand(shape, generator=g, device="cuda", dtype=torch.float64)
-        return torch.where(torch.rand(shape, generator=g, device="cuda", dtype=torch.float64) < 0.1, far, near)
-    ratio = draw_ratio(logp.shape)
-    for _ in range(50):
-        bad = ((ratio[..., None] - kinks).abs() < KINK).any(-1)
-        if not bool(bad.any()):
-            break
-        ratio = _redraw(bad, draw_ratio, ratio)
     rows = lambda k: rnn_ref64.rows(buf[k])   # noqa: E731
-    rows("action_log_probs")[rp] = (logp - ratio.log()).float()
-    lp32 = rows("action_log_probs")[rp].double()
-    assert bool((((logp - lp32).exp()[..., None] - kinks).abs() >= KINK / 2).all())
-
-    draw_delta = lambda shape: 0.4 * torch.randn(shape, generator=g, device="cuda", dtype=torch.float64)   # noqa: E731
-    delta = draw_delta(v.shape)
-    for _ in range(50):
-        bad = (delta.abs() - cfg.clip_param).abs() < KINK
-        if not bool(bad.any()):
-            break
-        delta = _redraw(bad, draw_delta, delta)
-    rows("value_preds")[rc] = (v - delta).float()
-    vp = rows("value_preds")[rc].double()
-    draw_ret = lambda shape: 2 * torch.randn(shape, generator=g, device="cuda", dtype=torch.float64) + 0.5   # noqa: E731
-    ret = draw_ret(v.shape)
-    for it in range(100):
-        r32 = ret.float().double()
-        target = r32
-        if cfg.use_valuenorm:
-            target = rnn_ref64.vn_normalize(rnn_ref64.vn_update(state["vn"].double(), r32, cfg.vn_beta), r32)
-        clipped = vp + (v - vp).clamp(-cfg.clip_param, cfg.clip_param)
-        e_o, e_c = (target - v).abs(), (target - clipped).abs()
-        outside = (v - vp).abs() > cfg.clip_param
-        bad = (((e_o - cfg.huber_delta).abs() < KINK) | ((e_c - cfg.huber_delta).abs() < KINK)
-               | (outside & ((e_o - e_c).abs() < KINK)))
-        if not bool(bad.any()):
-            break
-        ret = _redraw(bad, draw_ret, ret)
-    assert not bool(bad.any()), "returns kept landing on a kink"
-    rows("returns")[rc] = ret.float()
+    h.draw_kink_free(g, cfg, state["vn"], logp, v, rows("action_log_probs"), rp, rows("value_preds"), rows("returns"), rc,
+                   ratio_spread=0.25, returns_draw=(2.0, 0.5), both_clip_sides=False)
     return buf, state, ids
-
-
-def _gae_stats(buf):
-    adv = rnn_ref64.rows(buf["advantages"]).double()[:, 0]
-    act = rnn_ref64.rows(buf["active_masks"]).double()[:adv.numel(), 0] != 0
-    ret = rnn_ref64.rows(buf["returns"]).double()[:adv.numel(), 0]
-    return torch.stack([adv.sum(), (adv * adv).sum(), torch.tensor(float(adv.numel()), device="cuda", dtype=torch.float64),
-                        adv[act].sum(), (adv[act] ** 2).sum(), ret.sum(), (ret * ret).sum(), act.double().sum()])
 
 
 def _run_synthetic(case, cfg, dims, L, B, n_chunks, seed):
     """OrlRnnArgs built by hand for a synthetic buffer; kernel against both reference runs."""
-    lib, Lb = _lib()
+    lb, Lb = h.lib()
     from openrl_b200.buffers.replay_data import chunk_row_indices
 
     d, n, dc = dims
@@ -418,36 +240,33 @@ def _run_synthetic(case, cfg, dims, L, B, n_chunks, seed):
     dev = {k: state[k].clone() for k in ("pol", "cri", "pol_m", "pol_v", "cri_m", "cri_v", "vn")}
     steps = torch.tensor(state["steps"], dtype=torch.int32, device="cuda")
     lrs = torch.tensor([cfg.lr, cfg.critic_lr], dtype=torch.float32, device="cuda")
-    gae_stats = _gae_stats(buf)
-    mb_stats = _mb_stats(chunk_row_indices(ids, L, T, B), buf["returns"], buf["active_masks"])
+    gae = h.gae_stats({k: rnn_ref64.rows(buf[k]) for k in ("advantages", "active_masks", "returns")})
+    mb = h.mb_stats(chunk_row_indices(ids, L, T, B), buf["returns"], buf["active_masks"])
     tape = torch.empty(int(Lb.orl_rnn_workspace_floats(n_chunks * L, stride)), dtype=torch.float32, device="cuda")
     train_info = torch.zeros(6, dtype=torch.float32, device="cuda")
     ids = ids.contiguous()
-    a = lib.OrlRnnArgs()
+    a = lb.OrlRnnArgs()
     a.n_envs, a.n_agents, a.episode_length = B, 1, T
     a.obs_dim, a.critic_obs_dim, a.n_actions, a.activation_id = d, dc, n, cfg.activation_id
-    a.chunk_length, a.flags, a.n_chunks, a.chunk_ids = L, _flags(cfg), n_chunks, lib.ptr(ids)
-    a.policy_params, a.critic_params = lib.ptr(dev["pol"]), lib.ptr(dev["cri"])
+    a.chunk_length, a.flags, a.n_chunks, a.chunk_ids = L, h.ppo_flags(cfg), n_chunks, lb.ptr(ids)
+    a.policy_params, a.critic_params = lb.ptr(dev["pol"]), lb.ptr(dev["cri"])
     for k in ("policy_obs", "critic_obs", "rnn_states", "rnn_states_critic", "actions", "action_log_probs", "masks", "active_masks",
               "value_preds", "returns", "advantages"):
-        setattr(a, k, lib.ptr(buf[k]))
-    a.gae_stats, a.mb_stats, a.vn_state = lib.ptr(gae_stats), lib.ptr(mb_stats), lib.ptr(dev["vn"])
-    a.tape, a.grads, a.grads_stride, a.loss_acc = lib.ptr(tape), lib.ptr(grads), stride, lib.ptr(loss_acc)
-    a.policy_adam_m, a.policy_adam_v = lib.ptr(dev["pol_m"]), lib.ptr(dev["pol_v"])
-    a.critic_adam_m, a.critic_adam_v = lib.ptr(dev["cri_m"]), lib.ptr(dev["cri_v"])
-    a.adam_steps, a.lrs, a.train_info = lib.ptr(steps), lib.ptr(lrs), lib.ptr(train_info)
-    a.clip_param, a.entropy_coef, a.value_loss_coef = cfg.clip_param, cfg.entropy_coef, cfg.value_loss_coef
-    a.huber_delta, a.max_grad_norm, a.dual_clip_coeff = cfg.huber_delta, cfg.max_grad_norm, cfg.dual_clip_coeff
-    a.adam_beta1, a.adam_beta2, a.adam_eps, a.weight_decay = 0.9, 0.999, cfg.opti_eps, cfg.weight_decay
-    a.vn_beta, a.norm_rows = cfg.vn_beta, 0
-    g, la, after = _drive(a, grads, loss_acc, dev)
+        setattr(a, k, lb.ptr(buf[k]))
+    a.gae_stats, a.mb_stats, a.vn_state = lb.ptr(gae), lb.ptr(mb), lb.ptr(dev["vn"])
+    a.tape, a.grads, a.grads_stride, a.loss_acc = lb.ptr(tape), lb.ptr(grads), stride, lb.ptr(loss_acc)
+    a.policy_adam_m, a.policy_adam_v = lb.ptr(dev["pol_m"]), lb.ptr(dev["pol_v"])
+    a.critic_adam_m, a.critic_adam_v = lb.ptr(dev["cri_m"]), lb.ptr(dev["cri_v"])
+    a.adam_steps, a.lrs, a.train_info = lb.ptr(steps), lb.ptr(lrs), lb.ptr(train_info)
+    h.fill_coefs(a, cfg)
+    g, la, after = h.drive(a, grads, loss_acc, dev)
     del tape
     k = dict(grad_pol=g[0, :state["pol"].numel()], grad_cri=g[1, :state["cri"].numel()], losses=la,
              steps=[int(x) for x in steps], **after)
     r64, r32 = _refs(cfg, buf, state, ids, L, dims, False)
     if cfg.use_max_grad_norm and cfg.max_grad_norm < 1:   # the clip case: the clip must really act on both nets
         assert float(r64["norms"][0]) > cfg.max_grad_norm and float(r64["norms"][1]) > cfg.max_grad_norm
-    _compare(case, dims, k, r64, r32, check_vn=cfg.use_valuenorm)
+    h.rnn_compare(case, dims, k, r64, r32, check_vn=cfg.use_valuenorm)
     torch.cuda.empty_cache()
 
 

@@ -9,35 +9,14 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN
+from helpers import product
 
 pytestmark = pytest.mark.gpu
 
 
-def _product(env_id, env_num, flags, golden=None, **env_kw):
-    import torch
-
-    from openrl_b200.configs.config import create_config_parser
-    from openrl_b200.envs.common import make
-    from openrl_b200.modules.common import PPONet
-    from openrl_b200.runners.common import PPOAgent
-
-    cfg = create_config_parser().parse_args(flags + ["--parity_mode", "true", "--log_interval", "1"])
-    cfg.quiet = True
-    env = make(env_id, env_num=env_num, **env_kw)
-    net = PPONet(env, cfg=cfg, device="cuda:0")
-    if golden is not None:  # pin the initial weights to the reference's (QR in orthogonal_ may differ by 1 ulp across BLAS threads)
-        for mk in ("policy", "critic"):
-            sd = net.module.models[mk].state_dict()
-            for k in list(sd.keys()):
-                gk = f"init/{mk}.{k}"
-                if gk in golden:
-                    sd[k].copy_(torch.from_numpy(golden[gk]))
-    return cfg, env, net, PPOAgent(net)
-
-
 def test_seeded_init_matches_reference(cuda):
     d = np.load(os.path.join(GOLDEN, "trace_cartpole.npz"), allow_pickle=True)
-    cfg, env, net, agent = _product("CartPole-v1", 8, str(d["meta/flags"]).split())
+    cfg, env, net, agent = product("CartPole-v1", 8, str(d["meta/flags"]).split())
     for mk in ("policy", "critic"):
         for k, v in net.module.models[mk].state_dict().items():
             gk = f"init/{mk}.{k}"
@@ -52,7 +31,7 @@ def test_cartpole_rollout_matches_reference_trace(cuda, tag):
 
     d = np.load(os.path.join(GOLDEN, f"trace_{tag}.npz"), allow_pickle=True)
     flags = str(d["meta/flags"]).split()
-    cfg, env, net, agent = _product("CartPole-v1", int(d["meta/env_num"]), flags, golden=d)
+    cfg, env, net, agent = product("CartPole-v1", int(d["meta/env_num"]), flags, golden=d)
     from openrl_b200.algorithms.ppo import PPOAlgorithm
     from openrl_b200.buffers import NormalReplayBuffer
     from openrl_b200.drivers.onpolicy_driver import OnPolicyDriver
@@ -85,7 +64,7 @@ def test_rollout_single_launch_equals_per_step_launches(cuda):
 
     outs = []
     for per_step in (False, True):
-        cfg, env, net, agent = _product("CartPole-v1", 64, ["--seed", "3", "--episode_length", "40"])
+        cfg, env, net, agent = product("CartPole-v1", 64, ["--seed", "3", "--episode_length", "40"])
         from openrl_b200.algorithms.ppo import PPOAlgorithm
         from openrl_b200.buffers import NormalReplayBuffer
         from openrl_b200.drivers.onpolicy_driver import OnPolicyDriver

@@ -7,20 +7,15 @@
 - The sequential core of the CUDA kernels (openrl_b200/csrc/orl_deep_core.h), compiled with g++, against torch autograd
   of the oracle: the Gaussian parameter layout (logstd after the mean head's bias), the mean, and every parameter
   gradient from the Gaussian tape as dW = sum_rows P^T Q / column sums, logstd from the rows' dL/dlogstd field."""
-import ctypes
 import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN, ROOT
+from conftest import GOLDEN
+from helpers import TRACE_THREADS, grads_from_tape, gxx_shim, ptr
 from oracle import loop, nets
-from test_deep_core_cpu import grads_from_tape
-
-# the reference trace was recorded with 8 intra-op threads (see tests/test_oracle_loop.py)
-TRACE_THREADS = 8
 
 
 def test_oracle_reproduces_reference_share_gaussian_trace():
@@ -56,14 +51,7 @@ def test_oracle_reproduces_reference_share_gaussian_trace():
 
 @pytest.fixture(scope="module")
 def shim(tmp_path_factory):
-    out = tmp_path_factory.mktemp("deepg") / "libdeepgshim.so"
-    subprocess.run(["g++", "-O2", "-shared", "-fPIC", "-I", os.path.join(ROOT, "openrl_b200", "csrc"),
-                    os.path.join(ROOT, "tests", "deep_core_gaussian_shim.cpp"), "-o", str(out)], check=True)
-    return ctypes.CDLL(str(out))
-
-
-def _ptr(a):
-    return a.ctypes.data_as(ctypes.c_void_p)
+    return gxx_shim(tmp_path_factory, "deepg", "deep_core_gaussian_shim.cpp")
 
 
 @pytest.mark.parametrize("n", [1, 6, 8])
@@ -102,7 +90,7 @@ def test_gaussian_core_matches_torch_autograd(shim, d, n):
     v_out, m_out = np.zeros(rows, np.float32), np.zeros((rows, n), np.float32)
     Xn, dvn = X.numpy().copy(), dv.numpy().reshape(-1).copy()
     dmn, dlsn = mean.grad.numpy().astype(np.float32).copy(), logstd.grad.numpy().astype(np.float32).copy()
-    shim.shim_gauss_rows(_ptr(P), d, n, act, rows, _ptr(Xn), _ptr(v_out), _ptr(m_out), _ptr(dvn), _ptr(dmn), _ptr(dlsn), _ptr(tape))
+    shim.shim_gauss_rows(ptr(P), d, n, act, rows, ptr(Xn), ptr(v_out), ptr(m_out), ptr(dvn), ptr(dmn), ptr(dlsn), ptr(tape))
     np.testing.assert_allclose(v_out, values.detach().numpy().reshape(-1), rtol=1e-5, atol=5e-6)
     np.testing.assert_allclose(m_out, mean.detach().numpy(), rtol=1e-5, atol=5e-6)
     t64 = tape.astype(np.float64)

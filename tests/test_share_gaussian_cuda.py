@@ -18,12 +18,10 @@ import numpy as np
 import pytest
 
 from conftest import GOLDEN
-from test_action_noise_cuda import philox_units
+from helpers import KEYS, make_agent, philox_units
+from openrl_b200.envs.vec_env import HostVecEnv
 
 pytestmark = pytest.mark.gpu
-
-KEYS = ["value_loss", "critic_grad_norm", "policy_loss", "dist_entropy", "actor_grad_norm", "ratio"]
-
 
 class _IdentityHost:
     """Host vec-env with the reference's duck type, backed by the oracle's IdentityEnvcontinuous restatement."""
@@ -76,26 +74,6 @@ class _BoxHost:
         return self.step_range(0, self.parallel_env_num, actions)
 
 
-def _agent(host_env, flags, golden=None):
-    import torch
-
-    from openrl_b200.configs.config import create_config_parser
-    from openrl_b200.envs.vec_env import HostVecEnv
-    from openrl_b200.modules.common import PPONet
-    from openrl_b200.runners.common import PPOAgent
-
-    cfg = create_config_parser().parse_args(flags)
-    cfg.quiet = True
-    env = HostVecEnv(host_env)
-    net = PPONet(env, cfg=cfg, device="cuda:0")
-    if golden is not None:
-        sd = net.module.models["model"].state_dict()
-        for k in sd:
-            if f"init/model.{k}" in golden and "value_normalizer" not in k:
-                sd[k].copy_(torch.from_numpy(golden[f"init/model.{k}"]))
-    return cfg, env, net, PPOAgent(net)
-
-
 @pytest.mark.parametrize("grouped", ["false", "true"])
 def test_share_gaussian_host_env_matches_reference_trace(cuda, grouped):
     """Parity mode draws the reference's noise on the host step by step, which keeps the rollout on the synchronous loop
@@ -105,7 +83,8 @@ def test_share_gaussian_host_env_matches_reference_trace(cuda, grouped):
     d = np.load(os.path.join(GOLDEN, "trace_share_gaussian.npz"), allow_pickle=True)
     iters, N = int(d["meta/iters"]), int(d["meta/env_num"])
     flags = str(d["meta/flags"]).split() + ["--parity_mode", "true", "--log_interval", "1", "--host_env_groups", grouped]
-    cfg, env, net, agent = _agent(_IdentityHost(N), flags, golden=d)
+    env = HostVecEnv(_IdentityHost(N))
+    cfg, net, agent = make_agent(env, flags, golden=d, start=False)
     model = net.module.models["model"]
     assert cfg.use_share_model and model.head_kind == 1 and model.n_actions == 1
     keys = [k for k, _ in model.named_parameters()]
@@ -145,7 +124,8 @@ def test_share_gaussian_host_loops_agree(cuda):
              "--log_interval", "1"]
     runs = []
     for grouped in ("false", "true"):
-        cfg, env, net, agent = _agent(_BoxHost(N), flags + ["--host_env_groups", grouped])   # PPONet re-seeds: same weights
+        env = HostVecEnv(_BoxHost(N))
+        cfg, net, agent = make_agent(env, flags + ["--host_env_groups", grouped], start=False)   # PPONet re-seeds: same weights
         assert env.supports_groups
         out = []
         for _ in range(2):
@@ -309,7 +289,8 @@ def test_share_gaussian_config5_shape_trains(cuda):
     from openrl_b200.utils.logger import Logger
 
     flags = ["--seed", "1", "--episode_length", "16", "--ppo_epoch", "2", "--use_share_model", "true", "--log_interval", "1"]
-    cfg, env, net, agent = _agent(_BoxHost(1024), flags)
+    env = HostVecEnv(_BoxHost(1024))
+    cfg, net, agent = make_agent(env, flags, start=False)
     logger = Logger(quiet=True)
     agent.train(total_time_steps=16 * 1024 * 2, logger=logger)
     logs = [h[1] for h in logger.history if "value_loss" in h[1]]

@@ -15,7 +15,7 @@ wrong references (tests/share_ref64.py MUTANTS), to show that the bars catch a s
 
 The reference is tests/share_ref64.py over the oracle (oracle/ppo.py `ppo_update` with one parameter dict for both
 roles), pinned to the reference's traces by tests/test_share_ref64_cpu.py.  Bars are those of
-tests/test_rnn_scale_cuda.py: per parameter block, the kernel's relative L2 error against float64 may be at most
+tests/scale_harness.py: per parameter block, the kernel's relative L2 error against float64 may be at most
 4x the float32 reference's error against float64, clamped to [FLOOR, 1e-3]; loss sums are relative to the weighted sum
 of their absolute terms and Adam's exp_avg to the terms it combines.  The parameters and Adam moments after the step are
 compared with the float64 reference's, and also with the float64 step taken from the kernel's own gradient (the
@@ -42,16 +42,13 @@ import numpy as np
 import pytest
 import torch
 
-import rnn_ref64
+import scale_harness as h
 import share_ref64 as ref
-from test_ppo_ffma_scale_cuda import _flag_cfg, _flags, _gae_stats, _redraw
-from test_ppo_flags_cuda import CASES
-from test_rnn_scale_cuda import ATOL, KINK, Checker, _mb_stats, _rel, no_tf32  # noqa: F401  (no_tf32: pytest fixture)
+from scale_harness import ATOL, BASE, CASES, Checker, no_tf32  # noqa: F401  (no_tf32: pytest fixture)
 
 pytestmark = pytest.mark.gpu
 
 FLOOR = 3e-6
-ACT_KINK = 1e-4   # synthetic fc1 pre-activations (obs_prep and common) keep at least this distance from 0
 BLOCK = ref.TAPE_ROW_BLOCK
 SEED = 11
 C2_FLAGS = ["--seed", "0", "--episode_length", "128", "--ppo_epoch", "4", "--num_mini_batch", "1", "--log_interval", "1000000",
@@ -60,23 +57,8 @@ C5_FLAGS = ["--seed", "0", "--episode_length", "128", "--ppo_epoch", "4", "--num
             "--host_env_groups", "false", "--use_share_model", "true"]
 
 
-def _lib():
-    from openrl_b200 import lib
-    return lib, lib.load()
-
-
-def _moment_scales(r64, state, cfg):
-    """Per element, the magnitude of the terms an Adam step combines into exp_avg: beta1 |m| + (1 - beta1) |g|, g the
-    clipped gradient plus weight decay (see test_ppo_ffma_scale_cuda.py)."""
-    g = r64["grad"].abs()
-    if cfg.use_max_grad_norm:
-        g = g * min(1.0, cfg.max_grad_norm / (float(r64["norms"][0]) + 1e-6))
-    p, m = (state[key].to(g.device, torch.float64).abs() for key in ("p", "m"))
-    return 0.9 * m + 0.1 * (g + cfg.weight_decay * p)
-
-
 def _compare(case, dims, head, k, r64, r32, state, cfg, check_vn=True):
-    chk = Checker(case, floor=FLOOR)
+    chk = Checker(case, FLOOR)
     bl = ref.blocks(*dims, head)
     for name, s in bl.items():
         chk(f"grad {name}", k["grad"][s], r64["grad"][s], r32["grad"][s])
@@ -85,7 +67,7 @@ def _compare(case, dims, head, k, r64, r32, state, cfg, check_vn=True):
     for j, name in ((0, "actor grad norm"), (1, "critic grad norm")):
         chk(f"train_info {name}", k["norms"][j:j + 1], r64["norms"][j:j + 1], r32["norms"][j:j + 1])
     chk("train_info ratio mean", k["info"][5:6], r64["ratio_mean"].reshape(1), r32["ratio_mean"].reshape(1))
-    mscale = _moment_scales(r64, state, cfg)
+    mscale = h.moment_scale(cfg, r64["grad"], r64["norms"][0], state["p"], state["m"])
     for key, label in (("p", "param"), ("m", "exp_avg"), ("v", "exp_avg_sq")):
         for name, s in bl.items():
             chk(f"{label} {name}", k[key][s], r64[key][s], r32[key][s], scale=mscale[s].norm() if key == "m" else None)
@@ -106,10 +88,10 @@ def _check_mutant(case, mutant, k, r64, r32, bad, dims, head):
     violate its bar, and pass it against the correct reference."""
     what = ref.MUTANTS[mutant][1]
     got, want, wrong, w32 = (ref.target(x, what, dims, head) for x in (k, r64, bad, r32))
-    good = Checker(case, floor=FLOOR)
+    good = Checker(case, FLOOR)
     good(what, got, want, w32)
     good.done()
-    e_bad, bar = _rel(got, wrong), good.bar(_rel(w32, want))
+    e_bad, bar = h.rel(got, wrong), good.bar(h.rel(w32, want))
     print(f"  {case}: kernel against the mutant {e_bad:.2e}, bar {bar:.2e} ({e_bad / bar:.1f}x the bar)")
     assert e_bad > bar, f"{mutant}: the mistake ({ref.MUTANTS[mutant][0]}) passed the bar of {what}"
 
@@ -187,13 +169,12 @@ def c2():
 def c5s():
     """One rollout of the C5-shaped host env (obs 17, Box(6), 1024 envs) with use_share_model, and its returns."""
     from openrl_b200.envs.vec_env import HostVecEnv
-    from test_gaussian_cuda import _SyntheticHost
-    from test_rnn_host_cuda import _agent
+    from helpers import SyntheticHost, make_agent
 
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     torch.manual_seed(0)
-    cfg, net, agent = _agent(HostVecEnv(_SyntheticHost(1024)), C5_FLAGS)
+    cfg, net, agent = make_agent(HostVecEnv(SyntheticHost(1024)), C5_FLAGS)
     drv = agent.driver
     drv.actor_rollout()
     drv.compute_returns()
@@ -203,18 +184,6 @@ def c5s():
     yield c
     c.tr.share_ws = None
     torch.cuda.empty_cache()
-
-
-def _snapshot(c):
-    return {k: v.clone() for k, v in c.live.items()}, c.m.adam_steps.clone()
-
-
-def _restore(c, snap):
-    saved, steps = snap
-    for k, v in c.live.items():
-        v.copy_(saved[k])
-    c.m.adam_steps.copy_(steps)
-    c.tr.train_info.zero_()
 
 
 def _state(c):
@@ -302,7 +271,7 @@ def test_c2_rollout_teacher_forced(c2):
 def test_c2_four_epochs_contiguous(c2, no_tf32):
     """C2's four updates (indices == NULL, 524 288 rows, 512 tape row blocks, the GAE moments as minibatch moments),
     each teacher-forced from the device's own state.  Epoch 1 has every ratio at 1 up to rounding; epochs 2-4 do not."""
-    snap = _snapshot(c2)
+    snap = h.snapshot(c2)
     rows = torch.arange(c2.rows, device="cuda")
     try:
         for epoch in range(4):
@@ -314,24 +283,24 @@ def test_c2_four_epochs_contiguous(c2, no_tf32):
             assert (spread > 1e-4) if epoch else (spread < 1e-4), spread
             del r64, r32
     finally:
-        _restore(c2, snap)
+        h.restore(c2, snap)
     _peak("c2 four epochs")
 
 
 def test_c2_shuffled_partial_last_block(c2, no_tf32):
     """A shuffled index list of 131 405 rows (128 full tape row blocks and a partial one of 333 rows),
     orl_minibatch_stats."""
-    snap = _snapshot(c2)
+    snap = h.snapshot(c2)
     g = torch.Generator(device="cuda").manual_seed(4)
     idx = torch.randperm(c2.rows, device="cuda", generator=g)[:c2.rows // 4 + 333].contiguous()
     assert idx.numel() % BLOCK == 333
     try:
         state = _state(c2)
-        k = _kernel_update(c2, idx, _mb_stats(idx, c2.b.returns, c2.b.active_masks), idx.numel())
+        k = _kernel_update(c2, idx, h.mb_stats(idx, c2.b.returns, c2.b.active_masks), idx.numel())
         r64, r32 = _refs(c2, k, state, idx)
         _compare("c2-shuffled-131405rows(partial last block)", c2.dims, "categorical", k, r64, r32, state, c2.cfg)
     finally:
-        _restore(c2, snap)
+        h.restore(c2, snap)
 
 
 C2_MUTANTS = [m for m, e in ref.MUTANTS.items() if e[3] == "categorical"]
@@ -343,7 +312,7 @@ def test_c2_mutants_are_detected(c2, no_tf32, mutant):
     adam-with-critic-lr the kernel runs with critic_lr in the device's second learning-rate slot, so a shared Adam that
     read that slot would fail its bar against the correct reference."""
     _, what, opts, _ = ref.MUTANTS[mutant]
-    snap = _snapshot(c2)
+    snap = h.snapshot(c2)
     saved = {k: getattr(c2.tr.cfg, k) for k in opts}
     rows = torch.arange(c2.rows, device="cuda")
     try:
@@ -354,7 +323,7 @@ def test_c2_mutants_are_detected(c2, no_tf32, mutant):
     finally:
         for key, val in saved.items():
             setattr(c2.tr.cfg, key, val)
-        _restore(c2, snap)
+        h.restore(c2, snap)
     r64, r32, bad = _refs(c2, k, state, rows, opts, mutant)
     if mutant == "critic-norm-unclipped":
         assert float(r64["norms"][0]) > opts["max_grad_norm"]
@@ -372,7 +341,7 @@ def test_c5_share_log_probs_and_values(c5s):
 def test_c5_share_two_epochs_and_shuffled_quarter(c5s, no_tf32):
     """Two teacher-forced updates on the contiguous path (131 072 rows, 128 row blocks of the 1112-float Gaussian
     tape), then a shuffled quarter."""
-    snap = _snapshot(c5s)
+    snap = h.snapshot(c5s)
     rows = torch.arange(c5s.rows, device="cuda")
     g = torch.Generator(device="cuda").manual_seed(5)
     idx = torch.randperm(c5s.rows, device="cuda", generator=g)[:c5s.rows // 4].contiguous()
@@ -383,11 +352,11 @@ def test_c5_share_two_epochs_and_shuffled_quarter(c5s, no_tf32):
             r64, r32 = _refs(c5s, k, state, rows)
             _compare(f"c5share-epoch{epoch + 1}-contiguous-131072rows", c5s.dims, "gaussian", k, r64, r32, state, c5s.cfg)
         state = _state(c5s)
-        k = _kernel_update(c5s, idx, _mb_stats(idx, c5s.b.returns, c5s.b.active_masks), idx.numel())
+        k = _kernel_update(c5s, idx, h.mb_stats(idx, c5s.b.returns, c5s.b.active_masks), idx.numel())
         r64, r32 = _refs(c5s, k, state, idx)
         _compare("c5share-shuffled-32768rows", c5s.dims, "gaussian", k, r64, r32, state, c5s.cfg)
     finally:
-        _restore(c5s, snap)
+        h.restore(c5s, snap)
     _peak("c5 share")
 
 
@@ -396,7 +365,7 @@ def test_c5_share_entropy_mutant_is_detected(c5s, no_tf32):
 
     mutant = "entropy-weight-1/rows"
     _, what, opts, _ = ref.MUTANTS[mutant]
-    snap, flags = _snapshot(c5s), c5s.tr.flags
+    snap, flags = h.snapshot(c5s), c5s.tr.flags
     rows = torch.arange(c5s.rows, device="cuda")
     try:
         c5s.tr.flags &= ~lib.PPO_POLICY_ACTIVE_MASKS
@@ -404,7 +373,7 @@ def test_c5_share_entropy_mutant_is_detected(c5s, no_tf32):
         k = _kernel_update(c5s, None, c5s.b.gae_stats[5:8], c5s.rows)
     finally:
         c5s.tr.flags = flags
-        _restore(c5s, snap)
+        h.restore(c5s, snap)
     r64, r32, bad = _refs(c5s, k, state, rows, opts, mutant)
     _check_mutant(f"c5share-{mutant}", mutant, k, r64, r32, bad, c5s.dims, "gaussian")
 
@@ -467,28 +436,6 @@ def test_gridworld_share_rollout_at_4096_envs():
 
 # ---------------------------------------------------------------- synthetic buffers -----------------------------------
 
-BASE = dict(use_huber_loss=True, use_clipped_value_loss=True, use_value_active_masks=True, use_policy_active_masks=True,
-            use_valuenorm=True, use_adv_normalize=False, use_max_grad_norm=True, dual_clip_ppo=False, a2c=False, activation_id=1,
-            clip_param=0.2, entropy_coef=0.01, value_loss_coef=0.5, huber_delta=1.0, max_grad_norm=1e3, dual_clip_coeff=3.0,
-            lr=7e-4, critic_lr=5e-4, opti_eps=1e-5, weight_decay=0.0, vn_beta=0.99999)
-
-
-def _random_net(g, d, n, head):
-    parts = []
-    for name, shp in ref.param_shapes(d, n, head):
-        x = torch.randn(shp, generator=g, device="cuda")
-        if name.endswith("logstd._bias"):   # std ~ 0.74
-            x = 0.2 * x - 0.3
-        elif len(shp) == 2:
-            x *= (0.3 if name.startswith(("act.", "v_out")) else 1.0) / shp[1] ** 0.5
-        elif name.endswith(("fc1.2.weight", "fc3.1.weight")):   # LayerNorm gains
-            x = 1.0 + 0.2 * x
-        else:
-            x *= 0.1
-        parts.append(x.reshape(-1))
-    return torch.cat(parts)
-
-
 def _synthetic(cfg, dims, head, total, rows_idx, seed, masked=False, inactive=0.1):
     """A buffer of `total` random rows and a net with random weights, Adam moments mid-run, a fraction `inactive` of
     active masks at zero and, with `masked`, a Categorical action mask with ~30 % of the actions illegal (never the
@@ -514,21 +461,15 @@ def _synthetic(cfg, dims, head, total, rows_idx, seed, masked=False, inactive=0.
             am = (u(total, n) >= 0.3).float()
             am[torch.arange(total, device="cuda"), act] = 1.0
             buf["action_masks"] = am
-    state = dict(p=_random_net(g, d, n, head), vn=torch.tensor([0.3, 0.5, 0.8], device="cuda"), step=3)
+    state = dict(p=h.random_net(g, ref.param_shapes(d, n, head)), vn=torch.tensor([0.3, 0.5, 0.8], device="cuda"), step=3)
     state["m"] = 1e-3 * r(state["p"].numel())
     state["v"] = 1e-6 * u(state["p"].numel()) + 1e-8
 
     ncfg = types.SimpleNamespace(layer_N=1, activation_id=cfg.activation_id, use_recurrent_policy=False, use_policy_active_masks=True)
     p = ref.unflatten(state["p"].double(), d, n, head)
-    for _ in range(50):
-        x = buf["obs"][rows_idx].double()
-        z1 = x @ p["obs_prep.mlp.fc1.0.weight"].t() + p["obs_prep.mlp.fc1.0.bias"]
-        z5 = nets.mlp_base(p, "obs_prep", x, 1, cfg.activation_id) @ p["common.fc1.0.weight"].t() + p["common.fc1.0.bias"]
-        bad = (z1.abs() < ACT_KINK).any(-1) | (z5.abs() < ACT_KINK).any(-1)
-        if not bool(bad.any()):
-            break
-        buf["obs"][rows_idx[bad]] = r(int(bad.sum()), d)
-    assert not bool(bad.any()), "observations kept landing on an activation kink"
+    h.redraw_off_act_kink(g, buf["obs"], rows_idx, lambda x: [
+        x @ p["obs_prep.mlp.fc1.0.weight"].t() + p["obs_prep.mlp.fc1.0.bias"],
+        nets.mlp_base(p, "obs_prep", x, 1, cfg.activation_id) @ p["common.fc1.0.weight"].t() + p["common.fc1.0.bias"]])
     x = lambda k: buf[k].double()[rows_idx]   # noqa: E731
     with torch.no_grad():
         if gauss:
@@ -536,51 +477,9 @@ def _synthetic(cfg, dims, head, total, rows_idx, seed, masked=False, inactive=0.
         else:
             logp, _ = nets.policy_eval(p, ncfg, x("obs"), x("actions"), x("action_masks") if masked else None)
         v, _ = nets.critic_forward(p, ncfg, x("obs"))
-    kinks = torch.tensor([1 - cfg.clip_param, 1 + cfg.clip_param, cfg.dual_clip_coeff], device="cuda", dtype=torch.float64)
     many = rows_idx.numel() >= 1000   # enough rows to see both sides of every branch
-
-    def draw_ratio(shape):
-        near = torch.exp(0.15 * torch.randn(shape, generator=g, device="cuda", dtype=torch.float64))
-        far = 2.5 + 1.5 * torch.rand(shape, generator=g, device="cuda", dtype=torch.float64)
-        return torch.where(torch.rand(shape, generator=g, device="cuda", dtype=torch.float64) < 0.1, far, near)
-    ratio = draw_ratio(logp.shape)
-    for _ in range(50):
-        bad = ((ratio[..., None] - kinks).abs() < KINK).any(-1)
-        if not bool(bad.any()):
-            break
-        ratio = _redraw(bad, draw_ratio, ratio)
-    buf["action_log_probs"][rows_idx] = (logp - ratio.log()).float()
-    got = (logp - buf["action_log_probs"][rows_idx].double()).exp()
-    assert bool(((got[..., None] - kinks).abs() >= KINK / 2).all())
-    assert not many or (bool((got < 1 - cfg.clip_param).any()) and bool((got > 1 + cfg.clip_param).any()))
-
-    draw_delta = lambda shape: 0.4 * torch.randn(shape, generator=g, device="cuda", dtype=torch.float64)   # noqa: E731
-    delta = draw_delta(v.shape)
-    for _ in range(50):
-        bad = (delta.abs() - cfg.clip_param).abs() < KINK
-        if not bool(bad.any()):
-            break
-        delta = _redraw(bad, draw_delta, delta)
-    buf["value_preds"][rows_idx] = (v - delta).float()
-    vp = buf["value_preds"][rows_idx].double()
-    assert not many or (bool((v - vp > cfg.clip_param).any()) and bool((v - vp < -cfg.clip_param).any()))
-    draw_ret = lambda shape: 3 * torch.randn(shape, generator=g, device="cuda", dtype=torch.float64) + 2.0   # noqa: E731
-    ret = draw_ret(v.shape)
-    for _ in range(100):
-        r32 = ret.float().double()
-        target = r32
-        if cfg.use_valuenorm:
-            target = rnn_ref64.vn_normalize(rnn_ref64.vn_update(state["vn"].double(), r32, cfg.vn_beta), r32)
-        clipped = vp + (v - vp).clamp(-cfg.clip_param, cfg.clip_param)
-        e_o, e_c = (target - v).abs(), (target - clipped).abs()
-        outside = (v - vp).abs() > cfg.clip_param
-        bad = (((e_o - cfg.huber_delta).abs() < KINK) | ((e_c - cfg.huber_delta).abs() < KINK)
-               | (outside & ((e_o - e_c).abs() < KINK)))
-        if not bool(bad.any()):
-            break
-        ret = _redraw(bad, draw_ret, ret)
-    assert not bool(bad.any()), "returns kept landing on a kink"
-    buf["returns"][rows_idx] = ret.float()
+    h.draw_kink_free(g, cfg, state["vn"], logp, v, buf["action_log_probs"], rows_idx, buf["value_preds"], buf["returns"],
+                     rows_idx, both_clip_sides=many)
     return buf, state
 
 
@@ -588,18 +487,12 @@ def _run_synthetic(case, cfg, dims, head, batch_rows, contiguous_from=None, tota
                    mutant=None):
     """OrlPpoArgs built by hand for a synthetic buffer; orl_share_fwdbwd + orl_share_apply against both reference runs
     (and, with `mutant`, the check that the mistake fails its bar)."""
-    lib, L = _lib()
+    lb, L = h.lib()
     d, n = dims
     gauss = head == "gaussian"
-    hk = lib.HEAD_GAUSSIAN if gauss else lib.HEAD_CATEGORICAL
+    hk = lb.HEAD_GAUSSIAN if gauss else lb.HEAD_CATEGORICAL
     total = total or batch_rows + 301
-    g = torch.Generator(device="cuda").manual_seed(seed + 1)
-    if contiguous_from is None:
-        idx = torch.randperm(total, device="cuda", generator=g)[:batch_rows].contiguous()
-        rows_idx = idx
-    else:
-        idx = None
-        rows_idx = torch.arange(contiguous_from, contiguous_from + batch_rows, device="cuda")
+    idx, rows_idx = h.minibatch(total, batch_rows, contiguous_from, seed)
     buf, state = _synthetic(cfg, dims, head, total, rows_idx, seed, masked, inactive)
     count = int(L.orl_share_param_count_head(d, n, hk))
     assert state["p"].numel() == count
@@ -609,32 +502,14 @@ def _run_synthetic(case, cfg, dims, head, batch_rows, contiguous_from=None, tota
     dev = {k: state[k].clone() for k in ("p", "m", "v", "vn")}
     steps = torch.tensor([state["step"], 0], dtype=torch.int32, device="cuda")
     lrs = torch.tensor([cfg.lr, cfg.critic_lr], dtype=torch.float32, device="cuda")
-    gae_stats = _gae_stats(buf)
-    mb_stats = _mb_stats(rows_idx.contiguous(), buf["returns"], buf["active_masks"])
+    stats = h.gae_stats(buf), h.mb_stats(rows_idx.contiguous(), buf["returns"], buf["active_masks"])
     train_info = torch.zeros(6, device="cuda")
-    a = lib.OrlPpoArgs()
-    a.obs_dim, a.critic_obs_dim, a.n_actions, a.activation_id = d, d, n, cfg.activation_id
-    a.flags, a.grid_per_net, a.head_kind = _flags(cfg), 1, hk
-    a.batch_rows, a.row_begin, a.total_rows = batch_rows, contiguous_from or 0, total
-    a.indices = None if idx is None else lib.ptr(idx)
-    a.policy_obs = a.critic_obs = lib.ptr(buf["obs"])
-    for k, key in (("actions", "actions"), ("old_log_probs", "action_log_probs"), ("advantages", "advantages"),
-                   ("value_preds", "value_preds"), ("returns", "returns"), ("active_masks", "active_masks")):
-        setattr(a, k, lib.ptr(buf[key]))
-    a.action_masks = lib.ptr(buf["action_masks"]) if masked else None
-    a.gae_stats, a.mb_stats, a.vn_state = lib.ptr(gae_stats), lib.ptr(mb_stats), lib.ptr(dev["vn"])
-    a.policy_params = a.critic_params = lib.ptr(dev["p"])
-    a.policy_adam_m = a.critic_adam_m = lib.ptr(dev["m"])
-    a.policy_adam_v = a.critic_adam_v = lib.ptr(dev["v"])
-    a.adam_steps, a.lrs, a.train_info = lib.ptr(steps), lib.ptr(lrs), lib.ptr(train_info)
-    a.clip_param, a.entropy_coef, a.value_loss_coef = cfg.clip_param, cfg.entropy_coef, cfg.value_loss_coef
-    a.huber_delta, a.max_grad_norm, a.dual_clip_coeff = cfg.huber_delta, cfg.max_grad_norm, cfg.dual_clip_coeff
-    a.adam_beta1, a.adam_beta2, a.adam_eps, a.weight_decay = 0.9, 0.999, cfg.opti_eps, cfg.weight_decay
-    a.vn_beta, a.norm_rows = cfg.vn_beta, 0
-    a.partials, a.folded, a.grads = lib.ptr(ws), lib.ptr(folded), lib.ptr(grads)
-    s = lib.current_stream()
-    lib.check(L.orl_share_fwdbwd(a, s), "orl_share_fwdbwd")
-    lib.check(L.orl_share_apply(a, s), "orl_share_apply")
+    one_net = dict(pol=dev["p"], cri=dev["p"], pol_m=dev["m"], cri_m=dev["m"], pol_v=dev["v"], cri_v=dev["v"], vn=dev["vn"])
+    a = h.ppo_args(cfg, (d, n, d), hk, h.ppo_flags(cfg), 1, dict(buf, policy_obs=buf["obs"], critic_obs=buf["obs"]), batch_rows,
+                   total, idx, contiguous_from or 0, stats, one_net, steps, lrs, train_info, ws, folded, grads)
+    s = lb.current_stream()
+    lb.check(L.orl_share_fwdbwd(a, s), "orl_share_fwdbwd")
+    lb.check(L.orl_share_apply(a, s), "orl_share_apply")
     torch.cuda.synchronize()
     del ws
     k = dict(grad=grads[:count], losses=folded[:4], info=train_info, norms=train_info[[4, 1]], step=int(steps[0]), **dev)
@@ -703,7 +578,7 @@ def test_update_flag_sweep(no_tf32, flags, head):
     Huber off, value clip off, ValueNorm off, advantage normalisation, no gradient clip, weight decay with lr != critic_lr
     (the shared Adam steps with lr), the activations, other coefficients, a gradient clip that acts (both logged norms),
     dual clip and A2C; the GAE-only options run the default update."""
-    cfg = _flag_cfg(flags)
+    cfg = h.flag_cfg(flags)
     dims = (17, 6) if head == "gaussian" else (6, 5)
     _run_synthetic(f"flags-{'-'.join(flags) or 'default'}-{head}", cfg, dims, head, 3 * BLOCK + 37, seed=77,
                    masked=head == "categorical")

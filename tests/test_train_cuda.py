@@ -17,11 +17,11 @@ def test_train_matches_reference_trace(cuda, tag):
     import torch
 
     from openrl_b200.utils.logger import Logger
-    from test_rollout_cuda import _product
+    from helpers import product
 
     d = np.load(os.path.join(GOLDEN, f"trace_{tag}.npz"), allow_pickle=True)
     iters, N = int(d["meta/iters"]), int(d["meta/env_num"])
-    cfg, env, net, agent = _product("CartPole-v1", N, str(d["meta/flags"]).split(), golden=d)
+    cfg, env, net, agent = product("CartPole-v1", N, str(d["meta/flags"]).split(), golden=d)
     logger = Logger(quiet=True)
     agent.train(total_time_steps=cfg.episode_length * N * iters, logger=logger)
     train_logs = [h[1] for h in logger.history if "value_loss" in h[1]]
@@ -104,7 +104,7 @@ def test_gridworld_train_matches_reference_trace(cuda):
     import torch
 
     from openrl_b200.utils.logger import Logger
-    from test_rollout_cuda import _product
+    from helpers import product
 
     d = np.load(os.path.join(GOLDEN, "trace_gridworld.npz"), allow_pickle=True)
     iters, N = int(d["meta/iters"]), int(d["meta/env_num"])
@@ -122,7 +122,7 @@ def test_gridworld_train_matches_reference_trace(cuda):
                 if masks[t, e, 0, 0] == 0.0:
                     table[e, count[e]] = obs[t, e, 0, :2]
                     count[e] += 1
-    cfg, env, net, agent = _product("GridWorldEnv", N, str(d["meta/flags"]).split(), golden=d, reset_table=table)
+    cfg, env, net, agent = product("GridWorldEnv", N, str(d["meta/flags"]).split(), golden=d, reset_table=table)
     logger = Logger(quiet=True)
     agent.train(total_time_steps=cfg.episode_length * N * iters, logger=logger)
     train_logs = [h[1] for h in logger.history if "value_loss" in h[1]]
@@ -168,7 +168,7 @@ def test_recurrent_cartpole_matches_reference_trace(cuda):
     data_chunk_length 4, two minibatches per epoch): episodes end INSIDE chunks here, so the masked hidden-state
     carry and its backward are exercised (the simple_spread trace only has episode ends at rollout boundaries).
     Added at the end of round 1 after the GPU budget was spent: first run is the driver's."""
-    from test_gru_cuda import check_recurrent_trace
+    from helpers import check_recurrent_trace
 
     check_recurrent_trace("cartpole_gru", "CartPole-v1")
 
@@ -205,12 +205,12 @@ def test_train_matches_reference_flag_variants(cuda, tag):
     option branch (oracle/gen_golden.py FLAG_VARIANTS): bit-exact actions, the six scalars within 1e-4."""
     from openrl_b200.algorithms import A2CAlgorithm, PPOAlgorithm
     from openrl_b200.utils.logger import Logger
-    from test_rollout_cuda import _product
+    from helpers import product
 
     d = np.load(os.path.join(GOLDEN, f"trace_flag_{tag}.npz"), allow_pickle=True)
     iters, N = int(d["meta/iters"]), int(d["meta/env_num"])
     a2c = str(d["meta/algo"]) == "a2c"
-    cfg, env, net, agent = _product("CartPole-v1", N, str(d["meta/flags"]).split(), golden=d)
+    cfg, env, net, agent = product("CartPole-v1", N, str(d["meta/flags"]).split(), golden=d)
     logger = Logger(quiet=True)
     agent.train(total_time_steps=cfg.episode_length * N * iters, logger=logger, train_algo_class=A2CAlgorithm if a2c else PPOAlgorithm)
     train_logs = [h[1] for h in logger.history if "value_loss" in h[1]]
@@ -316,11 +316,11 @@ def test_parity_mode_at_4096_envs_matches_oracle(cuda):
     8-env reference traces cannot reach.)"""
     from openrl_b200.utils.logger import Logger
     from oracle import loop as oloop
-    from test_rollout_cuda import _product
+    from helpers import product
 
     N, T, iters = 4096, 8, 2
     flags = ["--seed", "0", "--episode_length", str(T), "--ppo_epoch", "2", "--num_mini_batch", "2"]
-    cfg, env, net, agent = _product("CartPole-v1", N, flags)
+    cfg, env, net, agent = product("CartPole-v1", N, flags)
     tr = oloop.Trainer(oloop.cfg_from_flags(" ".join(flags)), "CartPole-v1", N)
     # same initial weights (the oracle consumes the generator like the reference; pin them anyway)
     import torch
