@@ -141,7 +141,8 @@ typedef struct OrlRolloutArgs {
     int32_t t_begin, t_end; /* steps to run, 0 <= t_begin < t_end <= T */
     int32_t obs_dim;        /* d, policy observation width (<= 64) */
     int32_t critic_obs_dim; /* 0: critic obs == policy obs (critic_obs may be NULL) */
-    int32_t n_actions;      /* n <= 8, Discrete(n) */
+    int32_t n_actions;      /* n: Discrete(n) 1..64 with ORL_ENV_NONE (host-stepped envs), 1..8 otherwise and for
+                               DiagGaussian heads; ORL_ERR_BAD_ARG outside */
     int32_t activation_id;  /* cfg.activation_id: 0 tanh, 1 relu, 2 leaky_relu, 3 elu */
     int32_t deterministic;
     int32_t env_table_len;
@@ -194,7 +195,8 @@ int orl_critic_values(const float* critic_params, int obs_dim, int activation_id
  * running env).  Pointers address the given slot / row range (rows of a group are contiguous).
  * action_masks_next (nullable): when the envs reported legal-move masks (`info["action_masks"]`, prepare_action_masks,
  * envs/vec_env/utils/util.py:54-88) for this step, the staged block carries them after the dones, [... | action masks
- * (B*n_actions)], and they are written to slot t+1 of action_masks (replay_data.py:282-283); NULL writes nothing there,
+ * (B*n_actions), n_actions in 1..64], and they are written to slot t+1 of action_masks (replay_data.py:282-283); NULL
+ * writes nothing there,
  * so the slot keeps what it held, as in the reference.
  * critic_obs_next (nullable): for an env whose observation space is Dict {"policy", "critic"} (a separate critic
  * observation, as the reference's MAPPO envs give it: get_critic_obs, buffers/utils/util.py:22-55) the block carries the
@@ -209,7 +211,8 @@ int orl_host_insert(const float* staged, int n_envs, int n_agents, int obs_dim, 
  * Replaces PolicyNetwork.eval_actions (policy_network.py:164-203) -> ACTLayer.evaluate_actions (act.py:130-172), the
  * policy half of PPOModule.evaluate_actions (ppo_module.py:147-193), outside the fused update: obs (rows, d), actions
  * (rows) [Categorical: index as float32] or (rows, n) [DiagGaussian] -> log_probs and entropy with the shape of
- * `actions` (per row / per dimension; the caller takes the active-mask mean, act.py:160-168). */
+ * `actions` (per row / per dimension; the caller takes the active-mask mean, act.py:160-168).  n_actions: 1..64 for
+ * Categorical heads, 1..8 for DiagGaussian heads (ORL_ERR_BAD_ARG otherwise). */
 int orl_policy_eval(const float* policy_params, int obs_dim, int n_actions, int activation_id, int head_kind,
                     const float* obs, const float* actions, const float* action_masks, float* log_probs,
                     float* entropy, long long rows, void* stream);
@@ -255,7 +258,8 @@ int orl_policy_eval(const float* policy_params, int obs_dim, int n_actions, int 
 typedef struct OrlPpoArgs {
     int32_t obs_dim;         /* d  policy obs width  (<= 64) */
     int32_t critic_obs_dim;  /* dc critic obs width  (<= 64) */
-    int32_t n_actions;       /* n <= 8 */
+    int32_t n_actions;       /* n: 1..64 for Categorical heads, 1..8 for DiagGaussian heads and with ORL_PPO_TENSORCORE
+                                (ORL_ERR_BAD_ARG otherwise) */
     int32_t activation_id;
     int32_t flags;           /* ORL_PPO_* */
     int32_t grid_per_net;    /* CTAs per net in orl_ppo_fwdbwd (partials has 2*grid_per_net rows) */

@@ -34,9 +34,10 @@ class PPOAlgorithm:
         # naive_recurrent_generator (replay_data.py:806-946) == chunks of the WHOLE trajectory: chunk length = episode_length,
         # chunk c = buffer row c, one randperm over rows per epoch (ppo.py:363-381: taken only when use_recurrent_policy is off)
         self.naive = bool(getattr(cfg, "use_naive_recurrent_policy", False)) and not cfg.use_recurrent_policy
-        # tensor-core update (wgmma, split fp16, fp32-class accuracy): Categorical heads, obs widths <= 8
+        # tensor-core update (wgmma, split fp16, fp32-class accuracy): Categorical heads of up to 8 actions, obs widths <= 8
         self.use_tensor_cores = (bool(getattr(cfg, "use_tensor_cores", True)) and bool(getattr(cfg, "use_tf32", True))
-                                 and max(self.d, self.dc) <= 8 and self.head_kind == lib.HEAD_CATEGORICAL and not self.recurrent)
+                                 and max(self.d, self.dc) <= 8 and self.n <= 8 and self.head_kind == lib.HEAD_CATEGORICAL
+                                 and not self.recurrent)
         sm = torch.cuda.get_device_properties(self.device).multi_processor_count
         # CTAs per net: #SMs for the tensor-core kernel (one 256-thread CTA per SM, so policy and critic run as two
         # waves), #SMs / 2 for the FFMA kernel (its policy and critic CTAs share the SMs in one wave)

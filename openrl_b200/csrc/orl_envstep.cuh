@@ -185,6 +185,9 @@ __device__ __forceinline__ uint4 action_philox(uint64_t seed, uint64_t step, uin
 
 // Exp(1) noise q[0..n) of (step, row): the reference-order table exp_noise[grow * n + j] when one is given (parity mode),
 // else -log U of the 8 draws of Philox lanes `lane`, `lane + 1`.
+// Lanes of one (step, row): 0, 1 the noise of actions 0..7 (wide_action_noise4 keeps them for those actions); 2..5 the
+// DiagGaussian normals (gaussian_act), and in the self-play rollout 2, 3 the opponent's noise and 4 its pick; 8..21 the
+// noise of actions 8..63 of a wide head, action j from draw (j - 8) % 4 of lane 8 + (j - 8) / 4.
 __device__ __forceinline__ void action_noise(const float* exp_noise, size_t grow, int n, uint64_t seed, uint64_t step,
                                              uint32_t row, float (&q)[MAX_OUT], uint32_t lane = 0u) {
     if (exp_noise) {
@@ -222,6 +225,48 @@ __device__ __forceinline__ int sample_action(float (&logit)[MAX_OUT], int n, con
         act = best;
     }
     lp = log_prob_of(nl, n, act);
+    return act;
+}
+
+// Exp(1) noise q[0..4) of actions j0..j0+3 (j0 % 4 == 0) of a wide head's row: the table entries j < n in parity mode,
+// else -log U of Philox lane j0 / 4 (actions 0..7, the draws action_noise gives them) or 8 + (j0 - 8) / 4.
+__device__ __forceinline__ void wide_action_noise4(const float* exp_noise, size_t grow, int n, uint64_t seed, uint64_t step,
+                                                   uint32_t row, int j0, float (&q)[4]) {
+    if (exp_noise) {
+#pragma unroll
+        for (int c = 0; c < 4; ++c) q[c] = (j0 + c < n) ? exp_noise[grow * n + j0 + c] : 1.f;
+    } else {
+        const uint4 r = action_philox(seed, step, row, j0 < 8 ? (uint32_t)(j0 / 4) : 8u + (uint32_t)((j0 - 8) / 4));
+        q[0] = -logf(u32_to_unit_open(r.x)); q[1] = -logf(u32_to_unit_open(r.y));
+        q[2] = -logf(u32_to_unit_open(r.z)); q[3] = -logf(u32_to_unit_open(r.w));
+    }
+}
+
+// sample_action of a wide head's row x[0..n) in shared memory (masked in place): the first-max mode when deterministic,
+// else argmax(probs / q) with the first index winning ties, q from noise4(j0, q[4]) four actions at a time.
+template <typename Noise4>
+__device__ __forceinline__ int wide_sample_action(float* x, int n, const float* mask_row, bool deterministic, Noise4&& noise4,
+                                                  float& lp) {
+    const WideSoftmax sm = wide_log_softmax(x, n, mask_row);
+    int act = 0;
+    float bv = sm.pr(x, 0);
+    if (deterministic) {
+        for (int j = 1; j < n; ++j) { const float v = sm.pr(x, j); if (v > bv) { bv = v; act = j; } }
+    } else {
+        for (int j0 = 0; j0 < n; j0 += 4) {
+            float q[4];
+            noise4(j0, q);
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                const int j = j0 + c;
+                if (j < n) {
+                    const float v = sm.pr(x, j) / q[c];
+                    if (j == 0 || v > bv) { bv = v; act = j; }
+                }
+            }
+        }
+    }
+    lp = wide_log_prob_of(sm, x, n, act);
     return act;
 }
 

@@ -183,6 +183,61 @@ __device__ __forceinline__ CatRow categorical_row(const Args& a, float (&logit)[
     return CatRow{pg.loss, ent, pg.ratio};
 }
 
+// ---- the wide Categorical head (NB = 64): one row's logits x[0..n) in shared memory, owned by one thread -------------------
+// The same maths as log_softmax_n / categorical_row, streamed over the row instead of held in per-thread arrays (a 64-entry
+// array per thread would spill): a first pass masks (-6e4) and takes the max, a second the sum of exponentials, and every
+// later pass recomputes nl[j] = x[j] - lse and p[j] = exp(nl[j] - mx2) / s2 on the fly.  mx2 = max_j (x[j] - lse) is
+// mx - lse: rounding is monotone, so the max of the rounded differences is the rounded difference of the max.
+struct WideSoftmax {
+    float lse, mx2, s2;
+    uint64_t masked;   // masked-out actions
+    __device__ __forceinline__ float nl(const float* x, int j) const { return x[j] - lse; }
+    __device__ __forceinline__ float pr(const float* x, int j) const { return expf(x[j] - lse - mx2) / s2; }
+};
+__device__ __forceinline__ WideSoftmax wide_log_softmax(float* x, int n, const float* mask_row) {
+    WideSoftmax r;
+    r.masked = 0;
+    if (mask_row) {
+        for (int j = 0; j < n; ++j)
+            if (mask_row[j] == 0.f) { x[j] = -6e4f; r.masked |= 1ull << j; }
+    }
+    float mx = x[0];
+    for (int j = 1; j < n; ++j) mx = fmaxf(mx, x[j]);
+    float s = 0.f;
+    for (int j = 0; j < n; ++j) s += expf(x[j] - mx);
+    r.lse = mx + logf(s);
+    r.mx2 = mx - r.lse;
+    float s2 = 0.f;
+    for (int j = 0; j < n; ++j) s2 += expf(x[j] - r.lse - r.mx2);
+    r.s2 = s2;
+    return r;
+}
+__device__ __forceinline__ float wide_log_prob_of(const WideSoftmax& sm, const float* x, int n, int act) {
+    return sm.nl(x, (act >= 0 && act < n) ? act : 0);
+}
+__device__ __forceinline__ float wide_entropy(const WideSoftmax& sm, const float* x, int n) {
+    float ent = 0.f;
+    for (int j = 0; j < n; ++j) ent -= sm.pr(x, j) * sm.nl(x, j);
+    return ent;
+}
+
+// categorical_row of a wide head: masks the row's logits, then overwrites x[0..pad4(n)) with dL/dlogits (0 for the
+// masked-out actions and the padding), the K = pad4(n) operand of dn3 = dL . Whf and GH += dL^T n3.
+template <class Args>
+__device__ __forceinline__ CatRow wide_categorical_row(const Args& a, float* x, int n, const float* mask_row, int act,
+                                                       float old_lp, float adv, float wrow) {
+    const WideSoftmax sm = wide_log_softmax(x, n, mask_row);
+    const PgTerm pg = pg_term(wide_log_prob_of(sm, x, n, act), old_lp, adv, a.clip_param, a.flags, a.dual_clip_coeff);
+    const float ent = wide_entropy(sm, x, n);
+    const float dlp = pg.dlogp * wrow, went = a.entropy_coef * wrow;
+    for (int j = 0; j < n; ++j) {
+        const float p = sm.pr(x, j), nl = sm.nl(x, j);
+        x[j] = ((sm.masked >> j) & 1ull) ? 0.f : dlp * ((j == act ? 1.f : 0.f) - p) + went * p * (nl + ent);
+    }
+    for (int j = n; j < pad4(n); ++j) x[j] = 0.f;
+    return CatRow{pg.loss, ent, pg.ratio};
+}
+
 // DiagGaussian head (distributions.py:34-47, 75-98): Normal.log_prob of one dimension at distance diff = x - mean,
 // -diff^2 / (2 var) - log(std) - log(sqrt(2 pi)), and Normal.entropy of one dimension, 0.5 + 0.5 log(2 pi) + log(std)
 __device__ __forceinline__ float gaussian_log_prob(float diff, float std, float logstd) {

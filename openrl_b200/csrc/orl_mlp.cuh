@@ -27,7 +27,8 @@ namespace orl {
 
 constexpr int H = 64;     // hidden width (cfg.hidden_size), fixed in this build
 constexpr int LDA = 68;   // leading dimension of H-wide activation tiles in smem
-constexpr int MAX_OUT = 8;  // max head width (n actions)
+constexpr int MAX_OUT = 8;  // head width bound NB of the per-thread head code (head_dots, sample_action, categorical_row)
+constexpr int MAX_OUT_WIDE = 64;  // head width bound NB of the wide Categorical head: a logits tile in shared memory
 constexpr float LN_EPS = 1e-5f;
 
 struct NetOffsets {
@@ -112,34 +113,47 @@ __device__ __forceinline__ float unfolded_grad(const float* P, const NetOffsets&
 
 __host__ __device__ inline int pad4(int x) { return (x + 3) & ~3; }
 
-// Shared-memory weight block of one net (folded).  Sizes in floats.
+// Shared-memory weight block of one net (folded).  Sizes in floats.  NB is the head width bound: NB = 8 holds the head
+// as 8 natural rows for the per-thread head dots; NB = 64 (Categorical heads of 9..64 actions) holds it k-major for the
+// logits tile GEMM (head_tile) and, for the backward pass, natural for dn3 = dL . Whf.
 struct SmemWeights {
     float* w1t;   // [dp][64]  k-major: w1t[k*64 + j] = W1[j][k]        (dp = pad4(d), zero padded)
     float* b1;    // [64]
     float* w3t;   // [64][64]  k-major folded: w3t[k*64 + j] = W3[j][k]*g1[k]
     float* w3n;   // [64][64]  natural folded: w3n[j*64 + k] = W3[j][k]*g1[k]   (backward only)
     float* b3f;   // [64]
-    float* whf;   // [8][64]   natural folded: whf[j*64 + k] = Wh[j][k]*g3[k]   (rows >= n zero)
-    float* bhf;   // [8]
+    float* whf;   // [NB][64]  natural folded: whf[j*64 + k] = Wh[j][k]*g3[k]   (rows >= n zero; NB = 64: backward only)
+    float* wht;   // [64][64]  k-major folded: wht[k*64 + j] = Wh[j][k]*g3[k]   (NB = 64 only; columns >= n zero)
+    float* bhf;   // [NB]
 };
+template <int NB = MAX_OUT>
 __host__ __device__ inline int smem_weights_floats(int d, bool backward) {
-    return pad4(d) * H + H + H * H + (backward ? H * H : 0) + H + MAX_OUT * H + MAX_OUT;
+    const int head = NB == MAX_OUT ? MAX_OUT * H : (backward ? H * H : 0) + H * H;
+    return pad4(d) * H + H + H * H + (backward ? H * H : 0) + H + head + NB;
 }
+template <int NB = MAX_OUT>
 __device__ inline SmemWeights carve_weights(float*& p, int d, bool backward) {
+    static_assert(NB == MAX_OUT || NB == MAX_OUT_WIDE, "head width bound");
     SmemWeights w;
     w.w1t = p; p += pad4(d) * H;
     w.b1 = p; p += H;
     w.w3t = p; p += H * H;
     w.w3n = backward ? p : nullptr; if (backward) p += H * H;
     w.b3f = p; p += H;
-    w.whf = p; p += MAX_OUT * H;
-    w.bhf = p; p += MAX_OUT;
+    if (NB == MAX_OUT) {
+        w.whf = p; p += MAX_OUT * H;
+        w.wht = nullptr;
+    } else {
+        w.whf = backward ? p : nullptr; if (backward) p += H * H;
+        w.wht = p; p += H * H;
+    }
+    w.bhf = p; p += NB;
     return w;
 }
 
 // Stage + fold one net's parameters from the flat global buffer.  All threads of the CTA call it;
 // ends with __syncthreads().
-template <int NT>
+template <int NT, int NB = MAX_OUT>
 __device__ inline void load_weights_folded(const SmemWeights& w, const float* __restrict__ params, int d, int n,
                                            bool backward) {
     const NetOffsets o = net_offsets(d, n);
@@ -155,10 +169,19 @@ __device__ inline void load_weights_folded(const SmemWeights& w, const float* __
         w.w3t[k * H + j] = v;
         if (backward) w.w3n[i] = v;
     }
-    for (int i = tid; i < MAX_OUT * H; i += NT) w.whf[i] = folded_wh(params, o, i / H, i % H);
+    if (NB == MAX_OUT) {
+        for (int i = tid; i < MAX_OUT * H; i += NT) w.whf[i] = folded_wh(params, o, i / H, i % H);
+    } else {
+        for (int i = tid; i < H * H; i += NT) {
+            const int j = i / H, k = i % H;
+            const float v = folded_wh(params, o, j, k);
+            w.wht[k * H + j] = v;
+            if (backward) w.whf[i] = v;
+        }
+    }
     // folded biases: one warp-sized group of threads per output
     for (int j = tid; j < H; j += NT) w.b3f[j] = folded_b3(params, o, j);
-    for (int j = tid; j < MAX_OUT; j += NT) w.bhf[j] = folded_bh(params, o, j);
+    for (int j = tid; j < NB; j += NT) w.bhf[j] = folded_bh(params, o, j);
     __syncthreads();
 }
 
@@ -333,6 +356,20 @@ __device__ __forceinline__ void head_dots(const SmemWeights& w, const float* __r
             out[j] += w.bhf[j];
         }
     }
+}
+
+// Logits tile of a wide head (NB = 64): Ls[m][j] = bhf[j] + sum_k N3s[m][k] Whf[j][k] for all 64 columns j (0 for j >= n),
+// an M x 64 tile GEMM in the trunk's layout, stored with leading dimension LDA.  Callers sync before reading Ls.
+template <int M, int NT>
+__device__ __forceinline__ void head_tile(const SmemWeights& w, const float* __restrict__ N3s, float* __restrict__ Ls) {
+    constexpr int TY = NT / 16, RPT = M / TY;
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    float acc[RPT][4];
+    const float4 b = *reinterpret_cast<const float4*>(w.bhf + 4 * tx);
+#pragma unroll
+    for (int i = 0; i < RPT; ++i) { acc[i][0] = b.x; acc[i][1] = b.y; acc[i][2] = b.z; acc[i][3] = b.w; }
+    gemm_tile<RPT, TY>(N3s, LDA, w.wht, H, acc, tx, ty);
+    store_tile<RPT, TY>(Ls, acc, tx, ty);
 }
 
 }  // namespace orl

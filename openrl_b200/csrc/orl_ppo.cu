@@ -99,8 +99,14 @@ __device__ __forceinline__ void wgrad_flush(float* __restrict__ scratch, const W
 }
 
 
-template <bool POLICY>
+// NB: head width bound of the policy pass (orl_mlp.cuh).  NB = 64, Categorical heads of 9..64 actions: the logits are a
+// 128 x 64 tile (head_tile) in the DZs buffer, which the row loss overwrites with dL/dlogits; dn3 = dL . Whf is a tile
+// GEMM with K = pad4(n) and GH += dL^T n3 a wgrad_acc with JB = ceil(n / 4).  dZ3 goes to DZs only after both have read
+// dL, so the dL tile needs no buffer of its own (that keeps obs width 64 within the 227 KB of shared memory).
+template <bool POLICY, int NB = MAX_OUT>
 __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, int cta, int G) {
+    constexpr bool WIDE = NB == MAX_OUT_WIDE;
+    static_assert(POLICY || !WIDE, "the critic's head is one value");
     const int d = POLICY ? a.obs_dim : a.critic_obs_dim;
     const int n = POLICY ? a.n_actions : 1;
     const float* params = POLICY ? a.policy_params : a.critic_params;
@@ -109,12 +115,12 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
 
     float* p = smem;
-    SmemWeights w = carve_weights(p, d, true);
+    SmemWeights w = carve_weights<NB>(p, d, true);
     float* Xs = p;  p += P_M * ldx;
     float* N1s = p; p += P_M * LDA;
     float* N3s = p; p += P_M * LDA;
     float* DZs = p; p += P_M * LDA;
-    float* DLs = p; p += P_M * DLW;
+    float* DLs = p; if (!WIDE) p += P_M * DLW;
     float* row_a = p; p += P_M;   // policy: action      | critic: value_pred
     float* row_b = p; p += P_M;   // policy: old logp    | critic: return
     float* row_c = p; p += P_M;   // policy: raw adv
@@ -122,17 +128,17 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
     float* red = p; p += 32;
     long long* row_idx = reinterpret_cast<long long*>(p); p += 2 * P_M;
 
-    load_weights_folded<P_NT>(w, params, d, n, true);
+    load_weights_folded<P_NT, NB>(w, params, d, n, true);
 
     const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS, val_masks = a.flags & ORL_PPO_VALUE_ACTIVE_MASKS;
     const MbConsts mb = mb_consts(a);
 
     const WgMap map3 = wg_map(16, 16);
     const WgMap map1 = wg_map(16, dp / 4);
-    const int JBH = n > 4 ? 2 : 1;
+    const int JBH = WIDE ? (n + 3) / 4 : n > 4 ? 2 : 1;
     const WgMap maph = wg_map(JBH, 16);
     float g3[4][4] = {}, g1[4][4] = {}, gh[4][4] = {}, db3[4] = {}, db1[4] = {}, dbh[4] = {};
-    const bool gaussian = POLICY && a.head_kind == ORL_HEAD_GAUSSIAN;
+    const bool gaussian = POLICY && !WIDE && a.head_kind == ORL_HEAD_GAUSSIAN;
     float dls_acc[MAX_OUT] = {};   // dL/dlogstd partial sums of this thread's rows (Gaussian head)
     float loss0 = 0.f, loss1 = 0.f, loss2 = 0.f;  // policy: policy_loss, entropy, ratio | critic: value_loss
 
@@ -164,67 +170,100 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
         unsigned posmask;
         trunk_forward<P_M, P_NT, true>(w, Xs, ldx, d, a.activation_id, N1s, N3s, mu1, rstd1, rstd3, posmask);
         __syncthreads();
-        float out[MAX_OUT];
-        head_dots<P_M, P_NT>(w, N3s, n, out);
-        {
-            constexpr int PPR = P_NT / P_M;
-            const int row = tid / PPR;
-            if (tid % PPR == 0) {
-                float dl[DLW];
-#pragma unroll
-                for (int j = 0; j < DLW; ++j) dl[j] = 0.f;
-                if (row < rows_here) {
-                    const float active = row_act[row];
-                    if (POLICY && gaussian) {
-                        const long long gi = row_idx[row];
-                        const float went_row = pol_masks ? active * mb.inv_act : mb.inv_rows / (float)n;
-                        gaussian_row(a, out, n, params + net_offsets(d, n, 1).ls, a.actions + gi * n, a.old_log_probs + gi * n,
-                                     apply_adv_norm(mb.adv, row_c[row]), mb.weight(pol_masks, active), went_row, dl, dls_acc,
-                                     loss0, loss1, loss2);
-                    } else if (POLICY) {
-                        const long long gi = row_idx[row];
-                        const float wrow = mb.weight(pol_masks, active);
-                        const CatRow c = categorical_row(a, out, n, a.action_masks ? a.action_masks + gi * n : nullptr, (int)row_a[row],
-                                                         row_b[row], apply_adv_norm(mb.adv, row_c[row]), wrow, dl);
-                        loss0 += c.loss * wrow;
-                        loss1 += c.ent * wrow;
-                        loss2 += c.ratio;
-                    } else {
-                        const float ret = row_b[row];
-                        const float target = (a.flags & ORL_PPO_VALUENORM) ? (ret - mb.vn_mean) / mb.vn_std : ret;
-                        const ValueTerm vt = value_term(out[0], row_a[row], target, a.clip_param, a.huber_delta, a.flags);
-                        const float wrow = mb.weight(val_masks, active);
-                        loss0 += vt.loss * wrow;
-                        dl[0] = a.value_loss_coef * wrow * vt.dv;
-                    }
-                }
-                *reinterpret_cast<float4*>(DLs + row * DLW) = make_float4(dl[0], dl[1], dl[2], dl[3]);
-                *reinterpret_cast<float4*>(DLs + row * DLW + 4) = make_float4(dl[4], dl[5], dl[6], dl[7]);
-            }
-        }
-        __syncthreads();
-
-        // ---- backward: head -> LN3 ----
         float acc[P_RPT][4];
-#pragma unroll
-        for (int i = 0; i < P_RPT; ++i) { acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f; }
-        for (int j = 0; j < n; ++j) {
-            const float4 wv = *reinterpret_cast<const float4*>(w.whf + j * H + 4 * tx);
-#pragma unroll
-            for (int i = 0; i < P_RPT; ++i) {
-                const float dlv = DLs[(ty + P_TY * i) * DLW + j];
-                acc[i][0] = fmaf(dlv, wv.x, acc[i][0]); acc[i][1] = fmaf(dlv, wv.y, acc[i][1]);
-                acc[i][2] = fmaf(dlv, wv.z, acc[i][2]); acc[i][3] = fmaf(dlv, wv.w, acc[i][3]);
+        if constexpr (WIDE) {
+            head_tile<P_M, P_NT>(w, N3s, DZs);
+            __syncthreads();
+            if (tid < P_M) {   // one thread per row: the logits row becomes the dL/dlogits row
+                float* x = DZs + tid * LDA;
+                if (tid < rows_here) {
+                    const long long gi = row_idx[tid];
+                    const float wrow = mb.weight(pol_masks, row_act[tid]);
+                    const CatRow c = wide_categorical_row(a, x, n, a.action_masks ? a.action_masks + gi * n : nullptr, (int)row_a[tid],
+                                                          row_b[tid], apply_adv_norm(mb.adv, row_c[tid]), wrow);
+                    loss0 += c.loss * wrow;
+                    loss1 += c.ent * wrow;
+                    loss2 += c.ratio;
+                } else {
+                    for (int j = 0; j < pad4(n); ++j) x[j] = 0.f;
+                }
             }
+            __syncthreads();
+            // ---- backward: head -> LN3 ----
+#pragma unroll
+            for (int i = 0; i < P_RPT; ++i) { acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f; }
+            gemm_tile<P_RPT, P_TY>(DZs, LDA, w.whf, pad4(n), acc, tx, ty);   // dn3 = dL . Whf
+            wgrad_acc(DZs, LDA, N3s, LDA, maph, gh, dbh);                   // GH += dL^T n3
+            {
+                float nrm[P_RPT][4];
+                load_tile<P_RPT, P_TY>(N3s, nrm, tx, ty);
+                layernorm_bwd_rows<P_RPT>(acc, nrm, rstd3);
+            }
+            __syncthreads();                                                 // all reads of dL done
+            store_tile<P_RPT, P_TY>(DZs, acc, tx, ty);                       // dZ3
+            __syncthreads();
+        } else {
+            float out[MAX_OUT];
+            head_dots<P_M, P_NT>(w, N3s, n, out);
+            {
+                constexpr int PPR = P_NT / P_M;
+                const int row = tid / PPR;
+                if (tid % PPR == 0) {
+                    float dl[DLW];
+#pragma unroll
+                    for (int j = 0; j < DLW; ++j) dl[j] = 0.f;
+                    if (row < rows_here) {
+                        const float active = row_act[row];
+                        if (POLICY && gaussian) {
+                            const long long gi = row_idx[row];
+                            const float went_row = pol_masks ? active * mb.inv_act : mb.inv_rows / (float)n;
+                            gaussian_row(a, out, n, params + net_offsets(d, n, 1).ls, a.actions + gi * n, a.old_log_probs + gi * n,
+                                         apply_adv_norm(mb.adv, row_c[row]), mb.weight(pol_masks, active), went_row, dl, dls_acc,
+                                         loss0, loss1, loss2);
+                        } else if (POLICY) {
+                            const long long gi = row_idx[row];
+                            const float wrow = mb.weight(pol_masks, active);
+                            const CatRow c = categorical_row(a, out, n, a.action_masks ? a.action_masks + gi * n : nullptr, (int)row_a[row],
+                                                             row_b[row], apply_adv_norm(mb.adv, row_c[row]), wrow, dl);
+                            loss0 += c.loss * wrow;
+                            loss1 += c.ent * wrow;
+                            loss2 += c.ratio;
+                        } else {
+                            const float ret = row_b[row];
+                            const float target = (a.flags & ORL_PPO_VALUENORM) ? (ret - mb.vn_mean) / mb.vn_std : ret;
+                            const ValueTerm vt = value_term(out[0], row_a[row], target, a.clip_param, a.huber_delta, a.flags);
+                            const float wrow = mb.weight(val_masks, active);
+                            loss0 += vt.loss * wrow;
+                            dl[0] = a.value_loss_coef * wrow * vt.dv;
+                        }
+                    }
+                    *reinterpret_cast<float4*>(DLs + row * DLW) = make_float4(dl[0], dl[1], dl[2], dl[3]);
+                    *reinterpret_cast<float4*>(DLs + row * DLW + 4) = make_float4(dl[4], dl[5], dl[6], dl[7]);
+                }
+            }
+            __syncthreads();
+
+            // ---- backward: head -> LN3 ----
+#pragma unroll
+            for (int i = 0; i < P_RPT; ++i) { acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f; }
+            for (int j = 0; j < n; ++j) {
+                const float4 wv = *reinterpret_cast<const float4*>(w.whf + j * H + 4 * tx);
+#pragma unroll
+                for (int i = 0; i < P_RPT; ++i) {
+                    const float dlv = DLs[(ty + P_TY * i) * DLW + j];
+                    acc[i][0] = fmaf(dlv, wv.x, acc[i][0]); acc[i][1] = fmaf(dlv, wv.y, acc[i][1]);
+                    acc[i][2] = fmaf(dlv, wv.z, acc[i][2]); acc[i][3] = fmaf(dlv, wv.w, acc[i][3]);
+                }
+            }
+            {
+                float nrm[P_RPT][4];
+                load_tile<P_RPT, P_TY>(N3s, nrm, tx, ty);
+                layernorm_bwd_rows<P_RPT>(acc, nrm, rstd3);
+            }
+            store_tile<P_RPT, P_TY>(DZs, acc, tx, ty);   // dZ3
+            wgrad_acc(DLs, DLW, N3s, LDA, maph, gh, dbh);  // GH += dL^T n3
+            __syncthreads();
         }
-        {
-            float nrm[P_RPT][4];
-            load_tile<P_RPT, P_TY>(N3s, nrm, tx, ty);
-            layernorm_bwd_rows<P_RPT>(acc, nrm, rstd3);
-        }
-        store_tile<P_RPT, P_TY>(DZs, acc, tx, ty);   // dZ3
-        wgrad_acc(DLs, DLW, N3s, LDA, maph, gh, dbh);  // GH += dL^T n3
-        __syncthreads();
 
         // ---- fc3 backward ----
         wgrad_acc(DZs, LDA, N1s, LDA, map3, g3, db3);  // G3 += dZ3^T n1
@@ -261,7 +300,9 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
     wgrad_flush(scratch, map3, 16, 16, g3, db3, H, H, part + fo.g3, part + fo.db3);
     wgrad_flush(scratch, maph, JBH, 16, gh, dbh, n, H, part + fo.gh, part + fo.dbh);
     __syncthreads();
-    if (POLICY) {   // dL/dlogstd: block reduction of the per-thread partial sums (zero for categorical heads)
+    if (WIDE) {     // no logstd: a Categorical head
+        if (tid < n) part[fo.dls + tid] = 0.f;
+    } else if (POLICY) {   // dL/dlogstd: block reduction of the per-thread partial sums (zero for categorical heads)
         const int lane = tid & 31, warp = tid >> 5;
 #pragma unroll
         for (int j = 0; j < MAX_OUT; ++j) {
@@ -295,10 +336,11 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
     }
 }
 
+template <int NB>
 __global__ void __launch_bounds__(P_NT, 1) ppo_fwdbwd_kernel(const OrlPpoArgs a) {
     extern __shared__ __align__(16) float smem[];
     const int G = a.grid_per_net;
-    if ((int)blockIdx.x < G) ppo_net_pass<true>(a, smem, blockIdx.x, G);
+    if ((int)blockIdx.x < G) ppo_net_pass<true, NB>(a, smem, blockIdx.x, G);
     else ppo_net_pass<false>(a, smem, blockIdx.x - G, G);
 }
 
@@ -507,10 +549,19 @@ size_t fwdbwd_smem_bytes(int d, int dc) {
                           (size_t)P_M * DLW + 4 * P_M + 32 + 4 * P_M /* row_idx as 2 floats each */ + 16;
     return floats * sizeof(float);
 }
+// the wide policy pass (no separate dL tile) or the critic pass, whichever needs more
+size_t fwdbwd_wide_smem_bytes(int d, int dc) {
+    const size_t rest = (size_t)4 * P_M + 32 + 4 * P_M + 16;
+    const size_t pol = orl::smem_weights_floats<orl::MAX_OUT_WIDE>(d, true) + (size_t)P_M * (orl::pad4(d) + 4) + 3 * (size_t)P_M * orl::LDA + rest;
+    const size_t cri = orl::smem_weights_floats(dc, true) + (size_t)P_M * (orl::pad4(dc) + 4) + 3 * (size_t)P_M * orl::LDA + (size_t)P_M * DLW + rest;
+    return std::max(pol, cri) * sizeof(float);
+}
 
 int check_ppo_args(const OrlPpoArgs& a) {
     ORL_CHECK_ARG(a.obs_dim > 0 && a.obs_dim <= 64 && a.critic_obs_dim > 0 && a.critic_obs_dim <= 64, "obs dims must be in 1..64");
-    ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= orl::MAX_OUT, "n_actions must be in 1..8");
+    ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= orl::MAX_OUT_WIDE, "n_actions must be in 1..64");
+    ORL_CHECK_ARG(a.n_actions <= orl::MAX_OUT || a.head_kind == ORL_HEAD_CATEGORICAL,
+                  "n_actions must be in 1..8 for Gaussian heads (1..64 for Categorical heads)");
     ORL_CHECK_ARG(a.activation_id >= 0 && a.activation_id <= 3, "activation_id");
     ORL_CHECK_ARG(a.grid_per_net > 0, "grid_per_net");
     ORL_CHECK_ARG(a.batch_rows > 0, "batch_rows");
@@ -545,15 +596,18 @@ extern "C" int orl_ppo_fwdbwd(const OrlPpoArgs* args, void* stream) {
     ORL_CHECK_ARG(a.indices || (a.row_begin >= 0 && a.row_begin + a.batch_rows <= a.total_rows), "row range");
     ORL_CHECK_ARG(a.head_kind == ORL_HEAD_CATEGORICAL || a.head_kind == ORL_HEAD_GAUSSIAN, "head_kind");
     if (a.flags & ORL_PPO_TF32) {
+        ORL_CHECK_ARG(a.n_actions <= orl::MAX_OUT, "ORL_PPO_TENSORCORE: n_actions must be in 1..8");
         if (a.head_kind != ORL_HEAD_CATEGORICAL) {
             orl::set_last_error("orl_ppo_fwdbwd: ORL_PPO_TENSORCORE supports categorical heads only");
             return ORL_ERR_UNSUPPORTED;
         }
         return orl::launch_ppo_fwdbwd_tc(a, reinterpret_cast<cudaStream_t>(stream));
     }
-    const size_t smem = fwdbwd_smem_bytes(a.obs_dim, a.critic_obs_dim);
-    if (int e = orl::allow_dynamic_smem(ppo_fwdbwd_kernel, 227 * 1024)) return e;
-    ppo_fwdbwd_kernel<<<2 * a.grid_per_net, P_NT, smem, reinterpret_cast<cudaStream_t>(stream)>>>(a);
+    const bool wide = a.n_actions > orl::MAX_OUT;
+    const size_t smem = wide ? fwdbwd_wide_smem_bytes(a.obs_dim, a.critic_obs_dim) : fwdbwd_smem_bytes(a.obs_dim, a.critic_obs_dim);
+    void (*const kern)(OrlPpoArgs) = wide ? ppo_fwdbwd_kernel<orl::MAX_OUT_WIDE> : ppo_fwdbwd_kernel<orl::MAX_OUT>;
+    if (int e = orl::allow_dynamic_smem(kern, 227 * 1024)) return e;
+    kern<<<2 * a.grid_per_net, P_NT, smem, reinterpret_cast<cudaStream_t>(stream)>>>(a);
     ORL_LAUNCH_CHECK("ppo_fwdbwd_kernel");
     return 0;
 }

@@ -49,13 +49,15 @@ __global__ void env_step_kernel(int kind, int N, EnvPtrs E, const float* __restr
 }
 
 
-template <int R_M, int ENV>
+// NB: head width bound (orl_mlp.cuh); NB = 64 is the wide Categorical head of host-stepped envs (ORL_ENV_NONE), whose
+// logits tile reuses N1s once the trunk is done with it.
+template <int R_M, int ENV, int NB = MAX_OUT>
 __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
     extern __shared__ __align__(16) float smem[];
     const int N = a.n_envs, A = a.n_agents, B = N * A, d = a.obs_dim, n = a.n_actions;
     const int ldx = pad4(d) + 4;
     float* p = smem;
-    SmemWeights w = carve_weights(p, d, false);
+    SmemWeights w = carve_weights<NB>(p, d, false);
     float* Xs = p;  p += R_M * ldx;
     float* N1s = p; p += R_M * LDA;
     float* N3s = p; p += R_M * LDA;
@@ -69,7 +71,7 @@ __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
     const int rows_here = n_env_here * A;
     const int tid = threadIdx.x;
 
-    load_weights_folded<R_NT>(w, a.policy_params, d, n, false);   // (the logstd tail, if any, is read directly)
+    load_weights_folded<R_NT, NB>(w, a.policy_params, d, n, false);   // (the logstd tail, if any, is read directly)
 
     // stage obs of slot t_begin (zero padding for the k tail and for idle rows)
     for (int i = tid; i < R_M * ldx; i += R_NT) {
@@ -87,6 +89,25 @@ __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
         unsigned pm;
         trunk_forward<R_M, R_NT, false>(w, Xs, ldx, d, a.activation_id, N1s, N3s, mu1, rstd1, rstd3, pm);
         __syncthreads();
+        if constexpr (NB == MAX_OUT_WIDE) {
+            static_assert(ENV == ORL_ENV_NONE, "wide heads act on host-stepped envs");
+            head_tile<R_M, R_NT>(w, N3s, N1s);
+            __syncthreads();
+            if (tid < rows_here) {   // one thread per row
+                const size_t grow = (size_t)t * B + row0 + tid;
+                const uint64_t step = rng_base + (uint64_t)t;
+                const uint32_t grow32 = (uint32_t)(row0 + tid + a.rng_row_offset);
+                float lp;
+                const int act = wide_sample_action(N1s + tid * LDA, n, a.action_masks ? a.action_masks + grow * n : nullptr,
+                                                   a.deterministic != 0, [&](int j0, float (&q)[4]) {
+                                                       wide_action_noise4(a.exp_noise, grow, n, a.rng_seed, step, grow32, j0, q);
+                                                   }, lp);
+                a.actions[grow] = (float)act;
+                a.action_log_probs[grow] = lp;
+            }
+            __syncthreads();
+            continue;
+        }
         float logit[MAX_OUT];
         head_dots<R_M, R_NT>(w, N3s, n, logit);
         if (hpart == 0 && hrow < rows_here && a.head_kind == ORL_HEAD_GAUSSIAN)
@@ -160,18 +181,19 @@ __global__ void env_reset_kernel(int env_kind, int N, double* env_f64, uint64_t*
 // epilogue(g, out) on the thread that owns row g, with out[0..n) the head outputs of that row.
 constexpr int C_M = 128, C_NT = 256;
 
-template <typename Epilogue>
+// NB = 64 (wide Categorical heads): the logits go to a tile in N1s and epilogue(g, x) gets the row's logits x[0..n) there.
+template <int NB = MAX_OUT, typename Epilogue>
 __device__ __forceinline__ void rows_forward(const float* __restrict__ params, int d, int n, int activation_id,
                                              const float* __restrict__ obs, long long rows, Epilogue&& epilogue) {
     extern __shared__ __align__(16) float smem[];
     const int ldx = pad4(d) + 4;
     float* p = smem;
-    SmemWeights w = carve_weights(p, d, false);
+    SmemWeights w = carve_weights<NB>(p, d, false);
     float* Xs = p;  p += C_M * ldx;
     float* N1s = p; p += C_M * LDA;
     float* N3s = p; p += C_M * LDA;
     const int tid = threadIdx.x;
-    load_weights_folded<C_NT>(w, params, d, n, false);
+    load_weights_folded<C_NT, NB>(w, params, d, n, false);
     const long long n_tiles = (rows + C_M - 1) / C_M;
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const long long r0 = tile * C_M;
@@ -185,10 +207,16 @@ __device__ __forceinline__ void rows_forward(const float* __restrict__ params, i
         unsigned pm;
         trunk_forward<C_M, C_NT, false>(w, Xs, ldx, d, activation_id, N1s, N3s, mu1, rstd1, rstd3, pm);
         __syncthreads();
-        float out[MAX_OUT];
-        head_dots<C_M, C_NT>(w, N3s, n, out);
-        constexpr int PPR = C_NT / C_M;
-        if (tid % PPR == 0 && tid / PPR < rows_here) epilogue(r0 + tid / PPR, out);
+        if constexpr (NB == MAX_OUT_WIDE) {
+            head_tile<C_M, C_NT>(w, N3s, N1s);
+            __syncthreads();
+            if (tid < rows_here) epilogue(r0 + tid, N1s + tid * LDA);
+        } else {
+            float out[MAX_OUT];
+            head_dots<C_M, C_NT>(w, N3s, n, out);
+            constexpr int PPR = C_NT / C_M;
+            if (tid % PPR == 0 && tid / PPR < rows_here) epilogue(r0 + tid / PPR, out);
+        }
         __syncthreads();
     }
 }
@@ -220,6 +248,18 @@ __global__ void __launch_bounds__(C_NT) policy_eval_kernel(const float* __restri
             logp_out[g] = log_prob_of(nl, n, (int)actions[g]);
             entropy_out[g] = categorical_entropy(nl, pr, n);
         }
+    });
+}
+
+// policy_eval_kernel of a wide Categorical head (9..64 actions)
+__global__ void __launch_bounds__(C_NT) policy_eval_wide_kernel(const float* __restrict__ params, int d, int n, int activation_id,
+                                                                const float* __restrict__ obs, const float* __restrict__ actions,
+                                                                const float* __restrict__ action_masks, float* __restrict__ logp_out,
+                                                                float* __restrict__ entropy_out, long long rows) {
+    rows_forward<MAX_OUT_WIDE>(params, d, n, activation_id, obs, rows, [&](long long g, float* x) {
+        const WideSoftmax sm = wide_log_softmax(x, n, action_masks ? action_masks + g * n : nullptr);
+        logp_out[g] = wide_log_prob_of(sm, x, n, (int)actions[g]);
+        entropy_out[g] = wide_entropy(sm, x, n);
     });
 }
 
@@ -284,10 +324,10 @@ __global__ void host_insert_rnn_kernel(const float* __restrict__ staged, int n_e
 }
 
 // launch of a row-batch forward kernel over `rows` rows of obs_dim d: grid = min(tiles, 2 x SMs)
-template <typename... Params, typename... Args>
+template <int NB = MAX_OUT, typename... Params, typename... Args>
 int launch_rows_forward(void (*kern)(Params...), const char* name, int d, long long rows, cudaStream_t st, Args... args) {
     const int ldx = pad4(d) + 4;
-    const size_t smem = sizeof(float) * (smem_weights_floats(d, false) + C_M * ldx + 2 * C_M * LDA);
+    const size_t smem = sizeof(float) * (smem_weights_floats<NB>(d, false) + C_M * ldx + 2 * C_M * LDA);
     if (int e = allow_dynamic_smem(kern, 200 * 1024)) return e;
     const long long n_tiles = (rows + C_M - 1) / C_M;
     const int grid = (int)std::min<long long>(n_tiles, 2LL * sm_count());
@@ -351,7 +391,9 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
     const OrlRolloutArgs& a = *args;
     ORL_CHECK_ARG(a.n_envs > 0 && a.n_agents > 0 && a.n_agents <= 32, "n_envs / n_agents");
     ORL_CHECK_ARG(a.obs_dim > 0 && a.obs_dim <= 64, "obs_dim must be in 1..64");
-    ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= orl::MAX_OUT, "n_actions must be in 1..8");
+    ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= orl::MAX_OUT_WIDE, "n_actions must be in 1..64");
+    ORL_CHECK_ARG(a.n_actions <= orl::MAX_OUT || (a.env_kind == ORL_ENV_NONE && a.head_kind == ORL_HEAD_CATEGORICAL),
+                  "n_actions must be in 1..8 (9..64: Categorical heads on host-stepped envs, ORL_ENV_NONE)");
     ORL_CHECK_ARG(a.t_begin >= 0 && a.t_begin < a.t_end && a.t_end <= a.episode_length, "step range");
     ORL_CHECK_ARG(a.activation_id >= 0 && a.activation_id <= 3, "activation_id");
     ORL_CHECK_ARG(a.policy_params && a.policy_obs && a.actions && a.action_log_probs, "null buffer");
@@ -394,10 +436,13 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
     const int envs_per_cta = rm / a.n_agents;
     const int grid = (a.n_envs + envs_per_cta - 1) / envs_per_cta;
     const int ldx = orl::pad4(a.obs_dim) + 4;
-    const size_t smem = sizeof(float) * (orl::smem_weights_floats(a.obs_dim, false) + rm * ldx + 2 * rm * orl::LDA + rm);
-    const bool mpe = a.env_kind == ORL_ENV_MPE_SPREAD;
+    const bool mpe = a.env_kind == ORL_ENV_MPE_SPREAD, wide = a.n_actions > orl::MAX_OUT;
+    const size_t smem = sizeof(float) * ((wide ? orl::smem_weights_floats<orl::MAX_OUT_WIDE>(a.obs_dim, false)
+                                               : orl::smem_weights_floats(a.obs_dim, false)) + rm * ldx + 2 * rm * orl::LDA + rm);
     void (*const kern)(OrlRolloutArgs) =
-        rm == 8 ? (mpe ? rollout_kernel<8, ORL_ENV_MPE_SPREAD> : rollout_kernel<8, ORL_ENV_NONE>)
+        wide ? (rm == 8 ? rollout_kernel<8, ORL_ENV_NONE, orl::MAX_OUT_WIDE>
+                : rm == 16 ? rollout_kernel<16, ORL_ENV_NONE, orl::MAX_OUT_WIDE> : rollout_kernel<32, ORL_ENV_NONE, orl::MAX_OUT_WIDE>)
+        : rm == 8 ? (mpe ? rollout_kernel<8, ORL_ENV_MPE_SPREAD> : rollout_kernel<8, ORL_ENV_NONE>)
         : rm == 16 ? (mpe ? rollout_kernel<16, ORL_ENV_MPE_SPREAD> : rollout_kernel<16, ORL_ENV_NONE>)
                    : (mpe ? rollout_kernel<32, ORL_ENV_MPE_SPREAD> : rollout_kernel<32, ORL_ENV_NONE>);
     if (int e = orl::allow_dynamic_smem(kern, 200 * 1024)) return e;
@@ -423,9 +468,15 @@ extern "C" int orl_policy_eval(const float* policy_params, int obs_dim, int n_ac
                                const float* obs, const float* actions, const float* action_masks, float* log_probs,
                                float* entropy, long long rows, void* stream) {
     ORL_CHECK_ARG(policy_params && obs && actions && log_probs && entropy, "null buffer");
-    ORL_CHECK_ARG(obs_dim > 0 && obs_dim <= 64 && n_actions > 0 && n_actions <= orl::MAX_OUT, "shapes");
+    ORL_CHECK_ARG(obs_dim > 0 && obs_dim <= 64 && n_actions > 0 && n_actions <= orl::MAX_OUT_WIDE, "shapes");
     ORL_CHECK_ARG(rows > 0 && activation_id >= 0 && activation_id <= 3, "rows / activation_id");
     ORL_CHECK_ARG(head_kind == ORL_HEAD_CATEGORICAL || head_kind == ORL_HEAD_GAUSSIAN, "head_kind");
+    ORL_CHECK_ARG(n_actions <= orl::MAX_OUT || head_kind == ORL_HEAD_CATEGORICAL,
+                  "n_actions must be in 1..8 for Gaussian heads (1..64 for Categorical heads)");
+    if (n_actions > orl::MAX_OUT)
+        return launch_rows_forward<orl::MAX_OUT_WIDE>(policy_eval_wide_kernel, "policy_eval_wide_kernel", obs_dim, rows,
+                                                      reinterpret_cast<cudaStream_t>(stream), policy_params, obs_dim, n_actions,
+                                                      activation_id, obs, actions, action_masks, log_probs, entropy, rows);
     return launch_rows_forward(policy_eval_kernel, "policy_eval_kernel", obs_dim, rows, reinterpret_cast<cudaStream_t>(stream),
                                policy_params, obs_dim, n_actions, activation_id, head_kind, obs, actions, action_masks,
                                log_probs, entropy, rows);
@@ -436,7 +487,7 @@ extern "C" int orl_host_insert(const float* staged, int n_envs, int n_agents, in
                                float* critic_obs_next, int critic_obs_dim, void* stream) {
     ORL_CHECK_ARG(staged && policy_obs_next && rewards && masks_next && active_masks_next, "null buffer");
     ORL_CHECK_ARG(n_envs > 0 && n_agents > 0 && obs_dim > 0, "shapes");
-    ORL_CHECK_ARG(!action_masks_next || (n_actions > 0 && n_actions <= orl::MAX_OUT), "n_actions must be in 1..8");
+    ORL_CHECK_ARG(!action_masks_next || (n_actions > 0 && n_actions <= orl::MAX_OUT_WIDE), "n_actions must be in 1..64");
     ORL_CHECK_ARG(!critic_obs_next || (critic_obs_dim > 0 && critic_obs_dim <= 64), "critic_obs_dim must be in 1..64");
     const int B = n_envs * n_agents;
     host_insert_kernel<<<(B + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(staged, n_envs, n_agents, obs_dim, policy_obs_next,

@@ -28,8 +28,14 @@ class PolicyNetwork(nn.Module):
         self.n_actions = action_space.shape[0] if self.act.continuous_action else action_space.n  # head width
         if self.recurrent and self.act.continuous_action:
             raise NotImplementedError("recurrent policies are built for Discrete action spaces")
-        if self.n_actions > 8:
-            raise NotImplementedError("head widths up to 8 are built")
+        # a feed-forward Categorical head runs up to 64 actions (a logits tile in the kernels); the GRU policy's heads and
+        # the DiagGaussian heads keep the per-thread head of up to 8 outputs
+        if self.n_actions > 64:
+            raise NotImplementedError("Discrete action spaces of up to 64 actions are built")
+        if self.n_actions > 8 and self.recurrent:
+            raise NotImplementedError("recurrent policies are built for up to 8 actions")
+        if self.n_actions > 8 and self.act.continuous_action:
+            raise NotImplementedError("DiagGaussian heads are built for Box action spaces of width up to 8")
         self.device = torch.device(device)
         self._flat = FlatParams(self, self.device)
 
