@@ -366,7 +366,8 @@ int orl_minibatch_stats(const int64_t* indices, int64_t batch_rows, const float*
 typedef struct OrlRnnArgs {
     int32_t env_kind, n_envs, n_agents, episode_length;   /* N, A, T; rows B = N*A */
     int32_t t_begin, t_end;
-    int32_t obs_dim, critic_obs_dim, n_actions, activation_id;
+    int32_t obs_dim, critic_obs_dim, n_actions, activation_id;   /* n_actions 1..64; 1..8 for orl_rnn_rollout and with
+                                                                   ORL_PPO_JOINT_ACTION (ORL_ERR_BAD_ARG otherwise) */
     int32_t deterministic, chunk_length;                  /* L = cfg.data_chunk_length (<= 32) */
     int32_t flags;                                        /* ORL_PPO_* */
     int32_t env_table_len;
@@ -383,7 +384,7 @@ typedef struct OrlRnnArgs {
     double* env_f64; uint64_t* env_u64; int32_t* env_i32; const int32_t* env_table;
     float* ep_return; int32_t* ep_length; double* episode_stats;
     const double* gae_stats; const double* mb_stats; float* vn_state;
-    float* tape;                                          /* workspace: orl_rnn_workspace_floats(n_chunks*L, grads_stride) floats (tape rows, then reduction partials) */
+    float* tape;                                          /* workspace: orl_rnn_workspace_floats_for(n_chunks*L, grads_stride, n_actions) floats (tape rows, then reduction partials) */
     float* grads;                                         /* (2, grads_stride) true gradients, policy then critic */
     int32_t grads_stride; int32_t reserved1;
     float* loss_acc;                                      /* (8) zeroed by orl_rnn_fwdbwd: policy_loss, entropy, ratio, value_loss sums */
@@ -406,8 +407,12 @@ typedef struct OrlRnnArgs {
 } OrlRnnArgs;
 int orl_rnn_param_count(int obs_dim, int n_out);
 int orl_rnn_tape_width(void);
-/* floats of OrlRnnArgs.tape for a minibatch of `rows` = n_chunks * chunk_length row-steps (times A with ORL_PPO_JOINT_ACTION) */
+/* floats of OrlRnnArgs.tape for a minibatch of `rows` = n_chunks * chunk_length row-steps (times A with ORL_PPO_JOINT_ACTION)
+ * of a policy with at most 8 actions */
 long long orl_rnn_workspace_floats(long long rows, int grads_stride);
+/* the same for a policy of n_actions actions: a wide head (9..64 actions) tapes dL/dlogits in 64 more floats per row
+ * (orl_rnn_tape_width() + 64); equal to orl_rnn_workspace_floats for n_actions <= 8 */
+long long orl_rnn_workspace_floats_for(long long rows, int grads_stride, int n_actions);
 /* policy GRU rollout for steps [t_begin, t_end) fused with the device env (simple_spread, CartPole, GridWorld); device
  * envs only: ORL_ENV_NONE is rejected (the policy step of host-stepped rows is orl_rnn_act_rows).  CartPole and
  * GridWorld need 16-byte aligned policy_obs and critic_obs (ORL_ERR_BAD_ARG otherwise). */
@@ -422,10 +427,15 @@ int orl_rnn_act_rows(const OrlRnnArgs* args, void* stream);
 /* orl_host_insert for a recurrent policy: additionally zeroes the 64-float rnn_states_next row of every agent of an env
  * whose agents are all done (rnn_states[dones_env] = 0, onpolicy_driver.py:262-269).  rnn_states_next addresses slot
  * t+1 at the same first row as the other pointers; action_masks_next / n_actions and critic_obs_next / critic_obs_dim
- * as in orl_host_insert. */
+ * as in orl_host_insert, except that masks take n_actions in 1..8 (ORL_ERR_BAD_ARG otherwise). */
 int orl_host_insert_rnn(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
                         float* masks_next, float* active_masks_next, float* rnn_states_next, float* action_masks_next,
                         int n_actions, float* critic_obs_next, int critic_obs_dim, void* stream);
+/* orl_host_insert_rnn for masks of n_actions in 1..64, the widths of a GRU policy's wide head (9..64 actions) included;
+ * the same kernel, so for 1..8 actions it writes what orl_host_insert_rnn writes. */
+int orl_host_insert_rnn_wide(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
+                             float* masks_next, float* active_masks_next, float* rnn_states_next, float* action_masks_next,
+                             int n_actions, float* critic_obs_next, int critic_obs_dim, void* stream);
 /* recurrent critic over slots 0..T: value_preds[t] and rnn_states_critic[t+1] */
 int orl_rnn_critic(const OrlRnnArgs* args, void* stream);
 /* chunked BPTT forward + loss + backward of both nets over the minibatch chunks -> grads, loss_acc */

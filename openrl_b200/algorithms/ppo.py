@@ -91,6 +91,8 @@ class PPOAlgorithm:
             raise NotImplementedError("use_joint_action_loss (JRPO) is built for the chunked recurrent update: it needs "
                                       "use_recurrent_policy and is not built with use_share_model or the feed-forward / "
                                       "naive-recurrent generators")
+        if self.joint_action and self.n > 8:
+            raise NotImplementedError("use_joint_action_loss (JRPO) is built for Discrete action spaces of up to 8 actions")
         if self.recurrent:
             if self.head_kind != lib.HEAD_CATEGORICAL:
                 raise NotImplementedError("recurrent policies are built for Discrete action spaces")
@@ -249,7 +251,7 @@ class PPOAlgorithm:
         mbc = data_chunks // self.num_mini_batch
         rows = mbc * L
         tape_rows = rows * buf.num_agents if joint else rows   # the joint policy tapes every agent row of a step
-        need = int(self._lib.orl_rnn_workspace_floats(tape_rows, self.rnn_stride))   # tape rows + reduction partials
+        need = int(self._lib.orl_rnn_workspace_floats_for(tape_rows, self.rnn_stride, self.n))   # tape rows + reduction partials
         if self.tape is None or self.tape.numel() < need:
             self.tape = torch.empty(need, dtype=torch.float32, device=self.device)
         whole = self.num_mini_batch == 1 and rows == total and not joint

@@ -66,6 +66,10 @@ FLAGS = [
     # other.  Pays off when env.step is slow relative to the per-step launch cost (MuJoCo-class); for cheap host envs the
     # doubled launch count costs more than the overlap hides (bench extras, c5: 54 ms vs 44 ms per iteration), so off by default
     ("host_env_groups", _bool, False),
+    # GRU policies (use_recurrent_policy / use_naive_recurrent_policy) with Discrete action spaces of 9..64 actions: the
+    # 64-wide head of the GRU act and update kernels.  Off, a GRU policy keeps its limit of 8 actions (NotImplementedError
+    # above); heads of up to 8 actions run the same kernels either way
+    ("use_wide_recurrent_head", _bool, False),
     ("use_tf32", _bool, True),
 ]
 

@@ -29,7 +29,7 @@ using namespace orl;
 namespace rc = orl_rnn;
 namespace rw = orl_rnnw;
 
-static_assert(rc::MAXN == MAX_OUT, "head width limits must agree");
+static_assert(rc::MAXN == MAX_OUT && rw::MAXN == MAX_OUT && rw::MAXN_WIDE == MAX_OUT_WIDE, "head width limits must agree");
 constexpr int LMAX = 32;     // data_chunk_length limit accepted by the host API (the chunk kernels loop over l; the tape is n_chunks * L rows)
 constexpr int JOINT_A = 3;   // agents of the joint-action update (simple_spread, the multi-agent device env)
 
@@ -96,25 +96,67 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_rollout_warp_kernel(const OrlRnnA
     }
 }
 
+// ---- the wide head (NB = 64) of one row, on the lane-owned logits x of step_forward<R, 64> ----
+// sample_action of a wide row: the first-max mode when deterministic, else argmax(probs / q) with the first index winning
+// ties; q of action j is noise(j) (identical for a given j on every lane).  Returns the action on every lane.
+template <typename Noise>
+__device__ __forceinline__ int warp_sample_action(rw::V2 x, int n, const float* mask_row, bool deterministic, Noise&& noise,
+                                                  float& lp, int lane) {
+    const rw::WarpSoftmax sm = rw::warp_log_softmax(x, n, mask_row, lane);
+    rw::V2 v{sm.in_a ? sm.pr(x.a) : 0.f, sm.in_b ? sm.pr(x.b) : 0.f};
+    if (!deterministic) {
+        if (sm.in_a) v.a = v.a / noise(lane);
+        if (sm.in_b) v.b = v.b / noise(lane + 32);
+    }
+    const int act = rw::warp_argmax(v, sm.in_a, sm.in_b, lane);
+    lp = sm.nl(rw::warp_pick(x, act));
+    return act;
+}
+// Exp(1) noise of action j of a wide row: draw j % 4 of wide_action_noise4 (Philox lanes 0, 1 for actions 0..7, 8..21 beyond)
+__device__ __forceinline__ float wide_action_noise1(const float* exp_noise, size_t grow, int n, uint64_t seed, uint64_t step,
+                                                    uint32_t row, int j) {
+    float q[4];
+    wide_action_noise4(exp_noise, grow, n, seed, step, row, j & ~3, q);
+    const int c = j & 3;
+    return c == 0 ? q[0] : c == 1 ? q[1] : c == 2 ? q[2] : q[3];
+}
+// categorical_row of a wide row (the maths and masking of wide_categorical_row): masks x in place, then overwrites it with
+// dL/dlogits (0 for the masked-out actions and for j >= n)
+template <class Args>
+__device__ __forceinline__ CatRow warp_categorical_row(const Args& a, rw::V2& x, int n, const float* mask_row, int act, float old_lp,
+                                                       float adv, float wrow, int lane) {
+    const rw::WarpSoftmax sm = rw::warp_log_softmax(x, n, mask_row, lane);
+    const PgTerm pg = pg_term(sm.nl(rw::warp_pick(x, (act >= 0 && act < n) ? act : 0)), old_lp, adv, a.clip_param, a.flags,
+                              a.dual_clip_coeff);
+    const float pa = sm.pr(x.a), pb = sm.pr(x.b), nla = sm.nl(x.a), nlb = sm.nl(x.b);
+    const float ent = -warp_sum((sm.in_a ? pa * nla : 0.f) + (sm.in_b ? pb * nlb : 0.f));
+    const float dlp = pg.dlogp * wrow, went = a.entropy_coef * wrow;
+    x.a = sm.live_a ? dlp * ((lane == act ? 1.f : 0.f) - pa) + went * pa * (nla + ent) : 0.f;
+    x.b = sm.live_b ? dlp * ((lane + 32 == act ? 1.f : 0.f) - pb) + went * pb * (nlb + ent) : 0.f;
+    return CatRow{pg.loss, ent, pg.ratio};
+}
+
 // ---- act over host-stepped rows: rows [row_begin, row_end) of slot t = t_begin, R rows per warp ----
 // The host steps the env between two launches; this kernel writes actions[t], action_log_probs[t] and rnn_states[t+1]
 // (orl_host_insert_rnn zeroes the rows of the envs that finish at step t).  Same staged weights, step_forward and
 // sampler as rnn_rollout_warp_kernel: a row's state, logits and action depend neither on R nor on the warp that runs it.
-template <int R>
+// NB = 64: the wide head (9..64 actions), sampled by warp_sample_action with the noise keys of the feed-forward wide head.
+template <int R, int NB = MAX_OUT>
 __global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnnArgs a) {
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * a.n_agents, d = a.obs_dim, n = a.n_actions, t = a.t_begin;
     const rc::Offsets o = rc::rnn_offsets(d, n);
-    const rw::SmemNet W = rw::load_net(smem, a.policy_params, o, threadIdx.x, W_NT);
+    const rw::SmemNet W = rw::load_net<NB>(smem, a.policy_params, o, threadIdx.x, W_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* scr = smem + rw::smem_net_floats() + warp * R * rw::SCR;
+    float* scr = smem + rw::smem_net_floats<NB>() + warp * R * rw::SCR;
     const uint64_t step = a.rng_step_base + (a.rng_counter ? *a.rng_counter : 0ull);
     float* const no_tape[R] = {};
     const int rows = a.row_end - a.row_begin, groups = (rows + R - 1) / R;
     for (int g = blockIdx.x * W_WPC + warp; g < groups; g += gridDim.x * W_WPC) {
         rw::V2 x[R], h[R], hn[R];
-        float mk[R], logit[R][MAX_OUT];
+        float mk[R];
+        typename rw::HeadOut<NB>::type logit[R];
         int row[R];
 #pragma unroll
         for (int r = 0; r < R; ++r) {
@@ -125,10 +167,21 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnn
             h[r] = rw::ldv(a.rnn_states + grow * rc::H, lane);
             mk[r] = a.masks[grow];
         }
-        rw::step_forward<R>(W, scr, d, n, a.activation_id, x, h, mk, hn, logit, no_tape, lane);
+        rw::step_forward<R, NB>(W, scr, d, n, a.activation_id, x, h, mk, hn, logit, no_tape, lane);
 #pragma unroll
         for (int r = 0; r < R; ++r) {
-            if (g * R + r < rows) {
+            if constexpr (NB == MAX_OUT_WIDE) {
+                const size_t grow = (size_t)t * B + row[r];
+                float lp;
+                const int act = warp_sample_action(logit[r], n, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0,
+                                                   [&](int j) {
+                    return wide_action_noise1(a.exp_noise, (size_t)row[r], n, a.rng_seed, step, (uint32_t)(row[r] + a.rng_row_offset), j);
+                }, lp, lane);
+                if (g * R + r < rows) {
+                    if (lane == 0) { a.actions[grow] = (float)act; a.action_log_probs[grow] = lp; }
+                    rw::stv(a.rnn_states + (grow + B) * rc::H, lane, hn[r]);
+                }
+            } else if (g * R + r < rows) {
                 const size_t grow = (size_t)t * B + row[r];
                 float lp;
                 const int act = sample_action(logit[r], n, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0,
@@ -174,19 +227,21 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_critic_warp_kernel(const OrlRnnAr
 // ---- update: one warp per C_R chunks; L forward steps (tape), per-step loss, L backward steps ----
 // AGENT0 (the critic under ORL_PPO_JOINT_ACTION): chunks are recurrent_generator_v3 chunks over f = n*T + t and the
 // critic sees agent 0's row of every step only (to_single_np, ppo.py:222-224, 254-262), buffer row t*B + n*A.
-template <bool POLICY, bool AGENT0, int C_R, int C_NT>
+// NB = 64 (policy only): the wide head; dL/dlogits goes to the tape field TW_DLW of the wider tape rows (TAPE_WIDE).
+template <bool POLICY, bool AGENT0, int C_R, int C_NT, int NB = MAX_OUT>
 __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArgs a) {
-    constexpr int C_WPC = C_NT / 32;
+    static_assert(NB == MAX_OUT || POLICY, "the critic's head is one value");
+    constexpr int C_WPC = C_NT / 32, TW = NB == MAX_OUT ? rw::TAPE_W : rw::TAPE_WIDE;
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * a.n_agents, T = a.episode_length, L = a.chunk_length;
     const int d = POLICY ? a.obs_dim : a.critic_obs_dim, n = POLICY ? a.n_actions : 1;
     const float* obs = POLICY ? a.policy_obs : a.critic_obs;
     const float* states = POLICY ? a.rnn_states : a.rnn_states_critic;
     const rc::Offsets o = rc::rnn_offsets(d, n);
-    const rw::SmemNet W = rw::load_net(smem, POLICY ? a.policy_params : a.critic_params, o, threadIdx.x, C_NT);
+    const rw::SmemNet W = rw::load_net<NB>(smem, POLICY ? a.policy_params : a.critic_params, o, threadIdx.x, C_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* scr = smem + rw::smem_net_floats() + warp * C_R * rw::SCR;
+    float* scr = smem + rw::smem_net_floats<NB>() + warp * C_R * rw::SCR;
     float loss0 = 0.f, loss1 = 0.f, loss2 = 0.f;   // identical on every lane; lane 0's copy is reduced
 
     const MbConsts mb = mb_consts(a);
@@ -207,7 +262,8 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
         }
         for (int l = 0; l < L; ++l) {
             rw::V2 x[C_R], h2[C_R];
-            float mk[C_R], out[C_R][MAX_OUT];
+            float mk[C_R];
+            typename rw::HeadOut<NB>::type out[C_R];
             float* tape[C_R];
             size_t bi[C_R];
 #pragma unroll
@@ -217,35 +273,45 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
                 const float* ob = obs + bi[r] * d;
                 x[r] = rw::V2{lane < d ? ob[lane] : 0.f, lane + 32 < d ? ob[lane + 32] : 0.f};
                 mk[r] = a.masks[bi[r]];
-                tape[r] = a.tape + ((size_t)cpos[r] * L + l) * rw::TAPE_W;
+                tape[r] = a.tape + ((size_t)cpos[r] * L + l) * TW;
             }
-            rw::step_forward<C_R>(W, scr, d, n, a.activation_id, x, h, mk, h2, out, tape, lane);
+            rw::step_forward<C_R, NB>(W, scr, d, n, a.activation_id, x, h, mk, h2, out, tape, lane);
 #pragma unroll
             for (int r = 0; r < C_R; ++r) {
                 h[r] = h2[r];
-                float dl[MAX_OUT];
-#pragma unroll
-                for (int j = 0; j < MAX_OUT; ++j) dl[j] = 0.f;
-                const float active = a.active_masks[bi[r]];
-                const float keep = valid[r] ? 1.f : 0.f;
-                if (POLICY) {
-                    const float wrow = mb.weight(pol_masks, active);
-                    const CatRow c = categorical_row(a, out[r], n, a.action_masks ? a.action_masks + bi[r] * n : nullptr,
-                                                     (int)a.actions[bi[r]], a.action_log_probs[bi[r]],
-                                                     apply_adv_norm(mb.adv, a.advantages[bi[r]]), wrow, dl);
+                if constexpr (NB == MAX_OUT_WIDE) {
+                    const float keep = valid[r] ? 1.f : 0.f;
+                    const float wrow = mb.weight(pol_masks, a.active_masks[bi[r]]);
+                    const CatRow c = warp_categorical_row(a, out[r], n, a.action_masks ? a.action_masks + bi[r] * n : nullptr,
+                                                          (int)a.actions[bi[r]], a.action_log_probs[bi[r]],
+                                                          apply_adv_norm(mb.adv, a.advantages[bi[r]]), wrow, lane);
                     loss0 += keep * c.loss * wrow; loss1 += keep * c.ent * wrow; loss2 += keep * c.ratio;
+                    rw::stv(tape[r] + rw::TW_DLW, lane, out[r]);
                 } else {
-                    const float ret = a.returns[bi[r]];
-                    const float target = (a.flags & ORL_PPO_VALUENORM) ? (ret - mb.vn_mean) / mb.vn_std : ret;
-                    const ValueTerm vt = value_term(out[r][0], a.value_preds[bi[r]], target, a.clip_param, a.huber_delta, a.flags);
-                    const float wrow = mb.weight(val_masks, active);
-                    loss0 += keep * vt.loss * wrow;
-                    dl[0] = a.value_loss_coef * wrow * vt.dv;
-                }
-                float mine = 0.f;   // lane m < 8 stores dL/dout[m]
+                    float dl[MAX_OUT];
 #pragma unroll
-                for (int j = 0; j < MAX_OUT; ++j) if (lane == j) mine = dl[j];
-                if (lane < MAX_OUT) tape[r][rc::TP_DLOG + lane] = mine;
+                    for (int j = 0; j < MAX_OUT; ++j) dl[j] = 0.f;
+                    const float active = a.active_masks[bi[r]];
+                    const float keep = valid[r] ? 1.f : 0.f;
+                    if (POLICY) {
+                        const float wrow = mb.weight(pol_masks, active);
+                        const CatRow c = categorical_row(a, out[r], n, a.action_masks ? a.action_masks + bi[r] * n : nullptr,
+                                                         (int)a.actions[bi[r]], a.action_log_probs[bi[r]],
+                                                         apply_adv_norm(mb.adv, a.advantages[bi[r]]), wrow, dl);
+                        loss0 += keep * c.loss * wrow; loss1 += keep * c.ent * wrow; loss2 += keep * c.ratio;
+                    } else {
+                        const float ret = a.returns[bi[r]];
+                        const float target = (a.flags & ORL_PPO_VALUENORM) ? (ret - mb.vn_mean) / mb.vn_std : ret;
+                        const ValueTerm vt = value_term(out[r][0], a.value_preds[bi[r]], target, a.clip_param, a.huber_delta, a.flags);
+                        const float wrow = mb.weight(val_masks, active);
+                        loss0 += keep * vt.loss * wrow;
+                        dl[0] = a.value_loss_coef * wrow * vt.dv;
+                    }
+                    float mine = 0.f;   // lane m < 8 stores dL/dout[m]
+#pragma unroll
+                    for (int j = 0; j < MAX_OUT; ++j) if (lane == j) mine = dl[j];
+                    if (lane < MAX_OUT) tape[r][rc::TP_DLOG + lane] = mine;
+                }
             }
         }
         __syncwarp();   // tape scalars (lane 0) and dL/dout (lanes < 8) are read by every lane below
@@ -255,8 +321,8 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
         for (int l = L - 1; l >= 0; --l) {
             float* tape[C_R];
 #pragma unroll
-            for (int r = 0; r < C_R; ++r) tape[r] = a.tape + ((size_t)cpos[r] * L + l) * rw::TAPE_W;
-            rw::step_backward<C_R>(W, scr, n, a.activation_id, tape, dh, lane);
+            for (int r = 0; r < C_R; ++r) tape[r] = a.tape + ((size_t)cpos[r] * L + l) * TW;
+            rw::step_backward<C_R, NB>(W, scr, n, a.activation_id, tape, dh, lane);
         }
     }
     __shared__ float red[3][C_WPC];
@@ -366,6 +432,7 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_joint_policy_warp_kernel(const Or
 }
 
 // ---- parameter gradients of one net from its tape (orl::reduce_tape); every job fits the gemm tiles: TQ_X + 64 <= TAPE_W ----
+// A wide head (n > 8) reads dL/dlogits from the appended field TW_DLW of its TAPE_WIDE rows.
 TapeJobs make_jobs(int d, int n) {
     const rc::Offsets o = rc::rnn_offsets(d, n);
     TapeJobs t; int g = 0, c = 0;
@@ -378,13 +445,14 @@ TapeJobs make_jobs(int d, int n) {
     gemm(rc::TP_DGI, rc::G3, rc::TQ_Y3, rc::H, o.wih); gemm(rc::TP_DGH, rc::G3, rc::TQ_HM, rc::H, o.whh);
     col(rc::TP_DGI, rc::G3, o.bih);                  col(rc::TP_DGH, rc::G3, o.bhh);
     col(rc::TS_DONO, rc::H, o.gr);                   col(rc::TS_DO, rc::H, o.ber);
-    gemm(rc::TP_DLOG, n, rc::TQ_O, rc::H, o.wh);     col(rc::TP_DLOG, n, o.bh);
+    const int dlog = n > MAX_OUT ? rw::TW_DLW : rc::TP_DLOG;
+    gemm(dlog, n, rc::TQ_O, rc::H, o.wh);            col(dlog, n, o.bh);
     t.n_gemm = g; t.n_col = c;
     return t;
 }
 
-// workspace = tape (rows x TAPE_W) followed by the reduction partials (row blocks x grads_stride)
-long long ws_tape_floats(long long rows) { return rows * rw::TAPE_W; }
+// workspace = tape (rows x tape_width(n_actions)) followed by the reduction partials (row blocks x grads_stride)
+long long ws_tape_floats(long long rows, int n_actions) { return rows * rw::tape_width(n_actions); }
 
 // ---- optimizer: per-net global-norm clip + Adam on the true-layout gradients (one CTA per net) ----
 __global__ void __launch_bounds__(1024) rnn_apply_kernel(const OrlRnnArgs a) {
@@ -402,9 +470,11 @@ __global__ void __launch_bounds__(1024) rnn_apply_kernel(const OrlRnnArgs a) {
     }
 }
 
+template <int NB = MAX_OUT>
 constexpr size_t w_smem(int rows_per_warp) {   // weights of one net + the per-warp mat-vec scratch
-    return (size_t)(rw::smem_net_floats() + rw::smem_scratch_floats(W_WPC, rows_per_warp)) * sizeof(float);
+    return (size_t)(rw::smem_net_floats<NB>() + rw::smem_scratch_floats(W_WPC, rows_per_warp)) * sizeof(float);
 }
+static_assert(w_smem<MAX_OUT_WIDE>(2) <= 227 * 1024, "the wide policy's weights and scratch fit the opt-in shared memory");
 int warp_grid(long long units) {   // persistent CTAs: one per SM, never more than the work needs
     const long long need = (units + W_WPC - 1) / W_WPC;
     return (int)std::max(1LL, std::min<long long>(need, orl::sm_count()));
@@ -413,7 +483,7 @@ int warp_grid(long long units) {   // persistent CTAs: one per SM, never more th
 int check_common(const OrlRnnArgs& a) {
     ORL_CHECK_ARG(a.n_envs > 0 && a.n_agents > 0 && a.episode_length > 0, "n_envs / n_agents / episode_length");
     ORL_CHECK_ARG(a.obs_dim > 0 && a.obs_dim <= rc::MAXD && a.critic_obs_dim > 0 && a.critic_obs_dim <= rc::MAXD, "obs dims (<= 64)");
-    ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= MAX_OUT, "n_actions (<= 8)");
+    ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= MAX_OUT_WIDE, "n_actions must be in 1..64");
     ORL_CHECK_ARG(a.activation_id >= 0 && a.activation_id <= 3, "activation_id");
     return 0;
 }
@@ -424,8 +494,9 @@ extern "C" {
 
 int orl_rnn_param_count(int obs_dim, int n_out) { return rc::rnn_offsets(obs_dim, n_out).total; }
 int orl_rnn_tape_width(void) { return rw::TAPE_W; }
-long long orl_rnn_workspace_floats(long long rows, int grads_stride) {
-    return ws_tape_floats(rows) + (rows + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK * grads_stride;
+long long orl_rnn_workspace_floats(long long rows, int grads_stride) { return orl_rnn_workspace_floats_for(rows, grads_stride, 1); }
+long long orl_rnn_workspace_floats_for(long long rows, int grads_stride, int n_actions) {
+    return ws_tape_floats(rows, n_actions) + (rows + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK * grads_stride;
 }
 
 int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
@@ -433,6 +504,7 @@ int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
     const OrlRnnArgs& a = *ap;
     if (int e = check_common(a)) return e;
     ORL_CHECK_ARG(a.env_kind != ORL_ENV_NONE, "ORL_ENV_NONE: the act of host-stepped rows is orl_rnn_act_rows");
+    ORL_CHECK_ARG(a.n_actions <= MAX_OUT, "n_actions must be in 1..8 for the device envs (they have at most 5 actions)");
     ORL_CHECK_ARG(a.policy_params && a.policy_obs && a.rnn_states && a.actions && a.action_log_probs && a.masks, "null rollout buffer");
     ORL_CHECK_ARG(a.t_begin >= 0 && a.t_end <= a.episode_length && a.t_begin <= a.t_end, "t range");
     ORL_CHECK_ARG(a.critic_obs && a.rewards && a.active_masks, "null rollout buffer");
@@ -478,7 +550,15 @@ int orl_rnn_act_rows(const OrlRnnArgs* ap, void* stream) {
     if (rows > 0) {
         // one row per warp while the rows leave warps of the persistent grid idle, two (every weight read feeds both) beyond
         int e = 0;
-        if (rows <= orl::sm_count() * W_WPC) {
+        if (a.n_actions > MAX_OUT) {   // the wide head: same row grouping
+            if (rows <= orl::sm_count() * W_WPC) {
+                if ((e = orl::allow_dynamic_smem(rnn_act_rows_warp_kernel<1, MAX_OUT_WIDE>, w_smem<MAX_OUT_WIDE>(1)))) return e;
+                rnn_act_rows_warp_kernel<1, MAX_OUT_WIDE><<<warp_grid(rows), W_NT, w_smem<MAX_OUT_WIDE>(1), st>>>(a);
+            } else {
+                if ((e = orl::allow_dynamic_smem(rnn_act_rows_warp_kernel<2, MAX_OUT_WIDE>, w_smem<MAX_OUT_WIDE>(2)))) return e;
+                rnn_act_rows_warp_kernel<2, MAX_OUT_WIDE><<<warp_grid((rows + 1) / 2), W_NT, w_smem<MAX_OUT_WIDE>(2), st>>>(a);
+            }
+        } else if (rows <= orl::sm_count() * W_WPC) {
             if ((e = orl::allow_dynamic_smem(rnn_act_rows_warp_kernel<1>, w_smem(1)))) return e;
             rnn_act_rows_warp_kernel<1><<<warp_grid(rows), W_NT, w_smem(1), st>>>(a);
         } else {
@@ -520,19 +600,24 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
         ORL_CHECK_ARG(a.n_agents == JOINT_A, "ORL_PPO_JOINT_ACTION is built for 3 agents (simple_spread)");
         ORL_CHECK_ARG(a.n_chunks * a.chunk_length <= (long long)a.n_envs * a.episode_length, "v3 chunks exceed the N*T samples");
         ORL_CHECK_ARG(!a.action_masks, "ORL_PPO_JOINT_ACTION takes no action_masks (simple_spread reports none)");
+        ORL_CHECK_ARG(a.n_actions <= MAX_OUT, "ORL_PPO_JOINT_ACTION is built for up to 8 actions");
     }
+    const bool wide = a.n_actions > MAX_OUT;
     cudaStream_t st = (cudaStream_t)stream;
     int e = orl::check_cuda(cudaMemsetAsync(a.loss_acc, 0, 8 * sizeof(float), st), "memset loss_acc");
     if (e) return e;
     const long long steps = a.n_chunks * a.chunk_length;
     const long long net_rows[2] = {joint ? steps * JOINT_A : steps, steps};
-    float* partials = a.tape + ws_tape_floats(net_rows[0]);   // the policy's tape is the larger one
+    float* partials = a.tape + ws_tape_floats(net_rows[0], a.n_actions);   // the policy's tape is the larger one
     // two chunks per warp: every weight read from shared memory feeds two rows
     constexpr int C_R = 2;
     const int cgrid = warp_grid((a.n_chunks + C_R - 1) / C_R);
     if (joint) {
         if ((e = orl::allow_dynamic_smem(rnn_joint_policy_warp_kernel<JOINT_A, W_NT>, w_smem(JOINT_A)))) return e;
         if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<false, true, C_R, W_NT>, w_smem(C_R)))) return e;
+    } else if (wide) {
+        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<true, false, C_R, W_NT, MAX_OUT_WIDE>, w_smem<MAX_OUT_WIDE>(C_R)))) return e;
+        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<false, false, C_R, W_NT>, w_smem(C_R)))) return e;
     } else {
         if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<true, false, C_R, W_NT>, w_smem(C_R)))) return e;
         if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<false, false, C_R, W_NT>, w_smem(C_R)))) return e;
@@ -540,10 +625,12 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
     for (int net = 0; net < 2; ++net) {
         const int d = net == 0 ? a.obs_dim : a.critic_obs_dim, n = net == 0 ? a.n_actions : 1;
         if (net == 0 && joint) rnn_joint_policy_warp_kernel<JOINT_A, W_NT><<<warp_grid(a.n_chunks), W_NT, w_smem(JOINT_A), st>>>(a);
+        else if (net == 0 && wide)
+            rnn_chunk_warp_kernel<true, false, C_R, W_NT, MAX_OUT_WIDE><<<cgrid, W_NT, w_smem<MAX_OUT_WIDE>(C_R), st>>>(a);
         else if (net == 0) rnn_chunk_warp_kernel<true, false, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
         else if (joint) rnn_chunk_warp_kernel<false, true, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
         else rnn_chunk_warp_kernel<false, false, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
-        if ((e = orl::reduce_tape(a.tape, rw::TAPE_W, net_rows[net], make_jobs(d, n), partials, a.grads_stride,
+        if ((e = orl::reduce_tape(a.tape, rw::tape_width(n), net_rows[net], make_jobs(d, n), partials, a.grads_stride,
                                   rc::rnn_offsets(d, n).total, a.grads + (size_t)net * a.grads_stride, st))) return e;
     }
     return orl::check_cuda(cudaGetLastError(), "rnn update launches");

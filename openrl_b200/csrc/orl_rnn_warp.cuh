@@ -13,7 +13,13 @@
 //
 // Tape row (floats): [0,1224) the P / Q / S fields of orl_rnn_core.h (inputs of the dW = sum P^T Q
 // reductions), then the forward activations the backward step re-reads: A1 N1 N3 R Z NN GHN NO (64 each)
-// and 8 scalars (rstd1, rstd3, rstd_rnn, mask, -).
+// and 8 scalars (rstd1, rstd3, rstd_rnn, mask, -).  A wide policy head (9..64 actions, NB = 64) appends dL/dlogits as
+// a 64-vector at [TAPE_W, TAPE_WIDE); the 8-wide TP_DLOG field is left unused there.
+//
+// Head width bound NB (a template parameter): NB = 8 (MAXN) stages an 8-row head block and reduces each logit with a
+// warp_sum into out[R][8] on every lane.  NB = 64 (MAXN_WIDE) treats the logits as one more lane-owned 64-vector
+// (lane l owns actions l and l + 32): matvec64 over a 64-row head block whose rows >= n and bias entries >= n are zero.
+// Per-lane arrays of 64 logits would spill under the 128-register cap of the 512-thread kernels.
 #pragma once
 #include "orl_mlp.cuh"
 #include "orl_rnn_core.h"
@@ -22,9 +28,12 @@ namespace orl_rnnw {
 using orl::warp_sum;
 namespace rc = orl_rnn;
 
-constexpr int H = 64, G3 = 192, LD = 65, MAXN = 8;
+constexpr int H = 64, G3 = 192, LD = 65, MAXN = 8, MAXN_WIDE = 64;
 constexpr int TW_A1 = rc::TAPE, TW_N1 = TW_A1 + 64, TW_N3 = TW_N1 + 64, TW_R = TW_N3 + 64, TW_Z = TW_R + 64, TW_NN = TW_Z + 64,
               TW_GHN = TW_NN + 64, TW_NO = TW_GHN + 64, TW_SC = TW_NO + 64, TAPE_W = TW_SC + 8;   // 1744
+constexpr int TW_DLW = TAPE_W, TAPE_WIDE = TW_DLW + 64;   // 1808: the wide policy head's dL/dlogits (P operand of Wh, bh)
+__host__ __device__ constexpr int head_bound(int n) { return n > MAXN ? MAXN_WIDE : MAXN; }
+__host__ __device__ constexpr int tape_width(int n) { return n > MAXN ? TAPE_WIDE : TAPE_W; }
 
 struct V2 { float a, b; };
 
@@ -32,16 +41,19 @@ struct SmemNet {
     const float *w1, *w3, *wih, *whh, *wh;                                  // [rows][LD]
     const float *b1, *g1, *be1, *b3, *g3, *be3, *bih, *bhh, *gr, *ber, *bh;  // vectors
 };
-__host__ __device__ constexpr int smem_net_floats() { return (H + H + G3 + G3 + MAXN) * LD + 8 * H + 2 * G3 + MAXN; }
+template <int NB = MAXN>
+__host__ __device__ constexpr int smem_net_floats() { return (H + H + G3 + G3 + NB) * LD + 8 * H + 2 * G3 + NB; }
 
 // Stage one net (flat layout of rc::rnn_offsets) into shared memory; W1 columns k >= d and head rows m >= n are zero.
+template <int NB = MAXN>
 __device__ inline SmemNet load_net(float* s, const float* __restrict__ P, const rc::Offsets& o, int tid, int nthreads) {
+    static_assert(NB == MAXN || NB == MAXN_WIDE, "head width bound");
     float* w1 = s; s += H * LD;
     float* w3 = s; s += H * LD;
     float* wih = s; s += G3 * LD;
     float* whh = s; s += G3 * LD;
-    float* wh = s; s += MAXN * LD;
-    float* vec = s;   // b1 g1 be1 b3 g3 be3 gr ber (64 each) | bih bhh (192 each) | bh (8)
+    float* wh = s; s += NB * LD;
+    float* vec = s;   // b1 g1 be1 b3 g3 be3 gr ber (64 each) | bih bhh (192 each) | bh (NB)
     for (int i = tid; i < H * LD; i += nthreads) {
         const int j = i / LD, k = i % LD;
         w1[i] = k < o.d ? P[o.w1 + j * o.d + k] : 0.f;
@@ -52,7 +64,7 @@ __device__ inline SmemNet load_net(float* s, const float* __restrict__ P, const 
         wih[i] = k < H ? P[o.wih + j * H + k] : 0.f;
         whh[i] = k < H ? P[o.whh + j * H + k] : 0.f;
     }
-    for (int i = tid; i < MAXN * LD; i += nthreads) {
+    for (int i = tid; i < NB * LD; i += nthreads) {
         const int j = i / LD, k = i % LD;
         wh[i] = (j < o.n && k < H) ? P[o.wh + j * H + k] : 0.f;
     }
@@ -62,7 +74,7 @@ __device__ inline SmemNet load_net(float* s, const float* __restrict__ P, const 
         vec[6 * H + i] = P[o.gr + i]; vec[7 * H + i] = P[o.ber + i];
     }
     for (int i = tid; i < G3; i += nthreads) { vec[8 * H + i] = P[o.bih + i]; vec[8 * H + G3 + i] = P[o.bhh + i]; }
-    for (int i = tid; i < MAXN; i += nthreads) vec[8 * H + 2 * G3 + i] = i < o.n ? P[o.bh + i] : 0.f;
+    for (int i = tid; i < NB; i += nthreads) vec[8 * H + 2 * G3 + i] = i < o.n ? P[o.bh + i] : 0.f;
     SmemNet n;
     n.w1 = w1; n.w3 = w3; n.wih = wih; n.whh = whh; n.wh = wh;
     n.b1 = vec; n.g1 = vec + H; n.be1 = vec + 2 * H; n.b3 = vec + 3 * H; n.g3 = vec + 4 * H; n.be3 = vec + 5 * H;
@@ -151,13 +163,63 @@ __device__ __forceinline__ void matvecT(const float* W, const float* scr, int of
 
 __device__ __forceinline__ float sigm(float x) { return 1.f / (1.f + expf(-x)); }
 
-// One forward step of R rows.  x: observation (zero beyond d), h_in: hidden state, out[r][m] valid for m < n on
-// every lane.  tape[r] != nullptr: the Q operands and the activations for the backward step go to the row's tape.
+// ---- the wide head's row reductions over lane-owned logits (lane l: action l in .a, action l + 32 in .b) ----
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+// x_j of one action j (the same j on every lane), on every lane
+__device__ __forceinline__ float warp_pick(V2 x, int j) { return __shfl_sync(0xffffffffu, j < 32 ? x.a : x.b, j & 31); }
+// index of the first maximum of the lane-owned values over the actions marked ok (action 0 always is), on every lane
+__device__ __forceinline__ int warp_argmax(V2 v, bool ok_a, bool ok_b, int lane) {
+    float bv = ok_a ? v.a : -INFINITY;
+    int bi = lane;
+    if (ok_b && v.b > bv) { bv = v.b; bi = lane + 32; }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+    }
+    return bi;
+}
+// log-softmax of the logits of actions 0..n-1, masked in place (-6e4 where mask_row[j] == 0), the maths of
+// log_softmax_n with the max and the sums as warp reductions: lse = mx + log sum exp(x - mx), mx2 = mx - lse (the max of
+// the rounded x - lse, rounding being monotone), p = exp(x - lse - mx2) / s2.  Actions j >= n take no part.
+struct WarpSoftmax {
+    float lse, mx2, s2;
+    bool in_a, in_b;       // this lane's actions are < n
+    bool live_a, live_b;   // ... and legal
+    __device__ __forceinline__ float nl(float x) const { return x - lse; }
+    __device__ __forceinline__ float pr(float x) const { return expf(x - lse - mx2) / s2; }
+};
+__device__ __forceinline__ WarpSoftmax warp_log_softmax(V2& x, int n, const float* mask_row, int lane) {
+    WarpSoftmax r;
+    r.in_a = lane < n; r.in_b = lane + 32 < n;
+    r.live_a = r.in_a; r.live_b = r.in_b;
+    if (mask_row) {
+        if (r.in_a && mask_row[lane] == 0.f) { x.a = -6e4f; r.live_a = false; }
+        if (r.in_b && mask_row[lane + 32] == 0.f) { x.b = -6e4f; r.live_b = false; }
+    }
+    const float mx = warp_max(fmaxf(r.in_a ? x.a : -INFINITY, r.in_b ? x.b : -INFINITY));
+    r.lse = mx + logf(warp_sum((r.in_a ? expf(x.a - mx) : 0.f) + (r.in_b ? expf(x.b - mx) : 0.f)));
+    r.mx2 = mx - r.lse;
+    r.s2 = warp_sum((r.in_a ? expf(x.a - r.lse - r.mx2) : 0.f) + (r.in_b ? expf(x.b - r.lse - r.mx2) : 0.f));
+    return r;
+}
+
+// head outputs of one row: NB = 8, out[m] for m < n on every lane; NB = 64, the lane-owned logits
+template <int NB> struct HeadOut { using type = float[MAXN]; };
+template <> struct HeadOut<MAXN_WIDE> { using type = V2; };
+
+// One forward step of R rows.  x: observation (zero beyond d), h_in: hidden state, out[r]: the head outputs (HeadOut).
+// tape[r] != nullptr: the Q operands and the activations for the backward step go to the row's tape.
 // scr: this warp's scratch (R * SCR floats of shared memory).
-template <int R>
+template <int R, int NB = MAXN>
 __device__ __forceinline__ void step_forward(const SmemNet& W, float* scr, int d, int n, int act_id, const V2 (&x)[R], const V2 (&h_in)[R],
-                                             const float (&mask)[R], V2 (&h_out)[R], float (&out)[R][MAXN], float* const (&tape)[R],
-                                             int lane) {
+                                             const float (&mask)[R], V2 (&h_out)[R], typename HeadOut<NB>::type (&out)[R],
+                                             float* const (&tape)[R], int lane) {
     const V2 g1 = ldv(W.g1, lane), be1 = ldv(W.be1, lane), g3 = ldv(W.g3, lane), be3 = ldv(W.be3, lane);
     V2 t0[R], y1[R], y3[R], hm[R];
     park<R>(scr, 0, x, lane);
@@ -193,6 +255,7 @@ __device__ __forceinline__ void step_forward(const SmemNet& W, float* scr, int d
     park<R>(scr, 0, hm, lane);
     matvec192<R>(W.whh, W.bhh, scr, 0, lane, gh);
     const V2 gr = ldv(W.gr, lane), ber = ldv(W.ber, lane);
+    [[maybe_unused]] V2 ov[R];
 #pragma unroll
     for (int r = 0; r < R; ++r) {
         const V2 rg{sigm(gi[0][r].a + gh[0][r].a), sigm(gi[0][r].b + gh[0][r].b)};
@@ -202,10 +265,14 @@ __device__ __forceinline__ void step_forward(const SmemNet& W, float* scr, int d
         float rstdr;
         const V2 no = ln_fwd(h_out[r], rstdr);
         const V2 o{fmaf(no.a, gr.a, ber.a), fmaf(no.b, gr.b, ber.b)};
+        if constexpr (NB == MAXN) {
 #pragma unroll
-        for (int m = 0; m < MAXN; ++m) {
-            out[r][m] = 0.f;
-            if (m < n) out[r][m] = W.bh[m] + warp_sum(fmaf(W.wh[m * LD + lane], o.a, W.wh[m * LD + 32 + lane] * o.b));
+            for (int m = 0; m < MAXN; ++m) {
+                out[r][m] = 0.f;
+                if (m < n) out[r][m] = W.bh[m] + warp_sum(fmaf(W.wh[m * LD + lane], o.a, W.wh[m * LD + 32 + lane] * o.b));
+            }
+        } else {
+            ov[r] = o;
         }
         if (tape[r]) {
             stv(tape[r] + rc::TQ_O, lane, o); stv(tape[r] + TW_R, lane, rg); stv(tape[r] + TW_Z, lane, z);
@@ -213,27 +280,46 @@ __device__ __forceinline__ void step_forward(const SmemNet& W, float* scr, int d
             if (lane == 0) tape[r][TW_SC + 2] = rstdr;
         }
     }
+    if constexpr (NB == MAXN_WIDE) {   // logits = bh + Wh o over the 64-row head block (zero rows and bias beyond n)
+        park<R>(scr, 0, ov, lane);
+        matvec64<R>(W.wh, W.bh, scr, 0, H, lane, out);
+    }
 }
 
-// Backward of one step of R rows from their tape rows (written by step_forward; dL/dout in TP_DLOG).  dh holds
-// dL/dh_out arriving from the following step on entry and dL/dh_in (already multiplied by the mask) on exit;
-// the P / S tape fields are written.
-template <int R>
+// Backward of one step of R rows from their tape rows (written by step_forward; dL/dout in TP_DLOG, or for NB = 64 the
+// lane-owned 64-vector at TW_DLW, zero beyond n).  dh holds dL/dh_out arriving from the following step on entry and
+// dL/dh_in (already multiplied by the mask) on exit; the P / S tape fields are written.
+template <int R, int NB = MAXN>
 __device__ __forceinline__ void step_backward(const SmemNet& W, float* scr, int n, int act_id, float* const (&tape)[R], V2 (&dh)[R], int lane) {
     const V2 gr = ldv(W.gr, lane), g3 = ldv(W.g3, lane), g1 = ldv(W.g1, lane);
     V2 dgi[3][R], dgh[3][R], dhm[R];
     float mask[R];
+    [[maybe_unused]] V2 dovw[R];
+    if constexpr (NB == MAXN_WIDE) {   // dL/do = Wh^T dL/dlogits over the pad4(n) head rows
+        V2 dl[R];
+#pragma unroll
+        for (int r = 0; r < R; ++r) dl[r] = ldv(tape[r] + TW_DLW, lane);
+        park<R>(scr, 0, dl, lane);
+        matvecT<R>(W.wh, scr, 0, (n + 3) & ~3, lane, dovw);
+    }
 #pragma unroll
     for (int r = 0; r < R; ++r) {
-        float dl[MAXN];
-#pragma unroll
-        for (int m = 0; m < MAXN; ++m) dl[m] = tape[r][rc::TP_DLOG + m];
-        const float rstdr = tape[r][TW_SC + 2];
-        mask[r] = tape[r][TW_SC + 3];
         V2 dov{0.f, 0.f};
+        float rstdr;
+        if constexpr (NB == MAXN) {
+            float dl[MAXN];
 #pragma unroll
-        for (int m = 0; m < MAXN; ++m)
-            if (m < n) { dov.a = fmaf(W.wh[m * LD + lane], dl[m], dov.a); dov.b = fmaf(W.wh[m * LD + 32 + lane], dl[m], dov.b); }
+            for (int m = 0; m < MAXN; ++m) dl[m] = tape[r][rc::TP_DLOG + m];
+            rstdr = tape[r][TW_SC + 2];
+            mask[r] = tape[r][TW_SC + 3];
+#pragma unroll
+            for (int m = 0; m < MAXN; ++m)
+                if (m < n) { dov.a = fmaf(W.wh[m * LD + lane], dl[m], dov.a); dov.b = fmaf(W.wh[m * LD + 32 + lane], dl[m], dov.b); }
+        } else {
+            rstdr = tape[r][TW_SC + 2];
+            mask[r] = tape[r][TW_SC + 3];
+            dov = dovw[r];
+        }
         const V2 no = ldv(tape[r] + TW_NO, lane);
         stv(tape[r] + rc::TS_DONO, lane, V2{dov.a * no.a, dov.b * no.b});
         stv(tape[r] + rc::TS_DO, lane, dov);

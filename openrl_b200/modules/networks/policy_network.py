@@ -28,12 +28,13 @@ class PolicyNetwork(nn.Module):
         self.n_actions = action_space.shape[0] if self.act.continuous_action else action_space.n  # head width
         if self.recurrent and self.act.continuous_action:
             raise NotImplementedError("recurrent policies are built for Discrete action spaces")
-        # a feed-forward Categorical head runs up to 64 actions (a logits tile in the kernels); the GRU policy's heads and
-        # the DiagGaussian heads keep the per-thread head of up to 8 outputs
+        # a feed-forward Categorical head runs up to 64 actions (a logits tile in the kernels); a GRU policy's head runs up
+        # to 64 with cfg.use_wide_recurrent_head (a lane-owned 64-vector in the GRU kernels) and up to 8 without; the
+        # DiagGaussian heads keep the per-thread head of up to 8 outputs
         if self.n_actions > 64:
             raise NotImplementedError("Discrete action spaces of up to 64 actions are built")
-        if self.n_actions > 8 and self.recurrent:
-            raise NotImplementedError("recurrent policies are built for up to 8 actions")
+        if self.n_actions > 8 and self.recurrent and not getattr(cfg, "use_wide_recurrent_head", False):
+            raise NotImplementedError("recurrent policies are built for up to 8 actions (9..64 with use_wide_recurrent_head)")
         if self.n_actions > 8 and self.act.continuous_action:
             raise NotImplementedError("DiagGaussian heads are built for Box action spaces of width up to 8")
         self.device = torch.device(device)
