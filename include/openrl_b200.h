@@ -139,7 +139,8 @@ typedef struct OrlRolloutArgs {
     int32_t n_agents;       /* A; rows B = N*A */
     int32_t episode_length; /* T: depth of the (T[+1], B, .) buffers */
     int32_t t_begin, t_end; /* steps to run, 0 <= t_begin < t_end <= T */
-    int32_t obs_dim;        /* d, policy observation width (<= 64) */
+    int32_t obs_dim;        /* d, policy observation width: 1..256 with ORL_ENV_NONE (host-stepped envs), 1..64
+                               otherwise; ORL_ERR_BAD_ARG outside */
     int32_t critic_obs_dim; /* 0: critic obs == policy obs (critic_obs may be NULL) */
     int32_t n_actions;      /* n: Discrete(n) 1..64 with ORL_ENV_NONE (host-stepped envs), 1..8 otherwise and for
                                DiagGaussian heads; ORL_ERR_BAD_ARG outside */
@@ -183,7 +184,7 @@ int orl_rollout(const OrlRolloutArgs* args, void* stream);
 /* ---- critic forward over a flat batch of rows ------------------------------------------
  * Replaces the critic half of act() (ValueNetwork.forward, value_network.py:113-136) for all
  * T+1 slots at once and the bootstrap forward of OnPolicyDriver.compute_returns
- * (onpolicy_driver.py:206-215).  obs (rows, d) -> values (rows). */
+ * (onpolicy_driver.py:206-215).  obs (rows, d) -> values (rows), d in 1..256 (ORL_ERR_BAD_ARG otherwise). */
 int orl_critic_values(const float* critic_params, int obs_dim, int activation_id,
                       const float* obs, float* values, long long rows, void* stream);
 
@@ -206,13 +207,18 @@ int orl_critic_values(const float* critic_params, int obs_dim, int activation_id
 int orl_host_insert(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
                     float* masks_next, float* active_masks_next, float* action_masks_next, int n_actions,
                     float* critic_obs_next, int critic_obs_dim, void* stream);
+/* orl_host_insert for critic sections of critic_obs_dim in 1..256, the widths of the feed-forward critic on host-stepped
+ * envs; the same kernel, so for 1..64 it writes what orl_host_insert writes. */
+int orl_host_insert_wide_obs(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
+                             float* masks_next, float* active_masks_next, float* action_masks_next, int n_actions,
+                             float* critic_obs_next, int critic_obs_dim, void* stream);
 
 /* ---- policy evaluation of given actions over a flat batch of rows ------------------------
  * Replaces PolicyNetwork.eval_actions (policy_network.py:164-203) -> ACTLayer.evaluate_actions (act.py:130-172), the
  * policy half of PPOModule.evaluate_actions (ppo_module.py:147-193), outside the fused update: obs (rows, d), actions
  * (rows) [Categorical: index as float32] or (rows, n) [DiagGaussian] -> log_probs and entropy with the shape of
  * `actions` (per row / per dimension; the caller takes the active-mask mean, act.py:160-168).  n_actions: 1..64 for
- * Categorical heads, 1..8 for DiagGaussian heads (ORL_ERR_BAD_ARG otherwise). */
+ * Categorical heads, 1..8 for DiagGaussian heads; obs_dim: 1..256 (ORL_ERR_BAD_ARG otherwise). */
 int orl_policy_eval(const float* policy_params, int obs_dim, int n_actions, int activation_id, int head_kind,
                     const float* obs, const float* actions, const float* action_masks, float* log_probs,
                     float* entropy, long long rows, void* stream);
@@ -256,8 +262,8 @@ int orl_policy_eval(const float* policy_params, int obs_dim, int n_actions, int 
                                          see orl_rnn_fwdbwd */
 
 typedef struct OrlPpoArgs {
-    int32_t obs_dim;         /* d  policy obs width  (<= 64) */
-    int32_t critic_obs_dim;  /* dc critic obs width  (<= 64) */
+    int32_t obs_dim;         /* d  policy obs width  1..256; 1..64 with ORL_PPO_TENSORCORE (ORL_ERR_BAD_ARG otherwise) */
+    int32_t critic_obs_dim;  /* dc critic obs width  1..256; 1..64 with ORL_PPO_TENSORCORE */
     int32_t n_actions;       /* n: 1..64 for Categorical heads, 1..8 for DiagGaussian heads and with ORL_PPO_TENSORCORE
                                 (ORL_ERR_BAD_ARG otherwise) */
     int32_t activation_id;

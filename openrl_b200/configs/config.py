@@ -70,6 +70,11 @@ FLAGS = [
     # 64-wide head of the GRU act and update kernels.  Off, a GRU policy keeps its limit of 8 actions (NotImplementedError
     # above); heads of up to 8 actions run the same kernels either way
     ("use_wide_recurrent_head", _bool, False),
+    # feed-forward policies and critics with observations of 65..256 features (the policy's, and the critic's of a Dict
+    # {"policy", "critic"} env), such as the centralised critic of a many-agent MAPPO env: fc1 as a loop over 64-wide
+    # panels of the observation in the act, value, eval and FFMA update kernels.  Off, every network keeps its limit of
+    # 64 features (NotImplementedError); GRU policies, use_share_model and the device envs keep it either way
+    ("use_wide_observations", _bool, False),
     ("use_tf32", _bool, True),
 ]
 

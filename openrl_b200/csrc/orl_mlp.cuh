@@ -29,6 +29,9 @@ constexpr int H = 64;     // hidden width (cfg.hidden_size), fixed in this build
 constexpr int LDA = 68;   // leading dimension of H-wide activation tiles in smem
 constexpr int MAX_OUT = 8;  // head width bound NB of the per-thread head code (head_dots, sample_action, categorical_row)
 constexpr int MAX_OUT_WIDE = 64;  // head width bound NB of the wide Categorical head: a logits tile in shared memory
+constexpr int OBS_PANEL = 64;     // observation columns per fc1 K-panel of a wide observation (fc1_panels)
+constexpr int LDX_PANEL = OBS_PANEL + 4;   // leading dimension of a staged observation panel
+constexpr int MAX_OBS_WIDE = 256; // observation width bound of the panelled fc1 (widths <= 64 stage all of W1 at once)
 constexpr float LN_EPS = 1e-5f;
 
 struct NetOffsets {
@@ -152,15 +155,18 @@ __device__ inline SmemWeights carve_weights(float*& p, int d, bool backward) {
 }
 
 // Stage + fold one net's parameters from the flat global buffer.  All threads of the CTA call it;
-// ends with __syncthreads().
-template <int NT, int NB = MAX_OUT>
+// ends with __syncthreads().  PANELS (d > 64): W1 is left out; fc1_panels stages it one panel at a time into a w1t
+// carved at d = 64.
+template <int NT, int NB = MAX_OUT, bool PANELS = false>
 __device__ inline void load_weights_folded(const SmemWeights& w, const float* __restrict__ params, int d, int n,
                                            bool backward) {
     const NetOffsets o = net_offsets(d, n);
     const int tid = threadIdx.x, dp = pad4(d);
-    for (int i = tid; i < dp * H; i += NT) {
-        const int k = i / H, j = i % H;
-        w.w1t[i] = (k < d) ? params[o.w1 + j * d + k] : 0.f;
+    if (!PANELS) {
+        for (int i = tid; i < dp * H; i += NT) {
+            const int k = i / H, j = i % H;
+            w.w1t[i] = (k < d) ? params[o.w1 + j * d + k] : 0.f;
+        }
     }
     for (int i = tid; i < H; i += NT) w.b1[i] = params[o.b1 + i];
     for (int i = tid; i < H * H; i += NT) {
@@ -287,24 +293,17 @@ __device__ __forceinline__ void load_tile(const float* __restrict__ S, float (&a
     }
 }
 
-// Trunk forward of one tile: Xs [M][ldx] (raw obs, zero padded to pad4(d)) -> N1s, N3s (normalised
-// activations).  Optionally returns the per-row statistics and the activation sign bits needed by
-// the backward pass.  Contains the __syncthreads() between the two layers; callers must sync
-// before reading N3s from other threads.
+// The trunk after fc1's GEMM: acc holds Z1 = b1 + X W1^T on entry; activation + LayerNorm -> N1s, fc3 + LayerNorm ->
+// N3s (normalised activations).  Optionally returns the per-row statistics and the activation sign bits needed by the
+// backward pass.  Contains the __syncthreads() between the two layers; callers must sync before reading N3s from other
+// threads.
 template <int M, int NT, bool KEEP>
-__device__ __forceinline__ void trunk_forward(const SmemWeights& w, const float* __restrict__ Xs, int ldx, int d,
-                                              int activation_id, float* __restrict__ N1s, float* __restrict__ N3s,
+__device__ __forceinline__ void trunk_from_z1(const SmemWeights& w, float (&acc)[M / (NT / 16)][4], int activation_id,
+                                              float* __restrict__ N1s, float* __restrict__ N3s,
                                               float (&mu1)[M / (NT / 16)], float (&rstd1)[M / (NT / 16)],
                                               float (&rstd3)[M / (NT / 16)], unsigned& posmask) {
     constexpr int TY = NT / 16, RPT = M / TY;
     const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-    float acc[RPT][4];
-    {
-        const float4 b = *reinterpret_cast<const float4*>(w.b1 + 4 * tx);
-#pragma unroll
-        for (int i = 0; i < RPT; ++i) { acc[i][0] = b.x; acc[i][1] = b.y; acc[i][2] = b.z; acc[i][3] = b.w; }
-    }
-    gemm_tile<RPT, TY>(Xs, ldx, w.w1t, pad4(d), acc, tx, ty);
     unsigned pm = 0;
 #pragma unroll
     for (int i = 0; i < RPT; ++i)
@@ -326,6 +325,69 @@ __device__ __forceinline__ void trunk_forward(const SmemWeights& w, const float*
     float mu3[RPT];
     layernorm_rows<RPT>(acc, mu3, rstd3);
     store_tile<RPT, TY>(N3s, acc, tx, ty);
+}
+
+// Trunk forward of one tile: Xs [M][ldx] (raw obs, zero padded to pad4(d)) -> N1s, N3s (trunk_from_z1).
+template <int M, int NT, bool KEEP>
+__device__ __forceinline__ void trunk_forward(const SmemWeights& w, const float* __restrict__ Xs, int ldx, int d,
+                                              int activation_id, float* __restrict__ N1s, float* __restrict__ N3s,
+                                              float (&mu1)[M / (NT / 16)], float (&rstd1)[M / (NT / 16)],
+                                              float (&rstd3)[M / (NT / 16)], unsigned& posmask) {
+    constexpr int TY = NT / 16, RPT = M / TY;
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    float acc[RPT][4];
+    {
+        const float4 b = *reinterpret_cast<const float4*>(w.b1 + 4 * tx);
+#pragma unroll
+        for (int i = 0; i < RPT; ++i) { acc[i][0] = b.x; acc[i][1] = b.y; acc[i][2] = b.z; acc[i][3] = b.w; }
+    }
+    gemm_tile<RPT, TY>(Xs, ldx, w.w1t, pad4(d), acc, tx, ty);
+    trunk_from_z1<M, NT, KEEP>(w, acc, activation_id, N1s, N3s, mu1, rstd1, rstd3, posmask);
+}
+
+// ---- fc1 of wide observations (64 < d <= 256) ------------------------------------------------------------------------
+// A tile of d = 256 with all of W1 staged k-major would need 64 KB of W1 and a 128 x 260 observation tile: the update
+// kernel would no longer fit in shared memory.  So fc1 runs as a loop over the P = ceil(d / 64) K-panels of the
+// observation: Z1 = b1 + sum_p X[:, 64p..64p+64) W1[:, 64p..64p+64)^T, with the panel's W1 columns staged into a 64 x 64
+// k-major w1t and the tile's observation columns into an M x LDX_PANEL Xs (the buffers of the d = 64 layout).  Panels
+// are summed in order 0..P-1, so the bits do not depend on the grid.  row(r) gives the observation row r of the tile in
+// global memory, or nullptr for a row outside it (staged as zeros).
+
+// Xs[r][k] = obs row r, column 64p + k (0 beyond d).  No syncs.
+template <int M, int NT, typename RowPtr>
+__device__ __forceinline__ void stage_obs_panel(float* __restrict__ Xs, int d, int p, RowPtr&& row) {
+    for (int i = threadIdx.x; i < M * LDX_PANEL; i += NT) {
+        const int r = i / LDX_PANEL, k = i % LDX_PANEL, c = OBS_PANEL * p + k;
+        const float* src = row(r);
+        Xs[i] = (src != nullptr && k < OBS_PANEL && c < d) ? src[c] : 0.f;
+    }
+}
+
+// acc = Z1 of the tile (b1 + X W1^T) over every panel.  W1 = params + net_offsets(d, n).w1.  Syncs before staging each
+// panel and after it, so the caller need not sync before the call; on return Xs holds the last panel, P - 1.
+template <int M, int NT, typename RowPtr>
+__device__ __forceinline__ void fc1_panels(const SmemWeights& w, const float* __restrict__ W1, int d, float* __restrict__ Xs,
+                                           RowPtr&& row, float (&acc)[M / (NT / 16)][4]) {
+    constexpr int TY = NT / 16, RPT = M / TY;
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    {
+        const float4 b = *reinterpret_cast<const float4*>(w.b1 + 4 * tx);
+#pragma unroll
+        for (int i = 0; i < RPT; ++i) { acc[i][0] = b.x; acc[i][1] = b.y; acc[i][2] = b.z; acc[i][3] = b.w; }
+    }
+    const int P = (d + OBS_PANEL - 1) / OBS_PANEL;
+    for (int p = 0; p < P; ++p) {
+        __syncthreads();   // the previous panel's GEMM (or the caller's last reads of Xs / w1t) is done
+        // 8 adjacent threads read 8 consecutive columns of one W1 row (32 bytes, where one column per thread would take
+        // a sector each); the shared stores of a warp then fall into 4 banks
+        for (int i = threadIdx.x; i < OBS_PANEL * H; i += NT) {
+            const int k = 8 * (i / (8 * H)) + i % 8, j = (i / 8) % H, c = OBS_PANEL * p + k;
+            w.w1t[k * H + j] = c < d ? W1[j * d + c] : 0.f;
+        }
+        stage_obs_panel<M, NT>(Xs, d, p, row);
+        __syncthreads();
+        gemm_tile<RPT, TY>(Xs, LDX_PANEL, w.w1t, min(OBS_PANEL, pad4(d - OBS_PANEL * p)), acc, tx, ty);
+    }
 }
 
 // Head dot products for the row owned by this thread group: PPR = NT / M threads per row

@@ -103,7 +103,11 @@ __device__ __forceinline__ void wgrad_flush(float* __restrict__ scratch, const W
 // 128 x 64 tile (head_tile) in the DZs buffer, which the row loss overwrites with dL/dlogits; dn3 = dL . Whf is a tile
 // GEMM with K = pad4(n) and GH += dL^T n3 a wgrad_acc with JB = ceil(n / 4).  dZ3 goes to DZs only after both have read
 // dL, so the dL tile needs no buffer of its own (that keeps obs width 64 within the 227 KB of shared memory).
-template <bool POLICY, int NB = MAX_OUT>
+// PANELS: an observation wider than 64 (orl_mlp.cuh, fc1_panels) in the buffers of the d = 64 layout.  The forward runs
+// fc1 panel by panel; the backward re-stages each panel (the last one is still in Xs) and forms G1_p = dZ1^T X_p with
+// one 4x4 block per thread (MG = 1), which the thread adds into its own elements of this CTA's partial row: one owner
+// per element, tiles in the CTA's order, no atomics.
+template <bool POLICY, int NB = MAX_OUT, bool PANELS = false>
 __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, int cta, int G) {
     constexpr bool WIDE = NB == MAX_OUT_WIDE;
     static_assert(POLICY || !WIDE, "the critic's head is one value");
@@ -111,11 +115,11 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
     const int n = POLICY ? a.n_actions : 1;
     const float* params = POLICY ? a.policy_params : a.critic_params;
     const float* obs = POLICY ? a.policy_obs : a.critic_obs;
-    const int dp = pad4(d), ldx = dp + 4;
+    const int dp = PANELS ? OBS_PANEL : pad4(d), ldx = dp + 4;
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
 
     float* p = smem;
-    SmemWeights w = carve_weights<NB>(p, d, true);
+    SmemWeights w = carve_weights<NB>(p, PANELS ? OBS_PANEL : d, true);
     float* Xs = p;  p += P_M * ldx;
     float* N1s = p; p += P_M * LDA;
     float* N3s = p; p += P_M * LDA;
@@ -128,7 +132,7 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
     float* red = p; p += 32;
     long long* row_idx = reinterpret_cast<long long*>(p); p += 2 * P_M;
 
-    load_weights_folded<P_NT, NB>(w, params, d, n, true);
+    load_weights_folded<P_NT, NB, PANELS>(w, params, d, n, true);
 
     const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS, val_masks = a.flags & ORL_PPO_VALUE_ACTIVE_MASKS;
     const MbConsts mb = mb_consts(a);
@@ -141,6 +145,26 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
     const bool gaussian = POLICY && !WIDE && a.head_kind == ORL_HEAD_GAUSSIAN;
     float dls_acc[MAX_OUT] = {};   // dL/dlogstd partial sums of this thread's rows (Gaussian head)
     float loss0 = 0.f, loss1 = 0.f, loss2 = 0.f;  // policy: policy_loss, entropy, ratio | critic: value_loss
+
+    // G1 element (row 4 jb + r, column 64 pnl + 4 kb + c) of a panelled pass lives in this CTA's partial row; its owner
+    // zeroes it first
+    const int n_panels = (d + OBS_PANEL - 1) / OBS_PANEL;
+    float* g1_part = nullptr;
+    if constexpr (PANELS)
+        g1_part = a.partials + (size_t)((POLICY ? 0 : G) + cta) * ppo_stride(a.obs_dim, a.critic_obs_dim, a.n_actions) +
+                  fold_offsets(d, n).g1;
+    auto g1_at = [&](int pnl, int r, int c) -> float* {
+        return g1_part + (4 * map1.jb + r) * d + OBS_PANEL * pnl + 4 * map1.kb + c;
+    };
+    if constexpr (PANELS) {
+        for (int pnl = 0; pnl < n_panels; ++pnl)
+#pragma unroll
+            for (int r = 0; r < 4; ++r)
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+                    if (OBS_PANEL * pnl + 4 * map1.kb + c < d) *g1_at(pnl, r, c) = 0.f;
+    }
+    auto obs_row = [&](int r) -> const float* { return row_idx[r] >= 0 ? obs + row_idx[r] * d : nullptr; };
 
     const long long n_tiles = (a.batch_rows + P_M - 1) / P_M;
     for (long long tile = cta; tile < n_tiles; tile += G) {
@@ -158,19 +182,23 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
             }
         }
         __syncthreads();
-        for (int i = tid; i < P_M * ldx; i += P_NT) {
-            const int r = i / ldx, k = i % ldx;
-            const long long gi = row_idx[r];
-            Xs[i] = (gi >= 0 && k < d) ? obs[gi * d + k] : 0.f;
-        }
-        __syncthreads();
-
-        // ---- forward ----
+        // ---- (gather +) forward ----
         float mu1[P_RPT], rstd1[P_RPT], rstd3[P_RPT];
         unsigned posmask;
-        trunk_forward<P_M, P_NT, true>(w, Xs, ldx, d, a.activation_id, N1s, N3s, mu1, rstd1, rstd3, posmask);
-        __syncthreads();
         float acc[P_RPT][4];
+        if constexpr (PANELS) {
+            fc1_panels<P_M, P_NT>(w, params + net_offsets(d, n).w1, d, Xs, obs_row, acc);
+            trunk_from_z1<P_M, P_NT, true>(w, acc, a.activation_id, N1s, N3s, mu1, rstd1, rstd3, posmask);
+        } else {
+            for (int i = tid; i < P_M * ldx; i += P_NT) {
+                const int r = i / ldx, k = i % ldx;
+                const long long gi = row_idx[r];
+                Xs[i] = (gi >= 0 && k < d) ? obs[gi * d + k] : 0.f;
+            }
+            __syncthreads();
+            trunk_forward<P_M, P_NT, true>(w, Xs, ldx, d, a.activation_id, N1s, N3s, mu1, rstd1, rstd3, posmask);
+        }
+        __syncthreads();
         if constexpr (WIDE) {
             head_tile<P_M, P_NT>(w, N3s, DZs);
             __syncthreads();
@@ -287,8 +315,27 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
         __syncthreads();                               // all reads of dZ3 done
         store_tile<P_RPT, P_TY>(DZs, acc, tx, ty);     // dZ1
         __syncthreads();
-        wgrad_acc(DZs, LDA, Xs, ldx, map1, g1, db1);   // G1 += dZ1^T X
-        __syncthreads();
+        if constexpr (PANELS) {   // G1_p = dZ1^T X_p, last panel first (it is still in Xs); db1 with panel 0
+            for (int pnl = n_panels - 1; pnl >= 0; --pnl) {
+                if (pnl != n_panels - 1) {
+                    stage_obs_panel<P_M, P_NT>(Xs, d, pnl, obs_row);
+                    __syncthreads();
+                }
+                float gp[4][4] = {}, dbp[4] = {};
+                wgrad_acc(DZs, LDA, Xs, LDX_PANEL, map1, gp, dbp);
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+                    if (pnl == 0) db1[r] += dbp[r];
+#pragma unroll
+                    for (int c = 0; c < 4; ++c)
+                        if (OBS_PANEL * pnl + 4 * map1.kb + c < d) *g1_at(pnl, r, c) += gp[r][c];
+                }
+                __syncthreads();
+            }
+        } else {
+            wgrad_acc(DZs, LDA, Xs, ldx, map1, g1, db1);   // G1 += dZ1^T X
+            __syncthreads();
+        }
     }
 
     // ---- flush this CTA's partial folded gradients + loss sums ----
@@ -296,7 +343,14 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
     float* part = a.partials + (size_t)((POLICY ? 0 : G) + cta) * stride;
     const FoldOffsets fo = fold_offsets(d, n);
     float* scratch = N1s;  // >= 16*(64*4+64) floats needed at most; N1s..DZs is 3*128*68 floats
-    wgrad_flush(scratch, map1, 16, dp / 4, g1, db1, H, d, part + fo.g1, part + fo.db1);
+    if constexpr (PANELS) {   // G1 is in place; one thread per 4 rows of db1 (MG = 1)
+        if (map1.kb == 0) {
+#pragma unroll
+            for (int r = 0; r < 4; ++r) part[fo.db1 + 4 * map1.jb + r] = db1[r];
+        }
+    } else {
+        wgrad_flush(scratch, map1, 16, dp / 4, g1, db1, H, d, part + fo.g1, part + fo.db1);
+    }
     wgrad_flush(scratch, map3, 16, 16, g3, db3, H, H, part + fo.g3, part + fo.db3);
     wgrad_flush(scratch, maph, JBH, 16, gh, dbh, n, H, part + fo.gh, part + fo.dbh);
     __syncthreads();
@@ -342,6 +396,16 @@ __global__ void __launch_bounds__(P_NT, 1) ppo_fwdbwd_kernel(const OrlPpoArgs a)
     const int G = a.grid_per_net;
     if ((int)blockIdx.x < G) ppo_net_pass<true, NB>(a, smem, blockIdx.x, G);
     else ppo_net_pass<false>(a, smem, blockIdx.x - G, G);
+}
+
+// ppo_fwdbwd_kernel when either net's observation is wider than 64: the pass of a net with PANELS_* runs fc1 in panels,
+// the other one is the pass of ppo_fwdbwd_kernel<NB>
+template <int NB, bool PANELS_POLICY, bool PANELS_CRITIC>
+__global__ void __launch_bounds__(P_NT, 1) ppo_fwdbwd_wide_obs_kernel(const OrlPpoArgs a) {
+    extern __shared__ __align__(16) float smem[];
+    const int G = a.grid_per_net;
+    if ((int)blockIdx.x < G) ppo_net_pass<true, NB, PANELS_POLICY>(a, smem, blockIdx.x, G);
+    else ppo_net_pass<false, MAX_OUT, PANELS_CRITIC>(a, smem, blockIdx.x - G, G);
 }
 
 // Sum over the G partial rows of one net for 32 consecutive bucket elements per CTA (8 warps): warp w adds rows
@@ -558,7 +622,8 @@ size_t fwdbwd_wide_smem_bytes(int d, int dc) {
 }
 
 int check_ppo_args(const OrlPpoArgs& a) {
-    ORL_CHECK_ARG(a.obs_dim > 0 && a.obs_dim <= 64 && a.critic_obs_dim > 0 && a.critic_obs_dim <= 64, "obs dims must be in 1..64");
+    ORL_CHECK_ARG(a.obs_dim > 0 && a.obs_dim <= orl::MAX_OBS_WIDE && a.critic_obs_dim > 0 && a.critic_obs_dim <= orl::MAX_OBS_WIDE,
+                  "obs dims must be in 1..256");
     ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= orl::MAX_OUT_WIDE, "n_actions must be in 1..64");
     ORL_CHECK_ARG(a.n_actions <= orl::MAX_OUT || a.head_kind == ORL_HEAD_CATEGORICAL,
                   "n_actions must be in 1..8 for Gaussian heads (1..64 for Categorical heads)");
@@ -597,6 +662,7 @@ extern "C" int orl_ppo_fwdbwd(const OrlPpoArgs* args, void* stream) {
     ORL_CHECK_ARG(a.head_kind == ORL_HEAD_CATEGORICAL || a.head_kind == ORL_HEAD_GAUSSIAN, "head_kind");
     if (a.flags & ORL_PPO_TF32) {
         ORL_CHECK_ARG(a.n_actions <= orl::MAX_OUT, "ORL_PPO_TENSORCORE: n_actions must be in 1..8");
+        ORL_CHECK_ARG(a.obs_dim <= orl::OBS_PANEL && a.critic_obs_dim <= orl::OBS_PANEL, "ORL_PPO_TENSORCORE: obs dims must be in 1..64");
         if (a.head_kind != ORL_HEAD_CATEGORICAL) {
             orl::set_last_error("orl_ppo_fwdbwd: ORL_PPO_TENSORCORE supports categorical heads only");
             return ORL_ERR_UNSUPPORTED;
@@ -604,8 +670,17 @@ extern "C" int orl_ppo_fwdbwd(const OrlPpoArgs* args, void* stream) {
         return orl::launch_ppo_fwdbwd_tc(a, reinterpret_cast<cudaStream_t>(stream));
     }
     const bool wide = a.n_actions > orl::MAX_OUT;
-    const size_t smem = wide ? fwdbwd_wide_smem_bytes(a.obs_dim, a.critic_obs_dim) : fwdbwd_smem_bytes(a.obs_dim, a.critic_obs_dim);
-    void (*const kern)(OrlPpoArgs) = wide ? ppo_fwdbwd_kernel<orl::MAX_OUT_WIDE> : ppo_fwdbwd_kernel<orl::MAX_OUT>;
+    // a panelled pass uses the buffers of the d = 64 layout
+    const bool wide_obs = std::max(a.obs_dim, a.critic_obs_dim) > orl::OBS_PANEL;
+    const int ds = std::min(a.obs_dim, orl::OBS_PANEL), dcs = std::min(a.critic_obs_dim, orl::OBS_PANEL);
+    const size_t smem = wide ? fwdbwd_wide_smem_bytes(ds, dcs) : fwdbwd_smem_bytes(ds, dcs);
+    const bool pp = a.obs_dim > orl::OBS_PANEL, pc = a.critic_obs_dim > orl::OBS_PANEL;
+    void (*const kern)(OrlPpoArgs) =
+        !wide_obs ? (wide ? ppo_fwdbwd_kernel<orl::MAX_OUT_WIDE> : ppo_fwdbwd_kernel<orl::MAX_OUT>)
+        : wide ? (pp && pc ? ppo_fwdbwd_wide_obs_kernel<orl::MAX_OUT_WIDE, true, true>
+                  : pp ? ppo_fwdbwd_wide_obs_kernel<orl::MAX_OUT_WIDE, true, false> : ppo_fwdbwd_wide_obs_kernel<orl::MAX_OUT_WIDE, false, true>)
+               : (pp && pc ? ppo_fwdbwd_wide_obs_kernel<orl::MAX_OUT, true, true>
+                  : pp ? ppo_fwdbwd_wide_obs_kernel<orl::MAX_OUT, true, false> : ppo_fwdbwd_wide_obs_kernel<orl::MAX_OUT, false, true>);
     if (int e = orl::allow_dynamic_smem(kern, 227 * 1024)) return e;
     kern<<<2 * a.grid_per_net, P_NT, smem, reinterpret_cast<cudaStream_t>(stream)>>>(a);
     ORL_LAUNCH_CHECK("ppo_fwdbwd_kernel");

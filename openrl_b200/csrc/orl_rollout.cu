@@ -49,15 +49,20 @@ __global__ void env_step_kernel(int kind, int N, EnvPtrs E, const float* __restr
 }
 
 
+// ENV of the host act (ORL_ENV_NONE) for observations of 65..256 features: fc1 in panels (orl_mlp.cuh, fc1_panels) in
+// the buffers of the d = 64 layout
+constexpr int ENV_NONE_WIDE_OBS = -1;
+
 // NB: head width bound (orl_mlp.cuh); NB = 64 is the wide Categorical head of host-stepped envs (ORL_ENV_NONE), whose
 // logits tile reuses N1s once the trunk is done with it.
 template <int R_M, int ENV, int NB = MAX_OUT>
 __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
+    constexpr bool PANELS = ENV == ENV_NONE_WIDE_OBS;
     extern __shared__ __align__(16) float smem[];
     const int N = a.n_envs, A = a.n_agents, B = N * A, d = a.obs_dim, n = a.n_actions;
-    const int ldx = pad4(d) + 4;
+    const int ldx = PANELS ? LDX_PANEL : pad4(d) + 4;
     float* p = smem;
-    SmemWeights w = carve_weights<NB>(p, d, false);
+    SmemWeights w = carve_weights<NB>(p, PANELS ? OBS_PANEL : d, false);
     float* Xs = p;  p += R_M * ldx;
     float* N1s = p; p += R_M * LDA;
     float* N3s = p; p += R_M * LDA;
@@ -71,14 +76,16 @@ __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
     const int rows_here = n_env_here * A;
     const int tid = threadIdx.x;
 
-    load_weights_folded<R_NT, NB>(w, a.policy_params, d, n, false);   // (the logstd tail, if any, is read directly)
+    load_weights_folded<R_NT, NB, PANELS>(w, a.policy_params, d, n, false);   // (the logstd tail, if any, is read directly)
 
-    // stage obs of slot t_begin (zero padding for the k tail and for idle rows)
-    for (int i = tid; i < R_M * ldx; i += R_NT) {
-        const int r = i / ldx, k = i % ldx;
-        Xs[i] = (r < rows_here && k < d) ? a.policy_obs[((size_t)a.t_begin * B + row0 + r) * d + k] : 0.f;
+    // stage obs of slot t_begin (zero padding for the k tail and for idle rows); a panelled fc1 stages its own
+    if constexpr (!PANELS) {
+        for (int i = tid; i < R_M * ldx; i += R_NT) {
+            const int r = i / ldx, k = i % ldx;
+            Xs[i] = (r < rows_here && k < d) ? a.policy_obs[((size_t)a.t_begin * B + row0 + r) * d + k] : 0.f;
+        }
+        __syncthreads();
     }
-    __syncthreads();
 
     constexpr int PPR = R_NT / R_M;
     const int hrow = tid / PPR, hpart = tid % PPR;
@@ -87,10 +94,18 @@ __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
     for (int t = a.t_begin; t < a.t_end; ++t) {
         float mu1[R_M / (R_NT / 16)], rstd1[R_M / (R_NT / 16)], rstd3[R_M / (R_NT / 16)];
         unsigned pm;
-        trunk_forward<R_M, R_NT, false>(w, Xs, ldx, d, a.activation_id, N1s, N3s, mu1, rstd1, rstd3, pm);
+        if constexpr (PANELS) {   // ORL_ENV_NONE: t == t_begin, the one step of the call
+            float acc[R_M / (R_NT / 16)][4];
+            fc1_panels<R_M, R_NT>(w, a.policy_params + net_offsets(d, n).w1, d, Xs, [&](int r) -> const float* {
+                return r < rows_here ? a.policy_obs + ((size_t)t * B + row0 + r) * d : nullptr;
+            }, acc);
+            trunk_from_z1<R_M, R_NT, false>(w, acc, a.activation_id, N1s, N3s, mu1, rstd1, rstd3, pm);
+        } else {
+            trunk_forward<R_M, R_NT, false>(w, Xs, ldx, d, a.activation_id, N1s, N3s, mu1, rstd1, rstd3, pm);
+        }
         __syncthreads();
         if constexpr (NB == MAX_OUT_WIDE) {
-            static_assert(ENV == ORL_ENV_NONE, "wide heads act on host-stepped envs");
+            static_assert(ENV == ORL_ENV_NONE || PANELS, "wide heads act on host-stepped envs");
             head_tile<R_M, R_NT>(w, N3s, N1s);
             __syncthreads();
             if (tid < rows_here) {   // one thread per row
@@ -182,30 +197,38 @@ __global__ void env_reset_kernel(int env_kind, int N, double* env_f64, uint64_t*
 constexpr int C_M = 128, C_NT = 256;
 
 // NB = 64 (wide Categorical heads): the logits go to a tile in N1s and epilogue(g, x) gets the row's logits x[0..n) there.
-template <int NB = MAX_OUT, typename Epilogue>
+// PANELS: observations of 65..256 features, fc1 in panels (orl_mlp.cuh, fc1_panels) in the buffers of the d = 64 layout.
+template <int NB = MAX_OUT, bool PANELS = false, typename Epilogue>
 __device__ __forceinline__ void rows_forward(const float* __restrict__ params, int d, int n, int activation_id,
                                              const float* __restrict__ obs, long long rows, Epilogue&& epilogue) {
     extern __shared__ __align__(16) float smem[];
-    const int ldx = pad4(d) + 4;
+    const int ldx = PANELS ? LDX_PANEL : pad4(d) + 4;
     float* p = smem;
-    SmemWeights w = carve_weights<NB>(p, d, false);
+    SmemWeights w = carve_weights<NB>(p, PANELS ? OBS_PANEL : d, false);
     float* Xs = p;  p += C_M * ldx;
     float* N1s = p; p += C_M * LDA;
     float* N3s = p; p += C_M * LDA;
     const int tid = threadIdx.x;
-    load_weights_folded<C_NT, NB>(w, params, d, n, false);
+    load_weights_folded<C_NT, NB, PANELS>(w, params, d, n, false);
     const long long n_tiles = (rows + C_M - 1) / C_M;
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         const long long r0 = tile * C_M;
         const int rows_here = (int)min((long long)C_M, rows - r0);
-        for (int i = tid; i < C_M * ldx; i += C_NT) {
-            const int r = i / ldx, k = i % ldx;
-            Xs[i] = (r < rows_here && k < d) ? obs[(r0 + r) * d + k] : 0.f;
-        }
-        __syncthreads();
         float mu1[C_M / (C_NT / 16)], rstd1[C_M / (C_NT / 16)], rstd3[C_M / (C_NT / 16)];
         unsigned pm;
-        trunk_forward<C_M, C_NT, false>(w, Xs, ldx, d, activation_id, N1s, N3s, mu1, rstd1, rstd3, pm);
+        if constexpr (PANELS) {
+            float acc[C_M / (C_NT / 16)][4];
+            fc1_panels<C_M, C_NT>(w, params + net_offsets(d, n).w1, d, Xs,
+                                  [&](int r) -> const float* { return r < rows_here ? obs + (r0 + r) * d : nullptr; }, acc);
+            trunk_from_z1<C_M, C_NT, false>(w, acc, activation_id, N1s, N3s, mu1, rstd1, rstd3, pm);
+        } else {
+            for (int i = tid; i < C_M * ldx; i += C_NT) {
+                const int r = i / ldx, k = i % ldx;
+                Xs[i] = (r < rows_here && k < d) ? obs[(r0 + r) * d + k] : 0.f;
+            }
+            __syncthreads();
+            trunk_forward<C_M, C_NT, false>(w, Xs, ldx, d, activation_id, N1s, N3s, mu1, rstd1, rstd3, pm);
+        }
         __syncthreads();
         if constexpr (NB == MAX_OUT_WIDE) {
             head_tile<C_M, C_NT>(w, N3s, N1s);
@@ -222,20 +245,31 @@ __device__ __forceinline__ void rows_forward(const float* __restrict__ params, i
 }
 
 // ValueNetwork.forward (value_network.py:113-136)
+template <bool PANELS>
+__device__ __forceinline__ void critic_values_body(const float* __restrict__ params, int d, int activation_id,
+                                                   const float* __restrict__ obs, float* __restrict__ values, long long rows) {
+    rows_forward<MAX_OUT, PANELS>(params, d, 1, activation_id, obs, rows, [&](long long g, float (&out)[MAX_OUT]) { values[g] = out[0]; });
+}
 __global__ void __launch_bounds__(C_NT) critic_values_kernel(const float* __restrict__ params, int d, int activation_id,
                                                              const float* __restrict__ obs, float* __restrict__ values,
                                                              long long rows) {
-    rows_forward(params, d, 1, activation_id, obs, rows, [&](long long g, float (&out)[MAX_OUT]) { values[g] = out[0]; });
+    critic_values_body<false>(params, d, activation_id, obs, values, rows);
+}
+__global__ void __launch_bounds__(C_NT) critic_values_wide_obs_kernel(const float* __restrict__ params, int d, int activation_id,
+                                                                      const float* __restrict__ obs, float* __restrict__ values,
+                                                                      long long rows) {
+    critic_values_body<true>(params, d, activation_id, obs, values, rows);
 }
 
 // PolicyNetwork.eval_actions (policy_network.py:164-203, act.py:160-168 / 150-158): the log-prob of the given action and
 // the entropy of the action distribution per row (the caller takes the masked mean); per dimension for a Gaussian head.
-__global__ void __launch_bounds__(C_NT) policy_eval_kernel(const float* __restrict__ params, int d, int n, int activation_id, int head_kind,
-                                                           const float* __restrict__ obs, const float* __restrict__ actions,
-                                                           const float* __restrict__ action_masks, float* __restrict__ logp_out,
-                                                           float* __restrict__ entropy_out, long long rows) {
+template <bool PANELS>
+__device__ __forceinline__ void policy_eval_body(const float* __restrict__ params, int d, int n, int activation_id, int head_kind,
+                                                 const float* __restrict__ obs, const float* __restrict__ actions,
+                                                 const float* __restrict__ action_masks, float* __restrict__ logp_out,
+                                                 float* __restrict__ entropy_out, long long rows) {
     const float* logstd = params + net_offsets(d, n, 1).ls;
-    rows_forward(params, d, n, activation_id, obs, rows, [&](long long g, float (&out)[MAX_OUT]) {
+    rows_forward<MAX_OUT, PANELS>(params, d, n, activation_id, obs, rows, [&](long long g, float (&out)[MAX_OUT]) {
         if (head_kind == ORL_HEAD_GAUSSIAN) {
             for (int j = 0; j < n; ++j) {
                 const float ls = logstd[j];
@@ -250,17 +284,42 @@ __global__ void __launch_bounds__(C_NT) policy_eval_kernel(const float* __restri
         }
     });
 }
+__global__ void __launch_bounds__(C_NT) policy_eval_kernel(const float* __restrict__ params, int d, int n, int activation_id, int head_kind,
+                                                           const float* __restrict__ obs, const float* __restrict__ actions,
+                                                           const float* __restrict__ action_masks, float* __restrict__ logp_out,
+                                                           float* __restrict__ entropy_out, long long rows) {
+    policy_eval_body<false>(params, d, n, activation_id, head_kind, obs, actions, action_masks, logp_out, entropy_out, rows);
+}
+__global__ void __launch_bounds__(C_NT) policy_eval_wide_obs_kernel(const float* __restrict__ params, int d, int n, int activation_id,
+                                                                    int head_kind, const float* __restrict__ obs,
+                                                                    const float* __restrict__ actions, const float* __restrict__ action_masks,
+                                                                    float* __restrict__ logp_out, float* __restrict__ entropy_out, long long rows) {
+    policy_eval_body<true>(params, d, n, activation_id, head_kind, obs, actions, action_masks, logp_out, entropy_out, rows);
+}
 
 // policy_eval_kernel of a wide Categorical head (9..64 actions)
-__global__ void __launch_bounds__(C_NT) policy_eval_wide_kernel(const float* __restrict__ params, int d, int n, int activation_id,
-                                                                const float* __restrict__ obs, const float* __restrict__ actions,
-                                                                const float* __restrict__ action_masks, float* __restrict__ logp_out,
-                                                                float* __restrict__ entropy_out, long long rows) {
-    rows_forward<MAX_OUT_WIDE>(params, d, n, activation_id, obs, rows, [&](long long g, float* x) {
+template <bool PANELS>
+__device__ __forceinline__ void policy_eval_wide_body(const float* __restrict__ params, int d, int n, int activation_id,
+                                                      const float* __restrict__ obs, const float* __restrict__ actions,
+                                                      const float* __restrict__ action_masks, float* __restrict__ logp_out,
+                                                      float* __restrict__ entropy_out, long long rows) {
+    rows_forward<MAX_OUT_WIDE, PANELS>(params, d, n, activation_id, obs, rows, [&](long long g, float* x) {
         const WideSoftmax sm = wide_log_softmax(x, n, action_masks ? action_masks + g * n : nullptr);
         logp_out[g] = wide_log_prob_of(sm, x, n, (int)actions[g]);
         entropy_out[g] = wide_entropy(sm, x, n);
     });
+}
+__global__ void __launch_bounds__(C_NT) policy_eval_wide_kernel(const float* __restrict__ params, int d, int n, int activation_id,
+                                                                const float* __restrict__ obs, const float* __restrict__ actions,
+                                                                const float* __restrict__ action_masks, float* __restrict__ logp_out,
+                                                                float* __restrict__ entropy_out, long long rows) {
+    policy_eval_wide_body<false>(params, d, n, activation_id, obs, actions, action_masks, logp_out, entropy_out, rows);
+}
+__global__ void __launch_bounds__(C_NT) policy_eval_wide_wide_obs_kernel(const float* __restrict__ params, int d, int n, int activation_id,
+                                                                         const float* __restrict__ obs, const float* __restrict__ actions,
+                                                                         const float* __restrict__ action_masks, float* __restrict__ logp_out,
+                                                                         float* __restrict__ entropy_out, long long rows) {
+    policy_eval_wide_body<true>(params, d, n, activation_id, obs, actions, action_masks, logp_out, entropy_out, rows);
 }
 
 // ---- insert of one host env.step into the rollout buffer (OnPolicyDriver.add2buffer, onpolicy_driver.py:80-152) -----------
@@ -323,9 +382,11 @@ __global__ void host_insert_rnn_kernel(const float* __restrict__ staged, int n_e
     }
 }
 
-// launch of a row-batch forward kernel over `rows` rows of obs_dim d: grid = min(tiles, 2 x SMs)
+// launch of a row-batch forward kernel over `rows` rows of obs_dim d: grid = min(tiles, 2 x SMs).  A panelled kernel
+// (d > 64) takes the layout of d = 64.
 template <int NB = MAX_OUT, typename... Params, typename... Args>
 int launch_rows_forward(void (*kern)(Params...), const char* name, int d, long long rows, cudaStream_t st, Args... args) {
+    d = std::min(d, OBS_PANEL);
     const int ldx = pad4(d) + 4;
     const size_t smem = sizeof(float) * (smem_weights_floats<NB>(d, false) + C_M * ldx + 2 * C_M * LDA);
     if (int e = allow_dynamic_smem(kern, 200 * 1024)) return e;
@@ -390,7 +451,9 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
     ORL_CHECK_ARG(args, "args");
     const OrlRolloutArgs& a = *args;
     ORL_CHECK_ARG(a.n_envs > 0 && a.n_agents > 0 && a.n_agents <= 32, "n_envs / n_agents");
-    ORL_CHECK_ARG(a.obs_dim > 0 && a.obs_dim <= 64, "obs_dim must be in 1..64");
+    ORL_CHECK_ARG(a.obs_dim > 0 && a.obs_dim <= orl::MAX_OBS_WIDE, "obs_dim must be in 1..256");
+    ORL_CHECK_ARG(a.obs_dim <= orl::OBS_PANEL || a.env_kind == ORL_ENV_NONE,
+                  "obs_dim must be in 1..64 (65..256: host-stepped envs, ORL_ENV_NONE)");
     ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= orl::MAX_OUT_WIDE, "n_actions must be in 1..64");
     ORL_CHECK_ARG(a.n_actions <= orl::MAX_OUT || (a.env_kind == ORL_ENV_NONE && a.head_kind == ORL_HEAD_CATEGORICAL),
                   "n_actions must be in 1..8 (9..64: Categorical heads on host-stepped envs, ORL_ENV_NONE)");
@@ -435,12 +498,18 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
     while (rm < a.n_agents) rm *= 2;
     const int envs_per_cta = rm / a.n_agents;
     const int grid = (a.n_envs + envs_per_cta - 1) / envs_per_cta;
-    const int ldx = orl::pad4(a.obs_dim) + 4;
-    const bool mpe = a.env_kind == ORL_ENV_MPE_SPREAD, wide = a.n_actions > orl::MAX_OUT;
-    const size_t smem = sizeof(float) * ((wide ? orl::smem_weights_floats<orl::MAX_OUT_WIDE>(a.obs_dim, false)
-                                               : orl::smem_weights_floats(a.obs_dim, false)) + rm * ldx + 2 * rm * orl::LDA + rm);
+    const int ds = std::min(a.obs_dim, orl::OBS_PANEL);   // a panelled fc1 takes the layout of d = 64
+    const int ldx = orl::pad4(ds) + 4;
+    const bool mpe = a.env_kind == ORL_ENV_MPE_SPREAD, wide = a.n_actions > orl::MAX_OUT, wide_obs = a.obs_dim > orl::OBS_PANEL;
+    const size_t smem = sizeof(float) * ((wide ? orl::smem_weights_floats<orl::MAX_OUT_WIDE>(ds, false)
+                                               : orl::smem_weights_floats(ds, false)) + rm * ldx + 2 * rm * orl::LDA + rm);
     void (*const kern)(OrlRolloutArgs) =
-        wide ? (rm == 8 ? rollout_kernel<8, ORL_ENV_NONE, orl::MAX_OUT_WIDE>
+        wide_obs ? (wide ? (rm == 8 ? rollout_kernel<8, ENV_NONE_WIDE_OBS, orl::MAX_OUT_WIDE>
+                            : rm == 16 ? rollout_kernel<16, ENV_NONE_WIDE_OBS, orl::MAX_OUT_WIDE>
+                                       : rollout_kernel<32, ENV_NONE_WIDE_OBS, orl::MAX_OUT_WIDE>)
+                         : (rm == 8 ? rollout_kernel<8, ENV_NONE_WIDE_OBS>
+                            : rm == 16 ? rollout_kernel<16, ENV_NONE_WIDE_OBS> : rollout_kernel<32, ENV_NONE_WIDE_OBS>))
+        : wide ? (rm == 8 ? rollout_kernel<8, ORL_ENV_NONE, orl::MAX_OUT_WIDE>
                 : rm == 16 ? rollout_kernel<16, ORL_ENV_NONE, orl::MAX_OUT_WIDE> : rollout_kernel<32, ORL_ENV_NONE, orl::MAX_OUT_WIDE>)
         : rm == 8 ? (mpe ? rollout_kernel<8, ORL_ENV_MPE_SPREAD> : rollout_kernel<8, ORL_ENV_NONE>)
         : rm == 16 ? (mpe ? rollout_kernel<16, ORL_ENV_MPE_SPREAD> : rollout_kernel<16, ORL_ENV_NONE>)
@@ -454,12 +523,15 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
 extern "C" int orl_critic_values(const float* critic_params, int obs_dim, int activation_id, const float* obs,
                                  float* values, long long rows, void* stream) {
     ORL_CHECK_ARG(critic_params && obs && values, "null buffer");
-    ORL_CHECK_ARG(obs_dim > 0 && obs_dim <= 64, "obs_dim must be in 1..64");
+    ORL_CHECK_ARG(obs_dim > 0 && obs_dim <= orl::MAX_OBS_WIDE, "obs_dim must be in 1..256");
     ORL_CHECK_ARG(rows > 0, "rows");
     ORL_CHECK_ARG(activation_id >= 0 && activation_id <= 3, "activation_id");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (obs_dim <= 8)   // tensor-core forward (orl_fwd_tc.cu)
         return orl::launch_critic_values_tc(critic_params, obs_dim, activation_id, obs, values, rows, st);
+    if (obs_dim > orl::OBS_PANEL)
+        return launch_rows_forward(critic_values_wide_obs_kernel, "critic_values_wide_obs_kernel", obs_dim, rows, st, critic_params,
+                                   obs_dim, activation_id, obs, values, rows);
     return launch_rows_forward(critic_values_kernel, "critic_values_kernel", obs_dim, rows, st, critic_params, obs_dim,
                                activation_id, obs, values, rows);
 }
@@ -468,11 +540,21 @@ extern "C" int orl_policy_eval(const float* policy_params, int obs_dim, int n_ac
                                const float* obs, const float* actions, const float* action_masks, float* log_probs,
                                float* entropy, long long rows, void* stream) {
     ORL_CHECK_ARG(policy_params && obs && actions && log_probs && entropy, "null buffer");
-    ORL_CHECK_ARG(obs_dim > 0 && obs_dim <= 64 && n_actions > 0 && n_actions <= orl::MAX_OUT_WIDE, "shapes");
+    ORL_CHECK_ARG(obs_dim > 0 && obs_dim <= orl::MAX_OBS_WIDE, "obs_dim must be in 1..256");
+    ORL_CHECK_ARG(n_actions > 0 && n_actions <= orl::MAX_OUT_WIDE, "n_actions must be in 1..64");
     ORL_CHECK_ARG(rows > 0 && activation_id >= 0 && activation_id <= 3, "rows / activation_id");
     ORL_CHECK_ARG(head_kind == ORL_HEAD_CATEGORICAL || head_kind == ORL_HEAD_GAUSSIAN, "head_kind");
     ORL_CHECK_ARG(n_actions <= orl::MAX_OUT || head_kind == ORL_HEAD_CATEGORICAL,
                   "n_actions must be in 1..8 for Gaussian heads (1..64 for Categorical heads)");
+    const bool wide_obs = obs_dim > orl::OBS_PANEL;
+    if (n_actions > orl::MAX_OUT && wide_obs)
+        return launch_rows_forward<orl::MAX_OUT_WIDE>(policy_eval_wide_wide_obs_kernel, "policy_eval_wide_wide_obs_kernel", obs_dim,
+                                                      rows, reinterpret_cast<cudaStream_t>(stream), policy_params, obs_dim, n_actions,
+                                                      activation_id, obs, actions, action_masks, log_probs, entropy, rows);
+    if (wide_obs)
+        return launch_rows_forward(policy_eval_wide_obs_kernel, "policy_eval_wide_obs_kernel", obs_dim, rows,
+                                   reinterpret_cast<cudaStream_t>(stream), policy_params, obs_dim, n_actions, activation_id, head_kind,
+                                   obs, actions, action_masks, log_probs, entropy, rows);
     if (n_actions > orl::MAX_OUT)
         return launch_rows_forward<orl::MAX_OUT_WIDE>(policy_eval_wide_kernel, "policy_eval_wide_kernel", obs_dim, rows,
                                                       reinterpret_cast<cudaStream_t>(stream), policy_params, obs_dim, n_actions,
@@ -482,13 +564,16 @@ extern "C" int orl_policy_eval(const float* policy_params, int obs_dim, int n_ac
                                log_probs, entropy, rows);
 }
 
-extern "C" int orl_host_insert(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
-                               float* masks_next, float* active_masks_next, float* action_masks_next, int n_actions,
-                               float* critic_obs_next, int critic_obs_dim, void* stream) {
+// the two feed-forward inserts: critic sections of 1..max_critic features
+static int host_insert(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
+                       float* masks_next, float* active_masks_next, float* action_masks_next, int n_actions,
+                       float* critic_obs_next, int critic_obs_dim, void* stream, int max_critic) {
     ORL_CHECK_ARG(staged && policy_obs_next && rewards && masks_next && active_masks_next, "null buffer");
     ORL_CHECK_ARG(n_envs > 0 && n_agents > 0 && obs_dim > 0, "shapes");
     ORL_CHECK_ARG(!action_masks_next || (n_actions > 0 && n_actions <= orl::MAX_OUT_WIDE), "n_actions must be in 1..64");
-    ORL_CHECK_ARG(!critic_obs_next || (critic_obs_dim > 0 && critic_obs_dim <= 64), "critic_obs_dim must be in 1..64");
+    ORL_CHECK_ARG(!critic_obs_next || (critic_obs_dim > 0 && critic_obs_dim <= max_critic),
+                  max_critic == orl::OBS_PANEL ? "critic_obs_dim must be in 1..64 (orl_host_insert_wide_obs: 1..256)"
+                                               : "critic_obs_dim must be in 1..256");
     const int B = n_envs * n_agents;
     host_insert_kernel<<<(B + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(staged, n_envs, n_agents, obs_dim, policy_obs_next,
                                                                                          rewards, masks_next, active_masks_next,
@@ -496,6 +581,20 @@ extern "C" int orl_host_insert(const float* staged, int n_envs, int n_agents, in
                                                                                          critic_obs_next, critic_obs_dim);
     ORL_LAUNCH_CHECK("host_insert_kernel");
     return 0;
+}
+
+extern "C" int orl_host_insert(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
+                               float* masks_next, float* active_masks_next, float* action_masks_next, int n_actions,
+                               float* critic_obs_next, int critic_obs_dim, void* stream) {
+    return host_insert(staged, n_envs, n_agents, obs_dim, policy_obs_next, rewards, masks_next, active_masks_next, action_masks_next,
+                       n_actions, critic_obs_next, critic_obs_dim, stream, orl::OBS_PANEL);
+}
+
+extern "C" int orl_host_insert_wide_obs(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next,
+                                        float* rewards, float* masks_next, float* active_masks_next, float* action_masks_next,
+                                        int n_actions, float* critic_obs_next, int critic_obs_dim, void* stream) {
+    return host_insert(staged, n_envs, n_agents, obs_dim, policy_obs_next, rewards, masks_next, active_masks_next, action_masks_next,
+                       n_actions, critic_obs_next, critic_obs_dim, stream, orl::MAX_OBS_WIDE);
 }
 
 // the two GRU inserts: masks of 1..max_actions actions

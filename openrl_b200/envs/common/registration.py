@@ -35,4 +35,7 @@ def make(id: str, env_num: int = 1, asynchronous: bool = False, add_monitor: boo
         env_fns = _gymnasium_thunks(id, env_num, render_mode, **kwargs)
     # `asynchronous` selects the reference's AsyncVectorEnv (one process per env); the host stepping here is synchronous —
     # the overlap with the device comes from HostVecEnv's double-buffered staging, not from worker processes
-    return HostVecEnv(SyncHostVecEnv(env_fns, auto_reset=auto_reset, env_name=id), device=device)
+    # the reference's make receives cfg in kwargs (registration.py:45); its option lets Dict entries be 65..256 wide
+    cfg = kwargs.get("cfg")
+    wide = bool(getattr(cfg, "use_wide_observations", False)) if cfg is not None else False
+    return HostVecEnv(SyncHostVecEnv(env_fns, auto_reset=auto_reset, env_name=id), device=device, wide_observations=wide)

@@ -34,9 +34,11 @@ def prepare_action_masks(info, agent_num=1):
     return np.asarray(rows, dtype=np.int8).reshape(len(rows), -1)
 
 
-def dict_obs_dims(space):
+def dict_obs_dims(space, wide_observations=False):
     """(policy width, critic width) of a Dict observation space with exactly the keys "policy" and "critic", each a flat
-    Box of width 1..64 (the widths the device networks take); NotImplementedError naming the cause otherwise."""
+    Box of width 1..64 (the widths the device networks take), or 1..256 with `wide_observations` (the feed-forward nets
+    of cfg.use_wide_observations); NotImplementedError naming the cause otherwise."""
+    bound = 256 if wide_observations else 64
     keys = sorted(space.keys())
     if keys != ["critic", "policy"]:
         raise NotImplementedError(f"HostVecEnv stages Dict observation spaces with exactly the keys 'policy' and 'critic'; "
@@ -47,14 +49,15 @@ def dict_obs_dims(space):
         shape = getattr(sub, "shape", None)
         if sub.__class__.__name__ != "Box" or shape is None or len(shape) != 1:
             raise NotImplementedError(f"HostVecEnv stages flat Box entries of a Dict observation space; '{k}' is {sub}")
-        if not 1 <= shape[0] <= 64:
-            raise NotImplementedError(f"the '{k}' observation has width {shape[0]}; the device networks take widths 1..64")
+        if not 1 <= shape[0] <= bound:
+            raise NotImplementedError(f"the '{k}' observation has width {shape[0]}; the device networks take widths 1..{bound}"
+                                      + ("" if wide_observations else " (1..256 with use_wide_observations)"))
         dims.append(int(shape[0]))
     return tuple(dims)
 
 
 class HostVecEnv:
-    def __init__(self, env, device="cuda:0"):
+    def __init__(self, env, device="cuda:0", wide_observations=False):
         self.env = env
         self.kind = lib.ENV_NONE
         self.device = torch.device(device)
@@ -69,7 +72,7 @@ class HostVecEnv:
         self.d2h_bytes = 0
         self.dict_obs = self.observation_space.__class__.__name__ == "Dict"
         if self.dict_obs:
-            self.obs_dim, self.critic_obs_dim = dict_obs_dims(self.observation_space)
+            self.obs_dim, self.critic_obs_dim = dict_obs_dims(self.observation_space, wide_observations)
         else:
             if not hasattr(self.observation_space, "shape") or self.observation_space.shape is None:
                 raise NotImplementedError(f"HostVecEnv stages flat Box or Dict {{'policy', 'critic'}} observations; "

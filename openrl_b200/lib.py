@@ -172,6 +172,7 @@ _SIGNATURES.update({
     "orl_share_fwdbwd": [_c.POINTER(OrlPpoArgs), _P],
     "orl_share_apply": [_c.POINTER(OrlPpoArgs), _P],
     "orl_host_insert": [_P, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _I, _P],
+    "orl_host_insert_wide_obs": [_P, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _I, _P],
     "orl_policy_eval": [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _L, _P],
     "orl_ppo_stride": [_I, _I, _I],
     "orl_ppo_grads_stride": [_I, _I, _I],

@@ -22,6 +22,18 @@ def _init(module, gain, use_orthogonal=True):
     return module
 
 
+def check_obs_shape(shape, wide=False):
+    """The observation shapes the kernels take: flat vectors of width 1..64, and of 65..256 when `wide` (a feed-forward
+    policy or critic with cfg.use_wide_observations: fc1 runs over 64-wide panels of the observation)."""
+    if len(shape) == 1 and shape[0] <= (256 if wide else 64):
+        return
+    if wide:
+        raise NotImplementedError("vector observations of width <= 256 only (the bound of use_wide_observations); "
+                                  f"got shape {tuple(shape)}")
+    raise NotImplementedError("vector observations of width <= 64 only (65..256: feed-forward policies and critics "
+                              f"with use_wide_observations, not GRU policies or use_share_model); got shape {tuple(shape)}")
+
+
 class MLPLayer(nn.Module):
     def __init__(self, input_dim, hidden_size, layer_N, use_orthogonal, activation_id):
         super().__init__()

@@ -2,7 +2,7 @@
 import torch
 import torch.nn as nn
 
-from .base import ACTLayer, FlatParams, MLPBase, RNNLayer
+from .base import ACTLayer, FlatParams, MLPBase, RNNLayer, check_obs_shape
 
 
 def _policy_shape(space):
@@ -16,8 +16,7 @@ class PolicyNetwork(nn.Module):
         self.recurrent = bool(cfg.use_recurrent_policy or cfg.use_naive_recurrent_policy)
         self.hidden_size = cfg.hidden_size
         shape = _policy_shape(input_space)
-        if len(shape) != 1 or shape[0] > 64:
-            raise NotImplementedError("vector observations of width <= 64 only")
+        check_obs_shape(shape, wide=getattr(cfg, "use_wide_observations", False) and not self.recurrent)
         self.obs_dim = shape[0]
         self.activation_id = cfg.activation_id
         self.base = MLPBase(cfg, shape)

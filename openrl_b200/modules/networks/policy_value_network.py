@@ -6,7 +6,7 @@ Categorical head, Box spaces of width <= 8 a DiagGaussian head (fc_mean + logstd
 import torch
 import torch.nn as nn
 
-from .base import ACT_NAMES, ACTLayer, FlatParams, MLPBase, ValueNorm, _init
+from .base import ACT_NAMES, ACTLayer, FlatParams, MLPBase, ValueNorm, _init, check_obs_shape
 from .policy_network import _policy_shape
 
 
@@ -30,8 +30,7 @@ class PolicyValueNetwork(nn.Module):
         self.recurrent = False
         self.hidden_size = cfg.hidden_size
         shape = _policy_shape(input_space)
-        if len(shape) != 1 or shape[0] > 64:
-            raise NotImplementedError("vector observations of width <= 64 only")
+        check_obs_shape(shape)
         self.obs_dim = shape[0]
         self.activation_id = cfg.activation_id
         self.obs_prep = MLPBase(cfg, shape)
