@@ -373,7 +373,10 @@ typedef struct OrlRnnArgs {
     int32_t env_kind, n_envs, n_agents, episode_length;   /* N, A, T; rows B = N*A */
     int32_t t_begin, t_end;
     int32_t obs_dim, critic_obs_dim, n_actions, activation_id;   /* n_actions 1..64; 1..8 for orl_rnn_rollout and with
-                                                                   ORL_PPO_JOINT_ACTION (ORL_ERR_BAD_ARG otherwise) */
+                                                                   ORL_PPO_JOINT_ACTION (ORL_ERR_BAD_ARG otherwise).
+                                                                   obs_dim / critic_obs_dim 1..256 for orl_rnn_act_rows,
+                                                                   orl_rnn_critic, orl_rnn_fwdbwd and orl_rnn_apply; 1..64 for
+                                                                   orl_rnn_rollout and with ORL_PPO_JOINT_ACTION */
     int32_t deterministic, chunk_length;                  /* L = cfg.data_chunk_length (<= 32) */
     int32_t flags;                                        /* ORL_PPO_* */
     int32_t env_table_len;
@@ -390,7 +393,8 @@ typedef struct OrlRnnArgs {
     double* env_f64; uint64_t* env_u64; int32_t* env_i32; const int32_t* env_table;
     float* ep_return; int32_t* ep_length; double* episode_stats;
     const double* gae_stats; const double* mb_stats; float* vn_state;
-    float* tape;                                          /* workspace: orl_rnn_workspace_floats_for(n_chunks*L, grads_stride, n_actions) floats (tape rows, then reduction partials) */
+    float* tape;                                          /* workspace: orl_rnn_workspace_floats_for(n_chunks*L, grads_stride, n_actions) floats (tape rows, then reduction partials);
+                                                             orl_rnn_workspace_floats_wide_obs(...) when obs_dim or critic_obs_dim > 64 */
     float* grads;                                         /* (2, grads_stride) true gradients, policy then critic */
     int32_t grads_stride; int32_t reserved1;
     float* loss_acc;                                      /* (8) zeroed by orl_rnn_fwdbwd: policy_loss, entropy, ratio, value_loss sums */
@@ -419,6 +423,10 @@ long long orl_rnn_workspace_floats(long long rows, int grads_stride);
 /* the same for a policy of n_actions actions: a wide head (9..64 actions) tapes dL/dlogits in 64 more floats per row
  * (orl_rnn_tape_width() + 64); equal to orl_rnn_workspace_floats for n_actions <= 8 */
 long long orl_rnn_workspace_floats_for(long long rows, int grads_stride, int n_actions);
+/* the same for observations of obs_dim / critic_obs_dim 1..256: a net wider than 64 tapes its observation in 256 more
+ * floats per row, and its W1 gradient takes a panel buffer of 64 x 256 floats after the partials; equal to
+ * orl_rnn_workspace_floats_for when both widths are <= 64 */
+long long orl_rnn_workspace_floats_wide_obs(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim);
 /* policy GRU rollout for steps [t_begin, t_end) fused with the device env (simple_spread, CartPole, GridWorld); device
  * envs only: ORL_ENV_NONE is rejected (the policy step of host-stepped rows is orl_rnn_act_rows).  CartPole and
  * GridWorld need 16-byte aligned policy_obs and critic_obs (ORL_ERR_BAD_ARG otherwise). */
@@ -442,6 +450,11 @@ int orl_host_insert_rnn(const float* staged, int n_envs, int n_agents, int obs_d
 int orl_host_insert_rnn_wide(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
                              float* masks_next, float* active_masks_next, float* rnn_states_next, float* action_masks_next,
                              int n_actions, float* critic_obs_next, int critic_obs_dim, void* stream);
+/* orl_host_insert_rnn_wide for critic sections of critic_obs_dim in 1..256 (ORL_ERR_BAD_ARG otherwise), the critic of a
+ * GRU MAPPO env wider than 64 included; the same kernel, so for 1..64 it writes what orl_host_insert_rnn_wide writes. */
+int orl_host_insert_rnn_wide_obs(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
+                                 float* masks_next, float* active_masks_next, float* rnn_states_next, float* action_masks_next,
+                                 int n_actions, float* critic_obs_next, int critic_obs_dim, void* stream);
 /* recurrent critic over slots 0..T: value_preds[t] and rnn_states_critic[t+1] */
 int orl_rnn_critic(const OrlRnnArgs* args, void* stream);
 /* chunked BPTT forward + loss + backward of both nets over the minibatch chunks -> grads, loss_acc */

@@ -251,7 +251,10 @@ class PPOAlgorithm:
         mbc = data_chunks // self.num_mini_batch
         rows = mbc * L
         tape_rows = rows * buf.num_agents if joint else rows   # the joint policy tapes every agent row of a step
-        need = int(self._lib.orl_rnn_workspace_floats_for(tape_rows, self.rnn_stride, self.n))   # tape rows + reduction partials
+        if max(self.d, self.dc) > 64:   # wider tape rows (the X field) and the dW1 panel buffer
+            need = int(self._lib.orl_rnn_workspace_floats_wide_obs(tape_rows, self.rnn_stride, self.n, self.d, self.dc))
+        else:
+            need = int(self._lib.orl_rnn_workspace_floats_for(tape_rows, self.rnn_stride, self.n))   # tape rows + reduction partials
         if self.tape is None or self.tape.numel() < need:
             self.tape = torch.empty(need, dtype=torch.float32, device=self.device)
         whole = self.num_mini_batch == 1 and rows == total and not joint

@@ -75,6 +75,11 @@ FLAGS = [
     # panels of the observation in the act, value, eval and FFMA update kernels.  Off, every network keeps its limit of
     # 64 features (NotImplementedError); GRU policies, use_share_model and the device envs keep it either way
     ("use_wide_observations", _bool, False),
+    # GRU policies and critics (use_recurrent_policy / use_naive_recurrent_policy) with observations of 65..256 features,
+    # such as SMAC maps beyond the smallest: W1 staged at a wider leading dimension in the GRU act, critic and update
+    # kernels, and dW1 reduced in 64-column panels.  Off, a GRU net keeps its limit of 64 features (NotImplementedError);
+    # JRPO, use_share_model and the device-env GRU rollout keep it either way
+    ("use_wide_recurrent_observations", _bool, False),
     ("use_tf32", _bool, True),
 ]
 

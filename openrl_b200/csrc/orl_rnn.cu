@@ -141,20 +141,23 @@ __device__ __forceinline__ CatRow warp_categorical_row(const Args& a, rw::V2& x,
 // (orl_host_insert_rnn zeroes the rows of the envs that finish at step t).  Same staged weights, step_forward and
 // sampler as rnn_rollout_warp_kernel: a row's state, logits and action depend neither on R nor on the warp that runs it.
 // NB = 64: the wide head (9..64 actions), sampled by warp_sample_action with the noise keys of the feed-forward wide head.
-template <int R, int NB = MAX_OUT>
-__global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnnArgs a) {
+// DX = 256 (rnn_act_rows_wide_obs_kernel): observations of 65..256 features, W1 staged by load_net_wide.
+template <int R, int NB, int DX>
+__device__ __forceinline__ void act_rows(const OrlRnnArgs& a) {
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * a.n_agents, d = a.obs_dim, n = a.n_actions, t = a.t_begin;
     const rc::Offsets o = rc::rnn_offsets(d, n);
-    const rw::SmemNet W = rw::load_net<NB>(smem, a.policy_params, o, threadIdx.x, W_NT);
+    const rw::SmemNet W = DX == rc::H ? rw::load_net<NB>(smem, a.policy_params, o, threadIdx.x, W_NT)
+                                     : rw::load_net_wide<NB>(smem, a.policy_params, o, threadIdx.x, W_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* scr = smem + rw::smem_net_floats<NB>() + warp * R * rw::SCR;
+    float* scr = smem + (DX == rc::H ? rw::smem_net_floats<NB>() : rw::smem_net_floats_wide<NB>(d)) + warp * R * rw::SCR;
     const uint64_t step = a.rng_step_base + (a.rng_counter ? *a.rng_counter : 0ull);
     float* const no_tape[R] = {};
     const int rows = a.row_end - a.row_begin, groups = (rows + R - 1) / R;
     for (int g = blockIdx.x * W_WPC + warp; g < groups; g += gridDim.x * W_WPC) {
-        rw::V2 x[R], h[R], hn[R];
+        typename rw::XIn<DX>::type x[R];
+        rw::V2 h[R], hn[R];
         float mk[R];
         typename rw::HeadOut<NB>::type logit[R];
         int row[R];
@@ -163,11 +166,12 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnn
             row[r] = a.row_begin + min(g * R + r, rows - 1);   // a ragged tail recomputes the last row; its stores are skipped
             const size_t grow = (size_t)t * B + row[r];
             const float* ob = a.policy_obs + grow * d;
-            x[r] = rw::V2{lane < d ? ob[lane] : 0.f, lane + 32 < d ? ob[lane + 32] : 0.f};
+            if constexpr (DX == rc::H) x[r] = rw::V2{lane < d ? ob[lane] : 0.f, lane + 32 < d ? ob[lane + 32] : 0.f};
+            else x[r] = ob;
             h[r] = rw::ldv(a.rnn_states + grow * rc::H, lane);
             mk[r] = a.masks[grow];
         }
-        rw::step_forward<R, NB>(W, scr, d, n, a.activation_id, x, h, mk, hn, logit, no_tape, lane);
+        rw::step_forward<R, NB, DX>(W, scr, d, n, a.activation_id, x, h, mk, hn, logit, no_tape, lane);
 #pragma unroll
         for (int r = 0; r < R; ++r) {
             if constexpr (NB == MAX_OUT_WIDE) {
@@ -194,26 +198,34 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnn
         }
     }
 }
+template <int R, int NB = MAX_OUT>
+__global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnnArgs a) { act_rows<R, NB, rc::H>(a); }
+template <int R, int NB>
+__global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_wide_obs_kernel(const OrlRnnArgs a) { act_rows<R, NB, rw::MAXD_WIDE>(a); }
 
-// ---- recurrent critic over all T+1 slots: one warp per row ----
-__global__ void __launch_bounds__(W_NT, 1) rnn_critic_warp_kernel(const OrlRnnArgs a) {
+// ---- recurrent critic over all T+1 slots: one warp per row (DX = 256: rnn_critic_wide_obs_kernel) ----
+template <int DX>
+__device__ __forceinline__ void critic_rows(const OrlRnnArgs& a) {
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * a.n_agents, T = a.episode_length, dc = a.critic_obs_dim;
     const rc::Offsets o = rc::rnn_offsets(dc, 1);
-    const rw::SmemNet W = rw::load_net(smem, a.critic_params, o, threadIdx.x, W_NT);
+    const rw::SmemNet W = DX == rc::H ? rw::load_net(smem, a.critic_params, o, threadIdx.x, W_NT)
+                                     : rw::load_net_wide(smem, a.critic_params, o, threadIdx.x, W_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* scr = smem + rw::smem_net_floats() + warp * rw::SCR;
+    float* scr = smem + (DX == rc::H ? rw::smem_net_floats() : rw::smem_net_floats_wide(dc)) + warp * rw::SCR;
     float* const no_tape[1] = {nullptr};
     for (int row = blockIdx.x * W_WPC + warp; row < B; row += gridDim.x * W_WPC) {
         rw::V2 h[1] = {rw::ldv(a.rnn_states_critic + (size_t)row * rc::H, lane)};
         for (int t = 0; t <= T; ++t) {
             const size_t grow = (size_t)t * B + row;
             const float* ob = a.critic_obs + grow * dc;
-            const rw::V2 x[1] = {rw::V2{lane < dc ? ob[lane] : 0.f, lane + 32 < dc ? ob[lane + 32] : 0.f}};
+            typename rw::XIn<DX>::type x[1];
+            if constexpr (DX == rc::H) x[0] = rw::V2{lane < dc ? ob[lane] : 0.f, lane + 32 < dc ? ob[lane + 32] : 0.f};
+            else x[0] = ob;
             const float mk[1] = {a.masks[grow]};
             rw::V2 hn[1]; float out[1][MAX_OUT];
-            rw::step_forward<1>(W, scr, dc, 1, a.activation_id, x, h, mk, hn, out, no_tape, lane);
+            rw::step_forward<1, MAX_OUT, DX>(W, scr, dc, 1, a.activation_id, x, h, mk, hn, out, no_tape, lane);
             if (lane == 0) a.value_preds[grow] = out[0][0];
             if (t < T) {
                 const float keep = a.masks[grow + B] == 0.f ? 0.f : 1.f;   // rnn_states_critic[dones_env] = 0
@@ -223,25 +235,29 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_critic_warp_kernel(const OrlRnnAr
         }
     }
 }
+__global__ void __launch_bounds__(W_NT, 1) rnn_critic_warp_kernel(const OrlRnnArgs a) { critic_rows<rc::H>(a); }
+__global__ void __launch_bounds__(W_NT, 1) rnn_critic_wide_obs_kernel(const OrlRnnArgs a) { critic_rows<rw::MAXD_WIDE>(a); }
 
 // ---- update: one warp per C_R chunks; L forward steps (tape), per-step loss, L backward steps ----
 // AGENT0 (the critic under ORL_PPO_JOINT_ACTION): chunks are recurrent_generator_v3 chunks over f = n*T + t and the
 // critic sees agent 0's row of every step only (to_single_np, ppo.py:222-224, 254-262), buffer row t*B + n*A.
 // NB = 64 (policy only): the wide head; dL/dlogits goes to the tape field TW_DLW of the wider tape rows (TAPE_WIDE).
-template <bool POLICY, bool AGENT0, int C_R, int C_NT, int NB = MAX_OUT>
-__global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArgs a) {
+// DX = 256 (rnn_chunk_wide_obs_kernel): observations of 65..256 features; the rows carry the X field (tape_width_x).
+template <bool POLICY, bool AGENT0, int C_R, int C_NT, int NB, int DX>
+__device__ __forceinline__ void chunk_rows(const OrlRnnArgs& a) {
     static_assert(NB == MAX_OUT || POLICY, "the critic's head is one value");
-    constexpr int C_WPC = C_NT / 32, TW = NB == MAX_OUT ? rw::TAPE_W : rw::TAPE_WIDE;
+    constexpr int C_WPC = C_NT / 32, TW = (NB == MAX_OUT ? rw::TAPE_W : rw::TAPE_WIDE) + (DX == rc::H ? 0 : rw::MAXD_WIDE);
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * a.n_agents, T = a.episode_length, L = a.chunk_length;
     const int d = POLICY ? a.obs_dim : a.critic_obs_dim, n = POLICY ? a.n_actions : 1;
     const float* obs = POLICY ? a.policy_obs : a.critic_obs;
     const float* states = POLICY ? a.rnn_states : a.rnn_states_critic;
     const rc::Offsets o = rc::rnn_offsets(d, n);
-    const rw::SmemNet W = rw::load_net<NB>(smem, POLICY ? a.policy_params : a.critic_params, o, threadIdx.x, C_NT);
+    const rw::SmemNet W = DX == rc::H ? rw::load_net<NB>(smem, POLICY ? a.policy_params : a.critic_params, o, threadIdx.x, C_NT)
+                                     : rw::load_net_wide<NB>(smem, POLICY ? a.policy_params : a.critic_params, o, threadIdx.x, C_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* scr = smem + rw::smem_net_floats<NB>() + warp * C_R * rw::SCR;
+    float* scr = smem + (DX == rc::H ? rw::smem_net_floats<NB>() : rw::smem_net_floats_wide<NB>(d)) + warp * C_R * rw::SCR;
     float loss0 = 0.f, loss1 = 0.f, loss2 = 0.f;   // identical on every lane; lane 0's copy is reduced
 
     const MbConsts mb = mb_consts(a);
@@ -261,7 +277,8 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
             h[r] = rw::ldv(states + ((size_t)(f0[r] % T) * B + row0) * rc::H, lane);
         }
         for (int l = 0; l < L; ++l) {
-            rw::V2 x[C_R], h2[C_R];
+            typename rw::XIn<DX>::type x[C_R];
+            rw::V2 h2[C_R];
             float mk[C_R];
             typename rw::HeadOut<NB>::type out[C_R];
             float* tape[C_R];
@@ -271,11 +288,12 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
                 const long long f = f0[r] + l, row = AGENT0 ? f / T * a.n_agents : f / T, t = f % T;
                 bi[r] = (size_t)t * B + row;
                 const float* ob = obs + bi[r] * d;
-                x[r] = rw::V2{lane < d ? ob[lane] : 0.f, lane + 32 < d ? ob[lane + 32] : 0.f};
+                if constexpr (DX == rc::H) x[r] = rw::V2{lane < d ? ob[lane] : 0.f, lane + 32 < d ? ob[lane + 32] : 0.f};
+                else x[r] = ob;
                 mk[r] = a.masks[bi[r]];
                 tape[r] = a.tape + ((size_t)cpos[r] * L + l) * TW;
             }
-            rw::step_forward<C_R, NB>(W, scr, d, n, a.activation_id, x, h, mk, h2, out, tape, lane);
+            rw::step_forward<C_R, NB, DX>(W, scr, d, n, a.activation_id, x, h, mk, h2, out, tape, lane);
 #pragma unroll
             for (int r = 0; r < C_R; ++r) {
                 h[r] = h2[r];
@@ -334,6 +352,12 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
         if (POLICY) atomicAdd(a.loss_acc + threadIdx.x, s);
         else if (threadIdx.x == 0) atomicAdd(a.loss_acc + 3, s);
     }
+}
+template <bool POLICY, bool AGENT0, int C_R, int C_NT, int NB = MAX_OUT>
+__global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArgs a) { chunk_rows<POLICY, AGENT0, C_R, C_NT, NB, rc::H>(a); }
+template <bool POLICY, int C_R, int NB>
+__global__ void __launch_bounds__(W_NT, 1) rnn_chunk_wide_obs_kernel(const OrlRnnArgs a) {
+    chunk_rows<POLICY, false, C_R, W_NT, NB, rw::MAXD_WIDE>(a);
 }
 
 // ---- joint-action policy update (ORL_PPO_JOINT_ACTION, JRPO): one warp per recurrent_generator_v3 chunk ----
@@ -432,13 +456,15 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_joint_policy_warp_kernel(const Or
 }
 
 // ---- parameter gradients of one net from its tape (orl::reduce_tape); every job fits the gemm tiles: TQ_X + 64 <= TAPE_W ----
-// A wide head (n > 8) reads dL/dlogits from the appended field TW_DLW of its TAPE_WIDE rows.
+// A wide head (n > 8) reads dL/dlogits from the appended field TW_DLW of its TAPE_WIDE rows.  A wide observation (d > 64)
+// has no W1 job here: its gradient comes from w1_panel_jobs.
 TapeJobs make_jobs(int d, int n) {
     const rc::Offsets o = rc::rnn_offsets(d, n);
     TapeJobs t; int g = 0, c = 0;
     auto gemm = [&](int p, int M, int q, int N, int out) { t.gemm[g++] = TapeJob{p, M, q, N, out}; };
     auto col = [&](int p, int M, int out) { t.col[c++] = TapeJob{p, M, -1, 1, out}; };
-    gemm(rc::TP_DZ1, rc::H, rc::TQ_X, d, o.w1);     col(rc::TP_DZ1, rc::H, o.b1);
+    if (d <= rc::MAXD) gemm(rc::TP_DZ1, rc::H, rc::TQ_X, d, o.w1);
+    col(rc::TP_DZ1, rc::H, o.b1);
     col(rc::TS_DY1N1, rc::H, o.g1);                  col(rc::TS_DY1, rc::H, o.be1);
     gemm(rc::TP_DZ3, rc::H, rc::TQ_Y1, rc::H, o.w3); col(rc::TP_DZ3, rc::H, o.b3);
     col(rc::TS_DY3N3, rc::H, o.g3);                  col(rc::TS_DY3, rc::H, o.be3);
@@ -453,6 +479,28 @@ TapeJobs make_jobs(int d, int n) {
 
 // workspace = tape (rows x tape_width(n_actions)) followed by the reduction partials (row blocks x grads_stride)
 long long ws_tape_floats(long long rows, int n_actions) { return rows * rw::tape_width(n_actions); }
+
+// dW1 of a wide observation (d > 64) as 64-column panels sum_rows dZ1^T X_p over the X field: panel p lands at
+// W1P_PANEL * p as [64][min(64, d - 64 p)], in a panel buffer of W1P_FLOATS that w1_scatter_kernel unpacks into W1's [64][d]
+constexpr int W1P_PANEL = rc::H * 64, W1P_FLOATS = W1P_PANEL * rw::MAXD_WIDE / 64;
+TapeJobs w1_panel_jobs(int d, int n) {
+    TapeJobs t; t.n_gemm = 0; t.n_col = 0;
+    for (int p = 0; 64 * p < d; ++p)
+        t.gemm[t.n_gemm++] = TapeJob{rc::TP_DZ1, rc::H, rw::tape_width(n) + 64 * p, std::min(64, d - 64 * p), W1P_PANEL * p};
+    return t;
+}
+__global__ void w1_scatter_kernel(const float* __restrict__ panels, int d, float* __restrict__ w1) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= rc::H * d) return;
+    const int m = i / d, k = i % d, p = k / 64, np = min(64, d - 64 * p);
+    w1[i] = panels[W1P_PANEL * p + m * np + (k - 64 * p)];
+}
+// the update's workspace: the larger of the two nets' tapes, the reduction partials and, with a wide observation, the panel buffer
+long long ws_floats(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim) {
+    const long long tw = std::max(rw::tape_width_x(n_actions, obs_dim), rw::tape_width_x(1, critic_obs_dim));
+    const bool wide = obs_dim > rc::MAXD || critic_obs_dim > rc::MAXD;
+    return rows * tw + (rows + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK * grads_stride + (wide ? W1P_FLOATS : 0);
+}
 
 // ---- optimizer: per-net global-norm clip + Adam on the true-layout gradients (one CTA per net) ----
 __global__ void __launch_bounds__(1024) rnn_apply_kernel(const OrlRnnArgs a) {
@@ -475,17 +523,87 @@ constexpr size_t w_smem(int rows_per_warp) {   // weights of one net + the per-w
     return (size_t)(rw::smem_net_floats<NB>() + rw::smem_scratch_floats(W_WPC, rows_per_warp)) * sizeof(float);
 }
 static_assert(w_smem<MAX_OUT_WIDE>(2) <= 227 * 1024, "the wide policy's weights and scratch fit the opt-in shared memory");
+// A wide observation (d > 64): W1 at w1_ld(d).  Rows per warp: two where the weights, the scratch and the chunk kernel's
+// 192 B of static loss slots fit the 227 KB opt-in limit, else one.  Only the wide head's net at d > 240 needs one.
+constexpr size_t SMEM_OPTIN = 227 * 1024, CHUNK_STATIC_SMEM = 3 * W_WPC * sizeof(float);
+template <int NB = MAX_OUT>
+constexpr size_t w_smem_wide(int d, int rows_per_warp) {
+    return (size_t)(rw::smem_net_floats_wide<NB>(d) + rw::smem_scratch_floats(W_WPC, rows_per_warp)) * sizeof(float);
+}
+template <int NB = MAX_OUT>
+constexpr int wide_rows_per_warp(int d) { return w_smem_wide<NB>(d, 2) + CHUNK_STATIC_SMEM <= SMEM_OPTIN ? 2 : 1; }
+static_assert(wide_rows_per_warp<MAX_OUT>(rw::MAXD_WIDE) == 2, "a narrow-head net of any width runs two rows per warp");
+static_assert(wide_rows_per_warp<MAX_OUT_WIDE>(240) == 2 && wide_rows_per_warp<MAX_OUT_WIDE>(241) == 1, "the R switch");
+static_assert(w_smem_wide<MAX_OUT_WIDE>(rw::MAXD_WIDE, 1) + CHUNK_STATIC_SMEM <= SMEM_OPTIN, "every width fits at one row per warp");
 int warp_grid(long long units) {   // persistent CTAs: one per SM, never more than the work needs
     const long long need = (units + W_WPC - 1) / W_WPC;
     return (int)std::max(1LL, std::min<long long>(need, orl::sm_count()));
 }
 
-int check_common(const OrlRnnArgs& a) {
+// max_obs: 64 for the device-env rollout, 256 (MAXD_WIDE) for the host-stepped entries
+int check_common(const OrlRnnArgs& a, int max_obs = rc::MAXD) {
     ORL_CHECK_ARG(a.n_envs > 0 && a.n_agents > 0 && a.episode_length > 0, "n_envs / n_agents / episode_length");
-    ORL_CHECK_ARG(a.obs_dim > 0 && a.obs_dim <= rc::MAXD && a.critic_obs_dim > 0 && a.critic_obs_dim <= rc::MAXD, "obs dims (<= 64)");
+    if (max_obs == rc::MAXD) {
+        ORL_CHECK_ARG(a.obs_dim > 0 && a.obs_dim <= rc::MAXD && a.critic_obs_dim > 0 && a.critic_obs_dim <= rc::MAXD, "obs dims (<= 64)");
+    } else {
+        ORL_CHECK_ARG(a.obs_dim > 0 && a.obs_dim <= max_obs && a.critic_obs_dim > 0 && a.critic_obs_dim <= max_obs,
+                      "obs dims must be in 1..256");
+    }
     ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= MAX_OUT_WIDE, "n_actions must be in 1..64");
     ORL_CHECK_ARG(a.activation_id >= 0 && a.activation_id <= 3, "activation_id");
     return 0;
+}
+
+// the chunk kernel of one net for orl_rnn_fwdbwd with a wide observation on either net: the parent's instances for a
+// net of d <= 64, else rnn_chunk_wide_obs_kernel at the rows per warp that fit
+template <bool POLICY>
+int launch_chunks_wide_obs(const OrlRnnArgs& a, cudaStream_t st) {
+    const int d = POLICY ? a.obs_dim : a.critic_obs_dim;
+    const bool wide_head = POLICY && a.n_actions > MAX_OUT;
+    const int g2 = warp_grid((a.n_chunks + 1) / 2);
+    int e = 0;
+    if (d <= rc::MAXD && wide_head) {
+        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<true, false, 2, W_NT, MAX_OUT_WIDE>, w_smem<MAX_OUT_WIDE>(2)))) return e;
+        rnn_chunk_warp_kernel<true, false, 2, W_NT, MAX_OUT_WIDE><<<g2, W_NT, w_smem<MAX_OUT_WIDE>(2), st>>>(a);
+    } else if (d <= rc::MAXD) {
+        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<POLICY, false, 2, W_NT>, w_smem(2)))) return e;
+        rnn_chunk_warp_kernel<POLICY, false, 2, W_NT><<<g2, W_NT, w_smem(2), st>>>(a);
+    } else if (wide_head && wide_rows_per_warp<MAX_OUT_WIDE>(d) == 1) {
+        if ((e = orl::allow_dynamic_smem(rnn_chunk_wide_obs_kernel<true, 1, MAX_OUT_WIDE>, w_smem_wide<MAX_OUT_WIDE>(d, 1)))) return e;
+        rnn_chunk_wide_obs_kernel<true, 1, MAX_OUT_WIDE><<<warp_grid(a.n_chunks), W_NT, w_smem_wide<MAX_OUT_WIDE>(d, 1), st>>>(a);
+    } else if (wide_head) {
+        if ((e = orl::allow_dynamic_smem(rnn_chunk_wide_obs_kernel<true, 2, MAX_OUT_WIDE>, w_smem_wide<MAX_OUT_WIDE>(d, 2)))) return e;
+        rnn_chunk_wide_obs_kernel<true, 2, MAX_OUT_WIDE><<<g2, W_NT, w_smem_wide<MAX_OUT_WIDE>(d, 2), st>>>(a);
+    } else {
+        if ((e = orl::allow_dynamic_smem(rnn_chunk_wide_obs_kernel<POLICY, 2, MAX_OUT>, w_smem_wide(d, 2)))) return e;
+        rnn_chunk_wide_obs_kernel<POLICY, 2, MAX_OUT><<<g2, W_NT, w_smem_wide(d, 2), st>>>(a);
+    }
+    return 0;
+}
+
+// orl_rnn_fwdbwd with a wide observation on either net (not JRPO).  Each net's tape rows are tape_width_x wide; a wide
+// net's W1 gradient is a second reduction, of the 64-column panels into the panel buffer, unpacked into W1's rows.
+int fwdbwd_wide_obs(const OrlRnnArgs& a, cudaStream_t st) {
+    int e = orl::check_cuda(cudaMemsetAsync(a.loss_acc, 0, 8 * sizeof(float), st), "memset loss_acc");
+    if (e) return e;
+    const long long rows = a.n_chunks * a.chunk_length;
+    const long long tw = std::max(rw::tape_width_x(a.n_actions, a.obs_dim), rw::tape_width_x(1, a.critic_obs_dim));
+    float* partials = a.tape + rows * tw;
+    float* panels = partials + (rows + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK * a.grads_stride;
+    for (int net = 0; net < 2; ++net) {
+        const int d = net == 0 ? a.obs_dim : a.critic_obs_dim, n = net == 0 ? a.n_actions : 1;
+        if ((e = net == 0 ? launch_chunks_wide_obs<true>(a, st) : launch_chunks_wide_obs<false>(a, st))) return e;
+        const rc::Offsets o = rc::rnn_offsets(d, n);
+        float* grads = a.grads + (size_t)net * a.grads_stride;
+        const int tw_net = rw::tape_width_x(n, d);
+        if ((e = orl::reduce_tape(a.tape, tw_net, rows, make_jobs(d, n), partials, a.grads_stride, o.total, grads, st))) return e;
+        if (d > rc::MAXD) {   // W1's entries of the first reduction are overwritten here
+            const int last = (d - 1) / 64, used = W1P_PANEL * last + rc::H * (d - 64 * last);
+            if ((e = orl::reduce_tape(a.tape, tw_net, rows, w1_panel_jobs(d, n), partials, W1P_FLOATS, used, panels, st))) return e;
+            w1_scatter_kernel<<<(rc::H * d + 255) / 256, 256, 0, st>>>(panels, d, grads + o.w1);
+        }
+    }
+    return orl::check_cuda(cudaGetLastError(), "rnn update launches");
 }
 
 }  // namespace
@@ -494,6 +612,9 @@ extern "C" {
 
 int orl_rnn_param_count(int obs_dim, int n_out) { return rc::rnn_offsets(obs_dim, n_out).total; }
 int orl_rnn_tape_width(void) { return rw::TAPE_W; }
+long long orl_rnn_workspace_floats_wide_obs(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim) {
+    return ws_floats(rows, grads_stride, n_actions, obs_dim, critic_obs_dim);
+}
 long long orl_rnn_workspace_floats(long long rows, int grads_stride) { return orl_rnn_workspace_floats_for(rows, grads_stride, 1); }
 long long orl_rnn_workspace_floats_for(long long rows, int grads_stride, int n_actions) {
     return ws_tape_floats(rows, n_actions) + (rows + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK * grads_stride;
@@ -541,7 +662,7 @@ int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
 int orl_rnn_act_rows(const OrlRnnArgs* ap, void* stream) {
     ORL_CHECK_ARG(ap, "args");
     const OrlRnnArgs& a = *ap;
-    if (int e = check_common(a)) return e;
+    if (int e = check_common(a, rw::MAXD_WIDE)) return e;
     ORL_CHECK_ARG(a.policy_params && a.policy_obs && a.rnn_states && a.actions && a.action_log_probs && a.masks, "null act buffer");
     ORL_CHECK_ARG(a.t_begin >= 0 && a.t_begin < a.episode_length, "slot t_begin");
     ORL_CHECK_ARG(a.row_begin >= 0 && a.row_begin <= a.row_end && (long long)a.row_end <= (long long)a.n_envs * a.n_agents, "row range");
@@ -550,7 +671,24 @@ int orl_rnn_act_rows(const OrlRnnArgs* ap, void* stream) {
     if (rows > 0) {
         // one row per warp while the rows leave warps of the persistent grid idle, two (every weight read feeds both) beyond
         int e = 0;
-        if (a.n_actions > MAX_OUT) {   // the wide head: same row grouping
+        const int d = a.obs_dim, R = rows <= orl::sm_count() * W_WPC ? 1 : 2;
+        if (d > rc::MAXD && a.n_actions > MAX_OUT) {   // wide observation: R = 2 only where it fits
+            if (R == 1 || wide_rows_per_warp<MAX_OUT_WIDE>(d) == 1) {
+                if ((e = orl::allow_dynamic_smem(rnn_act_rows_wide_obs_kernel<1, MAX_OUT_WIDE>, w_smem_wide<MAX_OUT_WIDE>(d, 1)))) return e;
+                rnn_act_rows_wide_obs_kernel<1, MAX_OUT_WIDE><<<warp_grid(rows), W_NT, w_smem_wide<MAX_OUT_WIDE>(d, 1), st>>>(a);
+            } else {
+                if ((e = orl::allow_dynamic_smem(rnn_act_rows_wide_obs_kernel<2, MAX_OUT_WIDE>, w_smem_wide<MAX_OUT_WIDE>(d, 2)))) return e;
+                rnn_act_rows_wide_obs_kernel<2, MAX_OUT_WIDE><<<warp_grid((rows + 1) / 2), W_NT, w_smem_wide<MAX_OUT_WIDE>(d, 2), st>>>(a);
+            }
+        } else if (d > rc::MAXD) {
+            if (R == 1) {
+                if ((e = orl::allow_dynamic_smem(rnn_act_rows_wide_obs_kernel<1, MAX_OUT>, w_smem_wide(d, 1)))) return e;
+                rnn_act_rows_wide_obs_kernel<1, MAX_OUT><<<warp_grid(rows), W_NT, w_smem_wide(d, 1), st>>>(a);
+            } else {
+                if ((e = orl::allow_dynamic_smem(rnn_act_rows_wide_obs_kernel<2, MAX_OUT>, w_smem_wide(d, 2)))) return e;
+                rnn_act_rows_wide_obs_kernel<2, MAX_OUT><<<warp_grid((rows + 1) / 2), W_NT, w_smem_wide(d, 2), st>>>(a);
+            }
+        } else if (a.n_actions > MAX_OUT) {   // the wide head: same row grouping
             if (rows <= orl::sm_count() * W_WPC) {
                 if ((e = orl::allow_dynamic_smem(rnn_act_rows_warp_kernel<1, MAX_OUT_WIDE>, w_smem<MAX_OUT_WIDE>(1)))) return e;
                 rnn_act_rows_warp_kernel<1, MAX_OUT_WIDE><<<warp_grid(rows), W_NT, w_smem<MAX_OUT_WIDE>(1), st>>>(a);
@@ -573,9 +711,15 @@ int orl_rnn_act_rows(const OrlRnnArgs* ap, void* stream) {
 int orl_rnn_critic(const OrlRnnArgs* ap, void* stream) {
     ORL_CHECK_ARG(ap, "args");
     const OrlRnnArgs& a = *ap;
-    if (int e = check_common(a)) return e;
+    if (int e = check_common(a, rw::MAXD_WIDE)) return e;
     ORL_CHECK_ARG(a.critic_params && a.critic_obs && a.rnn_states_critic && a.masks && a.value_preds, "null critic buffer");
     const int B = a.n_envs * a.n_agents;
+    if (a.critic_obs_dim > rc::MAXD) {
+        const size_t sm = w_smem_wide(a.critic_obs_dim, 1);
+        if (int e = orl::allow_dynamic_smem(rnn_critic_wide_obs_kernel, sm)) return e;
+        rnn_critic_wide_obs_kernel<<<warp_grid(B), W_NT, sm, (cudaStream_t)stream>>>(a);
+        return orl::check_cuda(cudaGetLastError(), "rnn_critic_wide_obs_kernel launch");
+    }
     if (int e = orl::allow_dynamic_smem(rnn_critic_warp_kernel, w_smem(1))) return e;
     rnn_critic_warp_kernel<<<warp_grid(B), W_NT, w_smem(1), (cudaStream_t)stream>>>(a);
     return orl::check_cuda(cudaGetLastError(), "rnn_critic_warp_kernel launch");
@@ -584,7 +728,7 @@ int orl_rnn_critic(const OrlRnnArgs* ap, void* stream) {
 int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
     ORL_CHECK_ARG(ap, "args");
     const OrlRnnArgs& a = *ap;
-    if (int e = check_common(a)) return e;
+    if (int e = check_common(a, rw::MAXD_WIDE)) return e;
     ORL_CHECK_ARG(a.chunk_length >= 1 && a.chunk_length <= LMAX, "chunk_length (data_chunk_length) must be in [1, 32]");
     ORL_CHECK_ARG(a.n_chunks > 0 && a.chunk_ids, "chunks");
     ORL_CHECK_ARG(a.policy_params && a.critic_params && a.policy_obs && a.critic_obs && a.rnn_states && a.rnn_states_critic &&
@@ -601,7 +745,9 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
         ORL_CHECK_ARG(a.n_chunks * a.chunk_length <= (long long)a.n_envs * a.episode_length, "v3 chunks exceed the N*T samples");
         ORL_CHECK_ARG(!a.action_masks, "ORL_PPO_JOINT_ACTION takes no action_masks (simple_spread reports none)");
         ORL_CHECK_ARG(a.n_actions <= MAX_OUT, "ORL_PPO_JOINT_ACTION is built for up to 8 actions");
+        ORL_CHECK_ARG(a.obs_dim <= rc::MAXD && a.critic_obs_dim <= rc::MAXD, "ORL_PPO_JOINT_ACTION is built for obs dims 1..64");
     }
+    if (a.obs_dim > rc::MAXD || a.critic_obs_dim > rc::MAXD) return fwdbwd_wide_obs(a, (cudaStream_t)stream);
     const bool wide = a.n_actions > MAX_OUT;
     cudaStream_t st = (cudaStream_t)stream;
     int e = orl::check_cuda(cudaMemsetAsync(a.loss_acc, 0, 8 * sizeof(float), st), "memset loss_acc");
@@ -639,7 +785,7 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
 int orl_rnn_apply(const OrlRnnArgs* ap, void* stream) {
     ORL_CHECK_ARG(ap, "args");
     const OrlRnnArgs& a = *ap;
-    if (int e = check_common(a)) return e;
+    if (int e = check_common(a, rw::MAXD_WIDE)) return e;
     ORL_CHECK_ARG(a.policy_params && a.critic_params && a.grads && a.loss_acc && a.policy_adam_m && a.policy_adam_v &&
                       a.critic_adam_m && a.critic_adam_v && a.adam_steps && a.lrs && a.train_info && a.mb_stats, "null optimizer buffer");
     ORL_CHECK_ARG(a.n_chunks > 0 && a.chunk_length >= 1, "chunks");

@@ -20,6 +20,12 @@
 // warp_sum into out[R][8] on every lane.  NB = 64 (MAXN_WIDE) treats the logits as one more lane-owned 64-vector
 // (lane l owns actions l and l + 32): matvec64 over a 64-row head block whose rows >= n and bias entries >= n are zero.
 // Per-lane arrays of 64 logits would spill under the 128-register cap of the 512-thread kernels.
+//
+// Observation width bound DX (a template parameter of step_forward): DX = 64 (H) takes x as a V2 and stages W1 at LD.
+// DX = 256 (MAXD_WIDE, observations of 65..256 features): a row's x is loaded from global memory straight into its
+// scratch row (SCR = 256 floats), W1 is staged at the odd leading dimension w1_ld(d) = pad4(d) + 1 (load_net_wide) and
+// fc1 is matvec64 with K = pad4(d).  With a tape, x also goes to an X field of MAXD_WIDE floats appended to the row
+// (tape_width_x), the Q operand of the 64-column panels of dW1; TQ_X is left unused there.  Only fc1 depends on d.
 #pragma once
 #include "orl_mlp.cuh"
 #include "orl_rnn_core.h"
@@ -34,6 +40,10 @@ constexpr int TW_A1 = rc::TAPE, TW_N1 = TW_A1 + 64, TW_N3 = TW_N1 + 64, TW_R = T
 constexpr int TW_DLW = TAPE_W, TAPE_WIDE = TW_DLW + 64;   // 1808: the wide policy head's dL/dlogits (P operand of Wh, bh)
 __host__ __device__ constexpr int head_bound(int n) { return n > MAXN ? MAXN_WIDE : MAXN; }
 __host__ __device__ constexpr int tape_width(int n) { return n > MAXN ? TAPE_WIDE : TAPE_W; }
+constexpr int MAXD_WIDE = 256;
+__host__ __device__ constexpr int w1_ld(int d) { return ((d + 3) & ~3) + 1; }
+// a wide-observation row (d > 64): the X field [tape_width(n), tape_width(n) + MAXD_WIDE) follows the row
+__host__ __device__ constexpr int tape_width_x(int n, int d) { return tape_width(n) + (d > H ? MAXD_WIDE : 0); }
 
 struct V2 { float a, b; };
 
@@ -43,6 +53,10 @@ struct SmemNet {
 };
 template <int NB = MAXN>
 __host__ __device__ constexpr int smem_net_floats() { return (H + H + G3 + G3 + NB) * LD + 8 * H + 2 * G3 + NB; }
+
+// the same net with W1 at leading dimension w1_ld(d) (load_net_wide)
+template <int NB = MAXN>
+__host__ __device__ constexpr int smem_net_floats_wide(int d) { return smem_net_floats<NB>() + H * (w1_ld(d) - LD); }
 
 // Stage one net (flat layout of rc::rnn_offsets) into shared memory; W1 columns k >= d and head rows m >= n are zero.
 template <int NB = MAXN>
@@ -57,6 +71,48 @@ __device__ inline SmemNet load_net(float* s, const float* __restrict__ P, const 
     for (int i = tid; i < H * LD; i += nthreads) {
         const int j = i / LD, k = i % LD;
         w1[i] = k < o.d ? P[o.w1 + j * o.d + k] : 0.f;
+        w3[i] = k < H ? P[o.w3 + j * H + k] : 0.f;
+    }
+    for (int i = tid; i < G3 * LD; i += nthreads) {
+        const int j = i / LD, k = i % LD;
+        wih[i] = k < H ? P[o.wih + j * H + k] : 0.f;
+        whh[i] = k < H ? P[o.whh + j * H + k] : 0.f;
+    }
+    for (int i = tid; i < NB * LD; i += nthreads) {
+        const int j = i / LD, k = i % LD;
+        wh[i] = (j < o.n && k < H) ? P[o.wh + j * H + k] : 0.f;
+    }
+    for (int i = tid; i < H; i += nthreads) {
+        vec[i] = P[o.b1 + i]; vec[H + i] = P[o.g1 + i]; vec[2 * H + i] = P[o.be1 + i];
+        vec[3 * H + i] = P[o.b3 + i]; vec[4 * H + i] = P[o.g3 + i]; vec[5 * H + i] = P[o.be3 + i];
+        vec[6 * H + i] = P[o.gr + i]; vec[7 * H + i] = P[o.ber + i];
+    }
+    for (int i = tid; i < G3; i += nthreads) { vec[8 * H + i] = P[o.bih + i]; vec[8 * H + G3 + i] = P[o.bhh + i]; }
+    for (int i = tid; i < NB; i += nthreads) vec[8 * H + 2 * G3 + i] = i < o.n ? P[o.bh + i] : 0.f;
+    SmemNet n;
+    n.w1 = w1; n.w3 = w3; n.wih = wih; n.whh = whh; n.wh = wh;
+    n.b1 = vec; n.g1 = vec + H; n.be1 = vec + 2 * H; n.b3 = vec + 3 * H; n.g3 = vec + 4 * H; n.be3 = vec + 5 * H;
+    n.gr = vec + 6 * H; n.ber = vec + 7 * H; n.bih = vec + 8 * H; n.bhh = vec + 8 * H + G3; n.bh = vec + 8 * H + 2 * G3;
+    return n;
+}
+
+// load_net for d > 64: W1 [64][w1_ld(d)] first (columns k >= d zero), then the rest in load_net's layout
+template <int NB = MAXN>
+__device__ inline SmemNet load_net_wide(float* s, const float* __restrict__ P, const rc::Offsets& o, int tid, int nthreads) {
+    static_assert(NB == MAXN || NB == MAXN_WIDE, "head width bound");
+    const int ld1 = w1_ld(o.d);
+    float* w1 = s; s += H * ld1;
+    float* w3 = s; s += H * LD;
+    float* wih = s; s += G3 * LD;
+    float* whh = s; s += G3 * LD;
+    float* wh = s; s += NB * LD;
+    float* vec = s;
+    for (int i = tid; i < H * ld1; i += nthreads) {
+        const int j = i / ld1, k = i % ld1;
+        w1[i] = k < o.d ? P[o.w1 + j * o.d + k] : 0.f;
+    }
+    for (int i = tid; i < H * LD; i += nthreads) {
+        const int j = i / LD, k = i % LD;
         w3[i] = k < H ? P[o.w3 + j * H + k] : 0.f;
     }
     for (int i = tid; i < G3 * LD; i += nthreads) {
@@ -111,15 +167,16 @@ __device__ __forceinline__ void park(float* scr, int off, const V2 (&v)[R], int 
     __syncwarp();
 }
 
-// out[r]_j = bias_j + sum_{k<K4} W[j][k] * in[r][k]; lane owns rows j = lane, lane+32 of the 64-row block at W;
-// in = scratch slot (K4 = K rounded up to 4: the inputs / weight columns beyond K are zero).
+// out[r]_j = bias_j + sum_{k<K4} W[j][k] * in[r][k]; lane owns rows j = lane, lane+32 of the 64-row block at W (leading
+// dimension ld, odd); in = scratch slot (K4 = K rounded up to 4: the inputs / weight columns beyond K are zero).
 template <int R>
-__device__ __forceinline__ void matvec64(const float* W, const float* bias, const float* scr, int off, int K, int lane, V2 (&out)[R]) {
+__device__ __forceinline__ void matvec64(const float* W, const float* bias, const float* scr, int off, int K, int lane, V2 (&out)[R],
+                                         int ld = LD) {
     float s0[R], s1[R];
 #pragma unroll
     for (int r = 0; r < R; ++r) { s0[r] = bias[lane]; s1[r] = bias[lane + 32]; }
-    const float* r0 = W + lane * LD;
-    const float* r1 = W + (lane + 32) * LD;
+    const float* r0 = W + lane * ld;
+    const float* r1 = W + (lane + 32) * ld;
     const int K4 = (K + 3) & ~3;
     for (int k = 0; k < K4; k += 4) {
         const float w00 = r0[k], w01 = r0[k + 1], w02 = r0[k + 2], w03 = r0[k + 3];
@@ -212,18 +269,44 @@ __device__ __forceinline__ WarpSoftmax warp_log_softmax(V2& x, int n, const floa
 // head outputs of one row: NB = 8, out[m] for m < n on every lane; NB = 64, the lane-owned logits
 template <int NB> struct HeadOut { using type = float[MAXN]; };
 template <> struct HeadOut<MAXN_WIDE> { using type = V2; };
+// observation of one row: DX = 64, lane-owned (zero beyond d); DX = 256, the row's d floats in global memory
+template <int DX> struct XIn { using type = V2; };
+template <> struct XIn<MAXD_WIDE> { using type = const float*; };
 
-// One forward step of R rows.  x: observation (zero beyond d), h_in: hidden state, out[r]: the head outputs (HeadOut).
+// Load R observation rows of d <= 256 features into their scratch rows, zero from d up to the end of the last 64-column
+// panel; with a tape, also into its X field at xoff (the Q operand of the dW1 panels: every column a panel reads is finite).
+template <int R>
+__device__ __forceinline__ void stage_x(float* scr, const float* const (&x)[R], int d, float* const (&tape)[R], int xoff, int lane) {
+    const int kp = (d + 63) & ~63;
+    __syncwarp();   // every lane is done reading what the scratch held before
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+        for (int k = lane; k < kp; k += 32) {
+            const float v = k < d ? x[r][k] : 0.f;
+            scr[r * SCR + k] = v;
+            if (tape[r]) tape[r][xoff + k] = v;
+        }
+    }
+    __syncwarp();
+}
+
+// One forward step of R rows.  x: observation (XIn; zero beyond d), h_in: hidden state, out[r]: the head outputs (HeadOut).
 // tape[r] != nullptr: the Q operands and the activations for the backward step go to the row's tape.
-// scr: this warp's scratch (R * SCR floats of shared memory).
-template <int R, int NB = MAXN>
-__device__ __forceinline__ void step_forward(const SmemNet& W, float* scr, int d, int n, int act_id, const V2 (&x)[R], const V2 (&h_in)[R],
-                                             const float (&mask)[R], V2 (&h_out)[R], typename HeadOut<NB>::type (&out)[R],
-                                             float* const (&tape)[R], int lane) {
+// scr: this warp's scratch (R * SCR floats of shared memory).  DX = 256: W from load_net_wide.
+template <int R, int NB = MAXN, int DX = H>
+__device__ __forceinline__ void step_forward(const SmemNet& W, float* scr, int d, int n, int act_id, const typename XIn<DX>::type (&x)[R],
+                                             const V2 (&h_in)[R], const float (&mask)[R], V2 (&h_out)[R],
+                                             typename HeadOut<NB>::type (&out)[R], float* const (&tape)[R], int lane) {
+    static_assert(DX == H || DX == MAXD_WIDE, "observation width bound");
     const V2 g1 = ldv(W.g1, lane), be1 = ldv(W.be1, lane), g3 = ldv(W.g3, lane), be3 = ldv(W.be3, lane);
     V2 t0[R], y1[R], y3[R], hm[R];
-    park<R>(scr, 0, x, lane);
-    matvec64<R>(W.w1, W.b1, scr, 0, d, lane, t0);
+    if constexpr (DX == H) {
+        park<R>(scr, 0, x, lane);
+        matvec64<R>(W.w1, W.b1, scr, 0, d, lane, t0);
+    } else {
+        stage_x<R>(scr, x, d, tape, NB == MAXN ? TAPE_W : TAPE_WIDE, lane);
+        matvec64<R>(W.w1, W.b1, scr, 0, d, lane, t0, w1_ld(d));
+    }
 #pragma unroll
     for (int r = 0; r < R; ++r) {
         const V2 a1{rc::act_fwd(t0[r].a, act_id), rc::act_fwd(t0[r].b, act_id)};
@@ -231,7 +314,8 @@ __device__ __forceinline__ void step_forward(const SmemNet& W, float* scr, int d
         const V2 n1 = ln_fwd(a1, rstd1);
         y1[r] = V2{fmaf(n1.a, g1.a, be1.a), fmaf(n1.b, g1.b, be1.b)};
         if (tape[r]) {
-            stv(tape[r] + rc::TQ_X, lane, x[r]); stv(tape[r] + TW_A1, lane, a1); stv(tape[r] + TW_N1, lane, n1);
+            if constexpr (DX == H) stv(tape[r] + rc::TQ_X, lane, x[r]);
+            stv(tape[r] + TW_A1, lane, a1); stv(tape[r] + TW_N1, lane, n1);
             stv(tape[r] + rc::TQ_Y1, lane, y1[r]);
             if (lane == 0) { tape[r][TW_SC] = rstd1; tape[r][TW_SC + 3] = mask[r]; }
         }

@@ -597,16 +597,18 @@ extern "C" int orl_host_insert_wide_obs(const float* staged, int n_envs, int n_a
                        n_actions, critic_obs_next, critic_obs_dim, stream, orl::MAX_OBS_WIDE);
 }
 
-// the two GRU inserts: masks of 1..max_actions actions
+// the three GRU inserts: masks of 1..max_actions actions, critic sections of 1..max_critic features
 static int host_insert_rnn(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next, float* rewards,
                            float* masks_next, float* active_masks_next, float* rnn_states_next, float* action_masks_next,
-                           int n_actions, float* critic_obs_next, int critic_obs_dim, void* stream, int max_actions) {
+                           int n_actions, float* critic_obs_next, int critic_obs_dim, void* stream, int max_actions,
+                           int max_critic = orl::OBS_PANEL) {
     ORL_CHECK_ARG(staged && policy_obs_next && rewards && masks_next && active_masks_next && rnn_states_next, "null buffer");
     ORL_CHECK_ARG(n_envs > 0 && n_agents > 0 && obs_dim > 0, "shapes");
     ORL_CHECK_ARG(!action_masks_next || (n_actions > 0 && n_actions <= max_actions),
                   max_actions == orl::MAX_OUT ? "n_actions must be in 1..8 (orl_host_insert_rnn_wide: 1..64)"
                                               : "n_actions must be in 1..64");
-    ORL_CHECK_ARG(!critic_obs_next || (critic_obs_dim > 0 && critic_obs_dim <= 64), "critic_obs_dim must be in 1..64");
+    ORL_CHECK_ARG(!critic_obs_next || (critic_obs_dim > 0 && critic_obs_dim <= max_critic),
+                  max_critic == orl::OBS_PANEL ? "critic_obs_dim must be in 1..64" : "critic_obs_dim must be in 1..256");
     ORL_CHECK_ARG(reinterpret_cast<uintptr_t>(rnn_states_next) % 16 == 0, "rnn_states_next must be 16-byte aligned");
     const int B = n_envs * n_agents;
     host_insert_rnn_kernel<<<(B + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
@@ -629,4 +631,12 @@ extern "C" int orl_host_insert_rnn_wide(const float* staged, int n_envs, int n_a
                                         void* stream) {
     return host_insert_rnn(staged, n_envs, n_agents, obs_dim, policy_obs_next, rewards, masks_next, active_masks_next, rnn_states_next,
                            action_masks_next, n_actions, critic_obs_next, critic_obs_dim, stream, orl::MAX_OUT_WIDE);
+}
+
+extern "C" int orl_host_insert_rnn_wide_obs(const float* staged, int n_envs, int n_agents, int obs_dim, float* policy_obs_next,
+                                            float* rewards, float* masks_next, float* active_masks_next, float* rnn_states_next,
+                                            float* action_masks_next, int n_actions, float* critic_obs_next, int critic_obs_dim,
+                                            void* stream) {
+    return host_insert_rnn(staged, n_envs, n_agents, obs_dim, policy_obs_next, rewards, masks_next, active_masks_next, rnn_states_next,
+                           action_masks_next, n_actions, critic_obs_next, critic_obs_dim, stream, orl::MAX_OUT_WIDE, orl::MAX_OBS_WIDE);
 }

@@ -4,7 +4,8 @@
 //   gemm job   part[out_off + m*N + k] = sum_rows tape[r][p_off+m] * tape[r][q_off+k]     (register-tiled, 12x4 per thread)
 //   column job part[out_off + m]       = sum_rows tape[r][p_off+m]
 // Stage 2: grads[i] = sum over row blocks of partials[rb][i], pairwise in a fixed order.
-// The kernels are built per tape width (the GRU's, the wide-head GRU policy's and the shared model's): with the width a runtime value the gemm
+// The kernels are built per tape width (the GRU's and the wide-head GRU policy's, each with or without the X field of a
+// wide observation, and the shared model's): with the width a runtime value the gemm
 // kernel's row addressing takes 92 registers instead of 80 on sm_90a, one CTA less per SM.
 #include "orl_common.cuh"
 #include "orl_deep_core.h"
@@ -122,7 +123,8 @@ __global__ void row_block_sum_kernel(const float* __restrict__ partials, int row
 // the tile loads of tape_gemm_kernel: 16-byte cp.async of whole float4 (aligned offsets), a Q tile of TR_N columns
 // and a P tile of 16*ceil(M/16) columns, all inside the tape row
 bool jobs_fit(const TapeJobs& jobs, int tape_width) {
-    if (tape_width % 4 != 0 || jobs.n_gemm < 1 || jobs.n_gemm > TAPE_MAX_GEMM_JOBS || jobs.n_col < 1 || jobs.n_col > TAPE_MAX_COL_JOBS)
+    if (tape_width % 4 != 0 || jobs.n_gemm < 0 || jobs.n_gemm > TAPE_MAX_GEMM_JOBS || jobs.n_col < 0 || jobs.n_col > TAPE_MAX_COL_JOBS ||
+        jobs.n_gemm + jobs.n_col < 1)
         return false;
     for (int j = 0; j < jobs.n_gemm; ++j) {
         const TapeJob& g = jobs.gemm[j];
@@ -139,9 +141,11 @@ bool jobs_fit(const TapeJobs& jobs, int tape_width) {
 
 template <int TAPE_W>
 int launch_jobs(const float* tape, long long rows, const TapeJobs& jobs, float* partials, int stride, int rb, cudaStream_t st) {
-    if (int e = allow_dynamic_smem(tape_gemm_kernel<TAPE_W>, TR_SMEM)) return e;
-    tape_gemm_kernel<TAPE_W><<<dim3(rb, jobs.n_gemm), TR_NT, TR_SMEM, st>>>(tape, rows, jobs, partials, stride);
-    tape_colsum_kernel<TAPE_W><<<dim3(rb, jobs.n_col), TR_MAX_M, 0, st>>>(tape, rows, jobs, partials, stride);
+    if (jobs.n_gemm > 0) {
+        if (int e = allow_dynamic_smem(tape_gemm_kernel<TAPE_W>, TR_SMEM)) return e;
+        tape_gemm_kernel<TAPE_W><<<dim3(rb, jobs.n_gemm), TR_NT, TR_SMEM, st>>>(tape, rows, jobs, partials, stride);
+    }
+    if (jobs.n_col > 0) tape_colsum_kernel<TAPE_W><<<dim3(rb, jobs.n_col), TR_MAX_M, 0, st>>>(tape, rows, jobs, partials, stride);
     return 0;
 }
 
@@ -158,6 +162,10 @@ int reduce_tape(const float* tape, int tape_width, long long rows, const TapeJob
     switch (tape_width) {
         case orl_rnnw::TAPE_W: e = launch_jobs<orl_rnnw::TAPE_W>(tape, rows, jobs, partials, stride, rb, st); break;
         case orl_rnnw::TAPE_WIDE: e = launch_jobs<orl_rnnw::TAPE_WIDE>(tape, rows, jobs, partials, stride, rb, st); break;
+        case orl_rnnw::TAPE_W + orl_rnnw::MAXD_WIDE:   // the GRU's rows with the X field of a wide observation
+            e = launch_jobs<orl_rnnw::TAPE_W + orl_rnnw::MAXD_WIDE>(tape, rows, jobs, partials, stride, rb, st); break;
+        case orl_rnnw::TAPE_WIDE + orl_rnnw::MAXD_WIDE:
+            e = launch_jobs<orl_rnnw::TAPE_WIDE + orl_rnnw::MAXD_WIDE>(tape, rows, jobs, partials, stride, rb, st); break;
         case orl_deep::TAPE: e = launch_jobs<orl_deep::TAPE>(tape, rows, jobs, partials, stride, rb, st); break;
         case orl_deep::TAPE_GAUSSIAN: e = launch_jobs<orl_deep::TAPE_GAUSSIAN>(tape, rows, jobs, partials, stride, rb, st); break;
         default: ORL_CHECK_ARG(false, "tape_width (one of the GRU's or the shared model's tapes)");

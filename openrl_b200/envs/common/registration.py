@@ -35,7 +35,8 @@ def make(id: str, env_num: int = 1, asynchronous: bool = False, add_monitor: boo
         env_fns = _gymnasium_thunks(id, env_num, render_mode, **kwargs)
     # `asynchronous` selects the reference's AsyncVectorEnv (one process per env); the host stepping here is synchronous —
     # the overlap with the device comes from HostVecEnv's double-buffered staging, not from worker processes
-    # the reference's make receives cfg in kwargs (registration.py:45); its option lets Dict entries be 65..256 wide
+    # the reference's make receives cfg in kwargs (registration.py:45); either wide-observation option (feed-forward or
+    # GRU nets) lets Dict entries be 65..256 wide, and each network checks the option of its own kind
     cfg = kwargs.get("cfg")
-    wide = bool(getattr(cfg, "use_wide_observations", False)) if cfg is not None else False
+    wide = cfg is not None and bool(getattr(cfg, "use_wide_observations", False) or getattr(cfg, "use_wide_recurrent_observations", False))
     return HostVecEnv(SyncHostVecEnv(env_fns, auto_reset=auto_reset, env_name=id), device=device, wide_observations=wide)

@@ -22,16 +22,25 @@ def _init(module, gain, use_orthogonal=True):
     return module
 
 
-def check_obs_shape(shape, wide=False):
+def check_obs_shape(shape, wide=False, option="use_wide_observations"):
     """The observation shapes the kernels take: flat vectors of width 1..64, and of 65..256 when `wide` (a feed-forward
-    policy or critic with cfg.use_wide_observations: fc1 runs over 64-wide panels of the observation)."""
+    policy or critic with cfg.use_wide_observations: fc1 runs over 64-wide panels of the observation; a GRU policy or
+    critic with cfg.use_wide_recurrent_observations, named by `option`)."""
     if len(shape) == 1 and shape[0] <= (256 if wide else 64):
         return
     if wide:
-        raise NotImplementedError("vector observations of width <= 256 only (the bound of use_wide_observations); "
+        raise NotImplementedError(f"vector observations of width <= 256 only (the bound of {option}); "
                                   f"got shape {tuple(shape)}")
     raise NotImplementedError("vector observations of width <= 64 only (65..256: feed-forward policies and critics "
                               f"with use_wide_observations, not GRU policies or use_share_model); got shape {tuple(shape)}")
+
+
+def recurrent_obs_check(cfg, recurrent):
+    """check_obs_shape's options for a policy or critic: feed-forward nets take 65..256 features with
+    cfg.use_wide_observations, GRU nets with cfg.use_wide_recurrent_observations."""
+    if recurrent:
+        return {"wide": bool(getattr(cfg, "use_wide_recurrent_observations", False)), "option": "use_wide_recurrent_observations"}
+    return {"wide": bool(getattr(cfg, "use_wide_observations", False))}
 
 
 class MLPLayer(nn.Module):

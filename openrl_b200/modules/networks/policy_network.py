@@ -2,7 +2,7 @@
 import torch
 import torch.nn as nn
 
-from .base import ACTLayer, FlatParams, MLPBase, RNNLayer, check_obs_shape
+from .base import ACTLayer, FlatParams, MLPBase, RNNLayer, check_obs_shape, recurrent_obs_check
 
 
 def _policy_shape(space):
@@ -16,7 +16,7 @@ class PolicyNetwork(nn.Module):
         self.recurrent = bool(cfg.use_recurrent_policy or cfg.use_naive_recurrent_policy)
         self.hidden_size = cfg.hidden_size
         shape = _policy_shape(input_space)
-        check_obs_shape(shape, wide=getattr(cfg, "use_wide_observations", False) and not self.recurrent)
+        check_obs_shape(shape, **recurrent_obs_check(cfg, self.recurrent))
         self.obs_dim = shape[0]
         self.activation_id = cfg.activation_id
         self.base = MLPBase(cfg, shape)

@@ -3,7 +3,7 @@ with the `value_normalizer` attribute the algorithm looks up (ppo_module.py:212-
 import torch
 import torch.nn as nn
 
-from .base import FlatParams, MLPBase, PopArt, RNNLayer, ValueNorm, _init, check_obs_shape
+from .base import FlatParams, MLPBase, PopArt, RNNLayer, ValueNorm, _init, check_obs_shape, recurrent_obs_check
 
 
 def _critic_shape(space):
@@ -15,7 +15,7 @@ class ValueNetwork(nn.Module):
         super().__init__()
         self.recurrent = bool(cfg.use_recurrent_policy or cfg.use_naive_recurrent_policy)
         shape = _critic_shape(input_space)
-        check_obs_shape(shape, wide=getattr(cfg, "use_wide_observations", False) and not self.recurrent)
+        check_obs_shape(shape, **recurrent_obs_check(cfg, self.recurrent))
         self.obs_dim = shape[0]
         self.activation_id = cfg.activation_id
         self.base = MLPBase(cfg, shape)
