@@ -393,8 +393,9 @@ typedef struct OrlRnnArgs {
     double* env_f64; uint64_t* env_u64; int32_t* env_i32; const int32_t* env_table;
     float* ep_return; int32_t* ep_length; double* episode_stats;
     const double* gae_stats; const double* mb_stats; float* vn_state;
-    float* tape;                                          /* workspace: orl_rnn_workspace_floats_for(n_chunks*L, grads_stride, n_actions) floats (tape rows, then reduction partials);
-                                                             orl_rnn_workspace_floats_wide_obs(...) when obs_dim or critic_obs_dim > 64 */
+    float* tape;                                          /* workspace: orl_rnn_workspace_floats_wide_obs(n_chunks*L, grads_stride, n_actions, obs_dim,
+                                                             critic_obs_dim) floats (the larger net's tape rows, the reduction partials, then with a
+                                                             net wider than 64 the dW1 panel buffer); n_chunks*L*A rows with ORL_PPO_JOINT_ACTION */
     float* grads;                                         /* (2, grads_stride) true gradients, policy then critic */
     int32_t grads_stride; int32_t reserved1;
     float* loss_acc;                                      /* (8) zeroed by orl_rnn_fwdbwd: policy_loss, entropy, ratio, value_loss sums */

@@ -390,18 +390,9 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
     }
 }
 
-template <int NB>
-__global__ void __launch_bounds__(P_NT, 1) ppo_fwdbwd_kernel(const OrlPpoArgs a) {
-    extern __shared__ __align__(16) float smem[];
-    const int G = a.grid_per_net;
-    if ((int)blockIdx.x < G) ppo_net_pass<true, NB>(a, smem, blockIdx.x, G);
-    else ppo_net_pass<false>(a, smem, blockIdx.x - G, G);
-}
-
-// ppo_fwdbwd_kernel when either net's observation is wider than 64: the pass of a net with PANELS_* runs fc1 in panels,
-// the other one is the pass of ppo_fwdbwd_kernel<NB>
+// PANELS_POLICY / PANELS_CRITIC: that net's observation is wider than 64 and its pass runs fc1 in panels
 template <int NB, bool PANELS_POLICY, bool PANELS_CRITIC>
-__global__ void __launch_bounds__(P_NT, 1) ppo_fwdbwd_wide_obs_kernel(const OrlPpoArgs a) {
+__global__ void __launch_bounds__(P_NT, 1) ppo_fwdbwd_kernel(const OrlPpoArgs a) {
     extern __shared__ __align__(16) float smem[];
     const int G = a.grid_per_net;
     if ((int)blockIdx.x < G) ppo_net_pass<true, NB, PANELS_POLICY>(a, smem, blockIdx.x, G);
@@ -671,16 +662,15 @@ extern "C" int orl_ppo_fwdbwd(const OrlPpoArgs* args, void* stream) {
     }
     const bool wide = a.n_actions > orl::MAX_OUT;
     // a panelled pass uses the buffers of the d = 64 layout
-    const bool wide_obs = std::max(a.obs_dim, a.critic_obs_dim) > orl::OBS_PANEL;
     const int ds = std::min(a.obs_dim, orl::OBS_PANEL), dcs = std::min(a.critic_obs_dim, orl::OBS_PANEL);
     const size_t smem = wide ? fwdbwd_wide_smem_bytes(ds, dcs) : fwdbwd_smem_bytes(ds, dcs);
     const bool pp = a.obs_dim > orl::OBS_PANEL, pc = a.critic_obs_dim > orl::OBS_PANEL;
     void (*const kern)(OrlPpoArgs) =
-        !wide_obs ? (wide ? ppo_fwdbwd_kernel<orl::MAX_OUT_WIDE> : ppo_fwdbwd_kernel<orl::MAX_OUT>)
-        : wide ? (pp && pc ? ppo_fwdbwd_wide_obs_kernel<orl::MAX_OUT_WIDE, true, true>
-                  : pp ? ppo_fwdbwd_wide_obs_kernel<orl::MAX_OUT_WIDE, true, false> : ppo_fwdbwd_wide_obs_kernel<orl::MAX_OUT_WIDE, false, true>)
-               : (pp && pc ? ppo_fwdbwd_wide_obs_kernel<orl::MAX_OUT, true, true>
-                  : pp ? ppo_fwdbwd_wide_obs_kernel<orl::MAX_OUT, true, false> : ppo_fwdbwd_wide_obs_kernel<orl::MAX_OUT, false, true>);
+        !pp && !pc ? (wide ? ppo_fwdbwd_kernel<orl::MAX_OUT_WIDE, false, false> : ppo_fwdbwd_kernel<orl::MAX_OUT, false, false>)
+        : wide ? (pp && pc ? ppo_fwdbwd_kernel<orl::MAX_OUT_WIDE, true, true>
+                  : pp ? ppo_fwdbwd_kernel<orl::MAX_OUT_WIDE, true, false> : ppo_fwdbwd_kernel<orl::MAX_OUT_WIDE, false, true>)
+               : (pp && pc ? ppo_fwdbwd_kernel<orl::MAX_OUT, true, true>
+                  : pp ? ppo_fwdbwd_kernel<orl::MAX_OUT, true, false> : ppo_fwdbwd_kernel<orl::MAX_OUT, false, true>);
     if (int e = orl::allow_dynamic_smem(kern, 227 * 1024)) return e;
     kern<<<2 * a.grid_per_net, P_NT, smem, reinterpret_cast<cudaStream_t>(stream)>>>(a);
     ORL_LAUNCH_CHECK("ppo_fwdbwd_kernel");

@@ -46,7 +46,7 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_rollout_warp_kernel(const OrlRnnA
     const rw::SmemNet W = rw::load_net(smem, a.policy_params, o, threadIdx.x, W_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* scr = smem + rw::smem_net_floats() + warp * A * rw::SCR;
+    float* scr = smem + rw::smem_net_floats(D) + warp * A * rw::SCR;
     const EnvPtrs E = env_ptrs(a, 0);   // the env randomness is keyed by the launch's env index, like the action noise
     const uint64_t rng_base = a.rng_step_base + (a.rng_counter ? *a.rng_counter : 0ull);
     float* const no_tape[A] = {};
@@ -141,17 +141,16 @@ __device__ __forceinline__ CatRow warp_categorical_row(const Args& a, rw::V2& x,
 // (orl_host_insert_rnn zeroes the rows of the envs that finish at step t).  Same staged weights, step_forward and
 // sampler as rnn_rollout_warp_kernel: a row's state, logits and action depend neither on R nor on the warp that runs it.
 // NB = 64: the wide head (9..64 actions), sampled by warp_sample_action with the noise keys of the feed-forward wide head.
-// DX = 256 (rnn_act_rows_wide_obs_kernel): observations of 65..256 features, W1 staged by load_net_wide.
+// DX = 256: observations of 65..256 features.
 template <int R, int NB, int DX>
-__device__ __forceinline__ void act_rows(const OrlRnnArgs& a) {
+__global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnnArgs a) {
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * a.n_agents, d = a.obs_dim, n = a.n_actions, t = a.t_begin;
     const rc::Offsets o = rc::rnn_offsets(d, n);
-    const rw::SmemNet W = DX == rc::H ? rw::load_net<NB>(smem, a.policy_params, o, threadIdx.x, W_NT)
-                                     : rw::load_net_wide<NB>(smem, a.policy_params, o, threadIdx.x, W_NT);
+    const rw::SmemNet W = rw::load_net<NB, DX>(smem, a.policy_params, o, threadIdx.x, W_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* scr = smem + (DX == rc::H ? rw::smem_net_floats<NB>() : rw::smem_net_floats_wide<NB>(d)) + warp * R * rw::SCR;
+    float* scr = smem + rw::smem_net_floats<NB, DX>(d) + warp * R * rw::SCR;
     const uint64_t step = a.rng_step_base + (a.rng_counter ? *a.rng_counter : 0ull);
     float* const no_tape[R] = {};
     const int rows = a.row_end - a.row_begin, groups = (rows + R - 1) / R;
@@ -198,22 +197,17 @@ __device__ __forceinline__ void act_rows(const OrlRnnArgs& a) {
         }
     }
 }
-template <int R, int NB = MAX_OUT>
-__global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnnArgs a) { act_rows<R, NB, rc::H>(a); }
-template <int R, int NB>
-__global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_wide_obs_kernel(const OrlRnnArgs a) { act_rows<R, NB, rw::MAXD_WIDE>(a); }
 
-// ---- recurrent critic over all T+1 slots: one warp per row (DX = 256: rnn_critic_wide_obs_kernel) ----
+// ---- recurrent critic over all T+1 slots: one warp per row (DX = 256: observations of 65..256 features) ----
 template <int DX>
-__device__ __forceinline__ void critic_rows(const OrlRnnArgs& a) {
+__global__ void __launch_bounds__(W_NT, 1) rnn_critic_warp_kernel(const OrlRnnArgs a) {
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * a.n_agents, T = a.episode_length, dc = a.critic_obs_dim;
     const rc::Offsets o = rc::rnn_offsets(dc, 1);
-    const rw::SmemNet W = DX == rc::H ? rw::load_net(smem, a.critic_params, o, threadIdx.x, W_NT)
-                                     : rw::load_net_wide(smem, a.critic_params, o, threadIdx.x, W_NT);
+    const rw::SmemNet W = rw::load_net<MAX_OUT, DX>(smem, a.critic_params, o, threadIdx.x, W_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* scr = smem + (DX == rc::H ? rw::smem_net_floats() : rw::smem_net_floats_wide(dc)) + warp * rw::SCR;
+    float* scr = smem + rw::smem_net_floats<MAX_OUT, DX>(dc) + warp * rw::SCR;
     float* const no_tape[1] = {nullptr};
     for (int row = blockIdx.x * W_WPC + warp; row < B; row += gridDim.x * W_WPC) {
         rw::V2 h[1] = {rw::ldv(a.rnn_states_critic + (size_t)row * rc::H, lane)};
@@ -235,36 +229,33 @@ __device__ __forceinline__ void critic_rows(const OrlRnnArgs& a) {
         }
     }
 }
-__global__ void __launch_bounds__(W_NT, 1) rnn_critic_warp_kernel(const OrlRnnArgs a) { critic_rows<rc::H>(a); }
-__global__ void __launch_bounds__(W_NT, 1) rnn_critic_wide_obs_kernel(const OrlRnnArgs a) { critic_rows<rw::MAXD_WIDE>(a); }
 
-// ---- update: one warp per C_R chunks; L forward steps (tape), per-step loss, L backward steps ----
+// ---- update: one warp per R chunks; L forward steps (tape), per-step loss, L backward steps ----
 // AGENT0 (the critic under ORL_PPO_JOINT_ACTION): chunks are recurrent_generator_v3 chunks over f = n*T + t and the
 // critic sees agent 0's row of every step only (to_single_np, ppo.py:222-224, 254-262), buffer row t*B + n*A.
 // NB = 64 (policy only): the wide head; dL/dlogits goes to the tape field TW_DLW of the wider tape rows (TAPE_WIDE).
-// DX = 256 (rnn_chunk_wide_obs_kernel): observations of 65..256 features; the rows carry the X field (tape_width_x).
-template <bool POLICY, bool AGENT0, int C_R, int C_NT, int NB, int DX>
-__device__ __forceinline__ void chunk_rows(const OrlRnnArgs& a) {
+// DX = 256: observations of 65..256 features; the rows carry the X field (tape_width_x).
+template <bool POLICY, bool AGENT0, int C_R, int NB, int DX>
+__global__ void __launch_bounds__(W_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArgs a) {
     static_assert(NB == MAX_OUT || POLICY, "the critic's head is one value");
-    constexpr int C_WPC = C_NT / 32, TW = (NB == MAX_OUT ? rw::TAPE_W : rw::TAPE_WIDE) + (DX == rc::H ? 0 : rw::MAXD_WIDE);
+    constexpr int TW = (NB == MAX_OUT ? rw::TAPE_W : rw::TAPE_WIDE) + (DX == rc::H ? 0 : rw::MAXD_WIDE);
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * a.n_agents, T = a.episode_length, L = a.chunk_length;
     const int d = POLICY ? a.obs_dim : a.critic_obs_dim, n = POLICY ? a.n_actions : 1;
     const float* obs = POLICY ? a.policy_obs : a.critic_obs;
     const float* states = POLICY ? a.rnn_states : a.rnn_states_critic;
     const rc::Offsets o = rc::rnn_offsets(d, n);
-    const rw::SmemNet W = DX == rc::H ? rw::load_net<NB>(smem, POLICY ? a.policy_params : a.critic_params, o, threadIdx.x, C_NT)
-                                     : rw::load_net_wide<NB>(smem, POLICY ? a.policy_params : a.critic_params, o, threadIdx.x, C_NT);
+    const rw::SmemNet W = rw::load_net<NB, DX>(smem, POLICY ? a.policy_params : a.critic_params, o, threadIdx.x, W_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* scr = smem + (DX == rc::H ? rw::smem_net_floats<NB>() : rw::smem_net_floats_wide<NB>(d)) + warp * C_R * rw::SCR;
+    float* scr = smem + rw::smem_net_floats<NB, DX>(d) + warp * C_R * rw::SCR;
     float loss0 = 0.f, loss1 = 0.f, loss2 = 0.f;   // identical on every lane; lane 0's copy is reduced
 
     const MbConsts mb = mb_consts(a);
     const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS, val_masks = a.flags & ORL_PPO_VALUE_ACTIVE_MASKS;
 
     const long long n_groups = (a.n_chunks + C_R - 1) / C_R;
-    for (long long grp = (long long)blockIdx.x * C_WPC + warp; grp < n_groups; grp += (long long)gridDim.x * C_WPC) {
+    for (long long grp = (long long)blockIdx.x * W_WPC + warp; grp < n_groups; grp += (long long)gridDim.x * W_WPC) {
         long long cpos[C_R], f0[C_R];
         bool valid[C_R];
         rw::V2 h[C_R];
@@ -343,21 +334,15 @@ __device__ __forceinline__ void chunk_rows(const OrlRnnArgs& a) {
             rw::step_backward<C_R, NB>(W, scr, n, a.activation_id, tape, dh, lane);
         }
     }
-    __shared__ float red[3][C_WPC];
+    __shared__ float red[3][W_WPC];
     if (lane == 0) { red[0][warp] = loss0; red[1][warp] = loss1; red[2][warp] = loss2; }
     __syncthreads();
     if (threadIdx.x < 3) {
         float s = 0.f;
-        for (int w = 0; w < C_WPC; ++w) s += red[threadIdx.x][w];
+        for (int w = 0; w < W_WPC; ++w) s += red[threadIdx.x][w];
         if (POLICY) atomicAdd(a.loss_acc + threadIdx.x, s);
         else if (threadIdx.x == 0) atomicAdd(a.loss_acc + 3, s);
     }
-}
-template <bool POLICY, bool AGENT0, int C_R, int C_NT, int NB = MAX_OUT>
-__global__ void __launch_bounds__(C_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArgs a) { chunk_rows<POLICY, AGENT0, C_R, C_NT, NB, rc::H>(a); }
-template <bool POLICY, int C_R, int NB>
-__global__ void __launch_bounds__(W_NT, 1) rnn_chunk_wide_obs_kernel(const OrlRnnArgs a) {
-    chunk_rows<POLICY, false, C_R, W_NT, NB, rw::MAXD_WIDE>(a);
 }
 
 // ---- joint-action policy update (ORL_PPO_JOINT_ACTION, JRPO): one warp per recurrent_generator_v3 chunk ----
@@ -367,17 +352,16 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_chunk_wide_obs_kernel(const OrlRn
 // mask over the agent-0 active sum (mb_stats[2]) or 1/groups; every agent row receives the same dL/dlogp.  The
 // entropy stays per agent row, weighted by every agent's active mask over the all-agent active sum (mb_stats[5]) or
 // 1/(groups*A) (ppo.py:254-319).  Tape row of (chunk c, step l, agent ag): (c*L + l)*A + ag.
-template <int A, int C_NT>
-__global__ void __launch_bounds__(C_NT, 1) rnn_joint_policy_warp_kernel(const OrlRnnArgs a) {
-    constexpr int C_WPC = C_NT / 32;
+template <int A>
+__global__ void __launch_bounds__(W_NT, 1) rnn_joint_policy_warp_kernel(const OrlRnnArgs a) {
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * A, T = a.episode_length, L = a.chunk_length;
     const int d = a.obs_dim, n = a.n_actions;
     const rc::Offsets o = rc::rnn_offsets(d, n);
-    const rw::SmemNet W = rw::load_net(smem, a.policy_params, o, threadIdx.x, C_NT);
+    const rw::SmemNet W = rw::load_net(smem, a.policy_params, o, threadIdx.x, W_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    float* scr = smem + rw::smem_net_floats() + warp * A * rw::SCR;
+    float* scr = smem + rw::smem_net_floats(d) + warp * A * rw::SCR;
     float loss0 = 0.f, loss1 = 0.f, loss2 = 0.f;   // identical on every lane; lane 0's copy is reduced
 
     const double groups_d = loss_rows(a);
@@ -386,7 +370,7 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_joint_policy_warp_kernel(const Or
     const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS;
     const AdvNorm advn = make_adv_norm(a.gae_stats, a.flags & ORL_PPO_ADV_NORMALIZE);
 
-    for (long long c = (long long)blockIdx.x * C_WPC + warp; c < a.n_chunks; c += (long long)gridDim.x * C_WPC) {
+    for (long long c = (long long)blockIdx.x * W_WPC + warp; c < a.n_chunks; c += (long long)gridDim.x * W_WPC) {
         const long long f0 = a.chunk_ids[c] * (long long)L;
         const size_t s0 = (size_t)(f0 % T) * B + (size_t)(f0 / T) * A;   // agent 0 of the chunk's first sample
         rw::V2 h[A];
@@ -445,12 +429,12 @@ __global__ void __launch_bounds__(C_NT, 1) rnn_joint_policy_warp_kernel(const Or
             rw::step_backward<A>(W, scr, n, a.activation_id, tape, dh, lane);
         }
     }
-    __shared__ float red[3][C_WPC];
+    __shared__ float red[3][W_WPC];
     if (lane == 0) { red[0][warp] = loss0; red[1][warp] = loss1; red[2][warp] = loss2; }
     __syncthreads();
     if (threadIdx.x < 3) {
         float s = 0.f;
-        for (int w = 0; w < C_WPC; ++w) s += red[threadIdx.x][w];
+        for (int w = 0; w < W_WPC; ++w) s += red[threadIdx.x][w];
         atomicAdd(a.loss_acc + threadIdx.x, s);
     }
 }
@@ -477,9 +461,6 @@ TapeJobs make_jobs(int d, int n) {
     return t;
 }
 
-// workspace = tape (rows x tape_width(n_actions)) followed by the reduction partials (row blocks x grads_stride)
-long long ws_tape_floats(long long rows, int n_actions) { return rows * rw::tape_width(n_actions); }
-
 // dW1 of a wide observation (d > 64) as 64-column panels sum_rows dZ1^T X_p over the X field: panel p lands at
 // W1P_PANEL * p as [64][min(64, d - 64 p)], in a panel buffer of W1P_FLOATS that w1_scatter_kernel unpacks into W1's [64][d]
 constexpr int W1P_PANEL = rc::H * 64, W1P_FLOATS = W1P_PANEL * rw::MAXD_WIDE / 64;
@@ -495,7 +476,8 @@ __global__ void w1_scatter_kernel(const float* __restrict__ panels, int d, float
     const int m = i / d, k = i % d, p = k / 64, np = min(64, d - 64 * p);
     w1[i] = panels[W1P_PANEL * p + m * np + (k - 64 * p)];
 }
-// the update's workspace: the larger of the two nets' tapes, the reduction partials and, with a wide observation, the panel buffer
+// the update's workspace: the larger of the two nets' tapes, the reduction partials and, with a wide observation, the panel
+// buffer.  JRPO sizes it with rows = its policy tape's A rows per chunk step, the larger tape there.
 long long ws_floats(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim) {
     const long long tw = std::max(rw::tape_width_x(n_actions, obs_dim), rw::tape_width_x(1, critic_obs_dim));
     const bool wide = obs_dim > rc::MAXD || critic_obs_dim > rc::MAXD;
@@ -518,26 +500,33 @@ __global__ void __launch_bounds__(1024) rnn_apply_kernel(const OrlRnnArgs a) {
     }
 }
 
-template <int NB = MAX_OUT>
-constexpr size_t w_smem(int rows_per_warp) {   // weights of one net + the per-warp mat-vec scratch
-    return (size_t)(rw::smem_net_floats<NB>() + rw::smem_scratch_floats(W_WPC, rows_per_warp)) * sizeof(float);
+// weights of one net staged by load_net<NB, DX> + the per-warp mat-vec scratch of R rows
+template <int NB, int DX>
+constexpr size_t w_smem(int d, int rows_per_warp) {
+    return (size_t)(rw::smem_net_floats<NB, DX>(d) + rw::smem_scratch_floats(W_WPC, rows_per_warp)) * sizeof(float);
 }
-static_assert(w_smem<MAX_OUT_WIDE>(2) <= 227 * 1024, "the wide policy's weights and scratch fit the opt-in shared memory");
+static_assert(w_smem<MAX_OUT_WIDE, rc::H>(rc::MAXD, 2) <= 227 * 1024, "the wide policy's weights and scratch fit the opt-in shared memory");
 // A wide observation (d > 64): W1 at w1_ld(d).  Rows per warp: two where the weights, the scratch and the chunk kernel's
 // 192 B of static loss slots fit the 227 KB opt-in limit, else one.  Only the wide head's net at d > 240 needs one.
 constexpr size_t SMEM_OPTIN = 227 * 1024, CHUNK_STATIC_SMEM = 3 * W_WPC * sizeof(float);
-template <int NB = MAX_OUT>
-constexpr size_t w_smem_wide(int d, int rows_per_warp) {
-    return (size_t)(rw::smem_net_floats_wide<NB>(d) + rw::smem_scratch_floats(W_WPC, rows_per_warp)) * sizeof(float);
-}
-template <int NB = MAX_OUT>
-constexpr int wide_rows_per_warp(int d) { return w_smem_wide<NB>(d, 2) + CHUNK_STATIC_SMEM <= SMEM_OPTIN ? 2 : 1; }
+template <int NB>
+constexpr int wide_rows_per_warp(int d) { return w_smem<NB, rw::MAXD_WIDE>(d, 2) + CHUNK_STATIC_SMEM <= SMEM_OPTIN ? 2 : 1; }
 static_assert(wide_rows_per_warp<MAX_OUT>(rw::MAXD_WIDE) == 2, "a narrow-head net of any width runs two rows per warp");
 static_assert(wide_rows_per_warp<MAX_OUT_WIDE>(240) == 2 && wide_rows_per_warp<MAX_OUT_WIDE>(241) == 1, "the R switch");
-static_assert(w_smem_wide<MAX_OUT_WIDE>(rw::MAXD_WIDE, 1) + CHUNK_STATIC_SMEM <= SMEM_OPTIN, "every width fits at one row per warp");
+static_assert(w_smem<MAX_OUT_WIDE, rw::MAXD_WIDE>(rw::MAXD_WIDE, 1) + CHUNK_STATIC_SMEM <= SMEM_OPTIN, "every width fits at one row per warp");
+// the only bounds at which two rows per warp may not fit (the static_asserts above)
+template <int NB, int DX>
+constexpr bool may_need_one_row = NB == MAX_OUT_WIDE && DX == rw::MAXD_WIDE;
+
 int warp_grid(long long units) {   // persistent CTAs: one per SM, never more than the work needs
     const long long need = (units + W_WPC - 1) / W_WPC;
     return (int)std::max(1LL, std::min<long long>(need, orl::sm_count()));
+}
+// every launch of a dynamic-shared-memory kernel here: `units` warp work items (envs, rows, row pairs, chunks)
+int launch(void (*kern)(OrlRnnArgs), long long units, size_t smem, const OrlRnnArgs& a, cudaStream_t st) {
+    if (int e = orl::allow_dynamic_smem(kern, smem)) return e;
+    kern<<<warp_grid(units), W_NT, smem, st>>>(a);
+    return 0;
 }
 
 // max_obs: 64 for the device-env rollout, 256 (MAXD_WIDE) for the host-stepped entries
@@ -554,56 +543,39 @@ int check_common(const OrlRnnArgs& a, int max_obs = rc::MAXD) {
     return 0;
 }
 
-// the chunk kernel of one net for orl_rnn_fwdbwd with a wide observation on either net: the parent's instances for a
-// net of d <= 64, else rnn_chunk_wide_obs_kernel at the rows per warp that fit
-template <bool POLICY>
-int launch_chunks_wide_obs(const OrlRnnArgs& a, cudaStream_t st) {
-    const int d = POLICY ? a.obs_dim : a.critic_obs_dim;
-    const bool wide_head = POLICY && a.n_actions > MAX_OUT;
-    const int g2 = warp_grid((a.n_chunks + 1) / 2);
-    int e = 0;
-    if (d <= rc::MAXD && wide_head) {
-        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<true, false, 2, W_NT, MAX_OUT_WIDE>, w_smem<MAX_OUT_WIDE>(2)))) return e;
-        rnn_chunk_warp_kernel<true, false, 2, W_NT, MAX_OUT_WIDE><<<g2, W_NT, w_smem<MAX_OUT_WIDE>(2), st>>>(a);
-    } else if (d <= rc::MAXD) {
-        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<POLICY, false, 2, W_NT>, w_smem(2)))) return e;
-        rnn_chunk_warp_kernel<POLICY, false, 2, W_NT><<<g2, W_NT, w_smem(2), st>>>(a);
-    } else if (wide_head && wide_rows_per_warp<MAX_OUT_WIDE>(d) == 1) {
-        if ((e = orl::allow_dynamic_smem(rnn_chunk_wide_obs_kernel<true, 1, MAX_OUT_WIDE>, w_smem_wide<MAX_OUT_WIDE>(d, 1)))) return e;
-        rnn_chunk_wide_obs_kernel<true, 1, MAX_OUT_WIDE><<<warp_grid(a.n_chunks), W_NT, w_smem_wide<MAX_OUT_WIDE>(d, 1), st>>>(a);
-    } else if (wide_head) {
-        if ((e = orl::allow_dynamic_smem(rnn_chunk_wide_obs_kernel<true, 2, MAX_OUT_WIDE>, w_smem_wide<MAX_OUT_WIDE>(d, 2)))) return e;
-        rnn_chunk_wide_obs_kernel<true, 2, MAX_OUT_WIDE><<<g2, W_NT, w_smem_wide<MAX_OUT_WIDE>(d, 2), st>>>(a);
-    } else {
-        if ((e = orl::allow_dynamic_smem(rnn_chunk_wide_obs_kernel<POLICY, 2, MAX_OUT>, w_smem_wide(d, 2)))) return e;
-        rnn_chunk_wide_obs_kernel<POLICY, 2, MAX_OUT><<<g2, W_NT, w_smem_wide(d, 2), st>>>(a);
-    }
-    return 0;
+// the act over `rows` host-stepped rows: one row per warp while the rows leave warps of the persistent grid idle, else
+// two (every weight read feeds both) where they fit
+template <int NB, int DX>
+int launch_act_rows(const OrlRnnArgs& a, int rows, cudaStream_t st) {
+    const bool one = rows <= orl::sm_count() * W_WPC || (may_need_one_row<NB, DX> && wide_rows_per_warp<NB>(a.obs_dim) == 1);
+    return one ? launch(rnn_act_rows_warp_kernel<1, NB, DX>, rows, w_smem<NB, DX>(a.obs_dim, 1), a, st)
+               : launch(rnn_act_rows_warp_kernel<2, NB, DX>, (rows + 1) / 2, w_smem<NB, DX>(a.obs_dim, 2), a, st);
 }
 
-// orl_rnn_fwdbwd with a wide observation on either net (not JRPO).  Each net's tape rows are tape_width_x wide; a wide
-// net's W1 gradient is a second reduction, of the 64-column panels into the panel buffer, unpacked into W1's rows.
-int fwdbwd_wide_obs(const OrlRnnArgs& a, cudaStream_t st) {
-    int e = orl::check_cuda(cudaMemsetAsync(a.loss_acc, 0, 8 * sizeof(float), st), "memset loss_acc");
-    if (e) return e;
-    const long long rows = a.n_chunks * a.chunk_length;
-    const long long tw = std::max(rw::tape_width_x(a.n_actions, a.obs_dim), rw::tape_width_x(1, a.critic_obs_dim));
-    float* partials = a.tape + rows * tw;
-    float* panels = partials + (rows + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK * a.grads_stride;
-    for (int net = 0; net < 2; ++net) {
-        const int d = net == 0 ? a.obs_dim : a.critic_obs_dim, n = net == 0 ? a.n_actions : 1;
-        if ((e = net == 0 ? launch_chunks_wide_obs<true>(a, st) : launch_chunks_wide_obs<false>(a, st))) return e;
-        const rc::Offsets o = rc::rnn_offsets(d, n);
-        float* grads = a.grads + (size_t)net * a.grads_stride;
-        const int tw_net = rw::tape_width_x(n, d);
-        if ((e = orl::reduce_tape(a.tape, tw_net, rows, make_jobs(d, n), partials, a.grads_stride, o.total, grads, st))) return e;
-        if (d > rc::MAXD) {   // W1's entries of the first reduction are overwritten here
-            const int last = (d - 1) / 64, used = W1P_PANEL * last + rc::H * (d - 64 * last);
-            if ((e = orl::reduce_tape(a.tape, tw_net, rows, w1_panel_jobs(d, n), partials, W1P_FLOATS, used, panels, st))) return e;
-            w1_scatter_kernel<<<(rc::H * d + 255) / 256, 256, 0, st>>>(panels, d, grads + o.w1);
-        }
+// the chunk kernel of one net of d features: two chunks per warp (every weight read feeds both) where they fit
+template <bool POLICY, bool AGENT0, int NB, int DX>
+int launch_chunks(const OrlRnnArgs& a, int d, cudaStream_t st) {
+    if constexpr (may_need_one_row<NB, DX>) {
+        if (wide_rows_per_warp<NB>(d) == 1)
+            return launch(rnn_chunk_warp_kernel<POLICY, AGENT0, 1, NB, DX>, a.n_chunks, w_smem<NB, DX>(d, 1), a, st);
     }
-    return orl::check_cuda(cudaGetLastError(), "rnn update launches");
+    return launch(rnn_chunk_warp_kernel<POLICY, AGENT0, 2, NB, DX>, (a.n_chunks + 1) / 2, w_smem<NB, DX>(d, 2), a, st);
+}
+
+// the forward / backward pass of one net over its chunks, writing its tape; JRPO (joint): the joint policy kernel, and the
+// critic on agent 0's rows
+int launch_net(const OrlRnnArgs& a, int net, bool joint, cudaStream_t st) {
+    const int d = net == 0 ? a.obs_dim : a.critic_obs_dim;
+    const bool wide_obs = d > rc::MAXD, wide_head = a.n_actions > MAX_OUT;
+    constexpr int XW = rw::MAXD_WIDE;
+    if (net == 1) {
+        if (joint) return launch_chunks<false, true, MAX_OUT, rc::H>(a, d, st);
+        return wide_obs ? launch_chunks<false, false, MAX_OUT, XW>(a, d, st) : launch_chunks<false, false, MAX_OUT, rc::H>(a, d, st);
+    }
+    if (joint) return launch(rnn_joint_policy_warp_kernel<JOINT_A>, a.n_chunks, w_smem<MAX_OUT, rc::H>(d, JOINT_A), a, st);
+    if (wide_obs)
+        return wide_head ? launch_chunks<true, false, MAX_OUT_WIDE, XW>(a, d, st) : launch_chunks<true, false, MAX_OUT, XW>(a, d, st);
+    return wide_head ? launch_chunks<true, false, MAX_OUT_WIDE, rc::H>(a, d, st) : launch_chunks<true, false, MAX_OUT, rc::H>(a, d, st);
 }
 
 }  // namespace
@@ -615,9 +587,9 @@ int orl_rnn_tape_width(void) { return rw::TAPE_W; }
 long long orl_rnn_workspace_floats_wide_obs(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim) {
     return ws_floats(rows, grads_stride, n_actions, obs_dim, critic_obs_dim);
 }
-long long orl_rnn_workspace_floats(long long rows, int grads_stride) { return orl_rnn_workspace_floats_for(rows, grads_stride, 1); }
+long long orl_rnn_workspace_floats(long long rows, int grads_stride) { return ws_floats(rows, grads_stride, 1, rc::MAXD, rc::MAXD); }
 long long orl_rnn_workspace_floats_for(long long rows, int grads_stride, int n_actions) {
-    return ws_tape_floats(rows, n_actions) + (rows + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK * grads_stride;
+    return ws_floats(rows, grads_stride, n_actions, rc::MAXD, rc::MAXD);
 }
 
 int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
@@ -639,24 +611,15 @@ int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
         ORL_CHECK_ARG(a.n_agents == 1 && a.obs_dim == 4, "single-agent env shapes");
         ORL_CHECK_ARG(single_obs_aligned(a), "policy_obs and critic_obs must be 16-byte aligned");
     }
-    cudaStream_t st = (cudaStream_t)stream;
     if (a.t_end > a.t_begin) {
-        const int wg = warp_grid(a.n_envs);
-        int e = 0;
-        switch (a.env_kind) {
-            case ORL_ENV_MPE_SPREAD:
-                if ((e = orl::allow_dynamic_smem(rnn_rollout_warp_kernel<ORL_ENV_MPE_SPREAD>, w_smem(3)))) return e;
-                rnn_rollout_warp_kernel<ORL_ENV_MPE_SPREAD><<<wg, W_NT, w_smem(3), st>>>(a); break;
-            case ORL_ENV_CARTPOLE:
-                if ((e = orl::allow_dynamic_smem(rnn_rollout_warp_kernel<ORL_ENV_CARTPOLE>, w_smem(1)))) return e;
-                rnn_rollout_warp_kernel<ORL_ENV_CARTPOLE><<<wg, W_NT, w_smem(1), st>>>(a); break;
-            default:
-                if ((e = orl::allow_dynamic_smem(rnn_rollout_warp_kernel<ORL_ENV_GRIDWORLD>, w_smem(1)))) return e;
-                rnn_rollout_warp_kernel<ORL_ENV_GRIDWORLD><<<wg, W_NT, w_smem(1), st>>>(a); break;
-        }
+        const bool mpe = a.env_kind == ORL_ENV_MPE_SPREAD;
+        void (*const kern)(OrlRnnArgs) = mpe ? rnn_rollout_warp_kernel<ORL_ENV_MPE_SPREAD>
+                                         : a.env_kind == ORL_ENV_CARTPOLE ? rnn_rollout_warp_kernel<ORL_ENV_CARTPOLE>
+                                                                          : rnn_rollout_warp_kernel<ORL_ENV_GRIDWORLD>;
+        if (int e = launch(kern, a.n_envs, w_smem<MAX_OUT, rc::H>(a.obs_dim, mpe ? 3 : 1), a, (cudaStream_t)stream)) return e;
     }
     if (int e = orl::check_cuda(cudaGetLastError(), "rnn_rollout_warp_kernel launch")) return e;
-    return orl::bump_rng_counter(a.rng_counter, a.t_end - a.t_begin, st);
+    return orl::bump_rng_counter(a.rng_counter, a.t_end - a.t_begin, (cudaStream_t)stream);
 }
 
 int orl_rnn_act_rows(const OrlRnnArgs* ap, void* stream) {
@@ -669,40 +632,11 @@ int orl_rnn_act_rows(const OrlRnnArgs* ap, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     const int rows = a.row_end - a.row_begin;
     if (rows > 0) {
-        // one row per warp while the rows leave warps of the persistent grid idle, two (every weight read feeds both) beyond
-        int e = 0;
-        const int d = a.obs_dim, R = rows <= orl::sm_count() * W_WPC ? 1 : 2;
-        if (d > rc::MAXD && a.n_actions > MAX_OUT) {   // wide observation: R = 2 only where it fits
-            if (R == 1 || wide_rows_per_warp<MAX_OUT_WIDE>(d) == 1) {
-                if ((e = orl::allow_dynamic_smem(rnn_act_rows_wide_obs_kernel<1, MAX_OUT_WIDE>, w_smem_wide<MAX_OUT_WIDE>(d, 1)))) return e;
-                rnn_act_rows_wide_obs_kernel<1, MAX_OUT_WIDE><<<warp_grid(rows), W_NT, w_smem_wide<MAX_OUT_WIDE>(d, 1), st>>>(a);
-            } else {
-                if ((e = orl::allow_dynamic_smem(rnn_act_rows_wide_obs_kernel<2, MAX_OUT_WIDE>, w_smem_wide<MAX_OUT_WIDE>(d, 2)))) return e;
-                rnn_act_rows_wide_obs_kernel<2, MAX_OUT_WIDE><<<warp_grid((rows + 1) / 2), W_NT, w_smem_wide<MAX_OUT_WIDE>(d, 2), st>>>(a);
-            }
-        } else if (d > rc::MAXD) {
-            if (R == 1) {
-                if ((e = orl::allow_dynamic_smem(rnn_act_rows_wide_obs_kernel<1, MAX_OUT>, w_smem_wide(d, 1)))) return e;
-                rnn_act_rows_wide_obs_kernel<1, MAX_OUT><<<warp_grid(rows), W_NT, w_smem_wide(d, 1), st>>>(a);
-            } else {
-                if ((e = orl::allow_dynamic_smem(rnn_act_rows_wide_obs_kernel<2, MAX_OUT>, w_smem_wide(d, 2)))) return e;
-                rnn_act_rows_wide_obs_kernel<2, MAX_OUT><<<warp_grid((rows + 1) / 2), W_NT, w_smem_wide(d, 2), st>>>(a);
-            }
-        } else if (a.n_actions > MAX_OUT) {   // the wide head: same row grouping
-            if (rows <= orl::sm_count() * W_WPC) {
-                if ((e = orl::allow_dynamic_smem(rnn_act_rows_warp_kernel<1, MAX_OUT_WIDE>, w_smem<MAX_OUT_WIDE>(1)))) return e;
-                rnn_act_rows_warp_kernel<1, MAX_OUT_WIDE><<<warp_grid(rows), W_NT, w_smem<MAX_OUT_WIDE>(1), st>>>(a);
-            } else {
-                if ((e = orl::allow_dynamic_smem(rnn_act_rows_warp_kernel<2, MAX_OUT_WIDE>, w_smem<MAX_OUT_WIDE>(2)))) return e;
-                rnn_act_rows_warp_kernel<2, MAX_OUT_WIDE><<<warp_grid((rows + 1) / 2), W_NT, w_smem<MAX_OUT_WIDE>(2), st>>>(a);
-            }
-        } else if (rows <= orl::sm_count() * W_WPC) {
-            if ((e = orl::allow_dynamic_smem(rnn_act_rows_warp_kernel<1>, w_smem(1)))) return e;
-            rnn_act_rows_warp_kernel<1><<<warp_grid(rows), W_NT, w_smem(1), st>>>(a);
-        } else {
-            if ((e = orl::allow_dynamic_smem(rnn_act_rows_warp_kernel<2>, w_smem(2)))) return e;
-            rnn_act_rows_warp_kernel<2><<<warp_grid((rows + 1) / 2), W_NT, w_smem(2), st>>>(a);
-        }
+        constexpr int XW = rw::MAXD_WIDE;
+        const bool wide_obs = a.obs_dim > rc::MAXD, wide_head = a.n_actions > MAX_OUT;
+        int e = wide_obs ? (wide_head ? launch_act_rows<MAX_OUT_WIDE, XW>(a, rows, st) : launch_act_rows<MAX_OUT, XW>(a, rows, st))
+                         : (wide_head ? launch_act_rows<MAX_OUT_WIDE, rc::H>(a, rows, st) : launch_act_rows<MAX_OUT, rc::H>(a, rows, st));
+        if (e) return e;
         if ((e = orl::check_cuda(cudaGetLastError(), "rnn_act_rows_warp_kernel launch"))) return e;
     }
     return orl::bump_rng_counter(a.rng_counter, 1, st);
@@ -713,16 +647,10 @@ int orl_rnn_critic(const OrlRnnArgs* ap, void* stream) {
     const OrlRnnArgs& a = *ap;
     if (int e = check_common(a, rw::MAXD_WIDE)) return e;
     ORL_CHECK_ARG(a.critic_params && a.critic_obs && a.rnn_states_critic && a.masks && a.value_preds, "null critic buffer");
-    const int B = a.n_envs * a.n_agents;
-    if (a.critic_obs_dim > rc::MAXD) {
-        const size_t sm = w_smem_wide(a.critic_obs_dim, 1);
-        if (int e = orl::allow_dynamic_smem(rnn_critic_wide_obs_kernel, sm)) return e;
-        rnn_critic_wide_obs_kernel<<<warp_grid(B), W_NT, sm, (cudaStream_t)stream>>>(a);
-        return orl::check_cuda(cudaGetLastError(), "rnn_critic_wide_obs_kernel launch");
-    }
-    if (int e = orl::allow_dynamic_smem(rnn_critic_warp_kernel, w_smem(1))) return e;
-    rnn_critic_warp_kernel<<<warp_grid(B), W_NT, w_smem(1), (cudaStream_t)stream>>>(a);
-    return orl::check_cuda(cudaGetLastError(), "rnn_critic_warp_kernel launch");
+    const int B = a.n_envs * a.n_agents, dc = a.critic_obs_dim;
+    const int e = dc > rc::MAXD ? launch(rnn_critic_warp_kernel<rw::MAXD_WIDE>, B, w_smem<MAX_OUT, rw::MAXD_WIDE>(dc, 1), a, (cudaStream_t)stream)
+                                : launch(rnn_critic_warp_kernel<rc::H>, B, w_smem<MAX_OUT, rc::H>(dc, 1), a, (cudaStream_t)stream);
+    return e ? e : orl::check_cuda(cudaGetLastError(), "rnn_critic_warp_kernel launch");
 }
 
 int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
@@ -747,37 +675,25 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
         ORL_CHECK_ARG(a.n_actions <= MAX_OUT, "ORL_PPO_JOINT_ACTION is built for up to 8 actions");
         ORL_CHECK_ARG(a.obs_dim <= rc::MAXD && a.critic_obs_dim <= rc::MAXD, "ORL_PPO_JOINT_ACTION is built for obs dims 1..64");
     }
-    if (a.obs_dim > rc::MAXD || a.critic_obs_dim > rc::MAXD) return fwdbwd_wide_obs(a, (cudaStream_t)stream);
-    const bool wide = a.n_actions > MAX_OUT;
     cudaStream_t st = (cudaStream_t)stream;
     int e = orl::check_cuda(cudaMemsetAsync(a.loss_acc, 0, 8 * sizeof(float), st), "memset loss_acc");
     if (e) return e;
     const long long steps = a.n_chunks * a.chunk_length;
     const long long net_rows[2] = {joint ? steps * JOINT_A : steps, steps};
-    float* partials = a.tape + ws_tape_floats(net_rows[0], a.n_actions);   // the policy's tape is the larger one
-    // two chunks per warp: every weight read from shared memory feeds two rows
-    constexpr int C_R = 2;
-    const int cgrid = warp_grid((a.n_chunks + C_R - 1) / C_R);
-    if (joint) {
-        if ((e = orl::allow_dynamic_smem(rnn_joint_policy_warp_kernel<JOINT_A, W_NT>, w_smem(JOINT_A)))) return e;
-        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<false, true, C_R, W_NT>, w_smem(C_R)))) return e;
-    } else if (wide) {
-        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<true, false, C_R, W_NT, MAX_OUT_WIDE>, w_smem<MAX_OUT_WIDE>(C_R)))) return e;
-        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<false, false, C_R, W_NT>, w_smem(C_R)))) return e;
-    } else {
-        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<true, false, C_R, W_NT>, w_smem(C_R)))) return e;
-        if ((e = orl::allow_dynamic_smem(rnn_chunk_warp_kernel<false, false, C_R, W_NT>, w_smem(C_R)))) return e;
-    }
+    const int tw[2] = {rw::tape_width_x(a.n_actions, a.obs_dim), rw::tape_width_x(1, a.critic_obs_dim)};
+    float* partials = a.tape + std::max(net_rows[0] * tw[0], net_rows[1] * tw[1]);   // after the larger of the two tapes
+    float* panels = partials + (std::max(net_rows[0], net_rows[1]) + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK * a.grads_stride;
     for (int net = 0; net < 2; ++net) {
         const int d = net == 0 ? a.obs_dim : a.critic_obs_dim, n = net == 0 ? a.n_actions : 1;
-        if (net == 0 && joint) rnn_joint_policy_warp_kernel<JOINT_A, W_NT><<<warp_grid(a.n_chunks), W_NT, w_smem(JOINT_A), st>>>(a);
-        else if (net == 0 && wide)
-            rnn_chunk_warp_kernel<true, false, C_R, W_NT, MAX_OUT_WIDE><<<cgrid, W_NT, w_smem<MAX_OUT_WIDE>(C_R), st>>>(a);
-        else if (net == 0) rnn_chunk_warp_kernel<true, false, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
-        else if (joint) rnn_chunk_warp_kernel<false, true, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
-        else rnn_chunk_warp_kernel<false, false, C_R, W_NT><<<cgrid, W_NT, w_smem(C_R), st>>>(a);
-        if ((e = orl::reduce_tape(a.tape, rw::tape_width(n), net_rows[net], make_jobs(d, n), partials, a.grads_stride,
-                                  rc::rnn_offsets(d, n).total, a.grads + (size_t)net * a.grads_stride, st))) return e;
+        if ((e = launch_net(a, net, joint, st))) return e;
+        const rc::Offsets o = rc::rnn_offsets(d, n);
+        float* grads = a.grads + (size_t)net * a.grads_stride;
+        if ((e = orl::reduce_tape(a.tape, tw[net], net_rows[net], make_jobs(d, n), partials, a.grads_stride, o.total, grads, st))) return e;
+        if (d > rc::MAXD) {   // W1's entries of the first reduction are overwritten here
+            const int last = (d - 1) / 64, used = W1P_PANEL * last + rc::H * (d - 64 * last);
+            if ((e = orl::reduce_tape(a.tape, tw[net], net_rows[net], w1_panel_jobs(d, n), partials, W1P_FLOATS, used, panels, st))) return e;
+            w1_scatter_kernel<<<(rc::H * d + 255) / 256, 256, 0, st>>>(panels, d, grads + o.w1);
+        }
     }
     return orl::check_cuda(cudaGetLastError(), "rnn update launches");
 }

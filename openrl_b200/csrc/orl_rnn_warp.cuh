@@ -23,7 +23,7 @@
 //
 // Observation width bound DX (a template parameter of step_forward): DX = 64 (H) takes x as a V2 and stages W1 at LD.
 // DX = 256 (MAXD_WIDE, observations of 65..256 features): a row's x is loaded from global memory straight into its
-// scratch row (SCR = 256 floats), W1 is staged at the odd leading dimension w1_ld(d) = pad4(d) + 1 (load_net_wide) and
+// scratch row (SCR = 256 floats), W1 is staged at the odd leading dimension w1_ld(d) = pad4(d) + 1 (load_net<NB, 256>) and
 // fc1 is matvec64 with K = pad4(d).  With a tape, x also goes to an X field of MAXD_WIDE floats appended to the row
 // (tape_width_x), the Q operand of the 64-column panels of dW1; TQ_X is left unused there.  Only fc1 depends on d.
 #pragma once
@@ -51,69 +51,40 @@ struct SmemNet {
     const float *w1, *w3, *wih, *whh, *wh;                                  // [rows][LD]
     const float *b1, *g1, *be1, *b3, *g3, *be3, *bih, *bhh, *gr, *ber, *bh;  // vectors
 };
-template <int NB = MAXN>
-__host__ __device__ constexpr int smem_net_floats() { return (H + H + G3 + G3 + NB) * LD + 8 * H + 2 * G3 + NB; }
-
-// the same net with W1 at leading dimension w1_ld(d) (load_net_wide)
-template <int NB = MAXN>
-__host__ __device__ constexpr int smem_net_floats_wide(int d) { return smem_net_floats<NB>() + H * (w1_ld(d) - LD); }
-
-// Stage one net (flat layout of rc::rnn_offsets) into shared memory; W1 columns k >= d and head rows m >= n are zero.
-template <int NB = MAXN>
-__device__ inline SmemNet load_net(float* s, const float* __restrict__ P, const rc::Offsets& o, int tid, int nthreads) {
-    static_assert(NB == MAXN || NB == MAXN_WIDE, "head width bound");
-    float* w1 = s; s += H * LD;
-    float* w3 = s; s += H * LD;
-    float* wih = s; s += G3 * LD;
-    float* whh = s; s += G3 * LD;
-    float* wh = s; s += NB * LD;
-    float* vec = s;   // b1 g1 be1 b3 g3 be3 gr ber (64 each) | bih bhh (192 each) | bh (NB)
-    for (int i = tid; i < H * LD; i += nthreads) {
-        const int j = i / LD, k = i % LD;
-        w1[i] = k < o.d ? P[o.w1 + j * o.d + k] : 0.f;
-        w3[i] = k < H ? P[o.w3 + j * H + k] : 0.f;
-    }
-    for (int i = tid; i < G3 * LD; i += nthreads) {
-        const int j = i / LD, k = i % LD;
-        wih[i] = k < H ? P[o.wih + j * H + k] : 0.f;
-        whh[i] = k < H ? P[o.whh + j * H + k] : 0.f;
-    }
-    for (int i = tid; i < NB * LD; i += nthreads) {
-        const int j = i / LD, k = i % LD;
-        wh[i] = (j < o.n && k < H) ? P[o.wh + j * H + k] : 0.f;
-    }
-    for (int i = tid; i < H; i += nthreads) {
-        vec[i] = P[o.b1 + i]; vec[H + i] = P[o.g1 + i]; vec[2 * H + i] = P[o.be1 + i];
-        vec[3 * H + i] = P[o.b3 + i]; vec[4 * H + i] = P[o.g3 + i]; vec[5 * H + i] = P[o.be3 + i];
-        vec[6 * H + i] = P[o.gr + i]; vec[7 * H + i] = P[o.ber + i];
-    }
-    for (int i = tid; i < G3; i += nthreads) { vec[8 * H + i] = P[o.bih + i]; vec[8 * H + G3 + i] = P[o.bhh + i]; }
-    for (int i = tid; i < NB; i += nthreads) vec[8 * H + 2 * G3 + i] = i < o.n ? P[o.bh + i] : 0.f;
-    SmemNet n;
-    n.w1 = w1; n.w3 = w3; n.wih = wih; n.whh = whh; n.wh = wh;
-    n.b1 = vec; n.g1 = vec + H; n.be1 = vec + 2 * H; n.b3 = vec + 3 * H; n.g3 = vec + 4 * H; n.be3 = vec + 5 * H;
-    n.gr = vec + 6 * H; n.ber = vec + 7 * H; n.bih = vec + 8 * H; n.bhh = vec + 8 * H + G3; n.bh = vec + 8 * H + 2 * G3;
-    return n;
+// shared-memory floats of one net staged by load_net<NB, DX>: W1 at LD (DX = 64) or at w1_ld(d) (DX = 256), then the rest
+template <int NB = MAXN, int DX = H>
+__host__ __device__ constexpr int smem_net_floats(int d) {
+    return (H + H + G3 + G3 + NB) * LD + 8 * H + 2 * G3 + NB + (DX == H ? 0 : H * (w1_ld(d) - LD));
 }
 
-// load_net for d > 64: W1 [64][w1_ld(d)] first (columns k >= d zero), then the rest in load_net's layout
-template <int NB = MAXN>
-__device__ inline SmemNet load_net_wide(float* s, const float* __restrict__ P, const rc::Offsets& o, int tid, int nthreads) {
+// Stage one net (flat layout of rc::rnn_offsets) into shared memory; W1 columns k >= d and head rows m >= n are zero.
+// DX = 64: W1 at LD, staged in one loop with W3.  DX = 256: W1 [64][w1_ld(d)].
+template <int NB = MAXN, int DX = H>
+__device__ inline SmemNet load_net(float* s, const float* __restrict__ P, const rc::Offsets& o, int tid, int nthreads) {
     static_assert(NB == MAXN || NB == MAXN_WIDE, "head width bound");
-    const int ld1 = w1_ld(o.d);
+    static_assert(DX == H || DX == MAXD_WIDE, "observation width bound");
+    const int ld1 = DX == H ? LD : w1_ld(o.d);
     float* w1 = s; s += H * ld1;
     float* w3 = s; s += H * LD;
     float* wih = s; s += G3 * LD;
     float* whh = s; s += G3 * LD;
     float* wh = s; s += NB * LD;
-    float* vec = s;
-    for (int i = tid; i < H * ld1; i += nthreads) {
-        const int j = i / ld1, k = i % ld1;
-        w1[i] = k < o.d ? P[o.w1 + j * o.d + k] : 0.f;
-    }
-    for (int i = tid; i < H * LD; i += nthreads) {
-        const int j = i / LD, k = i % LD;
-        w3[i] = k < H ? P[o.w3 + j * H + k] : 0.f;
+    float* vec = s;   // b1 g1 be1 b3 g3 be3 gr ber (64 each) | bih bhh (192 each) | bh (NB)
+    if constexpr (DX == H) {
+        for (int i = tid; i < H * LD; i += nthreads) {
+            const int j = i / LD, k = i % LD;
+            w1[i] = k < o.d ? P[o.w1 + j * o.d + k] : 0.f;
+            w3[i] = k < H ? P[o.w3 + j * H + k] : 0.f;
+        }
+    } else {
+        for (int i = tid; i < H * ld1; i += nthreads) {
+            const int j = i / ld1, k = i % ld1;
+            w1[i] = k < o.d ? P[o.w1 + j * o.d + k] : 0.f;
+        }
+        for (int i = tid; i < H * LD; i += nthreads) {
+            const int j = i / LD, k = i % LD;
+            w3[i] = k < H ? P[o.w3 + j * H + k] : 0.f;
+        }
     }
     for (int i = tid; i < G3 * LD; i += nthreads) {
         const int j = i / LD, k = i % LD;
@@ -292,7 +263,7 @@ __device__ __forceinline__ void stage_x(float* scr, const float* const (&x)[R], 
 
 // One forward step of R rows.  x: observation (XIn; zero beyond d), h_in: hidden state, out[r]: the head outputs (HeadOut).
 // tape[r] != nullptr: the Q operands and the activations for the backward step go to the row's tape.
-// scr: this warp's scratch (R * SCR floats of shared memory).  DX = 256: W from load_net_wide.
+// scr: this warp's scratch (R * SCR floats of shared memory).  W: staged by load_net<NB, DX>.
 template <int R, int NB = MAXN, int DX = H>
 __device__ __forceinline__ void step_forward(const SmemNet& W, float* scr, int d, int n, int act_id, const typename XIn<DX>::type (&x)[R],
                                              const V2 (&h_in)[R], const float (&mask)[R], V2 (&h_out)[R],

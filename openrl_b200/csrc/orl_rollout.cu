@@ -48,16 +48,12 @@ __global__ void env_step_kernel(int kind, int N, EnvPtrs E, const float* __restr
     dones_out[e] = done ? 1.f : 0.f;
 }
 
-
-// ENV of the host act (ORL_ENV_NONE) for observations of 65..256 features: fc1 in panels (orl_mlp.cuh, fc1_panels) in
-// the buffers of the d = 64 layout
-constexpr int ENV_NONE_WIDE_OBS = -1;
-
 // NB: head width bound (orl_mlp.cuh); NB = 64 is the wide Categorical head of host-stepped envs (ORL_ENV_NONE), whose
-// logits tile reuses N1s once the trunk is done with it.
-template <int R_M, int ENV, int NB = MAX_OUT>
+// logits tile reuses N1s once the trunk is done with it.  PANELS: the host act (ORL_ENV_NONE) of observations of 65..256
+// features, fc1 in panels (orl_mlp.cuh, fc1_panels) in the buffers of the d = 64 layout.
+template <int R_M, int ENV, int NB = MAX_OUT, bool PANELS = false>
 __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
-    constexpr bool PANELS = ENV == ENV_NONE_WIDE_OBS;
+    static_assert(ENV == ORL_ENV_NONE || !PANELS, "panelled observations come from host-stepped envs");
     extern __shared__ __align__(16) float smem[];
     const int N = a.n_envs, A = a.n_agents, B = N * A, d = a.obs_dim, n = a.n_actions;
     const int ldx = PANELS ? LDX_PANEL : pad4(d) + 4;
@@ -105,7 +101,7 @@ __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
         }
         __syncthreads();
         if constexpr (NB == MAX_OUT_WIDE) {
-            static_assert(ENV == ORL_ENV_NONE || PANELS, "wide heads act on host-stepped envs");
+            static_assert(ENV == ORL_ENV_NONE, "wide heads act on host-stepped envs");
             head_tile<R_M, R_NT>(w, N3s, N1s);
             __syncthreads();
             if (tid < rows_here) {   // one thread per row
@@ -246,28 +242,19 @@ __device__ __forceinline__ void rows_forward(const float* __restrict__ params, i
 
 // ValueNetwork.forward (value_network.py:113-136)
 template <bool PANELS>
-__device__ __forceinline__ void critic_values_body(const float* __restrict__ params, int d, int activation_id,
-                                                   const float* __restrict__ obs, float* __restrict__ values, long long rows) {
-    rows_forward<MAX_OUT, PANELS>(params, d, 1, activation_id, obs, rows, [&](long long g, float (&out)[MAX_OUT]) { values[g] = out[0]; });
-}
 __global__ void __launch_bounds__(C_NT) critic_values_kernel(const float* __restrict__ params, int d, int activation_id,
                                                              const float* __restrict__ obs, float* __restrict__ values,
                                                              long long rows) {
-    critic_values_body<false>(params, d, activation_id, obs, values, rows);
-}
-__global__ void __launch_bounds__(C_NT) critic_values_wide_obs_kernel(const float* __restrict__ params, int d, int activation_id,
-                                                                      const float* __restrict__ obs, float* __restrict__ values,
-                                                                      long long rows) {
-    critic_values_body<true>(params, d, activation_id, obs, values, rows);
+    rows_forward<MAX_OUT, PANELS>(params, d, 1, activation_id, obs, rows, [&](long long g, float (&out)[MAX_OUT]) { values[g] = out[0]; });
 }
 
 // PolicyNetwork.eval_actions (policy_network.py:164-203, act.py:160-168 / 150-158): the log-prob of the given action and
 // the entropy of the action distribution per row (the caller takes the masked mean); per dimension for a Gaussian head.
 template <bool PANELS>
-__device__ __forceinline__ void policy_eval_body(const float* __restrict__ params, int d, int n, int activation_id, int head_kind,
-                                                 const float* __restrict__ obs, const float* __restrict__ actions,
-                                                 const float* __restrict__ action_masks, float* __restrict__ logp_out,
-                                                 float* __restrict__ entropy_out, long long rows) {
+__global__ void __launch_bounds__(C_NT) policy_eval_kernel(const float* __restrict__ params, int d, int n, int activation_id, int head_kind,
+                                                           const float* __restrict__ obs, const float* __restrict__ actions,
+                                                           const float* __restrict__ action_masks, float* __restrict__ logp_out,
+                                                           float* __restrict__ entropy_out, long long rows) {
     const float* logstd = params + net_offsets(d, n, 1).ls;
     rows_forward<MAX_OUT, PANELS>(params, d, n, activation_id, obs, rows, [&](long long g, float (&out)[MAX_OUT]) {
         if (head_kind == ORL_HEAD_GAUSSIAN) {
@@ -284,42 +271,18 @@ __device__ __forceinline__ void policy_eval_body(const float* __restrict__ param
         }
     });
 }
-__global__ void __launch_bounds__(C_NT) policy_eval_kernel(const float* __restrict__ params, int d, int n, int activation_id, int head_kind,
-                                                           const float* __restrict__ obs, const float* __restrict__ actions,
-                                                           const float* __restrict__ action_masks, float* __restrict__ logp_out,
-                                                           float* __restrict__ entropy_out, long long rows) {
-    policy_eval_body<false>(params, d, n, activation_id, head_kind, obs, actions, action_masks, logp_out, entropy_out, rows);
-}
-__global__ void __launch_bounds__(C_NT) policy_eval_wide_obs_kernel(const float* __restrict__ params, int d, int n, int activation_id,
-                                                                    int head_kind, const float* __restrict__ obs,
-                                                                    const float* __restrict__ actions, const float* __restrict__ action_masks,
-                                                                    float* __restrict__ logp_out, float* __restrict__ entropy_out, long long rows) {
-    policy_eval_body<true>(params, d, n, activation_id, head_kind, obs, actions, action_masks, logp_out, entropy_out, rows);
-}
 
 // policy_eval_kernel of a wide Categorical head (9..64 actions)
 template <bool PANELS>
-__device__ __forceinline__ void policy_eval_wide_body(const float* __restrict__ params, int d, int n, int activation_id,
-                                                      const float* __restrict__ obs, const float* __restrict__ actions,
-                                                      const float* __restrict__ action_masks, float* __restrict__ logp_out,
-                                                      float* __restrict__ entropy_out, long long rows) {
+__global__ void __launch_bounds__(C_NT) policy_eval_wide_kernel(const float* __restrict__ params, int d, int n, int activation_id,
+                                                                const float* __restrict__ obs, const float* __restrict__ actions,
+                                                                const float* __restrict__ action_masks, float* __restrict__ logp_out,
+                                                                float* __restrict__ entropy_out, long long rows) {
     rows_forward<MAX_OUT_WIDE, PANELS>(params, d, n, activation_id, obs, rows, [&](long long g, float* x) {
         const WideSoftmax sm = wide_log_softmax(x, n, action_masks ? action_masks + g * n : nullptr);
         logp_out[g] = wide_log_prob_of(sm, x, n, (int)actions[g]);
         entropy_out[g] = wide_entropy(sm, x, n);
     });
-}
-__global__ void __launch_bounds__(C_NT) policy_eval_wide_kernel(const float* __restrict__ params, int d, int n, int activation_id,
-                                                                const float* __restrict__ obs, const float* __restrict__ actions,
-                                                                const float* __restrict__ action_masks, float* __restrict__ logp_out,
-                                                                float* __restrict__ entropy_out, long long rows) {
-    policy_eval_wide_body<false>(params, d, n, activation_id, obs, actions, action_masks, logp_out, entropy_out, rows);
-}
-__global__ void __launch_bounds__(C_NT) policy_eval_wide_wide_obs_kernel(const float* __restrict__ params, int d, int n, int activation_id,
-                                                                         const float* __restrict__ obs, const float* __restrict__ actions,
-                                                                         const float* __restrict__ action_masks, float* __restrict__ logp_out,
-                                                                         float* __restrict__ entropy_out, long long rows) {
-    policy_eval_wide_body<true>(params, d, n, activation_id, obs, actions, action_masks, logp_out, entropy_out, rows);
 }
 
 // ---- insert of one host env.step into the rollout buffer (OnPolicyDriver.add2buffer, onpolicy_driver.py:80-152) -----------
@@ -380,6 +343,12 @@ __global__ void host_insert_rnn_kernel(const float* __restrict__ staged, int n_e
 #pragma unroll
         for (int k = 0; k < RNN_HIDDEN / 4; ++k) h[k] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
+}
+
+// the rollout_kernel instance of rm (8, 16 or 32) rows per CTA
+template <int ENV, int NB = MAX_OUT, bool PANELS = false>
+auto rollout_rows(int rm) {
+    return rm == 8 ? rollout_kernel<8, ENV, NB, PANELS> : rm == 16 ? rollout_kernel<16, ENV, NB, PANELS> : rollout_kernel<32, ENV, NB, PANELS>;
 }
 
 // launch of a row-batch forward kernel over `rows` rows of obs_dim d: grid = min(tiles, 2 x SMs).  A panelled kernel
@@ -503,17 +472,11 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
     const bool mpe = a.env_kind == ORL_ENV_MPE_SPREAD, wide = a.n_actions > orl::MAX_OUT, wide_obs = a.obs_dim > orl::OBS_PANEL;
     const size_t smem = sizeof(float) * ((wide ? orl::smem_weights_floats<orl::MAX_OUT_WIDE>(ds, false)
                                                : orl::smem_weights_floats(ds, false)) + rm * ldx + 2 * rm * orl::LDA + rm);
+    // simple_spread has neither wide observations nor a wide head
     void (*const kern)(OrlRolloutArgs) =
-        wide_obs ? (wide ? (rm == 8 ? rollout_kernel<8, ENV_NONE_WIDE_OBS, orl::MAX_OUT_WIDE>
-                            : rm == 16 ? rollout_kernel<16, ENV_NONE_WIDE_OBS, orl::MAX_OUT_WIDE>
-                                       : rollout_kernel<32, ENV_NONE_WIDE_OBS, orl::MAX_OUT_WIDE>)
-                         : (rm == 8 ? rollout_kernel<8, ENV_NONE_WIDE_OBS>
-                            : rm == 16 ? rollout_kernel<16, ENV_NONE_WIDE_OBS> : rollout_kernel<32, ENV_NONE_WIDE_OBS>))
-        : wide ? (rm == 8 ? rollout_kernel<8, ORL_ENV_NONE, orl::MAX_OUT_WIDE>
-                : rm == 16 ? rollout_kernel<16, ORL_ENV_NONE, orl::MAX_OUT_WIDE> : rollout_kernel<32, ORL_ENV_NONE, orl::MAX_OUT_WIDE>)
-        : rm == 8 ? (mpe ? rollout_kernel<8, ORL_ENV_MPE_SPREAD> : rollout_kernel<8, ORL_ENV_NONE>)
-        : rm == 16 ? (mpe ? rollout_kernel<16, ORL_ENV_MPE_SPREAD> : rollout_kernel<16, ORL_ENV_NONE>)
-                   : (mpe ? rollout_kernel<32, ORL_ENV_MPE_SPREAD> : rollout_kernel<32, ORL_ENV_NONE>);
+        mpe ? rollout_rows<ORL_ENV_MPE_SPREAD>(rm)
+        : wide ? (wide_obs ? rollout_rows<ORL_ENV_NONE, orl::MAX_OUT_WIDE, true>(rm) : rollout_rows<ORL_ENV_NONE, orl::MAX_OUT_WIDE>(rm))
+               : (wide_obs ? rollout_rows<ORL_ENV_NONE, orl::MAX_OUT, true>(rm) : rollout_rows<ORL_ENV_NONE>(rm));
     if (int e = orl::allow_dynamic_smem(kern, 200 * 1024)) return e;
     kern<<<grid, R_NT, smem, st>>>(a);
     ORL_LAUNCH_CHECK("rollout_kernel");
@@ -529,11 +492,8 @@ extern "C" int orl_critic_values(const float* critic_params, int obs_dim, int ac
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (obs_dim <= 8)   // tensor-core forward (orl_fwd_tc.cu)
         return orl::launch_critic_values_tc(critic_params, obs_dim, activation_id, obs, values, rows, st);
-    if (obs_dim > orl::OBS_PANEL)
-        return launch_rows_forward(critic_values_wide_obs_kernel, "critic_values_wide_obs_kernel", obs_dim, rows, st, critic_params,
-                                   obs_dim, activation_id, obs, values, rows);
-    return launch_rows_forward(critic_values_kernel, "critic_values_kernel", obs_dim, rows, st, critic_params, obs_dim,
-                               activation_id, obs, values, rows);
+    return launch_rows_forward(obs_dim > orl::OBS_PANEL ? critic_values_kernel<true> : critic_values_kernel<false>,
+                               "critic_values_kernel", obs_dim, rows, st, critic_params, obs_dim, activation_id, obs, values, rows);
 }
 
 extern "C" int orl_policy_eval(const float* policy_params, int obs_dim, int n_actions, int activation_id, int head_kind,
@@ -547,20 +507,13 @@ extern "C" int orl_policy_eval(const float* policy_params, int obs_dim, int n_ac
     ORL_CHECK_ARG(n_actions <= orl::MAX_OUT || head_kind == ORL_HEAD_CATEGORICAL,
                   "n_actions must be in 1..8 for Gaussian heads (1..64 for Categorical heads)");
     const bool wide_obs = obs_dim > orl::OBS_PANEL;
-    if (n_actions > orl::MAX_OUT && wide_obs)
-        return launch_rows_forward<orl::MAX_OUT_WIDE>(policy_eval_wide_wide_obs_kernel, "policy_eval_wide_wide_obs_kernel", obs_dim,
-                                                      rows, reinterpret_cast<cudaStream_t>(stream), policy_params, obs_dim, n_actions,
-                                                      activation_id, obs, actions, action_masks, log_probs, entropy, rows);
-    if (wide_obs)
-        return launch_rows_forward(policy_eval_wide_obs_kernel, "policy_eval_wide_obs_kernel", obs_dim, rows,
-                                   reinterpret_cast<cudaStream_t>(stream), policy_params, obs_dim, n_actions, activation_id, head_kind,
-                                   obs, actions, action_masks, log_probs, entropy, rows);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (n_actions > orl::MAX_OUT)
-        return launch_rows_forward<orl::MAX_OUT_WIDE>(policy_eval_wide_kernel, "policy_eval_wide_kernel", obs_dim, rows,
-                                                      reinterpret_cast<cudaStream_t>(stream), policy_params, obs_dim, n_actions,
+        return launch_rows_forward<orl::MAX_OUT_WIDE>(wide_obs ? policy_eval_wide_kernel<true> : policy_eval_wide_kernel<false>,
+                                                      "policy_eval_wide_kernel", obs_dim, rows, st, policy_params, obs_dim, n_actions,
                                                       activation_id, obs, actions, action_masks, log_probs, entropy, rows);
-    return launch_rows_forward(policy_eval_kernel, "policy_eval_kernel", obs_dim, rows, reinterpret_cast<cudaStream_t>(stream),
-                               policy_params, obs_dim, n_actions, activation_id, head_kind, obs, actions, action_masks,
+    return launch_rows_forward(wide_obs ? policy_eval_kernel<true> : policy_eval_kernel<false>, "policy_eval_kernel", obs_dim, rows,
+                               st, policy_params, obs_dim, n_actions, activation_id, head_kind, obs, actions, action_masks,
                                log_probs, entropy, rows);
 }
 

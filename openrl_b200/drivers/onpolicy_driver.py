@@ -287,11 +287,10 @@ class OnPolicyDriver:
         return a
 
     def _host_insert(self, staged, step, lo, hi, has_masks=False):
-        """One host env.step of envs [lo, hi) into slot step + 1 (rewards: slot step): orl_host_insert (orl_host_insert_wide_obs
-        for a critic section wider than 64), or orl_host_insert_rnn_wide (the GRU insert for masks of every head width,
-        1..64 actions; orl_host_insert_rnn_wide_obs for a critic section wider than 64), which also zeroes
-        rnn_states[step + 1] of the envs that finished.  With `has_masks` the
-        staged block carries the envs' action masks, written to action_masks[step + 1] (replay_data.py:282-283); the
+        """One host env.step of envs [lo, hi) into slot step + 1 (rewards: slot step): orl_host_insert_wide_obs, or for a GRU
+        policy orl_host_insert_rnn_wide_obs, which also zeroes rnn_states[step + 1] of the envs that finished (the inserts
+        that take every width the nets take: masks of 1..64 actions, critic sections of 1..256 features).  With `has_masks`
+        the staged block carries the envs' action masks, written to action_masks[step + 1] (replay_data.py:282-283); the
         buffer's masks stop being trivial for good.  A buffer with its own critic_obs (Dict observations) takes the
         block's critic section into critic_obs[step + 1]."""
         d, A = self.buffer.data, self.envs.agent_num
@@ -304,17 +303,12 @@ class OnPolicyDriver:
         if has_masks:
             d.action_masks_trivial = False
             am = d.action_masks[step + 1].view(-1, d.n_actions)[r0:r1]
+        tail = (lib.ptr(am), d.n_actions, lib.ptr(cri), d.critic_obs_dim, lib.current_stream())
         if self.recurrent:
             states = d.rnn_states[step + 1].view(d.n_rollout_threads * A, -1)[r0:r1]
-            name = "orl_host_insert_rnn_wide_obs" if cri is not None and d.critic_obs_dim > 64 else "orl_host_insert_rnn_wide"
-            lib.check(getattr(self._lib, name)(*args, lib.ptr(states), lib.ptr(am), d.n_actions, lib.ptr(cri), d.critic_obs_dim,
-                                               lib.current_stream()), name)
-        elif cri is not None and d.critic_obs_dim > 64:
-            lib.check(self._lib.orl_host_insert_wide_obs(*args, lib.ptr(am), d.n_actions, lib.ptr(cri), d.critic_obs_dim,
-                                                         lib.current_stream()), "orl_host_insert_wide_obs")
+            lib.check(self._lib.orl_host_insert_rnn_wide_obs(*args, lib.ptr(states), *tail), "orl_host_insert_rnn_wide_obs")
         else:
-            lib.check(self._lib.orl_host_insert(*args, lib.ptr(am), d.n_actions, lib.ptr(cri), d.critic_obs_dim,
-                                                lib.current_stream()), "orl_host_insert")
+            lib.check(self._lib.orl_host_insert_wide_obs(*args, *tail), "orl_host_insert_wide_obs")
         self.gpu_launches += 1
 
     def _launch_steps(self, t_begin, t_end, noise):

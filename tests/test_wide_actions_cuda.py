@@ -1,6 +1,6 @@
 """Discrete action spaces of 9..64 actions on the feed-forward policy: the wide Categorical head of the host act
 (rollout_kernel<*, ORL_ENV_NONE, 64>), of orl_policy_eval (policy_eval_wide_kernel) and of the FFMA PPO update
-(ppo_fwdbwd_kernel<64>).
+(ppo_fwdbwd_kernel<64, ...>).
 
 Bars: the reference's traces on the masked env widened to 9 and 64 actions (tests/golden/trace_wide_actions_*.npz)
 through PPOAgent over HostVecEnv in parity mode, at the bars of tests/test_host_action_masks_cuda.py; the FFMA update at

@@ -1,5 +1,5 @@
-"""Discrete action spaces of 9..64 actions on the GRU policy: the wide head of the host act (rnn_act_rows_warp_kernel<R, 64>)
-and of the chunked recurrent update (the policy instance rnn_chunk_warp_kernel<true, false, 2, 512, 64>, its tape rows of
+"""Discrete action spaces of 9..64 actions on the GRU policy: the wide head of the host act (rnn_act_rows_warp_kernel<R, 64, DX>)
+and of the chunked recurrent update (the policy instance rnn_chunk_warp_kernel<true, false, R, 64, DX>, its tape rows of
 TAPE_WIDE floats and their reduction).
 
 Bars: the reference's traces on the masked env widened to 9 and 64 actions with a GRU policy

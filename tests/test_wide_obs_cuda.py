@@ -1,7 +1,7 @@
 """Observations of 65..256 features on the feed-forward policy and critic (cfg.use_wide_observations): fc1 as a loop over
-64-wide panels of the observation (orl_mlp.cuh, fc1_panels) in the host act (rollout_kernel<*, ENV_NONE_WIDE_OBS, *>),
-orl_critic_values (critic_values_wide_obs_kernel), orl_policy_eval (policy_eval_wide_obs_kernel,
-policy_eval_wide_wide_obs_kernel) and the FFMA PPO update (ppo_fwdbwd_wide_obs_kernel), and the insert of a critic
+64-wide panels of the observation (orl_mlp.cuh, fc1_panels) in the host act (rollout_kernel<*, ORL_ENV_NONE, *, true>),
+orl_critic_values (critic_values_kernel<true>), orl_policy_eval (policy_eval_kernel<true>, policy_eval_wide_kernel<true>)
+and the FFMA PPO update (the panelled ppo_fwdbwd_kernel<NB, PANELS_POLICY, PANELS_CRITIC> instances), and the insert of a critic
 section wider than 64 (orl_host_insert_wide_obs).
 
 Bars: the reference's traces on the envs of tests/wide_obs_oracle.py through PPOAgent in parity mode; the FFMA update on a shuffled minibatch of a C5-sized buffer (1024 envs x 128 steps) with a partial last tile,

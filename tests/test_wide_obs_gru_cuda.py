@@ -1,6 +1,6 @@
 """Observations of 65..256 features on GRU policies and critics (cfg.use_wide_recurrent_observations): the host act
-(rnn_act_rows_wide_obs_kernel<R, NB>), the recurrent critic (rnn_critic_wide_obs_kernel), the chunked update
-(rnn_chunk_wide_obs_kernel<POLICY, R, NB>, its tape rows with the X field and the 64-column dW1 panels) and the insert of
+(rnn_act_rows_warp_kernel<R, NB, 256>), the recurrent critic (rnn_critic_warp_kernel<256>), the chunked update
+(rnn_chunk_warp_kernel<POLICY, false, R, NB, 256>, its tape rows with the X field and the 64-column dW1 panels) and the insert of
 critic sections wider than 64 (orl_host_insert_rnn_wide_obs).
 
 Bars: one update over the whole buffer of a host rollout against rnn_ref64 driven with the masks (tests/rnn_ref64_masked.py)

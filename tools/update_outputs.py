@@ -7,7 +7,9 @@
 family and each rollout kernel at a small shape: C2 on tensor cores, on FFMA, with the shared model and with dual clip /
 plain MSE value loss; C2's flags on GridWorldEnv (rollout_tc_kernel) and with a GRU policy; C4 (GridWorld self-play,
 5 actions); C3 GRU, C3 JRPO and C3 with MLP nets (the simple_spread FFMA rollout); C5 (Gaussian head, host-stepped
-synthetic env).  Per path it saves the policy and critic (or shared model) `flat_params`, their Adam moment buffers,
+synthetic env); and host-stepped synthetic envs of wide shapes: SMAC 8m's (8 agents, Dict observations of 80 policy and
+168 critic features, Discrete(14) with env-reported masks) with GRU and with MLP nets, and Box(256) observations with
+Discrete(64) and GRU nets (the one-row-per-warp GRU act and update).  Per path it saves the policy and critic (or shared model) `flat_params`, their Adam moment buffers,
 `adam_steps`, the ValueNorm state, `train_info` and the rollout buffer the last iteration leaves (`buffer_<name>`) as
 DIR/<path>/<name>.npy.  `--compare` prints the largest distance in units in the last place per array, so a refactor
 that must not change results can be checked bit for bit (distance 0) against its parent commit.
@@ -35,7 +37,16 @@ PATHS = {
     "c3_jrpo": ("c3", ["--use_joint_action_loss", "true"]),
     "c3_mlp": ("c3", ["--use_recurrent_policy", "false"]),
     "c5_gaussian_host": (None, []),
+    "smac8m_gru_host": ("host", ["--use_recurrent_policy", "true", "--use_wide_recurrent_head", "true",
+                                 "--use_wide_recurrent_observations", "true"]),
+    "smac8m_mlp_host": ("host", ["--use_wide_observations", "true"]),
+    "box256_gru_host": ("host", ["--use_recurrent_policy", "true", "--use_wide_recurrent_head", "true",
+                                 "--use_wide_recurrent_observations", "true"]),
 }
+# host-stepped wide paths: (agents, policy features, critic features or None for a Box observation, actions, masks)
+HOST_SHAPES = {"smac8m_gru_host": (8, 80, 168, 14, True), "smac8m_mlp_host": (8, 80, 168, 14, True),
+               "box256_gru_host": (1, 256, None, 64, False)}
+HOST_ENVS, HOST_T = 16, 16
 
 
 BUFFER = ("actions", "action_log_probs", "policy_obs", "critic_obs", "rewards", "masks", "active_masks", "value_preds", "returns",
@@ -91,12 +102,64 @@ def run_host_gaussian():
     return state_arrays(agent.driver)
 
 
+class WideHostEnv:
+    """Host-stepped synthetic env: n envs x agents, observations ~ N(0, 1) (a Dict {"policy": d, "critic": dc}, or a Box
+    of d when dc is None), Discrete(n_actions) with a random legal subset in info["action_masks"] when masks, rewards
+    ~ N(0, 1), done ~ Bernoulli(0.05) per env."""
+
+    def __init__(self, n, agents, d, dc, n_actions, masks, seed=0):
+        from openrl_b200 import spaces
+
+        box = lambda w: spaces.Box(-np.inf, np.inf, (w,), np.float32)  # noqa: E731
+        self.parallel_env_num, self.agent_num, self.d, self.dc, self.n, self.masks = n, agents, d, dc, n_actions, masks
+        self.observation_space = box(d) if dc is None else spaces.Dict({"policy": box(d), "critic": box(dc)})
+        self.action_space = spaces.Discrete(n_actions)
+        self.rng = np.random.default_rng(seed)
+
+    def _obs(self):
+        x = lambda w: self.rng.standard_normal((self.parallel_env_num, self.agent_num, w)).astype(np.float32)  # noqa: E731
+        return x(self.d) if self.dc is None else {"policy": x(self.d), "critic": x(self.dc)}
+
+    def _infos(self):
+        if not self.masks:
+            return [{} for _ in range(self.parallel_env_num)]
+        m = (self.rng.random((self.parallel_env_num, self.agent_num, self.n)) < 0.7).astype(np.int8)
+        m[..., 0] = 1
+        return [{"action_masks": m[i]} for i in range(self.parallel_env_num)]
+
+    def reset(self, seed=None):
+        return self._obs(), self._infos()
+
+    def step(self, actions):
+        done = np.repeat(self.rng.random((self.parallel_env_num, 1)) < 0.05, self.agent_num, axis=1)
+        return self._obs(), self.rng.standard_normal((self.parallel_env_num, self.agent_num, 1)), done, self._infos()
+
+
+def run_host_wide(name, flags):
+    import torch
+
+    from openrl_b200.configs.config import create_config_parser
+    from openrl_b200.envs.vec_env import HostVecEnv
+    from openrl_b200.modules.common import PPONet
+    from openrl_b200.runners.common import PPOAgent
+    from openrl_b200.utils.logger import Logger
+
+    cfg = create_config_parser().parse_args(["--seed", "0", "--episode_length", str(HOST_T), "--ppo_epoch", "2", "--num_mini_batch",
+                                             "2", "--data_chunk_length", "8", "--log_interval", "1000000"] + flags)
+    cfg.quiet = True
+    env = HostVecEnv(WideHostEnv(HOST_ENVS, *HOST_SHAPES[name]), wide_observations=True)
+    agent = PPOAgent(PPONet(env, cfg=cfg, device=f"cuda:{torch.cuda.current_device()}"))
+    agent.train(total_time_steps=HOST_ENVS * HOST_T * K, logger=Logger(quiet=True))
+    return state_arrays(agent.driver)
+
+
 def save(out_dir):
     import torch
 
     assert torch.cuda.is_available(), "update_outputs.py --out needs a CUDA device"
     for name, (workload, flags) in PATHS.items():
-        arrays = run_host_gaussian() if workload is None else run_device(workload, flags)
+        arrays = (run_host_gaussian() if workload is None else run_host_wide(name, flags) if workload == "host"
+                  else run_device(workload, flags))
         d = os.path.join(out_dir, name)
         os.makedirs(d, exist_ok=True)
         for k, a in arrays.items():
