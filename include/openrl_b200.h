@@ -98,6 +98,11 @@ int orl_gae(const float* rewards, float* value_preds, const float* masks,
  */
 #define ORL_HEAD_CATEGORICAL 0
 #define ORL_HEAD_GAUSSIAN 1
+/* DiagGaussian head of 1..64 dimensions (Box(n) with n up to 64): the parameter layout, actions and log-probs of
+ * ORL_HEAD_GAUSSIAN, run on the 64-wide head tile.  Taken by orl_rollout (ORL_ENV_NONE only), orl_policy_eval,
+ * orl_ppo_fwdbwd, orl_ppo_reduce, orl_ppo_apply and their peer variants; ORL_ERR_BAD_ARG on the tensor-core update,
+ * the orl_share_* entries, the self-play rollout and every device env.  ORL_HEAD_GAUSSIAN keeps 1..8. */
+#define ORL_HEAD_GAUSSIAN_WIDE 2
 #define ORL_ENV_NONE 0
 #define ORL_ENV_CARTPOLE 1
 #define ORL_ENV_GRIDWORLD 2
@@ -218,7 +223,7 @@ int orl_host_insert_wide_obs(const float* staged, int n_envs, int n_agents, int 
  * policy half of PPOModule.evaluate_actions (ppo_module.py:147-193), outside the fused update: obs (rows, d), actions
  * (rows) [Categorical: index as float32] or (rows, n) [DiagGaussian] -> log_probs and entropy with the shape of
  * `actions` (per row / per dimension; the caller takes the active-mask mean, act.py:160-168).  n_actions: 1..64 for
- * Categorical heads, 1..8 for DiagGaussian heads; obs_dim: 1..256 (ORL_ERR_BAD_ARG otherwise). */
+ * Categorical heads and ORL_HEAD_GAUSSIAN_WIDE, 1..8 for ORL_HEAD_GAUSSIAN; obs_dim: 1..256 (ORL_ERR_BAD_ARG otherwise). */
 int orl_policy_eval(const float* policy_params, int obs_dim, int n_actions, int activation_id, int head_kind,
                     const float* obs, const float* actions, const float* action_masks, float* log_probs,
                     float* entropy, long long rows, void* stream);
@@ -301,7 +306,7 @@ typedef struct OrlPpoArgs {
     float* grads;                /* (2, orl_ppo_grads_stride): true gradients, parameter layout (written by apply) */
     float* train_info;           /* (6) += {value_loss, critic_grad_norm, policy_loss, dist_entropy,
                                              actor_grad_norm, ratio}  (ppo.py:430-451) */
-    int32_t head_kind;           /* ORL_HEAD_*: with GAUSSIAN actions / old_log_probs are (T*B, n) */
+    int32_t head_kind;           /* ORL_HEAD_*: with GAUSSIAN or GAUSSIAN_WIDE actions / old_log_probs are (T*B, n) */
     float dual_clip_coeff;       /* cfg.dual_clip_coeff (used with ORL_PPO_DUAL_CLIP) */
     int64_t norm_rows;           /* rows of the GLOBAL minibatch (all ranks): the 1/rows loss weights, the reported
                                     ratio mean and the ValueNorm batch moments (mb_stats / norm_rows) refer to it, so

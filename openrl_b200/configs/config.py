@@ -80,6 +80,11 @@ FLAGS = [
     # kernels, and dW1 reduced in 64-column panels.  Off, a GRU net keeps its limit of 64 features (NotImplementedError);
     # JRPO, use_share_model and the device-env GRU rollout keep it either way
     ("use_wide_recurrent_observations", _bool, False),
+    # feed-forward policies with DiagGaussian heads of 9..64 dimensions (Box action spaces such as dm_control's humanoid,
+    # 21 actions): the 64-wide head tile of the host act, eval and FFMA update kernels (ORL_HEAD_GAUSSIAN_WIDE).  Off, a
+    # DiagGaussian head keeps its limit of 8 dimensions (NotImplementedError above); heads of up to 8 dimensions run the
+    # same kernels either way, and GRU policies, use_share_model and JRPO keep the limit with the option on
+    ("use_wide_gaussian_head", _bool, False),
     ("use_tf32", _bool, True),
 ]
 

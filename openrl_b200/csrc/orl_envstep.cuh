@@ -185,9 +185,11 @@ __device__ __forceinline__ uint4 action_philox(uint64_t seed, uint64_t step, uin
 
 // Exp(1) noise q[0..n) of (step, row): the reference-order table exp_noise[grow * n + j] when one is given (parity mode),
 // else -log U of the 8 draws of Philox lanes `lane`, `lane + 1`.
-// Lanes of one (step, row): 0, 1 the noise of actions 0..7 (wide_action_noise4 keeps them for those actions); 2..5 the
-// DiagGaussian normals (gaussian_act), and in the self-play rollout 2, 3 the opponent's noise and 4 its pick; 8..21 the
-// noise of actions 8..63 of a wide head, action j from draw (j - 8) % 4 of lane 8 + (j - 8) / 4.
+// Lanes of one (step, row): 0, 1 the noise of actions 0..7 (wide_action_noise4 keeps them for those actions); 2..33 the
+// DiagGaussian normals, dimensions [4k, 4k + 4) by Box-Muller of u1 from lane 2 + 2k and u2 from lane 3 + 2k (k = 0, 1:
+// gaussian_act's lanes 2..5; k = 0..15: gaussian_noise4 of a wide head), and in the self-play rollout 2, 3 the opponent's
+// noise and 4 its pick; 8..21 the noise of actions 8..63 of a wide Categorical head, action j from draw (j - 8) % 4 of
+// lane 8 + (j - 8) / 4.  A row has one head, so no two uses of one draw meet within a row.
 __device__ __forceinline__ void action_noise(const float* exp_noise, size_t grow, int n, uint64_t seed, uint64_t step,
                                              uint32_t row, float (&q)[MAX_OUT], uint32_t lane = 0u) {
     if (exp_noise) {
@@ -297,6 +299,44 @@ __device__ __forceinline__ void gaussian_act(const float (&mean)[MAX_OUT], int n
             if (!deterministic) {
                 const float eps = noise_table ? noise_table[grow * n + j] : __uint_as_float(rr[j]);
                 act = __fadd_rn(__fmul_rn(eps, std), mean[j]);
+            }
+            actions[grow * n + j] = act;
+            log_probs[grow * n + j] = gaussian_log_prob(act - mean[j], std, ls);
+        }
+    }
+}
+
+// N(0, 1) noise eps[0..4) of dimensions j0..j0+3 (j0 % 4 == 0) of a wide DiagGaussian head's row: Box-Muller of u1 from
+// Philox lane 2 + j0 / 2 and u2 from lane 3 + j0 / 2, gaussian_act's expression, so dimensions 0..7 draw what
+// gaussian_act draws for them, bit for bit
+__device__ __forceinline__ void gaussian_noise4(uint64_t seed, uint64_t step, uint32_t row, int j0, float (&eps)[4]) {
+    const uint32_t lane = 2u + (uint32_t)(j0 / 2);
+    const uint4 r1 = action_philox(seed, step, row, lane), r2 = action_philox(seed, step, row, lane + 1u);
+    const uint32_t u1[4] = {r1.x, r1.y, r1.z, r1.w}, u2[4] = {r2.x, r2.y, r2.z, r2.w};
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        const float rad = sqrtf(-2.0f * logf(u32_to_unit_open(u1[c])));
+        eps[c] = rad * cospif(2.0f * u32_to_unit_open(u2[c]));
+    }
+}
+
+// DiagGaussian act of dimensions j0..j0+3 (those < n) of one row of a wide head (1..64 dimensions): gaussian_act's
+// arithmetic on the means mean[0..n) of the row, in shared memory.  The noise is the table entries in parity mode, else
+// gaussian_noise4; deterministic calls return the mean.
+__device__ __forceinline__ void gaussian_act4(const float* mean, int n, int j0, const float* logstd, bool deterministic,
+                                              const float* noise_table, uint64_t seed, uint64_t step, uint32_t row, size_t grow,
+                                              float* actions, float* log_probs) {
+    float eps[4] = {0.f, 0.f, 0.f, 0.f};
+    if (!noise_table && !deterministic) gaussian_noise4(seed, step, row, j0, eps);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        const int j = j0 + c;
+        if (j < n) {
+            const float ls = logstd[j], std = expf(ls);
+            float act = mean[j];
+            if (!deterministic) {
+                const float e = noise_table ? noise_table[grow * n + j] : eps[c];
+                act = __fadd_rn(__fmul_rn(e, std), mean[j]);
             }
             actions[grow * n + j] = act;
             log_probs[grow * n + j] = gaussian_log_prob(act - mean[j], std, ls);

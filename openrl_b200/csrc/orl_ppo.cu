@@ -107,10 +107,16 @@ __device__ __forceinline__ void wgrad_flush(float* __restrict__ scratch, const W
 // fc1 panel by panel; the backward re-stages each panel (the last one is still in Xs) and forms G1_p = dZ1^T X_p with
 // one 4x4 block per thread (MG = 1), which the thread adds into its own elements of this CTA's partial row: one owner
 // per element, tiles in the CTA's order, no atomics.
-template <bool POLICY, int NB = MAX_OUT, bool PANELS = false>
+// GAUSS (NB = 64): a DiagGaussian head of 1..64 dimensions (ORL_HEAD_GAUSSIAN_WIDE) on the same tiles.  The means are the
+// head tile; the loss is elementwise per (row, dimension), so it runs dimension-parallel: thread t owns dimension
+// j = t % 64 of rows t / 64, t / 64 + 4, ..., writes dL/dmean over the mean (the dL tile of the Categorical pass) and
+// keeps dL/dlogstd of its rows in one register; the 4 partials of a dimension are added in row-group order at the flush.
+template <bool POLICY, int NB = MAX_OUT, bool PANELS = false, bool GAUSS = false>
 __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, int cta, int G) {
     constexpr bool WIDE = NB == MAX_OUT_WIDE;
     static_assert(POLICY || !WIDE, "the critic's head is one value");
+    static_assert(WIDE || !GAUSS, "GAUSS is the wide DiagGaussian head");
+    static_assert(P_NT % MAX_OUT_WIDE == 0, "whole row groups of the dimension-parallel loss");
     const int d = POLICY ? a.obs_dim : a.critic_obs_dim;
     const int n = POLICY ? a.n_actions : 1;
     const float* params = POLICY ? a.policy_params : a.critic_params;
@@ -144,6 +150,7 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
     float g3[4][4] = {}, g1[4][4] = {}, gh[4][4] = {}, db3[4] = {}, db1[4] = {}, dbh[4] = {};
     const bool gaussian = POLICY && !WIDE && a.head_kind == ORL_HEAD_GAUSSIAN;
     float dls_acc[MAX_OUT] = {};   // dL/dlogstd partial sums of this thread's rows (Gaussian head)
+    float dls_wide = 0.f;          // GAUSS: dL/dlogstd[tid % 64] over this thread's rows
     float loss0 = 0.f, loss1 = 0.f, loss2 = 0.f;  // policy: policy_loss, entropy, ratio | critic: value_loss
 
     // G1 element (row 4 jb + r, column 64 pnl + 4 kb + c) of a panelled pass lives in this CTA's partial row; its owner
@@ -202,7 +209,34 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
         if constexpr (WIDE) {
             head_tile<P_M, P_NT>(w, N3s, DZs);
             __syncthreads();
-            if (tid < P_M) {   // one thread per row: the logits row becomes the dL/dlogits row
+            if constexpr (GAUSS) {   // the means tile becomes the dL/dmean tile, K = pad4(n) columns
+                constexpr int RG = P_NT / MAX_OUT_WIDE;   // row groups
+                const int j = tid % MAX_OUT_WIDE;
+                if (j < pad4(n)) {
+                    const float ls = j < n ? params[net_offsets(d, n, 1).ls + j] : 0.f, std = expf(ls), var = std * std;
+                    const float ent_j = gaussian_entropy(ls);
+                    for (int r = tid / MAX_OUT_WIDE; r < P_M; r += RG) {
+                        float* x = DZs + r * LDA + j;
+                        if (r < rows_here && j < n) {
+                            const long long gi = row_idx[r];
+                            const float active = row_act[r];
+                            const float wrow = mb.weight(pol_masks, active);
+                            const float went_row = pol_masks ? active * mb.inv_act : mb.inv_rows / (float)n;
+                            const float diff = a.actions[gi * n + j] - *x;
+                            const PgTerm pg = pg_term(gaussian_log_prob(diff, std, ls), a.old_log_probs[gi * n + j],
+                                                      apply_adv_norm(mb.adv, row_c[r]), a.clip_param, a.flags, a.dual_clip_coeff);
+                            loss0 += pg.loss * wrow;
+                            loss1 += ent_j * went_row;
+                            loss2 += pg.ratio / (float)n;
+                            const float dlp = pg.dlogp * wrow;
+                            *x = dlp * diff / var;
+                            dls_wide += dlp * (diff * diff / var - 1.0f) - a.entropy_coef * went_row;
+                        } else {
+                            *x = 0.f;
+                        }
+                    }
+                }
+            } else if (tid < P_M) {   // one thread per row: the logits row becomes the dL/dlogits row
                 float* x = DZs + tid * LDA;
                 if (tid < rows_here) {
                     const long long gi = row_idx[tid];
@@ -354,7 +388,16 @@ __device__ __forceinline__ void ppo_net_pass(const OrlPpoArgs& a, float* smem, i
     wgrad_flush(scratch, map3, 16, 16, g3, db3, H, H, part + fo.g3, part + fo.db3);
     wgrad_flush(scratch, maph, JBH, 16, gh, dbh, n, H, part + fo.gh, part + fo.dbh);
     __syncthreads();
-    if (WIDE) {     // no logstd: a Categorical head
+    if (GAUSS) {    // dL/dlogstd: the 4 row groups' partials of each dimension, in row-group order
+        scratch[tid] = dls_wide;
+        __syncthreads();
+        if (tid < n) {
+            float sv = 0.f;
+            for (int g2 = 0; g2 < P_NT / MAX_OUT_WIDE; ++g2) sv += scratch[g2 * MAX_OUT_WIDE + tid];
+            part[fo.dls + tid] = sv;
+        }
+        __syncthreads();
+    } else if (WIDE) {     // no logstd: a Categorical head
         if (tid < n) part[fo.dls + tid] = 0.f;
     } else if (POLICY) {   // dL/dlogstd: block reduction of the per-thread partial sums (zero for categorical heads)
         const int lane = tid & 31, warp = tid >> 5;
@@ -396,6 +439,15 @@ __global__ void __launch_bounds__(P_NT, 1) ppo_fwdbwd_kernel(const OrlPpoArgs a)
     extern __shared__ __align__(16) float smem[];
     const int G = a.grid_per_net;
     if ((int)blockIdx.x < G) ppo_net_pass<true, NB, PANELS_POLICY>(a, smem, blockIdx.x, G);
+    else ppo_net_pass<false, MAX_OUT, PANELS_CRITIC>(a, smem, blockIdx.x - G, G);
+}
+
+// the update of a DiagGaussian head of 1..64 dimensions (ORL_HEAD_GAUSSIAN_WIDE); the critic pass is the NB = 8 one
+template <bool PANELS_POLICY, bool PANELS_CRITIC>
+__global__ void __launch_bounds__(P_NT, 1) ppo_fwdbwd_gaussian_wide_kernel(const OrlPpoArgs a) {
+    extern __shared__ __align__(16) float smem[];
+    const int G = a.grid_per_net;
+    if ((int)blockIdx.x < G) ppo_net_pass<true, MAX_OUT_WIDE, PANELS_POLICY, true>(a, smem, blockIdx.x, G);
     else ppo_net_pass<false, MAX_OUT, PANELS_CRITIC>(a, smem, blockIdx.x - G, G);
 }
 
@@ -612,11 +664,19 @@ size_t fwdbwd_wide_smem_bytes(int d, int dc) {
     return std::max(pol, cri) * sizeof(float);
 }
 
+// The arguments ppo_apply_kernel runs on: both DiagGaussian kinds have one parameter layout (logstd[n] after bh) and one
+// folded layout, and the kernel finds logstd from head_kind == ORL_HEAD_GAUSSIAN; so ORL_HEAD_GAUSSIAN_WIDE runs as that.
+OrlPpoArgs apply_args(const OrlPpoArgs& a) {
+    OrlPpoArgs b = a;
+    if (b.head_kind == ORL_HEAD_GAUSSIAN_WIDE) b.head_kind = ORL_HEAD_GAUSSIAN;
+    return b;
+}
+
 int check_ppo_args(const OrlPpoArgs& a) {
     ORL_CHECK_ARG(a.obs_dim > 0 && a.obs_dim <= orl::MAX_OBS_WIDE && a.critic_obs_dim > 0 && a.critic_obs_dim <= orl::MAX_OBS_WIDE,
                   "obs dims must be in 1..256");
     ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= orl::MAX_OUT_WIDE, "n_actions must be in 1..64");
-    ORL_CHECK_ARG(a.n_actions <= orl::MAX_OUT || a.head_kind == ORL_HEAD_CATEGORICAL,
+    ORL_CHECK_ARG(a.n_actions <= orl::MAX_OUT || a.head_kind == ORL_HEAD_CATEGORICAL || a.head_kind == ORL_HEAD_GAUSSIAN_WIDE,
                   "n_actions must be in 1..8 for Gaussian heads (1..64 for Categorical heads)");
     ORL_CHECK_ARG(a.activation_id >= 0 && a.activation_id <= 3, "activation_id");
     ORL_CHECK_ARG(a.grid_per_net > 0, "grid_per_net");
@@ -650,8 +710,10 @@ extern "C" int orl_ppo_fwdbwd(const OrlPpoArgs* args, void* stream) {
                       a.returns && a.active_masks && a.gae_stats && a.mb_stats, "null rollout buffer");
     ORL_CHECK_ARG(!(a.flags & ORL_PPO_VALUENORM) || a.vn_state, "vn_state required with VALUENORM");
     ORL_CHECK_ARG(a.indices || (a.row_begin >= 0 && a.row_begin + a.batch_rows <= a.total_rows), "row range");
-    ORL_CHECK_ARG(a.head_kind == ORL_HEAD_CATEGORICAL || a.head_kind == ORL_HEAD_GAUSSIAN, "head_kind");
+    ORL_CHECK_ARG(a.head_kind == ORL_HEAD_CATEGORICAL || a.head_kind == ORL_HEAD_GAUSSIAN || a.head_kind == ORL_HEAD_GAUSSIAN_WIDE,
+                  "head_kind");
     if (a.flags & ORL_PPO_TF32) {
+        ORL_CHECK_ARG(a.head_kind != ORL_HEAD_GAUSSIAN_WIDE, "ORL_PPO_TENSORCORE: ORL_HEAD_GAUSSIAN_WIDE is not supported");
         ORL_CHECK_ARG(a.n_actions <= orl::MAX_OUT, "ORL_PPO_TENSORCORE: n_actions must be in 1..8");
         ORL_CHECK_ARG(a.obs_dim <= orl::OBS_PANEL && a.critic_obs_dim <= orl::OBS_PANEL, "ORL_PPO_TENSORCORE: obs dims must be in 1..64");
         if (a.head_kind != ORL_HEAD_CATEGORICAL) {
@@ -671,6 +733,20 @@ extern "C" int orl_ppo_fwdbwd(const OrlPpoArgs* args, void* stream) {
                   : pp ? ppo_fwdbwd_kernel<orl::MAX_OUT_WIDE, true, false> : ppo_fwdbwd_kernel<orl::MAX_OUT_WIDE, false, true>)
                : (pp && pc ? ppo_fwdbwd_kernel<orl::MAX_OUT, true, true>
                   : pp ? ppo_fwdbwd_kernel<orl::MAX_OUT, true, false> : ppo_fwdbwd_kernel<orl::MAX_OUT, false, true>);
+    if (a.head_kind == ORL_HEAD_GAUSSIAN_WIDE) {   // the wide layout whatever the width (fwdbwd_wide_smem_bytes)
+        void (*const gk)(OrlPpoArgs) = pp && pc ? ppo_fwdbwd_gaussian_wide_kernel<true, true>
+                                       : pp ? ppo_fwdbwd_gaussian_wide_kernel<true, false>
+                                       : pc ? ppo_fwdbwd_gaussian_wide_kernel<false, true> : ppo_fwdbwd_gaussian_wide_kernel<false, false>;
+        const size_t gsmem = fwdbwd_wide_smem_bytes(ds, dcs);   // 226 240 B at d = dc = 256 (the d = 64 layout)
+        if (gsmem > 227 * 1024) {
+            orl::set_last_error("orl_ppo_fwdbwd: the wide DiagGaussian pass needs %zu bytes of shared memory", gsmem);
+            return ORL_ERR_UNSUPPORTED;
+        }
+        if (int e = orl::allow_dynamic_smem(gk, 227 * 1024)) return e;
+        gk<<<2 * a.grid_per_net, P_NT, gsmem, reinterpret_cast<cudaStream_t>(stream)>>>(a);
+        ORL_LAUNCH_CHECK("ppo_fwdbwd_gaussian_wide_kernel");
+        return 0;
+    }
     if (int e = orl::allow_dynamic_smem(kern, 227 * 1024)) return e;
     kern<<<2 * a.grid_per_net, P_NT, smem, reinterpret_cast<cudaStream_t>(stream)>>>(a);
     ORL_LAUNCH_CHECK("ppo_fwdbwd_kernel");
@@ -730,7 +806,7 @@ extern "C" int orl_ppo_apply_peer(const OrlPpoArgs* args, const OrlPeerArgs* pee
     ORL_CHECK_ARG(a.policy_adam_m && a.policy_adam_v && a.critic_adam_m && a.critic_adam_v && a.adam_steps && a.lrs,
                   "null optimiser state");
     ORL_CHECK_ARG(a.mb_stats, "mb_stats");
-    ppo_apply_kernel<true><<<2, 1024, 0, reinterpret_cast<cudaStream_t>(stream)>>>(a, *peer);
+    ppo_apply_kernel<true><<<2, 1024, 0, reinterpret_cast<cudaStream_t>(stream)>>>(apply_args(a), *peer);
     ORL_LAUNCH_CHECK("ppo_apply_kernel(peer)");
     return 0;
 }
@@ -742,7 +818,7 @@ extern "C" int orl_ppo_apply(const OrlPpoArgs* args, void* stream) {
     ORL_CHECK_ARG(a.policy_adam_m && a.policy_adam_v && a.critic_adam_m && a.critic_adam_v && a.adam_steps && a.lrs,
                   "null optimiser state");
     ORL_CHECK_ARG(a.mb_stats, "mb_stats");
-    ppo_apply_kernel<false><<<2, 1024, 0, reinterpret_cast<cudaStream_t>(stream)>>>(a, OrlPeerArgs{});
+    ppo_apply_kernel<false><<<2, 1024, 0, reinterpret_cast<cudaStream_t>(stream)>>>(apply_args(a), OrlPeerArgs{});
     ORL_LAUNCH_CHECK("ppo_apply_kernel");
     return 0;
 }

@@ -151,6 +151,52 @@ __global__ void __launch_bounds__(R_NT) rollout_kernel(const OrlRolloutArgs a) {
     }
 }
 
+// The host act (ORL_ENV_NONE, one step per call) of a DiagGaussian head of 1..64 dimensions (ORL_HEAD_GAUSSIAN_WIDE):
+// rollout_kernel's ORL_ENV_NONE path at NB = 64 up to the means tile in N1s, then one thread per (row, 4 dimensions).
+// A kernel of its own, so that rollout_kernel's instances keep their code.
+template <int R_M, bool PANELS>
+__global__ void __launch_bounds__(R_NT) rollout_gaussian_wide_kernel(const OrlRolloutArgs a) {
+    extern __shared__ __align__(16) float smem[];
+    const int N = a.n_envs, A = a.n_agents, B = N * A, d = a.obs_dim, n = a.n_actions, t = a.t_begin;
+    const int ldx = PANELS ? LDX_PANEL : pad4(d) + 4;
+    float* p = smem;
+    SmemWeights w = carve_weights<MAX_OUT_WIDE>(p, PANELS ? OBS_PANEL : d, false);
+    float* Xs = p;  p += R_M * ldx;
+    float* N1s = p; p += R_M * LDA;
+    float* N3s = p; p += R_M * LDA;
+    const int envs_per_cta = R_M / A;
+    const int env0 = blockIdx.x * envs_per_cta;
+    const int row0 = env0 * A, rows_here = min(envs_per_cta, N - env0) * A;
+    const int tid = threadIdx.x;
+    load_weights_folded<R_NT, MAX_OUT_WIDE, PANELS>(w, a.policy_params, d, n, false);
+    auto obs_row = [&](int r) -> const float* { return r < rows_here ? a.policy_obs + ((size_t)t * B + row0 + r) * d : nullptr; };
+    float mu1[R_M / (R_NT / 16)], rstd1[R_M / (R_NT / 16)], rstd3[R_M / (R_NT / 16)];
+    unsigned pm;
+    if constexpr (PANELS) {
+        float acc[R_M / (R_NT / 16)][4];
+        fc1_panels<R_M, R_NT>(w, a.policy_params + net_offsets(d, n).w1, d, Xs, obs_row, acc);
+        trunk_from_z1<R_M, R_NT, false>(w, acc, a.activation_id, N1s, N3s, mu1, rstd1, rstd3, pm);
+    } else {
+        for (int i = tid; i < R_M * ldx; i += R_NT) {
+            const int r = i / ldx, k = i % ldx;
+            Xs[i] = (r < rows_here && k < d) ? obs_row(r)[k] : 0.f;
+        }
+        __syncthreads();
+        trunk_forward<R_M, R_NT, false>(w, Xs, ldx, d, a.activation_id, N1s, N3s, mu1, rstd1, rstd3, pm);
+    }
+    __syncthreads();
+    head_tile<R_M, R_NT>(w, N3s, N1s);
+    __syncthreads();
+    const int groups = (n + 3) / 4;
+    const float* logstd = a.policy_params + net_offsets(d, n, 1).ls;
+    const uint64_t step = a.rng_step_base + (a.rng_counter ? *a.rng_counter : 0ull) + (uint64_t)t;
+    for (int i = tid; i < rows_here * groups; i += R_NT) {
+        const int r = i / groups;
+        gaussian_act4(N1s + r * LDA, n, 4 * (i % groups), logstd, a.deterministic != 0, a.exp_noise, a.rng_seed, step,
+                      (uint32_t)(row0 + r + a.rng_row_offset), (size_t)t * B + row0 + r, a.actions, a.action_log_probs);
+    }
+}
+
 __global__ void env_reset_kernel(int env_kind, int N, double* env_f64, uint64_t* env_u64, int32_t* env_i32,
                                  const int32_t* env_table, int env_table_len, uint64_t seed, float* obs_out,
                                  float* critic_obs_out) {
@@ -285,6 +331,23 @@ __global__ void __launch_bounds__(C_NT) policy_eval_wide_kernel(const float* __r
     });
 }
 
+// policy_eval_kernel of a DiagGaussian head of 1..64 dimensions (ORL_HEAD_GAUSSIAN_WIDE): the means x[0..n) of the row
+// from the 64-wide head tile, then policy_eval_kernel's per-dimension log-prob and entropy
+template <bool PANELS>
+__global__ void __launch_bounds__(C_NT) policy_eval_gaussian_wide_kernel(const float* __restrict__ params, int d, int n, int activation_id,
+                                                                         const float* __restrict__ obs, const float* __restrict__ actions,
+                                                                         float* __restrict__ logp_out, float* __restrict__ entropy_out,
+                                                                         long long rows) {
+    const float* logstd = params + net_offsets(d, n, 1).ls;
+    rows_forward<MAX_OUT_WIDE, PANELS>(params, d, n, activation_id, obs, rows, [&](long long g, float* x) {
+        for (int j = 0; j < n; ++j) {
+            const float ls = logstd[j];
+            logp_out[g * n + j] = gaussian_log_prob(actions[g * n + j] - x[j], expf(ls), ls);
+            entropy_out[g * n + j] = gaussian_entropy(ls);
+        }
+    });
+}
+
 // ---- insert of one host env.step into the rollout buffer (OnPolicyDriver.add2buffer, onpolicy_driver.py:80-152) -----------
 // staged = [obs (B*d) (| critic obs (B*dc)) | rewards (B) | dones (B) (| action masks (B*n))] as uploaded from the host in
 // ONE copy; one thread per row.  Row r of the insert; returns whether every agent of the row's env is done.  The critic
@@ -349,6 +412,12 @@ __global__ void host_insert_rnn_kernel(const float* __restrict__ staged, int n_e
 template <int ENV, int NB = MAX_OUT, bool PANELS = false>
 auto rollout_rows(int rm) {
     return rm == 8 ? rollout_kernel<8, ENV, NB, PANELS> : rm == 16 ? rollout_kernel<16, ENV, NB, PANELS> : rollout_kernel<32, ENV, NB, PANELS>;
+}
+
+template <bool PANELS>
+auto rollout_gaussian_wide_rows(int rm) {
+    return rm == 8 ? rollout_gaussian_wide_kernel<8, PANELS> : rm == 16 ? rollout_gaussian_wide_kernel<16, PANELS>
+                                                                        : rollout_gaussian_wide_kernel<32, PANELS>;
 }
 
 // launch of a row-batch forward kernel over `rows` rows of obs_dim d: grid = min(tiles, 2 x SMs).  A panelled kernel
@@ -424,12 +493,14 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
     ORL_CHECK_ARG(a.obs_dim <= orl::OBS_PANEL || a.env_kind == ORL_ENV_NONE,
                   "obs_dim must be in 1..64 (65..256: host-stepped envs, ORL_ENV_NONE)");
     ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= orl::MAX_OUT_WIDE, "n_actions must be in 1..64");
-    ORL_CHECK_ARG(a.n_actions <= orl::MAX_OUT || (a.env_kind == ORL_ENV_NONE && a.head_kind == ORL_HEAD_CATEGORICAL),
+    ORL_CHECK_ARG(a.n_actions <= orl::MAX_OUT || (a.env_kind == ORL_ENV_NONE && a.head_kind == ORL_HEAD_CATEGORICAL) ||
+                      (a.env_kind == ORL_ENV_NONE && a.head_kind == ORL_HEAD_GAUSSIAN_WIDE),
                   "n_actions must be in 1..8 (9..64: Categorical heads on host-stepped envs, ORL_ENV_NONE)");
     ORL_CHECK_ARG(a.t_begin >= 0 && a.t_begin < a.t_end && a.t_end <= a.episode_length, "step range");
     ORL_CHECK_ARG(a.activation_id >= 0 && a.activation_id <= 3, "activation_id");
     ORL_CHECK_ARG(a.policy_params && a.policy_obs && a.actions && a.action_log_probs, "null buffer");
-    ORL_CHECK_ARG(a.head_kind == ORL_HEAD_CATEGORICAL || (a.head_kind == ORL_HEAD_GAUSSIAN && a.env_kind == ORL_ENV_NONE),
+    ORL_CHECK_ARG(a.head_kind == ORL_HEAD_CATEGORICAL || (a.head_kind == ORL_HEAD_GAUSSIAN && a.env_kind == ORL_ENV_NONE) ||
+                      (a.head_kind == ORL_HEAD_GAUSSIAN_WIDE && a.env_kind == ORL_ENV_NONE),
                   "Gaussian heads act on host-stepped envs (ORL_ENV_NONE)");
     if (a.env_kind == ORL_ENV_NONE) {
         ORL_CHECK_ARG(a.t_end == a.t_begin + 1, "ORL_ENV_NONE acts for one step per call");
@@ -469,14 +540,17 @@ extern "C" int orl_rollout(const OrlRolloutArgs* args, void* stream) {
     const int grid = (a.n_envs + envs_per_cta - 1) / envs_per_cta;
     const int ds = std::min(a.obs_dim, orl::OBS_PANEL);   // a panelled fc1 takes the layout of d = 64
     const int ldx = orl::pad4(ds) + 4;
-    const bool mpe = a.env_kind == ORL_ENV_MPE_SPREAD, wide = a.n_actions > orl::MAX_OUT, wide_obs = a.obs_dim > orl::OBS_PANEL;
+    // a DiagGaussian head of ORL_HEAD_GAUSSIAN_WIDE runs on the 64-wide head tile whatever its width
+    const bool gw = a.head_kind == ORL_HEAD_GAUSSIAN_WIDE;
+    const bool mpe = a.env_kind == ORL_ENV_MPE_SPREAD, wide = a.n_actions > orl::MAX_OUT || gw, wide_obs = a.obs_dim > orl::OBS_PANEL;
     const size_t smem = sizeof(float) * ((wide ? orl::smem_weights_floats<orl::MAX_OUT_WIDE>(ds, false)
                                                : orl::smem_weights_floats(ds, false)) + rm * ldx + 2 * rm * orl::LDA + rm);
     // simple_spread has neither wide observations nor a wide head
-    void (*const kern)(OrlRolloutArgs) =
+    void (*kern)(OrlRolloutArgs) =
         mpe ? rollout_rows<ORL_ENV_MPE_SPREAD>(rm)
         : wide ? (wide_obs ? rollout_rows<ORL_ENV_NONE, orl::MAX_OUT_WIDE, true>(rm) : rollout_rows<ORL_ENV_NONE, orl::MAX_OUT_WIDE>(rm))
                : (wide_obs ? rollout_rows<ORL_ENV_NONE, orl::MAX_OUT, true>(rm) : rollout_rows<ORL_ENV_NONE>(rm));
+    if (gw) kern = wide_obs ? rollout_gaussian_wide_rows<true>(rm) : rollout_gaussian_wide_rows<false>(rm);
     if (int e = orl::allow_dynamic_smem(kern, 200 * 1024)) return e;
     kern<<<grid, R_NT, smem, st>>>(a);
     ORL_LAUNCH_CHECK("rollout_kernel");
@@ -503,11 +577,15 @@ extern "C" int orl_policy_eval(const float* policy_params, int obs_dim, int n_ac
     ORL_CHECK_ARG(obs_dim > 0 && obs_dim <= orl::MAX_OBS_WIDE, "obs_dim must be in 1..256");
     ORL_CHECK_ARG(n_actions > 0 && n_actions <= orl::MAX_OUT_WIDE, "n_actions must be in 1..64");
     ORL_CHECK_ARG(rows > 0 && activation_id >= 0 && activation_id <= 3, "rows / activation_id");
-    ORL_CHECK_ARG(head_kind == ORL_HEAD_CATEGORICAL || head_kind == ORL_HEAD_GAUSSIAN, "head_kind");
-    ORL_CHECK_ARG(n_actions <= orl::MAX_OUT || head_kind == ORL_HEAD_CATEGORICAL,
+    ORL_CHECK_ARG(head_kind == ORL_HEAD_CATEGORICAL || head_kind == ORL_HEAD_GAUSSIAN || head_kind == ORL_HEAD_GAUSSIAN_WIDE, "head_kind");
+    ORL_CHECK_ARG(n_actions <= orl::MAX_OUT || head_kind == ORL_HEAD_CATEGORICAL || head_kind == ORL_HEAD_GAUSSIAN_WIDE,
                   "n_actions must be in 1..8 for Gaussian heads (1..64 for Categorical heads)");
     const bool wide_obs = obs_dim > orl::OBS_PANEL;
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (head_kind == ORL_HEAD_GAUSSIAN_WIDE)
+        return launch_rows_forward<orl::MAX_OUT_WIDE>(wide_obs ? policy_eval_gaussian_wide_kernel<true> : policy_eval_gaussian_wide_kernel<false>,
+                                                      "policy_eval_gaussian_wide_kernel", obs_dim, rows, st, policy_params, obs_dim,
+                                                      n_actions, activation_id, obs, actions, log_probs, entropy, rows);
     if (n_actions > orl::MAX_OUT)
         return launch_rows_forward<orl::MAX_OUT_WIDE>(wide_obs ? policy_eval_wide_kernel<true> : policy_eval_wide_kernel<false>,
                                                       "policy_eval_wide_kernel", obs_dim, rows, st, policy_params, obs_dim, n_actions,

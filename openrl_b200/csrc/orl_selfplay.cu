@@ -180,6 +180,7 @@ int check_selfplay(const OrlSelfPlayArgs& s) {
     ORL_CHECK_ARG(a.env_i32 && s.pool_count && s.pool_stats, "env state / pool buffers");
     ORL_CHECK_ARG(s.pool_capacity >= 0 && (s.pool_capacity == 0 || (s.pool_params && s.pool_stride > 0)), "pool");
     ORL_CHECK_ARG(s.strategy == ORL_SP_RANDOM || s.strategy == ORL_SP_LAST, "strategy");
+    ORL_CHECK_ARG(a.head_kind != ORL_HEAD_GAUSSIAN_WIDE, "the self-play rollout acts with Categorical heads");
     return 0;
 }
 

@@ -336,7 +336,7 @@ class OnPolicyDriver:
         d = self.buffer.data
         B, n = d.n_rollout_threads * d.num_agents, d.n_actions
         host = torch.empty(self.episode_length, B, n, dtype=torch.float32, pin_memory=True)
-        gaussian = self.trainer.algo_module.models["policy"].head_kind == lib.HEAD_GAUSSIAN
+        gaussian = lib.is_gaussian(self.trainer.algo_module.models["policy"].head_kind)
         for t in range(self.episode_length):
             if gaussian:
                 host[t].normal_()       # Normal.sample() == torch.normal(mean, std) == N(0,1)*std + mean
@@ -429,7 +429,7 @@ class OnPolicyDriver:
             return None
         d = self.buffer.data
         noise = torch.empty(d.n_rollout_threads * d.num_agents, d.n_actions, dtype=torch.float32)
-        noise.normal_() if self.trainer.algo_module.models["policy"].head_kind == lib.HEAD_GAUSSIAN else noise.exponential_(1)
+        noise.normal_() if lib.is_gaussian(self.trainer.algo_module.models["policy"].head_kind) else noise.exponential_(1)
         self.h2d_bytes += noise.numel() * 4
         return noise.to(self.device)
 

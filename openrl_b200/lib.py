@@ -239,6 +239,12 @@ _SIGNATURES.update({
 ENV_NONE, ENV_CARTPOLE, ENV_GRIDWORLD, ENV_MPE_SPREAD, ENV_GRIDWORLD_2P = 0, 1, 2, 3, 4
 SP_RANDOM, SP_LAST = 0, 1
 HEAD_CATEGORICAL, HEAD_GAUSSIAN = 0, 1
+HEAD_GAUSSIAN_WIDE = 2   # a DiagGaussian head of 1..64 dimensions on the 64-wide head tile (cfg.use_wide_gaussian_head)
+
+
+def is_gaussian(head_kind):
+    """Whether a head kind is a DiagGaussian head: actions and log-probs (rows, n), N(0, 1) parity noise."""
+    return head_kind in (HEAD_GAUSSIAN, HEAD_GAUSSIAN_WIDE)
 GAE_USE_GAE, GAE_PROPER_TIME_LIMITS, GAE_DENORM = 1, 2, 4
 PPO_HUBER, PPO_CLIP_VALUE, PPO_VALUE_ACTIVE_MASKS, PPO_POLICY_ACTIVE_MASKS = 1, 2, 4, 8
 PPO_VALUENORM, PPO_ADV_NORMALIZE, PPO_MAX_GRAD_NORM, PPO_TENSORCORE = 16, 32, 64, 128

@@ -29,13 +29,20 @@ class PolicyNetwork(nn.Module):
             raise NotImplementedError("recurrent policies are built for Discrete action spaces")
         # a feed-forward Categorical head runs up to 64 actions (a logits tile in the kernels); a GRU policy's head runs up
         # to 64 with cfg.use_wide_recurrent_head (a lane-owned 64-vector in the GRU kernels) and up to 8 without; the
-        # DiagGaussian heads keep the per-thread head of up to 8 outputs
+        # DiagGaussian heads keep the per-thread head of up to 8 outputs, and run up to 64 with cfg.use_wide_gaussian_head
+        # (the 64-wide head tile, lib.HEAD_GAUSSIAN_WIDE, for widths above 8)
+        wide_gaussian = self.act.continuous_action and bool(getattr(cfg, "use_wide_gaussian_head", False))
+        if wide_gaussian and self.n_actions > 64:
+            raise NotImplementedError("DiagGaussian heads are built for Box action spaces of width up to 64 "
+                                      "(use_wide_gaussian_head)")
         if self.n_actions > 64:
             raise NotImplementedError("Discrete action spaces of up to 64 actions are built")
         if self.n_actions > 8 and self.recurrent and not getattr(cfg, "use_wide_recurrent_head", False):
             raise NotImplementedError("recurrent policies are built for up to 8 actions (9..64 with use_wide_recurrent_head)")
-        if self.n_actions > 8 and self.act.continuous_action:
+        if self.n_actions > 8 and self.act.continuous_action and not wide_gaussian:
             raise NotImplementedError("DiagGaussian heads are built for Box action spaces of width up to 8")
+        if self.n_actions > 8 and wide_gaussian:
+            self.head_kind = 2                                           # lib.HEAD_GAUSSIAN_WIDE
         self.device = torch.device(device)
         self._flat = FlatParams(self, self.device)
 

@@ -127,7 +127,7 @@ class PPOModule:
             raise NotImplementedError("evaluate_actions for recurrent / shared nets runs inside the fused update kernels")
         o = torch.as_tensor(obs, dtype=torch.float32).to(self.device).contiguous().view(-1, pol.obs_dim)
         rows = o.shape[0]
-        gauss = pol.head_kind == lib.HEAD_GAUSSIAN
+        gauss = lib.is_gaussian(pol.head_kind)
         w = pol.n_actions if gauss else 1
         act = torch.as_tensor(action, dtype=torch.float32).to(self.device).contiguous().view(rows, w)
         am = None if (action_masks is None or gauss) else torch.as_tensor(action_masks, dtype=torch.float32).to(self.device).contiguous()
@@ -160,7 +160,7 @@ class PPOModule:
         dev = lambda x: None if x is None else torch.as_tensor(x, dtype=torch.float32).to(self.device).contiguous()  # noqa: E731
         obs = dev(obs).view(-1, pol.obs_dim)
         rows = obs.shape[0]
-        act_w = pol.n_actions if pol.head_kind == lib.HEAD_GAUSSIAN else 1
+        act_w = pol.n_actions if lib.is_gaussian(pol.head_kind) else 1
         actions = torch.empty(rows, act_w, dtype=torch.float32, device=self.device)
         logp = torch.empty(rows, act_w, dtype=torch.float32, device=self.device)
         if not getattr(pol, "recurrent", False):
