@@ -420,8 +420,17 @@ typedef struct OrlRnnArgs {
      * ORL_PPO_JOINT_ACTION flag is set, orl_rnn_fwdbwd rejects it (ORL_ERR_BAD_ARG); orl_rnn_rollout (device envs, which
      * report no masks) ignores it. */
     const float* action_masks;
+    /* ORL_HEAD_CATEGORICAL (0, a zeroed struct) or ORL_HEAD_GAUSSIAN: a DiagGaussian policy head of 1..8 dimensions, whose
+     * parameters end in logstd[n] (orl_rnn_param_count_head) and whose actions / action_log_probs are (T, B, n); the
+     * parity-mode exp_noise of orl_rnn_act_rows is then a (B, n) table of N(0, 1) draws.  Taken by orl_rnn_act_rows,
+     * orl_rnn_critic, orl_rnn_fwdbwd and orl_rnn_apply; ORL_ERR_BAD_ARG from orl_rnn_rollout (device envs are Discrete),
+     * with ORL_PPO_JOINT_ACTION, with n_actions > 8 and for any other value. */
+    int32_t head_kind;
+    int32_t reserved3;
 } OrlRnnArgs;
 int orl_rnn_param_count(int obs_dim, int n_out);
+/* parameters of a GRU policy of head_kind: orl_rnn_param_count plus n for the logstd of ORL_HEAD_GAUSSIAN */
+int orl_rnn_param_count_head(int obs_dim, int n_out, int head_kind);
 int orl_rnn_tape_width(void);
 /* floats of OrlRnnArgs.tape for a minibatch of `rows` = n_chunks * chunk_length row-steps (times A with ORL_PPO_JOINT_ACTION)
  * of a policy with at most 8 actions */
@@ -433,6 +442,10 @@ long long orl_rnn_workspace_floats_for(long long rows, int grads_stride, int n_a
  * floats per row, and its W1 gradient takes a panel buffer of 64 x 256 floats after the partials; equal to
  * orl_rnn_workspace_floats_for when both widths are <= 64 */
 long long orl_rnn_workspace_floats_wide_obs(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim);
+/* the same for a policy head of head_kind: an ORL_HEAD_GAUSSIAN policy tapes dL/dlogstd in 8 more floats per row (before
+ * the observation field of a net wider than 64); equal to orl_rnn_workspace_floats_wide_obs for ORL_HEAD_CATEGORICAL */
+long long orl_rnn_workspace_floats_head(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim,
+                                        int head_kind);
 /* policy GRU rollout for steps [t_begin, t_end) fused with the device env (simple_spread, CartPole, GridWorld); device
  * envs only: ORL_ENV_NONE is rejected (the policy step of host-stepped rows is orl_rnn_act_rows).  CartPole and
  * GridWorld need 16-byte aligned policy_obs and critic_obs (ORL_ERR_BAD_ARG otherwise). */
@@ -442,7 +455,9 @@ int orl_rnn_rollout(const OrlRnnArgs* args, void* stream);
  * rnn_states[t+1] (orl_host_insert_rnn zeroes the rows of the envs that finish at step t).  The action noise of row r is
  * keyed by (rng_seed, rng_step_base + *rng_counter, r + rng_row_offset) — the slot index is not added — and rng_counter
  * (nullable) advances by one per call; exp_noise (parity mode, nullable) is the (B, n) Exp(1) table of this slot,
- * indexed by buffer row. */
+ * indexed by buffer row.  With head_kind ORL_HEAD_GAUSSIAN (1..8 dimensions) it writes the (B, n) actions and log-probs
+ * of slot t: mean + std * N(0, 1), the normals drawn as the feed-forward act draws them for the same key (Box-Muller of
+ * Philox lanes 2..5), or read from exp_noise, then a (B, n) table of N(0, 1) draws; deterministic returns the mean. */
 int orl_rnn_act_rows(const OrlRnnArgs* args, void* stream);
 /* orl_host_insert for a recurrent policy: additionally zeroes the 64-float rnn_states_next row of every agent of an env
  * whose agents are all done (rnn_states[dones_env] = 0, onpolicy_driver.py:262-269).  rnn_states_next addresses slot

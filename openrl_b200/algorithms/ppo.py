@@ -94,13 +94,17 @@ class PPOAlgorithm:
         if self.joint_action and self.n > 8:
             raise NotImplementedError("use_joint_action_loss (JRPO) is built for Discrete action spaces of up to 8 actions")
         if self.recurrent:
-            if self.head_kind != lib.HEAD_CATEGORICAL:
+            gaussian_ok = self.head_kind == lib.HEAD_GAUSSIAN and bool(getattr(cfg, "use_recurrent_gaussian_head", False))
+            if self.head_kind != lib.HEAD_CATEGORICAL and not gaussian_ok:
                 raise NotImplementedError("recurrent policies are built for Discrete action spaces")
+            if gaussian_ok and self.joint_action:
+                raise NotImplementedError("use_joint_action_loss (JRPO) is built for Discrete action spaces")
             self.chunk_length = cfg.episode_length if self.naive else cfg.data_chunk_length
             if not 1 <= self.chunk_length <= 32:
                 raise NotImplementedError("the recurrent kernels take chunks of 1..32 steps (data_chunk_length, or episode_length "
                                           "with use_naive_recurrent_policy)")
-            self.rnn_stride = (max(self._lib.orl_rnn_param_count(self.d, self.n), self._lib.orl_rnn_param_count(self.dc, 1)) + 3) & ~3
+            self.rnn_stride = (max(self._lib.orl_rnn_param_count_head(self.d, self.n, self.head_kind),
+                                   self._lib.orl_rnn_param_count(self.dc, 1)) + 3) & ~3
             # one bucket = gradients of both nets + the loss sums: a single all-reduce per update with >1 GPU
             self.rnn_bucket = torch.zeros(2 * self.rnn_stride + 8, dtype=torch.float32, device=dev)
             self.rnn_grads = self.rnn_bucket[:2 * self.rnn_stride].view(2, self.rnn_stride)
@@ -213,6 +217,7 @@ class PPOAlgorithm:
         a.value_preds, a.returns, a.advantages = lib.ptr(buf.value_preds), lib.ptr(buf.returns), lib.ptr(buf.advantages)
         a.gae_stats, a.mb_stats = lib.ptr(buf.gae_stats), lib.ptr(mb_stats)
         a.tape, a.grads, a.grads_stride, a.loss_acc = lib.ptr(self.tape), lib.ptr(self.rnn_grads), self.rnn_stride, lib.ptr(self.loss_acc)
+        a.head_kind = self.head_kind
         return a
 
     def _joint(self, buf):
@@ -251,8 +256,9 @@ class PPOAlgorithm:
         mbc = data_chunks // self.num_mini_batch
         rows = mbc * L
         tape_rows = rows * buf.num_agents if joint else rows   # the joint policy tapes every agent row of a step
-        # tape rows + reduction partials (+ the X field and the dW1 panel buffer with an observation wider than 64)
-        need = int(self._lib.orl_rnn_workspace_floats_wide_obs(tape_rows, self.rnn_stride, self.n, self.d, self.dc))
+        # tape rows + reduction partials (+ the X field and the dW1 panel buffer with an observation wider than 64; + the
+        # dL/dlogstd field of a DiagGaussian head)
+        need = int(self._lib.orl_rnn_workspace_floats_head(tape_rows, self.rnn_stride, self.n, self.d, self.dc, self.head_kind))
         if self.tape is None or self.tape.numel() < need:
             self.tape = torch.empty(need, dtype=torch.float32, device=self.device)
         whole = self.num_mini_batch == 1 and rows == total and not joint

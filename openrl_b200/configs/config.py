@@ -85,6 +85,11 @@ FLAGS = [
     # DiagGaussian head keeps its limit of 8 dimensions (NotImplementedError above); heads of up to 8 dimensions run the
     # same kernels either way, and GRU policies, use_share_model and JRPO keep the limit with the option on
     ("use_wide_gaussian_head", _bool, False),
+    # GRU policies (use_recurrent_policy / use_naive_recurrent_policy) with DiagGaussian heads of 1..8 dimensions on
+    # host-stepped Box-action envs (continuous control under partial observability): the GRU act and chunked update with
+    # the head as ORL_HEAD_GAUSSIAN.  Off, a GRU policy on a Box action space is refused (NotImplementedError above);
+    # Box(9+), JRPO, use_share_model and the device-env GRU rollout refuse it with the option on
+    ("use_recurrent_gaussian_head", _bool, False),
     ("use_tf32", _bool, True),
 ]
 

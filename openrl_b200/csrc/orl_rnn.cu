@@ -141,12 +141,15 @@ __device__ __forceinline__ CatRow warp_categorical_row(const Args& a, rw::V2& x,
 // (orl_host_insert_rnn zeroes the rows of the envs that finish at step t).  Same staged weights, step_forward and
 // sampler as rnn_rollout_warp_kernel: a row's state, logits and action depend neither on R nor on the warp that runs it.
 // NB = 64: the wide head (9..64 actions), sampled by warp_sample_action with the noise keys of the feed-forward wide head.
-// DX = 256: observations of 65..256 features.
-template <int R, int NB, int DX>
+// DX = 256: observations of 65..256 features.  HEAD = ORL_HEAD_GAUSSIAN (NB = 8): the n means out[r][0..n) go to
+// gaussian_act, whose key (seed, step, row + rng_row_offset) is the feed-forward act's; the (B, n) noise table of parity
+// mode is read by buffer row, the (B, n) actions and log-probs are written into slot t.
+template <int R, int NB, int DX, int HEAD>
 __global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnnArgs a) {
+    static_assert(HEAD == ORL_HEAD_CATEGORICAL || NB == MAX_OUT, "a DiagGaussian head has up to 8 dimensions");
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * a.n_agents, d = a.obs_dim, n = a.n_actions, t = a.t_begin;
-    const rc::Offsets o = rc::rnn_offsets(d, n);
+    const rc::Offsets o = rc::rnn_offsets(d, n, HEAD == ORL_HEAD_GAUSSIAN);
     const rw::SmemNet W = rw::load_net<NB, DX>(smem, a.policy_params, o, threadIdx.x, W_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -182,6 +185,15 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnn
                 }, lp, lane);
                 if (g * R + r < rows) {
                     if (lane == 0) { a.actions[grow] = (float)act; a.action_log_probs[grow] = lp; }
+                    rw::stv(a.rnn_states + (grow + B) * rc::H, lane, hn[r]);
+                }
+            } else if constexpr (HEAD == ORL_HEAD_GAUSSIAN) {
+                if (g * R + r < rows) {
+                    const size_t grow = (size_t)t * B + row[r];
+                    if (lane == 0)   // noise row and output slot differ: the table is (B, n), the outputs (T, B, n)
+                        gaussian_act(logit[r], n, a.policy_params + o.ls, a.deterministic != 0,
+                                     a.exp_noise ? a.exp_noise + (size_t)row[r] * n : nullptr, a.rng_seed, step,
+                                     (uint32_t)(row[r] + a.rng_row_offset), 0, a.actions + grow * n, a.action_log_probs + grow * n);
                     rw::stv(a.rnn_states + (grow + B) * rc::H, lane, hn[r]);
                 }
             } else if (g * R + r < rows) {
@@ -235,16 +247,20 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_critic_warp_kernel(const OrlRnnAr
 // critic sees agent 0's row of every step only (to_single_np, ppo.py:222-224, 254-262), buffer row t*B + n*A.
 // NB = 64 (policy only): the wide head; dL/dlogits goes to the tape field TW_DLW of the wider tape rows (TAPE_WIDE).
 // DX = 256: observations of 65..256 features; the rows carry the X field (tape_width_x).
-template <bool POLICY, bool AGENT0, int C_R, int NB, int DX>
+// HEAD = ORL_HEAD_GAUSSIAN (policy, NB = 8): gaussian_row per row step on the row's n actions and old log-probs at bi * n;
+// dL/dmean goes to TP_DLOG (the head is the same linear layer) and dL/dlogstd to the field TW_DLS of TAPE_GAUSS rows.
+template <bool POLICY, bool AGENT0, int C_R, int NB, int DX, int HEAD>
 __global__ void __launch_bounds__(W_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArgs a) {
     static_assert(NB == MAX_OUT || POLICY, "the critic's head is one value");
-    constexpr int TW = (NB == MAX_OUT ? rw::TAPE_W : rw::TAPE_WIDE) + (DX == rc::H ? 0 : rw::MAXD_WIDE);
+    constexpr bool GAUSS = HEAD == ORL_HEAD_GAUSSIAN;
+    static_assert(!GAUSS || (POLICY && NB == MAX_OUT && !AGENT0), "a DiagGaussian policy head has up to 8 dimensions");
+    constexpr int TW = (GAUSS ? rw::TAPE_GAUSS : NB == MAX_OUT ? rw::TAPE_W : rw::TAPE_WIDE) + (DX == rc::H ? 0 : rw::MAXD_WIDE);
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * a.n_agents, T = a.episode_length, L = a.chunk_length;
     const int d = POLICY ? a.obs_dim : a.critic_obs_dim, n = POLICY ? a.n_actions : 1;
     const float* obs = POLICY ? a.policy_obs : a.critic_obs;
     const float* states = POLICY ? a.rnn_states : a.rnn_states_critic;
-    const rc::Offsets o = rc::rnn_offsets(d, n);
+    const rc::Offsets o = rc::rnn_offsets(d, n, GAUSS);
     const rw::SmemNet W = rw::load_net<NB, DX>(smem, POLICY ? a.policy_params : a.critic_params, o, threadIdx.x, W_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -284,7 +300,7 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
                 mk[r] = a.masks[bi[r]];
                 tape[r] = a.tape + ((size_t)cpos[r] * L + l) * TW;
             }
-            rw::step_forward<C_R, NB, DX>(W, scr, d, n, a.activation_id, x, h, mk, h2, out, tape, lane);
+            rw::step_forward<C_R, NB, DX, GAUSS>(W, scr, d, n, a.activation_id, x, h, mk, h2, out, tape, lane);
 #pragma unroll
             for (int r = 0; r < C_R; ++r) {
                 h[r] = h2[r];
@@ -296,6 +312,22 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
                                                           apply_adv_norm(mb.adv, a.advantages[bi[r]]), wrow, lane);
                     loss0 += keep * c.loss * wrow; loss1 += keep * c.ent * wrow; loss2 += keep * c.ratio;
                     rw::stv(tape[r] + rw::TW_DLW, lane, out[r]);
+                } else if constexpr (GAUSS) {
+                    // the entropy is the mean over rows and dimensions (act.py:150-158): active / sum(active) per dimension
+                    // with the active-mask option, else 1 / (rows n)
+                    const float active = a.active_masks[bi[r]];
+                    const float keep = valid[r] ? 1.f : 0.f;
+                    const float wrow = mb.weight(pol_masks, active), went = pol_masks ? active * mb.inv_act : mb.inv_rows / (float)n;
+                    float dl[MAX_OUT], dls[MAX_OUT], l0 = 0.f, l1 = 0.f, l2 = 0.f;
+#pragma unroll
+                    for (int j = 0; j < MAX_OUT; ++j) { dl[j] = 0.f; dls[j] = 0.f; }
+                    gaussian_row(a, out[r], n, a.policy_params + o.ls, a.actions + bi[r] * n, a.action_log_probs + bi[r] * n,
+                                 apply_adv_norm(mb.adv, a.advantages[bi[r]]), wrow, went, dl, dls, l0, l1, l2);
+                    loss0 += keep * l0; loss1 += keep * l1; loss2 += keep * l2;
+                    float mine = 0.f, mine_ls = 0.f;   // lane m < 8 stores dL/dmean[m] and dL/dlogstd[m]
+#pragma unroll
+                    for (int j = 0; j < MAX_OUT; ++j) if (lane == j) { mine = dl[j]; mine_ls = dls[j]; }
+                    if (lane < MAX_OUT) { tape[r][rc::TP_DLOG + lane] = mine; tape[r][rw::TW_DLS + lane] = mine_ls; }
                 } else {
                     float dl[MAX_OUT];
 #pragma unroll
@@ -440,10 +472,10 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_joint_policy_warp_kernel(const Or
 }
 
 // ---- parameter gradients of one net from its tape (orl::reduce_tape); every job fits the gemm tiles: TQ_X + 64 <= TAPE_W ----
-// A wide head (n > 8) reads dL/dlogits from the appended field TW_DLW of its TAPE_WIDE rows.  A wide observation (d > 64)
-// has no W1 job here: its gradient comes from w1_panel_jobs.
-TapeJobs make_jobs(int d, int n) {
-    const rc::Offsets o = rc::rnn_offsets(d, n);
+// A wide head (n > 8) reads dL/dlogits from the appended field TW_DLW of its TAPE_WIDE rows; a DiagGaussian head adds the
+// logstd column sum over TW_DLS.  A wide observation (d > 64) has no W1 job here: its gradient comes from w1_panel_jobs.
+TapeJobs make_jobs(int d, int n, bool gauss) {
+    const rc::Offsets o = rc::rnn_offsets(d, n, gauss);
     TapeJobs t; int g = 0, c = 0;
     auto gemm = [&](int p, int M, int q, int N, int out) { t.gemm[g++] = TapeJob{p, M, q, N, out}; };
     auto col = [&](int p, int M, int out) { t.col[c++] = TapeJob{p, M, -1, 1, out}; };
@@ -457,6 +489,7 @@ TapeJobs make_jobs(int d, int n) {
     col(rc::TS_DONO, rc::H, o.gr);                   col(rc::TS_DO, rc::H, o.ber);
     const int dlog = n > MAX_OUT ? rw::TW_DLW : rc::TP_DLOG;
     gemm(dlog, n, rc::TQ_O, rc::H, o.wh);            col(dlog, n, o.bh);
+    if (gauss) col(rw::TW_DLS, n, o.ls);
     t.n_gemm = g; t.n_col = c;
     return t;
 }
@@ -464,10 +497,10 @@ TapeJobs make_jobs(int d, int n) {
 // dW1 of a wide observation (d > 64) as 64-column panels sum_rows dZ1^T X_p over the X field: panel p lands at
 // W1P_PANEL * p as [64][min(64, d - 64 p)], in a panel buffer of W1P_FLOATS that w1_scatter_kernel unpacks into W1's [64][d]
 constexpr int W1P_PANEL = rc::H * 64, W1P_FLOATS = W1P_PANEL * rw::MAXD_WIDE / 64;
-TapeJobs w1_panel_jobs(int d, int n) {
+TapeJobs w1_panel_jobs(int d, int n, bool gauss) {
     TapeJobs t; t.n_gemm = 0; t.n_col = 0;
     for (int p = 0; 64 * p < d; ++p)
-        t.gemm[t.n_gemm++] = TapeJob{rc::TP_DZ1, rc::H, rw::tape_width(n) + 64 * p, std::min(64, d - 64 * p), W1P_PANEL * p};
+        t.gemm[t.n_gemm++] = TapeJob{rc::TP_DZ1, rc::H, rw::tape_width(n, gauss) + 64 * p, std::min(64, d - 64 * p), W1P_PANEL * p};
     return t;
 }
 __global__ void w1_scatter_kernel(const float* __restrict__ panels, int d, float* __restrict__ w1) {
@@ -478,16 +511,20 @@ __global__ void w1_scatter_kernel(const float* __restrict__ panels, int d, float
 }
 // the update's workspace: the larger of the two nets' tapes, the reduction partials and, with a wide observation, the panel
 // buffer.  JRPO sizes it with rows = its policy tape's A rows per chunk step, the larger tape there.
-long long ws_floats(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim) {
-    const long long tw = std::max(rw::tape_width_x(n_actions, obs_dim), rw::tape_width_x(1, critic_obs_dim));
+long long ws_floats(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim, bool gauss = false) {
+    const long long tw = std::max(rw::tape_width_x(n_actions, obs_dim, gauss), rw::tape_width_x(1, critic_obs_dim));
     const bool wide = obs_dim > rc::MAXD || critic_obs_dim > rc::MAXD;
     return rows * tw + (rows + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK * grads_stride + (wide ? W1P_FLOATS : 0);
 }
 
 // ---- optimizer: per-net global-norm clip + Adam on the true-layout gradients (one CTA per net) ----
+// HEAD = ORL_HEAD_GAUSSIAN: the policy's total includes logstd, so it is in the clip norm and takes its Adam step
+// (clip_grad_norm_ over every policy parameter, ppo.py:120-158)
+template <int HEAD>
 __global__ void __launch_bounds__(1024) rnn_apply_kernel(const OrlRnnArgs a) {
     const int net = blockIdx.x;
-    const int total = net == 0 ? rc::rnn_offsets(a.obs_dim, a.n_actions).total : rc::rnn_offsets(a.critic_obs_dim, 1).total;
+    const int total = net == 0 ? rc::rnn_offsets(a.obs_dim, a.n_actions, HEAD == ORL_HEAD_GAUSSIAN).total
+                               : rc::rnn_offsets(a.critic_obs_dim, 1).total;
     const float* grads = a.grads + (size_t)net * a.grads_stride;
     float sq = 0.f;
     for (int i = threadIdx.x; i < total; i += blockDim.x) sq = fmaf(grads[i], grads[i], sq);
@@ -540,26 +577,29 @@ int check_common(const OrlRnnArgs& a, int max_obs = rc::MAXD) {
     }
     ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= MAX_OUT_WIDE, "n_actions must be in 1..64");
     ORL_CHECK_ARG(a.activation_id >= 0 && a.activation_id <= 3, "activation_id");
+    ORL_CHECK_ARG(a.head_kind == ORL_HEAD_CATEGORICAL || a.head_kind == ORL_HEAD_GAUSSIAN,
+                  "head_kind must be ORL_HEAD_CATEGORICAL or ORL_HEAD_GAUSSIAN");
+    ORL_CHECK_ARG(a.head_kind != ORL_HEAD_GAUSSIAN || a.n_actions <= MAX_OUT, "ORL_HEAD_GAUSSIAN is built for 1..8 dimensions");
     return 0;
 }
 
 // the act over `rows` host-stepped rows: one row per warp while the rows leave warps of the persistent grid idle, else
 // two (every weight read feeds both) where they fit
-template <int NB, int DX>
+template <int NB, int DX, int HEAD = ORL_HEAD_CATEGORICAL>
 int launch_act_rows(const OrlRnnArgs& a, int rows, cudaStream_t st) {
     const bool one = rows <= orl::sm_count() * W_WPC || (may_need_one_row<NB, DX> && wide_rows_per_warp<NB>(a.obs_dim) == 1);
-    return one ? launch(rnn_act_rows_warp_kernel<1, NB, DX>, rows, w_smem<NB, DX>(a.obs_dim, 1), a, st)
-               : launch(rnn_act_rows_warp_kernel<2, NB, DX>, (rows + 1) / 2, w_smem<NB, DX>(a.obs_dim, 2), a, st);
+    return one ? launch(rnn_act_rows_warp_kernel<1, NB, DX, HEAD>, rows, w_smem<NB, DX>(a.obs_dim, 1), a, st)
+               : launch(rnn_act_rows_warp_kernel<2, NB, DX, HEAD>, (rows + 1) / 2, w_smem<NB, DX>(a.obs_dim, 2), a, st);
 }
 
 // the chunk kernel of one net of d features: two chunks per warp (every weight read feeds both) where they fit
-template <bool POLICY, bool AGENT0, int NB, int DX>
+template <bool POLICY, bool AGENT0, int NB, int DX, int HEAD = ORL_HEAD_CATEGORICAL>
 int launch_chunks(const OrlRnnArgs& a, int d, cudaStream_t st) {
     if constexpr (may_need_one_row<NB, DX>) {
         if (wide_rows_per_warp<NB>(d) == 1)
-            return launch(rnn_chunk_warp_kernel<POLICY, AGENT0, 1, NB, DX>, a.n_chunks, w_smem<NB, DX>(d, 1), a, st);
+            return launch(rnn_chunk_warp_kernel<POLICY, AGENT0, 1, NB, DX, HEAD>, a.n_chunks, w_smem<NB, DX>(d, 1), a, st);
     }
-    return launch(rnn_chunk_warp_kernel<POLICY, AGENT0, 2, NB, DX>, (a.n_chunks + 1) / 2, w_smem<NB, DX>(d, 2), a, st);
+    return launch(rnn_chunk_warp_kernel<POLICY, AGENT0, 2, NB, DX, HEAD>, (a.n_chunks + 1) / 2, w_smem<NB, DX>(d, 2), a, st);
 }
 
 // the forward / backward pass of one net over its chunks, writing its tape; JRPO (joint): the joint policy kernel, and the
@@ -573,6 +613,9 @@ int launch_net(const OrlRnnArgs& a, int net, bool joint, cudaStream_t st) {
         return wide_obs ? launch_chunks<false, false, MAX_OUT, XW>(a, d, st) : launch_chunks<false, false, MAX_OUT, rc::H>(a, d, st);
     }
     if (joint) return launch(rnn_joint_policy_warp_kernel<JOINT_A>, a.n_chunks, w_smem<MAX_OUT, rc::H>(d, JOINT_A), a, st);
+    if (a.head_kind == ORL_HEAD_GAUSSIAN)
+        return wide_obs ? launch_chunks<true, false, MAX_OUT, XW, ORL_HEAD_GAUSSIAN>(a, d, st)
+                        : launch_chunks<true, false, MAX_OUT, rc::H, ORL_HEAD_GAUSSIAN>(a, d, st);
     if (wide_obs)
         return wide_head ? launch_chunks<true, false, MAX_OUT_WIDE, XW>(a, d, st) : launch_chunks<true, false, MAX_OUT, XW>(a, d, st);
     return wide_head ? launch_chunks<true, false, MAX_OUT_WIDE, rc::H>(a, d, st) : launch_chunks<true, false, MAX_OUT, rc::H>(a, d, st);
@@ -583,9 +626,15 @@ int launch_net(const OrlRnnArgs& a, int net, bool joint, cudaStream_t st) {
 extern "C" {
 
 int orl_rnn_param_count(int obs_dim, int n_out) { return rc::rnn_offsets(obs_dim, n_out).total; }
+int orl_rnn_param_count_head(int obs_dim, int n_out, int head_kind) {
+    return rc::rnn_offsets(obs_dim, n_out, head_kind == ORL_HEAD_GAUSSIAN).total;
+}
 int orl_rnn_tape_width(void) { return rw::TAPE_W; }
 long long orl_rnn_workspace_floats_wide_obs(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim) {
     return ws_floats(rows, grads_stride, n_actions, obs_dim, critic_obs_dim);
+}
+long long orl_rnn_workspace_floats_head(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim, int head_kind) {
+    return ws_floats(rows, grads_stride, n_actions, obs_dim, critic_obs_dim, head_kind == ORL_HEAD_GAUSSIAN);
 }
 long long orl_rnn_workspace_floats(long long rows, int grads_stride) { return ws_floats(rows, grads_stride, 1, rc::MAXD, rc::MAXD); }
 long long orl_rnn_workspace_floats_for(long long rows, int grads_stride, int n_actions) {
@@ -598,6 +647,7 @@ int orl_rnn_rollout(const OrlRnnArgs* ap, void* stream) {
     if (int e = check_common(a)) return e;
     ORL_CHECK_ARG(a.env_kind != ORL_ENV_NONE, "ORL_ENV_NONE: the act of host-stepped rows is orl_rnn_act_rows");
     ORL_CHECK_ARG(a.n_actions <= MAX_OUT, "n_actions must be in 1..8 for the device envs (they have at most 5 actions)");
+    ORL_CHECK_ARG(a.head_kind == ORL_HEAD_CATEGORICAL, "the device envs are Discrete: orl_rnn_rollout takes ORL_HEAD_CATEGORICAL only");
     ORL_CHECK_ARG(a.policy_params && a.policy_obs && a.rnn_states && a.actions && a.action_log_probs && a.masks, "null rollout buffer");
     ORL_CHECK_ARG(a.t_begin >= 0 && a.t_end <= a.episode_length && a.t_begin <= a.t_end, "t range");
     ORL_CHECK_ARG(a.critic_obs && a.rewards && a.active_masks, "null rollout buffer");
@@ -634,7 +684,10 @@ int orl_rnn_act_rows(const OrlRnnArgs* ap, void* stream) {
     if (rows > 0) {
         constexpr int XW = rw::MAXD_WIDE;
         const bool wide_obs = a.obs_dim > rc::MAXD, wide_head = a.n_actions > MAX_OUT;
-        int e = wide_obs ? (wide_head ? launch_act_rows<MAX_OUT_WIDE, XW>(a, rows, st) : launch_act_rows<MAX_OUT, XW>(a, rows, st))
+        int e = a.head_kind == ORL_HEAD_GAUSSIAN
+                    ? (wide_obs ? launch_act_rows<MAX_OUT, XW, ORL_HEAD_GAUSSIAN>(a, rows, st)
+                                : launch_act_rows<MAX_OUT, rc::H, ORL_HEAD_GAUSSIAN>(a, rows, st))
+              : wide_obs ? (wide_head ? launch_act_rows<MAX_OUT_WIDE, XW>(a, rows, st) : launch_act_rows<MAX_OUT, XW>(a, rows, st))
                          : (wide_head ? launch_act_rows<MAX_OUT_WIDE, rc::H>(a, rows, st) : launch_act_rows<MAX_OUT, rc::H>(a, rows, st));
         if (e) return e;
         if ((e = orl::check_cuda(cudaGetLastError(), "rnn_act_rows_warp_kernel launch"))) return e;
@@ -663,7 +716,8 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
                       a.actions && a.action_log_probs && a.masks && a.active_masks && a.value_preds && a.returns && a.advantages,
                   "null update buffer");
     ORL_CHECK_ARG(a.gae_stats && a.mb_stats && a.tape && a.grads && a.loss_acc, "stats / workspace");
-    ORL_CHECK_ARG(a.grads_stride >= rc::rnn_offsets(a.obs_dim, a.n_actions).total &&
+    const bool gauss = a.head_kind == ORL_HEAD_GAUSSIAN;
+    ORL_CHECK_ARG(a.grads_stride >= rc::rnn_offsets(a.obs_dim, a.n_actions, gauss).total &&
                       a.grads_stride >= rc::rnn_offsets(a.critic_obs_dim, 1).total, "grads_stride");
     if (a.flags & ORL_PPO_VALUENORM) { ORL_CHECK_ARG(a.vn_state, "vn_state"); }
     // ORL_PPO_JOINT_ACTION: v3 chunks; the policy tape holds A rows per chunk step, the critic's one (agent 0)
@@ -673,6 +727,7 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
         ORL_CHECK_ARG(a.n_chunks * a.chunk_length <= (long long)a.n_envs * a.episode_length, "v3 chunks exceed the N*T samples");
         ORL_CHECK_ARG(!a.action_masks, "ORL_PPO_JOINT_ACTION takes no action_masks (simple_spread reports none)");
         ORL_CHECK_ARG(a.n_actions <= MAX_OUT, "ORL_PPO_JOINT_ACTION is built for up to 8 actions");
+        ORL_CHECK_ARG(!gauss, "ORL_PPO_JOINT_ACTION is built for Discrete action spaces (ORL_HEAD_CATEGORICAL)");
         ORL_CHECK_ARG(a.obs_dim <= rc::MAXD && a.critic_obs_dim <= rc::MAXD, "ORL_PPO_JOINT_ACTION is built for obs dims 1..64");
     }
     cudaStream_t st = (cudaStream_t)stream;
@@ -680,18 +735,19 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
     if (e) return e;
     const long long steps = a.n_chunks * a.chunk_length;
     const long long net_rows[2] = {joint ? steps * JOINT_A : steps, steps};
-    const int tw[2] = {rw::tape_width_x(a.n_actions, a.obs_dim), rw::tape_width_x(1, a.critic_obs_dim)};
+    const int tw[2] = {rw::tape_width_x(a.n_actions, a.obs_dim, gauss), rw::tape_width_x(1, a.critic_obs_dim)};
     float* partials = a.tape + std::max(net_rows[0] * tw[0], net_rows[1] * tw[1]);   // after the larger of the two tapes
     float* panels = partials + (std::max(net_rows[0], net_rows[1]) + TAPE_ROW_BLOCK - 1) / TAPE_ROW_BLOCK * a.grads_stride;
     for (int net = 0; net < 2; ++net) {
         const int d = net == 0 ? a.obs_dim : a.critic_obs_dim, n = net == 0 ? a.n_actions : 1;
         if ((e = launch_net(a, net, joint, st))) return e;
-        const rc::Offsets o = rc::rnn_offsets(d, n);
+        const bool g = net == 0 && gauss;
+        const rc::Offsets o = rc::rnn_offsets(d, n, g);
         float* grads = a.grads + (size_t)net * a.grads_stride;
-        if ((e = orl::reduce_tape(a.tape, tw[net], net_rows[net], make_jobs(d, n), partials, a.grads_stride, o.total, grads, st))) return e;
+        if ((e = orl::reduce_tape(a.tape, tw[net], net_rows[net], make_jobs(d, n, g), partials, a.grads_stride, o.total, grads, st))) return e;
         if (d > rc::MAXD) {   // W1's entries of the first reduction are overwritten here
             const int last = (d - 1) / 64, used = W1P_PANEL * last + rc::H * (d - 64 * last);
-            if ((e = orl::reduce_tape(a.tape, tw[net], net_rows[net], w1_panel_jobs(d, n), partials, W1P_FLOATS, used, panels, st))) return e;
+            if ((e = orl::reduce_tape(a.tape, tw[net], net_rows[net], w1_panel_jobs(d, n, g), partials, W1P_FLOATS, used, panels, st))) return e;
             w1_scatter_kernel<<<(rc::H * d + 255) / 256, 256, 0, st>>>(panels, d, grads + o.w1);
         }
     }
@@ -706,7 +762,8 @@ int orl_rnn_apply(const OrlRnnArgs* ap, void* stream) {
                       a.critic_adam_m && a.critic_adam_v && a.adam_steps && a.lrs && a.train_info && a.mb_stats, "null optimizer buffer");
     ORL_CHECK_ARG(a.n_chunks > 0 && a.chunk_length >= 1, "chunks");
     if (a.flags & ORL_PPO_VALUENORM) { ORL_CHECK_ARG(a.vn_state, "vn_state"); }
-    rnn_apply_kernel<<<2, 1024, 0, (cudaStream_t)stream>>>(a);
+    if (a.head_kind == ORL_HEAD_GAUSSIAN) rnn_apply_kernel<ORL_HEAD_GAUSSIAN><<<2, 1024, 0, (cudaStream_t)stream>>>(a);
+    else rnn_apply_kernel<ORL_HEAD_CATEGORICAL><<<2, 1024, 0, (cudaStream_t)stream>>>(a);
     return orl::check_cuda(cudaGetLastError(), "rnn_apply_kernel launch");
 }
 

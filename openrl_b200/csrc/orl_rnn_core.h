@@ -11,6 +11,7 @@
 //   x(d) -> fc1 -> act -> LN1 -> fc3 -> LN3 -> GRU(h*mask) -> LNr -> head(n)
 // Flat parameter layout (state_dict order of the reference, see rnn_offsets):
 //   W1[64][d] b1 g1 be1 | W3[64][64] b3 g3 be3 | Wih[192][64] Whh[192][64] bih[192] bhh[192] | gr ber | Wh[n][64] bh[n]
+// and, for a DiagGaussian head, | logstd[n] (act.action_out.fc_mean.*, then act.action_out.logstd._bias)
 // GRU gate order r, z, n (torch.nn.GRU).  The chunk backward writes a per-row "tape" of local gradients
 // and forward activations; the parameter gradients are tape reductions  dW = sum_rows P^T Q.
 #pragma once
@@ -29,15 +30,16 @@ constexpr float LN_EPS = 1e-5f;
 
 struct Offsets {
     int d, n;
-    int w1, b1, g1, be1, w3, b3, g3, be3, wih, whh, bih, bhh, gr, ber, wh, bh, total;
+    int w1, b1, g1, be1, w3, b3, g3, be3, wih, whh, bih, bhh, gr, ber, wh, bh, ls, total;
 };
-ORL_HD Offsets rnn_offsets(int d, int n) {
+ORL_HD Offsets rnn_offsets(int d, int n, bool gaussian = false) {
     Offsets o; o.d = d; o.n = n; int p = 0;
     o.w1 = p; p += H * d; o.b1 = p; p += H; o.g1 = p; p += H; o.be1 = p; p += H;
     o.w3 = p; p += H * H; o.b3 = p; p += H; o.g3 = p; p += H; o.be3 = p; p += H;
     o.wih = p; p += G3 * H; o.whh = p; p += G3 * H; o.bih = p; p += G3; o.bhh = p; p += G3;
     o.gr = p; p += H; o.ber = p; p += H;
     o.wh = p; p += n * H; o.bh = p; p += n;
+    o.ls = p; if (gaussian) p += n;   // logstd
     o.total = p;
     return o;
 }

@@ -272,6 +272,7 @@ class OnPolicyDriver:
         a.episode_length, a.t_begin, a.t_end = self.episode_length, t_begin, t_end
         a.obs_dim, a.critic_obs_dim, a.n_actions = d.obs_dim, d.critic_obs_dim, d.n_actions
         a.activation_id, a.deterministic = pol.activation_id, 0
+        a.head_kind = pol.head_kind
         a.env_table_len = env.env_table_len
         a.policy_params, a.critic_params = lib.ptr(pol.flat_params), lib.ptr(cri.flat_params)
         a.policy_obs, a.critic_obs = lib.ptr(d.policy_obs), lib.ptr(d.critic_obs)

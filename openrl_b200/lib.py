@@ -72,6 +72,7 @@ def load(path=None):
     lib.orl_rnn_workspace_floats.restype = _c.c_int64
     lib.orl_rnn_workspace_floats_for.restype = _c.c_int64
     lib.orl_rnn_workspace_floats_wide_obs.restype = _c.c_int64
+    lib.orl_rnn_workspace_floats_head.restype = _c.c_int64
     lib.orl_share_workspace_floats.restype = _c.c_int64
     lib.orl_share_workspace_floats_head.restype = _c.c_int64
     lib.orl_ppo_peer_bucket_bytes.restype = _c.c_int64
@@ -217,6 +218,7 @@ class OrlRnnArgs(ctypes.Structure):
         ("norm_rows", _c.c_int64),
         ("rng_row_offset", _c.c_int32), ("row_begin", _c.c_int32), ("row_end", _c.c_int32), ("reserved2", _c.c_int32),
         ("action_masks", _P),
+        ("head_kind", _c.c_int32), ("reserved3", _c.c_int32),
     ]
 
 
@@ -226,10 +228,12 @@ _SIGNATURES.update({
     "orl_host_insert_rnn_wide": [_P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _I, _P, _I, _P],
     "orl_host_insert_rnn_wide_obs": [_P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _I, _P, _I, _P],
     "orl_rnn_param_count": [_I, _I],
+    "orl_rnn_param_count_head": [_I, _I, _I],
     "orl_rnn_tape_width": [],
     "orl_rnn_workspace_floats": [_c.c_int64, _I],
     "orl_rnn_workspace_floats_for": [_c.c_int64, _I, _I],
     "orl_rnn_workspace_floats_wide_obs": [_c.c_int64, _I, _I, _I, _I],
+    "orl_rnn_workspace_floats_head": [_c.c_int64, _I, _I, _I, _I, _I],
     "orl_rnn_rollout": [_c.POINTER(OrlRnnArgs), _P],
     "orl_rnn_critic": [_c.POINTER(OrlRnnArgs), _P],
     "orl_rnn_fwdbwd": [_c.POINTER(OrlRnnArgs), _P],

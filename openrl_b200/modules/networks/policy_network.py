@@ -25,8 +25,13 @@ class PolicyNetwork(nn.Module):
         self.act = ACTLayer(action_space, self.base.output_size, cfg.use_orthogonal, cfg.gain)
         self.head_kind = 1 if self.act.continuous_action else 0          # lib.HEAD_GAUSSIAN / HEAD_CATEGORICAL
         self.n_actions = action_space.shape[0] if self.act.continuous_action else action_space.n  # head width
-        if self.recurrent and self.act.continuous_action:
+        # a GRU policy's DiagGaussian head (cfg.use_recurrent_gaussian_head): the 8-row head block of the GRU kernels
+        recurrent_gaussian = self.recurrent and self.act.continuous_action
+        if recurrent_gaussian and not getattr(cfg, "use_recurrent_gaussian_head", False):
             raise NotImplementedError("recurrent policies are built for Discrete action spaces")
+        if recurrent_gaussian and self.n_actions > 8:
+            raise NotImplementedError("recurrent policies with DiagGaussian heads are built for Box action spaces of width "
+                                      "up to 8 (use_recurrent_gaussian_head)")
         # a feed-forward Categorical head runs up to 64 actions (a logits tile in the kernels); a GRU policy's head runs up
         # to 64 with cfg.use_wide_recurrent_head (a lane-owned 64-vector in the GRU kernels) and up to 8 without; the
         # DiagGaussian heads keep the per-thread head of up to 8 outputs, and run up to 64 with cfg.use_wide_gaussian_head

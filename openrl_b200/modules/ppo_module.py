@@ -147,8 +147,8 @@ class PPOModule:
     def act(self, obs, rnn_states_actor=None, masks=None, action_masks=None, deterministic=False, exp_noise=None,
             rng_seed=None, rng_step=None):
         """PolicyNetwork.forward_original on a (rows, d) batch (ppo_module.py:195-210):
-        returns (actions (rows,1) float CUDA tensor, log-probs (rows,1)) and, for a GRU policy, the new rnn states
-        (rows, 1, H).  action_masks (rows, n) or None.
+        returns (actions (rows,1) float CUDA tensor, log-probs (rows,1); (rows, n) for a DiagGaussian head) and, for a GRU
+        policy, the new rnn states (rows, 1, H).  action_masks (rows, n) or None.
         Stochastic calls draw Philox noise keyed by (cfg.seed, call counter, row): every call sees fresh noise
         (the reference samples from torch's advancing global generator)."""
         pol = self.models["policy"]
@@ -205,6 +205,7 @@ class PPOModule:
         if recurrent:   # reads the noise table by buffer row
             a.critic_obs_dim, a.row_begin, a.row_end = pol.obs_dim, r0, r1
             a.rnn_states, a.masks = lib.ptr(rnn_states), lib.ptr(masks)
+            a.head_kind = pol.head_kind
             lib.check(self._lib.orl_rnn_act_rows(a, s), "orl_rnn_act_rows")
         else:
             a.head_kind = pol.head_kind
