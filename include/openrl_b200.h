@@ -101,7 +101,8 @@ int orl_gae(const float* rewards, float* value_preds, const float* masks,
 /* DiagGaussian head of 1..64 dimensions (Box(n) with n up to 64): the parameter layout, actions and log-probs of
  * ORL_HEAD_GAUSSIAN, run on the 64-wide head tile.  Taken by orl_rollout (ORL_ENV_NONE only), orl_policy_eval,
  * orl_ppo_fwdbwd, orl_ppo_reduce, orl_ppo_apply and their peer variants; ORL_ERR_BAD_ARG on the tensor-core update,
- * the orl_share_* entries, the self-play rollout and every device env.  ORL_HEAD_GAUSSIAN keeps 1..8. */
+ * the orl_share_* entries, the self-play rollout and every device env.  ORL_HEAD_GAUSSIAN keeps 1..8.  The GRU entries
+ * (OrlRnnArgs.head_kind) take it for 9..64 dimensions only. */
 #define ORL_HEAD_GAUSSIAN_WIDE 2
 #define ORL_ENV_NONE 0
 #define ORL_ENV_CARTPOLE 1
@@ -424,12 +425,15 @@ typedef struct OrlRnnArgs {
      * parameters end in logstd[n] (orl_rnn_param_count_head) and whose actions / action_log_probs are (T, B, n); the
      * parity-mode exp_noise of orl_rnn_act_rows is then a (B, n) table of N(0, 1) draws.  Taken by orl_rnn_act_rows,
      * orl_rnn_critic, orl_rnn_fwdbwd and orl_rnn_apply; ORL_ERR_BAD_ARG from orl_rnn_rollout (device envs are Discrete),
-     * with ORL_PPO_JOINT_ACTION, with n_actions > 8 and for any other value. */
+     * with ORL_PPO_JOINT_ACTION, with n_actions > 8 and for any other value.  ORL_HEAD_GAUSSIAN_WIDE: the same for a
+     * DiagGaussian policy head of 9..64 dimensions (ORL_ERR_BAD_ARG with n_actions <= 8), on the 64-wide head of the GRU
+     * kernels. */
     int32_t head_kind;
     int32_t reserved3;
 } OrlRnnArgs;
 int orl_rnn_param_count(int obs_dim, int n_out);
-/* parameters of a GRU policy of head_kind: orl_rnn_param_count plus n for the logstd of ORL_HEAD_GAUSSIAN */
+/* parameters of a GRU policy of head_kind: orl_rnn_param_count plus n for the logstd of ORL_HEAD_GAUSSIAN and
+ * ORL_HEAD_GAUSSIAN_WIDE */
 int orl_rnn_param_count_head(int obs_dim, int n_out, int head_kind);
 int orl_rnn_tape_width(void);
 /* floats of OrlRnnArgs.tape for a minibatch of `rows` = n_chunks * chunk_length row-steps (times A with ORL_PPO_JOINT_ACTION)
@@ -443,7 +447,9 @@ long long orl_rnn_workspace_floats_for(long long rows, int grads_stride, int n_a
  * orl_rnn_workspace_floats_for when both widths are <= 64 */
 long long orl_rnn_workspace_floats_wide_obs(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim);
 /* the same for a policy head of head_kind: an ORL_HEAD_GAUSSIAN policy tapes dL/dlogstd in 8 more floats per row (before
- * the observation field of a net wider than 64); equal to orl_rnn_workspace_floats_wide_obs for ORL_HEAD_CATEGORICAL */
+ * the observation field of a net wider than 64), an ORL_HEAD_GAUSSIAN_WIDE policy (9..64 dimensions) in 64 more floats
+ * after the wide head's dL/dmean (rows of 1872, or 2128 with the observation field); equal to
+ * orl_rnn_workspace_floats_wide_obs for ORL_HEAD_CATEGORICAL */
 long long orl_rnn_workspace_floats_head(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim,
                                         int head_kind);
 /* policy GRU rollout for steps [t_begin, t_end) fused with the device env (simple_spread, CartPole, GridWorld); device
@@ -457,7 +463,9 @@ int orl_rnn_rollout(const OrlRnnArgs* args, void* stream);
  * (nullable) advances by one per call; exp_noise (parity mode, nullable) is the (B, n) Exp(1) table of this slot,
  * indexed by buffer row.  With head_kind ORL_HEAD_GAUSSIAN (1..8 dimensions) it writes the (B, n) actions and log-probs
  * of slot t: mean + std * N(0, 1), the normals drawn as the feed-forward act draws them for the same key (Box-Muller of
- * Philox lanes 2..5), or read from exp_noise, then a (B, n) table of N(0, 1) draws; deterministic returns the mean. */
+ * Philox lanes 2..5), or read from exp_noise, then a (B, n) table of N(0, 1) draws; deterministic returns the mean.
+ * ORL_HEAD_GAUSSIAN_WIDE (9..64 dimensions) does the same with the feed-forward wide head's noise: dimensions
+ * [4k, 4k + 4) are Box-Muller of Philox lanes 2 + 2k and 3 + 2k, so dimensions 0..7 draw what ORL_HEAD_GAUSSIAN draws. */
 int orl_rnn_act_rows(const OrlRnnArgs* args, void* stream);
 /* orl_host_insert for a recurrent policy: additionally zeroes the 64-float rnn_states_next row of every agent of an env
  * whose agents are all done (rnn_states[dones_env] = 0, onpolicy_driver.py:262-269).  rnn_states_next addresses slot

@@ -94,7 +94,9 @@ class PPOAlgorithm:
         if self.joint_action and self.n > 8:
             raise NotImplementedError("use_joint_action_loss (JRPO) is built for Discrete action spaces of up to 8 actions")
         if self.recurrent:
-            gaussian_ok = self.head_kind == lib.HEAD_GAUSSIAN and bool(getattr(cfg, "use_recurrent_gaussian_head", False))
+            gaussian_ok = bool(getattr(cfg, "use_recurrent_gaussian_head", False)) and (
+                self.head_kind == lib.HEAD_GAUSSIAN
+                or (self.head_kind == lib.HEAD_GAUSSIAN_WIDE and bool(getattr(cfg, "use_wide_recurrent_gaussian_head", False))))
             if self.head_kind != lib.HEAD_CATEGORICAL and not gaussian_ok:
                 raise NotImplementedError("recurrent policies are built for Discrete action spaces")
             if gaussian_ok and self.joint_action:

@@ -90,6 +90,12 @@ FLAGS = [
     # the head as ORL_HEAD_GAUSSIAN.  Off, a GRU policy on a Box action space is refused (NotImplementedError above);
     # Box(9+), JRPO, use_share_model and the device-env GRU rollout refuse it with the option on
     ("use_recurrent_gaussian_head", _bool, False),
+    # with use_recurrent_gaussian_head: GRU policies with DiagGaussian heads of 9..64 dimensions (Box action spaces such
+    # as dm_control's humanoid, 21 actions, or quadruped, 12): the 64-wide head of the GRU act and update kernels
+    # (ORL_HEAD_GAUSSIAN_WIDE).  Off, a GRU policy's DiagGaussian head keeps its limit of 8 dimensions (NotImplementedError
+    # above); heads of up to 8 dimensions run the same kernels either way, and JRPO, use_share_model and the device-env
+    # GRU rollout refuse it with the option on
+    ("use_wide_recurrent_gaussian_head", _bool, False),
     ("use_tf32", _bool, True),
 ]
 

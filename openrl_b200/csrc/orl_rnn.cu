@@ -135,6 +135,33 @@ __device__ __forceinline__ CatRow warp_categorical_row(const Args& a, rw::V2& x,
     x.b = sm.live_b ? dlp * ((lane + 32 == act ? 1.f : 0.f) - pb) + went * pb * (nlb + ent) : 0.f;
     return CatRow{pg.loss, ent, pg.ratio};
 }
+// gaussian_row of a wide row (9..64 dimensions) on the lane-owned means x (lane l: dimensions l and l + 32): the same
+// per-dimension terms, each lane on its two dimensions.  Overwrites x with dL/dmean and writes dL/dlogstd to dls (0 for
+// j >= n).  The row's weighted loss, weighted entropy and ratio / n are warp sums (one xor tree: the same order on every
+// run), returned on every lane.
+template <class Args>
+__device__ __forceinline__ void warp_gaussian_row(const Args& a, rw::V2& x, int n, const float* logstd, const float* act,
+                                                  const float* old_lp, float adv, float wrow, float went, rw::V2& dls,
+                                                  float& loss, float& ent, float& ratio, int lane) {
+    float l0 = 0.f, l1 = 0.f, l2 = 0.f;
+    auto dim = [&](int j, float& m, float& ds) {
+        if (j < n) {
+            const float ls = logstd[j], std = expf(ls), var = std * std, diff = act[j] - m;
+            const PgTerm pg = pg_term(gaussian_log_prob(diff, std, ls), old_lp[j], adv, a.clip_param, a.flags, a.dual_clip_coeff);
+            l0 += pg.loss * wrow;
+            l1 += gaussian_entropy(ls) * went;
+            l2 += pg.ratio / (float)n;
+            const float dlp = pg.dlogp * wrow;
+            m = dlp * diff / var;
+            ds = dlp * (diff * diff / var - 1.0f) - a.entropy_coef * went;
+        } else {
+            m = 0.f; ds = 0.f;
+        }
+    };
+    dim(lane, x.a, dls.a);
+    dim(lane + 32, x.b, dls.b);
+    loss = warp_sum(l0); ent = warp_sum(l1); ratio = warp_sum(l2);
+}
 
 // ---- act over host-stepped rows: rows [row_begin, row_end) of slot t = t_begin, R rows per warp ----
 // The host steps the env between two launches; this kernel writes actions[t], action_log_probs[t] and rnn_states[t+1]
@@ -143,13 +170,16 @@ __device__ __forceinline__ CatRow warp_categorical_row(const Args& a, rw::V2& x,
 // NB = 64: the wide head (9..64 actions), sampled by warp_sample_action with the noise keys of the feed-forward wide head.
 // DX = 256: observations of 65..256 features.  HEAD = ORL_HEAD_GAUSSIAN (NB = 8): the n means out[r][0..n) go to
 // gaussian_act, whose key (seed, step, row + rng_row_offset) is the feed-forward act's; the (B, n) noise table of parity
-// mode is read by buffer row, the (B, n) actions and log-probs are written into slot t.
+// mode is read by buffer row, the (B, n) actions and log-probs are written into slot t.  HEAD = ORL_HEAD_GAUSSIAN_WIDE
+// (NB = 64, 9..64 dimensions): the lane-owned means are parked in the row's scratch and lanes 0..15 each run
+// gaussian_act4 on dimensions [4 lane, 4 lane + 4), with the same key, table and slot as the 8-wide head.
 template <int R, int NB, int DX, int HEAD>
 __global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnnArgs a) {
-    static_assert(HEAD == ORL_HEAD_CATEGORICAL || NB == MAX_OUT, "a DiagGaussian head has up to 8 dimensions");
+    static_assert(HEAD == ORL_HEAD_CATEGORICAL || (HEAD == ORL_HEAD_GAUSSIAN && NB == MAX_OUT) ||
+                      (HEAD == ORL_HEAD_GAUSSIAN_WIDE && NB == MAX_OUT_WIDE), "the DiagGaussian heads' widths");
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * a.n_agents, d = a.obs_dim, n = a.n_actions, t = a.t_begin;
-    const rc::Offsets o = rc::rnn_offsets(d, n, HEAD == ORL_HEAD_GAUSSIAN);
+    const rc::Offsets o = rc::rnn_offsets(d, n, HEAD != ORL_HEAD_CATEGORICAL);
     const rw::SmemNet W = rw::load_net<NB, DX>(smem, a.policy_params, o, threadIdx.x, W_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -174,9 +204,19 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_act_rows_warp_kernel(const OrlRnn
             mk[r] = a.masks[grow];
         }
         rw::step_forward<R, NB, DX>(W, scr, d, n, a.activation_id, x, h, mk, hn, logit, no_tape, lane);
+        if constexpr (HEAD == ORL_HEAD_GAUSSIAN_WIDE) rw::park<R>(scr, 0, logit, lane);
 #pragma unroll
         for (int r = 0; r < R; ++r) {
-            if constexpr (NB == MAX_OUT_WIDE) {
+            if constexpr (HEAD == ORL_HEAD_GAUSSIAN_WIDE) {
+                if (g * R + r < rows) {
+                    const size_t grow = (size_t)t * B + row[r];
+                    if (4 * lane < n)   // noise row and output slot differ: the table is (B, n), the outputs (T, B, n)
+                        gaussian_act4(scr + r * rw::SCR, n, 4 * lane, a.policy_params + o.ls, a.deterministic != 0,
+                                      a.exp_noise ? a.exp_noise + (size_t)row[r] * n : nullptr, a.rng_seed, step,
+                                      (uint32_t)(row[r] + a.rng_row_offset), 0, a.actions + grow * n, a.action_log_probs + grow * n);
+                    rw::stv(a.rnn_states + (grow + B) * rc::H, lane, hn[r]);
+                }
+            } else if constexpr (NB == MAX_OUT_WIDE) {
                 const size_t grow = (size_t)t * B + row[r];
                 float lp;
                 const int act = warp_sample_action(logit[r], n, a.action_masks ? a.action_masks + grow * n : nullptr, a.deterministic != 0,
@@ -249,18 +289,21 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_critic_warp_kernel(const OrlRnnAr
 // DX = 256: observations of 65..256 features; the rows carry the X field (tape_width_x).
 // HEAD = ORL_HEAD_GAUSSIAN (policy, NB = 8): gaussian_row per row step on the row's n actions and old log-probs at bi * n;
 // dL/dmean goes to TP_DLOG (the head is the same linear layer) and dL/dlogstd to the field TW_DLS of TAPE_GAUSS rows.
+// HEAD = ORL_HEAD_GAUSSIAN_WIDE (policy, NB = 64): warp_gaussian_row on the lane-owned means; dL/dmean goes to TW_DLW (the
+// wide head's field, zero for j >= n) and dL/dlogstd to TW_DLSW of TAPE_GAUSS_WIDE rows.
 template <bool POLICY, bool AGENT0, int C_R, int NB, int DX, int HEAD>
 __global__ void __launch_bounds__(W_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArgs a) {
     static_assert(NB == MAX_OUT || POLICY, "the critic's head is one value");
-    constexpr bool GAUSS = HEAD == ORL_HEAD_GAUSSIAN;
+    constexpr bool GAUSS = HEAD == ORL_HEAD_GAUSSIAN, GAUSS_W = HEAD == ORL_HEAD_GAUSSIAN_WIDE;
     static_assert(!GAUSS || (POLICY && NB == MAX_OUT && !AGENT0), "a DiagGaussian policy head has up to 8 dimensions");
-    constexpr int TW = (GAUSS ? rw::TAPE_GAUSS : NB == MAX_OUT ? rw::TAPE_W : rw::TAPE_WIDE) + (DX == rc::H ? 0 : rw::MAXD_WIDE);
+    static_assert(!GAUSS_W || (POLICY && NB == MAX_OUT_WIDE && !AGENT0), "a wide DiagGaussian policy head has 9..64 dimensions");
+    constexpr int TW = rw::tape_width(NB, GAUSS || GAUSS_W) + (DX == rc::H ? 0 : rw::MAXD_WIDE);
     extern __shared__ __align__(16) float smem[];
     const int B = a.n_envs * a.n_agents, T = a.episode_length, L = a.chunk_length;
     const int d = POLICY ? a.obs_dim : a.critic_obs_dim, n = POLICY ? a.n_actions : 1;
     const float* obs = POLICY ? a.policy_obs : a.critic_obs;
     const float* states = POLICY ? a.rnn_states : a.rnn_states_critic;
-    const rc::Offsets o = rc::rnn_offsets(d, n, GAUSS);
+    const rc::Offsets o = rc::rnn_offsets(d, n, GAUSS || GAUSS_W);
     const rw::SmemNet W = rw::load_net<NB, DX>(smem, POLICY ? a.policy_params : a.critic_params, o, threadIdx.x, W_NT);
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -300,11 +343,23 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_chunk_warp_kernel(const OrlRnnArg
                 mk[r] = a.masks[bi[r]];
                 tape[r] = a.tape + ((size_t)cpos[r] * L + l) * TW;
             }
-            rw::step_forward<C_R, NB, DX, GAUSS>(W, scr, d, n, a.activation_id, x, h, mk, h2, out, tape, lane);
+            rw::step_forward<C_R, NB, DX, GAUSS || GAUSS_W>(W, scr, d, n, a.activation_id, x, h, mk, h2, out, tape, lane);
 #pragma unroll
             for (int r = 0; r < C_R; ++r) {
                 h[r] = h2[r];
-                if constexpr (NB == MAX_OUT_WIDE) {
+                if constexpr (GAUSS_W) {
+                    // the entropy weight of the 8-wide head: active / sum(active) per dimension, else 1 / (rows n)
+                    const float active = a.active_masks[bi[r]];
+                    const float keep = valid[r] ? 1.f : 0.f;
+                    const float wrow = mb.weight(pol_masks, active), went = pol_masks ? active * mb.inv_act : mb.inv_rows / (float)n;
+                    rw::V2 dls;
+                    float l0, l1, l2;
+                    warp_gaussian_row(a, out[r], n, a.policy_params + o.ls, a.actions + bi[r] * n, a.action_log_probs + bi[r] * n,
+                                      apply_adv_norm(mb.adv, a.advantages[bi[r]]), wrow, went, dls, l0, l1, l2, lane);
+                    loss0 += keep * l0; loss1 += keep * l1; loss2 += keep * l2;
+                    rw::stv(tape[r] + rw::TW_DLW, lane, out[r]);
+                    rw::stv(tape[r] + rw::TW_DLSW, lane, dls);
+                } else if constexpr (NB == MAX_OUT_WIDE) {
                     const float keep = valid[r] ? 1.f : 0.f;
                     const float wrow = mb.weight(pol_masks, a.active_masks[bi[r]]);
                     const CatRow c = warp_categorical_row(a, out[r], n, a.action_masks ? a.action_masks + bi[r] * n : nullptr,
@@ -473,7 +528,8 @@ __global__ void __launch_bounds__(W_NT, 1) rnn_joint_policy_warp_kernel(const Or
 
 // ---- parameter gradients of one net from its tape (orl::reduce_tape); every job fits the gemm tiles: TQ_X + 64 <= TAPE_W ----
 // A wide head (n > 8) reads dL/dlogits from the appended field TW_DLW of its TAPE_WIDE rows; a DiagGaussian head adds the
-// logstd column sum over TW_DLS.  A wide observation (d > 64) has no W1 job here: its gradient comes from w1_panel_jobs.
+// logstd column sum over TW_DLS (TW_DLSW for n > 8).  A wide observation (d > 64) has no W1 job here: its gradient comes
+// from w1_panel_jobs.
 TapeJobs make_jobs(int d, int n, bool gauss) {
     const rc::Offsets o = rc::rnn_offsets(d, n, gauss);
     TapeJobs t; int g = 0, c = 0;
@@ -489,7 +545,7 @@ TapeJobs make_jobs(int d, int n, bool gauss) {
     col(rc::TS_DONO, rc::H, o.gr);                   col(rc::TS_DO, rc::H, o.ber);
     const int dlog = n > MAX_OUT ? rw::TW_DLW : rc::TP_DLOG;
     gemm(dlog, n, rc::TQ_O, rc::H, o.wh);            col(dlog, n, o.bh);
-    if (gauss) col(rw::TW_DLS, n, o.ls);
+    if (gauss) col(n > MAX_OUT ? rw::TW_DLSW : rw::TW_DLS, n, o.ls);
     t.n_gemm = g; t.n_col = c;
     return t;
 }
@@ -577,9 +633,11 @@ int check_common(const OrlRnnArgs& a, int max_obs = rc::MAXD) {
     }
     ORL_CHECK_ARG(a.n_actions > 0 && a.n_actions <= MAX_OUT_WIDE, "n_actions must be in 1..64");
     ORL_CHECK_ARG(a.activation_id >= 0 && a.activation_id <= 3, "activation_id");
-    ORL_CHECK_ARG(a.head_kind == ORL_HEAD_CATEGORICAL || a.head_kind == ORL_HEAD_GAUSSIAN,
-                  "head_kind must be ORL_HEAD_CATEGORICAL or ORL_HEAD_GAUSSIAN");
+    ORL_CHECK_ARG(a.head_kind == ORL_HEAD_CATEGORICAL || a.head_kind == ORL_HEAD_GAUSSIAN || a.head_kind == ORL_HEAD_GAUSSIAN_WIDE,
+                  "head_kind must be ORL_HEAD_CATEGORICAL, ORL_HEAD_GAUSSIAN or ORL_HEAD_GAUSSIAN_WIDE");
     ORL_CHECK_ARG(a.head_kind != ORL_HEAD_GAUSSIAN || a.n_actions <= MAX_OUT, "ORL_HEAD_GAUSSIAN is built for 1..8 dimensions");
+    ORL_CHECK_ARG(a.head_kind != ORL_HEAD_GAUSSIAN_WIDE || a.n_actions > MAX_OUT,
+                  "head_kind ORL_HEAD_GAUSSIAN_WIDE is built for 9..64 dimensions (ORL_HEAD_GAUSSIAN for 1..8)");
     return 0;
 }
 
@@ -616,6 +674,9 @@ int launch_net(const OrlRnnArgs& a, int net, bool joint, cudaStream_t st) {
     if (a.head_kind == ORL_HEAD_GAUSSIAN)
         return wide_obs ? launch_chunks<true, false, MAX_OUT, XW, ORL_HEAD_GAUSSIAN>(a, d, st)
                         : launch_chunks<true, false, MAX_OUT, rc::H, ORL_HEAD_GAUSSIAN>(a, d, st);
+    if (a.head_kind == ORL_HEAD_GAUSSIAN_WIDE)
+        return wide_obs ? launch_chunks<true, false, MAX_OUT_WIDE, XW, ORL_HEAD_GAUSSIAN_WIDE>(a, d, st)
+                        : launch_chunks<true, false, MAX_OUT_WIDE, rc::H, ORL_HEAD_GAUSSIAN_WIDE>(a, d, st);
     if (wide_obs)
         return wide_head ? launch_chunks<true, false, MAX_OUT_WIDE, XW>(a, d, st) : launch_chunks<true, false, MAX_OUT, XW>(a, d, st);
     return wide_head ? launch_chunks<true, false, MAX_OUT_WIDE, rc::H>(a, d, st) : launch_chunks<true, false, MAX_OUT, rc::H>(a, d, st);
@@ -627,14 +688,15 @@ extern "C" {
 
 int orl_rnn_param_count(int obs_dim, int n_out) { return rc::rnn_offsets(obs_dim, n_out).total; }
 int orl_rnn_param_count_head(int obs_dim, int n_out, int head_kind) {
-    return rc::rnn_offsets(obs_dim, n_out, head_kind == ORL_HEAD_GAUSSIAN).total;
+    return rc::rnn_offsets(obs_dim, n_out, head_kind == ORL_HEAD_GAUSSIAN || head_kind == ORL_HEAD_GAUSSIAN_WIDE).total;
 }
 int orl_rnn_tape_width(void) { return rw::TAPE_W; }
 long long orl_rnn_workspace_floats_wide_obs(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim) {
     return ws_floats(rows, grads_stride, n_actions, obs_dim, critic_obs_dim);
 }
 long long orl_rnn_workspace_floats_head(long long rows, int grads_stride, int n_actions, int obs_dim, int critic_obs_dim, int head_kind) {
-    return ws_floats(rows, grads_stride, n_actions, obs_dim, critic_obs_dim, head_kind == ORL_HEAD_GAUSSIAN);
+    return ws_floats(rows, grads_stride, n_actions, obs_dim, critic_obs_dim,
+                     head_kind == ORL_HEAD_GAUSSIAN || head_kind == ORL_HEAD_GAUSSIAN_WIDE);
 }
 long long orl_rnn_workspace_floats(long long rows, int grads_stride) { return ws_floats(rows, grads_stride, 1, rc::MAXD, rc::MAXD); }
 long long orl_rnn_workspace_floats_for(long long rows, int grads_stride, int n_actions) {
@@ -687,6 +749,9 @@ int orl_rnn_act_rows(const OrlRnnArgs* ap, void* stream) {
         int e = a.head_kind == ORL_HEAD_GAUSSIAN
                     ? (wide_obs ? launch_act_rows<MAX_OUT, XW, ORL_HEAD_GAUSSIAN>(a, rows, st)
                                 : launch_act_rows<MAX_OUT, rc::H, ORL_HEAD_GAUSSIAN>(a, rows, st))
+              : a.head_kind == ORL_HEAD_GAUSSIAN_WIDE
+                    ? (wide_obs ? launch_act_rows<MAX_OUT_WIDE, XW, ORL_HEAD_GAUSSIAN_WIDE>(a, rows, st)
+                                : launch_act_rows<MAX_OUT_WIDE, rc::H, ORL_HEAD_GAUSSIAN_WIDE>(a, rows, st))
               : wide_obs ? (wide_head ? launch_act_rows<MAX_OUT_WIDE, XW>(a, rows, st) : launch_act_rows<MAX_OUT, XW>(a, rows, st))
                          : (wide_head ? launch_act_rows<MAX_OUT_WIDE, rc::H>(a, rows, st) : launch_act_rows<MAX_OUT, rc::H>(a, rows, st));
         if (e) return e;
@@ -716,7 +781,7 @@ int orl_rnn_fwdbwd(const OrlRnnArgs* ap, void* stream) {
                       a.actions && a.action_log_probs && a.masks && a.active_masks && a.value_preds && a.returns && a.advantages,
                   "null update buffer");
     ORL_CHECK_ARG(a.gae_stats && a.mb_stats && a.tape && a.grads && a.loss_acc, "stats / workspace");
-    const bool gauss = a.head_kind == ORL_HEAD_GAUSSIAN;
+    const bool gauss = a.head_kind == ORL_HEAD_GAUSSIAN || a.head_kind == ORL_HEAD_GAUSSIAN_WIDE;
     ORL_CHECK_ARG(a.grads_stride >= rc::rnn_offsets(a.obs_dim, a.n_actions, gauss).total &&
                       a.grads_stride >= rc::rnn_offsets(a.critic_obs_dim, 1).total, "grads_stride");
     if (a.flags & ORL_PPO_VALUENORM) { ORL_CHECK_ARG(a.vn_state, "vn_state"); }
@@ -762,7 +827,9 @@ int orl_rnn_apply(const OrlRnnArgs* ap, void* stream) {
                       a.critic_adam_m && a.critic_adam_v && a.adam_steps && a.lrs && a.train_info && a.mb_stats, "null optimizer buffer");
     ORL_CHECK_ARG(a.n_chunks > 0 && a.chunk_length >= 1, "chunks");
     if (a.flags & ORL_PPO_VALUENORM) { ORL_CHECK_ARG(a.vn_state, "vn_state"); }
-    if (a.head_kind == ORL_HEAD_GAUSSIAN) rnn_apply_kernel<ORL_HEAD_GAUSSIAN><<<2, 1024, 0, (cudaStream_t)stream>>>(a);
+    // the wide DiagGaussian head has the 8-wide one's layout (logstd after the head): it runs as that
+    if (a.head_kind == ORL_HEAD_GAUSSIAN || a.head_kind == ORL_HEAD_GAUSSIAN_WIDE)
+        rnn_apply_kernel<ORL_HEAD_GAUSSIAN><<<2, 1024, 0, (cudaStream_t)stream>>>(a);
     else rnn_apply_kernel<ORL_HEAD_CATEGORICAL><<<2, 1024, 0, (cudaStream_t)stream>>>(a);
     return orl::check_cuda(cudaGetLastError(), "rnn_apply_kernel launch");
 }

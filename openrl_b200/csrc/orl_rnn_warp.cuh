@@ -15,7 +15,9 @@
 // reductions), then the forward activations the backward step re-reads: A1 N1 N3 R Z NN GHN NO (64 each)
 // and 8 scalars (rstd1, rstd3, rstd_rnn, mask, -).  A wide policy head (9..64 actions, NB = 64) appends dL/dlogits as
 // a 64-vector at [TAPE_W, TAPE_WIDE); the 8-wide TP_DLOG field is left unused there.  A DiagGaussian policy head (1..8
-// dimensions, NB = 8) keeps dL/dmean in TP_DLOG and appends the row's dL/dlogstd at [TAPE_W, TAPE_GAUSS).
+// dimensions, NB = 8) keeps dL/dmean in TP_DLOG and appends the row's dL/dlogstd at [TAPE_W, TAPE_GAUSS).  A wide
+// DiagGaussian policy head (9..64 dimensions, NB = 64) keeps dL/dmean in the wide head's TW_DLW field and appends
+// dL/dlogstd as a 64-vector at [TAPE_WIDE, TAPE_GAUSS_WIDE).
 //
 // Head width bound NB (a template parameter): NB = 8 (MAXN) stages an 8-row head block and reduces each logit with a
 // warp_sum into out[R][8] on every lane.  NB = 64 (MAXN_WIDE) treats the logits as one more lane-owned 64-vector
@@ -40,9 +42,12 @@ constexpr int TW_A1 = rc::TAPE, TW_N1 = TW_A1 + 64, TW_N3 = TW_N1 + 64, TW_R = T
               TW_GHN = TW_NN + 64, TW_NO = TW_GHN + 64, TW_SC = TW_NO + 64, TAPE_W = TW_SC + 8;   // 1744
 constexpr int TW_DLW = TAPE_W, TAPE_WIDE = TW_DLW + 64;   // 1808: the wide policy head's dL/dlogits (P operand of Wh, bh)
 constexpr int TW_DLS = TAPE_W, TAPE_GAUSS = TW_DLS + 8;   // 1752: a DiagGaussian policy head's dL/dlogstd (column sums)
+constexpr int TW_DLSW = TAPE_WIDE, TAPE_GAUSS_WIDE = TW_DLSW + 64;   // 1872: the wide DiagGaussian head's dL/dlogstd
 __host__ __device__ constexpr int head_bound(int n) { return n > MAXN ? MAXN_WIDE : MAXN; }
 // the row width before the X field: it depends on the head kind as well as on n
-__host__ __device__ constexpr int tape_width(int n, bool gauss = false) { return gauss ? TAPE_GAUSS : n > MAXN ? TAPE_WIDE : TAPE_W; }
+__host__ __device__ constexpr int tape_width(int n, bool gauss = false) {
+    return gauss ? (n > MAXN ? TAPE_GAUSS_WIDE : TAPE_GAUSS) : n > MAXN ? TAPE_WIDE : TAPE_W;
+}
 constexpr int MAXD_WIDE = 256;
 __host__ __device__ constexpr int w1_ld(int d) { return ((d + 3) & ~3) + 1; }
 // a wide-observation row (d > 64): the X field [tape_width(n, gauss), tape_width(n, gauss) + MAXD_WIDE) follows the row
@@ -267,20 +272,19 @@ __device__ __forceinline__ void stage_x(float* scr, const float* const (&x)[R], 
 // One forward step of R rows.  x: observation (XIn; zero beyond d), h_in: hidden state, out[r]: the head outputs (HeadOut).
 // tape[r] != nullptr: the Q operands and the activations for the backward step go to the row's tape.
 // scr: this warp's scratch (R * SCR floats of shared memory).  W: staged by load_net<NB, DX>.  GAUSS: a DiagGaussian
-// policy head (NB = 8), whose rows put the X field after TW_DLS.
+// policy head (NB = 8, or NB = 64 for 9..64 dimensions), whose rows put the X field after its dL/dlogstd field.
 template <int R, int NB = MAXN, int DX = H, bool GAUSS = false>
 __device__ __forceinline__ void step_forward(const SmemNet& W, float* scr, int d, int n, int act_id, const typename XIn<DX>::type (&x)[R],
                                              const V2 (&h_in)[R], const float (&mask)[R], V2 (&h_out)[R],
                                              typename HeadOut<NB>::type (&out)[R], float* const (&tape)[R], int lane) {
     static_assert(DX == H || DX == MAXD_WIDE, "observation width bound");
-    static_assert(!GAUSS || NB == MAXN, "a DiagGaussian head has up to 8 dimensions");
     const V2 g1 = ldv(W.g1, lane), be1 = ldv(W.be1, lane), g3 = ldv(W.g3, lane), be3 = ldv(W.be3, lane);
     V2 t0[R], y1[R], y3[R], hm[R];
     if constexpr (DX == H) {
         park<R>(scr, 0, x, lane);
         matvec64<R>(W.w1, W.b1, scr, 0, d, lane, t0);
     } else {
-        stage_x<R>(scr, x, d, tape, GAUSS ? TAPE_GAUSS : NB == MAXN ? TAPE_W : TAPE_WIDE, lane);
+        stage_x<R>(scr, x, d, tape, tape_width(NB, GAUSS), lane);
         matvec64<R>(W.w1, W.b1, scr, 0, d, lane, t0, w1_ld(d));
     }
 #pragma unroll

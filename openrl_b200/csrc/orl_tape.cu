@@ -4,8 +4,8 @@
 //   gemm job   part[out_off + m*N + k] = sum_rows tape[r][p_off+m] * tape[r][q_off+k]     (register-tiled, 12x4 per thread)
 //   column job part[out_off + m]       = sum_rows tape[r][p_off+m]
 // Stage 2: grads[i] = sum over row blocks of partials[rb][i], pairwise in a fixed order.
-// The kernels are built per tape width (the GRU's, the wide-head GRU policy's and the DiagGaussian GRU policy's, each with
-// or without the X field of a wide observation, and the shared model's): with the width a runtime value the gemm
+// The kernels are built per tape width (the GRU's, the wide-head GRU policy's and the two DiagGaussian GRU policies', each
+// with or without the X field of a wide observation, and the shared model's): with the width a runtime value the gemm
 // kernel's row addressing takes 92 registers instead of 80 on sm_90a, one CTA less per SM.
 #include "orl_common.cuh"
 #include "orl_deep_core.h"
@@ -169,6 +169,10 @@ int reduce_tape(const float* tape, int tape_width, long long rows, const TapeJob
         case orl_rnnw::TAPE_GAUSS: e = launch_jobs<orl_rnnw::TAPE_GAUSS>(tape, rows, jobs, partials, stride, rb, st); break;
         case orl_rnnw::TAPE_GAUSS + orl_rnnw::MAXD_WIDE:   // a DiagGaussian GRU policy's rows with the X field
             e = launch_jobs<orl_rnnw::TAPE_GAUSS + orl_rnnw::MAXD_WIDE>(tape, rows, jobs, partials, stride, rb, st); break;
+        case orl_rnnw::TAPE_GAUSS_WIDE:   // a wide DiagGaussian GRU policy's rows, without and with the X field
+            e = launch_jobs<orl_rnnw::TAPE_GAUSS_WIDE>(tape, rows, jobs, partials, stride, rb, st); break;
+        case orl_rnnw::TAPE_GAUSS_WIDE + orl_rnnw::MAXD_WIDE:
+            e = launch_jobs<orl_rnnw::TAPE_GAUSS_WIDE + orl_rnnw::MAXD_WIDE>(tape, rows, jobs, partials, stride, rb, st); break;
         case orl_deep::TAPE: e = launch_jobs<orl_deep::TAPE>(tape, rows, jobs, partials, stride, rb, st); break;
         case orl_deep::TAPE_GAUSSIAN: e = launch_jobs<orl_deep::TAPE_GAUSSIAN>(tape, rows, jobs, partials, stride, rb, st); break;
         default: ORL_CHECK_ARG(false, "tape_width (one of the GRU's or the shared model's tapes)");

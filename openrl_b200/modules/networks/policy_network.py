@@ -25,24 +25,32 @@ class PolicyNetwork(nn.Module):
         self.act = ACTLayer(action_space, self.base.output_size, cfg.use_orthogonal, cfg.gain)
         self.head_kind = 1 if self.act.continuous_action else 0          # lib.HEAD_GAUSSIAN / HEAD_CATEGORICAL
         self.n_actions = action_space.shape[0] if self.act.continuous_action else action_space.n  # head width
-        # a GRU policy's DiagGaussian head (cfg.use_recurrent_gaussian_head): the 8-row head block of the GRU kernels
+        # a GRU policy's DiagGaussian head (cfg.use_recurrent_gaussian_head): the 8-row head block of the GRU kernels, and
+        # with cfg.use_wide_recurrent_gaussian_head the 64-wide head (lib.HEAD_GAUSSIAN_WIDE) for widths above 8
         recurrent_gaussian = self.recurrent and self.act.continuous_action
         if recurrent_gaussian and not getattr(cfg, "use_recurrent_gaussian_head", False):
             raise NotImplementedError("recurrent policies are built for Discrete action spaces")
-        if recurrent_gaussian and self.n_actions > 8:
+        wide_recurrent_gaussian = recurrent_gaussian and bool(getattr(cfg, "use_wide_recurrent_gaussian_head", False))
+        if wide_recurrent_gaussian and self.n_actions > 64:
             raise NotImplementedError("recurrent policies with DiagGaussian heads are built for Box action spaces of width "
-                                      "up to 8 (use_recurrent_gaussian_head)")
+                                      "up to 64 (use_wide_recurrent_gaussian_head)")
+        if recurrent_gaussian and self.n_actions > 8 and not wide_recurrent_gaussian:
+            raise NotImplementedError("recurrent policies with DiagGaussian heads are built for Box action spaces of width "
+                                      "up to 8 (use_recurrent_gaussian_head; 9..64 with use_wide_recurrent_gaussian_head)")
         # a feed-forward Categorical head runs up to 64 actions (a logits tile in the kernels); a GRU policy's head runs up
         # to 64 with cfg.use_wide_recurrent_head (a lane-owned 64-vector in the GRU kernels) and up to 8 without; the
         # DiagGaussian heads keep the per-thread head of up to 8 outputs, and run up to 64 with cfg.use_wide_gaussian_head
-        # (the 64-wide head tile, lib.HEAD_GAUSSIAN_WIDE, for widths above 8)
-        wide_gaussian = self.act.continuous_action and bool(getattr(cfg, "use_wide_gaussian_head", False))
+        # (the 64-wide head tile, lib.HEAD_GAUSSIAN_WIDE, for widths above 8); a GRU policy's, with the two recurrent
+        # Gaussian options
+        wide_gaussian = wide_recurrent_gaussian or (self.act.continuous_action
+                                                    and bool(getattr(cfg, "use_wide_gaussian_head", False)))
         if wide_gaussian and self.n_actions > 64:
             raise NotImplementedError("DiagGaussian heads are built for Box action spaces of width up to 64 "
                                       "(use_wide_gaussian_head)")
         if self.n_actions > 64:
             raise NotImplementedError("Discrete action spaces of up to 64 actions are built")
-        if self.n_actions > 8 and self.recurrent and not getattr(cfg, "use_wide_recurrent_head", False):
+        if (self.n_actions > 8 and self.recurrent and not wide_recurrent_gaussian
+                and not getattr(cfg, "use_wide_recurrent_head", False)):
             raise NotImplementedError("recurrent policies are built for up to 8 actions (9..64 with use_wide_recurrent_head)")
         if self.n_actions > 8 and self.act.continuous_action and not wide_gaussian:
             raise NotImplementedError("DiagGaussian heads are built for Box action spaces of width up to 8")
