@@ -68,6 +68,8 @@ constexpr int N_LOSS_TC = 8;
 // staging tile of the per-tile GEMM results: 128 rows x 64 fp32 at row pitch S_LD (orl_tc16.cuh);
 // the final Ga [128][GA_LD] / Gb [64][GB_LD] staging reuses R1 / R2
 constexpr int GA_LD = 84, GB_LD = 20;
+// the fp32 W3f^T of the final GH contraction, in R3 at row pitch W3T_LD (conflict-free stores and reads)
+constexpr int W3T_LD = 65;
 // shared-memory carve-up (bytes)
 constexpr uint32_t OFF_R1H = 0, OFF_R1L = OFF_R1H + R1_PANELS * PANEL, OFF_R2H = OFF_R1L + R1_PANELS * PANEL,
                    OFF_R2L = OFF_R2H + R2_PANELS * PANEL, OFF_WH = OFF_R2L + R2_PANELS * PANEL, OFF_WL = OFF_WH + 8 * W_PANEL,
@@ -75,6 +77,8 @@ constexpr uint32_t OFF_R1H = 0, OFF_R1L = OFF_R1H + R1_PANELS * PANEL, OFF_R2H =
                    OFF_S = OFF_R3L + R3_PANELS * PANEL, OFF_STAGE = OFF_S + T_M * S_LD * 4;
 static_assert((T_M * GA_LD + 64 * GB_LD) * 4 <= OFF_WH, "the Ga / Gb staging fits in R1 + R2");
 static_assert(OFF_STAGE % 128 == 0, "TMA destination alignment");
+static_assert(H * W3T_LD * 4 <= OFF_S - OFF_R3H, "the W3f^T of the flush fits in R3");
+static_assert(H * 8 + 6 * H + H * H + MAX_OUT * (H + 1) <= (OFF_S - OFF_R3H) / 4, "the parameter copy of the prologue fits in R3");
 static_assert(OFF_R2L + 16 * PANEL <= OFF_R3H, "the 16-panel A descriptors of GEMM3a stop short of R3 (written while they run)");
 constexpr int N_SCAL = 4;                      // scalar columns staged per row
 
@@ -89,6 +93,27 @@ __host__ __device__ inline uint32_t tc_small_off(int d) { return OFF_STAGE + tc_
 constexpr uint32_t SMALL_FLOATS = 8 * H + H + H + MAX_OUT * H + 2 * MAX_OUT;
 constexpr uint32_t XCH_FLOATS = MAX_OUT * H + 3 * MAX_OUT + 3 * 8;
 __host__ __device__ inline uint32_t tc_smem_bytes(int d) { return tc_small_off(d) + 4 * (SMALL_FLOATS + XCH_FLOATS) + 8; }
+
+// Phase stamps for tools/update_epoch_profile.py, compiled in only with -DORL_PROFILE_PHASES (never in the normal
+// build): thread 0 of every CTA records %globaltimer and %clock64 at kernel entry, first tile staged, tile loop end and
+// kernel exit, and the SM it ran on.  orl_profile_phases_read copies the last launch's stamps to the host.
+constexpr int PH_MAX_CTAS = 1024, PH_WORDS = 9;
+#ifdef ORL_PROFILE_PHASES
+__device__ unsigned long long g_phases[PH_MAX_CTAS][PH_WORDS];
+__device__ __forceinline__ void phase_stamp(int k) {
+    if (threadIdx.x != 0 || blockIdx.x >= PH_MAX_CTAS) return;
+    unsigned long long t, c;
+    unsigned sm;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    asm volatile("mov.u64 %0, %%clock64;" : "=l"(c));
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+    g_phases[blockIdx.x][k] = t;
+    g_phases[blockIdx.x][4 + k] = c;
+    g_phases[blockIdx.x][8] = sm;
+}
+#else
+__device__ __forceinline__ void phase_stamp(int) {}
+#endif
 
 // the activation's derivative; ACT as for act_tc (orl_tc16.cuh)
 template <int ACT>
@@ -123,52 +148,6 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     float* qs = swh + MAX_OUT;                   // flush: [8][64] Q rows, then su[8], smu[8], sdl[8]
     float* red = qs + MAX_OUT * H + 3 * MAX_OUT; // flush: [3][8] per-warp loss sums
     uint64_t* bar_st = reinterpret_cast<uint64_t*>(red + 3 * 8);  // TMA staging
-
-    // ---- stage weights (folded); the fc3 matrix as split fp16 ----
-    stage_weights_tc(w1t, Wh, Wl, params, d, n, T_NT);
-    for (int j = tid; j < MAX_OUT; j += T_NT) {   // from the parameters, not from the rounded whf
-        float rs = 0.f;
-        if (j < n) for (int k = 0; k < H; ++k) rs += folded_wh(params, po, j, k);
-        swh[j] = rs;
-    }
-    // panels that are read before their first per-tile write: zero them (U of lanes beyond n, X beyond d are rewritten per tile)
-    if (half == 0) {
-        const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-        *reinterpret_cast<uint4*>(R1h + P_CST * PANEL + row * 16) = z; *reinterpret_cast<uint4*>(R1l + P_CST * PANEL + row * 16) = z;
-        *reinterpret_cast<uint4*>(R1h + P_X * PANEL + row * 16) = z;   *reinterpret_cast<uint4*>(R1l + P_X * PANEL + row * 16) = z;
-        *reinterpret_cast<uint4*>(R2h + P_U * PANEL + row * 16) = z;   *reinterpret_cast<uint4*>(R2l + P_U * PANEL + row * 16) = z;
-    }
-    if (tid == 0) mbar_init(bar_st, 1);
-    fence_proxy_async();
-    __syncthreads();
-    // weight-gradient accumulators for the whole kernel: Ga rows [64 half, +64), Gb (warpgroup 1)
-    float ga[40], gb[8];
-#pragma unroll
-    for (int i = 0; i < 40; ++i) ga[i] = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) gb[i] = 0.f;
-
-    // ---- minibatch constants ----
-    const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS, val_masks = a.flags & ORL_PPO_VALUE_ACTIVE_MASKS;
-    const MbConsts mb = mb_consts(a);
-    const double rows_d = loss_rows(a);
-    // operand scales of the backward GEMMs (powers of two; see the header comment)
-    float wmax = 0.f;
-    for (int i = 0; i < MAX_OUT * H; ++i) wmax = fmaxf(wmax, fabsf(whf[i]));   // smem broadcast reads, once per kernel
-    // with active masks a live row weighs active / sum(active), not 1 / rows: scale by the rows that carry the weight
-    const double live_d = (POLICY ? pol_masks : val_masks) ? fmin(rows_d, a.mb_stats[2]) : rows_d;
-    const int e_rows = (int)ceil(log2(fmax(live_d, 1.0)));
-    const int e_u = min(e_rows + 3, 60);
-    const int e_z = min(max(e_rows + 3 - (int)floorf(log2f(fmaxf(wmax, 1e-12f))), 0), 60);
-    const float Sz = exp2f((float)e_z), Su = exp2f((float)e_u);
-    constexpr float SX = 16.f, K1 = 0.25f;          // observations x 16; dZ1 is stored as S_z / 4
-    const float invSz = exp2f(-(float)e_z), invSu = exp2f(-(float)e_u), invS1 = invSz * (1.f / K1);
-
-    // ---- MMA descriptors (constant parts) ----
-    const uint64_t dK_A = desc_const(PANEL, 128), dK_W = desc_const(W_PANEL, 128);      // K-major
-    const uint64_t dMN_A = desc_const(128, PANEL), dMN_W = desc_const(128, W_PANEL);    // MN-major
-    const uint32_t aR1h = smem_u32(R1h), aR1l = smem_u32(R1l), aR2h = smem_u32(R2h), aR2l = smem_u32(R2l), aWh = smem_u32(Wh), aWl = smem_u32(Wl);
-    const uint32_t aR3h = smem_u32(R3h), aR3l = smem_u32(R3l);
 
     // ---- staging of the minibatch rows, one tile ahead ----
     const long long n_tiles = (a.batch_rows + T_M - 1) / T_M;
@@ -208,14 +187,79 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         if (r >= a.batch_rows) return -1;
         return a.indices ? a.indices[r] : a.row_begin + r;
     };
+    // the first tile's rows are requested before the weights are staged, so that their load runs under the fold below
     long long gi_next = -1;
     if (TMA) {
-        if (tid == 0 && cta < n_tiles) { tma_prefetch_desc(POLICY ? &maps.obs_p : &maps.obs_c); issue_tma(cta); }
+        if (tid == 0) {
+            mbar_init(bar_st, 1);
+            fence_proxy_async();   // the initialised barrier, before the TMA unit signals it
+            if (cta < n_tiles) { tma_prefetch_desc(POLICY ? &maps.obs_p : &maps.obs_c); issue_tma(cta); }
+        }
     } else {
         issue_gather(row_index(cta));
         gi_next = row_index(cta + G);
     }
     long long gi = row_index(cta);
+
+    // ---- stage weights (folded); the fc3 matrix as split fp16 ----
+    // The fold runs on a copy of the net's parameters in R3 (free until the first tile): one round of independent
+    // global loads, and the 64-deep chains of b3f, bhf and swh then read shared memory.  The same values through the
+    // same expressions: every staged weight keeps its bits.
+    float* pcopy = reinterpret_cast<float*>(R3h);
+    for (int i = tid; i < po.total; i += T_NT) pcopy[i] = params[i];
+    // the minibatch constants' global loads go out with the copy's
+    const bool pol_masks = a.flags & ORL_PPO_POLICY_ACTIVE_MASKS, val_masks = a.flags & ORL_PPO_VALUE_ACTIVE_MASKS;
+    const MbConsts mb = mb_consts(a);
+    const double rows_d = loss_rows(a);
+    __syncthreads();
+    stage_weights_tc(w1t, Wh, Wl, pcopy, d, n, T_NT);
+    // swh on warp 4, while warp 0 runs the b3f and bhf chains of stage_weights_tc
+    if (tid >= 4 * 32 && tid < 4 * 32 + MAX_OUT) {   // from the parameters, not from the rounded whf
+        const int j = tid - 4 * 32;
+        float rs = 0.f;
+        if (j < n) for (int k = 0; k < H; ++k) rs += folded_wh(pcopy, po, j, k);
+        swh[j] = rs;
+    }
+    // panels that are read before their first per-tile write: zero them (U of lanes beyond n, X beyond d are rewritten per tile)
+    if (half == 0) {
+        const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+        *reinterpret_cast<uint4*>(R1h + P_CST * PANEL + row * 16) = z; *reinterpret_cast<uint4*>(R1l + P_CST * PANEL + row * 16) = z;
+        *reinterpret_cast<uint4*>(R1h + P_X * PANEL + row * 16) = z;   *reinterpret_cast<uint4*>(R1l + P_X * PANEL + row * 16) = z;
+        *reinterpret_cast<uint4*>(R2h + P_U * PANEL + row * 16) = z;   *reinterpret_cast<uint4*>(R2l + P_U * PANEL + row * 16) = z;
+    }
+    fence_proxy_async();
+    __syncthreads();
+    // weight-gradient accumulators for the whole kernel: Ga rows [64 half, +64), Gb (warpgroup 1)
+    float ga[40], gb[8];
+#pragma unroll
+    for (int i = 0; i < 40; ++i) ga[i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) gb[i] = 0.f;
+
+    // operand scales of the backward GEMMs (powers of two; see the header comment)
+    // wmax = max |whf| over the CTA (a maximum: the same value in any order)
+    float wmax = 0.f;
+    for (int i = tid; i < MAX_OUT * H; i += T_NT) wmax = fmaxf(wmax, fabsf(whf[i]));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) wmax = fmaxf(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
+    if (lane == 0) red[warp] = wmax;
+    __syncthreads();
+#pragma unroll
+    for (int w = 0; w < T_NT / 32; ++w) wmax = fmaxf(wmax, red[w]);
+    // with active masks a live row weighs active / sum(active), not 1 / rows: scale by the rows that carry the weight
+    const double live_d = (POLICY ? pol_masks : val_masks) ? fmin(rows_d, a.mb_stats[2]) : rows_d;
+    const int e_rows = (int)ceil(log2(fmax(live_d, 1.0)));
+    const int e_u = min(e_rows + 3, 60);
+    const int e_z = min(max(e_rows + 3 - (int)floorf(log2f(fmaxf(wmax, 1e-12f))), 0), 60);
+    const float Sz = exp2f((float)e_z), Su = exp2f((float)e_u);
+    constexpr float SX = 16.f, K1 = 0.25f;          // observations x 16; dZ1 is stored as S_z / 4
+    const float invSz = exp2f(-(float)e_z), invSu = exp2f(-(float)e_u), invS1 = invSz * (1.f / K1);
+
+    // ---- MMA descriptors (constant parts) ----
+    const uint64_t dK_A = desc_const(PANEL, 128), dK_W = desc_const(W_PANEL, 128);      // K-major
+    const uint64_t dMN_A = desc_const(128, PANEL), dMN_W = desc_const(128, W_PANEL);    // MN-major
+    const uint32_t aR1h = smem_u32(R1h), aR1l = smem_u32(R1l), aR2h = smem_u32(R2h), aR2l = smem_u32(R2l), aWh = smem_u32(Wh), aWl = smem_u32(Wl);
+    const uint32_t aR3h = smem_u32(R3h), aR3l = smem_u32(R3l);
 
     float loss0 = 0.f, loss1 = 0.f, loss2 = 0.f;
     uint32_t it = 0;
@@ -224,6 +268,7 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         // ---- this tile's rows from the staging buffer ----
         if (TMA) mbar_wait(bar_st, par);
         else { cp_async_wait_all(); __syncwarp(); }   // a row's gathers are issued by its two lanes
+        if (it == 0) phase_stamp(1);
         const bool valid = gi >= 0;
         float x[8];
 #pragma unroll
@@ -422,6 +467,7 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         }
     }
     wgmma_wait<0>();   // the last tile's GEMM3a / GEMM3b
+    phase_stamp(2);
 
     // ---- flush: Ga / Gb (accumulator registers -> staging in R1 / R2) -> partial folded gradients ----
     float* part = a.partials + (size_t)((POLICY ? 0 : G) + cta) * stride;
@@ -430,22 +476,16 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
     if (it > 0) {
         float* gas = reinterpret_cast<float*>(smem);   // [128][GA_LD]
         float* gbs = gas + T_M * GA_LD;                // [64][GB_LD]
+        float* w3t = reinterpret_cast<float*>(R3h);    // [64][W3T_LD]
         __syncthreads();   // every MMA has completed: R1 / R2 are free
         frag_store<80>(ga, gas + wg * 64 * GA_LD, GA_LD);
         if (wg == 1) frag_store<16>(gb, gbs, GB_LD);
+        // W3f as fp32 for GH below, transposed into R3 (free once the last GEMM3b has completed): w3t[i][k] = W3f[k][i]
+        for (int e = tid; e < H * H; e += T_NT) w3t[(e & 63) * W3T_LD + (e >> 6)] = folded_w3(params, po, e >> 6, e & 63);
         __syncthreads();
-        {   // Ga columns [32*half, 32*half+32) of this row
-            float v[32];
-#pragma unroll
-            for (int c = 0; c < 32; ++c) v[c] = gas[row * GA_LD + 32 * half + c];
-            if (row < H) {
-#pragma unroll
-                for (int c = 0; c < 32; ++c) part[fo.g3 + row * H + 32 * half + c] = v[c] * invSz;
-            } else if (row < H + n) {
-#pragma unroll
-                for (int c = 0; c < 32; ++c) qs[(row - H) * H + 32 * half + c] = v[c];
-            }
-        }
+        // Ga rows [0, 64) are G3, rows [64, 64 + n) Q: consecutive threads take consecutive columns (coalesced stores)
+        for (int e = tid; e < H * H; e += T_NT) part[fo.g3 + e] = gas[(e >> 6) * GA_LD + (e & 63)] * invSz;
+        for (int e = tid; e < n * H; e += T_NT) qs[e] = gas[(H + (e >> 6)) * GA_LD + (e & 63)];
         if (half == 0) {
             const float* c8 = gas + row * GA_LD + 64;
             if (row < H) part[fo.db3 + row] = c8[0] * invSz;
@@ -462,7 +502,7 @@ __device__ __forceinline__ void tc_net_pass(const OrlPpoArgs& a, const TcMaps& m
         for (int o = tid; o < n * H; o += T_NT) {
             const int j = o >> 6, k = o & 63;
             float acc = 0.f;
-            for (int i = 0; i < H; ++i) acc = fmaf(qs[j * H + i], folded_w3(params, po, k, i), acc);
+            for (int i = 0; i < H; ++i) acc = fmaf(qs[j * H + i], w3t[i * W3T_LD + k], acc);
             acc = fmaf(b3f[k], qsu[j], acc) - qsu[8 + j];
             part[fo.gh + o] = acc * invSu;
             if (k == 0) { part[fo.dbh + j] = qsu[16 + j] * invSu; part[fo.dls + j] = 0.f; }
@@ -492,8 +532,10 @@ __global__ void __launch_bounds__(T_NT, 1) ppo_fwdbwd_tc_kernel(const OrlPpoArgs
     const int G = a.grid_per_net;
     const bool policy = (int)blockIdx.x < G;
     const int cta = policy ? (int)blockIdx.x : (int)blockIdx.x - G;
+    phase_stamp(0);
     if (policy) tc_net_pass<true, NOUT, ACT, TMA>(a, maps, smem_tc, cta, G, stride);
     else tc_net_pass<false, 1, ACT, TMA>(a, maps, smem_tc, cta, G, stride);
+    phase_stamp(3);
 }
 
 using TcKernel = void (*)(const OrlPpoArgs, const TcMaps, int);
@@ -593,3 +635,10 @@ int launch_ppo_fwdbwd_tc(const OrlPpoArgs& a, cudaStream_t st) {
     return check_cuda(cudaGetLastError(), "ppo_fwdbwd_tc_kernel");
 }
 }  // namespace orl
+
+#ifdef ORL_PROFILE_PHASES
+// the stamps of the last ppo_fwdbwd_tc_kernel launch: [PH_MAX_CTAS][PH_WORDS] u64 (not part of the declared C-ABI)
+extern "C" int orl_profile_phases_read(unsigned long long* host) {
+    return orl::check_cuda(cudaMemcpyFromSymbol(host, g_phases, sizeof(g_phases)), "orl_profile_phases_read");
+}
+#endif
